@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the Raindrop hot path on B200 (driver contract: see the task statement).
+"""Benchmark of the Raindrop hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one training step of Raindrop_v2 (forward + CrossEntropy + backward + Adam, dropout 0.2,
@@ -10,7 +10,7 @@ configuration is the one BASELINE.json's metric is quoted on (configs[1]: P19 sh
 GPU, 34 sensors, T_max = 60); `--config` selects the other BASELINE configurations:
 
     P12      configs[0]  B = 32,  36 sensors, T = 215   (the reference's CPU-runnable case)
-    P19      configs[1]  B = 128, 34 sensors, T = 60    (default; the driver's line)
+    P19      configs[1]  B = 128, 34 sensors, T = 60    (default)
     PAM      configs[2]  B = 256, 17 sensors, T = 600, 8 classes, no static branch
     P19x4    configs[3]  B = 256 per GPU (1024 over 4 GPUs), leave-10-sensors-out mask
     LARGEx8  configs[4]  B = 512 per GPU (4096 over 8 GPUs), 128 sensors, T = 256
@@ -32,7 +32,14 @@ Printed JSON line (rank 0):
             8*N*C per (sample, layer) / CUDA-event time, at a row count with >= 1 GiB of traffic
             (`rows`) and at the configuration's own batch (`at_config`)
   cpu_baseline  the CPU restatement of the reference (oracle/, same per-sample loop and per-edge
-            GEMMs as code/models_rd.py:322-343) timed on this box's host cores
+            GEMMs as code/models_rd.py:322-343) timed on the host's cores
+
+--dump-outputs DIR writes what the last timed step of the device-resident TrainStep computed, as float32 .npy files:
+logits.npy and loss.npy (what a caller of the step receives), and grad_<parameter>.npy / param_<parameter>.npy (the
+gradients of that step and the parameters after its Adam update, for every parameter the step uses).  All files
+together stay within 64 MB: when the full tensors would not fit, every tensor with more than c elements (the largest c
+that fits) is replaced by the 1-D sample flat[sorted(torch.randperm(n, generator seeded with DUMP_SEED)[:c])].  Inputs,
+weights and the dropout stream are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -56,7 +63,7 @@ from raindrop_b200.synth import make_batch, model_config  # noqa: E402
 from raindrop_b200.synth import synth_weights  # noqa: E402
 
 warnings.filterwarnings("ignore")
-L2_FLUSH_BYTES = 256 << 20   # > 126 MB L2
+L2_FLUSH_BYTES = 256 << 20   # > 50 MB L2 of an H100
 
 # name -> (synthetic model config, per-GPU batch, GPUs the BASELINE config names, make_batch options, workload string)
 BENCH_CONFIGS = {
@@ -75,11 +82,8 @@ def workload_string(name):
 
 
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.isfile(path):
-        p = json.load(open(path))
-        return float(p["hbm_gbs"]), float(p.get("bf16_tflops", 0.0)) or None, "measured (MEASURED_PEAKS.json)"
-    return 6650.0, None, "fallback (B200_PROFILING.md)"
+    """HBM GB/s and dense BF16 TFLOP/s of the H100 SXM data sheet (a card held below 700 W reaches less)."""
+    return 3350.0, 989.0, "NVIDIA H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -152,7 +156,7 @@ def build_model(cfg, device):
 
 def flush_l2(buf):
     """Write a buffer larger than L2, then read it back: the write evicts everything, the read leaves the
-    cache full of CLEAN lines (otherwise the timed kernel pays for writing back ~126 MB of dirty zeros)."""
+    cache full of CLEAN lines (otherwise the timed kernel pays for writing back ~50 MB of dirty zeros)."""
     buf.zero_()
     buf.sum()
 
@@ -229,22 +233,18 @@ def roofline_leg(cfg, batch, device):
         out[tag] = dict(rows=rows, ms=ms, achieved=gb / (ms * 1e-3), frac=gb / (ms * 1e-3) / hbm_peak,
                         tflops=2.0 * rows * C * C / (ms * 1e-3) / 1e12, ms_b2b=ms_b2b, frac_b2b=gb / (ms_b2b * 1e-3) / hbm_peak)
         del x, y
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "obprop_tc_traffic.json")
-    if os.path.isfile(tpath) and C == 240:
-        traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
     big = out["large"]
     tensor_frac = (big["tflops"] / tf32_peak) if tf32_peak else None
     # C/4 flop per byte against the TF32 ridge: HBM binds at C=240, both are close at 860/1024, tensor at 2400
     bound = "tensor" if (tensor_frac is not None and tensor_frac > big["frac"]) else "hbm"
-    r = {"kernel": "obprop_tc_kernel (tcgen05 TF32 + TMA, one ob-prop layer, C=%d)" % C, "bound": bound,
-         "peak_source": how, "rows": big["rows"], "ms_per_launch": round(big["ms"], 5), "traffic": traffic,
+    r = {"kernel": "tc_nt_kernel (wgmma TF32 + TMA, one ob-prop layer, C=%d)" % C, "bound": bound,
+         "peak_source": how, "rows": big["rows"], "ms_per_launch": round(big["ms"], 5),
          "algorithmic_bytes_per_launch": big["rows"] * C * 8, "algorithmic_flops_per_launch": 2 * big["rows"] * C * C,
          "hbm": {"achieved": round(big["achieved"], 1), "peak": hbm_peak, "unit": "GB/s", "frac": round(big["frac"], 4)},
-         "tensor": {"achieved": round(big["tflops"], 1), "peak": tf32_peak, "unit": "TFLOP/s (tf32 = measured bf16 peak / 2)",
+         "tensor": {"achieved": round(big["tflops"], 1), "peak": tf32_peak, "unit": "TFLOP/s (tf32 = bf16 peak / 2)",
                     "frac": round(tensor_frac, 4) if tensor_frac is not None else None},
          "back_to_back": {"ms_per_launch": round(big["ms_b2b"], 5), "frac": round(big["frac_b2b"], 4),
-                          "note": "no L2 flush between launches (same protocol as the measured copy peak)"},
+                          "note": "no L2 flush between launches"},
          "at_config": {"rows": out["at_config"]["rows"], "ms_per_launch": round(out["at_config"]["ms"], 5),
                        "achieved": round(out["at_config"]["achieved"], 1), "frac": round(out["at_config"]["frac"], 4),
                        "tflops": round(out["at_config"]["tflops"], 1),
@@ -343,6 +343,8 @@ def main():
     ap.add_argument("--config", default="P19", choices=sorted(BENCH_CONFIGS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed TrainStep's outputs as .npy files into DIR (see the module docstring)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -398,6 +400,8 @@ def main():
     ms_per_step = dev["median"]
     value = world * BATCH / (ms_per_step * 1e-3)
     loss_graph = float(ts.loss.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ts, model)
 
     # ---- leg 2: end to end through the drop-in module API, host batches ---------------------------
     model2 = build_model(cfg, device)
@@ -473,7 +477,9 @@ def main():
 
     # ---- leg 4: whole-validation-set evaluation (evaluate_standard, code/utils_rd.py:310-320), sharded ----------
     from raindrop_b200.train import evaluate_sharded
-    n_val = {"P19": 3880, "P12": 1199, "PAM": 533}.get(cfg_name, 4 * BATCH)          # SURVEY.md section 3.2
+    # validation-set sizes of the data sets (SURVEY.md section 3.2); the synthetic LARGE set is evaluated on 1024 samples,
+    # whose one-batch workspace (~13 GB) fits an 80 GB H100 beside the state of the training legs
+    n_val = {"P19": 3880, "P12": 1199, "PAM": 533, "LARGE": 1024}.get(cfg_name, 4 * BATCH)
     val = make_batch(cfg, n_val, seed=4242, **opts)
     val_dev = {k: (v.to(device) if v is not None else None) for k, v in val.items()}
     model2.eval()
@@ -540,6 +546,45 @@ def main():
                                     "sample": "cpu leg failed or timed out: %r" % (exc,)}
     print(json.dumps(line), flush=True)
     _finish(world)
+
+
+DUMP_BYTES = 64_000_000   # cap on everything --dump-outputs writes (data + .npy headers)
+DUMP_SEED = 20240917
+
+
+def dump_cap(sizes, budget):
+    """Largest per-tensor element count c with sum(min(n, c)) float32 elements + one header per file within budget."""
+    fits = lambda c: 4 * sum(min(n, c) for n in sizes) + 128 * len(sizes) <= budget
+    lo, hi = 1, max(sizes)
+    if fits(hi):
+        return hi
+    while lo < hi:                      # fits(lo) holds, fits(hi) does not
+        mid = (lo + hi + 1) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid - 1)
+    return lo
+
+
+def dump_outputs(out_dir, ts, model):
+    """What the last step of `ts` computed (logits, loss, gradients, updated parameters) as float32 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {"logits": ts.logits, "loss": ts.loss.reshape(1)}
+    for (name, _), prm, off in zip(ts.plan.fields, model.used_parameters(), ts.offsets):
+        key = name.replace(".", "_")
+        arrays["grad_" + key] = ts.flat_g[off:off + prm.numel()].view(prm.shape)
+        arrays["param_" + key] = prm.data
+    cap = dump_cap([t.numel() for t in arrays.values()], DUMP_BYTES)
+    written = 0
+    for name, t in arrays.items():
+        a = t.detach().float().cpu()
+        if a.numel() > cap:        # fixed, seeded sample of the flat tensor, in index order
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(DUMP_SEED))[:cap].sort().values
+            a = a.reshape(-1)[idx]
+        path = os.path.join(out_dir, name + ".npy")
+        np.save(path, a.numpy())
+        written += os.path.getsize(path)
+    assert written <= DUMP_BYTES, written
 
 
 def _finish(world):

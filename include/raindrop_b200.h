@@ -1,5 +1,5 @@
 /*
- * raindrop_b200.h -- C ABI of librd_b200.so (sm_100a), the device side of the Raindrop hot path.
+ * raindrop_b200.h -- C ABI of librd_b200.so (sm_90a, H100), the device side of the Raindrop hot path.
  *
  * The reference (mims-harvard/Raindrop) is pure Python; it has no FFI of its own.  The boundary
  * a maintainer binds is therefore the set of Python call sites listed beside each entry point
@@ -248,7 +248,7 @@ int rd_linear_fwd(const float* x, const float* weight, const float* bias, int64_
  *   ctx[t, b, h*hd:(h+1)*hd] = dropout(softmax_j(q_t . k_j / sqrt(hd), keys j >= lengths[b] masked)) . v
  * and its backward d_qkv [T, B, 3*H*hd] from d_ctx [T, B, H*hd] (probabilities are recomputed, nothing T x T is
  * stored).  rng_captured = 2 x uint64 {seed, counter} on the device (ignored when drop_p == 0); `site` selects the
- * dropout stream (16 + layer inside the model).  impl: 0 = automatic, 1 = tcgen05 tensor-core kernels
+ * dropout stream (16 + layer inside the model).  impl: 0 = automatic, 1 = tensor-core kernels
  * (T <= 64, hd <= 96, hd % 4 == 0), 2 = CUDA-core kernels (T <= 64, hd <= 96).  Longer sequences are handled inside
  * rd_raindrop_v2_fwd/_bwd (they need workspace). */
 int rd_temporal_attention_fwd(const float* qkv, const int64_t* lengths, int32_t B, int32_t H, int32_t T, int32_t hd,
@@ -340,10 +340,11 @@ int rd_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg
                  float lr, const float* lr_dev, float beta1, float beta2, float eps, float grad_scale,
                  int64_t* step, void* stream);
 
-/* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention forward kernel writes
- * %globaltimer phase stamps into it (tools/attn_timing.py); NULL switches it off. */
+/* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
+ * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);
-/* same for the projection GEMM kernel behind rd_linear_fwd: [n_ctas][8] uint64 */
+/* same for the tensor-core GEMM kernel (rd_linear_fwd, the encoder and ob-prop GEMMs): [n_ctas][8] uint64,
+ * %globaltimer at the CTA's start (slot 0) and end (slot 7) */
 int rd_debug_gemm_timing(uint64_t* buffer);
 
 /* debug: materialise the dropout keep/scale mask (0 or 1/(1-p)) of one dropout site, so tests can

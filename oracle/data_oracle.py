@@ -9,7 +9,7 @@ Each function follows the reference line by line:
   remove_features        code/Raindrop.py:214-231
   epoch_batches          code/Raindrop.py:261-309  (strategy 2 and 3)
 Pinned against the reference's own functions in tests/test_data_pipeline.py::test_data_oracle_matches_reference
-(runs wherever /root/reference is present).
+(against their outputs stored in tests/golden/data_utils.npz).
 """
 import numpy as np
 import torch
@@ -88,3 +88,18 @@ def epoch_batches(y, batch_size, strategy, state):
     else:
         out = [np.random.choice(list(range(len(y))), size=int(batch_size), replace=False) for _ in range(30)]
     return np.stack(out), state
+
+
+def synthetic_raw(n=23, T=17, F=6, D=4, seed=0):
+    """Raw arrays shaped like a loaded data set: P [n, T, F] (sparse, zero after each length), minutes [n, T], static
+    [n, D], y [n, 1] -- the inputs of the data-pipeline tests and of their reference fixture (oracle/make_golden.py)."""
+    g = np.random.default_rng(seed)
+    P = g.normal(50, 20, (n, T, F)) * (g.random((n, T, F)) < 0.35)
+    P[P < 0] = 0
+    lens = g.integers(2, T + 1, n)
+    for i in range(n):
+        P[i, lens[i]:] = 0
+    minutes = np.cumsum(g.random((n, T)) * 60 + 1, 1) * (np.arange(T)[None, :] < lens[:, None])
+    static = g.normal(1, 2, (n, D))
+    y = (g.random(n) < 0.3).astype(np.int64)[:, None]
+    return P, minutes, static, y

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.  Generates tests/golden/*.npz by running the reference's own,
 unmodified files (oracle/ref_harness.py) on CPU in the build container:
 
-    python -m oracle.make_golden            # from the repo root; needs /root/reference
+    RAINDROP_REFERENCE=<checkout of mims-harvard/Raindrop> python -m oracle.make_golden      # from the repo root
 
 A fixture stores seeds + the reference's outputs; inputs and weights are regenerated from the
 seeds by raindrop_b200.synth (make_batch / synth_weights), so the files stay small.  Stored per
@@ -10,6 +10,7 @@ attention, code/models_rd.py:341), the encoder output `enc` [T,B,D] (code/models
 cross-entropy loss and the gradient of every parameter that receives one -- in full for tiny
 shapes, as fingerprints (sum / abs-sum / l2 / strided sample) for the BASELINE shapes.
 """
+import hashlib
 import json
 import os
 import sys
@@ -232,6 +233,46 @@ def v1_case():
           (logits[0].tolist(), loss.item(), float(distance), sum(1 for k in out if k.startswith("grad."))))
 
 
+def data_utils_case():
+    """The reference's own host-side data functions (code/utils_rd.py) on oracle.data_oracle.synthetic_raw(seed=4)
+    -> data_utils.npz (pins oracle/data_oracle.py)."""
+    ref_harness.load_reference()                       # puts the reference's code/ on sys.path
+    import utils_rd as U
+    from oracle import data_oracle as DO
+    P, minutes, static, y = DO.synthetic_raw(seed=4)
+    out = {}
+    try:
+        mf, stdf = U.getStats(P)
+        out["getStats.mf"], out["getStats.stdf"] = mf, stdf
+    except ValueError:
+        # numpy >= 1.24 rejects `np.max([stdf[f], eps])` (code/utils_rd.py:160); the rest runs on the restatement's stats
+        mf, stdf = DO.get_stats(P)
+    out["mask_normalize"] = U.mask_normalize(P.copy(), mf, stdf)
+    ms, ss = U.getStats_static(static, dataset="P12")
+    out["getStats_static.ms"], out["getStats_static.ss"] = np.asarray(ms), np.asarray(ss)
+    out["mask_normalize_static"] = U.mask_normalize_static(static.copy(), ms, ss)
+    Plist = [{"arr": P[i], "time": minutes[i][:, None], "extended_static": static[i]} for i in range(len(P))]
+    for i, t in enumerate(U.tensorize_normalize(Plist, y, mf, stdf, ms, ss)):
+        out["tensorize_normalize.%d" % i] = t.numpy()
+    np.savez_compressed(os.path.join(GOLDEN, "data_utils.npz"), **out)
+    print("data_utils  %d arrays" % len(out))
+
+
+def live_tiny_case():
+    """Raindrop_v2 of the reference built and run on the TINY configuration -> live_tiny.npz: digests of its initial state
+    dict (in module order) and eval-mode logits on make_batch(cfg, 3, seed=1)."""
+    cfg = model_config("TINY", dropout=0.2)
+    ref = ref_harness.build_reference_model(cfg).eval()
+    batch = make_batch(cfg, 3, seed=1)
+    with torch.no_grad():
+        logits = ref.forward(batch["src"], batch["static"], batch["times"], batch["lengths"])[0]
+    # the state dict is pinned bit for bit through SHA-256 digests of its float32 bytes (the tensors themselves are 300 KB)
+    digests = [hashlib.sha256(v.contiguous().numpy().tobytes()).hexdigest() for v in ref.state_dict().values()]
+    out = {"state_sha256": np.array(digests), "logits": logits.numpy()}
+    np.savez_compressed(os.path.join(GOLDEN, "live_tiny.npz"), **out)
+    print("live_tiny  logits[0]=%s, %d state tensors" % (logits[0].tolist(), len(digests)))
+
+
 if __name__ == "__main__":
     os.makedirs(GOLDEN, exist_ok=True)
     torch.set_num_threads(8)
@@ -241,8 +282,14 @@ if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "v1":
         v1_case()
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "live":
+        data_utils_case()
+        live_tiny_case()
+        sys.exit(0)
     for case in CASES:
         run_case(*case)
     operator_cases()
     operator_grad_cases()
     v1_case()
+    data_utils_case()
+    live_tiny_case()

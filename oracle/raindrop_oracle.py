@@ -5,7 +5,7 @@ may import this file; the product path (raindrop_b200/) never does.
 
 What is restated (reference file:line given at each function):
   * PyG `utils.softmax` / `torch_scatter.scatter(reduce='add')` (third-party, NOT under
-    /root/reference, unpinned in requirements.txt:1-9)           -> segment_softmax, scatter_rows
+    the reference tree, unpinned in requirements.txt:1-9)        -> segment_softmax, scatter_rows
   * `Observation_progation.forward/message/aggregate`            -> ObPropOracle
     (code/Ob_propagation.py:94-132, 157-211, 213-228)
   * `TransformerConv.forward/message`                            -> TransformerConvOracle

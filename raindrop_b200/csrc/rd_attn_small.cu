@@ -3,8 +3,8 @@
 // softmax, attention dropout and PV are one launch (forward) and the whole backward is one launch
 // (probabilities are RECOMPUTED from Q, K and the counter-based dropout mask: nothing T x T is stored).
 // This is the temporal-attention stage of nn.TransformerEncoder as called at code/models_rd.py:358 for
-// the P19 shape (T = 60, hd = 76).  A 60 x 60 x 76 problem is far below one 128-row UMMA tile and needs
-// fp32 accuracy, so it runs on the CUDA cores with 4x4 / 4x5 register tiles; longer sequences take the
+// the P19 shape (T = 60, hd = 76), in fp32 on the CUDA cores with 4x4 / 4x5 register tiles (implementation 2 of
+// rd_temporal_attention_*; the tensor-core kernels in rd_attn_tc.cu are the default); longer sequences take the
 // batched-GEMM path (rd_model.cu).
 #include <stdlib.h>
 

@@ -1,32 +1,19 @@
-// Temporal self-attention for short sequences (T <= 64, head_dim <= 96) on the 5th-gen tensor cores.
+// Temporal self-attention for short sequences (T <= 64, head_dim <= 96) on the tensor cores (sm_90a).
 //
 // nn.TransformerEncoder's attention as called at code/models_rd.py:358 for the P19 shape (T = 60, hd = 76):
 // per (sample, head) S = scale * Q K^T, key-padding-masked softmax, attention dropout, O = P V -- and the whole
 // backward (dV = Pd^T dO, dP = dO V^T, dS = P * (dP - rowsum(dP * P)), dQ = scale * dS K, dK = scale * dS^T Q).
-// One CTA per (sample, head); every contraction is a tcgen05.mma.kind::tf32 with error compensation (operands split
-// as hi + lo, three MMAs per k-step: lo.hi + hi.lo + hi.hi), so the results are fp32-accurate like the CUDA-core
-// kernels they replace (rd_attn_small.cu).  Nothing T x T ever reaches HBM; the backward RECOMPUTES the
-// probabilities from Q, K and the counter-based dropout stream.
+// One CTA of four warps per (sample, head); warp w owns rows 16w .. 16w+15 of every product.  Every contraction is an
+// error-compensated mma.sync.m16n8k8 TF32 product (operands split into hi + lo in registers, three MMAs per k-step:
+// lo.hi + hi.lo + hi.hi), so the results are fp32-accurate like the CUDA-core kernels in rd_attn_small.cu.  Half of
+// these contractions run over the ROWS of a shared-memory tile (O = P V, dV, dQ, dK), which wgmma's TF32 form cannot
+// read; mma.sync takes fragments gathered per thread, so one row-major image per operand serves every role and nothing
+// is transposed.  Nothing T x T reaches HBM; the backward RECOMPUTES the probabilities from Q, K and the counter-based
+// dropout stream.
 //
-// Data movement: each [T x hd] head slice of the packed qkv / d(ctx) tensors is fetched by TMA as three
-// {32 column, 64 row} boxes (5-D tensor map over [T, B, 3, H, hd]: out-of-range columns >= hd and rows >= T arrive
-// as zeros).  An operand is used in one of two roles and each role has its own shared-memory image:
-//   * K-major   (contraction over the COLUMNS d):  S = Q K^T, dP = dO V^T   -- classic 128B swizzle (16-byte atoms)
-//   * MN-major  (contraction over the ROWS t):     O = P V, dV = Pd^T dO, dQ = dS K, dK = dS^T Q
-//                                                  -- 128B swizzle with 32-BYTE atoms, the only MN-major layout the
-//                                                     tensor core takes for 32-bit operands (rd_tc_common.cuh)
-// The same global tile is simply fetched through a second tensor map when the other role is needed.  The
-// probabilities / score gradients are written by the softmax threads as row-major [64 x 64] tiles in whichever
-// swizzle their consumer needs: read row-wise they are a K-major A operand (O = P V, dQ = dS K), read column-wise
-// an MN-major A operand (dV = Pd^T dO, dK = dS^T Q) -- no transposes anywhere.  M = 128 MMAs are issued on 64-row
-// tiles: rows 64..127 of the A operand read whatever follows in shared memory and only produce accumulator rows
-// nobody reads.
-//
-// Backward, shared-memory plan (four 48 KB regions, 200 KB with the tail pad):
-//   phase 1  R0 = Q, R1 = K, R2 = V, R3 = dO (K-major images)          S = Q K^T, dP = dO V^T
-//   phase 2  softmax threads: R0 <- Pd (MN image), R1 <- scale*dS (K-major image), R0/R1 tails <- scale*dS (MN image)
-//            TMA meanwhile:   R2 <- dO (MN image), R3 <- K (MN image)   dV = Pd^T dO, dQ = dS K
-//   phase 3  R2 <- Q (MN image)                                          dK = dS^T Q
+// Shared memory: head slices [64][LD] with LD = round_up(hd, 8) + 4 (a row stride of 4 mod 8 floats keeps the
+// row-wise fragment gathers free of bank conflicts), probability / score-gradient tiles [64][68].  At P19 (hd = 76,
+// LD = 84) the forward takes 80 KB and the backward 101 KB (Pd reuses the V slice), so two CTAs share an SM.
 #include <stdlib.h>
 
 #include "rd_kernels.cuh"
@@ -36,567 +23,263 @@ namespace rd {
 using namespace tc;
 namespace {
 
-constexpr int TR = 64;                    // rows (timestamps) per tile
-constexpr int NG = 3;                     // 32-column groups per head slice (hd <= 96)
-constexpr int GRP = TR * 128;             // one {32 col, 64 row} box: 8192 bytes
-constexpr int TILE = NG * GRP;            // 24576 bytes (hi); the lo image follows
-constexpr int PT = 2 * GRP;               // probability / score-gradient tile [64 x 64]: 16384 bytes
+constexpr int TR = 64;                    // rows (timestamps) per head slice
+constexpr int HD_MAX = 96;
+constexpr int LDP = TR + 4;               // probability / score-gradient tiles
 constexpr int NTHR = 128;
 
 struct AttnTcP {
   float* ctx; float* dqkv;
   const int64_t* lengths;
-  int B, H, T, hd, D;
+  int B, H, T, hd, D, ld;
   float scale, drop_p;
   const uint64_t* rng; uint32_t site;
-  unsigned long long* dbg;      // optional phase timestamps (rd_debug_attention_timing): [CTA][16] of %globaltimer
+  unsigned long long* dbg;      // optional start / end timestamps (rd_debug_attention_timing): [CTA][16] of clock64
 };
 
 __device__ __forceinline__ void stamp(const AttnTcP& p, int slot) {
-  if (p.dbg && threadIdx.x == 0) {
-    // SM cycle counter: a %globaltimer read costs 0.25-0.5 us (and ticks every 256 ns), which perturbed what it measured
-    p.dbg[(size_t)blockIdx.x * 16 + slot] = (unsigned long long)clock64();
+  if (p.dbg && threadIdx.x == 0) p.dbg[(size_t)blockIdx.x * 16 + slot] = (unsigned long long)clock64();
+}
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
+// rows t < T, columns d < hd of one head slice (row r of the slice at src + r * row_stride) -> s[64][ld], zero padded to
+// 64 rows and round_up(hd, 8) columns
+__device__ __forceinline__ void load_slice(float* s, const float* src, long long row_stride, const AttnTcP& p) {
+  const int q = ((p.hd + 7) & ~7) >> 2;          // float4 per padded row
+  for (int v = threadIdx.x; v < TR * q; v += NTHR) {
+    const int r = v / q, c = 4 * (v - r * q);
+    float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (r < p.T && c < p.hd) x = __ldg(reinterpret_cast<const float4*>(src + r * row_stride + c));
+    *reinterpret_cast<float4*>(s + r * p.ld + c) = x;
   }
 }
 
-__device__ __forceinline__ void stamp_by(const AttnTcP& p, int slot, int tid) {
-  if (p.dbg && (int)threadIdx.x == tid) p.dbg[(size_t)blockIdx.x * 16 + slot] = (unsigned long long)clock64();
-}
-__device__ __forceinline__ float lo_of(float v) { return v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u); }
-
-// lo image (at +lo_off) of `bytes` bytes of hi image; same addresses, so the swizzle never has to be undone
-__device__ __forceinline__ void lo_pass(uint32_t hi, uint32_t lo_off, uint32_t bytes) {
-  lo_image<6>(hi, hi + lo_off, bytes / 16u, threadIdx.x, (uint32_t)NTHR);
-}
-
-// D[128 x N] (+)= A . B with error compensation.  Operand images: hi at base, lo at base + *_lo.
-//   KMAJOR operand: contraction over columns; k-step ks covers columns 8*ks..8*ks+7 (group ks/4, 32 bytes * (ks%4))
-//   MN operand:     contraction over rows;    k-step ks covers rows 8*ks..8*ks+7 (1024 bytes apart), groups GRP apart,
-//                   image in the 32-byte-atom swizzle
-// The four base descriptors are built once; a k-step only moves the 14-bit start-address field (units of 16 bytes), so
-// the single issuing thread spends a handful of instructions per MMA (building descriptors inside the loop made the
-// issue of 36 MMAs take 3 us -- one thread's dependent 64-bit arithmetic, not the tensor pipe).
-__device__ __forceinline__ void umma_tf32_split(uint32_t d_tmem, uint32_t a_lo32, uint32_t a_hi32, uint32_t b_lo32, uint32_t b_hi32,
-                                                uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_lo32), "r"(a_hi32), "r"(b_lo32), "r"(b_hi32), "r"(idesc), "r"(acc) : "memory");
-}
-template <bool A_MN, bool B_MN, int MAXK>
-__device__ __forceinline__ void mma3(uint32_t d_tmem, uint32_t a_, uint32_t a_lo, uint32_t b_, uint32_t b_lo, int ksteps_,
-                                     uint32_t idesc) {
-  // called by a whole (converged) warp; lane 0 issues.  The broadcasts tell the compiler the operands are warp-uniform,
-  // so the descriptors live in uniform registers instead of going through a per-MMA R2UR waterfall
-  const uint32_t a = __shfl_sync(0xffffffffu, a_, 0), b = __shfl_sync(0xffffffffu, b_, 0);
-  const int ksteps = __shfl_sync(0xffffffffu, ksteps_, 0);
-  const bool leader = (threadIdx.x & 31) == 0;
-  // descriptors as (low word, high word): only the low word (start address, 16-byte units) changes between MMAs
-  const uint64_t a0 = A_MN ? umma_desc_mn_sw128(0, GRP) : umma_desc_sw128(0);
-  const uint64_t b0 = B_MN ? umma_desc_mn_sw128(0, GRP) : umma_desc_sw128(0);
-  const uint32_t a_hi32 = (uint32_t)(a0 >> 32), b_hi32 = (uint32_t)(b0 >> 32);
-  const uint32_t ah = (uint32_t)a0 | ((a >> 4) & 0x3FFFu), al = (uint32_t)a0 | (((a + a_lo) >> 4) & 0x3FFFu);
-  const uint32_t bh = (uint32_t)b0 | ((b >> 4) & 0x3FFFu), bl = (uint32_t)b0 | (((b + b_lo) >> 4) & 0x3FFFu);
-#pragma unroll
-  for (int ks = 0; ks < MAXK; ++ks) {
-    if (ks < ksteps && leader) {
-      const uint32_t ao = A_MN ? (uint32_t)ks * 64u : (uint32_t)((ks >> 2) * (GRP >> 4) + (ks & 3) * 2);
-      const uint32_t bo = B_MN ? (uint32_t)ks * 64u : (uint32_t)((ks >> 2) * (GRP >> 4) + (ks & 3) * 2);
-      umma_tf32_split(d_tmem, al + ao, a_hi32, bh + bo, b_hi32, idesc, ks ? 1u : 0u);     // small terms first
-      umma_tf32_split(d_tmem, ah + ao, a_hi32, bl + bo, b_hi32, idesc, 1u);
-      umma_tf32_split(d_tmem, ah + ao, a_hi32, bh + bo, b_hi32, idesc, 1u);
-    }
-  }
-}
-
-// four consecutive values (columns 4c..4c+3) of this thread's row i of a [64 x 64] tile: hi -> tile, lo -> tile + PT
-__device__ __forceinline__ void store_chunk_hi_lo(uint32_t tile, int i, int c, float v0, float v1, float v2, float v3) {
-  const uint32_t off = (uint32_t)((c >> 3) * GRP + i * 128 + (((c & 7) ^ (i & 7)) << 4));
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile + off), "f"(v0), "f"(v1), "f"(v2), "f"(v3) : "memory");
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile + PT + off), "f"(lo_of(v0)), "f"(lo_of(v1)), "f"(lo_of(v2)),
-               "f"(lo_of(v3)) : "memory");
-}
-
-// same values into an image that is read column-wise (MN-major A operand): 32-byte-atom swizzle
-__device__ __forceinline__ void store_chunk_mn(uint32_t hi, uint32_t lo, int i, int c, float v0, float v1, float v2, float v3) {
-  const uint32_t off = (uint32_t)((c >> 3) * GRP) + mn_sw_offset(i, c & 7);
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(hi + off), "f"(v0), "f"(v1), "f"(v2), "f"(v3) : "memory");
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(lo + off), "f"(lo_of(v0)), "f"(lo_of(v1)), "f"(lo_of(v2)),
-               "f"(lo_of(v3)) : "memory");
-}
-
-// keep/scale factors (0 or 1/(1-p)) of the attention-dropout decisions (i, 4c..4c+3): index space [B, H, T, T]
-__device__ __forceinline__ float4 mask4(const AttnTcP& p, const RngKey& key, uint64_t row_base, int c, float ik) {
-  if (p.drop_p <= 0.f) return make_float4(1.f, 1.f, 1.f, 1.f);
-  if (4 * c >= p.T) return make_float4(0.f, 0.f, 0.f, 0.f);
-  if ((p.T & 3) == 0) return dropout_scale4(key, p.site, row_base + 4 * c, p.drop_p, ik);     // row_base % 4 == 0
-  float4 q;
-  q.x = dropout_scale(key, p.site, row_base + 4 * c, p.drop_p, ik);
-  q.y = 4 * c + 1 < p.T ? dropout_scale(key, p.site, row_base + 4 * c + 1, p.drop_p, ik) : 0.f;
-  q.z = 4 * c + 2 < p.T ? dropout_scale(key, p.site, row_base + 4 * c + 2, p.drop_p, ik) : 0.f;
-  q.w = 4 * c + 3 < p.T ? dropout_scale(key, p.site, row_base + 4 * c + 3, p.drop_p, ik) : 0.f;
-  return q;
-}
-
-// Attention-dropout keep bits, computed by all 128 threads while the tiles are still in flight: the counter-based
-// stream needs nothing but indices.  Thread t covers row t & 63, columns 32*(t >> 6) .. +31 (8 Philox blocks, four
-// independent ones in flight: a fully rolled loop is one 10-round dependent chain after another and took 2.8 us, a
-// fully unrolled one is 1600 instructions of straight-line code).  bit j of keep[r] = element (r, j) is kept.
-__device__ __forceinline__ void precompute_keep_bits(const AttnTcP& p, const RngKey& key, int b, int h, unsigned long long* keep) {
-  if (p.drop_p <= 0.f) return;
-  const int r = threadIdx.x & 63, half = threadIdx.x >> 6;
-  const uint64_t row_base = ((uint64_t)(b * p.H + h) * p.T + r) * p.T;
-  uint32_t bits = 0u;
-  if (r < p.T) {
+// acc[j] (16 rows from r0) += A . B over `ksteps` k-steps of 8, n8 tiles j < nt.
+//   A_T:  A[m][k] = sa[k * lda + m]  (else sa[m * lda + k])
+//   B_KN: B[k][n] = sb[k * ldb + n]  (else sb[n * ldb + k])
+template <int NTMAX, bool A_T, bool B_KN>
+__device__ __forceinline__ void mma_rows16(float (&acc)[NTMAX][4], const float* sa, int lda, int r0, const float* sb, int ldb,
+                                           int nt, int ksteps) {
+  const int g = (threadIdx.x & 31) >> 2, t = threadIdx.x & 3;
 #pragma unroll 1
-    for (int c0 = 0; c0 < 8; c0 += 4) {
+  for (int ks = 0; ks < ksteps; ++ks) {
+    const int k0 = ks * 8;
+    float x0, x1, x2, x3;
+    if (A_T) {
+      x0 = sa[(k0 + t) * lda + r0 + g]; x1 = sa[(k0 + t) * lda + r0 + g + 8];
+      x2 = sa[(k0 + t + 4) * lda + r0 + g]; x3 = sa[(k0 + t + 4) * lda + r0 + g + 8];
+    } else {
+      x0 = sa[(r0 + g) * lda + k0 + t]; x1 = sa[(r0 + g + 8) * lda + k0 + t];
+      x2 = sa[(r0 + g) * lda + k0 + t + 4]; x3 = sa[(r0 + g + 8) * lda + k0 + t + 4];
+    }
+    const uint32_t ah[4] = {tf32_hi(x0), tf32_hi(x1), tf32_hi(x2), tf32_hi(x3)};
+    const uint32_t al[4] = {tf32_lo(x0), tf32_lo(x1), tf32_lo(x2), tf32_lo(x3)};
 #pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const float4 m = mask4(p, key, row_base, 8 * half + c0 + u, 1.f);
-        bits |= ((m.x > 0.f ? 1u : 0u) | (m.y > 0.f ? 2u : 0u) | (m.z > 0.f ? 4u : 0u) | (m.w > 0.f ? 8u : 0u)) << (4 * (c0 + u));
+    for (int j = 0; j < NTMAX; ++j) {
+      if (j < nt) {
+        const int n = j * 8 + g;
+        const float y0 = B_KN ? sb[(k0 + t) * ldb + n] : sb[n * ldb + k0 + t];
+        const float y1 = B_KN ? sb[(k0 + t + 4) * ldb + n] : sb[n * ldb + k0 + t + 4];
+        mma_tf32x3(acc[j], ah, al, tf32_hi(y0), tf32_hi(y1), tf32_lo(y0), tf32_lo(y1));
       }
     }
   }
-  reinterpret_cast<uint32_t*>(keep)[2 * r + half] = bits;      // little-endian halves of the 64-bit row mask
 }
 
-// Row softmax in rolled passes over 16-column chunks of the accumulator row (re-read from TMEM each pass): the kernel
-// runs each phase once per CTA, so fully unrolled 64-wide code was instruction-fetch bound (~7 clocks per instruction).
-// exp(x - m) = ex2((x - m) * log2 e), one MUFU per element.
-struct RowStat { float mxs, inv; };      // max * (scale * log2 e), 1 / sum (0 for a padded row)
-__device__ __forceinline__ float row_max(uint32_t trow, int nv) {
-  float mx = -INFINITY;
-#pragma unroll 1
-  for (int cc = 0; cc < 4; ++cc) {
-    float v[16];
-    tmem_ld16(trow + 16 * cc, v);
+template <int NTMAX>
+__device__ __forceinline__ void zero(float (&acc)[NTMAX][4]) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) mx = fmaxf(mx, 16 * cc + j < nv ? v[j] : -INFINITY);
-  }
-  return mx;
+  for (int j = 0; j < NTMAX; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
 }
-__device__ __forceinline__ float exp_el(float v, float sl2, float mxs, bool valid) { return valid ? ex2_approx(fmaf(v, sl2, -mxs)) : 0.f; }
+
+// keep factor (0 or ik) of attention-dropout element (i, j): index space [B, H, T, T]
+__device__ __forceinline__ float keep_at(const AttnTcP& p, const RngKey& key, int b, int h, int i, int j, float ik) {
+  if (p.drop_p <= 0.f) return 1.f;
+  if (i >= p.T || j >= p.T) return 0.f;
+  return dropout_scale(key, p.site, ((uint64_t)(b * p.H + h) * p.T + i) * p.T + j, p.drop_p, ik);
+}
+
+// accumulator rows 16w + g (+8) of an [64 x hd] product -> dst row r at dst + r * row_stride, r < T, d < hd
+__device__ __forceinline__ void store_rows(const float (&acc)[HD_MAX / 8][4], float* dst, long long row_stride, int r0,
+                                           const AttnTcP& p) {
+  const int g = (threadIdx.x & 31) >> 2, t = threadIdx.x & 3;
+#pragma unroll
+  for (int j = 0; j < HD_MAX / 8; ++j) {
+    const int d = j * 8 + 2 * t;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = r0 + g + 8 * i;
+      if (r < p.T && d < p.hd)
+        *reinterpret_cast<float2*>(dst + r * row_stride + d) = make_float2(acc[j][2 * i], acc[j][2 * i + 1]);
+    }
+  }
+}
+
+// row statistics of the masked softmax over the two rows (16w + g, +8) this thread holds a quarter of
+struct RowStat { float mxs[2], sum[2]; };
+__device__ __forceinline__ RowStat row_stats(const float (&s)[TR / 8][4], int nv, float sl2) {
+  const int t = threadIdx.x & 3;
+  RowStat r;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < TR / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) if (j * 8 + 2 * t + e < nv) mx = fmaxf(mx, s[j][2 * i + e]);
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    r.mxs[i] = mx * sl2;
+    float sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < TR / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) if (j * 8 + 2 * t + e < nv) sum += ex2_approx(fmaf(s[j][2 * i + e], sl2, -r.mxs[i]));
+    sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+    r.sum[i] = sum;
+  }
+  return r;
+}
 
 // =================================================================================================
 // forward: ctx[t, b, h*hd + d] = sum_j dropout(softmax(scale * Q K^T))[t, j] V[j, d]
-//   shared memory: [Q | later V : hi, lo] [K | later P : hi, lo]  = 96 KB -> two CTAs per SM
 // =================================================================================================
-__global__ void __launch_bounds__(NTHR) attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV,
-                                                           const __grid_constant__ CUtensorMap tmQKVm, const AttnTcP p) {
-  extern __shared__ uint8_t smem_raw[];
+__global__ void __launch_bounds__(NTHR) attn_tc_fwd_kernel(const float* __restrict__ qkv, const AttnTcP p) {
+  extern __shared__ float sm[];
   pdl_launch_dependents();
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.x / p.H, h = blockIdx.x - b * p.H;
-  const uint32_t QV = base, KP = base + 2u * TILE;
-  const uint32_t bar = base + 4u * TILE;
-  const uint32_t bar_qk = bar, bar_v = bar + 8, bar_s = bar + 16, bar_o = bar + 24, tmem_slot = bar + 32;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  unsigned long long* keep = reinterpret_cast<unsigned long long*>(smem_raw + (bar + 64 - smem_u32(smem_raw)));   // [64]
-
-  if (warp == 0) {
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKV) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKVm) : "memory");
-      mbar_init(bar_qk, 1); mbar_init(bar_v, 1); mbar_init(bar_s, 1); mbar_init(bar_o, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
   pdl_wait();
-  const RngKey key = load_rng_key(p.drop_p > 0.f ? p.rng : nullptr);     // one read per thread (after the dependency wait: nothing global is touched before it)
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tS = tmem, tO = tmem + 64;
   stamp(p, 0);
-
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(bar_qk, 2u * TILE);
-#pragma unroll
-    for (int g = 0; g < NG; ++g) {
-      tma_load_5d(&tmQKV, bar_qk, QV + g * GRP, 32 * g, h, 0, b, 0);
-      tma_load_5d(&tmQKV, bar_qk, KP + g * GRP, 32 * g, h, 1, b, 0);
-    }
-  }
-  precompute_keep_bits(p, key, b, h, keep);
-  stamp(p, 1);
-  mbar_wait(bar_qk, 0);
-  stamp(p, 2);
-  lo_pass(QV, TILE, TILE);
-  lo_pass(KP, TILE, TILE);
-  fence_async_smem();
-  __syncthreads();
-  stamp(p, 3);
-  if (warp == 0) {
-    tc_fence_after();
-    mma3<false, false, 4 * NG>(tS, QV, TILE, KP, TILE, (p.hd + 7) >> 3, umma_idesc_tf32(128, 64, false, false));
-  }
-  if (threadIdx.x == 0) {
-    umma_commit(bar_s);
-    stamp(p, 4);
-    mbar_wait(bar_s, 0);                       // Q is dead: its region receives V
-    stamp(p, 5);
-    mbar_expect_tx(bar_v, (uint32_t)TILE);
-#pragma unroll
-    for (int g = 0; g < NG; ++g) tma_load_5d(&tmQKVm, bar_v, QV + g * GRP, 32 * g, h, 2, b, 0);     // MN image
-  }
-  // Lanes 1..31 of warp 0 must not run ahead of lane 0: divergent paths of one warp execute one at a time, so sibling
-  // lanes spinning on an mbarrier (or starting their softmax) would time-slice with the MMA issue loop and lane 0 would
-  // then redo the softmax alone.  Park them at a warp barrier instead.
-  __syncwarp();
-  if (warp < 2) {      // rows 0..63: masked softmax + dropout; P (hi, lo) replaces K in shared memory
-    const int i = threadIdx.x;
-    const long long len = p.lengths[b];
-    const int nv = (int)(len < p.T ? (len < 0 ? 0 : len) : p.T);
-    mbar_wait(bar_s, 0);
-    __syncwarp();
-    tc_fence_after();
-    const uint32_t trow = tS + ((uint32_t)(warp * 32) << 16);
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const float mxs = row_max(trow, nv) * sl2;
-    float sum = 0.f;
-#pragma unroll 1
-    for (int cc = 0; cc < 4; ++cc) {
-      float v[16];
-      tmem_ld16(trow + 16 * cc, v);
-#pragma unroll
-      for (int j = 0; j < 16; ++j) sum += exp_el(v[j], sl2, mxs, 16 * cc + j < nv);
-    }
-    const bool drop = p.drop_p > 0.f;
-    const float invk = ((i < p.T && nv > 0) ? 1.f / sum : 0.f) * (drop ? 1.f / (1.f - p.drop_p) : 1.f);
-    const unsigned long long bits = drop ? keep[i] : ~0ull;
-#pragma unroll 1
-    for (int cc = 0; cc < 4; ++cc) {      // P * keep / (1 - p): hi and lo images for O = P V
-      float v[16];
-      tmem_ld16(trow + 16 * cc, v);
-      const unsigned kb = (unsigned)(bits >> (16 * cc)) & 0xFFFFu;
-#pragma unroll
-      for (int c4 = 0; c4 < 4; ++c4) {
-        float o[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int j = 4 * c4 + q;
-          const float e = exp_el(v[j], sl2, mxs, 16 * cc + j < nv);
-          o[q] = (kb >> j) & 1u ? e * invk : 0.f;
-        }
-        store_chunk_hi_lo(KP, i, 4 * cc + c4, o[0], o[1], o[2], o[3]);
-      }
-    }
-    fence_async_smem();
-    stamp(p, 6);
-  } else {      // warps 2, 3 meanwhile: remainder image of V (it lands during the softmax)
-    mbar_wait(bar_v, 0);
-    stamp_by(p, 7, 64);
-    lo_image<6>(QV, QV + TILE, TILE / 16u, threadIdx.x - 64u, 64u);
-    fence_async_smem();
-  }
-  tc_fence_before();
-  __syncthreads();
-  stamp(p, 8);
-  if (warp == 0) {
-    tc_fence_after();
-    mma3<false, true, 8>(tO, KP, PT, QV, TILE, 8, umma_idesc_tf32(128, 96, false, true));
-  }
-  if (threadIdx.x == 0) {
-    umma_commit(bar_o);
-    stamp(p, 9);
-  }
-  __syncwarp();
-  if (warp < 2) {
-    const int i = threadIdx.x;
-    mbar_wait(bar_o, 0);
-    __syncwarp();
-    stamp(p, 10);
-    tc_fence_after();
-    float* dst = p.ctx + ((long long)i * p.B + b) * p.D + h * p.hd;
-#pragma unroll
-    for (int ch = 0; ch < NG; ++ch) {
-      uint32_t v[32];
-      tmem_ld32(tO + ((uint32_t)(warp * 32) << 16) + ch * 32, v);
-      if (i < p.T) {
-#pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const int d = ch * 32 + 4 * q4;
-          if (d < p.hd) *reinterpret_cast<uint4*>(dst + d) = make_uint4(v[4 * q4], v[4 * q4 + 1], v[4 * q4 + 2], v[4 * q4 + 3]);
-        }
-      }
-    }
-  }
-  stamp(p, 11);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem) : "memory");
-  }
-  stamp(p, 12);
-}
-
-// =================================================================================================
-// backward (plan in the header comment)
-// =================================================================================================
-__global__ void __launch_bounds__(NTHR) attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV,
-                                                           const __grid_constant__ CUtensorMap tmQKVm,
-                                                           const __grid_constant__ CUtensorMap tmDO,
-                                                           const __grid_constant__ CUtensorMap tmDOm, const AttnTcP p) {
-  extern __shared__ uint8_t smem_raw[];
-  pdl_launch_dependents();
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x / p.H, h = blockIdx.x - b * p.H;
-  constexpr uint32_t REG = 2u * TILE;                              // 48 KB: hi + lo image of one head slice
-  const uint32_t R0 = base, R1 = base + REG, R2 = base + 2u * REG, R3 = base + 3u * REG;
-  const uint32_t Pd = R0, Pd_lo = R0 + PT;                         // MN image
-  const uint32_t dSk = R1;                                         // K-major image (hi, lo = +PT)
-  const uint32_t dSm = R0 + 2u * PT, dSm_lo = R1 + 2u * PT;        // MN image in the two region tails
-  const uint32_t bar = R3 + REG + GRP;                             // GRP bytes of pad: M = 128 over-read of the last region
-  const uint32_t bar_qk = bar, bar_gv = bar + 8, bar_s = bar + 16, bar_dp = bar + 24, bar_m1 = bar + 32, bar_2 = bar + 40,
-                 bar_m2 = bar + 48, bar_out = bar + 56, tmem_slot = bar + 64;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  unsigned long long* keep = reinterpret_cast<unsigned long long*>(smem_raw + (bar + 128 - smem_u32(smem_raw)));  // [64]
-
-  if (warp == 0) {
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKV) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQKVm) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmDO) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmDOm) : "memory");
-      for (int k = 0; k < 8; ++k) mbar_init(bar + 8u * k, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  pdl_wait();
+  const int w = threadIdx.x >> 5, g = (threadIdx.x & 31) >> 2, t = threadIdx.x & 3;
+  float* sQ = sm; float* sK = sQ + TR * p.ld; float* sV = sK + TR * p.ld; float* sP = sV + TR * p.ld;
+  const long long rs = (long long)p.B * 3 * p.D;
+  const float* base = qkv + (long long)b * 3 * p.D + h * p.hd;
+  load_slice(sQ, base, rs, p);
+  load_slice(sK, base + p.D, rs, p);
+  load_slice(sV, base + 2 * p.D, rs, p);
   const RngKey key = load_rng_key(p.drop_p > 0.f ? p.rng : nullptr);
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t tS = tmem, tDP = tmem + 64, tDV = tmem + 128, tDQ = tmem + 224, tDK = tmem + 320;
-  stamp(p, 0);
+  const long long len = p.lengths[b];
+  const int nv = (int)(len < p.T ? (len < 0 ? 0 : len) : p.T);
+  const int ksd = (p.hd + 7) >> 3;
+  __syncthreads();
 
-  // ---- phase 1: K-major images of Q, K, V, dO; S = Q K^T and dP = dO V^T ---------------------------
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(bar_qk, 2u * TILE);
+  float s[TR / 8][4];
+  zero(s);
+  mma_rows16<TR / 8, false, false>(s, sQ, p.ld, 16 * w, sK, p.ld, TR / 8, ksd);
+  const float sl2 = p.scale * 1.4426950408889634f;
+  const RowStat st = row_stats(s, nv, sl2);
+  const float ik = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
 #pragma unroll
-    for (int g = 0; g < NG; ++g) {
-      tma_load_5d(&tmQKV, bar_qk, R0 + g * GRP, 32 * g, h, 0, b, 0);
-      tma_load_5d(&tmQKV, bar_qk, R1 + g * GRP, 32 * g, h, 1, b, 0);
-    }
-    mbar_expect_tx(bar_gv, 2u * TILE);
+  for (int i = 0; i < 2; ++i) {
+    const int r = 16 * w + g + 8 * i;
+    const float invk = ((r < p.T && nv > 0) ? 1.f / st.sum[i] : 0.f);
 #pragma unroll
-    for (int g = 0; g < NG; ++g) {
-      tma_load_5d(&tmQKV, bar_gv, R2 + g * GRP, 32 * g, h, 2, b, 0);
-      tma_load_4d(&tmDO, bar_gv, R3 + g * GRP, 32 * g, h, b, 0);
-    }
-  }
-  precompute_keep_bits(p, key, b, h, keep);
-  mbar_wait(bar_qk, 0);
-  stamp(p, 1);
-  lo_pass(R0, TILE, TILE);
-  lo_pass(R1, TILE, TILE);
-  fence_async_smem();
-  __syncthreads();
-  if (warp == 0) {     // recompute the scores
-    tc_fence_after();
-    mma3<false, false, 4 * NG>(tS, R0, TILE, R1, TILE, (p.hd + 7) >> 3, umma_idesc_tf32(128, 64, false, false));
-  }
-  if (threadIdx.x == 0) {
-    umma_commit(bar_s);
-    stamp(p, 2);
-  }
-  __syncwarp();        // (see the forward kernel: sibling lanes must not spin while lane 0 issues MMAs)
-  mbar_wait(bar_gv, 0);
-  lo_pass(R2, TILE, TILE);
-  lo_pass(R3, TILE, TILE);
-  fence_async_smem();
-  __syncthreads();
-  if (warp == 0) {     // dPd[i, j] = sum_d dO[i, d] V[j, d]
-    tc_fence_after();
-    mma3<false, false, 4 * NG>(tDP, R3, TILE, R2, TILE, (p.hd + 7) >> 3, umma_idesc_tf32(128, 64, false, false));
-  }
-  if (threadIdx.x == 0) {
-    umma_commit(bar_dp);
-    stamp(p, 3);
-    // every phase-1 image is dead once both accumulators are complete: fetch the MN images of dO and K
-    mbar_wait(bar_s, 0);
-    mbar_wait(bar_dp, 0);
-    stamp(p, 4);
-    mbar_expect_tx(bar_m1, 2u * TILE);
+    for (int j = 0; j < TR / 8; ++j) {
+      float o[2];
 #pragma unroll
-    for (int g = 0; g < NG; ++g) {
-      tma_load_4d(&tmDOm, bar_m1, R2 + g * GRP, 32 * g, h, b, 0);
-      tma_load_5d(&tmQKVm, bar_m1, R3 + g * GRP, 32 * g, h, 1, b, 0);
-    }
-  }
-  __syncwarp();
-  // ---- phase 2: softmax / dS math on rows 0..63, Pd and dS images into R0 / R1 ----------------------
-  if (warp < 2) {
-    const int i = threadIdx.x;
-    const long long len = p.lengths[b];
-    const int nv = (int)(len < p.T ? (len < 0 ? 0 : len) : p.T);
-    const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-    mbar_wait(bar_s, 0);
-    __syncwarp();
-    tc_fence_after();
-    const uint32_t srow = tS + lane_addr, drow = tDP + lane_addr;
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const float mxs = row_max(srow, nv) * sl2;
-    mbar_wait(bar_dp, 0);                            // Q, K, V, dO images are dead from here on
-    __syncwarp();
-    tc_fence_after();
-    const bool drop = p.drop_p > 0.f;
-    const float ik = drop ? 1.f / (1.f - p.drop_p) : 1.f;
-    const unsigned long long bits = drop ? keep[i] : ~0ull;
-    float sum = 0.f, dotr = 0.f;
-#pragma unroll 1
-    for (int cc = 0; cc < 4; ++cc) {      // sum of exponentials and rowsum(dP * P) (un-normalised) in one pass
-      float v[16], g[16];
-      tmem_ld16(srow + 16 * cc, v);
-      tmem_ld16(drow + 16 * cc, g);
-      const unsigned kb = (unsigned)(bits >> (16 * cc)) & 0xFFFFu;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float e = exp_el(v[j], sl2, mxs, 16 * cc + j < nv);
-        sum += e;
-        dotr += (kb >> j) & 1u ? g[j] * e : 0.f;
+      for (int e = 0; e < 2; ++e) {
+        const int c = j * 8 + 2 * t + e;
+        const float ex = c < nv ? ex2_approx(fmaf(s[j][2 * i + e], sl2, -st.mxs[i])) : 0.f;
+        o[e] = (ex != 0.f && invk != 0.f) ? ex * invk * keep_at(p, key, b, h, r, c, ik) : 0.f;
       }
-    }
-    const float inv = (i < p.T && nv > 0) ? 1.f / sum : 0.f;
-    const float dot = dotr * ik * inv;
-#pragma unroll 1
-    for (int cc = 0; cc < 4; ++cc) {
-      float v[16], g[16];
-      tmem_ld16(srow + 16 * cc, v);
-      tmem_ld16(drow + 16 * cc, g);
-      const unsigned kb = (unsigned)(bits >> (16 * cc)) & 0xFFFFu;
-#pragma unroll
-      for (int c4 = 0; c4 < 4; ++c4) {
-        float pd[4], ds[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int j = 4 * c4 + q;
-          const float pr = exp_el(v[j], sl2, mxs, 16 * cc + j < nv) * inv;      // probability
-          const float m = (kb >> j) & 1u ? ik : 0.f;
-          pd[q] = pr * m;                                                        // Pd = P * mask (read column-wise by dV)
-          ds[q] = pr * (g[j] * m - dot) * p.scale;                               // scale * dS = scale * P * (dP - rowsum(dP * P))
-        }
-        const int c = 4 * cc + c4;
-        store_chunk_mn(Pd, Pd_lo, i, c, pd[0], pd[1], pd[2], pd[3]);
-        store_chunk_hi_lo(dSk, i, c, ds[0], ds[1], ds[2], ds[3]);                // row-wise image (dQ = dS K)
-        store_chunk_mn(dSm, dSm_lo, i, c, ds[0], ds[1], ds[2], ds[3]);           // column-wise image (dK = dS^T Q)
-      }
-    }
-    fence_async_smem();
-    stamp(p, 5);
-  } else {      // warps 2, 3 have no accumulator rows: they derive the remainder images of the MN tiles meanwhile
-    mbar_wait(bar_m1, 0);
-    stamp_by(p, 6, 64);
-    lo_image<6>(R2, R2 + TILE, TILE / 16u, threadIdx.x - 64u, 64u);
-    lo_image<6>(R3, R3 + TILE, TILE / 16u, threadIdx.x - 64u, 64u);
-    fence_async_smem();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    // dV[j, d] = sum_i Pd[i, j] dO[i, d]        A = Pd read column-wise (MN-major), B = dO (MN-major)
-    mma3<true, true, 8>(tDV, Pd, PT, R2, TILE, 8, umma_idesc_tf32(128, 96, true, true));
-    // dQ[i, d] = sum_j (scale dS)[i, j] K[j, d]
-    mma3<false, true, 8>(tDQ, dSk, PT, R3, TILE, 8, umma_idesc_tf32(128, 96, false, true));
-  }
-  if (threadIdx.x == 0) {
-    umma_commit(bar_2);
-    stamp(p, 7);
-    mbar_wait(bar_2, 0);                 // the dO image is dead: its region receives Q (MN image)
-    mbar_expect_tx(bar_m2, (uint32_t)TILE);
-#pragma unroll
-    for (int g = 0; g < NG; ++g) tma_load_5d(&tmQKVm, bar_m2, R2 + g * GRP, 32 * g, h, 0, b, 0);
-    stamp(p, 8);
-  }
-  __syncwarp();
-  auto store_out = [&](uint32_t t0, int which) {     // accumulator rows 0..63 -> d_qkv[t, b, which*D + h*hd + d]
-    const int i = threadIdx.x;
-    float* dst = p.dqkv + ((long long)i * p.B + b) * 3 * p.D + h * p.hd + which * p.D;
-#pragma unroll
-    for (int ch = 0; ch < NG; ++ch) {
-      uint32_t v[32];
-      tmem_ld32(t0 + ((uint32_t)(warp * 32) << 16) + ch * 32, v);
-      if (i < p.T) {
-#pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const int d = ch * 32 + 4 * q4;
-          if (d < p.hd) *reinterpret_cast<uint4*>(dst + d) = make_uint4(v[4 * q4], v[4 * q4 + 1], v[4 * q4 + 2], v[4 * q4 + 3]);
-        }
-      }
-    }
-  };
-  if (warp < 2) {                        // dQ and dV leave while warps 2, 3 prepare and issue the last product
-    mbar_wait(bar_2, 0);
-    __syncwarp();
-    tc_fence_after();
-    store_out(tDQ, 0);
-    store_out(tDV, 2);
-    stamp(p, 9);
-  } else {
-    // ---- phase 3: dK[j, d] = sum_i (scale dS)[i, j] Q[i, d] -------------------------------------------
-    mbar_wait(bar_m2, 0);
-    stamp_by(p, 10, 64);
-    lo_image<6>(R2, R2 + TILE, TILE / 16u, threadIdx.x - 64u, 64u);
-    fence_async_smem();
-    asm volatile("bar.sync 1, 64;" ::: "memory");      // warps 2 and 3
-    if (warp == 2) {
-      tc_fence_after();
-      mma3<true, true, 8>(tDK, dSm, dSm_lo - dSm, R2, TILE, 8, umma_idesc_tf32(128, 96, true, true));
-      if (lane == 0) umma_commit(bar_out);
-      stamp_by(p, 11, 64);
-      __syncwarp();
+      *reinterpret_cast<float2*>(sP + r * LDP + j * 8 + 2 * t) = make_float2(o[0], o[1]);
     }
   }
-  if (warp < 2) {
-    mbar_wait(bar_out, 0);
-    __syncwarp();
-    tc_fence_after();
-    store_out(tDK, 1);
-  }
+  __syncwarp();           // O rows 16w.. read only this warp's probability rows (V is complete since the barrier)
+  float o[HD_MAX / 8][4];
+  zero(o);
+  mma_rows16<HD_MAX / 8, false, true>(o, sP, LDP, 16 * w, sV, p.ld, ksd, TR / 8);
+  store_rows(o, p.ctx + (long long)b * p.D + h * p.hd, (long long)p.B * p.D, 16 * w, p);
   stamp(p, 12);
-  tc_fence_before();
+}
+
+// =================================================================================================
+// backward
+// =================================================================================================
+__global__ void __launch_bounds__(NTHR) attn_tc_bwd_kernel(const float* __restrict__ qkv, const float* __restrict__ dctx,
+                                                           const AttnTcP p) {
+  extern __shared__ float sm[];
+  pdl_launch_dependents();
+  pdl_wait();
+  stamp(p, 0);
+  const int b = blockIdx.x / p.H, h = blockIdx.x - b * p.H;
+  const int w = threadIdx.x >> 5, g = (threadIdx.x & 31) >> 2, t = threadIdx.x & 3;
+  float* sQ = sm; float* sK = sQ + TR * p.ld; float* sV = sK + TR * p.ld; float* sG = sV + TR * p.ld;
+  // V is dead once dP = dO V^T is formed: the masked probabilities Pd take its place when they fit there
+  float* sS = sG + TR * p.ld; float* sPd = p.ld >= LDP ? sV : sS + TR * LDP;
+  const long long rs = (long long)p.B * 3 * p.D;
+  const float* base = qkv + (long long)b * 3 * p.D + h * p.hd;
+  load_slice(sQ, base, rs, p);
+  load_slice(sK, base + p.D, rs, p);
+  load_slice(sV, base + 2 * p.D, rs, p);
+  load_slice(sG, dctx + (long long)b * p.D + h * p.hd, (long long)p.B * p.D, p);
+  const RngKey key = load_rng_key(p.drop_p > 0.f ? p.rng : nullptr);
+  const long long len = p.lengths[b];
+  const int nv = (int)(len < p.T ? (len < 0 ? 0 : len) : p.T);
+  const int ksd = (p.hd + 7) >> 3;
   __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
+
+  {
+    float s[TR / 8][4], dp[TR / 8][4];
+    zero(s); zero(dp);
+    mma_rows16<TR / 8, false, false>(s, sQ, p.ld, 16 * w, sK, p.ld, TR / 8, ksd);     // recompute the scores
+    mma_rows16<TR / 8, false, false>(dp, sG, p.ld, 16 * w, sV, p.ld, TR / 8, ksd);    // dPd[i, j] = sum_d dO[i, d] V[j, d]
+    __syncthreads();      // every warp has read V (Pd may overwrite it below)
+    const float sl2 = p.scale * 1.4426950408889634f;
+    const RowStat st = row_stats(s, nv, sl2);
+    const float ik = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = 16 * w + g + 8 * i;
+      const float inv = (r < p.T && nv > 0) ? 1.f / st.sum[i] : 0.f;
+      float pr[TR / 8][2], m[TR / 8][2];
+      float dot = 0.f;                 // rowsum(dP * P) with dP = dPd * mask
+#pragma unroll
+      for (int j = 0; j < TR / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = j * 8 + 2 * t + e;
+          pr[j][e] = c < nv ? ex2_approx(fmaf(s[j][2 * i + e], sl2, -st.mxs[i])) * inv : 0.f;
+          m[j][e] = pr[j][e] != 0.f ? keep_at(p, key, b, h, r, c, ik) : 0.f;
+          dot += dp[j][2 * i + e] * m[j][e] * pr[j][e];
+        }
+      dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+      dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+#pragma unroll
+      for (int j = 0; j < TR / 8; ++j) {
+        const int c = j * 8 + 2 * t;
+        *reinterpret_cast<float2*>(sPd + r * LDP + c) = make_float2(pr[j][0] * m[j][0], pr[j][1] * m[j][1]);   // Pd = P * mask
+        *reinterpret_cast<float2*>(sS + r * LDP + c) =                                                       // scale * dS
+            make_float2(pr[j][0] * (dp[j][2 * i] * m[j][0] - dot) * p.scale, pr[j][1] * (dp[j][2 * i + 1] * m[j][1] - dot) * p.scale);
+      }
+    }
   }
+  __syncthreads();        // dV and dK contract over all rows i of Pd / dS
+  float acc[HD_MAX / 8][4];
+  float* out = p.dqkv + (long long)b * 3 * p.D + h * p.hd;
+  // dV[j, d] = sum_i Pd[i, j] dO[i, d]
+  zero(acc);
+  mma_rows16<HD_MAX / 8, true, true>(acc, sPd, LDP, 16 * w, sG, p.ld, ksd, TR / 8);
+  store_rows(acc, out + 2 * p.D, rs, 16 * w, p);
+  // dQ[i, d] = sum_j (scale dS)[i, j] K[j, d]
+  zero(acc);
+  mma_rows16<HD_MAX / 8, false, true>(acc, sS, LDP, 16 * w, sK, p.ld, ksd, TR / 8);
+  store_rows(acc, out, rs, 16 * w, p);
+  // dK[j, d] = sum_i (scale dS)[i, j] Q[i, d]
+  zero(acc);
+  mma_rows16<HD_MAX / 8, true, true>(acc, sS, LDP, 16 * w, sQ, p.ld, ksd, TR / 8);
+  store_rows(acc, out + p.D, rs, 16 * w, p);
+  stamp(p, 12);
 }
 
-constexpr int FWD_SMEM = 1024 + 4 * TILE + 64 + 512;
-constexpr int BWD_SMEM = 1024 + 8 * TILE + GRP + 128 + 512;
-
-// qkv viewed as [T, B, 3, H, hd]: box = 32 columns x 64 timestamps of one (sample, q/k/v, head)
-int encode_qkv(CUtensorMap* m, const float* qkv, int B, int H, int T, int hd, CUtensorMapSwizzle sw) {
-  const cuuint64_t D = (cuuint64_t)H * hd;
-  cuuint64_t dims[5] = {(cuuint64_t)hd, (cuuint64_t)H, 3, (cuuint64_t)B, (cuuint64_t)T};
-  cuuint64_t str[4] = {(cuuint64_t)hd * 4, D * 4, 3 * D * 4, (cuuint64_t)B * 3 * D * 4};
-  cuuint32_t box[5] = {32, 1, 1, 1, TR};
-  return encode(m, qkv, 5, dims, str, box, sw, "attention qkv");
-}
-int encode_ctx(CUtensorMap* m, const float* x, int B, int H, int T, int hd, CUtensorMapSwizzle sw) {
-  const cuuint64_t D = (cuuint64_t)H * hd;
-  cuuint64_t dims[4] = {(cuuint64_t)hd, (cuuint64_t)H, (cuuint64_t)B, (cuuint64_t)T};
-  cuuint64_t str[3] = {(cuuint64_t)hd * 4, D * 4, (cuuint64_t)B * D * 4};
-  cuuint32_t box[4] = {32, 1, 1, TR};
-  return encode(m, x, 4, dims, str, box, sw, "attention d(ctx)");
-}
+int slice_ld(int hd) { return ((hd + 7) & ~7) + 4; }
+int fwd_smem(int hd) { return (3 * TR * slice_ld(hd) + TR * LDP) * (int)sizeof(float); }
+int bwd_smem(int hd) { return (4 * TR * slice_ld(hd) + (slice_ld(hd) >= LDP ? 1 : 2) * TR * LDP) * (int)sizeof(float); }
 
 }  // namespace
 
@@ -606,7 +289,7 @@ void attn_tc_set_debug(unsigned long long* buf) { g_attn_dbg = buf; }
 bool attn_tc_supported(int T, int hd) {
   static int env = -1;
   if (env < 0) { const char* e = getenv("RD_ATTN_TC"); env = (e && e[0] == '0') ? 0 : 1; }
-  return env == 1 && T <= TR && hd <= 32 * NG && hd % 4 == 0 && hd >= 4;
+  return env == 1 && T <= TR && hd <= HD_MAX && hd % 4 == 0 && hd >= 4;
 }
 
 int attn_tc_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p, const uint64_t* rng,
@@ -616,13 +299,10 @@ int attn_tc_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, i
     return -2;
   }
   AttnTcP p{};
-  p.ctx = ctx; p.lengths = lengths; p.B = B; p.H = H; p.T = T; p.hd = hd; p.D = H * hd;
+  p.ctx = ctx; p.lengths = lengths; p.B = B; p.H = H; p.T = T; p.hd = hd; p.D = H * hd; p.ld = slice_ld(hd);
   p.scale = 1.f / sqrtf((float)hd); p.drop_p = drop_p; p.rng = rng; p.site = site; p.dbg = g_attn_dbg;
-  CUtensorMap tm, tmm;
-  RD_TRY(encode_qkv(&tm, qkv, B, H, T, hd, CU_TENSOR_MAP_SWIZZLE_128B));
-  RD_TRY(encode_qkv(&tmm, qkv, B, H, T, hd, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B));
-  RD_TRY(ensure_max_smem((const void*)attn_tc_fwd_kernel, FWD_SMEM));
-  launch_pdl(attn_tc_fwd_kernel, dim3(B * H), dim3(NTHR), FWD_SMEM, st, tm, tmm, p);
+  RD_TRY(ensure_max_smem((const void*)attn_tc_fwd_kernel, fwd_smem(HD_MAX)));
+  launch_pdl(attn_tc_fwd_kernel, dim3(B * H), dim3(NTHR), fwd_smem(hd), st, qkv, p);
   RD_CHECK_LAUNCH("attn_tc_fwd_kernel");
   return 0;
 }
@@ -635,15 +315,10 @@ int attn_tc_bwd(const float* qkv, const float* dctx, const int64_t* lengths, int
     return -2;
   }
   AttnTcP p{};
-  p.dqkv = dqkv; p.lengths = lengths; p.B = B; p.H = H; p.T = T; p.hd = hd; p.D = H * hd;
+  p.dqkv = dqkv; p.lengths = lengths; p.B = B; p.H = H; p.T = T; p.hd = hd; p.D = H * hd; p.ld = slice_ld(hd);
   p.scale = 1.f / sqrtf((float)hd); p.drop_p = drop_p; p.rng = rng; p.site = site; p.dbg = g_attn_dbg;
-  CUtensorMap tq, tqm, tg, tgm;
-  RD_TRY(encode_qkv(&tq, qkv, B, H, T, hd, CU_TENSOR_MAP_SWIZZLE_128B));
-  RD_TRY(encode_qkv(&tqm, qkv, B, H, T, hd, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B));
-  RD_TRY(encode_ctx(&tg, dctx, B, H, T, hd, CU_TENSOR_MAP_SWIZZLE_128B));
-  RD_TRY(encode_ctx(&tgm, dctx, B, H, T, hd, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B));
-  RD_TRY(ensure_max_smem((const void*)attn_tc_bwd_kernel, BWD_SMEM));
-  launch_pdl(attn_tc_bwd_kernel, dim3(B * H), dim3(NTHR), BWD_SMEM, st, tq, tqm, tg, tgm, p);
+  RD_TRY(ensure_max_smem((const void*)attn_tc_bwd_kernel, bwd_smem(HD_MAX)));
+  launch_pdl(attn_tc_bwd_kernel, dim3(B * H), dim3(NTHR), bwd_smem(hd), st, qkv, dctx, p);
   RD_CHECK_LAUNCH("attn_tc_bwd_kernel");
   return 0;
 }

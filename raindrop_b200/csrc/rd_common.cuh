@@ -1,4 +1,4 @@
-// Shared device/host helpers for librd_b200 (sm_100a only).
+// Shared device/host helpers for librd_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,11 +28,10 @@ int check_launch(const char* what);  // cudaPeekAtLastError -> 0 / -1
 // A training step is ~40 dependent launches of 5-20 us each, so the ~2 us between "last CTA of kernel N exits" and
 // "first CTA of kernel N+1 runs" is ~10 % of the step.  Kernels launched through launch_pdl() may be scheduled as soon
 // as every CTA of the previous kernel has executed pdl_launch_dependents() (first instruction of our kernels): their
-// CTAs take free SMs, run their prologue (barrier init, TMEM allocation, tensor-map prefetch) and then block in
+// CTAs take free SMs, run their prologue (barrier init, tensor-map prefetch) and then block in
 // pdl_wait() until the previous kernel has COMPLETED and flushed its writes.  Every kernel calls pdl_wait() before its
 // first global read of produced data and before its first global write, so the dependency semantics are unchanged.
-// Stream capture records these as programmatic edges.  Measured on B200 (P19 B=128, graph replay): 0.698 ms with vs
-// 0.692 ms without -- inside a graph the launches are already back to back -- so it is OFF unless RD_PDL=1.
+// Stream capture records these as programmatic edges.  On by default; RD_PDL=0 turns it off (rd_kernels.cu).
 bool pdl_enabled();
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

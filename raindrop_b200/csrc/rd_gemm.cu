@@ -1,7 +1,7 @@
 // Generic strided/batched fp32 GEMM (CUDA cores) with a fused epilogue, plus the small reductions
 // that go with it (split-K reduce, column sums).  Used for every contraction whose accuracy budget
 // rules out single-pass TF32 (temporal attention, head) and for the weight-gradient reductions;
-// the observation-propagation forward has its own tcgen05 kernel (rd_obprop_tc.cu).
+// the observation-propagation forward has its own tensor-core kernel (rd_obprop_tc.cu).
 #include "rd_common.cuh"
 
 namespace rd {
@@ -179,7 +179,7 @@ __global__ void colsum_partial_kernel(const float* __restrict__ x, long long row
 
 int64_t gemm_splitk_plan(int M, int N, int K, int* nsplit) {
   int64_t tiles = ceil_div(M, BM) * ceil_div(N, BN);
-  int ns = (int)ceil_div(2 * 148, tiles);
+  int ns = (int)ceil_div(2 * 132, tiles);   // two CTAs per SM of an H100
   int maxs = (int)ceil_div(K, 4 * BK);  // at least 64 reduction steps per split
   if (ns > maxs) ns = maxs;
   if (ns > 256) ns = 256;

@@ -23,9 +23,8 @@ static unsigned long long g_launches = 0;
 unsigned long long launch_count() { return g_launches; }
 bool pdl_enabled() {
   static int v = -1;
-  // programmatic dependent launch: a kernel's prologue (barrier init, TMEM allocation, descriptor prefetch) overlaps the tail
-  // of its predecessor; every kernel waits (griddepcontrol.wait) before it touches global memory.  0.539 -> 0.518 ms per
-  // P19 step inside the graph (it measured at no gain before the kernels were shortened).  RD_PDL=0 turns it off.
+  // programmatic dependent launch: a kernel's prologue (barrier init, descriptor prefetch) overlaps the tail of its
+  // predecessor; every kernel waits (griddepcontrol.wait) before it touches global memory.  RD_PDL=0 turns it off.
   if (v < 0) { const char* e = getenv("RD_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
   return v == 1;
 }
@@ -950,9 +949,9 @@ int cross_entropy(const float* logits, const int64_t* y, int B, int ncls, float*
 int adam(float* p, const float* g, float* m, float* v, int64_t n, float lr, const float* lr_dev, float b1, float b2,
          float eps, float gscale, int64_t* step, cudaStream_t st) {
   const int vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15) == 0;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   long long blocks = ceil_div(n, (int64_t)TPB * 4);
   if (blocks > 4LL * sms) blocks = 4LL * sms;
   if (blocks < 1) blocks = 1;

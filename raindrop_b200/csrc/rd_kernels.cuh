@@ -77,9 +77,9 @@ int attn_small_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T
 int attn_small_bwd(const float* qkv, const float* dctx, const int64_t* lengths, int B, int H, int T, int hd,
                    float drop_p, const uint64_t* rng, uint32_t site, float* dqkv, cudaStream_t st);
 
-// the same on the tensor cores (rd_attn_tc.cu: tcgen05 3xTF32, TMA-staged head slices, T <= 64, hd <= 96, hd % 4 == 0)
+// the same on the tensor cores (rd_attn_tc.cu: mma.sync 3xTF32, T <= 64, hd <= 96, hd % 4 == 0)
 bool attn_tc_supported(int T, int hd);
-void attn_tc_set_debug(unsigned long long* buf);   // phase timestamps of the forward kernel: [CTA][16] (debug)
+void attn_tc_set_debug(unsigned long long* buf);   // start / end clock64 stamps per CTA: [CTA][16], slots 0 and 12 (debug)
 int attn_tc_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p,
                 const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st);
 int attn_tc_bwd(const float* qkv, const float* dctx, const int64_t* lengths, int B, int H, int T, int hd,

@@ -241,7 +241,7 @@ static bool linear_nt_is_tc(const GemmP& g, const float* W_lo) {
 }
 
 // ---- observation propagation layer (operator level) ---------------------------------------------
-// Forward goes to the tcgen05 kernel when the shape fits its tiling, otherwise to the generic
+// Forward goes to the tensor-core kernel when the shape fits its tiling, otherwise to the generic
 // CUDA-core GEMM (same epilogue).
 static int obprop_forward(const ObpropTcArgs& a, cudaStream_t st) {
   if (obprop_tc_supported(a.C) && (!a.perm || a.pdob == 4)) return obprop_tc_fwd(a, st);

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA kernel for one observation-propagation layer (rd_obprop_tc.cu).
+// Tensor-core (wgmma + TMA) path of one observation-propagation layer (rd_obprop_tc.cu).
 #pragma once
 #include "rd_common.cuh"
 
@@ -8,7 +8,7 @@ namespace rd {
 bool obprop_tc_supported(int C);
 
 // out[r, :] = epi(x[r, :] . W^T), W: [C, C] row-major ([out, in]); TF32 operands, fp32 accumulation
-// in TMEM.  The tensor core reads the top 19 bits of each fp32 operand (truncation), so callers
+// in registers.  The tensor core reads the top 19 bits of each fp32 operand (truncation), so callers
 // hand in operands that are already rounded to TF32 (round_tf32 below / round_out of the producing
 // layer); then the truncation is exact and the only error is the unbiased RN rounding.
 //   epi(v) = [relu](v + bias[c]) * scale[r % mod] * [gate[r, c] > 0], optionally RN-rounded to TF32

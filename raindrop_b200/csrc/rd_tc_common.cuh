@@ -1,5 +1,5 @@
-// Shared device-side PTX wrappers (mbarrier, TMA, tcgen05, TMEM) and host-side tensor-map helpers of
-// the tensor-core kernels (rd_obprop_tc.cu, rd_tc_gemm.cu).  sm_100a only.
+// Shared device-side PTX wrappers (mbarrier, TMA, wgmma, mma.sync) and host-side tensor-map helpers of
+// the tensor-core kernels (rd_obprop_tc.cu, rd_tc_gemm.cu, rd_attn_tc.cu).  sm_90a.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -47,140 +47,66 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint32_t bar
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint32_t bar, uint32_t dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+// 16-byte asynchronous global -> shared copy; src_bytes < 16 zero-fills the rest (0: a zero vector, nothing is read)
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ void tma_load_5d(const CUtensorMap* map, uint32_t bar, uint32_t dst, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
-__device__ __forceinline__ void bulk_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
+// ---- split of an fp32 operand for the error-compensated ("3xTF32") products ----------------------------------------
+// hi = the top 19 bits (exactly representable in TF32), lo = x - hi (exact).  hi*hi + hi*lo + lo*hi reproduces the fp32
+// product to ~2^-22 relative, independent of how the tensor core converts a raw fp32 bit pattern.
+__device__ __forceinline__ uint32_t tf32_hi(float x) { return __float_as_uint(x) & 0xFFFFE000u; }
+__device__ __forceinline__ uint32_t tf32_lo(float x) { return __float_as_uint(x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u)); }
+
+// ---- warp-level tensor-core MMA: D[16x8] += A[16x8] . B[8x8], TF32 operands, fp32 accumulate -------------------------
+// fragments (g = lane / 4, t = lane % 4):  a0 (g, t)  a1 (g+8, t)  a2 (g, t+4)  a3 (g+8, t+4)
+//                                          b0 (k=t, n=g)  b1 (k=t+4, n=g)
+//                                          d0 (g, 2t)  d1 (g, 2t+1)  d2 (g+8, 2t)  d3 (g+8, 2t+1)
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// A operand taken from tensor memory (lane = row, one 32-bit column per K element), B from shared memory
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
+// error-compensated: small terms first, then hi.hi
+__device__ __forceinline__ void mma_tf32x3(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint32_t bh0,
+                                           uint32_t bh1, uint32_t bl0, uint32_t bl1) {
+  mma_tf32(d, al, bh0, bh1);
+  mma_tf32(d, ah, bl0, bl1);
+  mma_tf32(d, ah, bh0, bh1);
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
+
+// ---- warpgroup MMA (wgmma): D[64 x 32] += A[64 x 8] (registers) . B[32 x 8]^T (shared memory, K-major) ----------------
+// A fragment of warp w of the warpgroup: rows 16w .. 16w+15, same (g, t) layout as mma_tf32 above.
+// Accumulator: d[4j + 0/1] = (16w + g, 8j + 2t + 0/1), d[4j + 2/3] = (16w + g + 8, 8j + 2t + 0/1), j < 4.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+__device__ __forceinline__ void wgmma_n32_tf32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-        "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-        "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-        "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
+// shared-memory matrix descriptor of a K-major tile written by TMA with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128 bytes
+// (32 fp32 of K), 8-row groups 1024 bytes apart (SBO), layout type 1 = 128-byte swizzle.  Moving along K inside the
+// 128-byte row is a plain advance of the start address (32 bytes per 8-wide k-step).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// K-major operand tile, rows of 128 bytes, 128B swizzle, 8-row groups 1024 bytes apart
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-
-// MN-major TF32 operand tile (the contraction index runs over the ROWS of a row-major tile).  For 32-bit operands the
-// tensor core accepts exactly one MN-major shared-memory layout: 128-byte lines of 32 consecutive M/N elements whose
-// 32-BYTE chunks are XOR-swizzled with (line & 3) -- Swizzle<2,5,2>, descriptor layout type SWIZZLE_128B_BASE32B,
-// which is what TMA produces with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  K atoms are 4 lines (SBO = 512 bytes),
-// 32-element M/N groups are `lbo_bytes` apart (LBO).  One kind::tf32 MMA (K = 8) consumes 8 lines = 1024 bytes.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (32ull << 32) | (1ull << 46) | (1ull << 61);
-}
-// byte offset of the 16-byte piece holding columns 4*q4 .. 4*q4+3 (q4 < 8) of line `r` inside one 32-column group
-__device__ __forceinline__ uint32_t mn_sw_offset(int r, int q4) {
-  return (uint32_t)(r * 128 + ((((q4 >> 1) ^ (r & 3))) << 5) + ((q4 & 1) << 4));
-}
-// instruction descriptor, kind::tf32, fp32 accumulate; a_mn / b_mn: operand is MN-major
-__device__ __forceinline__ uint32_t umma_idesc_tf32(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// Remainder images for the error-compensated ("3xTF32") products: dst[i] = x - trunc19(x) for `nvec` 16-byte vectors
-// starting at shared address `src`, vector index = tid + k * nthreads.  All loads of a batch of NB vectors are issued
-// before the first store, so a thread has NB shared-memory round trips in flight instead of one.
-template <int NB>
-__device__ __forceinline__ void lo_image(uint32_t src, uint32_t dst, uint32_t nvec, uint32_t tid, uint32_t nthreads) {
-  for (uint32_t v0 = tid; v0 < nvec; v0 += NB * nthreads) {
-    float4 x[NB];
-#pragma unroll
-    for (int k = 0; k < NB; ++k) {
-      const uint32_t v = v0 + k * nthreads;
-      if (v < nvec)
-        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x[k].x), "=f"(x[k].y), "=f"(x[k].z), "=f"(x[k].w) : "r"(src + v * 16u));
-    }
-#pragma unroll
-    for (int k = 0; k < NB; ++k) {
-      const uint32_t v = v0 + k * nthreads;
-      if (v < nvec) {
-        const float a = x[k].x - __uint_as_float(__float_as_uint(x[k].x) & 0xFFFFE000u);
-        const float b = x[k].y - __uint_as_float(__float_as_uint(x[k].y) & 0xFFFFE000u);
-        const float c = x[k].z - __uint_as_float(__float_as_uint(x[k].z) & 0xFFFFE000u);
-        const float d = x[k].w - __uint_as_float(__float_as_uint(x[k].w) & 0xFFFFE000u);
-        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + v * 16u), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-      }
-    }
-  }
+// byte offset of element (row, col) (col < 32) inside such a tile
+__device__ __forceinline__ uint32_t sw128_offset(int row, int col) {
+  return (uint32_t)(row * 128 + ((((col >> 2) ^ row) & 7) << 4) + (col & 3) * 4);
 }
 
 // ---- host side -----------------------------------------------------------------------------------
@@ -262,7 +188,7 @@ inline int num_sms() {
   const int slot = (dev >= 0 && dev < 16) ? dev : 0;
   if (n[slot] == 0) {
     cudaDeviceGetAttribute(&n[slot], cudaDevAttrMultiProcessorCount, dev);
-    if (n[slot] <= 0) n[slot] = 148;
+    if (n[slot] <= 0) n[slot] = 132;
   }
   return n[slot];
 }

@@ -1,19 +1,22 @@
-// fp32-accurate GEMM on the 5th-gen tensor cores for the temporal self-attention encoder: the dense
-// Wq/Wk/Wv/Wo and feed-forward projections (code/models_rd.py:232-237,358 -> nn.TransformerEncoder)
-// and their input gradients.  Single-pass TF32 is borderline for these layers (SURVEY.md section 7:
-// ~1e-3 on the logits), so every product is error-compensated: the MMA reads the top 19 bits of an
-// fp32 operand (= its "hi" part) and we feed the exact remainders as two more MMAs into the same TMEM
-// accumulator.  Warp roles (10 warps, one persistent CTA per SM):
-//   warp 0      TMA producer for the weight tile and its precomputed remainder (L2 resident)
-//   warp 1      one thread issuing 3 x tcgen05.mma.kind::tf32 per 8-wide k-step, TMEM accumulators
-//               double buffered so the epilogue of tile i overlaps the MMAs of tile i+1
-//   warps 2-5   epilogue: tcgen05.ld -> bias / relu / gate / dropout / residual -> swizzled smem ->
-//               TMA store (coalesced 128-byte lines)
-//   warps 6-9   stagers: the activation tile arrives by TMA like the weight tile; these warps move it from shared memory
-//               into TENSOR memory (tcgen05.st, thread = row), split into hi (raw) and lo = x - trunc19(x).  The MMAs then
-//               take A from tensor memory: with both operands in shared memory the three error-compensation passes read
-//               the 128-row A slice three times per k-step and the kernel was shared-memory-bandwidth bound (156 KB of
-//               shared-memory traffic per k-block at BN = 96, 0.56 us; the tensor pipe idle 97 % of the time)
+// Tensor-core GEMMs on Hopper (sm_90a).
+//
+// tc_nt: C = epi(A . B^T), A [M, K] and B [N, K] both row-major ("K-major").  It serves the encoder projections
+// (code/models_rd.py:232-237,358 -> nn.TransformerEncoder) and their input gradients in error-compensated form, and the
+// observation-propagation layer (rd_obprop_tc.cu) in single-pass or error-compensated form.  One persistent CTA per SM:
+//   warpgroup 2   TMA producer (one thread): A tile [128 x 32] and B tile [BN x 32] (+ its precomputed remainder B_lo)
+//                 per k-block into a <= 4-stage ring of 128B-swizzled shared memory, one mbarrier per stage and
+//                 direction.  It hands its registers to the MMA warpgroups (setmaxnreg 40 / 232).
+//   warpgroups    0 and 1, rows 0-63 and 64-127 of the tile: wgmma.m64n32k8 TF32 with A from REGISTERS and B from
+//                 shared memory, fp32 accumulators in registers (BN <= 256 -> <= 128 per thread).  A is split into
+//                 hi = top 19 bits and lo = the exact remainder in registers, so the error-compensated mode needs no
+//                 remainder image of the activations: every k-step issues lo.hi + hi.lo + hi.hi.  The epilogue (bias,
+//                 relu, row scale, gate, dropout + keep bits, residual, TF32 rounding, permuted store) runs on the
+//                 accumulator registers and stores straight to global memory; meanwhile the producer already fills
+//                 the ring for the next tile.
+//
+// tc_wgrad_group: dW = dY^T X (+ db) for up to WG_MAX problems in one launch.  Both operands are activations whose
+// contraction index runs over their ROWS; wgmma's TF32 form only reads K-major operands from shared memory, so these
+// tiles are staged row-major (cp.async, padded rows) and fed to mma.sync.m16n8k8 from fragments gathered per thread.
 #include <stdlib.h>
 
 #include "rd_tc_common.cuh"
@@ -23,26 +26,28 @@ namespace rd {
 using namespace tc;
 namespace {
 
-constexpr int BM = 128, BK = 32, MAX_STAGES = 4, NTHREADS = 320;
-constexpr int A_TILE = BM * BK * 4;        // 16 KB (hi) + 16 KB (lo)
-constexpr int STG_BYTES = 4096;
-constexpr int MAX_BN = 160;
-// tensor memory: two accumulators of ACC_COLS columns, then A_SLOTS activation slots of 64 columns (hi | lo, 32 each)
-constexpr uint32_t ACC_COLS = 160, A_COL0 = 2 * ACC_COLS;
-constexpr int A_SLOTS = 3;
+constexpr int BM = 128, BK = 32, MAX_STAGES = 4;
+constexpr int NT_THREADS = 384;            // warpgroups 0, 1: MMA + epilogue; warpgroup 2: TMA producer
+constexpr int NCH_MAX = 8;                 // 32-column accumulator chunks per tile: BN <= 256
+constexpr int A_TILE = BM * BK * 4;        // 16 KB
+constexpr int MAX_BN = 160;                // encoder GEMMs: narrower tiles spread the small problems over more SMs
 
-struct P {
-  const float* A; long long lda;
-  long long M; int N, K, BN, n_tiles, m_tiles, k_blocks, nstages;
-  const float* bias; int relu;
+enum : int { F_RELU = 1, F_SCALE = 2, F_GATE = 4, F_DROP = 8, F_RESID = 16, F_ROUND = 32, F_PERM = 64 };
+
+struct NtP {
+  long long M; int N, K, BN, nch, n_tiles, m_tiles, k_blocks, nstages;
+  float* C; long long ldc;
+  const float* bias;
+  const float* scale; int scale_mod;
   const float* gate; long long gate_ld; float gate_scale;
   float drop_p; const uint64_t* rng; uint32_t drop_site;
   uint32_t* drop_mask; int drop_mask_ld;
   const float* resid; long long resid_ld;
-  unsigned long long* dbg;     // optional %globaltimer phase stamps [CTA][8] (rd_debug_gemm_timing)
+  int pB, pN, pD;
+  unsigned long long* dbg;     // optional %globaltimer stamps [CTA][8] (rd_debug_gemm_timing)
 };
 
-__device__ __forceinline__ void gstamp(const P& p, int slot) {
+__device__ __forceinline__ void gstamp(const NtP& p, int slot) {
   if (p.dbg) {
     unsigned long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
@@ -50,269 +55,228 @@ __device__ __forceinline__ void gstamp(const P& p, int slot) {
   }
 }
 
-// epilogue features are compile-time: the epilogue is on the critical path of these small GEMMs
-template <bool RELU, bool GATE, bool DROP, bool RESID>
-__global__ void __launch_bounds__(NTHREADS, 1)
-tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmC, const P p) {
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+
+template <int NCH, bool EXACT>
+__device__ __forceinline__ void issue_kblock(float (&acc)[NCH_MAX][16], const uint32_t (&ah)[BK / 8][4],
+                                             const uint32_t (&al)[BK / 8][4], uint32_t sb, uint32_t b_tile) {
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < BK / 8; ++ks) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const uint32_t bo = sb + (uint32_t)c * 4096u + (uint32_t)ks * 32u;
+      const uint64_t bh = wgmma_desc_sw128(bo);
+      if (EXACT) {
+        const uint64_t bl = wgmma_desc_sw128(bo + b_tile);
+        wgmma_n32_tf32(acc[c], al[ks], bh);       // small terms first
+        wgmma_n32_tf32(acc[c], ah[ks], bl);
+      }
+      wgmma_n32_tf32(acc[c], ah[ks], bh);
+    }
+  }
+}
+
+template <int F, bool EXACT>
+__global__ void __launch_bounds__(NT_THREADS, 1)
+tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+             const __grid_constant__ CUtensorMap tmBlo, const NtP p) {
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();
-  if (threadIdx.x == 0) gstamp(p, 0);
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t b_tile = (uint32_t)p.BN * 128u;
-  const uint32_t stage_bytes = (uint32_t)A_TILE + 2u * b_tile;      // A (raw) | B hi | B lo
-  const uint32_t stg_base = base + (uint32_t)p.nstages * stage_bytes;
-  const uint32_t bias_base = stg_base + 8 * STG_BYTES;
-  const uint32_t bar_base = bias_base + 2 * 256 * 4;
+  const uint32_t stage_bytes = (uint32_t)A_TILE + (EXACT ? 2u : 1u) * b_tile;     // A | B hi [| B lo]
+  const uint32_t bar_base = base + (uint32_t)p.nstages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (MAX_STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * MAX_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * MAX_STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * MAX_STAGES + 4);
-  auto aready_bar = [&](int a) { return bar_base + 8u * (2 * MAX_STAGES + 5 + a); };    // A slot staged in tensor memory
-  auto aempty_bar = [&](int a) { return bar_base + 8u * (2 * MAX_STAGES + 5 + A_SLOTS + a); };   // MMAs have read it
-  float* bias_s = reinterpret_cast<float*>(smem_raw + (bias_base - smem_u32(smem_raw)));
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBlo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
+    if (EXACT) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBlo) : "memory");
+    for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-      for (int a = 0; a < A_SLOTS; ++a) { mbar_init(aready_bar(a), 4); mbar_init(aempty_bar(a), 1); }
-      for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_wait();          // everything above is private to this CTA; the previous kernel's output is first touched below
-  if (threadIdx.x == 0) gstamp(p, 1);
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  if (threadIdx.x == 0) gstamp(p, 0);
   const int total_tiles = p.m_tiles * p.n_tiles;
 
-  if (warp == 0) {
-    // ===== TMA producer: activation tile, weight tile (hi = the raw weight) and the weight remainder ==============
-    if (lane == 0) {
+  if (warp >= 8) {
+    // ===== TMA producer ==========================================================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int n_t = tile % p.n_tiles, m_t = tile / p.n_tiles;
+        const int m_t = tile / p.n_tiles, n_t = tile - m_t * p.n_tiles;
         for (int kb = 0; kb < p.k_blocks; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1u);
-          mbar_expect_tx(full_bar(stage), (uint32_t)A_TILE + 2u * b_tile);
-          tma_load_2d(&tmA, full_bar(stage), base + (uint32_t)stage * stage_bytes, kb * BK, m_t * BM);
-          const uint32_t sb = base + (uint32_t)stage * stage_bytes + (uint32_t)A_TILE;
-          tma_load_2d(&tmB, full_bar(stage), sb, kb * BK, n_t * p.BN);
-          tma_load_2d(&tmBlo, full_bar(stage), sb + b_tile, kb * BK, n_t * p.BN);     // (deriving it on chip like A_lo was slower:
-          // the remainder pass, not L2, paces the k-loop -- 0.73 vs 0.56 us per k-block)
+          mbar_expect_tx(full_bar(stage), stage_bytes);
+          const uint32_t sa = base + (uint32_t)stage * stage_bytes;
+          tma_load_2d(&tmA, full_bar(stage), sa, kb * BK, m_t * BM);
+          tma_load_2d(&tmB, full_bar(stage), sa + A_TILE, kb * BK, n_t * p.BN);
+          if (EXACT) tma_load_2d(&tmBlo, full_bar(stage), sa + A_TILE + b_tile, kb * BK, n_t * p.BN);
           if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer ================================================================================
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0; int slot = 0; uint32_t slot_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * ACC_COLS;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(full_bar(stage), phase);           // weight tiles (the stagers waited for the same barrier)
-          mbar_wait(aready_bar(slot), slot_phase);     // activation tile staged in tensor memory
-          if (kb == 0) gstamp(p, 2);
-          tc_fence_after();
-          const uint32_t sb = base + (uint32_t)stage * stage_bytes + (uint32_t)A_TILE;
-          const uint64_t b_hi = umma_desc_sw128(sb), b_lo = umma_desc_sw128(sb + b_tile);
-          const uint32_t a_hi = tmem_base + A_COL0 + (uint32_t)slot * 64u, a_lo = a_hi + 32u;
+    return;
+  }
+
+  // ===== warpgroups 0, 1: MMA and epilogue ========================================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int wg = warp >> 2, wq = warp & 3, g = lane >> 2, t = lane & 3;
+  const int arow = wg * 64 + wq * 16 + g;              // tile-local row of fragment elements a0 / a2
+  const float ik = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
+  const RngKey key = load_rng_key((F & F_DROP) ? p.rng : nullptr);
+  int stage = 0; uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int m_t = tile / p.n_tiles, n_t = tile - m_t * p.n_tiles;
+    float acc[NCH_MAX][16];
 #pragma unroll
-          for (int kk = 0; kk < BK / 8; ++kk) {
-            const uint64_t o = (uint64_t)(kk * 2);
-            const uint32_t ao = (uint32_t)(kk * 8);                                  // 8 columns = 8 tf32 of K
-            umma_tf32_ts(d_tmem, a_lo + ao, b_hi + o, idesc, (kb | kk) ? 1u : 0u);   // small terms first
-            umma_tf32_ts(d_tmem, a_hi + ao, b_lo + o, idesc, 1u);
-            umma_tf32_ts(d_tmem, a_hi + ao, b_hi + o, idesc, 1u);
-          }
-          umma_commit(empty_bar(stage));
-          umma_commit(aempty_bar(slot));
-          if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
-          if (++slot == A_SLOTS) { slot = 0; slot_phase ^= 1u; }
+    for (int c = 0; c < NCH_MAX; ++c)
+#pragma unroll
+      for (int e = 0; e < 16; ++e) acc[c][e] = 0.f;
+    for (int kb = 0; kb < p.k_blocks; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sa = base + (uint32_t)stage * stage_bytes, sb = sa + A_TILE;
+      uint32_t ah[BK / 8][4], al[BK / 8][4];
+#pragma unroll
+      for (int ks = 0; ks < BK / 8; ++ks) {
+        const int col = ks * 8 + t;
+        const float x0 = lds_f32(sa + sw128_offset(arow, col)), x1 = lds_f32(sa + sw128_offset(arow + 8, col));
+        const float x2 = lds_f32(sa + sw128_offset(arow, col + 4)), x3 = lds_f32(sa + sw128_offset(arow + 8, col + 4));
+        if (EXACT) {
+          ah[ks][0] = tf32_hi(x0); ah[ks][1] = tf32_hi(x1); ah[ks][2] = tf32_hi(x2); ah[ks][3] = tf32_hi(x3);
+          al[ks][0] = tf32_lo(x0); al[ks][1] = tf32_lo(x1); al[ks][2] = tf32_lo(x2); al[ks][3] = tf32_lo(x3);
+        } else {   // single pass: the producers keep these operands TF32-representable
+          ah[ks][0] = __float_as_uint(x0); ah[ks][1] = __float_as_uint(x1);
+          ah[ks][2] = __float_as_uint(x2); ah[ks][3] = __float_as_uint(x3);
         }
-        umma_commit(tfull_bar(acc));
-        gstamp(p, 3);
-        acc ^= 1; if (acc == 0) acc_phase ^= 1u;
       }
-    }
-  } else if (warp < 6) {
-    // ===== epilogue ====================================================================================
-    const int q = warp & 3;
-    const int et = threadIdx.x - 64;
-    const uint32_t my_stg = stg_base + (uint32_t)(warp - 2) * 2u * STG_BYTES;
-    int acc = 0; uint32_t acc_phase = 0; int buf = 0;
-    const int n_chunks = (p.BN + 31) / 32;
-    const float ik = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
-    const RngKey key = load_rng_key(DROP ? p.rng : nullptr);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m_t = tile / p.n_tiles, n_t = tile - m_t * p.n_tiles;
-      const int col0 = n_t * p.BN;
-      for (int c = et; c < 256; c += 128) bias_s[acc * 256 + c] = (p.bias && c < p.BN && col0 + c < p.N) ? __ldg(p.bias + col0 + c) : 0.f;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      const int row0 = m_t * BM + q * 32;
-      const long long row = (long long)row0 + lane;
-      const bool row_ok = row < p.M;
-      // gate / residual operands of chunk ch are fetched one chunk AHEAD (chunk 0 before the accumulator is even
-      // complete): their L2 round trips used to sit, one per chunk, on the critical path of the epilogue
-      float4 pg[8], pr[8];
-      auto prefetch = [&](int ch) {
 #pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const int c = col0 + ch * 32 + 4 * j4;
-          const bool ok = row_ok && c < p.N && ch * 32 + 4 * j4 < p.BN;
-          if (GATE) pg[j4] = ok ? __ldg(reinterpret_cast<const float4*>(p.gate + row * p.gate_ld + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          if (RESID) pr[j4] = ok ? __ldg(reinterpret_cast<const float4*>(p.resid + row * p.resid_ld + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      };
-      if (GATE || RESID) prefetch(0);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      if (threadIdx.x == 64) gstamp(p, 4);
-      tc_fence_after();
-      for (int ch = 0; ch < n_chunks; ++ch) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * ACC_COLS + (uint32_t)(ch * 32), v);
-        float4 cg[8], cr[8];
+      for (int c = 0; c < NCH_MAX; ++c)
 #pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) { if (GATE) cg[j4] = pg[j4]; if (RESID) cr[j4] = pr[j4]; }
-        if ((GATE || RESID) && ch + 1 < n_chunks) prefetch(ch + 1);
-        const float* bs = bias_s + acc * 256 + ch * 32;
-        const int c0 = col0 + ch * 32;
-        if (lane == 0) bulk_wait_read<1>();
-        __syncwarp();
-        const uint32_t stg = my_stg + (uint32_t)buf * STG_BYTES;
-        uint32_t keep_word = 0u;
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          float o[4];
-          const int c = c0 + 4 * j4;
-          const bool ok = row_ok && c < p.N;     // N % 4 == 0: a float4 is all in or all out
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float x = __uint_as_float(v[4 * j4 + e]) + bs[4 * j4 + e];
-            o[e] = RELU ? fmaxf(x, 0.f) : x;
-          }
-          if (GATE && ok) {
-            const float4 g = cg[j4];
-            o[0] = g.x > 0.f ? o[0] * p.gate_scale : 0.f; o[1] = g.y > 0.f ? o[1] * p.gate_scale : 0.f;
-            o[2] = g.z > 0.f ? o[2] * p.gate_scale : 0.f; o[3] = g.w > 0.f ? o[3] * p.gate_scale : 0.f;
-          }
-          if (DROP && ok) {   // row*N + c is a multiple of 4: one Philox block for the four columns
-            const float4 m = dropout_scale4(key, p.drop_site, (uint64_t)row * (uint64_t)p.N + (uint64_t)c, p.drop_p, ik);
-            o[0] *= m.x; o[1] *= m.y; o[2] *= m.z; o[3] *= m.w;
-            keep_word |= ((m.x > 0.f ? 1u : 0u) | (m.y > 0.f ? 2u : 0u) | (m.z > 0.f ? 4u : 0u) | (m.w > 0.f ? 8u : 0u)) << (4 * j4);
-          }
-          if (RESID && ok) {
-            const float4 r = cr[j4];
-            o[0] += r.x; o[1] += r.y; o[2] += r.z; o[3] += r.w;
-          }
-          const uint32_t off = (uint32_t)(lane * 128 + ((j4 ^ (lane & 7)) << 4));
-          asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stg + off), "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]) : "memory");
-        }
-        // the backward of the consumer (LayerNorm) reads these bits instead of regenerating the Philox stream
-        if (DROP && p.drop_mask && row_ok && c0 < p.N) p.drop_mask[row * p.drop_mask_ld + (c0 >> 5)] = keep_word;
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmC, stg, c0, row0);
-          bulk_commit();
-        }
-        buf ^= 1;
+        for (int e = 0; e < 16; ++e) fence_operand(acc[c][e]);
+      // the chunk count is a compile-time constant of each issue sequence: a runtime guard between the wgmma
+      // instructions makes ptxas fence (serialise) them
+      switch (p.nch) {
+        case 1: issue_kblock<1, EXACT>(acc, ah, al, sb, b_tile); break;
+        case 2: issue_kblock<2, EXACT>(acc, ah, al, sb, b_tile); break;
+        case 3: issue_kblock<3, EXACT>(acc, ah, al, sb, b_tile); break;
+        case 4: issue_kblock<4, EXACT>(acc, ah, al, sb, b_tile); break;
+        case 5: issue_kblock<5, EXACT>(acc, ah, al, sb, b_tile); break;
+        case 6: issue_kblock<6, EXACT>(acc, ah, al, sb, b_tile); break;
+        case 7: issue_kblock<7, EXACT>(acc, ah, al, sb, b_tile); break;
+        default: issue_kblock<8, EXACT>(acc, ah, al, sb, b_tile); break;
       }
-      tc_fence_before();
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < NCH_MAX; ++c)
+#pragma unroll
+        for (int e = 0; e < 16; ++e) fence_operand(acc[c][e]);
       __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      acc ^= 1; if (acc == 0) acc_phase ^= 1u;
+      if (lane == 0) mbar_arrive(empty_bar(stage));    // this warp's reads of the stage are complete
+      if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
     }
-    if (threadIdx.x == 64) gstamp(p, 5);
-    if (lane == 0) bulk_wait_read<0>();
-    if (threadIdx.x == 64) gstamp(p, 6);
-  } else {
-    // ===== stagers: activation tile shared memory -> tensor memory, split into hi (raw) and lo = x - trunc19(x) ==========
-    // thread = tile row (its TMEM lane); the row's 32 values of the k-block are 8 swizzled 16-byte pieces
-    const int q = warp & 3, row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    int stage = 0; uint32_t phase = 0; int slot = 0; uint32_t slot_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        const uint32_t sa = base + (uint32_t)stage * stage_bytes + (uint32_t)row * 128u;
-        uint32_t x[32], l[32];
+
+    // ---- epilogue on the accumulator registers: element (row0 + 8i, col0 + 32c + 8j + 2t + {0, 1}) ----
+    const long long row0 = (long long)m_t * BM + arow;
+    const int col0 = n_t * p.BN;
+    float sc[2] = {1.f, 1.f};
+    if (F & F_SCALE) {
 #pragma unroll
-        for (int c = 0; c < 8; ++c)
-          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(x[4 * c]), "=r"(x[4 * c + 1]), "=r"(x[4 * c + 2]), "=r"(x[4 * c + 3])
-                       : "r"(sa + (uint32_t)(((c ^ (row & 7)) << 4))));
+      for (int i = 0; i < 2; ++i) sc[i] = row0 + 8 * i < p.M ? __ldg(p.scale + ((row0 + 8 * i) % p.scale_mod)) : 0.f;
+    }
 #pragma unroll
-        for (int e = 0; e < 32; ++e) l[e] = __float_as_uint(__uint_as_float(x[e]) - __uint_as_float(x[e] & 0xFFFFE000u));
-        mbar_wait(aempty_bar(slot), slot_phase ^ 1u);      // the MMAs of three k-blocks ago have read this slot
-        tc_fence_after();
-        const uint32_t ta = tmem_base + lane_addr + A_COL0 + (uint32_t)slot * 64u;
-        tmem_st32(ta, x);
-        tmem_st32(ta + 32u, l);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(aready_bar(slot));
-        if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
-        if (++slot == A_SLOTS) { slot = 0; slot_phase ^= 1u; }
+    for (int c = 0; c < NCH_MAX; ++c) {
+      if (c >= p.nch) continue;
+      uint32_t bits[2] = {0u, 0u};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int col = col0 + c * 32 + 8 * j + 2 * t;
+        const bool col_ok = col < p.N;                 // N even, col even: the pair is all in or all out
+        float b0 = 0.f, b1 = 0.f;
+        if (p.bias && col_ok) { b0 = __ldg(p.bias + col); b1 = __ldg(p.bias + col + 1); }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const long long row = row0 + 8 * i;
+          const bool ok = col_ok && row < p.M;
+          float v0 = acc[c][4 * j + 2 * i] + b0, v1 = acc[c][4 * j + 2 * i + 1] + b1;
+          if (F & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (F & F_SCALE) { v0 *= sc[i]; v1 *= sc[i]; }
+          if (!ok) continue;
+          if (F & F_GATE) {   // backward: pass the gradient only where the forward output was positive
+            const float2 gv = __ldg(reinterpret_cast<const float2*>(p.gate + row * p.gate_ld + col));
+            v0 = gv.x > 0.f ? v0 * p.gate_scale : 0.f;
+            v1 = gv.y > 0.f ? v1 * p.gate_scale : 0.f;
+          }
+          if (F & F_DROP) {   // element index row*N + col; N % 4 == 0, so the pair shares one Philox block
+            const uint64_t idx = (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
+            const uint4 u = dropout_block(key, p.drop_site, idx);
+            const bool lo_half = (idx & 3u) == 0;
+            const float m0 = keep_scale(lo_half ? u.x : u.z, p.drop_p, ik), m1 = keep_scale(lo_half ? u.y : u.w, p.drop_p, ik);
+            v0 *= m0; v1 *= m1;
+            bits[i] |= ((m0 > 0.f ? 1u : 0u) | (m1 > 0.f ? 2u : 0u)) << (8 * j + 2 * t);
+          }
+          if (F & F_RESID) {
+            const float2 r = __ldg(reinterpret_cast<const float2*>(p.resid + row * p.resid_ld + col));
+            v0 += r.x; v1 += r.y;
+          }
+          if (F & F_ROUND) { v0 = rn_tf32(v0); v1 = rn_tf32(v1); }
+          float* dst;
+          if (F & F_PERM) {   // row = b*pN + n, col = tt*4 + k  ->  encoder input [T, B, D] (code/models_rd.py:338-341)
+            const long long b = row / p.pN, n = row - b * p.pN;
+            dst = p.C + ((long long)(col >> 2) * p.pB + b) * p.pD + n * 4 + (col & 3);
+          } else {
+            dst = p.C + row * p.ldc + col;
+          }
+          *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+        }
+      }
+      if ((F & F_DROP) && p.drop_mask) {
+        // the backward of the consumer (LayerNorm) reads these bits instead of regenerating the Philox stream
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          bits[i] |= __shfl_xor_sync(0xffffffffu, bits[i], 1);
+          bits[i] |= __shfl_xor_sync(0xffffffffu, bits[i], 2);
+          const long long row = row0 + 8 * i;
+          const int cw = col0 + c * 32;
+          if (t == 0 && row < p.M && cw < p.N) p.drop_mask[row * p.drop_mask_ld + (cw >> 5)] = bits[i];
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-    if (lane == 0) gstamp(p, 7);
-  }
+  if (threadIdx.x == 0) gstamp(p, 7);
 }
 
 // =================================================================================================
 // weight-gradient kernel ("TN"), GROUPED: one launch serves up to WG_MAX independent problems
 //   D_k[m, n] = sum_r A_k[r, m] * B_k[r, n]   over this CTA's row range of problem k
-// A training step has ten of these (8 encoder weights + 2 lin_value); launched one by one each was a
-// ~20 us latency chain (2 k-blocks per CTA).  Grouped, every CTA owns >= 8 k-blocks, the loader warps
-// prefetch the next k-block's global loads before they transpose/store the current one, and the
-// launch + prologue latency is paid once.
+// A training step has ten of these (8 encoder weights + 2 lin_value); grouped, the launch latency is paid once.
+// One CTA per work item (problem, m tile, n tile, row split): 8 warps, 4 (m: 32 rows) x 2 (n: BN/2 columns), row
+// blocks of 32 staged by cp.async into a two-stage ring.  Row strides of the staged tiles are 8 floats more than a
+// multiple of 32, so the fragment gathers (lanes g along M/N, lanes t along K) hit 32 distinct banks.  The bias
+// gradient falls out of the same MMAs as one extra "ones" column of X (column N).
 // =================================================================================================
-// Both operands are row-major activations [rows, cols] and the contraction runs over ROWS, i.e. they are
-// "MN-major" from the tensor core's point of view.  tcgen05 takes MN-major TF32 operands directly (instruction
-// descriptor bits 15/16) in exactly one shared-memory layout, the 128B swizzle with 32-byte atoms (rd_tc_common.cuh),
-// which TMA produces with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  So the tiles go global -> shared memory exactly as
-// they lie in memory: box {32 columns, 32 rows}; one 128-byte line = 32 consecutive columns of one row; the next 32
-// columns are the next box, LBO = 4096 B apart.  No register transposes; four warps only derive the
-// error-compensation remainders lo = x - trunc19(x) (same addresses, so the swizzle never has to be undone) and
-// plant the "ones" column that makes the bias gradient fall out of the same MMAs.
 struct WP {
+  const float* dY; const float* X; long long ldy, ldx;
   float* partial;                    // [nsplit][Mpad][Nld]
   long long rows; int M, N, BN, n_tiles, m_tiles, nsplit, rows_per_split, Mpad, Nld;
   int item0;                         // first work item of this problem inside the grouped list
 };
-struct WGroup { CUtensorMap tmA[WG_MAX]; CUtensorMap tmB[WG_MAX]; WP it[WG_MAX]; int n, total_items, nstages, stage_bytes; };
+struct WGroup { WP it[WG_MAX]; int n, total_items; };
 
-// PERSISTENT: one CTA per SM walks the work items (problem, m tile, n tile, row split) round-robin.  The accumulator is
-// double-buffered in tensor memory (2 x 256 columns), so the epilogue of item i (TMEM -> partial slab, 80 KB of stores)
-// overlaps the MMAs of item i+1, and the TMA ring runs ahead across item boundaries.  One CTA per item (the previous
-// design) paid prologue + pipeline fill + epilogue serially per item and ran 3.1 waves as 4.
-constexpr int W_THREADS = 320;       // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue, warps 6-9 remainder pass
-constexpr int MN_BOX = 32 * 32 * 4;  // one {32 col, 32 row} fp32 box = 4096 bytes
+constexpr int W_THREADS = 256;
+constexpr int WBK = 32;              // contraction rows per block
+constexpr int LDA_W = BM + 8;        // staged dY tile [32][BM + 8]
+constexpr int NJ_MAX = MAX_BN / 16;  // n8 tiles per warp
 
 struct WItem { int pi, n_t, m_t, split, k_blocks; long long r_begin, r_end; };
 __device__ __forceinline__ WItem wgrad_item(const WGroup& g, int w) {
@@ -325,168 +289,105 @@ __device__ __forceinline__ WItem wgrad_item(const WGroup& g, int w) {
   it.n_t = item % p.n_tiles; it.m_t = (item / p.n_tiles) % p.m_tiles; it.split = item / (p.n_tiles * p.m_tiles);
   it.r_begin = (long long)it.split * p.rows_per_split;
   it.r_end = min(p.rows, it.r_begin + p.rows_per_split);
-  it.k_blocks = (int)((it.r_end - it.r_begin + BK - 1) / BK);
+  it.k_blocks = (int)((it.r_end - it.r_begin + WBK - 1) / WBK);
   return it;
 }
 
-__global__ void __launch_bounds__(W_THREADS, 1)
+__global__ void __launch_bounds__(W_THREADS)
 tc_wgrad_kernel(const __grid_constant__ WGroup g) {
-  extern __shared__ uint8_t smem_raw[];
+  extern __shared__ float wsm[];
   pdl_launch_dependents();
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t stage_bytes = (uint32_t)g.stage_bytes;        // sized for the widest problem of the group
-  const int nstages = g.nstages;
-  const uint32_t bar_base = base + (uint32_t)nstages * stage_bytes;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };                    // TMA bytes landed
-  auto ready_bar = [&](int s) { return bar_base + 8u * (MAX_STAGES + s); };    // remainders written
-  auto empty_bar = [&](int s) { return bar_base + 8u * (2 * MAX_STAGES + s); };// MMAs have read the stage
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (3 * MAX_STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (3 * MAX_STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (3 * MAX_STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  if (warp == 0 && lane == 0) {
-    for (int k = 0; k < g.n; ++k) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&g.tmA[k]) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&g.tmB[k]) : "memory");
-    }
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(ready_bar(s), 4); mbar_init(empty_bar(s), 1); }
-      for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(tmem_slot) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
   pdl_wait();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  const WItem it = wgrad_item(g, blockIdx.x);
+  const WP& p = g.it[it.pi];
+  const int ldb = p.BN + 8;
+  const int stage_floats = WBK * LDA_W + WBK * ldb;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq = lane >> 2, t = lane & 3;
+  const int wm = warp & 3, wn = warp >> 2;
+  const int nj = p.BN >> 4;                      // n8 tiles of this warp (BN / 2 columns)
+  const int mcol0 = it.m_t * BM, ncol0 = it.n_t * p.BN;
 
-  if (warp == 0) {
-    // ===== TMA producer: raw row-major tiles, up to `nstages` k-blocks in flight ======================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
-        const WItem it = wgrad_item(g, w);
-        const WP& p = g.it[it.pi];
-        const int b_groups = p.BN >> 5;                       // 32-column groups of the B tile
-        for (int kb = 0; kb < it.k_blocks; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          mbar_expect_tx(full_bar(stage), (uint32_t)(4 + b_groups) * MN_BOX);
-          const uint32_t sa = base + (uint32_t)stage * stage_bytes;
-          const int r0 = (int)(it.r_begin + (long long)kb * BK);
+  auto load = [&](int kb, int s) {
+    float* sA = wsm + s * stage_floats;
+    float* sB = sA + WBK * LDA_W;
+    const long long r0 = it.r_begin + (long long)kb * WBK;
+    for (int v = threadIdx.x; v < WBK * (BM / 4); v += W_THREADS) {
+      const int r = v / (BM / 4), c = 4 * (v % (BM / 4));
+      const long long gr = r0 + r;
+      const bool ok = gr < it.r_end && mcol0 + c < p.M;
+      const float* src = ok ? p.dY + gr * p.ldy + mcol0 + c : p.dY;
+      cp_async16(smem_u32(sA + r * LDA_W + c), src, ok ? 16u : 0u);
+    }
+    const int bq = p.BN / 4;
+    for (int v = threadIdx.x; v < WBK * bq; v += W_THREADS) {
+      const int r = v / bq, c = 4 * (v % bq);
+      const long long gr = r0 + r;
+      const int gc = ncol0 + c;
+      float* dst = sB + r * ldb + c;
+      if (gc == p.N) {                          // X[r, N] := 1 for the valid rows: the bias gradient column
+        *reinterpret_cast<float4*>(dst) = make_float4(gr < it.r_end ? 1.f : 0.f, 0.f, 0.f, 0.f);
+      } else {
+        const bool ok = gr < it.r_end && gc < p.N;
+        cp_async16(smem_u32(dst), ok ? p.X + gr * p.ldx + gc : p.X, ok ? 16u : 0u);
+      }
+    }
+    cp_async_commit();
+  };
+
+  float acc[2][NJ_MAX][4];
 #pragma unroll
-          for (int gq = 0; gq < 4; ++gq) tma_load_2d(&g.tmA[it.pi], full_bar(stage), sa + gq * MN_BOX, it.m_t * BM + gq * 32, r0);
-          for (int gq = 0; gq < b_groups; ++gq)
-            tma_load_2d(&g.tmB[it.pi], full_bar(stage), sa + 2u * A_TILE + gq * MN_BOX, it.n_t * p.BN + gq * 32, r0);
-          if (++stage == nstages) { stage = 0; phase ^= 1u; }
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int j = 0; j < NJ_MAX; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[mi][j][e] = 0.f;
+
+  if (it.k_blocks > 0) load(0, 0);
+  for (int kb = 0; kb < it.k_blocks; ++kb) {
+    if (kb + 1 < it.k_blocks) { load(kb + 1, (kb + 1) & 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
+    __syncthreads();
+    const float* sA = wsm + (kb & 1) * stage_floats;
+    const float* sB = sA + WBK * LDA_W;
+#pragma unroll
+    for (int ks = 0; ks < WBK / 8; ++ks) {
+      const int k0 = ks * 8 + t;
+      uint32_t ah[2][4], al[2][4];
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi) {
+        const int m = wm * 32 + mi * 16 + gq;
+        const float x0 = sA[k0 * LDA_W + m], x1 = sA[k0 * LDA_W + m + 8];
+        const float x2 = sA[(k0 + 4) * LDA_W + m], x3 = sA[(k0 + 4) * LDA_W + m + 8];
+        ah[mi][0] = tf32_hi(x0); ah[mi][1] = tf32_hi(x1); ah[mi][2] = tf32_hi(x2); ah[mi][3] = tf32_hi(x3);
+        al[mi][0] = tf32_lo(x0); al[mi][1] = tf32_lo(x1); al[mi][2] = tf32_lo(x2); al[mi][3] = tf32_lo(x3);
+      }
+#pragma unroll
+      for (int j = 0; j < NJ_MAX; ++j) {
+        if (j < nj) {
+          const int n = wn * (p.BN >> 1) + j * 8 + gq;
+          const float y0 = sB[k0 * ldb + n], y1 = sB[(k0 + 4) * ldb + n];
+          const uint32_t bh0 = tf32_hi(y0), bh1 = tf32_hi(y1), bl0 = tf32_lo(y0), bl1 = tf32_lo(y1);
+          mma_tf32x3(acc[0][j], ah[0], al[0], bh0, bh1, bl0, bl1);
+          mma_tf32x3(acc[1][j], ah[1], al[1], bh0, bh1, bl0, bl1);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer ================================================================================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-      for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
-        const WItem it = wgrad_item(g, w);
-        const WP& p = g.it[it.pi];
-        const uint32_t b_tile = (uint32_t)p.BN * 128u;
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) |     // MN-major A and B
-                               ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * 256u;
-        for (int kb = 0; kb < it.k_blocks; ++kb) {
-          mbar_wait(ready_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = base + (uint32_t)stage * stage_bytes;
-          const uint64_t a_hi = umma_desc_mn_sw128(sa, MN_BOX), a_lo = umma_desc_mn_sw128(sa + A_TILE, MN_BOX);
-          const uint64_t b_hi = umma_desc_mn_sw128(sa + 2u * A_TILE, MN_BOX), b_lo = umma_desc_mn_sw128(sa + 2u * A_TILE + b_tile, MN_BOX);
-#pragma unroll
-          for (int kk = 0; kk < BK / 8; ++kk) {
-            const uint64_t o = (uint64_t)(kk * 64);            // next 8-row K group: +1024 bytes
-            umma_tf32(d_tmem, a_lo + o, b_hi + o, idesc, (kb | kk) ? 1u : 0u);
-            umma_tf32(d_tmem, a_hi + o, b_lo + o, idesc, 1u);
-            umma_tf32(d_tmem, a_hi + o, b_hi + o, idesc, 1u);
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == nstages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(tfull_bar(acc));
-        acc ^= 1; if (acc == 0) acc_phase ^= 1u;
-      }
-    }
-  } else if (warp < 6) {
-    // ===== epilogue: accumulator tile -> partial slab (each lane owns one row: 128-byte runs) ===========
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
-      const WItem it = wgrad_item(g, w);
-      const WP& p = g.it[it.pi];
-      const int n_chunks = (p.BN + 31) / 32;
-      float* prow = p.partial + ((long long)it.split * p.Mpad + it.m_t * BM + q * 32 + lane) * p.Nld + it.n_t * p.BN;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      for (int ch = 0; ch < n_chunks; ++ch) {
-        uint32_t v[32];
-        if (it.k_blocks > 0) {
-          tmem_ld32(tmem_base + (uint32_t)acc * 256u + ((uint32_t)(q * 32) << 16) + (uint32_t)(ch * 32), v);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = 0u;
-        }
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const int c = ch * 32 + 4 * j4;
-          if (c < p.BN)
-            *reinterpret_cast<uint4*>(prow + c) = make_uint4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      acc ^= 1; if (acc == 0) acc_phase ^= 1u;
-    }
-  } else {
-    // ===== warps 6-9: remainder pass per k-block (+ the implicit ones column of the bias gradient) ========
-    const int lt = threadIdx.x - 192;            // 0..127
-    int stage = 0; uint32_t phase = 0;
-    for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
-      const WItem it = wgrad_item(g, w);
-      const WP& p = g.it[it.pi];
-      const uint32_t b_tile = (uint32_t)p.BN * 128u;
-      const int ones_col = p.N - it.n_t * p.BN;    // tile-local column of the implicit ones column (bias gradient)
-      const bool has_ones = ones_col >= 0 && ones_col < p.BN;
-      const uint32_t a_vec = A_TILE / 16, b_vec = b_tile / 16;
-      for (int kb = 0; kb < it.k_blocks; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        const uint32_t sa = base + (uint32_t)stage * stage_bytes;
-        if (has_ones && lt < BK) {             // X[r, N] := 1 for the valid rows of this k-block (OOB columns arrived as 0)
-          const long long r = it.r_begin + (long long)kb * BK + lt;
-          const uint32_t off = (uint32_t)((ones_col >> 5) * MN_BOX) + mn_sw_offset(lt, (ones_col & 31) >> 2) + (uint32_t)(ones_col & 3) * 4u;
-          asm volatile("st.shared.f32 [%0], %1;" ::"r"(sa + 2u * A_TILE + off), "f"(r < it.r_end ? 1.f : 0.f) : "memory");
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        lo_image<6>(sa, sa + A_TILE, a_vec, (uint32_t)lt, 128u);                              // dY tile
-        lo_image<6>(sa + 2u * A_TILE, sa + 2u * A_TILE + b_tile, b_vec, (uint32_t)lt, 128u);  // X tile
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(ready_bar(stage));
-        if (++stage == nstages) { stage = 0; phase ^= 1u; }
-      }
-    }
+    __syncthreads();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+
+  // ---- partial tile -> slab [split][Mpad][Nld] ------------------------------------------------------
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi) {
+#pragma unroll
+    for (int j = 0; j < NJ_MAX; ++j) {
+      if (j < nj) {
+        const int n = ncol0 + wn * (p.BN >> 1) + j * 8 + 2 * t;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const long long m = (long long)it.split * p.Mpad + mcol0 + wm * 32 + mi * 16 + gq + 8 * i;
+          *reinterpret_cast<float2*>(p.partial + m * p.Nld + n) = make_float2(acc[mi][j][2 * i], acc[mi][j][2 * i + 1]);
+        }
+      }
+    }
   }
 }
 
@@ -552,7 +453,8 @@ __global__ void wgrad_reduce_kernel(const __grid_constant__ RGroup g) {
 
 struct WPlan { int BN, n_tiles, m_tiles, nsplit, rows_per_split, Mpad, Nld; };
 // `rows_target`: contraction rows per work item.  512 sizes the partial buffers (the CAPACITY in row splits); the grouped
-// launch may raise it so that the item count of the whole group fills whole rounds of the persistent grid.
+// launch may raise it so that the item count of the whole group fills whole waves (one CTA per work item; at ~170
+// registers x 256 threads one CTA is resident per SM, so a wave is num_sms() items).
 WPlan wgrad_plan(int M, int N, long long rows, int rows_target = 512) {
   WPlan w;
   w.m_tiles = (int)ceil_div(M, BM);
@@ -609,16 +511,94 @@ void plan(long long M, int N, int* BN, int* n_tiles) {
   int nt = (int)ceil_div(N, MAX_BN);
   while (m_tiles * nt < 120 && round_up(ceil_div(N, nt + 1), 32) >= 64) ++nt;   // spread over the SMs
   *n_tiles = nt;
-  *BN = nt == 1 ? (int)round_up(N, 16) : (int)round_up(ceil_div(N, nt), 32);
+  *BN = (int)round_up(ceil_div(N, nt), 32);     // whole 32-column MMA chunks
 }
 
-
-int ensure_attr(const void* fn, int) { return ensure_max_smem(fn, SMEM_LIMIT); }
 
 }  // namespace
 
 static unsigned long long* g_gemm_dbg = nullptr;
 void tc_gemm_set_debug(unsigned long long* buf) { g_gemm_dbg = buf; }
+
+int tc_nt(const TcNtArgs& a, cudaStream_t st) {
+  if (a.BN < 32 || a.BN > 32 * NCH_MAX || a.BN % 32 || a.n_tiles < 1 || a.M < 1 || a.M > 0x7fffffffLL || a.K % 4 ||
+      a.N % 4 || a.lda % 4) {
+    set_error("tc_nt: unsupported tiling / shape (M=%lld N=%d K=%d BN=%d)", a.M, a.N, a.K, a.BN);
+    return -2;
+  }
+  if ((reinterpret_cast<uintptr_t>(a.A) | reinterpret_cast<uintptr_t>(a.B) | reinterpret_cast<uintptr_t>(a.B_lo) |
+       reinterpret_cast<uintptr_t>(a.C) | reinterpret_cast<uintptr_t>(a.gate) | reinterpret_cast<uintptr_t>(a.resid)) & 15) {
+    set_error("tc_nt: pointers must be 16-byte aligned");
+    return -2;
+  }
+  const bool exact = a.B_lo != nullptr;
+  NtP p;
+  p.M = a.M; p.N = a.N; p.K = a.K; p.BN = a.BN; p.nch = a.BN / 32; p.n_tiles = a.n_tiles;
+  p.m_tiles = (int)ceil_div(a.M, BM);
+  p.k_blocks = (int)ceil_div(a.K, BK);
+  const int stage_bytes = A_TILE + (exact ? 2 : 1) * a.BN * 128;
+  const int fixed = 1024 + 256;
+  p.nstages = (SMEM_LIMIT - fixed) / stage_bytes;
+  if (p.nstages > MAX_STAGES) p.nstages = MAX_STAGES;
+  if (p.nstages < 2) { set_error("tc_nt: not enough shared memory"); return -2; }
+  const int smem_bytes = fixed + p.nstages * stage_bytes;
+  p.C = a.C; p.ldc = a.N;
+  p.bias = a.bias; p.scale = a.scale; p.scale_mod = a.scale_mod > 0 ? a.scale_mod : 1;
+  p.gate = a.gate; p.gate_ld = a.gate_ld; p.gate_scale = a.gate_scale;
+  p.drop_p = a.drop_p; p.rng = a.rng; p.drop_site = a.drop_site; p.drop_mask = a.drop_mask; p.drop_mask_ld = a.drop_mask_ld;
+  p.resid = a.resid; p.resid_ld = a.resid_ld;
+  p.pB = a.pB; p.pN = a.pN; p.pD = a.pD;
+  p.dbg = g_gemm_dbg;
+
+  CUtensorMap tmA, tmB, tmBlo;
+  {
+    cuuint64_t d[2] = {(cuuint64_t)a.K, (cuuint64_t)a.M};
+    cuuint64_t s[1] = {(cuuint64_t)a.lda * 4};
+    cuuint32_t b[2] = {BK, BM};
+    RD_TRY(encode(&tmA, a.A, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "A"));
+  }
+  {
+    cuuint64_t d[2] = {(cuuint64_t)a.K, (cuuint64_t)a.N};
+    cuuint64_t s[1] = {(cuuint64_t)a.K * 4};
+    cuuint32_t b[2] = {BK, (cuuint32_t)a.BN};
+    RD_TRY(encode(&tmB, a.B, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "B"));
+    if (exact) RD_TRY(encode(&tmBlo, a.B_lo, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "B_lo"));
+    else tmBlo = tmB;
+  }
+  const int total = p.m_tiles * p.n_tiles;
+  const int grid = total < num_sms() ? total : num_sms();
+  const int f = (a.relu ? F_RELU : 0) | (a.scale ? F_SCALE : 0) | (a.gate ? F_GATE : 0) | (a.drop_p > 0.f ? F_DROP : 0) |
+                (a.resid ? F_RESID : 0) | (a.round_out ? F_ROUND : 0) | (a.perm ? F_PERM : 0);
+  auto launch = [&](auto kern) -> int {
+    RD_TRY(ensure_max_smem((const void*)kern, SMEM_LIMIT));   // once per (instantiation, device)
+    launch_pdl(kern, dim3(grid), dim3(NT_THREADS), smem_bytes, st, tmA, tmB, tmBlo, p);
+    return 0;
+  };
+  int rc = -2;
+#define RD_NT_CASE(FLAGS, EX) \
+  if (f == (FLAGS) && exact == (EX)) rc = launch(tc_nt_kernel<(FLAGS), (EX)>); else
+  // observation propagation: layer 2 -> encoder input, layer 1 (rounded for the next single-pass layer), the plain
+  // operator, backward d(input); encoder: bias[,relu][,dropout][,residual] forward, [gate][,residual] backward
+  RD_NT_CASE(F_PERM | F_RELU | F_SCALE, false)
+  RD_NT_CASE(F_RELU | F_SCALE | F_ROUND, false)
+  RD_NT_CASE(F_RELU | F_SCALE, false)
+  RD_NT_CASE(F_GATE | F_SCALE, false)
+  RD_NT_CASE(F_PERM | F_RELU | F_SCALE, true)
+  RD_NT_CASE(F_RELU | F_SCALE, true)
+  RD_NT_CASE(F_GATE | F_SCALE, true)
+  RD_NT_CASE(0, true)
+  RD_NT_CASE(F_RESID, true)
+  RD_NT_CASE(F_DROP, true)
+  RD_NT_CASE(F_DROP | F_RESID, true)
+  RD_NT_CASE(F_GATE, true)
+  RD_NT_CASE(F_RELU, true)
+  RD_NT_CASE(F_RELU | F_DROP, true)
+  { set_error("tc_nt: epilogue combination %d (exact=%d) not instantiated", f, (int)exact); return -2; }
+#undef RD_NT_CASE
+  if (rc != 0) return rc;
+  RD_CHECK_LAUNCH("tc_nt_kernel");
+  return 0;
+}
 
 bool tc_gemm_supported(const TcGemmArgs& a) {
   static int env = -1;
@@ -635,60 +615,13 @@ bool tc_gemm_supported(const TcGemmArgs& a) {
 
 int tc_gemm(const TcGemmArgs& a, cudaStream_t st) {
   if (!tc_gemm_supported(a)) { set_error("tc_gemm: unsupported shape/alignment (M=%lld N=%d K=%d)", a.M, a.N, a.K); return -2; }
-  P p;
-  p.A = a.A; p.lda = a.lda; p.M = a.M; p.N = a.N; p.K = a.K;
-  plan(a.M, a.N, &p.BN, &p.n_tiles);
-  p.m_tiles = (int)ceil_div(a.M, BM);
-  p.k_blocks = (int)ceil_div(a.K, BK);
-  const int stage_bytes = A_TILE + 2 * p.BN * 128;
-  const int fixed = 1024 + 8 * STG_BYTES + 2 * 256 * 4 + 256;
-  p.nstages = (SMEM_LIMIT - fixed) / stage_bytes;
-  if (p.nstages > MAX_STAGES) p.nstages = MAX_STAGES;
-  if (p.nstages < 2) { set_error("tc_gemm: not enough shared memory"); return -2; }
-  const int smem_bytes = fixed + p.nstages * stage_bytes;
-  p.bias = a.bias; p.relu = a.relu; p.gate = a.gate; p.gate_ld = a.gate_ld; p.gate_scale = a.gate_scale;
-  p.drop_p = a.drop_p; p.rng = a.rng; p.drop_site = a.drop_site; p.resid = a.resid; p.resid_ld = a.resid_ld;
-  p.drop_mask = a.drop_mask; p.drop_mask_ld = a.drop_mask_ld;
-  p.dbg = g_gemm_dbg;
-
-  CUtensorMap tmA, tmB, tmBlo, tmC;
-  {
-    cuuint64_t ad[2] = {(cuuint64_t)a.K, (cuuint64_t)a.M};
-    cuuint64_t as_[1] = {(cuuint64_t)a.lda * 4};
-    cuuint32_t ab[2] = {BK, BM};
-    RD_TRY(encode(&tmA, a.A, 2, ad, as_, ab, CU_TENSOR_MAP_SWIZZLE_128B, "A"));
-  }
-  cuuint64_t bd[2] = {(cuuint64_t)a.K, (cuuint64_t)a.N};
-  cuuint64_t bs[1] = {(cuuint64_t)a.K * 4};
-  cuuint32_t bb[2] = {BK, (cuuint32_t)p.BN};
-  RD_TRY(encode(&tmB, a.B, 2, bd, bs, bb, CU_TENSOR_MAP_SWIZZLE_128B, "B"));
-  RD_TRY(encode(&tmBlo, a.B_lo, 2, bd, bs, bb, CU_TENSOR_MAP_SWIZZLE_128B, "B_lo"));
-  cuuint64_t cd[2] = {(cuuint64_t)a.N, (cuuint64_t)a.M};
-  cuuint64_t cs[1] = {(cuuint64_t)a.N * 4};
-  cuuint32_t cb[2] = {32, 32};
-  RD_TRY(encode(&tmC, a.C, 2, cd, cs, cb, CU_TENSOR_MAP_SWIZZLE_128B, "C"));
-  const int total = p.m_tiles * p.n_tiles;
-  const int grid = total < num_sms() ? total : num_sms();
-  auto launch = [&](auto kern, int id) -> int {
-    RD_TRY(ensure_attr((const void*)kern, id));
-    launch_pdl(kern, dim3(grid), dim3(NTHREADS), smem_bytes, st, tmA, tmB, tmBlo, tmC, p);
-    return 0;
-  };
-  const int id = (a.relu ? 8 : 0) | (a.gate ? 4 : 0) | (a.drop_p > 0.f ? 2 : 0) | (a.resid ? 1 : 0);
-  int rc = -2;
-  switch (id) {   // the combinations the encoder uses (forward: bias[,relu][,dropout][,residual]; backward: [gate][,residual])
-    case 0: rc = launch(tc_gemm_kernel<false, false, false, false>, id); break;
-    case 1: rc = launch(tc_gemm_kernel<false, false, false, true>, id); break;
-    case 2: rc = launch(tc_gemm_kernel<false, false, true, false>, id); break;
-    case 3: rc = launch(tc_gemm_kernel<false, false, true, true>, id); break;
-    case 4: rc = launch(tc_gemm_kernel<false, true, false, false>, id); break;
-    case 8: rc = launch(tc_gemm_kernel<true, false, false, false>, id); break;
-    case 10: rc = launch(tc_gemm_kernel<true, false, true, false>, id); break;
-    default: set_error("tc_gemm: epilogue combination %d not instantiated", id); return -2;
-  }
-  if (rc != 0) return rc;
-  RD_CHECK_LAUNCH("tc_gemm_kernel");
-  return 0;
+  TcNtArgs n;
+  n.A = a.A; n.lda = a.lda; n.B = a.B; n.B_lo = a.B_lo; n.M = a.M; n.N = a.N; n.K = a.K; n.C = a.C;
+  plan(a.M, a.N, &n.BN, &n.n_tiles);
+  n.bias = a.bias; n.relu = a.relu; n.gate = a.gate; n.gate_ld = a.gate_ld; n.gate_scale = a.gate_scale;
+  n.drop_p = a.drop_p; n.rng = a.rng; n.drop_site = a.drop_site; n.drop_mask = a.drop_mask; n.drop_mask_ld = a.drop_mask_ld;
+  n.resid = a.resid; n.resid_ld = a.resid_ld;
+  return tc_nt(n, st);
 }
 
 bool tc_wgrad_supported(int Nout, int Kin, long long ldy, long long ldx, const void* dY, const void* X) {
@@ -710,7 +643,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
   WGroup g;
   RGroup r;
   g.n = n; r.n = n + (ncs > 0 ? ncs : 0);
-  // rows per work item: the smallest target >= 512 for which the group's item count fills whole rounds of the grid
+  // rows per work item: the smallest target >= 512 for which the group's item count fills whole waves of the grid
   auto count_items = [&](int target) {
     long long t = 0;
     for (int i = 0; i < n; ++i) { const WPlan w = wgrad_plan(items[i].Nout, items[i].Kin, items[i].rows, target); t += (long long)w.nsplit * w.m_tiles * w.n_tiles; }
@@ -738,13 +671,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
     WP& p = g.it[i];
     p.partial = a.partial;
     p.rows = a.rows; p.M = a.Nout; p.N = a.Kin;
-    {
-      cuuint32_t box[2] = {32, BK};
-      cuuint64_t da[2] = {(cuuint64_t)a.Nout, (cuuint64_t)a.rows}, sa_[1] = {(cuuint64_t)a.ldy * 4};
-      RD_TRY(encode(&g.tmA[i], a.dY, 2, da, sa_, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, "wgrad dY"));
-      cuuint64_t db_[2] = {(cuuint64_t)a.Kin, (cuuint64_t)a.rows}, sb_[1] = {(cuuint64_t)a.ldx * 4};
-      RD_TRY(encode(&g.tmB[i], a.X, 2, db_, sb_, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, "wgrad X"));
-    }
+    p.dY = a.dY; p.X = a.X; p.ldy = a.ldy; p.ldx = a.ldx;
     p.BN = w.BN; p.n_tiles = w.n_tiles; p.m_tiles = w.m_tiles; p.nsplit = w.nsplit; p.rows_per_split = w.rows_per_split;
     p.Mpad = w.Mpad; p.Nld = w.Nld;
     if (p.BN > max_bn) max_bn = p.BN;
@@ -758,12 +685,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
     tot += (long long)a.Nout * (a.Kin / 4 + 1);
   }
   g.total_items = item;
-  g.stage_bytes = 2 * A_TILE + 2 * max_bn * 128;
-  const int fixed = 1024 + 256;
-  g.nstages = (SMEM_LIMIT - fixed) / g.stage_bytes;
-  if (g.nstages > MAX_STAGES) g.nstages = MAX_STAGES;
-  if (n > 0 && g.nstages < 2) { set_error("tc_wgrad_group: not enough shared memory"); return -2; }
-  const int smem_bytes = fixed + g.nstages * g.stage_bytes;
+  const int smem_bytes = 2 * (WBK * LDA_W + WBK * (max_bn + 8)) * (int)sizeof(float);
   for (int i = 0; i < ncs; ++i) {
     RItem& q = r.it[n + i];
     q.partial = cs[i].partial; q.dW = cs[i].out; q.db = nullptr; q.nsplit = cs[i].nsplit; q.M = 1; q.N = cs[i].ncols;
@@ -774,9 +696,8 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
   }
   r.total = tot;
   if (n > 0) {
-    RD_TRY(ensure_attr((const void*)tc_wgrad_kernel, 15));
-    const int grid = item < num_sms() ? item : num_sms();
-    launch_pdl(tc_wgrad_kernel, dim3(grid), dim3(W_THREADS), smem_bytes, st, g);
+    RD_TRY(ensure_max_smem((const void*)tc_wgrad_kernel, smem_bytes));
+    launch_pdl(tc_wgrad_kernel, dim3(item), dim3(W_THREADS), smem_bytes, st, g);
     RD_CHECK_LAUNCH("tc_wgrad_kernel");
   }
   launch_pdl(wgrad_reduce_kernel, dim3((unsigned)ceil_div(tot, 256)), dim3(256), 0, st, r);

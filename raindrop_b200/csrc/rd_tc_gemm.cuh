@@ -1,13 +1,35 @@
-// Error-compensated tensor-core GEMM for the temporal-attention encoder (rd_tc_gemm.cu).
+// Tensor-core GEMMs (rd_tc_gemm.cu): the shared wgmma NT kernel, the encoder's error-compensated GEMM and the grouped
+// weight gradients.
 #pragma once
 #include "rd_common.cuh"
 
 namespace rd {
 
+// C[M, N] = epi(A[M, K] . B[N, K]^T) on the wgmma tensor cores; B_lo != null selects the error-compensated mode
+// (3xTF32: A is split in registers, B_lo = B - trunc19(B) is precomputed), else single-pass TF32 on operands the caller
+// keeps TF32-representable.  epi = +bias[col] -> relu -> *scale[row % scale_mod] -> *(gate > 0 ? gate_scale : 0) ->
+// dropout (+ keep bits) -> +resid -> RN to TF32 (round_out); perm != 0 stores row b*pN + n, col t*4 + k into
+// C[(t*pB + b)*pD + n*4 + k].  BN (a multiple of 32, <= 256) and n_tiles are the caller's tiling of N.
+struct TcNtArgs {
+  const float* A = nullptr; long long lda = 0;
+  const float* B = nullptr; const float* B_lo = nullptr;
+  long long M = 0; int N = 0, K = 0, BN = 0, n_tiles = 0;
+  float* C = nullptr;
+  const float* bias = nullptr; int relu = 0;
+  const float* scale = nullptr; int scale_mod = 1;
+  const float* gate = nullptr; long long gate_ld = 0; float gate_scale = 1.f;
+  float drop_p = 0.f; const uint64_t* rng = nullptr; uint32_t drop_site = 0;
+  uint32_t* drop_mask = nullptr; int drop_mask_ld = 0;
+  const float* resid = nullptr; long long resid_ld = 0;
+  int round_out = 0;
+  int perm = 0, pB = 0, pN = 0, pD = 0;
+};
+int tc_nt(const TcNtArgs& a, cudaStream_t st);
+
 // C[M,N] = epi( A[M,K] . B[N,K]^T ) with fp32-level accuracy on the TF32 tensor cores ("3xTF32"):
 //   A = A_hi + A_lo, B = B_hi + B_lo (hi = top 19 bits, what the MMA reads; lo = exact remainder)
 //   A.B^T ~= A_hi.B_hi^T + A_lo.B_hi^T + A_hi.B_lo^T          (dropped term ~2^-22 relative)
-// A (activations) is split on the fly by the loader warps; B (a weight) comes with its precomputed
+// A (activations) is split on the fly in registers; B (a weight) comes with its precomputed
 // remainder B_lo (split_weights below).  epi = +bias[j] -> relu -> *gate -> dropout -> +resid.
 struct TcGemmArgs {
   const float* A = nullptr; long long lda = 0;
@@ -25,10 +47,8 @@ void tc_gemm_set_debug(unsigned long long* buf);     // %globaltimer phase stamp
 int tc_gemm(const TcGemmArgs& a, cudaStream_t st);
 
 // Weight gradient on the tensor cores: dW[Nout, Kin] = sum_r dY[r, Nout]^T X[r, Kin], db[Nout] = sum_r dY[r, :]
-// (the bias gradient rides along as one extra "ones" column of X).  Both operands are activations: the
-// loader warps read them row-major (coalesced), transpose 4x4 blocks in registers, split hi/lo and write
-// the K-major swizzled tiles.  The row range is split across CTAs; partial tiles go to `partial`
-// (tc_wgrad_partial_floats(...) floats) and are summed in a fixed order (deterministic).
+// (the bias gradient rides along as one extra "ones" column of X).  The row range is split across CTAs; partial tiles
+// go to `partial` (tc_wgrad_partial_floats(...) floats) and are summed in a fixed order (deterministic).
 bool tc_wgrad_supported(int Nout, int Kin, long long ldy, long long ldx, const void* dY, const void* X);
 long long tc_wgrad_partial_floats(int Nout, int Kin, long long rows);
 int tc_wgrad(const float* dY, long long ldy, const float* X, long long ldx, long long rows, int Nout, int Kin,

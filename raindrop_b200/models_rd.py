@@ -3,7 +3,7 @@
 `from models_rd import *` in code/Raindrop.py:19 must find `Raindrop_v2`, `Raindrop`,
 `PositionalEncodingTF`, `Observation_progation`, `TransformerConv` with the reference's constructor
 signatures, forward signatures and state-dict keys (SURVEY.md section 8b).  Everything numeric is
-done by librd_b200.so (hand-written sm_100a CUDA) through `raindrop_b200.functional`; the torch
+done by librd_b200.so (hand-written sm_90a CUDA) through `raindrop_b200.functional`; the torch
 modules below only hold parameters so that `.cuda()`, `.parameters()`, `state_dict()` and
 `load_state_dict()` behave exactly like the reference's.
 """

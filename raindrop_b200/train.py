@@ -1,5 +1,5 @@
 """Training-step plumbing around the C ABI: the ops code/Raindrop.py:319-324 performs per batch
-(forward, CrossEntropyLoss, backward, Adam) plus the one collective the B200 build adds -- a single
+(forward, CrossEntropyLoss, backward, Adam) plus the one collective the CUDA build adds -- a single
 NCCL all-reduce over the flat fp32 bucket of the gradients that exist (SURVEY.md section 8e).
 
 Two ways to run a step:

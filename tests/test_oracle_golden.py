@@ -1,5 +1,7 @@
 """CPU: pins the oracle restatement (oracle/raindrop_oracle.py) against the golden fixtures that were
 generated from the reference's own unmodified files (oracle/make_golden.py)."""
+import hashlib
+
 import numpy as np
 import pytest
 import torch
@@ -91,21 +93,20 @@ def test_graph_and_pe_conventions():
     assert abs(pe[0, 1, 7].item() - np.sin(np.float32(3.0) / np.float32(60.0))) < 1e-7
 
 
-def test_live_reference_if_present():
-    """In the build container the reference tree exists: run it directly against the oracle."""
-    from oracle import ref_harness
-    if not ref_harness.reference_available() or torch.cuda.is_available():
-        pytest.skip("reference tree only exists in the (GPU-less) build container")
+def test_reference_model_matches_oracle(golden_dir):
+    """The reference's own Raindrop_v2 on the TINY configuration (live_tiny.npz, oracle/make_golden.py) against the
+    oracle: bit-identical initial state dict (SHA-256 of every tensor), same eval-mode logits."""
     from raindrop_b200.synth import make_batch, model_config
+    z = np.load(golden_dir + "/live_tiny.npz")
     cfg = model_config("TINY", dropout=0.2)
-    ref = ref_harness.build_reference_model(cfg).eval()
     orc = build_oracle_model(cfg).eval()
-    assert all(torch.equal(a, b) for a, b in zip(ref.state_dict().values(), orc.state_dict().values()))
+    digests = [hashlib.sha256(v.contiguous().numpy().tobytes()).hexdigest() for v in orc.state_dict().values()]
+    assert digests == [str(d) for d in z["state_sha256"]]          # bit-identical initial weights
     batch = make_batch(cfg, 3, seed=1)
     with torch.no_grad():
-        a = ref.forward(batch["src"], batch["static"], batch["times"], batch["lengths"])[0]
         b = orc.forward(batch["src"], batch["static"], batch["times"], batch["lengths"])[0]
-    assert torch.equal(a, b)
+    # stored on another machine: the same float32 arithmetic, but the CPU kernels may sum in another order
+    assert normwise(b, z["logits"]) < 1e-6
 
 
 @pytest.mark.parametrize("seed", range(6))

@@ -1,4 +1,4 @@
-"""Scratch micro-benchmarks for the GPU box (not the driver's bench; see bench.py)."""
+"""Scratch micro-benchmarks of single kernels (the benchmark of record is bench.py)."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -33,8 +33,8 @@ def layer_bench(C, N, B):
     med, best = timeit(fn)
     gb = rows * C * 8 / 1e9
     tf = 2 * rows * C * C / 1e12
-    print("obprop layer C=%d rows=%d: median %.3f ms best %.3f ms -> %.0f GB/s (%.1f%% of 6571.9), %.1f TFLOP/s"
-          % (C, rows, med, best, gb / (best * 1e-3), 100 * gb / (best * 1e-3) / 6571.9, tf / (best * 1e-3)))
+    print("obprop layer C=%d rows=%d: median %.3f ms best %.3f ms -> %.0f GB/s (%.1f%% of the 3.35 TB/s H100 data sheet), %.1f TFLOP/s"
+          % (C, rows, med, best, gb / (best * 1e-3), 100 * gb / (best * 1e-3) / 3350.0, tf / (best * 1e-3)))
 
 
 if __name__ == "__main__":

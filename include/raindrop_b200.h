@@ -202,7 +202,10 @@ int rd_raindrop_v2_fwd(const rd_dims* dims, const rd_params* params, const float
  *   RD_BWD_ENCODER  head + temporal-attention encoder: every gradient except the two lin_value pairs is final
  *                   when the call's work completes; d(loss)/d(encoder input) stays in `scratch`
  *   RD_BWD_OBPROP   observation propagation: ob1/ob2 lin_value gradients (needs the same scratch, after ENCODER)
- *   both (3)        whole backward, weight gradients in one grouped tensor-core launch                    */
+ *   both (3)        whole backward, weight gradients in one grouped tensor-core launch
+ * grads == NULL (frozen parameters, e.g. attribution with model.requires_grad_(False)): only the data-gradient chain
+ * runs -- no weight-gradient GEMMs, column sums or head outer products -- and `scratch` is left holding the same
+ * activation gradients, ready for rd_raindrop_v2_input_grad.                                               */
 #define RD_BWD_ENCODER 1
 #define RD_BWD_OBPROP 2
 #define RD_BWD_ALL 3
@@ -218,13 +221,33 @@ int rd_raindrop_v2_bwd(const rd_dims* dims, const rd_params* params, const float
  * [T, B, D = N*d_ob + d_pe] into the workspace buffer RD_WS_ENC_IN first (rd_workspace_offset), then calls _fwd;
  * _bwd fills every encoder / emb / mlp_static gradient of `grads` (the ob-prop members are ignored) and writes
  * d(loss)/d(encoder input) to d_enc_in [T, B, D].  Same workspace / scratch sizes and rng protocol as
- * rd_raindrop_v2_fwd / _bwd. */
+ * rd_raindrop_v2_fwd / _bwd; grads may be NULL as there. */
 int rd_encoder_head_fwd(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
                         uint64_t* rng_state, void* workspace, float* logits, const int64_t* y, float* loss,
                         float* d_logits, void* stream);
 int rd_encoder_head_bwd(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
                         const void* workspace, const float* d_logits, const rd_grads* grads, void* scratch,
                         float* d_enc_in, void* stream);
+/* ---- gradients with respect to the inputs src, static and times ----------------------------------------------
+ * For saliency maps, integrated gradients and other attribution methods, and for adversarial training.  Call it
+ * after rd_raindrop_v2_bwd (phases including RD_BWD_OBPROP) or rd_encoder_head_bwd, on the same stream, with the
+ * same dims / params, the forward's workspace and the backward's scratch `bwd_scratch` untouched in between: the
+ * backward leaves d(loss)/d(encoder input), d(loss)/d(layer-1 pre-activation) and d(loss)/d(cat(pooled, emb)) there,
+ * and this call finishes the chain through the first ob-prop layer, the lift (code/models_rd.py:285-296,323-327),
+ * the positional encoding (:28-37) and emb = Linear(d_static, N) (:293-294).  Outputs (written, not accumulated;
+ * each may be NULL, which skips its part):
+ *   d_src     [T, B, 2N]  value half d(loss)/d(src[..., :N]); the mask half is unused on the live path and written
+ *                         as 0; 0 wherever the value is 0 (relu'(0) = 0).  Train mode replays the forward's lift
+ *                         dropout mask.  Needs `scratch` (rd_input_grad_scratch_bytes(dims) bytes) and `src`.
+ *   d_times   [T, B]      0 on padded rows t >= lengths[b] (lengths may be NULL: no forced zeros).
+ *   d_statics [B, d_static]
+ * d_src and d_times need the Raindrop_v2 workspace; after rd_encoder_head_bwd only d_statics is available (the
+ * encoder input gradient went to the caller's d_enc_in).  `scratch` may be NULL when d_src is NULL. */
+size_t rd_input_grad_scratch_bytes(const rd_dims* dims);
+int rd_raindrop_v2_input_grad(const rd_dims* dims, const rd_params* params, const float* src, const float* times,
+                              const int64_t* lengths, const void* workspace, const void* bwd_scratch, void* scratch,
+                              float* d_src, float* d_times, float* d_statics, void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);
@@ -234,6 +257,10 @@ int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured,
  * Replaces PositionalEncodingTF.getPE (code/models_rd.py:28-37) without the host round trip. */
 int rd_positional_encoding(const float* times, int64_t n_tokens, const float* timescales_host, int32_t d_pe,
                            float* out, int64_t ld, int32_t col0, void* stream);
+/* Its backward: d_times[tok] = sum_k d_pe[tok*ld + col0 + k] cos(times/ts_k)/ts_k - d_pe[tok*ld + col0 + d_pe_width/2 + k]
+ * sin(times/ts_k)/ts_k, k < d_pe_width/2 (the module-level PositionalEncodingTF is differentiable in times). */
+int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,
+                               int32_t d_pe_width, int64_t ld, int32_t col0, float* d_times, void* stream);
 
 /* out[rows, out_f] = [relu](x[rows, in_f] . weight[out_f, in_f]^T + bias): the encoder's projection
  * GEMM on its own (torch.nn.Linear inside nn.TransformerEncoderLayer, code/models_rd.py:232-237).

@@ -260,6 +260,80 @@ __global__ void lift_posenc_kernel(const float* __restrict__ src, const float* _
   pe_out[tok * ld + col0 + j] = (j < half) ? sinf(scaled) : cosf(scaled);
 }
 
+// Backward of lift_posenc_kernel plus the static embedding, one launch, three thread ranges:
+//   o <  n_lift : d_src[t,b,n] = sum_k dX0[(b*N+n), t*d_ob+k] * keep/(1-p) * [src*R_u > 0] * R_u[n*d_ob+k]  (one thread per
+//                 (row, t), same Philox block as the forward); d_src[t,b,N+n] = 0 (the mask half is unused)
+//   next n_tok  : d_times[tok] = sum_j g[tok*ld + col0 + j] cos(t/ts_j)/ts_j - g[tok*ld + col0 + half + j] sin(t/ts_j)/ts_j,
+//                 exactly 0 for t >= lengths[b] when lengths is given (padded rows get no gradient in the reference)
+//   rest        : d_static[b,k] = sum_n dfeat[b*Df + feat_col0 + n] * W_emb[n*ds + k]
+struct InputGradArgs {
+  const float* src; const float* R_u; const float* dX0; float* d_src; long long n_lift; int B, T, N, d_ob; float drop_p;
+  const uint64_t* rng;
+  const float* times; const float* g_pe; long long n_tokens, ld; int col0; const int64_t* lengths; float* d_times;
+  const float* dfeat; const float* W_emb; int Df, feat_col0, emb, ds; float* d_static; long long n_static;
+};
+__global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const __grid_constant__ TS8 ts) {
+  pdl_launch_dependents();
+  pdl_wait();
+  long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o < a.n_lift) {
+    const long long row = o / a.T;
+    const int t = (int)(o - row * a.T);
+    const int b = (int)(row / a.N), n = (int)(row - (long long)b * a.N);
+    float* ds = a.d_src + ((long long)t * a.B + b) * (2 * a.N);
+    const float sv = __ldg(a.src + ((long long)t * a.B + b) * (2 * a.N) + n);
+    const float ik = a.drop_p > 0.f ? 1.f / (1.f - a.drop_p) : 1.f;
+    const uint64_t idx0 = ((uint64_t)t * a.B + b) * (uint64_t)(a.N * a.d_ob) + (uint64_t)(n * a.d_ob);
+    const float* g = a.dX0 + row * ((long long)a.T * a.d_ob) + (long long)t * a.d_ob;
+    float acc = 0.f;
+    if (a.d_ob == 4) {
+      const float4 r = __ldg(reinterpret_cast<const float4*>(a.R_u) + n);
+      float4 d = __ldg(reinterpret_cast<const float4*>(g));
+      if (a.drop_p > 0.f) {
+        const float4 m = dropout_scale4(a.rng, SITE_LIFT, idx0, a.drop_p, ik);
+        d.x *= m.x; d.y *= m.y; d.z *= m.z; d.w *= m.w;
+      }
+      acc = (sv * r.x > 0.f ? d.x * r.x : 0.f) + (sv * r.y > 0.f ? d.y * r.y : 0.f) +
+            (sv * r.z > 0.f ? d.z * r.z : 0.f) + (sv * r.w > 0.f ? d.w * r.w : 0.f);
+    } else {
+      for (int k = 0; k < a.d_ob; ++k) {
+        const float r = __ldg(a.R_u + n * a.d_ob + k);
+        float d = __ldg(g + k);
+        if (a.drop_p > 0.f) d *= dropout_scale(a.rng, SITE_LIFT, idx0 + k, a.drop_p, ik);
+        acc += sv * r > 0.f ? d * r : 0.f;
+      }
+    }
+    ds[n] = acc;
+    ds[a.N + n] = 0.f;
+    return;
+  }
+  o -= a.n_lift;
+  if (o < a.n_tokens) {
+    const int half = ts.d_pe >> 1;
+    const float* g = a.g_pe + o * a.ld + a.col0;
+    const float tv = __ldg(a.times + o);
+    float acc = 0.f;
+    for (int j = 0; j < half; ++j) {
+      const float scaled = tv / ts.v[j];
+      acc += (__ldg(g + j) * cosf(scaled) - __ldg(g + half + j) * sinf(scaled)) / ts.v[j];
+    }
+    if (a.lengths) {      // token o = t*B + b
+      const long long t = o / a.B, b = o - t * a.B;
+      if (t >= __ldg(a.lengths + b)) acc = 0.f;
+    }
+    a.d_times[o] = acc;
+    return;
+  }
+  o -= a.n_tokens;
+  if (o >= a.n_static) return;
+  const long long b = o / a.ds;
+  const int k = (int)(o - b * a.ds);
+  const float* df = a.dfeat + b * a.Df + a.feat_col0;
+  float acc = 0.f;
+  for (int n = 0; n < a.emb; ++n) acc = fmaf(__ldg(df + n), __ldg(a.W_emb + (long long)n * a.ds + k), acc);
+  a.d_static[o] = acc;
+}
+
 // one warp per node: segment max, then sum of exp, then s = sum(exp / (sum + 1e-16))
 __global__ void node_scale_kernel(const int64_t* __restrict__ tgt, const float* __restrict__ w, int E, int N,
                                   float* __restrict__ s) {
@@ -837,6 +911,29 @@ int lift_posenc(const float* src, const float* R_u, int B, int T, int N, int d_o
 int posenc(const float* times, int64_t n_tokens, const float* ts_host, int d_pe, float* out, int64_t ld, int col0,
            cudaStream_t st) {
   return lift_posenc(nullptr, nullptr, 0, 0, 0, 0, 0.f, nullptr, 0, nullptr, times, n_tokens, ts_host, d_pe, out, ld, col0, st);
+}
+
+int input_grad(const float* src, const float* R_u, const float* dX0, int B, int T, int N, int d_ob, float drop_p,
+               const uint64_t* rng, float* d_src, const float* times, const float* g_pe, int64_t n_tokens, int64_t ld, int col0,
+               const float* ts_host, int d_pe, const int64_t* lengths, float* d_times, const float* dfeat, int Df, int feat_col0,
+               const float* W_emb, int emb, int ds, float* d_static, cudaStream_t st) {
+  if (d_times && (d_pe < 2 || d_pe > 64 || (d_pe & 1))) { set_error("positional encoding width must be even and <= 64"); return -2; }
+  InputGradArgs a;
+  a.src = src; a.R_u = R_u; a.dX0 = dX0; a.d_src = d_src; a.n_lift = d_src ? (int64_t)B * N * T : 0;
+  a.B = B; a.T = T; a.N = N; a.d_ob = d_ob; a.drop_p = drop_p; a.rng = rng;
+  a.times = times; a.g_pe = g_pe; a.n_tokens = d_times ? n_tokens : 0; a.ld = ld; a.col0 = col0; a.lengths = lengths;
+  a.d_times = d_times;
+  a.dfeat = dfeat; a.W_emb = W_emb; a.Df = Df; a.feat_col0 = feat_col0; a.emb = emb; a.ds = ds; a.d_static = d_static;
+  a.n_static = (d_static && ds > 0) ? (int64_t)B * ds : 0;
+  TS8 ts;
+  memset(&ts, 0, sizeof(ts));
+  ts.d_pe = d_times ? d_pe : 2;
+  if (d_times) memcpy(ts.v, ts_host, sizeof(float) * (d_pe / 2));
+  const int64_t total = a.n_lift + a.n_tokens + a.n_static;
+  if (total <= 0) return 0;
+  launch_pdl(input_grad_kernel, dim3(blocks_for(total)), dim3(TPB), 0, st, a, ts);
+  RD_CHECK_LAUNCH("input_grad_kernel");
+  return 0;
 }
 
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st) {

@@ -34,6 +34,17 @@ int transpose_round(const float* x, int rows, int cols, float* y, cudaStream_t s
 int posenc(const float* times, int64_t n_tokens, const float* ts_host, int d_pe, float* out, int64_t ld, int col0,
            cudaStream_t st);
 
+// Backward of lift_posenc and of the static embedding in one launch (each output may be null, which skips its part):
+//   d_src [T, B, 2N]  from dX0 = d(loss)/d(X0) [B*N, T*d_ob] (the forward's lift dropout mask is replayed from rng;
+//                     the mask half is written as 0)
+//   d_times [n_tokens] from the positional-encoding columns g_pe[tok*ld + col0 .. + d_pe); lengths (optional, token
+//                     = t*B + b) zeroes the padded rows t >= lengths[b]
+//   d_static [B, ds]  = dfeat[:, feat_col0 : feat_col0 + emb] . W_emb   (W_emb: [emb, ds])
+int input_grad(const float* src, const float* R_u, const float* dX0, int B, int T, int N, int d_ob, float drop_p,
+               const uint64_t* rng, float* d_src, const float* times, const float* g_pe, int64_t n_tokens, int64_t ld, int col0,
+               const float* ts_host, int d_pe, const int64_t* lengths, float* d_times, const float* dfeat, int Df, int feat_col0,
+               const float* W_emb, int emb, int ds, float* d_static, cudaStream_t st);
+
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 
 // y = LN(x) * gamma + beta over the last dim (width D); stats[row] = {mean, rstd}
@@ -65,7 +76,7 @@ int head_fwd(int B, int T, int D, int N, int ds, int ncls, const float* x, const
              const float* emb_w, const float* emb_b, const float* w0, const float* b0, const float* w2, const float* b2,
              float* feat, float* hpre, float* logits, const int64_t* y, float* loss_ps, float* dlogits, float* loss,
              unsigned* counter, cudaStream_t st);
-// dx = d(loss)/d(encoder output) [T, B, D] (masked-mean backward)
+// dx = d(loss)/d(encoder output) [T, B, D] (masked-mean backward); g_w0 == nullptr skips the weight gradients
 int head_bwd(int B, int T, int D, int N, int ds, int ncls, const int64_t* lengths, const float* statics, const float* w0,
              const float* w2, const float* feat, const float* hpre, const float* dlogits, float* dh, float* dfeat, float* dx,
              float* g_w0, float* g_b0, float* g_w2, float* g_b2, float* g_emb_w, float* g_emb_b, cudaStream_t st);

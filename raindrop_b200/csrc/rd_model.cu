@@ -155,6 +155,18 @@ BwLayout bw_layout(const Shape& s) {
   return b;
 }
 
+// Scratch of rd_raindrop_v2_input_grad: W1^T with its error-compensation remainder, and dX0 = d(loss)/d(X0) [B*N, C]
+struct IgLayout { int64_t W1t, W1tlo, dX0, total; };
+IgLayout input_grad_layout(const Shape& s) {
+  IgLayout l;
+  Arena a;
+  l.W1t = a.take((int64_t)s.C * s.C);
+  l.W1tlo = a.take((int64_t)s.C * s.C);
+  l.dX0 = a.take(s.M1 * s.C);
+  l.total = a.off;
+  return l;
+}
+
 // Y[M,N] = epi(X[M,K] . W[N,K]^T)
 GemmP nt(const float* X, int64_t ldx, const float* W, int64_t ldw, float* Y, int64_t ldy, int64_t M, int N, int K) {
   GemmP g;
@@ -396,6 +408,11 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   const float ik = s.p > 0.f ? 1.f / (1.f - s.p) : 1.f;
   float* gA = sc + b.gA; float* gB = sc + b.gB; float* gD = sc + b.gD; float* dP = sc + b.dP;
   WgradQueue wq;     // weight gradients wait here for ONE grouped tensor-core launch per phase
+  // G == NULL (frozen parameters): only the data-gradient chain runs -- no weight-gradient GEMMs, column sums or
+  // head outer products; the scratch ends up holding the same d(loss)/d(activation) buffers
+  const bool wg = G != nullptr;
+  static const rd_grads kNoGrads = {};
+  if (!wg) G = &kNoGrads;
 
   if (phases & RD_BWD_ENCODER) {
   // ---- head: logits = mlp2(relu(mlp0(feat))), pooled = masked mean          code/models_rd.py:366-385
@@ -433,15 +450,15 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     }
     RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, GE.norm2_weight, GE.norm2_bias,
                          sc + b.l[l].ln[0], K2, s.p, rng, SITE_RESID2 + l, &chunks, st, m2, mld));
-    RD_TRY(wq.colsum(sc + b.l[l].ln[0], 2 * s.D, chunks, s.D, GE.norm2_weight, st));
-    RD_TRY(wq.colsum(sc + b.l[l].ln[0] + s.D, 2 * s.D, chunks, s.D, GE.norm2_bias, st));
-    RD_TRY(tn(&wq, K2, s.D, f, s.nhid, GE.linear2_weight, GE.linear2_bias, s.D, s.nhid, s.M2, sc + b.l[l].wp[0], partial, st));
+    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0], 2 * s.D, chunks, s.D, GE.norm2_weight, st));
+    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0] + s.D, 2 * s.D, chunks, s.D, GE.norm2_bias, st));
+    if (wg) RD_TRY(tn(&wq, K2, s.D, f, s.nhid, GE.linear2_weight, GE.linear2_bias, s.D, s.nhid, s.M2, sc + b.l[l].wp[0], partial, st));
     {   // gF = (K2 . W2) * [f > 0] / (1-p)   ("NT" against W2^T so that the tensor-core kernel applies)
       GemmP g = nt(K2, s.D, ws + w.wsp[l].l2_t, s.D, gF, s.nhid, s.M2, s.nhid, s.D);
       g.gate = f; g.gate_ld = s.nhid; g.gate_scale = ik;  // relu' and the FFN dropout mask in one
       RD_TRY(linear_nt(g, ws + w.wsp[l].l2_tlo, st));
     }
-    RD_TRY(tn(&wq, gF, s.nhid, x1, s.D, GE.linear1_weight, GE.linear1_bias, s.nhid, s.D, s.M2, sc + b.l[l].wp[1], partial, st));
+    if (wg) RD_TRY(tn(&wq, gF, s.nhid, x1, s.D, GE.linear1_weight, GE.linear1_bias, s.nhid, s.D, s.M2, sc + b.l[l].wp[1], partial, st));
     {
       GemmP g = nt(gF, s.nhid, ws + w.wsp[l].l1_t, s.nhid, gA, s.D, s.M2, s.D, s.nhid);
       g.resid = res; g.resid_ld = s.D;
@@ -451,9 +468,9 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     res = s.p > 0.f ? gB : K1;
     RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, GE.norm1_weight, GE.norm1_bias,
                          sc + b.l[l].ln[1], K1, s.p, rng, SITE_RESID1 + l, &chunks, st, m1, mld));
-    RD_TRY(wq.colsum(sc + b.l[l].ln[1], 2 * s.D, chunks, s.D, GE.norm1_weight, st));
-    RD_TRY(wq.colsum(sc + b.l[l].ln[1] + s.D, 2 * s.D, chunks, s.D, GE.norm1_bias, st));
-    RD_TRY(tn(&wq, K1, s.D, ctx, s.D, GE.out_proj_weight, GE.out_proj_bias, s.D, s.D, s.M2, sc + b.l[l].wp[2], partial, st));
+    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1], 2 * s.D, chunks, s.D, GE.norm1_weight, st));
+    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1] + s.D, 2 * s.D, chunks, s.D, GE.norm1_bias, st));
+    if (wg) RD_TRY(tn(&wq, K1, s.D, ctx, s.D, GE.out_proj_weight, GE.out_proj_bias, s.D, s.D, s.M2, sc + b.l[l].wp[2], partial, st));
     RD_TRY(linear_nt(nt(K1, s.D, ws + w.wsp[l].out_t, s.D, gD, s.D, s.M2, s.D, s.D), ws + w.wsp[l].out_tlo, st));
     if (attn_tc_supported(s.T, s.hd)) {
       RD_TRY(attn_tc_bwd(qkv, gD, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, dqkv, st));
@@ -494,7 +511,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
         RD_TRY(gemm(g, st));
       }
     }
-    RD_TRY(tn(&wq, dqkv, 3 * s.D, x, s.D, GE.in_proj_weight, GE.in_proj_bias, 3 * s.D, s.D, s.M2, sc + b.l[l].wp[3], partial, st));
+    if (wg) RD_TRY(tn(&wq, dqkv, 3 * s.D, x, s.D, GE.in_proj_weight, GE.in_proj_bias, 3 * s.D, s.D, s.M2, sc + b.l[l].wp[3], partial, st));
     {
       // the first layer's input gradient is d(loss)/d(encoder input): optionally delivered straight to the caller
       GemmP g = nt(dqkv, 3 * s.D, ws + w.wsp[l].in_t, 3 * s.D, (l == 0 && d_z0_out) ? d_z0_out : gA, s.D, s.M2, s.D, 3 * s.D);
@@ -511,7 +528,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   const float* X0 = ws + w.X0; const float* H1 = ws + w.H1;
   const int tc = s.tc;
   RD_TRY(obprop_out_grad(gA, ws + w.Z[0], nscale, s.B, s.T, s.N, s.dob, s.D, tc && !s.exact, gO2, st));
-  RD_TRY(tn(&wq, gO2, s.C, H1, s.C, G->ob2_value_weight, G->ob2_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[0], partial, st));
+  if (wg) RD_TRY(tn(&wq, gO2, s.C, H1, s.C, G->ob2_value_weight, G->ob2_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[0], partial, st));
   if (tc) {
     // dZ1 = (dZ2 . W2) * s * [H1 > 0] on the tensor cores: "NT" form against a transposed, TF32-rounded W2
     const float* W2t = ws + w.W2t;      // written by the forward's weight-prep launch
@@ -525,7 +542,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     g.rowscale = nscale; g.rowscale_mod = s.N; g.gate = H1; g.gate_ld = s.C;
     RD_TRY(gemm(g, st));
   }
-  RD_TRY(tn(&wq, gO1, s.C, X0, s.C, G->ob1_value_weight, G->ob1_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[1], partial, st));
+  if (wg) RD_TRY(tn(&wq, gO1, s.C, X0, s.C, G->ob1_value_weight, G->ob1_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[1], partial, st));
   RD_TRY(wq.flush(st));
   }
   return 0;
@@ -718,12 +735,68 @@ int rd_raindrop_v2_fwd(const rd_dims* dims, const rd_params* params, const float
 int rd_raindrop_v2_bwd(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
                        const float* node_scale, const void* workspace, const float* d_logits, const rd_grads* grads,
                        void* scratch, int32_t phases, void* stream) {
-  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !grads || !scratch) {
+  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch) {
     set_error("rd_raindrop_v2_bwd: NULL argument");
     return -2;
   }
   return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, grads,
                       (float*)scratch, phases, nullptr, (cudaStream_t)stream);
+}
+
+size_t rd_input_grad_scratch_bytes(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return (size_t)input_grad_layout(s).total * sizeof(float);
+}
+
+int rd_raindrop_v2_input_grad(const rd_dims* dims, const rd_params* params, const float* src, const float* times,
+                              const int64_t* lengths, const void* workspace, const void* bwd_scratch, void* scratch,
+                              float* d_src, float* d_times, float* d_statics, void* stream) {
+  if (!dims || !params || !workspace || !bwd_scratch) { set_error("rd_raindrop_v2_input_grad: NULL argument"); return -2; }
+  if (d_src && (!src || !scratch || !params->R_u || !params->ob1_value_weight)) {
+    set_error("rd_raindrop_v2_input_grad: d_src needs src, scratch, R_u and ob1_value_weight");
+    return -2;
+  }
+  if (d_times && !times) { set_error("rd_raindrop_v2_input_grad: d_times needs times"); return -2; }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if ((d_src || d_times) && (s.dpe != RD_D_PE || s.emb != s.N)) {
+    set_error("rd_raindrop_v2_input_grad: d_src / d_times need the Raindrop_v2 workspace (d_pe = 16, emb_dim = d_inp)");
+    return -2;
+  }
+  if (d_statics && (s.ds == 0 || !params->emb_weight)) { set_error("rd_raindrop_v2_input_grad: no static branch"); return -2; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const WsLayout w = ws_layout(s);
+  const BwLayout b = bw_layout(s);
+  const float* ws = (const float*)workspace;
+  const float* sc = (const float*)bwd_scratch;
+  float* dX0 = nullptr;
+  if (d_src) {
+    // dX0 = gO1 . W1, "NT" against W1^T, always error-compensated: gO1 is not TF32-rounded in either mode
+    const IgLayout il = input_grad_layout(s);
+    float* W1t = (float*)scratch + il.W1t; float* W1tlo = (float*)scratch + il.W1tlo;
+    dX0 = (float*)scratch + il.dX0;
+    if (s.tc) {
+      const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
+      RD_TRY(split_weights(&it, 1, st));
+      ObpropTcArgs a;
+      a.x = sc + b.gO1; a.W = W1t; a.W_lo = W1tlo; a.bias = nullptr; a.relu = 0; a.rows = s.M1; a.C = s.C; a.out = dX0;
+      RD_TRY(obprop_tc_fwd(a, st));
+    } else {
+      RD_TRY(gemm(nn(sc + b.gO1, s.C, params->ob1_value_weight, s.C, dX0, s.C, s.M1, s.C, s.C), st));
+    }
+  }
+  return input_grad(src, params->R_u, dX0, s.B, s.T, s.N, s.dob, s.p, reinterpret_cast<const uint64_t*>(ws + w.rng), d_src,
+                    times, sc + b.gA, s.M2, s.D, s.Dm, dims->pe_timescales, s.dpe, lengths, d_times, sc + b.dfeat, s.Df, s.D,
+                    params->emb_weight, s.emb, s.ds, d_statics, st);
+}
+
+int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,
+                               int32_t d_pe_width, int64_t ld, int32_t col0, float* d_times, void* stream) {
+  if (!times || !d_pe || !timescales_host || !d_times || n_tokens < 0) { set_error("rd_positional_encoding_bwd: bad arguments"); return -2; }
+  if (n_tokens == 0) return 0;
+  return input_grad(nullptr, nullptr, nullptr, 1, 0, 0, 0, 0.f, nullptr, nullptr, times, d_pe, n_tokens, ld, col0, timescales_host,
+                    d_pe_width, nullptr, d_times, nullptr, 0, 0, nullptr, 0, 0, nullptr, (cudaStream_t)stream);
 }
 
 int rd_positional_encoding(const float* times, int64_t n_tokens, const float* timescales_host, int32_t d_pe, float* out,
@@ -744,7 +817,7 @@ int rd_encoder_head_fwd(const rd_dims* dims, const rd_params* params, const floa
 int rd_encoder_head_bwd(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
                         const void* workspace, const float* d_logits, const rd_grads* grads, void* scratch, float* d_enc_in,
                         void* stream) {
-  if (!dims || !params || !lengths || !workspace || !d_logits || !grads || !scratch || !d_enc_in) {
+  if (!dims || !params || !lengths || !workspace || !d_logits || !scratch || !d_enc_in) {
     set_error("rd_encoder_head_bwd: NULL argument");
     return -2;
   }

@@ -152,6 +152,7 @@ class RaindropV2Function(torch.autograd.Function):
         L.check(rc, "rd_raindrop_v2_fwd")
         ctx.plan, ctx.dims, ctx.P, ctx.ws, ctx.pool = plan, dims, P, ws, pool
         ctx.keep = (keep, static, lengths, plan.node_scale, plan.R_u)
+        ctx.inputs = (src, times) if any(ctx.needs_input_grad[2:5]) else None    # the lift / PE backward read them
         ctx.sc_bytes = sc_bytes
         if plan.debug_keep_workspace:      # parity tests read named activation buffers (workspace_view)
             plan.last_workspace = ws
@@ -172,6 +173,15 @@ class RaindropV2Function(torch.autograd.Function):
         d_logits = _as_f32(d_logits)
         dev = d_logits.device
         params = keep
+        if not any(ctx.needs_input_grad[6:]):
+            # frozen parameters (attribution): the data-gradient chain alone, no weight-gradient GEMMs
+            scratch = _bwd_scratch(plan, ctx.sc_bytes, dev)
+            L.check(lib.rd_raindrop_v2_bwd(C.byref(dims), C.byref(ctx.P), L.ptr(static), lengths.data_ptr(),
+                                           node_scale.data_ptr(), ctx.ws.data_ptr(), d_logits.data_ptr(), None,
+                                           scratch.data_ptr(), L.BWD_ALL, L.stream_ptr(dev)), "rd_raindrop_v2_bwd")
+            d_in = _input_grads(ctx, scratch) if ctx.inputs is not None else (None, None, None)
+            _release_workspace(ctx)
+            return (None, None) + d_in + (None,) + (None,) * len(params)
         layout = plan.__dict__.get("_grad_layout")
         if layout is None:      # tightly packed flat bucket, one offset per used parameter
             offs, total = [], 0
@@ -191,11 +201,7 @@ class RaindropV2Function(torch.autograd.Function):
             for (key, path), off in zip(plan.fields, offs):
                 _set_field(G, path, base + 4 * off)
             plan.__dict__["_grad_struct"] = (base, G)
-        scs = plan.__dict__.setdefault("_scratch", {})
-        skey = (ctx.sc_bytes, dev.index)
-        scratch = scs.get(skey)
-        if scratch is None:                  # backward scratch holds nothing across calls: one buffer per size
-            scratch = scs[skey] = torch.empty(ctx.sc_bytes // 4, dtype=torch.float32, device=dev)
+        scratch = _bwd_scratch(plan, ctx.sc_bytes, dev)
         rc = lib.rd_raindrop_v2_bwd(C.byref(dims), C.byref(ctx.P), L.ptr(static), lengths.data_ptr(),
                                     node_scale.data_ptr(), ctx.ws.data_ptr(), d_logits.data_ptr(), C.byref(G),
                                     scratch.data_ptr(), L.BWD_ALL, L.stream_ptr(dev))
@@ -203,10 +209,49 @@ class RaindropV2Function(torch.autograd.Function):
         grads = torch._utils._unflatten_dense_tensors(flat, params)      # views, one C++ call
         if owner is not None:
             owner._flat_grad = flat          # the DDP bucket: one all-reduce covers every gradient
-        if not plan.debug_keep_workspace:
-            ctx.pool.append(ctx.ws)
-        ctx.ws = None
-        return (None, None, None, None, None, None) + tuple(grads)
+        d_in = _input_grads(ctx, scratch) if ctx.inputs is not None else (None, None, None)
+        _release_workspace(ctx)
+        return (None, None) + d_in + (None,) + tuple(grads)
+
+
+def _bwd_scratch(plan, sc_bytes, dev):
+    scs = plan.__dict__.setdefault("_scratch", {})
+    skey = (sc_bytes, dev.index)
+    scratch = scs.get(skey)
+    if scratch is None:                  # backward scratch holds nothing across calls: one buffer per size
+        scratch = scs[skey] = torch.empty(sc_bytes // 4, dtype=torch.float32, device=dev)
+    return scratch
+
+
+def _release_workspace(ctx):
+    if not ctx.plan.debug_keep_workspace:
+        ctx.pool.append(ctx.ws)
+    ctx.ws = None
+
+
+def _input_grads(ctx, scratch):
+    """(d_src, d_static, d_times) for the inputs that need one (rd_raindrop_v2_input_grad, right after the backward
+    that left its activation gradients in `scratch`)."""
+    lib = L.load()
+    plan, dims = ctx.plan, ctx.dims
+    src, times = ctx.inputs
+    static, lengths = ctx.keep[1], ctx.keep[2]
+    need_src, need_static, need_times = ctx.needs_input_grad[2:5]
+    dev = src.device
+    d_src = torch.empty_like(src) if need_src else None
+    d_times = torch.empty_like(times) if need_times else None
+    d_static = torch.empty_like(static) if (need_static and static is not None) else None
+    ig = None
+    if need_src:
+        igs = plan.__dict__.setdefault("_ig_scratch", {})
+        key = (src.shape[1], dims.obprop_mode, dev.index)
+        ig = igs.get(key)
+        if ig is None:
+            ig = igs[key] = torch.empty(lib.rd_input_grad_scratch_bytes(C.byref(dims)) // 4, dtype=torch.float32, device=dev)
+    L.check(lib.rd_raindrop_v2_input_grad(C.byref(dims), C.byref(ctx.P), src.data_ptr(), times.data_ptr(), lengths.data_ptr(),
+                                          ctx.ws.data_ptr(), scratch.data_ptr(), L.ptr(ig), L.ptr(d_src), L.ptr(d_times),
+                                          L.ptr(d_static), L.stream_ptr(dev)), "rd_raindrop_v2_input_grad")
+    return d_src, d_static, d_times
 
 
 class _StepSlot:
@@ -320,6 +365,12 @@ def flat_forward(plan, training, flat, src, static, times, lengths):
     B = src.shape[1]
     if src.shape[0] != plan.T or src.shape[2] != 2 * plan.N:
         raise ValueError("src must be [max_len=%d, B, 2*d_inp=%d], got %s" % (plan.T, 2 * plan.N, tuple(src.shape)))
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (src, static, times)):
+        # input gradients come through the general path; its parameter gradients accumulate into the .grad windows of
+        # the bucket, so the bucket starts from zero (a backward overwrites the gradients, as on the fast path)
+        flat.flat_g.zero_()
+        flat.grads_ready = False
+        return None
     slots = plan.__dict__.setdefault("_slots", {})
     k = (B, bool(training), dev.index)
     slot = slots.get(k)
@@ -443,15 +494,35 @@ def node_scale(edge_index, edge_weights, n_nodes):
     return s
 
 
+class PositionalEncodingFunction(torch.autograd.Function):
+    """pe = [sin(times / ts), cos(times / ts)] (rd_positional_encoding), differentiable in times
+    (rd_positional_encoding_bwd)."""
+
+    @staticmethod
+    def forward(ctx, t, max_len, d_pe):
+        lib = L.load()
+        out = torch.empty(t.shape + (d_pe,), dtype=torch.float32, device=t.device)
+        ts = (C.c_float * (d_pe // 2))(*[float(v) for v in pe_timescales(max_len, d_pe)])
+        L.check(lib.rd_positional_encoding(t.data_ptr(), t.numel(), ts, d_pe, out.data_ptr(), d_pe, 0, L.stream_ptr(t.device)),
+                "rd_positional_encoding")
+        ctx.save_for_backward(t)
+        ctx.ts, ctx.d_pe = ts, d_pe
+        return out
+
+    @staticmethod
+    def backward(ctx, d_pe):
+        lib = L.load()
+        (t,) = ctx.saved_tensors
+        d_pe = _as_f32(d_pe)
+        d_t = torch.empty_like(t)
+        L.check(lib.rd_positional_encoding_bwd(t.data_ptr(), d_pe.data_ptr(), t.numel(), ctx.ts, ctx.d_pe, ctx.d_pe, 0,
+                                               d_t.data_ptr(), L.stream_ptr(t.device)), "rd_positional_encoding_bwd")
+        return d_t, None, None
+
+
 def positional_encoding(times, max_len, d_pe=16):
-    """[T, B] -> [T, B, d_pe] on the device (rd_positional_encoding); d_pe even, <= 64."""
-    lib = L.load()
-    t = _as_f32(times)
-    out = torch.empty(t.shape + (d_pe,), dtype=torch.float32, device=t.device)
-    ts = (C.c_float * (d_pe // 2))(*[float(v) for v in pe_timescales(max_len, d_pe)])
-    L.check(lib.rd_positional_encoding(t.data_ptr(), t.numel(), ts, d_pe, out.data_ptr(), d_pe, 0, L.stream_ptr(t.device)),
-            "rd_positional_encoding")
-    return out
+    """[T, B] -> [T, B, d_pe] on the device (rd_positional_encoding); d_pe even, <= 64.  Differentiable in times."""
+    return PositionalEncodingFunction.apply(_as_f32(times), max_len, d_pe)
 
 
 def linear(x, weight, bias=None, relu=False):
@@ -625,6 +696,7 @@ class EncoderHeadFunction(torch.autograd.Function):
         for t in keep:
             offs.append(total)
             total += t.numel()
+        need_params = any(ctx.needs_input_grad[5:])
         flat = torch.empty(total, dtype=torch.float32, device=dev)
         G = L.RdGrads()
         for (key, path), off in zip(plan.fields, offs):
@@ -632,11 +704,18 @@ class EncoderHeadFunction(torch.autograd.Function):
         sc = torch.empty(lib.rd_backward_scratch_bytes(C.byref(dims)) // 4, dtype=torch.float32, device=dev)
         dz = torch.empty(ctx.shape, dtype=torch.float32, device=dev)
         rc = lib.rd_encoder_head_bwd(C.byref(dims), C.byref(ctx.P), L.ptr(static), lengths.data_ptr(), ctx.ws.data_ptr(),
-                                     d_logits.data_ptr(), C.byref(G), sc.data_ptr(), dz.data_ptr(), L.stream_ptr(dev))
+                                     d_logits.data_ptr(), C.byref(G) if need_params else None, sc.data_ptr(), dz.data_ptr(),
+                                     L.stream_ptr(dev))
         L.check(rc, "rd_encoder_head_bwd")
-        grads = torch._utils._unflatten_dense_tensors(flat, keep)
+        d_static = None
+        if ctx.needs_input_grad[3] and static is not None:
+            d_static = torch.empty_like(static)
+            L.check(lib.rd_raindrop_v2_input_grad(C.byref(dims), C.byref(ctx.P), None, None, None, ctx.ws.data_ptr(),
+                                                  sc.data_ptr(), None, None, None, d_static.data_ptr(), L.stream_ptr(dev)),
+                    "rd_raindrop_v2_input_grad")
+        grads = torch._utils._unflatten_dense_tensors(flat, keep) if need_params else (None,) * len(keep)
         ctx.ws = None
-        return (None, None, dz, None, None) + tuple(grads)
+        return (None, None, dz, d_static, None) + tuple(grads)
 
 
 def workspace_view(plan, which):

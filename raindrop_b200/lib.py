@@ -93,6 +93,10 @@ SIGNATURES = {
                                      C.c_int32, C.c_void_p]),
     "rd_positional_encoding": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_float), C.c_int32, C.c_void_p,
                                          C.c_int64, C.c_int32, C.c_void_p]),
+    "rd_positional_encoding_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_float), C.c_int32,
+                                             C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
+    "rd_input_grad_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
+    "rd_raindrop_v2_input_grad": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 10),
     "rd_encoder_head_fwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
     "rd_encoder_head_bwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(RdGrads), C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -248,6 +248,33 @@ int rd_raindrop_v2_input_grad(const rd_dims* dims, const rd_params* params, cons
                               const int64_t* lengths, const void* workspace, const void* bwd_scratch, void* scratch,
                               float* d_src, float* d_times, float* d_statics, void* stream);
 
+/* ---- integrated gradients (IG) attribution of Raindrop_v2, in one call ------------------------------------------
+ * For F = logits[b, target[b]] and the straight path x' + alpha (x - x') from the baseline x' to the input x:
+ *   attr_src[t,b,n]     = (x - x')[t,b,n] . sum_k weights[k] dF/dsrc[t,b,n] at alpha = alphas[k]     (value half)
+ *   attr_statics[b,j]   = (s - s')[b,j]   . sum_k weights[k] dF/dstatic[b,j] at alphas[k]
+ * alphas / weights [n_steps] are the quadrature nodes and weights on [0, 1] (device fp32; any rule).  Only the value
+ * half of src and the statics are interpolated: the mask half is taken from src, times and lengths are held fixed
+ * (attribution over times is not provided; use rd_raindrop_v2_input_grad).  Eval arithmetic: dims->training must be 0,
+ * no dropout, the rng state is neither read nor advanced and no parameter gradient is written.
+ *   baseline_src     [T, B, 2N] (only the value half is read);  baseline_statics [B, d_static] or NULL when d_static == 0
+ *   target           [B] int64 class per sample, or NULL = argmax of the logits at x (read on the device)
+ *   attr_src         [T, B, 2N], the mask half written as 0;  attr_statics [B, d_static] or NULL (skipped)
+ *   endpoint_logits  [2, B, n_classes]: logits at the baseline ([0]) and at the input ([1]), for the completeness check
+ *                    sum(attr) ~ F(x) - F(x')
+ * Work: one forward on 2B rows for the endpoints, then chunks of `steps_per_chunk` steps on B*steps_per_chunk rows
+ * (step-major) -- inputs expanded in one launch, forward, frozen-parameter backward, dX0 GEMM, and one accumulation
+ * launch that adds the chunk's weighted lift / static-embedding backward to running sums in fp32, in a fixed order
+ * (deterministic, no atomics).  dims->obprop_mode 0 is resolved once from B*steps_per_chunk rows, so the endpoint
+ * forward and every chunk, including a shorter last one, use the same arithmetic.
+ * scratch: rd_integrated_gradients_scratch_bytes(dims, steps_per_chunk) bytes (dims->B = samples, training = 0). */
+size_t rd_integrated_gradients_scratch_bytes(const rd_dims* dims, int32_t steps_per_chunk);
+int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                        const float* times, const int64_t* lengths, const float* node_scale,
+                                        const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                        const float* alphas, const float* weights, int32_t n_steps, int32_t steps_per_chunk,
+                                        void* scratch, float* attr_src, float* attr_statics, float* endpoint_logits,
+                                        void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);

@@ -272,6 +272,37 @@ struct InputGradArgs {
   const float* times; const float* g_pe; long long n_tokens, ld; int col0; const int64_t* lengths; float* d_times;
   const float* dfeat; const float* W_emb; int Df, feat_col0, emb, ds; float* d_static; long long n_static;
 };
+// The lift backward of one (sample, t, sensor n) with value sv: sum_k g[k] * keep_k/(1-p) * [sv*R_u[n*d_ob+k] > 0] *
+// R_u[n*d_ob+k], g = d(loss)/d(X0) of that (row, t); idx0 = the forward's dropout element index of channel 0
+__device__ __forceinline__ float lift_bwd(float sv, const float* __restrict__ R_u, const float* __restrict__ g, int n,
+                                          int d_ob, float drop_p, const uint64_t* __restrict__ rng, uint64_t idx0) {
+  const float ik = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  float acc = 0.f;
+  if (d_ob == 4) {
+    const float4 r = __ldg(reinterpret_cast<const float4*>(R_u) + n);
+    float4 d = __ldg(reinterpret_cast<const float4*>(g));
+    if (drop_p > 0.f) {
+      const float4 m = dropout_scale4(rng, SITE_LIFT, idx0, drop_p, ik);
+      d.x *= m.x; d.y *= m.y; d.z *= m.z; d.w *= m.w;
+    }
+    acc = (sv * r.x > 0.f ? d.x * r.x : 0.f) + (sv * r.y > 0.f ? d.y * r.y : 0.f) +
+          (sv * r.z > 0.f ? d.z * r.z : 0.f) + (sv * r.w > 0.f ? d.w * r.w : 0.f);
+  } else {
+    for (int k = 0; k < d_ob; ++k) {
+      const float r = __ldg(R_u + n * d_ob + k);
+      float d = __ldg(g + k);
+      if (drop_p > 0.f) d *= dropout_scale(rng, SITE_LIFT, idx0 + k, drop_p, ik);
+      acc += sv * r > 0.f ? d * r : 0.f;
+    }
+  }
+  return acc;
+}
+// d(loss)/d(static[b, k]) = sum_n df[n] * W_emb[n*ds + k], df = d(loss)/d(emb output) of sample b
+__device__ __forceinline__ float emb_bwd(const float* __restrict__ df, const float* __restrict__ W_emb, int emb, int ds, int k) {
+  float acc = 0.f;
+  for (int n = 0; n < emb; ++n) acc = fmaf(__ldg(df + n), __ldg(W_emb + (long long)n * ds + k), acc);
+  return acc;
+}
 __global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const __grid_constant__ TS8 ts) {
   pdl_launch_dependents();
   pdl_wait();
@@ -282,28 +313,9 @@ __global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const
     const int b = (int)(row / a.N), n = (int)(row - (long long)b * a.N);
     float* ds = a.d_src + ((long long)t * a.B + b) * (2 * a.N);
     const float sv = __ldg(a.src + ((long long)t * a.B + b) * (2 * a.N) + n);
-    const float ik = a.drop_p > 0.f ? 1.f / (1.f - a.drop_p) : 1.f;
     const uint64_t idx0 = ((uint64_t)t * a.B + b) * (uint64_t)(a.N * a.d_ob) + (uint64_t)(n * a.d_ob);
     const float* g = a.dX0 + row * ((long long)a.T * a.d_ob) + (long long)t * a.d_ob;
-    float acc = 0.f;
-    if (a.d_ob == 4) {
-      const float4 r = __ldg(reinterpret_cast<const float4*>(a.R_u) + n);
-      float4 d = __ldg(reinterpret_cast<const float4*>(g));
-      if (a.drop_p > 0.f) {
-        const float4 m = dropout_scale4(a.rng, SITE_LIFT, idx0, a.drop_p, ik);
-        d.x *= m.x; d.y *= m.y; d.z *= m.z; d.w *= m.w;
-      }
-      acc = (sv * r.x > 0.f ? d.x * r.x : 0.f) + (sv * r.y > 0.f ? d.y * r.y : 0.f) +
-            (sv * r.z > 0.f ? d.z * r.z : 0.f) + (sv * r.w > 0.f ? d.w * r.w : 0.f);
-    } else {
-      for (int k = 0; k < a.d_ob; ++k) {
-        const float r = __ldg(a.R_u + n * a.d_ob + k);
-        float d = __ldg(g + k);
-        if (a.drop_p > 0.f) d *= dropout_scale(a.rng, SITE_LIFT, idx0 + k, a.drop_p, ik);
-        acc += sv * r > 0.f ? d * r : 0.f;
-      }
-    }
-    ds[n] = acc;
+    ds[n] = lift_bwd(sv, a.R_u, g, n, a.d_ob, a.drop_p, a.rng, idx0);
     ds[a.N + n] = 0.f;
     return;
   }
@@ -328,10 +340,125 @@ __global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const
   if (o >= a.n_static) return;
   const long long b = o / a.ds;
   const int k = (int)(o - b * a.ds);
-  const float* df = a.dfeat + b * a.Df + a.feat_col0;
-  float acc = 0.f;
-  for (int n = 0; n < a.emb; ++n) acc = fmaf(__ldg(df + n), __ldg(a.W_emb + (long long)n * a.ds + k), acc);
-  a.d_static[o] = acc;
+  a.d_static[o] = emb_bwd(a.dfeat + b * a.Df + a.feat_col0, a.W_emb, a.emb, a.ds, k);
+}
+
+// ---- integrated gradients (rd_raindrop_v2_integrated_gradients) ------------------------------------------------
+// Point alpha of the straight path from the baseline x0 to x.  Exact at both ends: alpha = 0 gives x0, alpha = 1 gives x.
+__device__ __forceinline__ float ig_interp(float x, float x0, float a) { return fmaf(a, x, (1.f - a) * x0); }
+
+// Inputs of one chunk of m path steps on B*m rows, step-major (row j = k*B + b), in one launch with four thread ranges:
+//   src_e[t, j, n] = interp(src[t, b, n], src0[t, b, n], alpha_k) (value half), src[t, b, n] (mask half, copied)
+//   times_e[t, j] = times[t, b]
+//   statics_e[j, :] = interp(statics[b, :], statics0[b, :], alpha_k)
+//   lengths_e[j] = lengths[b]; d_logits[j, :] = one-hot(target[b]) (target == NULL: argmax of logits_x[b, :])
+// alphas == NULL gives the two endpoints (m = 2: alpha_0 = 0, alpha_1 = 1).
+struct IgExpandArgs {
+  const float* src; const float* src0; const float* statics; const float* statics0; const float* times;
+  const int64_t* lengths; const float* alphas; const int64_t* target; const float* logits_x;
+  float* src_e; float* statics_e; float* times_e; int64_t* lengths_e; float* d_logits;
+  int m, B, T, N, ds, ncls;
+  long long n_src, n_tok, n_stat, n_rows;
+};
+__global__ void ig_expand_kernel(const __grid_constant__ IgExpandArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long rows = (long long)a.B * a.m;
+  if (o < a.n_src) {
+    const int w = 2 * a.N;
+    const long long tj = o / w;
+    const int c = (int)(o - tj * w);
+    const long long t = tj / rows;
+    const int j = (int)(tj - t * rows), k = j / a.B, b = j - k * a.B;
+    const long long i = (t * a.B + b) * w + c;
+    const float alpha = a.alphas ? __ldg(a.alphas + k) : (float)k;
+    a.src_e[o] = c < a.N ? ig_interp(__ldg(a.src + i), __ldg(a.src0 + i), alpha) : __ldg(a.src + i);
+    return;
+  }
+  o -= a.n_src;
+  if (o < a.n_tok) {
+    const long long t = o / rows;
+    const int b = (int)((o - t * rows) % a.B);
+    a.times_e[o] = __ldg(a.times + t * a.B + b);
+    return;
+  }
+  o -= a.n_tok;
+  if (o < a.n_stat) {
+    const long long j = o / a.ds;
+    const int kk = (int)(o - j * a.ds), k = (int)(j / a.B), b = (int)(j - (long long)k * a.B);
+    const float alpha = a.alphas ? __ldg(a.alphas + k) : (float)k;
+    const long long i = (long long)b * a.ds + kk;
+    a.statics_e[o] = ig_interp(__ldg(a.statics + i), __ldg(a.statics0 + i), alpha);
+    return;
+  }
+  o -= a.n_stat;
+  if (o >= a.n_rows) return;
+  const int b = (int)(o % a.B);
+  a.lengths_e[o] = __ldg(a.lengths + b);
+  if (!a.d_logits) return;
+  int tgt = 0;
+  if (a.target) {
+    tgt = (int)__ldg(a.target + b);
+  } else {       // first maximum, as torch.argmax
+    const float* l = a.logits_x + (long long)b * a.ncls;
+    float best = __ldg(l);
+    for (int c = 1; c < a.ncls; ++c) {
+      const float v = __ldg(l + c);
+      if (v > best) { best = v; tgt = c; }
+    }
+  }
+  float* d = a.d_logits + o * a.ncls;
+  for (int c = 0; c < a.ncls; ++c) d[c] = c == tgt ? 1.f : 0.f;
+}
+
+// Integrated-gradients accumulation over one chunk's m steps (after its backward and dX0 GEMM), two thread ranges:
+//   o <  n_lift : one thread per (row = b*N + n, t): acc += w_k * lift_bwd(interp(x, x0, alpha_k), dX0 row (k*B+b)*N + n)
+//                 for k = 0..m-1 in order, fp32; the gate value is recomputed, not read back.  acc_src carries the running
+//                 sum from chunk to chunk; the last chunk writes attr_src[t,b,n] = (x - x0) * acc and 0 on the mask half
+//   rest        : one thread per (b, j) of the statics: the same through d(F)/d(emb output) . W_emb
+// Fixed summation order, no atomics: deterministic.
+struct IgAccumArgs {
+  const float* src; const float* src0; const float* alphas; const float* weights; const float* R_u; const float* dX0;
+  float* acc_src; float* attr_src; long long n_lift; int m, B, T, N, d_ob;
+  const float* statics; const float* statics0; const float* dfeat; const float* W_emb; int Df, feat_col0, emb, ds;
+  float* acc_static; float* attr_static; long long n_static;
+  int first, last;
+};
+__global__ void ig_accum_kernel(const __grid_constant__ IgAccumArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o < a.n_lift) {
+    const long long row = o / a.T;
+    const int t = (int)(o - row * a.T);
+    const int b = (int)(row / a.N), n = (int)(row - (long long)b * a.N);
+    const long long i = ((long long)t * a.B + b) * (2 * a.N) + n;
+    const float xv = __ldg(a.src + i), x0 = __ldg(a.src0 + i);
+    const long long C = (long long)a.T * a.d_ob;
+    float acc = a.first ? 0.f : a.acc_src[o];
+    for (int k = 0; k < a.m; ++k) {
+      const float sv = ig_interp(xv, x0, __ldg(a.alphas + k));
+      const float* g = a.dX0 + ((long long)(k * a.B + b) * a.N + n) * C + (long long)t * a.d_ob;
+      acc = fmaf(__ldg(a.weights + k), lift_bwd(sv, a.R_u, g, n, a.d_ob, 0.f, nullptr, 0), acc);
+    }
+    if (a.last) {
+      a.attr_src[i] = (xv - x0) * acc + 0.f;      // + 0: an input of -0.0 (unobserved, padded) gives +0, not -0
+      a.attr_src[i + a.N] = 0.f;
+    } else {
+      a.acc_src[o] = acc;
+    }
+    return;
+  }
+  o -= a.n_lift;
+  if (o >= a.n_static) return;
+  const long long b = o / a.ds;
+  const int kk = (int)(o - b * a.ds);
+  float acc = a.first ? 0.f : a.acc_static[o];
+  for (int k = 0; k < a.m; ++k)
+    acc = fmaf(__ldg(a.weights + k), emb_bwd(a.dfeat + ((long long)k * a.B + b) * a.Df + a.feat_col0, a.W_emb, a.emb, a.ds, kk), acc);
+  if (a.last) a.attr_static[o] = (__ldg(a.statics + o) - __ldg(a.statics0 + o)) * acc + 0.f;
+  else a.acc_static[o] = acc;
 }
 
 // one warp per node: segment max, then sum of exp, then s = sum(exp / (sum + 1e-16))
@@ -933,6 +1060,38 @@ int input_grad(const float* src, const float* R_u, const float* dX0, int B, int 
   if (total <= 0) return 0;
   launch_pdl(input_grad_kernel, dim3(blocks_for(total)), dim3(TPB), 0, st, a, ts);
   RD_CHECK_LAUNCH("input_grad_kernel");
+  return 0;
+}
+
+int ig_expand(const float* src, const float* src0, const float* statics, const float* statics0, const float* times,
+              const int64_t* lengths, const float* alphas, int m, int B, int T, int N, int ds, int ncls, const int64_t* target,
+              const float* logits_x, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, float* d_logits,
+              cudaStream_t st) {
+  IgExpandArgs a;
+  a.src = src; a.src0 = src0; a.statics = statics; a.statics0 = statics0; a.times = times; a.lengths = lengths;
+  a.alphas = alphas; a.target = target; a.logits_x = logits_x;
+  a.src_e = src_e; a.statics_e = statics_e; a.times_e = times_e; a.lengths_e = lengths_e; a.d_logits = d_logits;
+  a.m = m; a.B = B; a.T = T; a.N = N; a.ds = ds; a.ncls = ncls;
+  const int64_t rows = (int64_t)B * m;
+  a.n_src = (int64_t)T * rows * 2 * N; a.n_tok = (int64_t)T * rows; a.n_stat = ds > 0 ? rows * ds : 0; a.n_rows = rows;
+  launch_pdl(ig_expand_kernel, dim3(blocks_for(a.n_src + a.n_tok + a.n_stat + a.n_rows)), dim3(TPB), 0, st, a);
+  RD_CHECK_LAUNCH("ig_expand_kernel");
+  return 0;
+}
+
+int ig_accumulate(const float* src, const float* src0, const float* alphas, const float* weights, int m, int B, int T, int N,
+                  int d_ob, const float* R_u, const float* dX0, float* acc_src, float* attr_src, const float* statics,
+                  const float* statics0, const float* dfeat, int Df, int feat_col0, const float* W_emb, int emb, int ds,
+                  float* acc_static, float* attr_static, int first, int last, cudaStream_t st) {
+  IgAccumArgs a;
+  a.src = src; a.src0 = src0; a.alphas = alphas; a.weights = weights; a.R_u = R_u; a.dX0 = dX0;
+  a.acc_src = acc_src; a.attr_src = attr_src; a.n_lift = (int64_t)B * N * T; a.m = m; a.B = B; a.T = T; a.N = N; a.d_ob = d_ob;
+  a.statics = statics; a.statics0 = statics0; a.dfeat = dfeat; a.W_emb = W_emb; a.Df = Df; a.feat_col0 = feat_col0;
+  a.emb = emb; a.ds = ds; a.acc_static = acc_static; a.attr_static = attr_static;
+  a.n_static = (attr_static && ds > 0) ? (int64_t)B * ds : 0;
+  a.first = first; a.last = last;
+  launch_pdl(ig_accum_kernel, dim3(blocks_for(a.n_lift + a.n_static)), dim3(TPB), 0, st, a);
+  RD_CHECK_LAUNCH("ig_accum_kernel");
   return 0;
 }
 

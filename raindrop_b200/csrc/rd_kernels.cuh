@@ -45,6 +45,23 @@ int input_grad(const float* src, const float* R_u, const float* dX0, int B, int 
                const float* ts_host, int d_pe, const int64_t* lengths, float* d_times, const float* dfeat, int Df, int feat_col0,
                const float* W_emb, int emb, int ds, float* d_static, cudaStream_t st);
 
+// Integrated gradients along the straight path x0 + alpha (x - x0), chunks of m steps on B*m rows, step-major (j = k*B + b).
+// ig_expand: the chunk's inputs src_e [T, B*m, 2N] (value half interpolated, mask half copied from src), statics_e,
+// times_e, lengths_e and one-hot d_logits [B*m, ncls] of target[b] (target == nullptr: argmax of logits_x [B, ncls];
+// d_logits == nullptr skips it).  alphas == nullptr: the two endpoints alpha = 0, 1 (m = 2).
+int ig_expand(const float* src, const float* src0, const float* statics, const float* statics0, const float* times,
+              const int64_t* lengths, const float* alphas, int m, int B, int T, int N, int ds, int ncls, const int64_t* target,
+              const float* logits_x, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, float* d_logits,
+              cudaStream_t st);
+// ig_accumulate: running sums over the chunk's steps of weights[k] * (lift backward of dX0 [B*m*N, T*d_ob]) per (b, n, t)
+// in acc_src [B*N*T], and of weights[k] * dfeat[:, feat_col0 : +emb] . W_emb per (b, j) in acc_static [B, ds];
+// first: start from 0; last: write attr_src [T, B, 2N] = (src - src0) * sum (mask half 0) and attr_static = (statics -
+// statics0) * sum instead of the running sums.  attr_static == nullptr skips the statics.
+int ig_accumulate(const float* src, const float* src0, const float* alphas, const float* weights, int m, int B, int T, int N,
+                  int d_ob, const float* R_u, const float* dX0, float* acc_src, float* attr_src, const float* statics,
+                  const float* statics0, const float* dfeat, int Df, int feat_col0, const float* W_emb, int emb, int ds,
+                  float* acc_static, float* attr_static, int first, int last, cudaStream_t st);
+
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 
 // y = LN(x) * gamma + beta over the last dim (width D); stats[row] = {mean, rstd}

@@ -167,6 +167,47 @@ IgLayout input_grad_layout(const Shape& s) {
   return l;
 }
 
+// ---- integrated gradients ------------------------------------------------------------------------------------------
+// A chunk of mc path steps runs on B*mc rows.  The arithmetic of its ob-prop GEMMs is resolved once, from the FULL
+// chunk's row count (obprop_mode 0 depends on it), and every chunk and the endpoint forward run with that explicit mode:
+// a ragged tail chunk with fewer rows cannot switch arithmetic.
+rd_dims ig_dims(const rd_dims* d, int rows, int mc) {
+  rd_dims e = *d;
+  e.obprop_mode = obprop_tc_exact((int64_t)d->B * mc * d->N, d->T * d->d_ob, d->obprop_mode) ? 2 : 1;
+  e.B = rows;
+  e.training = 0;
+  return e;
+}
+
+// Scratch of rd_raindrop_v2_integrated_gradients: the forward workspace of max(B*mc, 2B) rows (chunks and the endpoint
+// forward), the chunk's backward scratch, the input-gradient buffers (W1^T, its remainder, dX0), the expanded inputs
+// (max(B*mc, 2B) rows), the chunk's one-hot d_logits and logits, and the running sums [B*N*T] and [B, d_static].
+struct IgcLayout { int64_t ws, sc, W1t, W1tlo, dX0, src, statics, times, lengths, dlogits, logits, acc_src, acc_static, total; };
+int ig_layout(const rd_dims* dims, int mc, IgcLayout* l) {
+  if (mc < 1 || (int64_t)dims->B * mc > (1LL << 30)) { set_error("steps_per_chunk = %d out of range", mc); return -2; }
+  const int Bc = dims->B * mc, Bx = Bc > 2 * dims->B ? Bc : 2 * dims->B;
+  const rd_dims dc = ig_dims(dims, Bc, mc), dx = ig_dims(dims, Bx, mc);
+  Shape sc, sx;
+  RD_TRY(make_shape(&dc, &sc));
+  RD_TRY(make_shape(&dx, &sx));
+  Arena a;
+  l->ws = a.take(ws_layout(sx).total);
+  l->sc = a.take(bw_layout(sc).total);
+  l->W1t = a.take((int64_t)sc.C * sc.C);
+  l->W1tlo = a.take((int64_t)sc.C * sc.C);
+  l->dX0 = a.take(sc.M1 * sc.C);
+  l->src = a.take(sx.M2 * 2 * sx.N);
+  l->statics = a.take((int64_t)Bx * sx.ds);
+  l->times = a.take(sx.M2);
+  l->lengths = a.take(2LL * Bx);
+  l->dlogits = a.take((int64_t)Bc * sc.ncls);
+  l->logits = a.take((int64_t)Bc * sc.ncls);
+  l->acc_src = a.take((int64_t)dims->B * sc.N * sc.T);
+  l->acc_static = a.take((int64_t)dims->B * sc.ds);
+  l->total = a.off;
+  return 0;
+}
+
 // Y[M,N] = epi(X[M,K] . W[N,K]^T)
 GemmP nt(const float* X, int64_t ldx, const float* W, int64_t ldw, float* Y, int64_t ldy, int64_t M, int N, int K) {
   GemmP g;
@@ -262,6 +303,18 @@ static int obprop_forward(const ObpropTcArgs& a, cudaStream_t st) {
   g.gate = a.gate; g.gate_ld = a.C;
   g.perm = a.perm; g.pB = a.pB; g.pN = a.pN; g.pdob = a.pdob; g.pD = a.pD;
   return gemm(g, st);
+}
+
+// dX0 = gO1 . W1 [B*N, C]: on the tensor cores "NT" against W1^T (W1t / W1tlo from split_weights), always
+// error-compensated since gO1 is not TF32-rounded in either mode; on the CUDA cores straight from W1
+static int input_grad_dx0(const Shape& s, const rd_params* P, const float* gO1, const float* W1t, const float* W1tlo,
+                          float* dX0, cudaStream_t st) {
+  if (s.tc) {
+    ObpropTcArgs a;
+    a.x = gO1; a.W = W1t; a.W_lo = W1tlo; a.bias = nullptr; a.relu = 0; a.rows = s.M1; a.C = s.C; a.out = dX0;
+    return obprop_tc_fwd(a, st);
+  }
+  return gemm(nn(gO1, s.C, P->ob1_value_weight, s.C, dX0, s.C, s.M1, s.C, s.C), st);
 }
 
 static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* src, const float* statics,
@@ -772,23 +825,93 @@ int rd_raindrop_v2_input_grad(const rd_dims* dims, const rd_params* params, cons
   const float* sc = (const float*)bwd_scratch;
   float* dX0 = nullptr;
   if (d_src) {
-    // dX0 = gO1 . W1, "NT" against W1^T, always error-compensated: gO1 is not TF32-rounded in either mode
     const IgLayout il = input_grad_layout(s);
     float* W1t = (float*)scratch + il.W1t; float* W1tlo = (float*)scratch + il.W1tlo;
     dX0 = (float*)scratch + il.dX0;
     if (s.tc) {
       const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
       RD_TRY(split_weights(&it, 1, st));
-      ObpropTcArgs a;
-      a.x = sc + b.gO1; a.W = W1t; a.W_lo = W1tlo; a.bias = nullptr; a.relu = 0; a.rows = s.M1; a.C = s.C; a.out = dX0;
-      RD_TRY(obprop_tc_fwd(a, st));
-    } else {
-      RD_TRY(gemm(nn(sc + b.gO1, s.C, params->ob1_value_weight, s.C, dX0, s.C, s.M1, s.C, s.C), st));
     }
+    RD_TRY(input_grad_dx0(s, params, sc + b.gO1, W1t, W1tlo, dX0, st));
   }
   return input_grad(src, params->R_u, dX0, s.B, s.T, s.N, s.dob, s.p, reinterpret_cast<const uint64_t*>(ws + w.rng), d_src,
                     times, sc + b.gA, s.M2, s.D, s.Dm, dims->pe_timescales, s.dpe, lengths, d_times, sc + b.dfeat, s.Df, s.D,
                     params->emb_weight, s.emb, s.ds, d_statics, st);
+}
+
+size_t rd_integrated_gradients_scratch_bytes(const rd_dims* dims, int32_t steps_per_chunk) {
+  if (!dims) return 0;
+  IgcLayout l;
+  if (ig_layout(dims, steps_per_chunk, &l) != 0) return 0;
+  return (size_t)l.total * sizeof(float);
+}
+
+int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                        const float* times, const int64_t* lengths, const float* node_scale,
+                                        const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                        const float* alphas, const float* weights, int32_t n_steps, int32_t steps_per_chunk,
+                                        void* scratch, float* attr_src, float* attr_statics, float* endpoint_logits,
+                                        void* stream) {
+  if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !alphas || !weights || !scratch ||
+      !attr_src || !endpoint_logits || !params->R_u || !params->ob1_value_weight) {
+    set_error("rd_raindrop_v2_integrated_gradients: NULL argument");
+    return -2;
+  }
+  if (n_steps < 1 || steps_per_chunk < 1) { set_error("rd_raindrop_v2_integrated_gradients: n_steps and steps_per_chunk must be >= 1"); return -2; }
+  if (dims->training) { set_error("rd_raindrop_v2_integrated_gradients: runs eval arithmetic, dims->training must be 0"); return -2; }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s0.ds > 0 && (!statics || !baseline_statics)) {
+    set_error("rd_raindrop_v2_integrated_gradients: d_static > 0 needs statics and baseline_statics");
+    return -2;
+  }
+  IgcLayout l;
+  RD_TRY(ig_layout(dims, steps_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, mc = steps_per_chunk;
+  float* S = (float*)scratch;
+  float* ws = S + l.ws; float* sc = S + l.sc; float* dX0 = S + l.dX0;
+  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
+  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  float* dlog = S + l.dlogits;
+  float* W1t = S + l.W1t; float* W1tlo = S + l.W1tlo;
+  float* attr_st = s0.ds > 0 ? attr_statics : nullptr;
+
+  // 1. the endpoints: one forward on 2B rows (baseline rows, then input rows) -> endpoint_logits [2, B, ncls]
+  const rd_dims de = ig_dims(dims, 2 * B, mc);
+  RD_TRY(ig_expand(src, baseline_src, statics, baseline_statics, times, lengths, nullptr, 2, B, s0.T, s0.N, s0.ds, s0.ncls,
+                   nullptr, nullptr, src_e, stat_e, times_e, len_e, nullptr, st));
+  RD_TRY(raindrop_fwd(&de, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, endpoint_logits, nullptr, nullptr,
+                      nullptr, 0, st));
+  // 2. W1^T with its remainder, once per call
+  {
+    const rd_dims dc = ig_dims(dims, B * mc, mc);
+    Shape s;
+    RD_TRY(make_shape(&dc, &s));
+    if (s.tc) {
+      const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
+      RD_TRY(split_weights(&it, 1, st));
+    }
+  }
+  // 3. chunks of mc steps (the last one possibly shorter, same scratch, same arithmetic mode)
+  for (int c0 = 0; c0 < n_steps; c0 += mc) {
+    const int m = n_steps - c0 < mc ? n_steps - c0 : mc;
+    const rd_dims dc = ig_dims(dims, B * m, mc);
+    Shape s;
+    RD_TRY(make_shape(&dc, &s));
+    const BwLayout b = bw_layout(s);
+    RD_TRY(ig_expand(src, baseline_src, statics, baseline_statics, times, lengths, alphas + c0, m, B, s.T, s.N, s.ds, s.ncls,
+                     target, endpoint_logits + (int64_t)B * s.ncls, src_e, stat_e, times_e, len_e, dlog, st));
+    RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, S + l.logits, nullptr, nullptr,
+                        nullptr, 0, st));
+    RD_TRY(raindrop_bwd(&dc, params, stat_e, len_e, node_scale, ws, dlog, nullptr, sc, RD_BWD_ALL, nullptr, st));
+    RD_TRY(input_grad_dx0(s, params, sc + b.gO1, W1t, W1tlo, dX0, st));
+    RD_TRY(ig_accumulate(src, baseline_src, alphas + c0, weights + c0, m, B, s.T, s.N, s.dob, params->R_u, dX0, S + l.acc_src,
+                         attr_src, statics, baseline_statics, sc + b.dfeat, s.Df, s.D, params->emb_weight, s.emb, s.ds,
+                         S + l.acc_static, attr_st, c0 == 0, c0 + m >= n_steps, st));
+  }
+  return 0;
 }
 
 int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,

@@ -1,12 +1,18 @@
 #!/usr/bin/env python
 """Throughput of input gradients (the attribution workload: saliency maps, integrated gradients).
 
-    python tools/bench_input_grad.py [--config P19] [--steps 30] [--warmup 5]
+    python tools/bench_input_grad.py [--config P19] [--steps 30] [--warmup 5] [--ig-steps M]
 
 One call = eval-mode models_rd.Raindrop_v2.forward with frozen parameters (requires_grad_(False)) on the configuration's
 per-GPU batch, then torch.autograd.grad(logits[:, 0].sum(), [src, static, times]).  Timing follows bench.py: an L2 flush
 before every call outside the CUDA-event pair, median over calls.  Prints one JSON line with samples/s, ms per call, this
 library's kernel launches per call (rd_launch_count; torch's own ops are not counted) and the card's name and power limit.
+
+--ig-steps M [--ig-rows R] compares two ways of computing M-step integrated gradients (Gauss-Legendre nodes, zero
+baselines, target = the labels) of the same batch instead: one raindrop_b200.attribution.integrated_gradients call
+(internal_batch_size R), and the hand-written Python loop of M input-gradient calls on interpolated copies of the batch
+with host-side summing.  The two are timed in
+the same session, alternating call by call; samples/s counts the B samples of one call.
 """
 import argparse
 import json
@@ -32,11 +38,73 @@ def card():
         return "nvidia-smi unavailable (%r)" % (exc,)
 
 
+def launches_of(lib, fn):
+    torch.cuda.synchronize()
+    n0 = lib.rd_launch_count()
+    fn()
+    torch.cuda.synchronize()
+    return int(lib.rd_launch_count() - n0)
+
+
+def ig_compare(args, lib, cfg_name, model, b, device):
+    """Alternating timing of one integrated_gradients call and of the loop of M input-gradient calls."""
+    from raindrop_b200.attribution import _default_steps_per_chunk, integrated_gradients, quadrature
+    M = args.ig_steps
+    B = b["src"].shape[1]
+    N = b["src"].shape[2] // 2
+    a32, w32 = (torch.tensor(v, dtype=torch.float32) for v in quadrature(M, "gausslegendre"))
+    nodes = list(zip(a32.tolist(), w32.tolist()))
+    src, static, times, lengths, y = b["src"], b["static"], b["times"], b["lengths"], b["y"]
+
+    def batched():
+        integrated_gradients(model, src, static, times, lengths, target=y, n_steps=M, internal_batch_size=args.ig_rows)
+
+    def loop():
+        acc_src = torch.zeros_like(src)
+        acc_st = torch.zeros_like(static) if static is not None else None
+        for a, w in nodes:
+            xs = src.clone()
+            xs[:, :, :N] *= a
+            xs.requires_grad_(True)
+            leaves = [xs]
+            if static is not None:
+                leaves.append((static * a).requires_grad_(True))
+            logits, _, _ = model.forward(xs, leaves[1] if static is not None else None, times, lengths)
+            g = torch.autograd.grad(logits.gather(1, y[:, None]).sum(), leaves)
+            acc_src.add_(g[0], alpha=w)
+            if static is not None:
+                acc_st.add_(g[1], alpha=w)
+        return src * acc_src, (static * acc_st if static is not None else None)
+
+    for _ in range(max(1, args.warmup)):
+        batched()
+        loop()
+    n_batched, n_loop = launches_of(lib, batched), launches_of(lib, loop)
+    flush = torch.empty(L2_FLUSH_BYTES // 4, dtype=torch.float32, device=device)
+    t_b, t_l = [], []
+    for _ in range(args.steps):           # alternate: one timed call of each per round
+        t_b += timed_steps(batched, 1, flush)
+        t_l += timed_steps(loop, 1, flush)
+    sb, sl = summarize(t_b, 1, device), summarize(t_l, 1, device)
+    steps_per_chunk = min(M, max(1, args.ig_rows // B)) if args.ig_rows else \
+        _default_steps_per_chunk(lib, model._plan.dims(B, False), M)
+    res = {"metric": "integrated gradients, %d steps, samples/s (%s-shape synthetic)" % (M, cfg_name), "batch": B,
+           "ig_steps": M, "ig_rows": args.ig_rows, "steps_per_chunk": steps_per_chunk, "steps": args.steps, "card": card()}
+    for tag, t, n in (("batched", sb, n_batched), ("loop", sl, n_loop)):
+        res[tag] = {"samples_per_s": round(B / (t["median"] * 1e-3), 1), "ms_per_call": round(t["median"], 4),
+                    "ms_p90": round(t["p90"], 4), "launches_per_call": n}
+    res["speedup_batched_over_loop"] = round(sl["median"] / sb["median"], 3)
+    print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="P19", choices=sorted(BENCH_CONFIGS))
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--ig-steps", type=int, default=0, help="compare M-step integrated gradients, batched vs loop")
+    ap.add_argument("--ig-rows", type=int, default=None,
+                    help="internal_batch_size of the batched call ((sample, step) rows per chunk; default: 1 GiB scratch)")
     args = ap.parse_args()
     from raindrop_b200 import lib as L
     lib = L.load()
@@ -45,6 +113,9 @@ def main():
     cfg = model_config(cfg_name, dropout=0.2)
     model = build_model(cfg, device).eval().requires_grad_(False)
     b = {k: (v.to(device) if v is not None else None) for k, v in make_batch(cfg, batch, seed=2000, **opts).items()}
+    if args.ig_steps > 0:
+        ig_compare(args, lib, cfg_name, model, b, device)
+        return
     src = b["src"].clone().requires_grad_(True)
     times = b["times"].clone().requires_grad_(True)
     static = b["static"].clone().requires_grad_(True) if b["static"] is not None else None

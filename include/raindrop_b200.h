@@ -275,6 +275,39 @@ int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* pa
                                         void* scratch, float* attr_src, float* attr_statics, float* endpoint_logits,
                                         void* stream);
 
+/* ---- coalition attribution of Raindrop_v2: Shapley-value sampling and leave-one-out ablation, in one call ---------
+ * Players: sensor groups 0..G-1 (sensor_player [N], device int32, values in [0, G), every group non-empty) and, when
+ * d_static > 0, the static vector as player G; n_players = P = G + (d_static > 0).  Removing a player replaces the value
+ * columns src[:, b, n] of its sensors by baseline_src[:, b, n] (the static player: statics[b] by baseline_statics[b]);
+ * the mask half, times and lengths are never changed.  F(S) = logits[b, target[b]] of the eval-mode model on the input
+ * whose players outside S are removed; x = all players kept, x' = all removed.
+ *   RD_ATTR_SHAPLEY   attr[b, g] = (1/m) sum_p [F(S_pg + g) - F(S_pg)], S_pg = the players ahead of g in orders[p, :]
+ *                     (orders [m, P] device int32, each row a permutation of 0..P-1, shared by the batch); sum_g attr[b, g]
+ *                     = F(x) - F(x') up to rounding
+ *   RD_ATTR_ABLATION  attr[b, g] = F(x) - F(x without player g)   (orders may be NULL, m is ignored)
+ * Eval arithmetic: dims->training must be 0, the rng state is neither read nor advanced, no gradient is computed.
+ *   baseline_src     [T, B, 2N] (only the value half is read);  baseline_statics [B, d_static] or NULL when d_static == 0
+ *   target           [B] int64 class per sample, or NULL = argmax of the logits at x (read on the device)
+ *   attr             [B, P] fp32
+ *   endpoint_logits  [2, B, n_classes]: logits at x' ([0]) and at x ([1])
+ * Work: one forward on 2B rows for the endpoints, then the coalitions -- m*(P-1) for Shapley (the first k = 1..P-1
+ * players of each permutation; k = 0 and k = P are the endpoints), P for ablation (all but g) -- in chunks of
+ * `coalitions_per_chunk` coalitions on B*coalitions_per_chunk rows (coalition-major): the inputs expanded in one launch,
+ * the eval forward, and one launch that adds each coalition's F into fp64 running sums per (b, player) in a fixed order
+ * (deterministic, no atomics, independent of the chunking; a player whose removal changes no input bit gets exactly 0).
+ * dims->obprop_mode 0 is resolved once from B*coalitions_per_chunk rows, so the endpoint forward and every chunk use the
+ * same arithmetic.  scratch: rd_coalition_attribution_scratch_bytes(dims, n_players, coalitions_per_chunk) bytes
+ * (dims->B = samples, training = 0). */
+#define RD_ATTR_SHAPLEY 0
+#define RD_ATTR_ABLATION 1
+size_t rd_coalition_attribution_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t coalitions_per_chunk);
+int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                         const float* times, const int64_t* lengths, const float* node_scale,
+                                         const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                         const int32_t* sensor_player, int32_t n_players, const int32_t* orders, int32_t m,
+                                         int32_t method, int32_t coalitions_per_chunk, void* scratch, float* attr,
+                                         float* endpoint_logits, void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);

@@ -1,12 +1,18 @@
-"""Integrated-gradients (IG) attribution of Raindrop_v2, computed on the device in one call
-(rd_raindrop_v2_integrated_gradients), and the per-sensor ranking that the reference's leave-sensors-out experiment
-with feature_removal_level='set' reads (code/Raindrop.py:227-231, IG_density_scores_<dataset>.npy).
+"""Attribution of Raindrop_v2, computed on the device in one call per batch, and the per-sensor ranking that the
+reference's leave-sensors-out experiment with feature_removal_level='set' reads (code/Raindrop.py:227-231,
+IG_density_scores_<dataset>.npy):
+
+* integrated_gradients (rd_raindrop_v2_integrated_gradients): per input value, along the straight path from a baseline;
+* shapley_value_sampling and feature_ablation (rd_raindrop_v2_coalition_attribution): per sensor (group), of REMOVING
+  it -- replacing its value columns by the baseline, as the experiment does -- with the static vector one more player.
 
     attr_src, attr_static = integrated_gradients(model.eval(), src, static, times, lengths, target=y)
     ranking = sensor_ranking(sensor_importance(attr_src, model.d_inp), names)
+    phi, phi_static = shapley_value_sampling(model.eval(), src, static, times, lengths, target=y)
+    ranking = sensor_ranking(phi.abs().mean(dim=0), names)
     idx = data.removal_indices(B, model.d_inp, 0.5, level="set", density_scores=ranking[:, 0])
 
-Argument names follow Captum's IntegratedGradients.attribute.
+Argument names follow Captum's IntegratedGradients, ShapleyValueSampling and FeatureAblation.
 """
 import ctypes as C
 
@@ -18,6 +24,7 @@ from . import lib as L
 
 METHODS = ("gausslegendre", "riemann_trapezoid")
 DEFAULT_SCRATCH_BYTES = 1 << 30      # default chunking: the largest one whose scratch fits in 1 GiB
+RD_ATTR_SHAPLEY, RD_ATTR_ABLATION = 0, 1
 
 
 def quadrature(n_steps, method="gausslegendre"):
@@ -51,17 +58,28 @@ def _nodes(plan, n_steps, method, device):
     return got
 
 
-def _default_steps_per_chunk(lib, dims, n_steps, cap=DEFAULT_SCRATCH_BYTES):
-    """Largest steps_per_chunk <= n_steps whose scratch fits in `cap` bytes (host-only size queries); at least 1."""
-    lo, hi = 1, n_steps
+def _largest_chunk(scratch_bytes, n, cap=DEFAULT_SCRATCH_BYTES):
+    """Largest chunk c <= n whose scratch_bytes(c) fits in `cap` bytes (host-only size queries); at least 1."""
+    lo, hi = 1, max(1, n)
     while lo < hi:
         mid = (lo + hi + 1) // 2
-        nb = lib.rd_integrated_gradients_scratch_bytes(C.byref(dims), mid)
+        nb = scratch_bytes(mid)
         if 0 < nb <= cap:
             lo = mid
         else:
             hi = mid - 1
     return lo
+
+
+def _default_steps_per_chunk(lib, dims, n_steps, cap=DEFAULT_SCRATCH_BYTES):
+    """Largest steps_per_chunk <= n_steps whose integrated-gradients scratch fits in `cap` bytes; at least 1."""
+    return _largest_chunk(lambda c: lib.rd_integrated_gradients_scratch_bytes(C.byref(dims), c), n_steps, cap)
+
+
+def _default_coalitions_per_chunk(lib, dims, n_players, n_coalitions, cap=DEFAULT_SCRATCH_BYTES):
+    """Largest coalitions_per_chunk <= n_coalitions whose coalition-attribution scratch fits in `cap` bytes; at least 1."""
+    return _largest_chunk(lambda c: lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), n_players, c), n_coalitions,
+                          cap)
 
 
 def _check_target(target, B, n_classes):
@@ -103,6 +121,64 @@ def _baseline(b, like):
         raise ValueError("baseline of shape %s does not broadcast to %s" % (tuple(b.shape), tuple(like.shape))) from exc
 
 
+def _check_call(fn, model, src, static, baselines, internal_batch_size):
+    """The argument checks every attribution call shares (host only, before anything touches the device)."""
+    from .models_rd import Raindrop_v2
+    if not isinstance(model, Raindrop_v2):
+        raise TypeError("%s takes a raindrop_b200 Raindrop_v2 model, got %s" % (fn, type(model).__name__))
+    if model.training:
+        raise ValueError("%s runs the model in eval arithmetic: call model.eval() first" % fn)
+    if internal_batch_size is not None and int(internal_batch_size) < 1:
+        raise ValueError("internal_batch_size must be >= 1")
+    plan = model._plan
+    if src.dim() != 3 or src.shape[0] != plan.T or src.shape[2] != 2 * plan.N:
+        raise ValueError("src must be [max_len=%d, B, 2*d_inp=%d], got %s" % (plan.T, 2 * plan.N, tuple(src.shape)))
+    if model.static and static is None:
+        raise ValueError("this model was built with static=True: `static` must be a tensor")
+    if baselines is not None and (not isinstance(baselines, (tuple, list)) or len(baselines) != 2):
+        raise ValueError("baselines must be None or a pair (src_baseline, static_baseline)")
+
+
+class _Call:
+    """The device-side operands of one attribution call: inputs and baselines as contiguous fp32 / int64 device tensors,
+    the target, and the parameter pointers (rd_params; `keep` holds the tensors they point into)."""
+
+    def __init__(self, model, src, static, times, lengths, target, baselines):
+        from .models_rd import _device_of
+        B = src.shape[1]
+        target = _check_target(target, B, model._plan.n_classes)
+        self.device = device = _device_of(src)          # RaindropB200Error without CUDA
+        self.lib = L.load()
+        self.tgt = _target_tensor(target, B, device)
+        self.plan = plan = model._prepare(device)
+        f32 = dict(device=device, dtype=torch.float32)
+        self.x = src.detach().to(**f32).contiguous()
+        self.tm = times.detach().to(**f32).contiguous()
+        self.ln = lengths.detach().to(device=device, dtype=torch.int64).contiguous()
+        self.st = static.detach().to(**f32).contiguous() if model.static else None
+        b_src, b_st = baselines if baselines is not None else (None, None)
+        self.x0 = _baseline(b_src, self.x)
+        self.st0 = _baseline(b_st, self.st) if self.st is not None else None
+
+        params = [p.detach() for p in model.used_parameters()]
+        if params[0].device != device:
+            raise ValueError("the model's parameters are on %s, the inputs on %s" % (params[0].device, device))
+        self.keep = [t if (t.dtype == torch.float32 and t.is_contiguous()) else t.float().contiguous() for t in params]
+        self.params = L.RdParams()
+        self.params.R_u = plan.R_u.data_ptr()
+        for (_, path), t in zip(plan.fields, self.keep):
+            RF._set_field(self.params, path, t.data_ptr())
+
+    def scratch(self, name, key, nbytes):
+        """fp32 scratch of `nbytes`, one buffer per plan and entry point: a new key replaces the old one."""
+        plan = self.plan
+        cached = plan.__dict__.get(name)
+        if cached is None or cached[0] != key:
+            plan.__dict__[name] = None
+            cached = plan.__dict__[name] = (key, torch.empty(nbytes // 4, device=self.device, dtype=torch.float32))
+        return cached[1]
+
+
 def integrated_gradients(model, src, static, times, lengths, target=None, baselines=None, n_steps=50,
                          method="gausslegendre", internal_batch_size=None, return_convergence_delta=False):
     """Integrated gradients of F = logits[b, target[b]] of an eval-mode Raindrop_v2 with respect to the value half of
@@ -127,45 +203,11 @@ def integrated_gradients(model, src, static, times, lengths, target=None, baseli
     The call is stream-ordered and sync-free (a device-tensor target costs one sync for its range check): it neither
     changes the parameters, their .grad, the model's dropout rng state nor a bound FlatAdam.  Raises ValueError for a
     model in training mode and RaindropB200Error without CUDA."""
-    from .models_rd import Raindrop_v2, _device_of
-    if not isinstance(model, Raindrop_v2):
-        raise TypeError("integrated_gradients takes a raindrop_b200 Raindrop_v2 model, got %s" % type(model).__name__)
-    if model.training:
-        raise ValueError("integrated_gradients runs the model in eval arithmetic: call model.eval() first")
+    _check_call("integrated_gradients", model, src, static, baselines, internal_batch_size)
     n_steps = int(n_steps)
     quadrature(n_steps, method)                       # validates method and n_steps
-    if internal_batch_size is not None and int(internal_batch_size) < 1:
-        raise ValueError("internal_batch_size must be >= 1")
-    plan = model._plan
-    T, B = src.shape[0], src.shape[1]
-    if src.dim() != 3 or T != plan.T or src.shape[2] != 2 * plan.N:
-        raise ValueError("src must be [max_len=%d, B, 2*d_inp=%d], got %s" % (plan.T, 2 * plan.N, tuple(src.shape)))
-    if model.static and static is None:
-        raise ValueError("this model was built with static=True: `static` must be a tensor")
-    if baselines is not None and (not isinstance(baselines, (tuple, list)) or len(baselines) != 2):
-        raise ValueError("baselines must be None or a pair (src_baseline, static_baseline)")
-    target = _check_target(target, B, plan.n_classes)
-    device = _device_of(src)                          # RaindropB200Error without CUDA
-    lib = L.load()
-    tgt = _target_tensor(target, B, device)
-    plan = model._prepare(device)
-    f32 = dict(device=device, dtype=torch.float32)
-    x = src.detach().to(**f32).contiguous()
-    tm = times.detach().to(**f32).contiguous()
-    ln = lengths.detach().to(device=device, dtype=torch.int64).contiguous()
-    st = static.detach().to(**f32).contiguous() if model.static else None
-    b_src, b_st = baselines if baselines is not None else (None, None)
-    x0 = _baseline(b_src, x)
-    st0 = _baseline(b_st, st) if st is not None else None
-
-    params = [p.detach() for p in model.used_parameters()]
-    if params[0].device != device:
-        raise ValueError("the model's parameters are on %s, the inputs on %s" % (params[0].device, device))
-    keep = [t if (t.dtype == torch.float32 and t.is_contiguous()) else t.float().contiguous() for t in params]
-    P = L.RdParams()
-    P.R_u = plan.R_u.data_ptr()
-    for (_, path), t in zip(plan.fields, keep):
-        RF._set_field(P, path, t.data_ptr())
+    cl = _Call(model, src, static, times, lengths, target, baselines)
+    lib, plan, B = cl.lib, cl.plan, src.shape[1]
 
     dims = plan.dims(B, False)
     if internal_batch_size is None:
@@ -176,30 +218,189 @@ def integrated_gradients(model, src, static, times, lengths, target=None, baseli
     nbytes = lib.rd_integrated_gradients_scratch_bytes(C.byref(dims), mc)
     if nbytes == 0:
         L.check(-2, "rd_integrated_gradients_scratch_bytes")
-    key = (B, mc, dims.obprop_mode, device.index)
-    cached = plan.__dict__.get("_ig_attr_scratch")
-    if cached is None or cached[0] != key:             # one buffer per plan: a new shape replaces the old one
-        plan.__dict__["_ig_attr_scratch"] = None
-        cached = plan.__dict__["_ig_attr_scratch"] = (key, torch.empty(nbytes // 4, **f32))
-    scratch = cached[1]
-    alphas, weights = _nodes(plan, n_steps, method, device)
+    scratch = cl.scratch("_ig_attr_scratch", (B, mc, dims.obprop_mode, cl.device.index), nbytes)
+    alphas, weights = _nodes(plan, n_steps, method, cl.device)
 
-    attr_src = torch.empty_like(x)
-    attr_st = torch.empty_like(st) if st is not None else None
-    ends = torch.empty(2, B, plan.n_classes, **f32)
-    L.check(lib.rd_raindrop_v2_integrated_gradients(C.byref(dims), C.byref(P), x.data_ptr(), L.ptr(st), tm.data_ptr(),
-                                                    ln.data_ptr(), plan.node_scale.data_ptr(), x0.data_ptr(), L.ptr(st0),
-                                                    L.ptr(tgt), alphas.data_ptr(), weights.data_ptr(), n_steps, mc,
-                                                    scratch.data_ptr(), attr_src.data_ptr(), L.ptr(attr_st), ends.data_ptr(),
-                                                    L.stream_ptr(device)), "rd_raindrop_v2_integrated_gradients")
+    attr_src = torch.empty_like(cl.x)
+    attr_st = torch.empty_like(cl.st) if cl.st is not None else None
+    ends = torch.empty(2, B, plan.n_classes, device=cl.device, dtype=torch.float32)
+    L.check(lib.rd_raindrop_v2_integrated_gradients(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st),
+                                                    cl.tm.data_ptr(), cl.ln.data_ptr(), plan.node_scale.data_ptr(),
+                                                    cl.x0.data_ptr(), L.ptr(cl.st0), L.ptr(cl.tgt), alphas.data_ptr(),
+                                                    weights.data_ptr(), n_steps, mc, scratch.data_ptr(), attr_src.data_ptr(),
+                                                    L.ptr(attr_st), ends.data_ptr(), L.stream_ptr(cl.device)),
+            "rd_raindrop_v2_integrated_gradients")
     if not return_convergence_delta:
         return attr_src, attr_st
-    idx = tgt if tgt is not None else ends[1].argmax(dim=1)
-    f = ends.gather(2, idx.view(1, B, 1).expand(2, B, 1))[:, :, 0]          # [2, B]: F(x'), F(x)
+    f = _endpoint_values(ends, cl.tgt)
     total = attr_src.sum(dim=(0, 2))
     if attr_st is not None:
         total = total + attr_st.sum(dim=1)
     return attr_src, attr_st, total - (f[1] - f[0])
+
+
+def _endpoint_values(ends, tgt):
+    """[2, B]: F(x') and F(x) from the endpoint logits [2, B, n_classes] (tgt None: the argmax class at x)."""
+    B = ends.shape[1]
+    idx = tgt if tgt is not None else ends[1].argmax(dim=1)
+    return ends.gather(2, idx.view(1, B, 1).expand(2, B, 1))[:, :, 0]
+
+
+# ---- coalition attribution: Shapley-value sampling and leave-one-out ablation -----------------------------------------
+def sample_permutations(n_players, n_samples, seed=0):
+    """[n_samples, n_players] int64: n_samples permutations of range(n_players) drawn by numpy.random.default_rng(seed),
+    one rng.permutation call each.  The same seed gives the same permutations."""
+    n_players, n_samples = int(n_players), int(n_samples)
+    if n_players < 1 or n_samples < 1:
+        raise ValueError("n_players and n_samples must be >= 1, got %d and %d" % (n_players, n_samples))
+    rng = np.random.default_rng(seed)
+    return np.stack([rng.permutation(n_players) for _ in range(n_samples)]).astype(np.int64)
+
+
+def _check_groups(sensor_groups, N):
+    """int64 numpy [N] with values in [0, G), every group non-empty (default: one group per sensor), and G."""
+    if sensor_groups is None:
+        return np.arange(N, dtype=np.int64), N
+    g = torch.as_tensor(sensor_groups)
+    if g.is_floating_point() or g.is_complex() or g.dtype == torch.bool:
+        raise ValueError("sensor_groups must hold integer group indices")
+    g = g.cpu().numpy().astype(np.int64)
+    if g.shape != (N,):
+        raise ValueError("sensor_groups must have shape [d_inp=%d], got %s" % (N, g.shape))
+    if g.min() < 0:
+        raise ValueError("sensor_groups values must be >= 0, got %d" % g.min())
+    G = int(g.max()) + 1
+    empty = np.setdiff1d(np.arange(G), g)
+    if empty.size:
+        raise ValueError("sensor group(s) %s have no sensor: groups must be 0..G-1, each non-empty" % empty.tolist())
+    return g, G
+
+
+def _check_permutations(permutations, P):
+    p = torch.as_tensor(permutations)
+    if p.is_floating_point() or p.is_complex() or p.dtype == torch.bool:
+        raise ValueError("permutations must hold integer player indices")
+    p = p.cpu().numpy().astype(np.int64)
+    if p.ndim != 2 or p.shape[1] != P or p.shape[0] < 1:
+        raise ValueError("permutations must have shape [m >= 1, n_players=%d], got %s" % (P, p.shape))
+    bad = np.nonzero(np.any(np.sort(p, axis=1) != np.arange(P), axis=1))[0]
+    if bad.size:
+        raise ValueError("permutations row %d is not a permutation of range(%d)" % (bad[0], P))
+    return p
+
+
+def _device_int32(plan, kind, arr, device):
+    """Device int32 copy of a small host array, cached per plan (a CUDA-graph capture of a call copies nothing)."""
+    cache = plan.__dict__.setdefault("_coal_" + kind, {})
+    key = (arr.shape, arr.tobytes(), device.index)
+    got = cache.get(key)
+    if got is None:
+        got = cache[key] = torch.tensor(arr, dtype=torch.int32, device=device)
+    return got
+
+
+def _coalition_attribution(fn, method, model, src, static, times, lengths, target, baselines, sensor_groups,
+                           orders_host, internal_batch_size):
+    """attr [B, P] of rd_raindrop_v2_coalition_attribution, the endpoint logits [2, B, ncls], the target and G."""
+    groups, G = _check_groups(sensor_groups, model._plan.N)
+    P = G + (1 if model.static else 0)
+    orders = orders_host(P) if method == RD_ATTR_SHAPLEY else None
+    cl = _Call(model, src, static, times, lengths, target, baselines)
+    lib, plan, device, B = cl.lib, cl.plan, cl.device, src.shape[1]
+    if method == RD_ATTR_SHAPLEY:
+        m = orders.shape[0]
+        n_coal = m * (P - 1)
+        orders_d = _device_int32(plan, "orders", orders, device)
+    else:
+        m, n_coal, orders_d = 0, P, None
+    player = _device_int32(plan, "players", groups, device)
+
+    dims = plan.dims(B, False)
+    if internal_batch_size is None:
+        cc = _default_coalitions_per_chunk(lib, dims, P, n_coal)
+    else:
+        cc = max(1, int(internal_batch_size) // B)
+    cc = max(1, min(cc, n_coal))
+    nbytes = lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), P, cc)
+    if nbytes == 0:
+        L.check(-2, "rd_coalition_attribution_scratch_bytes")
+    scratch = cl.scratch("_coal_attr_scratch", (B, P, cc, dims.obprop_mode, device.index), nbytes)
+
+    attr = torch.empty(B, P, device=device, dtype=torch.float32)
+    ends = torch.empty(2, B, plan.n_classes, device=device, dtype=torch.float32)
+    L.check(lib.rd_raindrop_v2_coalition_attribution(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st),
+                                                     cl.tm.data_ptr(), cl.ln.data_ptr(), plan.node_scale.data_ptr(),
+                                                     cl.x0.data_ptr(), L.ptr(cl.st0), L.ptr(cl.tgt), player.data_ptr(), P,
+                                                     L.ptr(orders_d), m, method, cc, scratch.data_ptr(), attr.data_ptr(),
+                                                     ends.data_ptr(), L.stream_ptr(device)), fn)
+    return attr, ends, cl.tgt, G
+
+
+def _split(attr, G):
+    return attr[:, :G], (attr[:, G] if attr.shape[1] > G else None)
+
+
+def feature_ablation(model, src, static, times, lengths, target=None, baselines=None, sensor_groups=None,
+                     internal_batch_size=None):
+    """Leave-one-out ablation of F = logits[b, target[b]] of an eval-mode Raindrop_v2 over sensor groups and the static
+    vector:
+
+        attr[b, g] = F(x) - F(x with player g removed)
+
+    Players: the groups of `sensor_groups` (an int array [N] with values in [0, G), each group non-empty; default: one
+    group per sensor) and, when the model has statics, the static vector.  Removing a group replaces the value columns
+    src[:, b, n] of its sensors by the baseline (default 0: the reference's removal, data.remove_features_); removing
+    the static player replaces static[b] by its baseline.  The mask half, `times` and `lengths` never change.
+    Returns (attr_sensors [B, G], attr_static [B] or None), fp32 on the model's device.
+
+    target, baselines: as for integrated_gradients.  A static baseline equal to `static` holds the statics fixed (their
+                attribution is then exactly 0).
+    internal_batch_size: (sample, coalition) rows per chunk.  Default: the largest chunk whose scratch fits in 1 GiB.
+
+    The call runs one forward on 2B rows for F(x') and F(x) and one forward per coalition, all on the device, and is
+    stream-ordered, sync-free (a device-tensor target or sensor_groups costs one sync) and CUDA-graph capturable; it
+    changes neither the parameters, their .grad, the dropout rng state nor a bound FlatAdam.  Raises ValueError for a
+    model in training mode or bad arguments, TypeError for another model class and RaindropB200Error without CUDA."""
+    _check_call("feature_ablation", model, src, static, baselines, internal_batch_size)
+    attr, _, _, G = _coalition_attribution("rd_raindrop_v2_coalition_attribution", RD_ATTR_ABLATION, model, src, static,
+                                           times, lengths, target, baselines, sensor_groups, None, internal_batch_size)
+    return _split(attr, G)
+
+
+def shapley_value_sampling(model, src, static, times, lengths, target=None, baselines=None, sensor_groups=None,
+                           n_samples=25, seed=0, permutations=None, internal_batch_size=None,
+                           return_convergence_delta=False):
+    """Shapley values, by permutation sampling, of the game v(S) = F(x with the players outside S removed),
+    F = logits[b, target[b]] of an eval-mode Raindrop_v2; players and removal as for feature_ablation:
+
+        phi[b, g] = (1/m) sum_p [F(S_pg + {g}) - F(S_pg)],  S_pg = the players ahead of g in permutation p
+
+    The m permutations of the P players (the static player has index G) are shared by the batch, as in Captum: drawn
+    by sample_permutations(P, n_samples, seed), or given as `permutations` [m, P] (all P! of them give the exact
+    Shapley values).  Efficiency: sum_g phi[b, g] (+ the static player's) = F(x) - F(x') up to rounding.
+
+    Returns (attr_sensors [B, G], attr_static [B] or None), plus delta [B] = sum of the sample's attributions -
+    (F(x) - F(x')) when return_convergence_delta.  The call evaluates m*(P-1) coalitions on the device besides the
+    endpoints; everything else is as for feature_ablation."""
+    _check_call("shapley_value_sampling", model, src, static, baselines, internal_batch_size)
+    if permutations is None:
+        n_samples = int(n_samples)
+        if n_samples < 1:
+            raise ValueError("n_samples must be >= 1, got %d" % n_samples)
+
+        def orders_host(P):
+            return sample_permutations(P, n_samples, seed)
+    else:
+        def orders_host(P):
+            return _check_permutations(permutations, P)
+    attr, ends, tgt, G = _coalition_attribution("rd_raindrop_v2_coalition_attribution", RD_ATTR_SHAPLEY, model, src,
+                                                static, times, lengths, target, baselines, sensor_groups, orders_host,
+                                                internal_batch_size)
+    out = _split(attr, G)
+    if not return_convergence_delta:
+        return out
+    f = _endpoint_values(ends, tgt).double()
+    return out + ((attr.double().sum(dim=1) - (f[1] - f[0])).float(),)
 
 
 def sensor_importance(attr_src, n_sensors):

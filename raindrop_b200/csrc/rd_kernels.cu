@@ -347,6 +347,20 @@ __global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const
 // Point alpha of the straight path from the baseline x0 to x.  Exact at both ends: alpha = 0 gives x0, alpha = 1 gives x.
 __device__ __forceinline__ float ig_interp(float x, float x0, float a) { return fmaf(a, x, (1.f - a) * x0); }
 
+// The attributed class of sample b: target[b], or (target == NULL) the first maximum of logits_x[b, :], as torch.argmax
+__device__ __forceinline__ int target_class(const int64_t* __restrict__ target, const float* __restrict__ logits_x, int b,
+                                            int ncls) {
+  if (target) return (int)__ldg(target + b);
+  const float* l = logits_x + (long long)b * ncls;
+  float best = __ldg(l);
+  int tgt = 0;
+  for (int c = 1; c < ncls; ++c) {
+    const float v = __ldg(l + c);
+    if (v > best) { best = v; tgt = c; }
+  }
+  return tgt;
+}
+
 // Inputs of one chunk of m path steps on B*m rows, step-major (row j = k*B + b), in one launch with four thread ranges:
 //   src_e[t, j, n] = interp(src[t, b, n], src0[t, b, n], alpha_k) (value half), src[t, b, n] (mask half, copied)
 //   times_e[t, j] = times[t, b]
@@ -397,17 +411,7 @@ __global__ void ig_expand_kernel(const __grid_constant__ IgExpandArgs a) {
   const int b = (int)(o % a.B);
   a.lengths_e[o] = __ldg(a.lengths + b);
   if (!a.d_logits) return;
-  int tgt = 0;
-  if (a.target) {
-    tgt = (int)__ldg(a.target + b);
-  } else {       // first maximum, as torch.argmax
-    const float* l = a.logits_x + (long long)b * a.ncls;
-    float best = __ldg(l);
-    for (int c = 1; c < a.ncls; ++c) {
-      const float v = __ldg(l + c);
-      if (v > best) { best = v; tgt = c; }
-    }
-  }
+  const int tgt = target_class(a.target, a.logits_x, b, a.ncls);
   float* d = a.d_logits + o * a.ncls;
   for (int c = 0; c < a.ncls; ++c) d[c] = c == tgt ? 1.f : 0.f;
 }
@@ -459,6 +463,118 @@ __global__ void ig_accum_kernel(const __grid_constant__ IgAccumArgs a) {
     acc = fmaf(__ldg(a.weights + k), emb_bwd(a.dfeat + ((long long)k * a.B + b) * a.Df + a.feat_col0, a.W_emb, a.emb, a.ds, kk), acc);
   if (a.last) a.attr_static[o] = (__ldg(a.statics + o) - __ldg(a.statics0 + o)) * acc + 0.f;
   else a.acc_static[o] = acc;
+}
+
+// ---- coalition attribution: Shapley-value sampling, leave-one-out ablation (rd_raindrop_v2_coalition_attribution) --
+// Coalition c keeps the players it names and replaces every other player by its baseline.
+//   Shapley (method 0): c = p*(P-1) + k-1, k = 1..P-1, keeps the first k players of permutation p (orders[p, :k])
+//   ablation (method 1): c = g, keeps every player but g
+__device__ __forceinline__ bool coalition_keeps(const int32_t* __restrict__ orders, int P, int method, int c, int g) {
+  if (method == RD_ATTR_ABLATION) return c != g;
+  const int p = c / (P - 1), k = c - p * (P - 1) + 1;
+  const int32_t* o = orders + (long long)p * P;
+  for (int i = 0; i < k; ++i)
+    if (__ldg(o + i) == g) return true;
+  return false;
+}
+
+// Inputs of one chunk of nc coalitions c0 .. c0+nc-1 on B*nc rows, coalition-major (row j = ci*B + b), in one launch:
+//   src_e[t, j, n] = keep(player[n]) ? src[t, b, n] : src0[t, b, n] (value half), src[t, b, n] (mask half, copied)
+//   times_e[t, j] = times[t, b];  lengths_e[j] = lengths[b]
+//   statics_e[j, :] = keep(P-1) ? statics[b, :] : statics0[b, :]  (the static player is the last one)
+struct CoalitionExpandArgs {
+  const float* src; const float* src0; const float* statics; const float* statics0; const float* times;
+  const int64_t* lengths; const int32_t* player; const int32_t* orders;
+  float* src_e; float* statics_e; float* times_e; int64_t* lengths_e;
+  int P, method, c0, nc, B, T, N, ds;
+  long long n_src, n_tok, n_stat, n_rows;
+};
+__global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long rows = (long long)a.B * a.nc;
+  if (o < a.n_src) {
+    const int w = 2 * a.N;
+    const long long tj = o / w;
+    const int c = (int)(o - tj * w);
+    const long long t = tj / rows;
+    const int j = (int)(tj - t * rows), ci = j / a.B, b = j - ci * a.B;
+    const long long i = (t * a.B + b) * w + c;
+    const bool x = c >= a.N || coalition_keeps(a.orders, a.P, a.method, a.c0 + ci, __ldg(a.player + c));
+    a.src_e[o] = __ldg((x ? a.src : a.src0) + i);
+    return;
+  }
+  o -= a.n_src;
+  if (o < a.n_tok) {
+    const long long t = o / rows;
+    const int b = (int)((o - t * rows) % a.B);
+    a.times_e[o] = __ldg(a.times + t * a.B + b);
+    return;
+  }
+  o -= a.n_tok;
+  if (o < a.n_stat) {
+    const long long j = o / a.ds;
+    const int kk = (int)(o - j * a.ds), ci = (int)(j / a.B), b = (int)(j - (long long)ci * a.B);
+    const bool x = coalition_keeps(a.orders, a.P, a.method, a.c0 + ci, a.P - 1);
+    a.statics_e[o] = __ldg((x ? a.statics : a.statics0) + (long long)b * a.ds + kk);
+    return;
+  }
+  o -= a.n_stat;
+  if (o >= a.n_rows) return;
+  a.lengths_e[o] = __ldg(a.lengths + o % a.B);
+}
+
+// One thread per (b, player g) adds the chunk's coalition values F = logits_c[ci*B + b, target] into an fp64 running
+// sum acc[b, g], coalitions in order:
+//   Shapley : F(p, k) enters with + for the player at position k-1 of p and with - for the player at position k; the
+//             first chunk starts from the endpoints: + F(x) for each permutation's last player, - F(x') for its first
+//   ablation: the first chunk starts from F(x), coalition g enters with - for player g
+// The last chunk writes attr[b, g] = acc / m (Shapley) or acc (ablation) in fp32.  Fixed order, no atomics:
+// the fp32 values sum exactly in fp64 at logit magnitudes, so the result does not depend on the chunking.
+struct CoalitionAccumArgs {
+  const float* logits_c; const float* ends; const int64_t* target; const int32_t* orders;
+  double* acc; float* attr;
+  int P, method, m, c0, nc, B, ncls, first, last;
+};
+__global__ void coalition_accum_kernel(const __grid_constant__ CoalitionAccumArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= (long long)a.B * a.P) return;
+  const int b = (int)(o / a.P), g = (int)(o - (long long)b * a.P);
+  const int tgt = target_class(a.target, a.ends + (long long)a.B * a.ncls, b, a.ncls);
+  double s;
+  if (a.first) {
+    const double fx = __ldg(a.ends + ((long long)a.B + b) * a.ncls + tgt);
+    if (a.method == RD_ATTR_ABLATION) {
+      s = fx;
+    } else {
+      const double fx0 = __ldg(a.ends + (long long)b * a.ncls + tgt);
+      s = 0.0;
+      for (int p = 0; p < a.m; ++p) {
+        const int32_t* r = a.orders + (long long)p * a.P;
+        if (__ldg(r + a.P - 1) == g) s += fx;
+        if (__ldg(r) == g) s -= fx0;
+      }
+    }
+  } else {
+    s = a.acc[o];
+  }
+  for (int ci = 0; ci < a.nc; ++ci) {
+    const double f = __ldg(a.logits_c + ((long long)ci * a.B + b) * a.ncls + tgt);
+    const int c = a.c0 + ci;
+    if (a.method == RD_ATTR_ABLATION) {
+      if (c == g) s -= f;
+    } else {
+      const int p = c / (a.P - 1), k = c - p * (a.P - 1) + 1;
+      const int32_t* r = a.orders + (long long)p * a.P;
+      if (__ldg(r + k - 1) == g) s += f;
+      if (__ldg(r + k) == g) s -= f;
+    }
+  }
+  if (a.last) a.attr[o] = (float)(a.method == RD_ATTR_ABLATION ? s : s / a.m);
+  else a.acc[o] = s;
 }
 
 // one warp per node: segment max, then sum of exp, then s = sum(exp / (sum + 1e-16))
@@ -1092,6 +1208,33 @@ int ig_accumulate(const float* src, const float* src0, const float* alphas, cons
   a.first = first; a.last = last;
   launch_pdl(ig_accum_kernel, dim3(blocks_for(a.n_lift + a.n_static)), dim3(TPB), 0, st, a);
   RD_CHECK_LAUNCH("ig_accum_kernel");
+  return 0;
+}
+
+int coalition_expand(const float* src, const float* src0, const float* statics, const float* statics0, const float* times,
+                     const int64_t* lengths, const int32_t* player, const int32_t* orders, int P, int method, int c0, int nc,
+                     int B, int T, int N, int ds, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e,
+                     cudaStream_t st) {
+  CoalitionExpandArgs a;
+  a.src = src; a.src0 = src0; a.statics = statics; a.statics0 = statics0; a.times = times; a.lengths = lengths;
+  a.player = player; a.orders = orders;
+  a.src_e = src_e; a.statics_e = statics_e; a.times_e = times_e; a.lengths_e = lengths_e;
+  a.P = P; a.method = method; a.c0 = c0; a.nc = nc; a.B = B; a.T = T; a.N = N; a.ds = ds;
+  const int64_t rows = (int64_t)B * nc;
+  a.n_src = (int64_t)T * rows * 2 * N; a.n_tok = (int64_t)T * rows; a.n_stat = ds > 0 ? rows * ds : 0; a.n_rows = rows;
+  launch_pdl(coalition_expand_kernel, dim3(blocks_for(a.n_src + a.n_tok + a.n_stat + a.n_rows)), dim3(TPB), 0, st, a);
+  RD_CHECK_LAUNCH("coalition_expand_kernel");
+  return 0;
+}
+
+int coalition_accumulate(const float* logits_c, const float* ends, const int64_t* target, const int32_t* orders, int P,
+                         int method, int m, int c0, int nc, int B, int ncls, double* acc, float* attr, int first, int last,
+                         cudaStream_t st) {
+  CoalitionAccumArgs a;
+  a.logits_c = logits_c; a.ends = ends; a.target = target; a.orders = orders; a.acc = acc; a.attr = attr;
+  a.P = P; a.method = method; a.m = m; a.c0 = c0; a.nc = nc; a.B = B; a.ncls = ncls; a.first = first; a.last = last;
+  launch_pdl(coalition_accum_kernel, dim3(blocks_for((int64_t)B * P)), dim3(TPB), 0, st, a);
+  RD_CHECK_LAUNCH("coalition_accum_kernel");
   return 0;
 }
 

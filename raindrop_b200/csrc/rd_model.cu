@@ -208,6 +208,30 @@ int ig_layout(const rd_dims* dims, int mc, IgcLayout* l) {
   return 0;
 }
 
+// ---- coalition attribution (Shapley-value sampling, ablation) -------------------------------------------------------
+// Scratch of rd_raindrop_v2_coalition_attribution: the eval forward workspace and the expanded inputs of max(B*cc, 2B)
+// rows (chunks of cc coalitions and the endpoint forward), the chunk's logits and the fp64 running sums [B, P].  The
+// ob-prop mode is pinned from B*cc rows by ig_dims, as for integrated gradients.
+struct CoalLayout { int64_t ws, src, statics, times, lengths, logits, acc, total; };
+int coalition_layout(const rd_dims* dims, int n_players, int cc, CoalLayout* l) {
+  if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("coalitions_per_chunk = %d out of range", cc); return -2; }
+  if (n_players < 1) { set_error("n_players = %d must be >= 1", n_players); return -2; }
+  const int Bc = dims->B * cc, Bx = Bc > 2 * dims->B ? Bc : 2 * dims->B;
+  const rd_dims dx = ig_dims(dims, Bx, cc);
+  Shape sx;
+  RD_TRY(make_shape(&dx, &sx));
+  Arena a;
+  l->ws = a.take(ws_layout(sx).total);
+  l->src = a.take(sx.M2 * 2 * sx.N);
+  l->statics = a.take((int64_t)Bx * sx.ds);
+  l->times = a.take(sx.M2);
+  l->lengths = a.take(2LL * Bx);
+  l->logits = a.take((int64_t)Bc * sx.ncls);
+  l->acc = a.take(2LL * dims->B * n_players);
+  l->total = a.off;
+  return 0;
+}
+
 // Y[M,N] = epi(X[M,K] . W[N,K]^T)
 GemmP nt(const float* X, int64_t ldx, const float* W, int64_t ldw, float* Y, int64_t ldy, int64_t M, int N, int K) {
   GemmP g;
@@ -911,6 +935,78 @@ int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* pa
                          attr_src, statics, baseline_statics, sc + b.dfeat, s.Df, s.D, params->emb_weight, s.emb, s.ds,
                          S + l.acc_static, attr_st, c0 == 0, c0 + m >= n_steps, st));
   }
+  return 0;
+}
+
+size_t rd_coalition_attribution_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t coalitions_per_chunk) {
+  if (!dims) return 0;
+  CoalLayout l;
+  if (coalition_layout(dims, n_players, coalitions_per_chunk, &l) != 0) return 0;
+  return (size_t)l.total * sizeof(float);
+}
+
+int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                         const float* times, const int64_t* lengths, const float* node_scale,
+                                         const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                         const int32_t* sensor_player, int32_t n_players, const int32_t* orders, int32_t m,
+                                         int32_t method, int32_t coalitions_per_chunk, void* scratch, float* attr,
+                                         float* endpoint_logits, void* stream) {
+  if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !sensor_player || !scratch || !attr ||
+      !endpoint_logits || !params->R_u || !params->ob1_value_weight) {
+    set_error("rd_raindrop_v2_coalition_attribution: NULL argument");
+    return -2;
+  }
+  if (method != RD_ATTR_SHAPLEY && method != RD_ATTR_ABLATION) {
+    set_error("rd_raindrop_v2_coalition_attribution: method must be RD_ATTR_SHAPLEY or RD_ATTR_ABLATION, got %d", method);
+    return -2;
+  }
+  if (dims->training) { set_error("rd_raindrop_v2_coalition_attribution: runs eval arithmetic, dims->training must be 0"); return -2; }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s0.ds > 0 && (!statics || !baseline_statics)) {
+    set_error("rd_raindrop_v2_coalition_attribution: d_static > 0 needs statics and baseline_statics");
+    return -2;
+  }
+  const int P = n_players, G = P - (s0.ds > 0 ? 1 : 0);
+  if (G < 1 || G > s0.N) { set_error("rd_raindrop_v2_coalition_attribution: n_players = %d gives %d sensor groups for N = %d", P, G, s0.N); return -2; }
+  if (method == RD_ATTR_SHAPLEY && (!orders || m < 1 || (int64_t)m * (P - 1) > (1LL << 30))) {
+    set_error("rd_raindrop_v2_coalition_attribution: Shapley sampling needs orders and 1 <= m, m*(P-1) <= 2^30 (m = %d)", m);
+    return -2;
+  }
+  CoalLayout l;
+  RD_TRY(coalition_layout(dims, P, coalitions_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, cc = coalitions_per_chunk;
+  const int n_coal = method == RD_ATTR_SHAPLEY ? m * (P - 1) : P;
+  float* S = (float*)scratch;
+  float* ws = S + l.ws; float* logits = S + l.logits;
+  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
+  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  double* acc = reinterpret_cast<double*>(S + l.acc);
+
+  // 1. the endpoints: one forward on 2B rows (baseline rows, then input rows) -> endpoint_logits [2, B, ncls]
+  const rd_dims de = ig_dims(dims, 2 * B, cc);
+  RD_TRY(ig_expand(src, baseline_src, statics, baseline_statics, times, lengths, nullptr, 2, B, s0.T, s0.N, s0.ds, s0.ncls,
+                   nullptr, nullptr, src_e, stat_e, times_e, len_e, nullptr, st));
+  RD_TRY(raindrop_fwd(&de, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, endpoint_logits, nullptr, nullptr,
+                      nullptr, 0, st));
+  // 2. chunks of cc coalitions (the last one possibly shorter, same scratch, same arithmetic mode); with no coalition
+  //    (Shapley over one player) a single accumulation turns the endpoints into the result
+  int c0 = 0;
+  do {
+    const int nc = n_coal - c0 < cc ? n_coal - c0 : cc;
+    if (nc > 0) {
+      const rd_dims dc = ig_dims(dims, B * nc, cc);
+      RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, sensor_player, orders, P, method,
+                              c0, nc, B, s0.T, s0.N, s0.ds, src_e, stat_e, times_e, len_e, st));
+      RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, logits, nullptr, nullptr,
+                          nullptr, 0, st));
+    }
+    RD_TRY(coalition_accumulate(logits, endpoint_logits, target, orders, P, method, m, c0, nc, B, s0.ncls, acc, attr, c0 == 0,
+                                c0 + nc >= n_coal, st));
+    c0 += cc;
+  } while (c0 < n_coal);
   return 0;
 }
 

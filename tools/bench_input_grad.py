@@ -13,6 +13,11 @@ baselines, target = the labels) of the same batch instead: one raindrop_b200.att
 (internal_batch_size R), and the hand-written Python loop of M input-gradient calls on interpolated copies of the batch
 with host-side summing.  The two are timed in
 the same session, alternating call by call; samples/s counts the B samples of one call.
+
+--ablation or --shapley-samples M [--coalition-rows R] compare, the same way, one raindrop_b200.attribution
+feature_ablation / shapley_value_sampling call (one player per sensor plus the static vector, zero baselines, target =
+the labels, internal_batch_size R) with the hand-written loop of B-row module forwards over the same coalitions
+(P + 1 forwards for ablation; m*(P-1) + 2 for M permutations) summing F in fp64 tensors.
 """
 import argparse
 import json
@@ -97,6 +102,77 @@ def ig_compare(args, lib, cfg_name, model, b, device):
     print(json.dumps(res), flush=True)
 
 
+def coalition_compare(args, lib, cfg_name, model, b, device):
+    """Alternating timing of one feature_ablation / shapley_value_sampling call and of the loop of module forwards."""
+    from raindrop_b200.attribution import (_default_coalitions_per_chunk, feature_ablation, sample_permutations,
+                                           shapley_value_sampling)
+    src, static, times, lengths, y = b["src"], b["static"], b["times"], b["lengths"], b["y"]
+    B, N = src.shape[1], src.shape[2] // 2
+    P = N + (1 if static is not None else 0)
+    M = args.shapley_samples
+    orders = sample_permutations(P, M, 0).tolist() if M else None
+    n_coal = M * (P - 1) if M else P
+
+    def batched():
+        if M:
+            shapley_value_sampling(model, src, static, times, lengths, target=y, n_samples=M, seed=0,
+                                   internal_batch_size=args.coalition_rows)
+        else:
+            feature_ablation(model, src, static, times, lengths, target=y, internal_batch_size=args.coalition_rows)
+
+    def F(keep):                  # keep: [P] bool device tensor; players = sensors, then the static vector
+        x = src.clone()
+        x[:, :, :N] = torch.where(keep[:N], src[:, :, :N], 0.0)
+        st = None if static is None else torch.where(keep[N], static, 0.0)
+        logits, _, _ = model.forward(x, st, times, lengths)
+        return logits.gather(1, y[:, None])[:, 0].double()
+
+    ones = torch.ones(P, dtype=torch.bool, device=device)
+
+    def loop():
+        fx = F(ones)
+        attr = torch.zeros(B, P, dtype=torch.float64, device=device)
+        if not M:
+            for g in range(P):
+                keep = ones.clone()
+                keep[g] = False
+                attr[:, g] = fx - F(keep)
+            return attr
+        fx0 = F(~ones)
+        for p in orders:
+            keep = ~ones
+            prev = fx0
+            for k, g in enumerate(p):
+                keep = keep.clone()
+                keep[g] = True
+                cur = fx if k == P - 1 else F(keep)
+                attr[:, g] += cur - prev
+                prev = cur
+        return attr / M
+
+    for _ in range(max(1, args.warmup)):
+        batched()
+        loop()
+    n_batched, n_loop = launches_of(lib, batched), launches_of(lib, loop)
+    flush = torch.empty(L2_FLUSH_BYTES // 4, dtype=torch.float32, device=device)
+    t_b, t_l = [], []
+    for _ in range(args.steps):           # alternate: one timed call of each per round
+        t_b += timed_steps(batched, 1, flush)
+        t_l += timed_steps(loop, 1, flush)
+    sb, sl = summarize(t_b, 1, device), summarize(t_l, 1, device)
+    cc = min(n_coal, max(1, args.coalition_rows // B)) if args.coalition_rows else \
+        _default_coalitions_per_chunk(lib, model._plan.dims(B, False), P, n_coal)
+    what = "Shapley-value sampling, %d permutations" % M if M else "leave-one-out ablation"
+    res = {"metric": "%s, %d players, samples/s (%s-shape synthetic)" % (what, P, cfg_name), "batch": B,
+           "shapley_samples": M, "coalitions": n_coal, "coalition_rows": args.coalition_rows,
+           "coalitions_per_chunk": cc, "steps": args.steps, "card": card()}
+    for tag, t, n in (("batched", sb, n_batched), ("loop", sl, n_loop)):
+        res[tag] = {"samples_per_s": round(B / (t["median"] * 1e-3), 1), "ms_per_call": round(t["median"], 4),
+                    "ms_p90": round(t["p90"], 4), "launches_per_call": n}
+    res["speedup_batched_over_loop"] = round(sl["median"] / sb["median"], 3)
+    print(json.dumps(res), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="P19", choices=sorted(BENCH_CONFIGS))
@@ -105,6 +181,12 @@ def main():
     ap.add_argument("--ig-steps", type=int, default=0, help="compare M-step integrated gradients, batched vs loop")
     ap.add_argument("--ig-rows", type=int, default=None,
                     help="internal_batch_size of the batched call ((sample, step) rows per chunk; default: 1 GiB scratch)")
+    ap.add_argument("--ablation", action="store_true", help="compare leave-one-out sensor ablation, batched vs loop")
+    ap.add_argument("--shapley-samples", type=int, default=0,
+                    help="compare M-permutation sensor Shapley-value sampling, batched vs loop")
+    ap.add_argument("--coalition-rows", type=int, default=None,
+                    help="internal_batch_size of the batched ablation / Shapley call ((sample, coalition) rows per "
+                         "chunk; default: 1 GiB scratch)")
     args = ap.parse_args()
     from raindrop_b200 import lib as L
     lib = L.load()
@@ -115,6 +197,9 @@ def main():
     b = {k: (v.to(device) if v is not None else None) for k, v in make_batch(cfg, batch, seed=2000, **opts).items()}
     if args.ig_steps > 0:
         ig_compare(args, lib, cfg_name, model, b, device)
+        return
+    if args.ablation or args.shapley_samples > 0:
+        coalition_compare(args, lib, cfg_name, model, b, device)
         return
     src = b["src"].clone().requires_grad_(True)
     times = b["times"].clone().requires_grad_(True)

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Writes IG_density_scores_<name>.npy, the sensor ranking the reference's leave-sensors-out experiment with
-feature_removal_level='set' reads (code/Raindrop.py:227-231), from a trained Raindrop_v2 and a data set:
+feature_removal_level='set' reads (code/Raindrop.py:227-231), from a trained Raindrop_v2 and a data set (or, with
+--method ablation / shapley, Ablation_density_scores_<name>.npy / Shapley_density_scores_<name>.npy):
 
     python tools/ig_sensor_ranking.py --checkpoint model.pt --data P19data/processed_data/PTdict_list.npy \\
         --outcomes P19data/processed_data/arr_outcomes.npy --split P19data/splits/phy19_split1_new.npy --part test \\
@@ -17,6 +18,11 @@ label when --outcomes is given, else the predicted class) attributes the value h
 over samples of sum_t |attribution|, and the ranking lists (index, name) in descending score.  Column 0 of the file is
 what data.removal_indices(..., level="set", density_scores=...) takes.  The recipe behind the reference's shipped files
 is not recorded, so this ranking is not claimed to reproduce them.
+
+--method ablation / shapley rank by the attribution of REMOVING each sensor (zeroing its value columns, as the
+experiment does; the static vector is held fixed): raindrop_b200.attribution.feature_ablation, or
+shapley_value_sampling with --shapley-samples permutations (seed --seed).  A sensor's score is the mean over samples of
+|attribution|; the file has the same [N, 2] layout.
 """
 import argparse
 import os
@@ -62,18 +68,21 @@ def main():
     ap.add_argument("--part", default="test", choices=["train", "val", "test"])
     ap.add_argument("--n-samples", type=int, default=512, help="--synthetic: number of samples")
     ap.add_argument("--sensor-names", help="text file, one sensor name per line (default: the indices)")
-    ap.add_argument("--steps", type=int, default=50, help="Gauss-Legendre nodes per attribution")
+    ap.add_argument("--method", default="ig", choices=["ig", "ablation", "shapley"])
+    ap.add_argument("--steps", type=int, default=50, help="--method ig: Gauss-Legendre nodes per attribution")
+    ap.add_argument("--shapley-samples", type=int, default=25, help="--method shapley: permutations per batch")
     ap.add_argument("--batch-size", type=int, default=128)
     ap.add_argument("--name", help="file name suffix (default: the synthetic configuration or 'dataset')")
     ap.add_argument("--out-dir", default=".")
     args = ap.parse_args()
 
     from raindrop_b200 import data as RD
-    from raindrop_b200.attribution import integrated_gradients, sensor_importance, sensor_ranking
+    from raindrop_b200.attribution import (feature_ablation, integrated_gradients, sensor_importance, sensor_ranking,
+                                           shapley_value_sampling)
     from raindrop_b200.synth import make_batch, model_config
     device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else None
     if device is None:
-        raise SystemExit("integrated gradients run on a CUDA device")
+        raise SystemExit("attribution runs on a CUDA device")
     model = model_from_state_dict(torch.load(args.checkpoint, map_location="cpu"), args.nhead, args.seed, device)
     N, T = model.d_inp, model.max_len
 
@@ -118,11 +127,21 @@ def main():
         src, times = P[:, s:e], Ptime[:, s:e]
         lengths = torch.sum(times > 0, dim=0)
         static = None if Pstatic is None else Pstatic[s:e]
-        attr_src, _ = integrated_gradients(model, src, static, times, lengths, target=None if y is None else y[s:e],
-                                           n_steps=args.steps)
-        total += sensor_importance(attr_src, N).double() * (e - s)
+        target = None if y is None else y[s:e]
+        if args.method == "ig":
+            attr_src, _ = integrated_gradients(model, src, static, times, lengths, target=target, n_steps=args.steps)
+            total += sensor_importance(attr_src, N).double() * (e - s)
+            continue
+        fixed = (None, static)                  # statics held fixed: only sensors are players that change the input
+        if args.method == "ablation":
+            attr, _ = feature_ablation(model, src, static, times, lengths, target=target, baselines=fixed)
+        else:
+            attr, _ = shapley_value_sampling(model, src, static, times, lengths, target=target, baselines=fixed,
+                                             n_samples=args.shapley_samples, seed=args.seed)
+        total += attr.double().abs().sum(dim=0)
     ranking = sensor_ranking(total / n, names)
-    out = os.path.join(args.out_dir, "IG_density_scores_%s.npy" % name)
+    prefix = {"ig": "IG", "ablation": "Ablation", "shapley": "Shapley"}[args.method]
+    out = os.path.join(args.out_dir, "%s_density_scores_%s.npy" % (prefix, name))
     np.save(out, ranking)
     print("wrote %s: %d sensors, top 5 %s" % (out, N, ranking[:5].tolist()))
 

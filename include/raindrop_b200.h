@@ -280,7 +280,8 @@ int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* pa
  * d_static > 0, the static vector as player G; n_players = P = G + (d_static > 0).  Removing a player replaces the value
  * columns src[:, b, n] of its sensors by baseline_src[:, b, n] (the static player: statics[b] by baseline_statics[b]);
  * the mask half, times and lengths are never changed.  F(S) = logits[b, target[b]] of the eval-mode model on the input
- * whose players outside S are removed; x = all players kept, x' = all removed.
+ * whose players outside S are removed; x = all players kept, x' = all removed (with the cell entry point below, the cells
+ * of no player keep x in x' too).
  *   RD_ATTR_SHAPLEY   attr[b, g] = (1/m) sum_p [F(S_pg + g) - F(S_pg)], S_pg = the players ahead of g in orders[p, :]
  *                     (orders [m, P] device int32, each row a permutation of 0..P-1, shared by the batch); sum_g attr[b, g]
  *                     = F(x) - F(x') up to rounding
@@ -307,6 +308,29 @@ int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* p
                                          const int32_t* sensor_player, int32_t n_players, const int32_t* orders, int32_t m,
                                          int32_t method, int32_t coalitions_per_chunk, void* scratch, float* attr,
                                          float* endpoint_logits, void* stream);
+
+/* ---- coalition attribution of Raindrop_v2 over value cells: (sensor, time window) players and any other map ---------
+ * As rd_raindrop_v2_coalition_attribution, with a player per value cell instead of per sensor: cell (t, b, n) of the
+ * value half belongs to player cell_player[t*player_stride_t + b*player_stride_b + n] (device int32).  Ids 0..G-1 are
+ * players of the value cells, G = n_players - (d_static > 0), and when d_static > 0 the static vector is player G.  Any
+ * other id (negative, or >= G) belongs to no player: that cell always keeps x.  A player with no cell in sample b gets
+ * exactly 0 there; G may exceed N.  Strides select the map's layout (both >= 0):
+ *   (0, 0)     per sensor [N]  (rd_raindrop_v2_coalition_attribution's sensor_player)
+ *   (N, 0)     shared by the batch [T, N]
+ *   (B*N, N)   per sample [T, B, N]
+ * Removing a player writes the baseline into its cells of the value half; the mask half, times and lengths never
+ * change.  Methods, formulas, fp64 sums, chunking, endpoint_logits and scratch (rd_coalition_attribution_scratch_bytes
+ * with the same n_players) are those of rd_raindrop_v2_coalition_attribution; both entry points run the same code.  The
+ * kept-player test of a cell costs O(1) whatever P: for Shapley one launch per chunk fills the chunk's keep table
+ * [cc, P] (in scratch) before the expansion reads it; ablation and the endpoints need no table. */
+int rd_raindrop_v2_cell_coalition_attribution(const rd_dims* dims, const rd_params* params, const float* src,
+                                              const float* statics, const float* times, const int64_t* lengths,
+                                              const float* node_scale, const float* baseline_src,
+                                              const float* baseline_statics, const int64_t* target,
+                                              const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                                              int32_t n_players, const int32_t* orders, int32_t m, int32_t method,
+                                              int32_t coalitions_per_chunk, void* scratch, float* attr,
+                                              float* endpoint_logits, void* stream);
 
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */

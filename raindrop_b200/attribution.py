@@ -4,17 +4,25 @@ IG_density_scores_<dataset>.npy):
 
 * integrated_gradients (rd_raindrop_v2_integrated_gradients): per input value, along the straight path from a baseline;
 * shapley_value_sampling and feature_ablation (rd_raindrop_v2_coalition_attribution): per sensor (group), of REMOVING
-  it -- replacing its value columns by the baseline, as the experiment does -- with the static vector one more player.
+  it -- replacing its value columns by the baseline, as the experiment does -- with the static vector one more player;
+* the same two with feature_mask (rd_raindrop_v2_cell_coalition_attribution): per player of a map of the value cells
+  (t, b, n), e.g. (sensor, time window) players from time_window_mask -- "what does removing heart rate in hours 12-18
+  do to this prediction?".  Removing a player writes the baseline into its cells of the value half; cells with id -1
+  belong to no player and keep x.
 
     attr_src, attr_static = integrated_gradients(model.eval(), src, static, times, lengths, target=y)
     ranking = sensor_ranking(sensor_importance(attr_src, model.d_inp), names)
     phi, phi_static = shapley_value_sampling(model.eval(), src, static, times, lengths, target=y)
     ranking = sensor_ranking(phi.abs().mean(dim=0), names)
     idx = data.removal_indices(B, model.d_inp, 0.5, level="set", density_scores=ranking[:, 0])
+    mask, n_win = time_window_mask(times, 6.0, sensor_groups=model.d_inp)       # 6 units of `times` per window
+    phi, phi_static = shapley_value_sampling(model.eval(), src, static, times, lengths, target=y, feature_mask=mask)
+    per_cell = phi.view(-1, n_win, model.d_inp)                                  # [B, window, sensor]
 
 Argument names follow Captum's IntegratedGradients, ShapleyValueSampling and FeatureAblation.
 """
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -170,10 +178,11 @@ class _Call:
             RF._set_field(self.params, path, t.data_ptr())
 
     def scratch(self, name, key, nbytes):
-        """fp32 scratch of `nbytes`, one buffer per plan and entry point: a new key replaces the old one."""
+        """fp32 scratch of at least `nbytes`, one buffer per plan and entry point: a new key, or a call that needs more
+        bytes than the buffer holds, replaces the old one."""
         plan = self.plan
         cached = plan.__dict__.get(name)
-        if cached is None or cached[0] != key:
+        if cached is None or cached[0] != key or cached[1].numel() * 4 < nbytes:
             plan.__dict__[name] = None
             cached = plan.__dict__[name] = (key, torch.empty(nbytes // 4, device=self.device, dtype=torch.float32))
         return cached[1]
@@ -299,10 +308,116 @@ def _device_int32(plan, kind, arr, device):
     return got
 
 
+def _device_cells(plan, arr, device):
+    """Device int32 copy of a host feature mask, cached per plan in ONE entry that a mask of other content replaces:
+    repeated calls with the same mask, and a CUDA-graph capture after an eager call with it, copy nothing, while a loop
+    over batches with per-sample host masks keeps a single mask on the device.  A copy read by a call under CUDA-graph
+    capture is also held for the plan's lifetime (plan._coal_cells_captured), so replays stay valid after later calls
+    replace the entry."""
+    key = (arr.shape, arr.tobytes(), device.index)
+    cached = plan.__dict__.get("_coal_cells")
+    if cached is None or cached[0] != key:
+        plan.__dict__["_coal_cells"] = None
+        cached = plan.__dict__["_coal_cells"] = (key, torch.tensor(arr, dtype=torch.int32, device=device))
+    if device.type == "cuda" and torch.cuda.is_current_stream_capturing():
+        held = plan.__dict__.setdefault("_coal_cells_captured", [])
+        if not any(t is cached[1] for t in held):
+            held.append(cached[1])
+    return cached[1]
+
+
+def _check_feature_mask(feature_mask, T, B, N):
+    """The integer tensor feature_mask, [T, N] or [T, B, N] with ids >= -1, on the device it was given on, and
+    G = max id + 1 >= 1 (one sync for a device tensor)."""
+    m = torch.as_tensor(feature_mask)
+    if m.is_floating_point() or m.is_complex() or m.dtype == torch.bool:
+        raise ValueError("feature_mask must hold integer player ids")
+    if tuple(m.shape) not in ((T, N), (T, B, N)):
+        raise ValueError("feature_mask must have shape [max_len=%d, d_inp=%d] or [max_len=%d, B=%d, d_inp=%d], got %s"
+                         % (T, N, T, B, N, tuple(m.shape)))
+    lo, hi = torch.stack(torch.aminmax(m)).tolist()
+    if lo < -1:
+        raise ValueError("feature_mask ids must be >= -1 (-1: the cell belongs to no player), got %d" % lo)
+    if hi < 0:
+        raise ValueError("feature_mask names no player: every id is -1")
+    if hi >= 1 << 30:
+        raise ValueError("feature_mask ids must be < 2^30, got %d" % hi)
+    return m, hi + 1
+
+
+def _cell_players(plan, mask, device):
+    """(device int32 map, stride_t, stride_b) for rd_raindrop_v2_cell_coalition_attribution.  A host mask goes through
+    the plan's one-entry cache (_device_cells); a device mask is used in place when it is int32 with unit stride along
+    the sensors, and its strides select the layout (an expanded [T, B, N] view works)."""
+    if mask.device.type == "cpu":
+        mask = _device_cells(plan, np.ascontiguousarray(mask.numpy().astype(np.int32)), device)
+    else:
+        mask = mask.to(device=device, dtype=torch.int32)
+        if mask.stride(-1) != 1:
+            mask = mask.contiguous()
+    if mask.dim() == 2:
+        return mask, mask.stride(0), 0
+    return mask, mask.stride(0), mask.stride(1)
+
+
+def time_window_mask(times, window, n_windows=None, sensor_groups=None):
+    """(mask [T, B, N] int32 on the device of `times`, n_windows): a per-sample feature_mask of (sensor group, time
+    window) players for shapley_value_sampling and feature_ablation.  The value cell (t, b, n) belongs to player
+    w * G + g, g = sensor_groups[n], with the window of its row
+
+        w = min(floor(times[t, b] / window), n_windows - 1)        (window in the units of `times`, > 0)
+
+    so players 0..G-1 are the groups in window 0, G..2G-1 in window 1, and so on: phi.view(B, n_windows, G).
+    Padding rows -- rows t > 0 with times[t, b] == 0, the data pipeline's padding -- get -1 (no player): the ob-prop
+    GEMM mixes all T steps of a sensor, so a nonzero baseline written into padding rows would change F.  Row 0 is always
+    a real row, also when the first timestamp is 0 (first_time_zero data).  A window with no row in a sample is a player
+    with no cell there: it gets exactly 0.
+
+    times:          [T, B] (src's timestamps).
+    n_windows:      default max(1, ceil(max(times) / window)), one sync; give it to share one layout over batches.
+    sensor_groups:  required: d_inp (an int, one group per sensor) or an integer array [d_inp] of groups 0..G-1, each
+                    non-empty, as for sensor_groups of feature_ablation."""
+    tm = torch.as_tensor(times)
+    if tm.dim() != 2 or tm.is_complex():
+        raise ValueError("times must be a real [max_len, B] tensor, got shape %s" % (tuple(tm.shape),))
+    window = float(window)
+    if not (window > 0 and math.isfinite(window)):
+        raise ValueError("window must be a positive finite number, got %r" % window)
+    if sensor_groups is None:
+        raise ValueError("time_window_mask needs sensor_groups: d_inp (one group per sensor) or a group array [d_inp]")
+    if isinstance(sensor_groups, (int, np.integer)):
+        if int(sensor_groups) < 1:
+            raise ValueError("sensor_groups as a sensor count must be >= 1, got %d" % int(sensor_groups))
+        groups, G = np.arange(int(sensor_groups), dtype=np.int64), int(sensor_groups)
+    else:
+        g = torch.as_tensor(sensor_groups)
+        if g.dim() != 1:
+            raise ValueError("sensor_groups must be an int or a 1-D array [d_inp], got shape %s" % (tuple(g.shape),))
+        groups, G = _check_groups(g, g.shape[0])
+    t = tm.detach().double()
+    if n_windows is None:
+        n_windows = max(1, math.ceil(float(t.max()) / window)) if t.numel() else 1
+    n_windows = int(n_windows)
+    if n_windows < 1:
+        raise ValueError("n_windows must be >= 1, got %d" % n_windows)
+    w = torch.floor(t / window).clamp_(0, n_windows - 1).long()                              # [T, B]
+    row = torch.arange(t.shape[0], device=t.device)[:, None]
+    pad = (row > 0) & (t == 0)
+    ids = w[:, :, None] * G + torch.as_tensor(groups, device=t.device)[None, None, :]       # [T, B, N]
+    return torch.where(pad[:, :, None], -1, ids).to(torch.int32).contiguous(), n_windows
+
+
 def _coalition_attribution(fn, method, model, src, static, times, lengths, target, baselines, sensor_groups,
-                           orders_host, internal_batch_size):
-    """attr [B, P] of rd_raindrop_v2_coalition_attribution, the endpoint logits [2, B, ncls], the target and G."""
-    groups, G = _check_groups(sensor_groups, model._plan.N)
+                           orders_host, internal_batch_size, feature_mask=None):
+    """attr [B, P] of rd_raindrop_v2_coalition_attribution (sensor groups) or rd_raindrop_v2_cell_coalition_attribution
+    (feature_mask), the endpoint logits [2, B, ncls], the target and G."""
+    if feature_mask is None:
+        groups, G = _check_groups(sensor_groups, model._plan.N)
+    else:
+        if sensor_groups is not None:
+            raise ValueError("give sensor_groups or feature_mask, not both")
+        cells, G = _check_feature_mask(feature_mask, model._plan.T, src.shape[1], model._plan.N)
+        fn = "rd_raindrop_v2_cell_coalition_attribution"
     P = G + (1 if model.static else 0)
     orders = orders_host(P) if method == RD_ATTR_SHAPLEY else None
     cl = _Call(model, src, static, times, lengths, target, baselines)
@@ -313,7 +428,10 @@ def _coalition_attribution(fn, method, model, src, static, times, lengths, targe
         orders_d = _device_int32(plan, "orders", orders, device)
     else:
         m, n_coal, orders_d = 0, P, None
-    player = _device_int32(plan, "players", groups, device)
+    if feature_mask is None:
+        player = _device_int32(plan, "players", groups, device)
+    else:
+        player, stride_t, stride_b = _cell_players(plan, cells, device)
 
     dims = plan.dims(B, False)
     if internal_batch_size is None:
@@ -324,15 +442,20 @@ def _coalition_attribution(fn, method, model, src, static, times, lengths, targe
     nbytes = lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), P, cc)
     if nbytes == 0:
         L.check(-2, "rd_coalition_attribution_scratch_bytes")
-    scratch = cl.scratch("_coal_attr_scratch", (B, P, cc, dims.obprop_mode, device.index), nbytes)
+    # the scratch layout follows (B, P, cc) on every call, so a buffer that is large enough is reused: with feature_mask
+    # P changes whenever a batch does not reach the last time window, and that must not reallocate the scratch
+    scratch = cl.scratch("_coal_attr_scratch", device.index, nbytes)
 
     attr = torch.empty(B, P, device=device, dtype=torch.float32)
     ends = torch.empty(2, B, plan.n_classes, device=device, dtype=torch.float32)
-    L.check(lib.rd_raindrop_v2_coalition_attribution(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st),
-                                                     cl.tm.data_ptr(), cl.ln.data_ptr(), plan.node_scale.data_ptr(),
-                                                     cl.x0.data_ptr(), L.ptr(cl.st0), L.ptr(cl.tgt), player.data_ptr(), P,
-                                                     L.ptr(orders_d), m, method, cc, scratch.data_ptr(), attr.data_ptr(),
-                                                     ends.data_ptr(), L.stream_ptr(device)), fn)
+    head = (C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st), cl.tm.data_ptr(), cl.ln.data_ptr(),
+            plan.node_scale.data_ptr(), cl.x0.data_ptr(), L.ptr(cl.st0), L.ptr(cl.tgt), player.data_ptr())
+    tail = (P, L.ptr(orders_d), m, method, cc, scratch.data_ptr(), attr.data_ptr(), ends.data_ptr(), L.stream_ptr(device))
+    if feature_mask is None:
+        rc = lib.rd_raindrop_v2_coalition_attribution(*head, *tail)
+    else:
+        rc = lib.rd_raindrop_v2_cell_coalition_attribution(*head, stride_t, stride_b, *tail)
+    L.check(rc, fn)
     return attr, ends, cl.tgt, G
 
 
@@ -341,7 +464,7 @@ def _split(attr, G):
 
 
 def feature_ablation(model, src, static, times, lengths, target=None, baselines=None, sensor_groups=None,
-                     internal_batch_size=None):
+                     internal_batch_size=None, feature_mask=None):
     """Leave-one-out ablation of F = logits[b, target[b]] of an eval-mode Raindrop_v2 over sensor groups and the static
     vector:
 
@@ -353,6 +476,16 @@ def feature_ablation(model, src, static, times, lengths, target=None, baselines=
     the static player replaces static[b] by its baseline.  The mask half, `times` and `lengths` never change.
     Returns (attr_sensors [B, G], attr_static [B] or None), fp32 on the model's device.
 
+    feature_mask: instead of sensor_groups (giving both is a ValueError), an integer map of the value cells (Captum's
+                name): [T, N] shared by the batch or [T, B, N] per sample (time_window_mask builds (sensor, time window)
+                players).  Ids 0..G-1, G = max id + 1, are players, removing one writes the baseline into its cells of
+                the value half; -1 marks a cell of no player, which keeps x; the static vector is player G as before.
+                An id may have no cell (a time window can be empty in a batch): that player gets exactly 0.  The
+                result is (attr_players [B, G], attr_static [B] or None).  A host mask is kept on the device in a
+                one-entry cache per model that a mask of other content replaces: repeated calls with the same mask and
+                a CUDA-graph capture after an eager call with it copy nothing, and a loop over per-sample host masks
+                holds one mask on the device.  A device mask costs one sync for its range check (so it cannot be captured)
+                and is read in place.
     target, baselines: as for integrated_gradients.  A static baseline equal to `static` holds the statics fixed (their
                 attribution is then exactly 0).
     internal_batch_size: (sample, coalition) rows per chunk.  Default: the largest chunk whose scratch fits in 1 GiB.
@@ -363,19 +496,21 @@ def feature_ablation(model, src, static, times, lengths, target=None, baselines=
     model in training mode or bad arguments, TypeError for another model class and RaindropB200Error without CUDA."""
     _check_call("feature_ablation", model, src, static, baselines, internal_batch_size)
     attr, _, _, G = _coalition_attribution("rd_raindrop_v2_coalition_attribution", RD_ATTR_ABLATION, model, src, static,
-                                           times, lengths, target, baselines, sensor_groups, None, internal_batch_size)
+                                           times, lengths, target, baselines, sensor_groups, None, internal_batch_size,
+                                           feature_mask)
     return _split(attr, G)
 
 
 def shapley_value_sampling(model, src, static, times, lengths, target=None, baselines=None, sensor_groups=None,
                            n_samples=25, seed=0, permutations=None, internal_batch_size=None,
-                           return_convergence_delta=False):
+                           return_convergence_delta=False, feature_mask=None):
     """Shapley values, by permutation sampling, of the game v(S) = F(x with the players outside S removed),
     F = logits[b, target[b]] of an eval-mode Raindrop_v2; players and removal as for feature_ablation:
 
         phi[b, g] = (1/m) sum_p [F(S_pg + {g}) - F(S_pg)],  S_pg = the players ahead of g in permutation p
 
-    The m permutations of the P players (the static player has index G) are shared by the batch, as in Captum: drawn
+    Players are sensor groups or, with feature_mask, the players of a map of the value cells (see feature_ablation);
+    the m permutations of the P players (the static player has index G) are shared by the batch, as in Captum: drawn
     by sample_permutations(P, n_samples, seed), or given as `permutations` [m, P] (all P! of them give the exact
     Shapley values).  Efficiency: sum_g phi[b, g] (+ the static player's) = F(x) - F(x') up to rounding.
 
@@ -395,7 +530,7 @@ def shapley_value_sampling(model, src, static, times, lengths, target=None, base
             return _check_permutations(permutations, P)
     attr, ends, tgt, G = _coalition_attribution("rd_raindrop_v2_coalition_attribution", RD_ATTR_SHAPLEY, model, src,
                                                 static, times, lengths, target, baselines, sensor_groups, orders_host,
-                                                internal_batch_size)
+                                                internal_batch_size, feature_mask)
     out = _split(attr, G)
     if not return_convergence_delta:
         return out

@@ -465,30 +465,50 @@ __global__ void ig_accum_kernel(const __grid_constant__ IgAccumArgs a) {
   else a.acc_static[o] = acc;
 }
 
-// ---- coalition attribution: Shapley-value sampling, leave-one-out ablation (rd_raindrop_v2_coalition_attribution) --
+// ---- coalition attribution: Shapley-value sampling, leave-one-out ablation (rd_raindrop_v2_coalition_attribution,
+// rd_raindrop_v2_cell_coalition_attribution) --------------------------------------------------------------------------
 // Coalition c keeps the players it names and replaces every other player by its baseline.
 //   Shapley (method 0): c = p*(P-1) + k-1, k = 1..P-1, keeps the first k players of permutation p (orders[p, :k])
 //   ablation (method 1): c = g, keeps every player but g
-__device__ __forceinline__ bool coalition_keeps(const int32_t* __restrict__ orders, int P, int method, int c, int g) {
-  if (method == RD_ATTR_ABLATION) return c != g;
-  const int p = c / (P - 1), k = c - p * (P - 1) + 1;
-  const int32_t* o = orders + (long long)p * P;
-  for (int i = 0; i < k; ++i)
-    if (__ldg(o + i) == g) return true;
-  return false;
+// The test is O(1) per value cell whatever P: ablation and the endpoint rows (COALITION_ENDPOINTS, nc = 2: x' keeps no
+// player, x every player) compute it; Shapley reads keep[ci, g] (uint8 [nc, P]), filled per chunk by
+// coalition_keep_kernel, one thread per (ci, position i): the player at position i of permutation p is kept when i < k
+// (each row of orders is a permutation, so every keep[ci, :] entry is written exactly once; an id outside [0, P) in a
+// row that is not one writes nothing).
+struct CoalitionKeepArgs {
+  const int32_t* orders; uint8_t* keep;
+  int P, c0, nc;
+};
+__global__ void coalition_keep_kernel(const __grid_constant__ CoalitionKeepArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= (long long)a.nc * a.P) return;
+  const int ci = (int)(o / a.P), i = (int)(o - (long long)ci * a.P), c = a.c0 + ci;
+  const int p = c / (a.P - 1), k = c - p * (a.P - 1) + 1;
+  const int g = __ldg(a.orders + (long long)p * a.P + i);
+  if ((unsigned)g < (unsigned)a.P) a.keep[(long long)ci * a.P + g] = i < k;      // a bad orders row cannot write outside
 }
 
-// Inputs of one chunk of nc coalitions c0 .. c0+nc-1 on B*nc rows, coalition-major (row j = ci*B + b), in one launch:
-//   src_e[t, j, n] = keep(player[n]) ? src[t, b, n] : src0[t, b, n] (value half), src[t, b, n] (mask half, copied)
+// Inputs of one chunk of nc coalitions c0 .. c0+nc-1 on B*nc rows, coalition-major (row j = ci*B + b), in one launch,
+// with g = player[t*stride_t + b*stride_b + n] the player of value cell (t, b, n) (strides 0, 0: one player per sensor):
+//   src_e[t, j, n] = (g outside [0, G) or kept(ci, g)) ? src[t, b, n] : src0[t, b, n] (value half),
+//                    src[t, b, n] (mask half, copied)
 //   times_e[t, j] = times[t, b];  lengths_e[j] = lengths[b]
-//   statics_e[j, :] = keep(P-1) ? statics[b, :] : statics0[b, :]  (the static player is the last one)
+//   statics_e[j, :] = kept(ci, P-1) ? statics[b, :] : statics0[b, :]  (the static player is the last one, P = G + 1)
 struct CoalitionExpandArgs {
   const float* src; const float* src0; const float* statics; const float* statics0; const float* times;
-  const int64_t* lengths; const int32_t* player; const int32_t* orders;
+  const int64_t* lengths; const int32_t* player; const uint8_t* keep;
   float* src_e; float* statics_e; float* times_e; int64_t* lengths_e;
-  int P, method, c0, nc, B, T, N, ds;
+  long long stride_t, stride_b;
+  int P, G, method, c0, nc, B, T, N, ds;
   long long n_src, n_tok, n_stat, n_rows;
 };
+__device__ __forceinline__ bool coalition_kept(const CoalitionExpandArgs& a, int ci, int g) {
+  if (a.method == RD_ATTR_SHAPLEY) return __ldg(a.keep + (long long)ci * a.P + g);
+  if (a.method == RD_ATTR_ABLATION) return a.c0 + ci != g;
+  return ci != 0;                                             // COALITION_ENDPOINTS
+}
 __global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandArgs a) {
   pdl_launch_dependents();
   pdl_wait();
@@ -501,7 +521,11 @@ __global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandA
     const long long t = tj / rows;
     const int j = (int)(tj - t * rows), ci = j / a.B, b = j - ci * a.B;
     const long long i = (t * a.B + b) * w + c;
-    const bool x = c >= a.N || coalition_keeps(a.orders, a.P, a.method, a.c0 + ci, __ldg(a.player + c));
+    bool x = true;
+    if (c < a.N) {
+      const int g = __ldg(a.player + t * a.stride_t + b * a.stride_b + c);
+      x = (unsigned)g >= (unsigned)a.G || coalition_kept(a, ci, g);
+    }
     a.src_e[o] = __ldg((x ? a.src : a.src0) + i);
     return;
   }
@@ -516,7 +540,7 @@ __global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandA
   if (o < a.n_stat) {
     const long long j = o / a.ds;
     const int kk = (int)(o - j * a.ds), ci = (int)(j / a.B), b = (int)(j - (long long)ci * a.B);
-    const bool x = coalition_keeps(a.orders, a.P, a.method, a.c0 + ci, a.P - 1);
+    const bool x = coalition_kept(a, ci, a.P - 1);
     a.statics_e[o] = __ldg((x ? a.statics : a.statics0) + (long long)b * a.ds + kk);
     return;
   }
@@ -1212,14 +1236,21 @@ int ig_accumulate(const float* src, const float* src0, const float* alphas, cons
 }
 
 int coalition_expand(const float* src, const float* src0, const float* statics, const float* statics0, const float* times,
-                     const int64_t* lengths, const int32_t* player, const int32_t* orders, int P, int method, int c0, int nc,
-                     int B, int T, int N, int ds, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e,
-                     cudaStream_t st) {
+                     const int64_t* lengths, const int32_t* player, int64_t stride_t, int64_t stride_b, const int32_t* orders,
+                     int P, int G, int method, int c0, int nc, int B, int T, int N, int ds, uint8_t* keep, float* src_e,
+                     float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st) {
+  if (method == RD_ATTR_SHAPLEY) {
+    CoalitionKeepArgs k;
+    k.orders = orders; k.keep = keep; k.P = P; k.c0 = c0; k.nc = nc;
+    launch_pdl(coalition_keep_kernel, dim3(blocks_for((int64_t)nc * P)), dim3(TPB), 0, st, k);
+    RD_CHECK_LAUNCH("coalition_keep_kernel");
+  }
   CoalitionExpandArgs a;
   a.src = src; a.src0 = src0; a.statics = statics; a.statics0 = statics0; a.times = times; a.lengths = lengths;
-  a.player = player; a.orders = orders;
+  a.player = player; a.keep = keep;
   a.src_e = src_e; a.statics_e = statics_e; a.times_e = times_e; a.lengths_e = lengths_e;
-  a.P = P; a.method = method; a.c0 = c0; a.nc = nc; a.B = B; a.T = T; a.N = N; a.ds = ds;
+  a.stride_t = stride_t; a.stride_b = stride_b;
+  a.P = P; a.G = G; a.method = method; a.c0 = c0; a.nc = nc; a.B = B; a.T = T; a.N = N; a.ds = ds;
   const int64_t rows = (int64_t)B * nc;
   a.n_src = (int64_t)T * rows * 2 * N; a.n_tok = (int64_t)T * rows; a.n_stat = ds > 0 ? rows * ds : 0; a.n_rows = rows;
   launch_pdl(coalition_expand_kernel, dim3(blocks_for(a.n_src + a.n_tok + a.n_stat + a.n_rows)), dim3(TPB), 0, st, a);

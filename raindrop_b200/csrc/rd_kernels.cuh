@@ -62,15 +62,19 @@ int ig_accumulate(const float* src, const float* src0, const float* alphas, cons
                   const float* statics0, const float* dfeat, int Df, int feat_col0, const float* W_emb, int emb, int ds,
                   float* acc_static, float* attr_static, int first, int last, cudaStream_t st);
 
-// Coalition attribution over P players (sensor groups player[n] in [0, P-1), the static player P-1 when ds > 0),
-// chunks of nc coalitions c0 .. c0+nc-1 on B*nc rows, coalition-major (j = ci*B + b); method RD_ATTR_SHAPLEY: coalition
-// c = p*(P-1) + k-1 keeps orders[p, :k], RD_ATTR_ABLATION: coalition c keeps every player but c.
-// coalition_expand: src_e [T, B*nc, 2N] (value half of a kept player from src, else from src0; mask half copied),
+// Coalition attribution over P players (value cell (t, b, n) belongs to player[t*stride_t + b*stride_b + n], ids in
+// [0, G) are players, any other id none; the static player G = P-1 when ds > 0), chunks of nc coalitions c0 .. c0+nc-1
+// on B*nc rows, coalition-major (j = ci*B + b); method RD_ATTR_SHAPLEY: coalition c = p*(P-1) + k-1 keeps orders[p, :k],
+// RD_ATTR_ABLATION: coalition c keeps every player but c; COALITION_ENDPOINTS (nc = 2): the rows of x' (no player kept:
+// the cells of no player keep x) and of x.
+// coalition_expand: for Shapley one launch fills the chunk's keep table keep [nc, P] (uint8); then one launch writes
+// src_e [T, B*nc, 2N] (value cell of a kept player or of no player from src, else from src0; mask half copied),
 // statics_e, times_e, lengths_e.
+#define COALITION_ENDPOINTS 2
 int coalition_expand(const float* src, const float* src0, const float* statics, const float* statics0, const float* times,
-                     const int64_t* lengths, const int32_t* player, const int32_t* orders, int P, int method, int c0, int nc,
-                     int B, int T, int N, int ds, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e,
-                     cudaStream_t st);
+                     const int64_t* lengths, const int32_t* player, int64_t stride_t, int64_t stride_b, const int32_t* orders,
+                     int P, int G, int method, int c0, int nc, int B, int T, int N, int ds, uint8_t* keep, float* src_e,
+                     float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
 // coalition_accumulate: adds the chunk's F = logits_c [B*nc, ncls] at target[b] (nullptr: argmax of ends[1]) into the
 // fp64 running sums acc [B, P]; first: start from the endpoints ends [2, B, ncls] (at x', at x); last: write attr [B, P].
 int coalition_accumulate(const float* logits_c, const float* ends, const int64_t* target, const int32_t* orders, int P,

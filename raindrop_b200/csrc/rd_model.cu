@@ -209,10 +209,11 @@ int ig_layout(const rd_dims* dims, int mc, IgcLayout* l) {
 }
 
 // ---- coalition attribution (Shapley-value sampling, ablation) -------------------------------------------------------
-// Scratch of rd_raindrop_v2_coalition_attribution: the eval forward workspace and the expanded inputs of max(B*cc, 2B)
-// rows (chunks of cc coalitions and the endpoint forward), the chunk's logits and the fp64 running sums [B, P].  The
-// ob-prop mode is pinned from B*cc rows by ig_dims, as for integrated gradients.
-struct CoalLayout { int64_t ws, src, statics, times, lengths, logits, acc, total; };
+// Scratch of rd_raindrop_v2_coalition_attribution and rd_raindrop_v2_cell_coalition_attribution: the eval forward
+// workspace and the expanded inputs of max(B*cc, 2B) rows (chunks of cc coalitions and the endpoint forward), the
+// chunk's logits, the fp64 running sums [B, P] and the chunk's keep table [cc, P] (uint8, Shapley).  The ob-prop mode is pinned
+// from B*cc rows by ig_dims, as for integrated gradients.
+struct CoalLayout { int64_t ws, src, statics, times, lengths, logits, acc, keep, total; };
 int coalition_layout(const rd_dims* dims, int n_players, int cc, CoalLayout* l) {
   if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("coalitions_per_chunk = %d out of range", cc); return -2; }
   if (n_players < 1) { set_error("n_players = %d must be >= 1", n_players); return -2; }
@@ -228,6 +229,7 @@ int coalition_layout(const rd_dims* dims, int n_players, int cc, CoalLayout* l) 
   l->lengths = a.take(2LL * Bx);
   l->logits = a.take((int64_t)Bc * sx.ncls);
   l->acc = a.take(2LL * dims->B * n_players);
+  l->keep = a.take(ceil_div((int64_t)cc * n_players, 4));
   l->total = a.off;
   return 0;
 }
@@ -945,33 +947,38 @@ size_t rd_coalition_attribution_scratch_bytes(const rd_dims* dims, int32_t n_pla
   return (size_t)l.total * sizeof(float);
 }
 
-int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
-                                         const float* times, const int64_t* lengths, const float* node_scale,
-                                         const float* baseline_src, const float* baseline_statics, const int64_t* target,
-                                         const int32_t* sensor_player, int32_t n_players, const int32_t* orders, int32_t m,
-                                         int32_t method, int32_t coalitions_per_chunk, void* scratch, float* attr,
-                                         float* endpoint_logits, void* stream) {
-  if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !sensor_player || !scratch || !attr ||
+// The one implementation behind both coalition entry points: `fn` names the caller in error messages.
+static int coalition_attribution(const char* fn, const rd_dims* dims, const rd_params* params, const float* src,
+                                 const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
+                                 const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                 const int32_t* cell_player, int64_t stride_t, int64_t stride_b, int32_t n_players,
+                                 const int32_t* orders, int32_t m, int32_t method, int32_t coalitions_per_chunk, void* scratch,
+                                 float* attr, float* endpoint_logits, void* stream) {
+  if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !cell_player || !scratch || !attr ||
       !endpoint_logits || !params->R_u || !params->ob1_value_weight) {
-    set_error("rd_raindrop_v2_coalition_attribution: NULL argument");
+    set_error("%s: NULL argument", fn);
     return -2;
   }
   if (method != RD_ATTR_SHAPLEY && method != RD_ATTR_ABLATION) {
-    set_error("rd_raindrop_v2_coalition_attribution: method must be RD_ATTR_SHAPLEY or RD_ATTR_ABLATION, got %d", method);
+    set_error("%s: method must be RD_ATTR_SHAPLEY or RD_ATTR_ABLATION, got %d", fn, method);
     return -2;
   }
-  if (dims->training) { set_error("rd_raindrop_v2_coalition_attribution: runs eval arithmetic, dims->training must be 0"); return -2; }
+  if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
   Shape s0;
   RD_TRY(make_shape(dims, &s0));
   if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
   if (s0.ds > 0 && (!statics || !baseline_statics)) {
-    set_error("rd_raindrop_v2_coalition_attribution: d_static > 0 needs statics and baseline_statics");
+    set_error("%s: d_static > 0 needs statics and baseline_statics", fn);
     return -2;
   }
   const int P = n_players, G = P - (s0.ds > 0 ? 1 : 0);
-  if (G < 1 || G > s0.N) { set_error("rd_raindrop_v2_coalition_attribution: n_players = %d gives %d sensor groups for N = %d", P, G, s0.N); return -2; }
+  if (G < 1) { set_error("%s: n_players = %d gives %d players of the value cells, need >= 1", fn, P, G); return -2; }
+  if (stride_t < 0 || stride_b < 0) {
+    set_error("%s: player strides must be >= 0, got (%lld, %lld)", fn, (long long)stride_t, (long long)stride_b);
+    return -2;
+  }
   if (method == RD_ATTR_SHAPLEY && (!orders || m < 1 || (int64_t)m * (P - 1) > (1LL << 30))) {
-    set_error("rd_raindrop_v2_coalition_attribution: Shapley sampling needs orders and 1 <= m, m*(P-1) <= 2^30 (m = %d)", m);
+    set_error("%s: Shapley sampling needs orders and 1 <= m, m*(P-1) <= 2^30 (m = %d)", fn, m);
     return -2;
   }
   CoalLayout l;
@@ -984,11 +991,14 @@ int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* p
   float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
   int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
   double* acc = reinterpret_cast<double*>(S + l.acc);
+  uint8_t* keep = reinterpret_cast<uint8_t*>(S + l.keep);
 
-  // 1. the endpoints: one forward on 2B rows (baseline rows, then input rows) -> endpoint_logits [2, B, ncls]
+  // 1. the endpoints: one forward on 2B rows (x' rows: every player removed, cells of no player keep x; then x rows)
+  //    -> endpoint_logits [2, B, ncls]
   const rd_dims de = ig_dims(dims, 2 * B, cc);
-  RD_TRY(ig_expand(src, baseline_src, statics, baseline_statics, times, lengths, nullptr, 2, B, s0.T, s0.N, s0.ds, s0.ncls,
-                   nullptr, nullptr, src_e, stat_e, times_e, len_e, nullptr, st));
+  RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
+                          orders, P, G, COALITION_ENDPOINTS, 0, 2, B, s0.T, s0.N, s0.ds, keep, src_e, stat_e, times_e, len_e,
+                          st));
   RD_TRY(raindrop_fwd(&de, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, endpoint_logits, nullptr, nullptr,
                       nullptr, 0, st));
   // 2. chunks of cc coalitions (the last one possibly shorter, same scratch, same arithmetic mode); with no coalition
@@ -998,8 +1008,8 @@ int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* p
     const int nc = n_coal - c0 < cc ? n_coal - c0 : cc;
     if (nc > 0) {
       const rd_dims dc = ig_dims(dims, B * nc, cc);
-      RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, sensor_player, orders, P, method,
-                              c0, nc, B, s0.T, s0.N, s0.ds, src_e, stat_e, times_e, len_e, st));
+      RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
+                              orders, P, G, method, c0, nc, B, s0.T, s0.N, s0.ds, keep, src_e, stat_e, times_e, len_e, st));
       RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, logits, nullptr, nullptr,
                           nullptr, 0, st));
     }
@@ -1008,6 +1018,37 @@ int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* p
     c0 += cc;
   } while (c0 < n_coal);
   return 0;
+}
+
+int rd_raindrop_v2_coalition_attribution(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                         const float* times, const int64_t* lengths, const float* node_scale,
+                                         const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                         const int32_t* sensor_player, int32_t n_players, const int32_t* orders, int32_t m,
+                                         int32_t method, int32_t coalitions_per_chunk, void* scratch, float* attr,
+                                         float* endpoint_logits, void* stream) {
+  const char* fn = "rd_raindrop_v2_coalition_attribution";
+  if (!dims || !sensor_player) { set_error("%s: NULL argument", fn); return -2; }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  const int P = n_players, G = P - (s0.ds > 0 ? 1 : 0);
+  if (G < 1 || G > s0.N) { set_error("%s: n_players = %d gives %d sensor groups for N = %d", fn, P, G, s0.N); return -2; }
+  return coalition_attribution(fn, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                               target, sensor_player, 0, 0, n_players, orders, m, method, coalitions_per_chunk, scratch, attr,
+                               endpoint_logits, stream);
+}
+
+int rd_raindrop_v2_cell_coalition_attribution(const rd_dims* dims, const rd_params* params, const float* src,
+                                              const float* statics, const float* times, const int64_t* lengths,
+                                              const float* node_scale, const float* baseline_src,
+                                              const float* baseline_statics, const int64_t* target,
+                                              const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                                              int32_t n_players, const int32_t* orders, int32_t m, int32_t method,
+                                              int32_t coalitions_per_chunk, void* scratch, float* attr,
+                                              float* endpoint_logits, void* stream) {
+  return coalition_attribution("rd_raindrop_v2_cell_coalition_attribution", dims, params, src, statics, times, lengths,
+                               node_scale, baseline_src, baseline_statics, target, cell_player, player_stride_t,
+                               player_stride_b, n_players, orders, m, method, coalitions_per_chunk, scratch, attr,
+                               endpoint_logits, stream);
 }
 
 int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,

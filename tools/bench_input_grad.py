@@ -17,7 +17,9 @@ the same session, alternating call by call; samples/s counts the B samples of on
 --ablation or --shapley-samples M [--coalition-rows R] compare, the same way, one raindrop_b200.attribution
 feature_ablation / shapley_value_sampling call (one player per sensor plus the static vector, zero baselines, target =
 the labels, internal_batch_size R) with the hand-written loop of B-row module forwards over the same coalitions
-(P + 1 forwards for ablation; m*(P-1) + 2 for M permutations) summing F in fp64 tensors.
+(P + 1 forwards for ablation; m*(P-1) + 2 for M permutations) summing F in fp64 tensors.  With --window W the players
+are (sensor, time window) cells instead: feature_mask = time_window_mask(times, W, sensor_groups=d_inp) (W in the units
+of `times`; padding rows belong to no player), and the loop removes the same cells.
 """
 import argparse
 import json
@@ -105,10 +107,15 @@ def ig_compare(args, lib, cfg_name, model, b, device):
 def coalition_compare(args, lib, cfg_name, model, b, device):
     """Alternating timing of one feature_ablation / shapley_value_sampling call and of the loop of module forwards."""
     from raindrop_b200.attribution import (_default_coalitions_per_chunk, feature_ablation, sample_permutations,
-                                           shapley_value_sampling)
+                                           shapley_value_sampling, time_window_mask)
     src, static, times, lengths, y = b["src"], b["static"], b["times"], b["lengths"], b["y"]
     B, N = src.shape[1], src.shape[2] // 2
-    P = N + (1 if static is not None else 0)
+    mask, G = None, N
+    if args.window:
+        mask, n_win = time_window_mask(times, args.window, sensor_groups=N)
+        G = n_win * N
+        cell_player = mask.long()                              # id -1 indexes the appended "kept" entry below
+    P = G + (1 if static is not None else 0)
     M = args.shapley_samples
     orders = sample_permutations(P, M, 0).tolist() if M else None
     n_coal = M * (P - 1) if M else P
@@ -116,14 +123,18 @@ def coalition_compare(args, lib, cfg_name, model, b, device):
     def batched():
         if M:
             shapley_value_sampling(model, src, static, times, lengths, target=y, n_samples=M, seed=0,
-                                   internal_batch_size=args.coalition_rows)
+                                   internal_batch_size=args.coalition_rows, feature_mask=mask)
         else:
-            feature_ablation(model, src, static, times, lengths, target=y, internal_batch_size=args.coalition_rows)
+            feature_ablation(model, src, static, times, lengths, target=y, internal_batch_size=args.coalition_rows,
+                             feature_mask=mask)
 
-    def F(keep):                  # keep: [P] bool device tensor; players = sensors, then the static vector
+    kept = torch.ones(1, dtype=torch.bool, device=device)
+
+    def F(keep):                  # keep: [P] bool device tensor; players = sensors or cells, then the static vector
         x = src.clone()
-        x[:, :, :N] = torch.where(keep[:N], src[:, :, :N], 0.0)
-        st = None if static is None else torch.where(keep[N], static, 0.0)
+        k = keep[:N] if mask is None else torch.cat([keep[:G], kept])[cell_player]
+        x[:, :, :N] = torch.where(k, src[:, :, :N], 0.0)
+        st = None if static is None else torch.where(keep[G], static, 0.0)
         logits, _, _ = model.forward(x, st, times, lengths)
         return logits.gather(1, y[:, None])[:, 0].double()
 
@@ -163,8 +174,10 @@ def coalition_compare(args, lib, cfg_name, model, b, device):
     cc = min(n_coal, max(1, args.coalition_rows // B)) if args.coalition_rows else \
         _default_coalitions_per_chunk(lib, model._plan.dims(B, False), P, n_coal)
     what = "Shapley-value sampling, %d permutations" % M if M else "leave-one-out ablation"
+    if args.window:
+        what += " over (sensor, %g-unit time window) players" % args.window
     res = {"metric": "%s, %d players, samples/s (%s-shape synthetic)" % (what, P, cfg_name), "batch": B,
-           "shapley_samples": M, "coalitions": n_coal, "coalition_rows": args.coalition_rows,
+           "players": P, "window": args.window, "shapley_samples": M, "coalitions": n_coal, "coalition_rows": args.coalition_rows,
            "coalitions_per_chunk": cc, "steps": args.steps, "card": card()}
     for tag, t, n in (("batched", sb, n_batched), ("loop", sl, n_loop)):
         res[tag] = {"samples_per_s": round(B / (t["median"] * 1e-3), 1), "ms_per_call": round(t["median"], 4),
@@ -187,7 +200,11 @@ def main():
     ap.add_argument("--coalition-rows", type=int, default=None,
                     help="internal_batch_size of the batched ablation / Shapley call ((sample, coalition) rows per "
                          "chunk; default: 1 GiB scratch)")
+    ap.add_argument("--window", type=float, default=0.0,
+                    help="with --ablation / --shapley-samples: (sensor, time window) players, windows of W units of times")
     args = ap.parse_args()
+    if args.window and not (args.ablation or args.shapley_samples > 0):
+        ap.error("--window needs --ablation or --shapley-samples")
     from raindrop_b200 import lib as L
     lib = L.load()
     device = torch.device("cuda", 0)

@@ -23,6 +23,11 @@ is not recorded, so this ranking is not claimed to reproduce them.
 experiment does; the static vector is held fixed): raindrop_b200.attribution.feature_ablation, or
 shapley_value_sampling with --shapley-samples permutations (seed --seed).  A sensor's score is the mean over samples of
 |attribution|; the file has the same [N, 2] layout.
+
+--window W with --method ablation / shapley attributes (sensor, time window) cells instead
+(raindrop_b200.attribution.time_window_mask, windows of W units of `times`, padding rows in no window) and writes
+<Method>_time_sensor_scores_<name>.npy: float64 [n_windows, N], the mean over samples of |attribution| per (window,
+sensor).  n_windows = max(1, ceil(max(times) / W)) over the whole data set, so every batch shares the layout.
 """
 import argparse
 import os
@@ -71,14 +76,18 @@ def main():
     ap.add_argument("--method", default="ig", choices=["ig", "ablation", "shapley"])
     ap.add_argument("--steps", type=int, default=50, help="--method ig: Gauss-Legendre nodes per attribution")
     ap.add_argument("--shapley-samples", type=int, default=25, help="--method shapley: permutations per batch")
+    ap.add_argument("--window", type=float, default=0.0,
+                    help="--method ablation / shapley: (sensor, time window) players, windows of W units of times")
     ap.add_argument("--batch-size", type=int, default=128)
     ap.add_argument("--name", help="file name suffix (default: the synthetic configuration or 'dataset')")
     ap.add_argument("--out-dir", default=".")
     args = ap.parse_args()
+    if args.window and args.method == "ig":
+        ap.error("--window needs --method ablation or shapley")
 
     from raindrop_b200 import data as RD
     from raindrop_b200.attribution import (feature_ablation, integrated_gradients, sensor_importance, sensor_ranking,
-                                           shapley_value_sampling)
+                                           shapley_value_sampling, time_window_mask)
     from raindrop_b200.synth import make_batch, model_config
     device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else None
     if device is None:
@@ -120,7 +129,10 @@ def main():
         with open(args.sensor_names) as f:
             names = [s.strip() for s in f if s.strip()]
 
-    total = torch.zeros(N, dtype=torch.float64, device=device)
+    n_windows = 1
+    if args.window:
+        n_windows = max(1, int(np.ceil(float(Ptime.max()) / args.window)))
+    total = torch.zeros(n_windows * N, dtype=torch.float64, device=device)
     n = P.shape[1]
     for s in range(0, n, args.batch_size):
         e = min(n, s + args.batch_size)
@@ -133,14 +145,24 @@ def main():
             total += sensor_importance(attr_src, N).double() * (e - s)
             continue
         fixed = (None, static)                  # statics held fixed: only sensors are players that change the input
+        mask = None
+        if args.window:
+            mask, _ = time_window_mask(times, args.window, n_windows=n_windows, sensor_groups=N)
         if args.method == "ablation":
-            attr, _ = feature_ablation(model, src, static, times, lengths, target=target, baselines=fixed)
+            attr, _ = feature_ablation(model, src, static, times, lengths, target=target, baselines=fixed,
+                                       feature_mask=mask)
         else:
             attr, _ = shapley_value_sampling(model, src, static, times, lengths, target=target, baselines=fixed,
-                                             n_samples=args.shapley_samples, seed=args.seed)
-        total += attr.double().abs().sum(dim=0)
-    ranking = sensor_ranking(total / n, names)
+                                             n_samples=args.shapley_samples, seed=args.seed, feature_mask=mask)
+        total[:attr.shape[1]] += attr.double().abs().sum(dim=0)      # a batch may not reach the last windows
     prefix = {"ig": "IG", "ablation": "Ablation", "shapley": "Shapley"}[args.method]
+    if args.window:
+        scores = (total / n).view(n_windows, N).cpu().numpy()
+        out = os.path.join(args.out_dir, "%s_time_sensor_scores_%s.npy" % (prefix, name))
+        np.save(out, scores)
+        print("wrote %s: [%d windows of %g, %d sensors]" % (out, n_windows, args.window, N))
+        return
+    ranking = sensor_ranking(total / n, names)
     out = os.path.join(args.out_dir, "%s_density_scores_%s.npy" % (prefix, name))
     np.save(out, ranking)
     print("wrote %s: %d sensors, top 5 %s" % (out, N, ranking[:5].tolist()))

@@ -203,11 +203,22 @@ def positional_encoding(times, max_len, d_pe=16):
 # --------------------------------------------------------------------------------------------
 # Transformer encoder layer written out (torch.nn.TransformerEncoderLayer, post-LN, relu)
 # --------------------------------------------------------------------------------------------
-def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5):
+def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None):
     """x [T, B, D]; pad [B, T] bool (True = padded key); p = dict of the layer's tensors with the
-    state-dict suffixes as keys.  Eval-mode math of the module called at code/models_rd.py:358."""
+    state-dict suffixes as keys.  Eval-mode math of the module called at code/models_rd.py:358.
+
+    `masks` (optional) = dict of dropout multipliers (0 or 1/(1-p)), each optional, applied where the module's
+    dropouts sit in training: "attn" [B, H, T, T] (query, key) on the attention weights after the softmax,
+    "resid1" [T*B, D] on the out-projection (dropout1), "ffn" [T*B, nhid] on relu(linear1) (dropout) and
+    "resid2" [T*B, D] on linear2 (dropout2).  Train-mode math with those masks instead of torch's RNG."""
     T, B, D = x.shape
     hd = D // nhead
+    m = masks or {}
+
+    def drop(t, key):
+        mk = m.get(key)
+        return t if mk is None else t * torch.as_tensor(mk, dtype=t.dtype).reshape(t.shape)
+
     qkv = x @ p["self_attn.in_proj_weight"].T + p["self_attn.in_proj_bias"]
     q, k, v = qkv.split(D, dim=-1)
 
@@ -216,12 +227,12 @@ def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5):
 
     s = (heads(q) / math.sqrt(hd)) @ heads(k).transpose(-1, -2)
     s = s.masked_fill(pad[:, None, None, :], -math.inf)
-    a = torch.softmax(s, -1)
+    a = drop(torch.softmax(s, -1), "attn")
     o = (a @ heads(v)).permute(2, 0, 1, 3).reshape(T, B, D)
-    y = o @ p["self_attn.out_proj.weight"].T + p["self_attn.out_proj.bias"]
+    y = drop(o @ p["self_attn.out_proj.weight"].T + p["self_attn.out_proj.bias"], "resid1")
     x1 = F.layer_norm(x + y, (D,), p["norm1.weight"], p["norm1.bias"], eps)
-    f = F.relu(x1 @ p["linear1.weight"].T + p["linear1.bias"])
-    g = f @ p["linear2.weight"].T + p["linear2.bias"]
+    f = drop(F.relu(x1 @ p["linear1.weight"].T + p["linear1.bias"]), "ffn")
+    g = drop(f @ p["linear2.weight"].T + p["linear2.bias"], "resid2")
     return F.layer_norm(x1 + g, (D,), p["norm2.weight"], p["norm2.bias"], eps)
 
 
@@ -264,11 +275,13 @@ class RaindropV2Oracle(nn.Module):
         glorot_(self.R_u)
 
     # -- pieces shared by both evaluation modes ------------------------------------------------
-    def _lift(self, src):
+    def _lift(self, src, mask=None):
         """code/models_rd.py:285-296: drop the mask half, repeat each sensor d_ob times, scale by
-        R_u, relu, dropout."""
+        R_u, relu, dropout (or the given [T, B, N*d_ob] dropout multipliers in its place)."""
         vals = src[:, :, : src.shape[2] // 2]
         h = F.relu(torch.repeat_interleave(vals, self.d_ob, dim=-1) * self.R_u.to(src.dtype))
+        if mask is not None:
+            return h * torch.as_tensor(mask, dtype=h.dtype).reshape(h.shape)
         return self.dropout(h)
 
     def _graph(self):
@@ -277,10 +290,17 @@ class RaindropV2Oracle(nn.Module):
             gs = torch.ones(self.d_inp, self.d_inp)
         return graph_from_adjacency(gs.float())
 
-    def _tail(self, obs, pe, static, lengths, pad):
-        """code/models_rd.py:354-385: concat PE, temporal self-attention, masked mean, head."""
+    def _tail(self, obs, pe, static, lengths, pad, layer_masks=None):
+        """code/models_rd.py:354-385: concat PE, temporal self-attention, masked mean, head.  With `layer_masks`
+        (one encoder_layer_explicit mask dict per layer) the layers run written out, with those dropout masks."""
         z = torch.cat([obs, pe], dim=2)
-        r = self.transformer_encoder(z, src_key_padding_mask=pad)
+        if layer_masks is None:
+            r = self.transformer_encoder(z, src_key_padding_mask=pad)
+        else:
+            assert len(layer_masks) == self.nlayers, (len(layer_masks), self.nlayers)
+            r = z
+            for layer, lm in zip(self.transformer_encoder.layers, layer_masks):
+                r = encoder_layer_explicit(r, pad, dict(layer.named_parameters()), self.nhead, layer.norm1.eps, lm)
         keep = (~pad).T[:, :, None].to(r.dtype)                          # [T, B, 1]
         pooled = (r * keep).sum(0) / (lengths[:, None] + 1)
         if static is not None:
@@ -313,10 +333,14 @@ class RaindropV2Oracle(nn.Module):
         return logits, distance, None
 
     # -- independent closed form -----------------------------------------------------------------
-    def forward_dense(self, src, static, times, lengths, stages=None, tf32_model=False):
+    def forward_dense(self, src, static, times, lengths, stages=None, tf32_model=False, masks=None):
+        """`masks` (optional, oracle/dropout_masks.model_masks layout): {"lift": [T, B, N*d_ob], "layers": [one
+        encoder_layer_explicit mask dict per layer]} replace every dropout of the training forward, so that the
+        train-mode output and its autograd gradient are those of the given masks (run in float64 for an exact
+        reference).  Without masks the modules' own dropout applies (identity in eval)."""
         T, B = src.shape[0], src.shape[1]
         N, d_ob = self.d_inp, self.d_ob
-        h = self._lift(src)
+        h = self._lift(src, None if masks is None else masks["lift"])
         pe = positional_encoding(times, self.max_len).to(src.dtype)
         pad = torch.arange(T)[None, :] >= lengths[:, None]
         edge_index, edge_w = self._graph()
@@ -331,7 +355,7 @@ class RaindropV2Oracle(nn.Module):
             h1 = self.ob_propagation.forward_dense(x, s)
             h2 = self.ob_propagation_layer2.forward_dense(h1, s)
         obs = h2.view(B, N, T, d_ob).permute(2, 0, 1, 3).reshape(T, B, N * d_ob)
-        logits, r = self._tail(obs, pe, static, lengths, pad)
+        logits, r = self._tail(obs, pe, static, lengths, pad, None if masks is None else masks["layers"])
         if stages is not None:
             stages.update(lift=h, pe=pe, x0=x, h1=h1, obs=obs, enc=r)
         return logits, torch.zeros((), dtype=src.dtype), None

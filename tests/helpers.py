@@ -69,6 +69,23 @@ def check_against_golden(z, full, name, tensor, tol, errs, metric=normwise):
     assert e < tol, "%s: %s error %.3e >= %.1e" % (name, metric.__name__, e, tol)
 
 
+def random_shape_case(seed):
+    """(cfg, batch, weight_seed) of a seeded model shape the BASELINE configs do not hit: odd sensor counts (head dim
+    not a multiple of 4), tiny and ragged T, 1..8 classes, with / without statics, random sparse weighted graphs,
+    batch sizes around the 128-row tile edges."""
+    g = torch.Generator().manual_seed(1000 + seed)
+    ri = lambda lo, hi: int(torch.randint(lo, hi + 1, (1,), generator=g))
+    N, T, B = ri(1, 13), ri(2, 70), [1, 2, 3, 5, 9, 17, 33, 64, 130][ri(0, 8)]
+    static = bool(ri(0, 1))
+    cfg = dict(name="RND", d_inp=N, max_len=T, d_static=ri(1, 7) if static else 0, n_classes=ri(2, 8), static=static,
+               batch=B, p_obs=0.5, d_ob=4, d_model=4 * N, nhid=8 * N, nlayers=ri(1, 3), nhead=2, dropout=0.2, MAX=100)
+    if ri(0, 1):
+        a = (torch.rand(N, N, generator=g) < 0.4).float() * torch.rand(N, N, generator=g)
+        cfg["global_structure"] = a
+    batch = make_batch(cfg, B, seed=seed, first_time_zero=bool(ri(0, 1)))
+    return cfg, batch, 40 + seed
+
+
 def build_dropin(cfg, weight_seed, device="cuda"):
     from raindrop_b200.models_rd import Raindrop_v2
     torch.manual_seed(1)

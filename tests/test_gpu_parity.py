@@ -10,7 +10,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import (build_dropin, case_setup, check_against_golden, load_golden, normwise, rel_l2,
+from helpers import (build_dropin, case_setup, check_against_golden, load_golden, normwise, random_shape_case, rel_l2,
                      sparse_structure, to_dev)
 from raindrop_b200.synth import make_batch, model_config, synth_weights, used_param_keys
 
@@ -174,16 +174,7 @@ def test_random_shapes_against_oracle(seed):
     multiple of 4), tiny and ragged T, 1..8 classes, with / without statics, random sparse weighted graphs,
     batch sizes around the 128-row tile edges."""
     from oracle.raindrop_oracle import build_oracle_model
-    g = torch.Generator().manual_seed(1000 + seed)
-    ri = lambda lo, hi: int(torch.randint(lo, hi + 1, (1,), generator=g))
-    N, T, B = ri(1, 13), ri(2, 70), [1, 2, 3, 5, 9, 17, 33, 64, 130][ri(0, 8)]
-    static = bool(ri(0, 1))
-    cfg = dict(name="RND", d_inp=N, max_len=T, d_static=ri(1, 7) if static else 0, n_classes=ri(2, 8), static=static,
-               batch=B, p_obs=0.5, d_ob=4, d_model=4 * N, nhid=8 * N, nlayers=ri(1, 3), nhead=2, dropout=0.2, MAX=100)
-    if ri(0, 1):
-        a = (torch.rand(N, N, generator=g) < 0.4).float() * torch.rand(N, N, generator=g)
-        cfg["global_structure"] = a
-    batch = make_batch(cfg, B, seed=seed, first_time_zero=bool(ri(0, 1)))
+    cfg, batch, _ = random_shape_case(seed)
     oracle = build_oracle_model(cfg).eval()
     synth_weights(oracle, cfg, seed=40 + seed)
     shape = {kk: cfg[kk] for kk in ("d_inp", "max_len", "batch", "nlayers", "n_classes", "static")}
@@ -690,8 +681,10 @@ def test_grouped_weight_gradients(shapes):
 @pytest.mark.parametrize("B,H,T,hd", [(5, 2, 60, 76), (3, 2, 10, 20), (2, 4, 64, 96), (4, 1, 33, 8), (130, 2, 60, 76)])
 def test_temporal_attention_operator(B, H, T, hd):
     """rd_temporal_attention_fwd/_bwd (tensor-core kernels) vs an fp64 torch restatement of the masked softmax attention
-    of nn.TransformerEncoderLayer (code/models_rd.py:358), and vs the CUDA-core kernels under dropout (same
-    counter-based masks -> same result)."""
+    of nn.TransformerEncoderLayer (code/models_rd.py:358); under dropout, both the tensor-core (impl 1) and the
+    CUDA-core (impl 2) kernels vs the same restatement with the attention-probability mask rebuilt from the documented
+    Philox stream (oracle/dropout_masks.py), a key row of length 1 included."""
+    from oracle.dropout_masks import attention_mask
     from raindrop_b200 import lib as L
     lib = L.load()
     g = torch.Generator().manual_seed(B * 1000 + T)
@@ -700,6 +693,7 @@ def test_temporal_attention_operator(B, H, T, hd):
     dctx = torch.randn(T, B, D, generator=g).cuda()
     lengths = torch.randint(1, T + 1, (B,), generator=g).cuda()
     lengths[0] = T
+    lengths[-1] = 1
     rng = torch.tensor([12345, 7], dtype=torch.int64, device="cuda")
 
     def run(impl, p):
@@ -711,20 +705,35 @@ def test_temporal_attention_operator(B, H, T, hd):
         torch.cuda.synchronize()
         return ctx, dq
 
+    def reference(drop):
+        x = qkv.double().requires_grad_(True)
+        q, k, v = (x[:, :, i * D:(i + 1) * D].reshape(T, B, H, hd).permute(1, 2, 0, 3) for i in range(3))
+        s = q @ k.transpose(-1, -2) / hd ** 0.5
+        mask = torch.arange(T, device="cuda")[None, :] >= lengths[:, None]
+        s = s.masked_fill(mask[:, None, None, :], float("-inf"))
+        a = torch.softmax(s, -1)
+        if drop is not None:
+            a = a * drop
+        ref = (a @ v).permute(2, 0, 1, 3).reshape(T, B, D)
+        ref.backward(dctx.double())
+        return ref.detach(), x.grad
+
     ctx, dq = run(1, 0.0)
-    x = qkv.double().requires_grad_(True)
-    q, k, v = (x[:, :, i * D:(i + 1) * D].reshape(T, B, H, hd).permute(1, 2, 0, 3) for i in range(3))
-    s = q @ k.transpose(-1, -2) / hd ** 0.5
-    mask = torch.arange(T, device="cuda")[None, :] >= lengths[:, None]
-    s = s.masked_fill(mask[:, None, None, :], float("-inf"))
-    ref = (torch.softmax(s, -1) @ v).permute(2, 0, 1, 3).reshape(T, B, D)
-    ref.backward(dctx.double())
+    ref, dref = reference(None)
     assert normwise(ctx, ref) < 2e-5, normwise(ctx, ref)
-    assert normwise(dq, x.grad) < 2e-5, normwise(dq, x.grad)
+    assert normwise(dq, dref) < 2e-5, normwise(dq, dref)
     if T <= 64 and hd <= 96:
-        for p in (0.0, 0.2):
-            c1, d1 = run(1, p); c2, d2 = run(2, p)
-            assert normwise(c1, c2) < 2e-5 and normwise(d1, d2) < 2e-5, (p, normwise(c1, c2), normwise(d1, d2))
+        p = 0.2
+        drop = torch.from_numpy(attention_mask((12345, 7), p, 0, B, H, T)).double().cuda()   # site 16 = layer 0
+        assert (drop == 0).any() and abs((drop > 0).double().mean().item() - (1 - p)) < 6 * (p * (1 - p) / drop.numel()) ** 0.5
+        ref_d, dref_d = reference(drop)
+        assert normwise(ref_d, ref) > 1e-2          # the mask does change the result
+        for impl in (1, 2):
+            for pp, r, dr in ((0.0, ref, dref), (p, ref_d, dref_d)):
+                c, d = run(impl, pp)
+                e_c, e_d = normwise(c, r), normwise(d, dr)
+                print("attention impl", impl, "p", pp, (B, H, T, hd), "ctx", e_c, "d_qkv", e_d)
+                assert e_c < 2e-5 and e_d < 2e-5, (impl, pp, e_c, e_d)
 
 
 # ---- training mode --------------------------------------------------------------------------------

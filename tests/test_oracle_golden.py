@@ -81,6 +81,10 @@ def test_encoder_layer_explicit_matches_torch_module():
     out = encoder_layer_explicit(x, pad, p, H)
     valid = (~pad).T[:, :, None]
     assert normwise(out * valid, ref * valid) < 1e-5
+    # all-keep dropout masks (the train-mode oracle's hook, oracle/dropout_masks.py) change nothing
+    ones = dict(attn=torch.ones(B, H, T, T), resid1=torch.ones(T * B, D), ffn=torch.ones(T * B, 40),
+                resid2=torch.ones(T * B, D))
+    assert torch.equal(encoder_layer_explicit(x, pad, p, H, masks=ones), out)
 
 
 def test_graph_and_pe_conventions():

@@ -332,6 +332,31 @@ int rd_raindrop_v2_cell_coalition_attribution(const rd_dims* dims, const rd_para
                                               int32_t coalitions_per_chunk, void* scratch, float* attr,
                                               float* endpoint_logits, void* stream);
 
+/* ---- KernelSHAP of Raindrop_v2 over value-cell players, in one call -------------------------------------------------
+ * Players, removal, cell_player and its strides ((0, 0): one player per sensor), target, baselines, endpoint_logits and
+ * eval arithmetic as for rd_raindrop_v2_cell_coalition_attribution.  With v_b(S) = F(S) of sample b and the caller's
+ * coalitions z_j (coalitions [M, P] device uint8, nonzero = player kept) and weights w_j (weights [M] device fp64),
+ *   r_b[g]     = sum_j w_j z_j[g] (v_b(z_j) - v_b(empty))                          (fp64, per sample)
+ *   attr[b, g] = sum_h K[g, h] r_b[h] + k[g] (v_b(all) - v_b(empty))               (fp64, rounded to fp32)
+ * where solve = [K | k] [P, P+1] (device fp64, row-major) is the first P rows of pinv([[A, 1], [1^T, 0]]),
+ * A = sum_j w_j z_j z_j^T: the efficiency-constrained weighted least-squares fit of the coalition values.  The operator
+ * depends on the coalitions only and is computed by the caller (raindrop_b200.attribution computes it with numpy);
+ * with all 2^P - 2 proper non-empty coalitions and the Shapley-kernel weights the result is the exact Shapley values.
+ * 1 <= n_players <= RD_KERNEL_SHAP_MAX_PLAYERS; n_coalitions = M >= 0 (M = 0: attr = k (v(all) - v(empty))).
+ * Work: the endpoint forward on 2B rows, then the M coalitions in chunks of coalitions_per_chunk on B*coalitions_per_chunk
+ * rows (coalition-major): the inputs expanded in one launch that reads the chunk's rows of `coalitions` as its keep
+ * table, the eval forward, and one launch that adds the chunk into fp64 sums r [B, P] in coalition order (deterministic,
+ * no atomics, independent of the chunking); finally one launch of one CTA per sample applies [K | k].  dims->obprop_mode
+ * 0 is resolved once from B*coalitions_per_chunk rows.  scratch: rd_coalition_attribution_scratch_bytes(dims, n_players,
+ * coalitions_per_chunk) bytes.  Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+#define RD_KERNEL_SHAP_MAX_PLAYERS 4096
+int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                               const float* times, const int64_t* lengths, const float* node_scale, const float* baseline_src,
+                               const float* baseline_statics, const int64_t* target, const int32_t* cell_player,
+                               int64_t player_stride_t, int64_t player_stride_b, int32_t n_players, const uint8_t* coalitions,
+                               const double* weights, int32_t n_coalitions, const double* solve, int32_t coalitions_per_chunk,
+                               void* scratch, float* attr, float* endpoint_logits, void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);

@@ -8,7 +8,9 @@ IG_density_scores_<dataset>.npy):
 * the same two with feature_mask (rd_raindrop_v2_cell_coalition_attribution): per player of a map of the value cells
   (t, b, n), e.g. (sensor, time window) players from time_window_mask -- "what does removing heart rate in hours 12-18
   do to this prediction?".  Removing a player writes the baseline into its cells of the value half; cells with id -1
-  belong to no player and keep x.
+  belong to no player and keep x;
+* kernel_shap (rd_raindrop_v2_kernel_shap): Shapley values over the same players by KernelSHAP, the efficiency-
+  constrained weighted regression over sampled coalitions (any budget; all_coalitions gives the exact values).
 
     attr_src, attr_static = integrated_gradients(model.eval(), src, static, times, lengths, target=y)
     ranking = sensor_ranking(sensor_importance(attr_src, model.d_inp), names)
@@ -179,12 +181,18 @@ class _Call:
 
     def scratch(self, name, key, nbytes):
         """fp32 scratch of at least `nbytes`, one buffer per plan and entry point: a new key, or a call that needs more
-        bytes than the buffer holds, replaces the old one."""
+        bytes than the buffer holds, replaces the old one.  A buffer used by a call under CUDA-graph capture is also held
+        for the plan's lifetime (plan._scratch_captured), so the graph's replays stay valid after a later call has
+        replaced it."""
         plan = self.plan
         cached = plan.__dict__.get(name)
         if cached is None or cached[0] != key or cached[1].numel() * 4 < nbytes:
             plan.__dict__[name] = None
             cached = plan.__dict__[name] = (key, torch.empty(nbytes // 4, device=self.device, dtype=torch.float32))
+        if self.device.type == "cuda" and torch.cuda.is_current_stream_capturing():
+            held = plan.__dict__.setdefault("_scratch_captured", [])
+            if not any(t is cached[1] for t in held):
+                held.append(cached[1])
         return cached[1]
 
 
@@ -407,18 +415,26 @@ def time_window_mask(times, window, n_windows=None, sensor_groups=None):
     return torch.where(pad[:, :, None], -1, ids).to(torch.int32).contiguous(), n_windows
 
 
-def _coalition_attribution(fn, method, model, src, static, times, lengths, target, baselines, sensor_groups,
-                           orders_host, internal_batch_size, feature_mask=None):
-    """attr [B, P] of rd_raindrop_v2_coalition_attribution (sensor groups) or rd_raindrop_v2_cell_coalition_attribution
-    (feature_mask), the endpoint logits [2, B, ncls], the target and G."""
+def _players(model, src, sensor_groups, feature_mask):
+    """(groups [N] or None, feature mask or None, G, P = G + the static player) of an attribution call."""
     if feature_mask is None:
         groups, G = _check_groups(sensor_groups, model._plan.N)
+        cells = None
     else:
         if sensor_groups is not None:
             raise ValueError("give sensor_groups or feature_mask, not both")
         cells, G = _check_feature_mask(feature_mask, model._plan.T, src.shape[1], model._plan.N)
+        groups = None
+    return groups, cells, G, G + (1 if model.static else 0)
+
+
+def _coalition_attribution(fn, method, model, src, static, times, lengths, target, baselines, sensor_groups,
+                           orders_host, internal_batch_size, feature_mask=None):
+    """attr [B, P] of rd_raindrop_v2_coalition_attribution (sensor groups) or rd_raindrop_v2_cell_coalition_attribution
+    (feature_mask), the endpoint logits [2, B, ncls], the target and G."""
+    groups, cells, G, P = _players(model, src, sensor_groups, feature_mask)
+    if feature_mask is not None:
         fn = "rd_raindrop_v2_cell_coalition_attribution"
-    P = G + (1 if model.static else 0)
     orders = orders_host(P) if method == RD_ATTR_SHAPLEY else None
     cl = _Call(model, src, static, times, lengths, target, baselines)
     lib, plan, device, B = cl.lib, cl.plan, cl.device, src.shape[1]
@@ -535,6 +551,207 @@ def shapley_value_sampling(model, src, static, times, lengths, target=None, base
     if not return_convergence_delta:
         return out
     f = _endpoint_values(ends, tgt).double()
+    return out + ((attr.double().sum(dim=1) - (f[1] - f[0])).float(),)
+
+
+# ---- KernelSHAP: Shapley values by an efficiency-constrained weighted regression over sampled coalitions ---------------
+KERNEL_SHAP_MAX_PLAYERS = 4096       # the solve operator is P^2 fp64 on the device and a pinv of O(P^3) on the host
+ALL_COALITIONS_MAX_PLAYERS = 20
+
+
+def _shapley_kernel(P, sizes):
+    """Probability ~ (P-1) / (s (P-s)) of a coalition size s in [1, P-1] (the Shapley kernel summed over a size)."""
+    return (P - 1) / (sizes * (P - sizes))
+
+
+def sample_coalitions(n_players, n_samples, seed=0):
+    """(Z uint8 [M, P], w float64 [M]): paired coalitions for kernel_shap, drawn by numpy.random.default_rng(seed).
+    Each pair draws a size s in [1, P-1] with probability ~ (P-1) / (s (P-s)), then a uniform subset of that size (the
+    s players of smallest rng.random key); the subset is row 2i and its complement row 2i+1.  M = n_samples rounded up
+    to even, w = 1/M.  P = 1 has no proper non-empty coalition: M = 0.  The same seed gives the same set."""
+    P, n = int(n_players), int(n_samples)
+    if P < 1 or n < 1:
+        raise ValueError("n_players and n_samples must be >= 1, got %d and %d" % (P, n))
+    if P == 1:
+        return np.zeros((0, 1), dtype=np.uint8), np.zeros(0)
+    rng = np.random.default_rng(seed)
+    pairs = (n + 1) // 2
+    sizes = np.arange(1, P)
+    p = _shapley_kernel(P, sizes.astype(np.float64))
+    s = rng.choice(sizes, size=pairs, p=p / p.sum())
+    rank = np.argsort(np.argsort(rng.random((pairs, P)), axis=1), axis=1)
+    z = (rank < s[:, None]).astype(np.uint8)
+    Z = np.empty((2 * pairs, P), dtype=np.uint8)
+    Z[0::2], Z[1::2] = z, 1 - z
+    return Z, np.full(2 * pairs, 1.0 / (2 * pairs))
+
+
+def all_coalitions(n_players):
+    """(Z uint8 [2^P - 2, P], w float64): every proper non-empty coalition (row i - 1 keeps the players of the set bits
+    of i) with the Shapley-kernel weights w(s) = (P-1) / (C(P, s) s (P-s)); kernel_shap over these returns the exact
+    Shapley values.  P <= 20."""
+    P = int(n_players)
+    if not 1 <= P <= ALL_COALITIONS_MAX_PLAYERS:
+        raise ValueError("all_coalitions takes 1 <= n_players <= %d, got %d" % (ALL_COALITIONS_MAX_PLAYERS, P))
+    idx = np.arange(1, (1 << P) - 1, dtype=np.int64)
+    Z = ((idx[:, None] >> np.arange(P)) & 1).astype(np.uint8)
+    s = Z.sum(axis=1, dtype=np.int64)
+    comb = np.array([math.comb(P, k) for k in range(P + 1)], dtype=np.float64)
+    return Z, _shapley_kernel(P, s.astype(np.float64)) / comb[s]
+
+
+def kernel_shap_operator(Z, w):
+    """[K | k] float64 [P, P+1]: the first P rows of pinv([[A, 1], [1^T, 0]]), A = sum_j w_j z_j z_j^T, the KKT system
+    of the weighted least-squares fit of the coalition values under efficiency.  Any coalition set gives a well defined
+    operator (the minimum-norm solution when A is singular), and sum_g phi[g] = v(all) - v(empty) holds."""
+    Z = np.asarray(Z, dtype=np.float64)
+    w = np.asarray(w, dtype=np.float64)
+    P = Z.shape[1]
+    kkt = np.zeros((P + 1, P + 1))
+    kkt[:P, :P] = (Z.T * w) @ Z
+    kkt[:P, P] = kkt[P, :P] = 1.0
+    return np.linalg.pinv(kkt)[:P]
+
+
+def kernel_shap_from_values(values, v_empty, v_all, Z, w, operator=None):
+    """The KernelSHAP estimate on the host in fp64, [B, P]: phi_b = K r_b + k (v_b(all) - v_b(empty)),
+    r_b = sum_j w_j z_j (values[j, b] - v_b(empty)).  values [M, B] are v_b(z_j); v_empty, v_all [B]."""
+    Z = np.asarray(Z, dtype=np.float64)
+    w = np.asarray(w, dtype=np.float64)
+    v0, v1 = np.asarray(v_empty, dtype=np.float64), np.asarray(v_all, dtype=np.float64)
+    v = np.asarray(values, dtype=np.float64).reshape(Z.shape[0], v0.shape[0])
+    op = kernel_shap_operator(Z, w) if operator is None else operator
+    r = (Z * w[:, None]).T @ (v - v0[None, :])                                  # [P, B]
+    return (op[:, :-1] @ r + op[:, -1:] * (v1 - v0)[None, :]).T
+
+
+def _check_coalitions(coalitions, P):
+    """(Z uint8 [M, P] of 0/1, w float64 [M], finite and >= 0) from a pair (Z, w)."""
+    if not isinstance(coalitions, (tuple, list)) or len(coalitions) != 2:
+        raise ValueError("coalitions must be a pair (Z [M, n_players], w [M])")
+    z = torch.as_tensor(coalitions[0])
+    if z.is_floating_point() or z.is_complex():
+        raise ValueError("coalitions Z must hold 0/1 integers or booleans")
+    Z = z.cpu().numpy()
+    if Z.ndim != 2 or Z.shape[1] != P:
+        raise ValueError("coalitions Z must have shape [M, n_players=%d], got %s" % (P, Z.shape))
+    if Z.size and (Z.min() < 0 or Z.max() > 1):
+        raise ValueError("coalitions Z must hold 0/1 entries")
+    w = torch.as_tensor(coalitions[1]).detach().cpu().double().numpy()
+    if w.shape != (Z.shape[0],):
+        raise ValueError("coalition weights must have shape [M=%d], got %s" % (Z.shape[0], w.shape))
+    if not np.all(np.isfinite(w)) or np.any(w < 0):
+        raise ValueError("coalition weights must be finite and >= 0")
+    if Z.shape[0] >= 1 << 31:
+        raise ValueError("at most 2^31 - 1 coalitions")
+    return np.ascontiguousarray(Z.astype(np.uint8)), np.ascontiguousarray(w)
+
+
+def _sampled_key(P, n, seed):
+    """Cache key of sample_coalitions(P, n, seed): only an int seed names a fixed set; None, a Generator or a
+    SeedSequence draws anew on every call, so it gets None (never cached)."""
+    if isinstance(seed, (int, np.integer)) and not isinstance(seed, bool):
+        return ("sampled", P, n, int(seed))
+    return None
+
+
+def _kernel_shap_operands(plan, key, make, device):
+    """Device (Z uint8, w float64, [K | k] float64) of a coalition set, in ONE cache entry per plan that another set
+    replaces: the pinv runs and the copies are made once per set, so repeated calls and a CUDA-graph capture after an
+    eager call copy nothing, while the entry bounds the device memory to one set.  key None (a seed that is not an int,
+    e.g. None or a numpy Generator, whose draws differ from call to call) never hits.  Operands read under CUDA-graph
+    capture are held for the plan's lifetime (plan._kshap_captured), as are the scratch (_Call.scratch) and a host
+    feature mask (_device_cells), so a captured call's replays stay valid after later calls replace any of them."""
+    cached = plan.__dict__.get("_kshap")
+    if key is None or cached is None or cached[0] != key + (device.index,):
+        plan.__dict__["_kshap"] = None
+        Z, w = make()
+        op = kernel_shap_operator(Z, w)
+        got = (torch.tensor(Z, dtype=torch.uint8, device=device), torch.tensor(w, dtype=torch.float64, device=device),
+               torch.tensor(op, dtype=torch.float64, device=device))
+        cached = plan.__dict__["_kshap"] = (None if key is None else key + (device.index,), got)
+    if device.type == "cuda" and torch.cuda.is_current_stream_capturing():
+        held = plan.__dict__.setdefault("_kshap_captured", [])
+        if not any(t is cached[1] for t in held):
+            held.append(cached[1])
+    return cached[1]
+
+
+def kernel_shap(model, src, static, times, lengths, target=None, baselines=None, sensor_groups=None, feature_mask=None,
+                n_samples=None, seed=0, coalitions=None, internal_batch_size=None, return_convergence_delta=False):
+    """Shapley values by KernelSHAP of the game v(S) = F(x with the players outside S removed), F = logits[b, target[b]]
+    of an eval-mode Raindrop_v2; players (sensor_groups, or feature_mask, plus the static player G) and removal as for
+    shapley_value_sampling.  With coalitions z_j and weights w_j shared by the batch,
+
+        phi_b = K r_b + k (v_b(all) - v_b(empty)),   r_b = sum_j w_j z_j (v_b(z_j) - v_b(empty)),
+        [K | k] = the first P rows of pinv([[A, 1], [1^T, 0]]),   A = sum_j w_j z_j z_j^T
+
+    the weighted least-squares fit of the coalition values with efficiency as a constraint: sum_g phi[b, g] =
+    F(x) - F(x') up to rounding, for any coalition set.  Unlike permutation sampling, whose cost is m*(P-1) forwards,
+    any budget M works and every coalition informs every player.
+
+    n_samples:  coalitions to sample (default 2P + 2048), drawn paired by sample_coalitions(P, n_samples, seed).  An
+                int seed names a fixed set, which is cached; any other seed numpy.random.default_rng takes (None, a
+                Generator) draws a new set on every call.
+    coalitions: instead, a pair (Z [M, P] of 0/1, w [M] >= 0); all_coalitions(P) gives the exact Shapley values.
+    A player with no cell is fitted like any other: exhaustive coalitions give it 0 up to the rounding of the solve.
+
+    Returns (attr_players [B, G], attr_static [B] or None), plus delta [B] = sum of the sample's attributions -
+    (F(x) - F(x')) when return_convergence_delta.  The operator is computed on the host in fp64 once per coalition set and
+    kept on the device with the set in a one-entry cache per model.  The call evaluates M coalitions on the device besides
+    the endpoints, accumulates r in fp64 in coalition order (bitwise independent of internal_batch_size with the ob-prop
+    mode pinned) and applies the operator in fp64; everything else is as for shapley_value_sampling.  P is at most
+    KERNEL_SHAP_MAX_PLAYERS."""
+    _check_call("kernel_shap", model, src, static, baselines, internal_batch_size)
+    groups, cells, G, P = _players(model, src, sensor_groups, feature_mask)
+    if P > KERNEL_SHAP_MAX_PLAYERS:
+        raise ValueError("kernel_shap takes at most %d players, got %d" % (KERNEL_SHAP_MAX_PLAYERS, P))
+    if coalitions is None:
+        n = 2 * P + 2048 if n_samples is None else int(n_samples)
+        if n < 1:
+            raise ValueError("n_samples must be >= 1, got %d" % n)
+        key = _sampled_key(P, n, seed)
+
+        def make():
+            return sample_coalitions(P, n, seed)
+    else:
+        Z, w = _check_coalitions(coalitions, P)
+        key = ("given", Z.shape, Z.tobytes(), w.tobytes())
+
+        def make():
+            return Z, w
+    cl = _Call(model, src, static, times, lengths, target, baselines)
+    lib, plan, device, B = cl.lib, cl.plan, cl.device, src.shape[1]
+    z_d, w_d, op_d = _kernel_shap_operands(plan, key, make, device)
+    M = z_d.shape[0]
+    if groups is not None:
+        player, stride_t, stride_b = _device_int32(plan, "players", groups, device), 0, 0
+    else:
+        player, stride_t, stride_b = _cell_players(plan, cells, device)
+
+    dims = plan.dims(B, False)
+    if internal_batch_size is None:
+        cc = _default_coalitions_per_chunk(lib, dims, P, max(M, 1))
+    else:
+        cc = max(1, int(internal_batch_size) // B)
+    cc = max(1, min(cc, M))
+    nbytes = lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), P, cc)
+    if nbytes == 0:
+        L.check(-2, "rd_coalition_attribution_scratch_bytes")
+    scratch = cl.scratch("_coal_attr_scratch", device.index, nbytes)
+
+    attr = torch.empty(B, P, device=device, dtype=torch.float32)
+    ends = torch.empty(2, B, plan.n_classes, device=device, dtype=torch.float32)
+    L.check(lib.rd_raindrop_v2_kernel_shap(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st),
+                                           cl.tm.data_ptr(), cl.ln.data_ptr(), plan.node_scale.data_ptr(), cl.x0.data_ptr(),
+                                           L.ptr(cl.st0), L.ptr(cl.tgt), player.data_ptr(), stride_t, stride_b, P,
+                                           z_d.data_ptr() if M else 0, w_d.data_ptr() if M else 0, M, op_d.data_ptr(), cc,
+                                           scratch.data_ptr(), attr.data_ptr(), ends.data_ptr(), L.stream_ptr(device)),
+            "rd_raindrop_v2_kernel_shap")
+    out = _split(attr, G)
+    if not return_convergence_delta:
+        return out
+    f = _endpoint_values(ends, cl.tgt).double()
     return out + ((attr.double().sum(dim=1) - (f[1] - f[0])).float(),)
 
 

@@ -601,6 +601,60 @@ __global__ void coalition_accum_kernel(const __grid_constant__ CoalitionAccumArg
   else a.acc[o] = s;
 }
 
+// ---- KernelSHAP (rd_raindrop_v2_kernel_shap) ------------------------------------------------------------------------
+// The chunk's inputs come from coalition_expand with the caller's coalition rows z [M, P] as the keep table.
+// kernel_shap_accum_kernel, one thread per (b, player g): the fp64 regression right-hand side
+//   acc[b, g] += sum_ci w[c] * z[c, g] * (F(c) - F(x')),  c = c0 + ci,  F(c) = logits_c[ci*B + b, target]
+// coalitions in index order, no atomics: the sums, and so the result, do not depend on the chunking.  first: start from 0.
+struct KernelShapAccumArgs {
+  const float* logits_c; const float* ends; const int64_t* target; const uint8_t* z; const double* w;
+  double* acc;
+  int P, c0, nc, B, ncls, first;
+};
+__global__ void kernel_shap_accum_kernel(const __grid_constant__ KernelShapAccumArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= (long long)a.B * a.P) return;
+  const int b = (int)(o / a.P), g = (int)(o - (long long)b * a.P);
+  const int tgt = target_class(a.target, a.ends + (long long)a.B * a.ncls, b, a.ncls);
+  const double f0 = __ldg(a.ends + (long long)b * a.ncls + tgt);
+  double s = a.first ? 0.0 : a.acc[o];
+  for (int ci = 0; ci < a.nc; ++ci) {
+    const long long c = (long long)a.c0 + ci;
+    if (__ldg(a.z + c * a.P + g)) s += __ldg(a.w + c) * ((double)__ldg(a.logits_c + ((long long)ci * a.B + b) * a.ncls + tgt) - f0);
+  }
+  a.acc[o] = s;
+}
+
+// kernel_shap_solve_kernel, one CTA per sample b: acc[b, :] staged in shared memory (P doubles), one warp per output
+// player g at a time, lanes striding over h (coalesced rows of the operator) and a fixed butterfly reduction:
+//   attr[b, g] = sum_h K[g, h] acc[b, h] + k[g] (F(x) - F(x')),  solve [P, P+1] = [K | k] row-major, fp64, then fp32
+struct KernelShapSolveArgs {
+  const double* acc; const double* solve; const float* ends; const int64_t* target;
+  float* attr;
+  int P, B, ncls;
+};
+__global__ void kernel_shap_solve_kernel(const __grid_constant__ KernelShapSolveArgs a) {
+  extern __shared__ double r_s[];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x;
+  for (int h = threadIdx.x; h < a.P; h += blockDim.x) r_s[h] = a.acc[(long long)b * a.P + h];
+  const int tgt = target_class(a.target, a.ends + (long long)a.B * a.ncls, b, a.ncls);
+  const double delta = (double)__ldg(a.ends + ((long long)a.B + b) * a.ncls + tgt) -
+                       (double)__ldg(a.ends + (long long)b * a.ncls + tgt);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int g = threadIdx.x >> 5; g < a.P; g += nw) {
+    const double* row = a.solve + (long long)g * (a.P + 1);
+    double s = 0.0;
+    for (int h = lane; h < a.P; h += 32) s = fma(__ldg(row + h), r_s[h], s);
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    if (lane == 0) a.attr[(long long)b * a.P + g] = (float)fma(__ldg(row + a.P), delta, s);
+  }
+}
+
 // one warp per node: segment max, then sum of exp, then s = sum(exp / (sum + 1e-16))
 __global__ void node_scale_kernel(const int64_t* __restrict__ tgt, const float* __restrict__ w, int E, int N,
                                   float* __restrict__ s) {
@@ -1250,7 +1304,9 @@ int coalition_expand(const float* src, const float* src0, const float* statics, 
   a.player = player; a.keep = keep;
   a.src_e = src_e; a.statics_e = statics_e; a.times_e = times_e; a.lengths_e = lengths_e;
   a.stride_t = stride_t; a.stride_b = stride_b;
-  a.P = P; a.G = G; a.method = method; a.c0 = c0; a.nc = nc; a.B = B; a.T = T; a.N = N; a.ds = ds;
+  // COALITION_TABLE reads the caller's table exactly as Shapley reads the one its keep launch filled
+  a.P = P; a.G = G; a.method = method == COALITION_TABLE ? RD_ATTR_SHAPLEY : method; a.c0 = c0; a.nc = nc; a.B = B;
+  a.T = T; a.N = N; a.ds = ds;
   const int64_t rows = (int64_t)B * nc;
   a.n_src = (int64_t)T * rows * 2 * N; a.n_tok = (int64_t)T * rows; a.n_stat = ds > 0 ? rows * ds : 0; a.n_rows = rows;
   launch_pdl(coalition_expand_kernel, dim3(blocks_for(a.n_src + a.n_tok + a.n_stat + a.n_rows)), dim3(TPB), 0, st, a);
@@ -1266,6 +1322,25 @@ int coalition_accumulate(const float* logits_c, const float* ends, const int64_t
   a.P = P; a.method = method; a.m = m; a.c0 = c0; a.nc = nc; a.B = B; a.ncls = ncls; a.first = first; a.last = last;
   launch_pdl(coalition_accum_kernel, dim3(blocks_for((int64_t)B * P)), dim3(TPB), 0, st, a);
   RD_CHECK_LAUNCH("coalition_accum_kernel");
+  return 0;
+}
+
+int kernel_shap_accumulate(const float* logits_c, const float* ends, const int64_t* target, const uint8_t* z,
+                           const double* w, int P, int c0, int nc, int B, int ncls, double* acc, int first, cudaStream_t st) {
+  KernelShapAccumArgs a;
+  a.logits_c = logits_c; a.ends = ends; a.target = target; a.z = z; a.w = w; a.acc = acc;
+  a.P = P; a.c0 = c0; a.nc = nc; a.B = B; a.ncls = ncls; a.first = first;
+  launch_pdl(kernel_shap_accum_kernel, dim3(blocks_for((int64_t)B * P)), dim3(TPB), 0, st, a);
+  RD_CHECK_LAUNCH("kernel_shap_accum_kernel");
+  return 0;
+}
+
+int kernel_shap_solve(const double* acc, const double* solve, const float* ends, const int64_t* target, int P, int B,
+                      int ncls, float* attr, cudaStream_t st) {
+  KernelShapSolveArgs a;
+  a.acc = acc; a.solve = solve; a.ends = ends; a.target = target; a.attr = attr; a.P = P; a.B = B; a.ncls = ncls;
+  launch_pdl(kernel_shap_solve_kernel, dim3(B), dim3(TPB), (size_t)P * sizeof(double), st, a);
+  RD_CHECK_LAUNCH("kernel_shap_solve_kernel");
   return 0;
 }
 

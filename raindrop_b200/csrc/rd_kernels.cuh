@@ -80,6 +80,16 @@ int coalition_expand(const float* src, const float* src0, const float* statics, 
 int coalition_accumulate(const float* logits_c, const float* ends, const int64_t* target, const int32_t* orders, int P,
                          int method, int m, int c0, int nc, int B, int ncls, double* acc, float* attr, int first, int last,
                          cudaStream_t st);
+// COALITION_TABLE (KernelSHAP): coalition_expand reads `keep` as the chunk's rows of the caller's coalition table
+// [nc, P] (uint8, nonzero = kept) and launches nothing to fill it; orders is not read.
+#define COALITION_TABLE 3
+// kernel_shap_accumulate: adds sum_ci w[c] z[c, g] (F(c) - F(x')) over the chunk's coalitions c = c0 .. c0+nc-1 (F at
+// target[b], nullptr: argmax of ends[1]) into the fp64 sums acc [B, P]; first: start from 0.
+int kernel_shap_accumulate(const float* logits_c, const float* ends, const int64_t* target, const uint8_t* z,
+                           const double* w, int P, int c0, int nc, int B, int ncls, double* acc, int first, cudaStream_t st);
+// kernel_shap_solve: attr [B, P] = acc [B, P] . K^T + (F(x) - F(x')) k^T in fp64, solve = [K | k] [P, P+1]; P <= 4096.
+int kernel_shap_solve(const double* acc, const double* solve, const float* ends, const int64_t* target, int P, int B,
+                      int ncls, float* attr, cudaStream_t st);
 
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 

@@ -947,24 +947,25 @@ size_t rd_coalition_attribution_scratch_bytes(const rd_dims* dims, int32_t n_pla
   return (size_t)l.total * sizeof(float);
 }
 
-// The one implementation behind both coalition entry points: `fn` names the caller in error messages.
-static int coalition_attribution(const char* fn, const rd_dims* dims, const rd_params* params, const float* src,
-                                 const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
-                                 const float* baseline_src, const float* baseline_statics, const int64_t* target,
-                                 const int32_t* cell_player, int64_t stride_t, int64_t stride_b, int32_t n_players,
-                                 const int32_t* orders, int32_t m, int32_t method, int32_t coalitions_per_chunk, void* scratch,
-                                 float* attr, float* endpoint_logits, void* stream) {
+// What every coalition entry point (Shapley sampling and ablation, KernelSHAP) shares: the argument checks, the scratch
+// carved by coalition_layout and the endpoint forward.  `fn` names the caller in error messages.
+struct CoalRun {
+  Shape s0;
+  int P, G, B, cc;
+  float* ws; float* logits; float* src_e; float* stat_e; float* times_e; int64_t* len_e; double* acc; uint8_t* keep;
+};
+static int coalition_setup(const char* fn, const rd_dims* dims, const rd_params* params, const float* src,
+                           const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
+                           const float* baseline_src, const float* baseline_statics, const int32_t* cell_player,
+                           int64_t stride_t, int64_t stride_b, int32_t n_players, int32_t coalitions_per_chunk, void* scratch,
+                           const float* attr, const float* endpoint_logits, CoalRun* r) {
   if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !cell_player || !scratch || !attr ||
       !endpoint_logits || !params->R_u || !params->ob1_value_weight) {
     set_error("%s: NULL argument", fn);
     return -2;
   }
-  if (method != RD_ATTR_SHAPLEY && method != RD_ATTR_ABLATION) {
-    set_error("%s: method must be RD_ATTR_SHAPLEY or RD_ATTR_ABLATION, got %d", fn, method);
-    return -2;
-  }
   if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
-  Shape s0;
+  Shape& s0 = r->s0;
   RD_TRY(make_shape(dims, &s0));
   if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
   if (s0.ds > 0 && (!statics || !baseline_statics)) {
@@ -977,30 +978,57 @@ static int coalition_attribution(const char* fn, const rd_dims* dims, const rd_p
     set_error("%s: player strides must be >= 0, got (%lld, %lld)", fn, (long long)stride_t, (long long)stride_b);
     return -2;
   }
+  CoalLayout l;
+  RD_TRY(coalition_layout(dims, P, coalitions_per_chunk, &l));
+  r->P = P; r->G = G; r->B = s0.B; r->cc = coalitions_per_chunk;
+  float* S = (float*)scratch;
+  r->ws = S + l.ws; r->logits = S + l.logits;
+  r->src_e = S + l.src; r->stat_e = s0.ds > 0 ? S + l.statics : nullptr; r->times_e = S + l.times;
+  r->len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  r->acc = reinterpret_cast<double*>(S + l.acc);
+  r->keep = reinterpret_cast<uint8_t*>(S + l.keep);
+  return 0;
+}
+
+// The endpoints: one forward on 2B rows (x' rows: every player removed, cells of no player keep x; then x rows)
+// -> endpoint_logits [2, B, ncls], in the arithmetic mode pinned from B*cc rows.
+static int coalition_endpoints(const CoalRun& r, const rd_dims* dims, const rd_params* params, const float* src,
+                               const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
+                               const float* baseline_src, const float* baseline_statics, const int32_t* cell_player,
+                               int64_t stride_t, int64_t stride_b, float* endpoint_logits, cudaStream_t st) {
+  const rd_dims de = ig_dims(dims, 2 * r.B, r.cc);
+  RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
+                          nullptr, r.P, r.G, COALITION_ENDPOINTS, 0, 2, r.B, r.s0.T, r.s0.N, r.s0.ds, nullptr, r.src_e,
+                          r.stat_e, r.times_e, r.len_e, st));
+  return raindrop_fwd(&de, params, r.src_e, r.stat_e, r.times_e, r.len_e, node_scale, nullptr, r.ws, endpoint_logits, nullptr,
+                      nullptr, nullptr, 0, st);
+}
+
+// The one implementation behind both Shapley-sampling / ablation entry points.
+static int coalition_attribution(const char* fn, const rd_dims* dims, const rd_params* params, const float* src,
+                                 const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
+                                 const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                 const int32_t* cell_player, int64_t stride_t, int64_t stride_b, int32_t n_players,
+                                 const int32_t* orders, int32_t m, int32_t method, int32_t coalitions_per_chunk, void* scratch,
+                                 float* attr, float* endpoint_logits, void* stream) {
+  if (method != RD_ATTR_SHAPLEY && method != RD_ATTR_ABLATION) {
+    set_error("%s: method must be RD_ATTR_SHAPLEY or RD_ATTR_ABLATION, got %d", fn, method);
+    return -2;
+  }
+  CoalRun r;
+  RD_TRY(coalition_setup(fn, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                         cell_player, stride_t, stride_b, n_players, coalitions_per_chunk, scratch, attr, endpoint_logits, &r));
+  const int P = r.P, G = r.G, B = r.B, cc = r.cc;
   if (method == RD_ATTR_SHAPLEY && (!orders || m < 1 || (int64_t)m * (P - 1) > (1LL << 30))) {
     set_error("%s: Shapley sampling needs orders and 1 <= m, m*(P-1) <= 2^30 (m = %d)", fn, m);
     return -2;
   }
-  CoalLayout l;
-  RD_TRY(coalition_layout(dims, P, coalitions_per_chunk, &l));
   cudaStream_t st = (cudaStream_t)stream;
-  const int B = s0.B, cc = coalitions_per_chunk;
   const int n_coal = method == RD_ATTR_SHAPLEY ? m * (P - 1) : P;
-  float* S = (float*)scratch;
-  float* ws = S + l.ws; float* logits = S + l.logits;
-  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
-  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
-  double* acc = reinterpret_cast<double*>(S + l.acc);
-  uint8_t* keep = reinterpret_cast<uint8_t*>(S + l.keep);
 
-  // 1. the endpoints: one forward on 2B rows (x' rows: every player removed, cells of no player keep x; then x rows)
-  //    -> endpoint_logits [2, B, ncls]
-  const rd_dims de = ig_dims(dims, 2 * B, cc);
-  RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
-                          orders, P, G, COALITION_ENDPOINTS, 0, 2, B, s0.T, s0.N, s0.ds, keep, src_e, stat_e, times_e, len_e,
-                          st));
-  RD_TRY(raindrop_fwd(&de, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, endpoint_logits, nullptr, nullptr,
-                      nullptr, 0, st));
+  // 1. the endpoints
+  RD_TRY(coalition_endpoints(r, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                             cell_player, stride_t, stride_b, endpoint_logits, st));
   // 2. chunks of cc coalitions (the last one possibly shorter, same scratch, same arithmetic mode); with no coalition
   //    (Shapley over one player) a single accumulation turns the endpoints into the result
   int c0 = 0;
@@ -1009,12 +1037,13 @@ static int coalition_attribution(const char* fn, const rd_dims* dims, const rd_p
     if (nc > 0) {
       const rd_dims dc = ig_dims(dims, B * nc, cc);
       RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
-                              orders, P, G, method, c0, nc, B, s0.T, s0.N, s0.ds, keep, src_e, stat_e, times_e, len_e, st));
-      RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, logits, nullptr, nullptr,
-                          nullptr, 0, st));
+                              orders, P, G, method, c0, nc, B, r.s0.T, r.s0.N, r.s0.ds, r.keep, r.src_e, r.stat_e, r.times_e,
+                              r.len_e, st));
+      RD_TRY(raindrop_fwd(&dc, params, r.src_e, r.stat_e, r.times_e, r.len_e, node_scale, nullptr, r.ws, r.logits, nullptr,
+                          nullptr, nullptr, 0, st));
     }
-    RD_TRY(coalition_accumulate(logits, endpoint_logits, target, orders, P, method, m, c0, nc, B, s0.ncls, acc, attr, c0 == 0,
-                                c0 + nc >= n_coal, st));
+    RD_TRY(coalition_accumulate(r.logits, endpoint_logits, target, orders, P, method, m, c0, nc, B, r.s0.ncls, r.acc, attr,
+                                c0 == 0, c0 + nc >= n_coal, st));
     c0 += cc;
   } while (c0 < n_coal);
   return 0;
@@ -1049,6 +1078,58 @@ int rd_raindrop_v2_cell_coalition_attribution(const rd_dims* dims, const rd_para
                                node_scale, baseline_src, baseline_statics, target, cell_player, player_stride_t,
                                player_stride_b, n_players, orders, m, method, coalitions_per_chunk, scratch, attr,
                                endpoint_logits, stream);
+}
+
+// KernelSHAP: the checks, scratch and endpoint forward of coalition_attribution (coalition_setup, coalition_endpoints;
+// the layout's keep table is not used), then the chunked coalition forwards with the caller's coalition table as the
+// keep table, the regression right-hand side accumulated in the fp64 running sums (acc) and one solve launch at the end.
+int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                               const float* times, const int64_t* lengths, const float* node_scale, const float* baseline_src,
+                               const float* baseline_statics, const int64_t* target, const int32_t* cell_player,
+                               int64_t player_stride_t, int64_t player_stride_b, int32_t n_players, const uint8_t* coalitions,
+                               const double* weights, int32_t n_coalitions, const double* solve, int32_t coalitions_per_chunk,
+                               void* scratch, float* attr, float* endpoint_logits, void* stream) {
+  const char* fn = "rd_raindrop_v2_kernel_shap";
+  if (!solve) { set_error("%s: NULL argument", fn); return -2; }
+  if (n_coalitions < 0 || (n_coalitions > 0 && (!coalitions || !weights))) {
+    set_error("%s: n_coalitions = %d must be >= 0, and > 0 needs coalitions and weights", fn, n_coalitions);
+    return -2;
+  }
+  if (n_players > RD_KERNEL_SHAP_MAX_PLAYERS) {
+    set_error("%s: n_players = %d, at most %d", fn, n_players, RD_KERNEL_SHAP_MAX_PLAYERS);
+    return -2;
+  }
+  CoalRun r;
+  RD_TRY(coalition_setup(fn, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                         cell_player, player_stride_t, player_stride_b, n_players, coalitions_per_chunk, scratch, attr,
+                         endpoint_logits, &r));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int P = r.P, G = r.G, B = r.B, cc = r.cc;
+  const int64_t M = n_coalitions;
+
+  // 1. the endpoints
+  RD_TRY(coalition_endpoints(r, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                             cell_player, player_stride_t, player_stride_b, endpoint_logits, st));
+  // 2. chunks of cc coalitions (the last one possibly shorter, same scratch, same arithmetic mode); with no coalition a
+  //    single accumulation zeroes the sums and the solve returns k (F(x) - F(x')).  c0 runs in 64 bits: M may be up to
+  //    INT32_MAX, and c0 + cc past it must not wrap (inside the loop c0 < M fits an int).
+  int64_t c0 = 0;
+  do {
+    const int nc = (int)(M - c0 < cc ? M - c0 : cc);
+    if (nc > 0) {
+      const rd_dims dc = ig_dims(dims, B * nc, cc);
+      RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, player_stride_t,
+                              player_stride_b, nullptr, P, G, COALITION_TABLE, (int)c0, nc, B, r.s0.T, r.s0.N, r.s0.ds,
+                              const_cast<uint8_t*>(coalitions + c0 * P), r.src_e, r.stat_e, r.times_e, r.len_e, st));
+      RD_TRY(raindrop_fwd(&dc, params, r.src_e, r.stat_e, r.times_e, r.len_e, node_scale, nullptr, r.ws, r.logits, nullptr,
+                          nullptr, nullptr, 0, st));
+    }
+    RD_TRY(kernel_shap_accumulate(r.logits, endpoint_logits, target, coalitions, weights, P, (int)c0, nc, B, r.s0.ncls, r.acc,
+                                  c0 == 0, st));
+    c0 += cc;
+  } while (c0 < M);
+  // 3. attr = acc . K^T + (F(x) - F(x')) k^T
+  return kernel_shap_solve(r.acc, solve, endpoint_logits, target, P, B, r.s0.ncls, attr, st);
 }
 
 int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,

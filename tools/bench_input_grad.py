@@ -20,6 +20,10 @@ the labels, internal_batch_size R) with the hand-written loop of B-row module fo
 (P + 1 forwards for ablation; m*(P-1) + 2 for M permutations) summing F in fp64 tensors.  With --window W the players
 are (sensor, time window) cells instead: feature_mask = time_window_mask(times, W, sensor_groups=d_inp) (W in the units
 of `times`; padding rows belong to no player), and the loop removes the same cells.
+
+--kernel-shap-samples M compares, the same way, one kernel_shap call over M sampled coalitions (seed 0; the same
+players, --window included) with the loop of M + 2 B-row module forwards over the same coalitions followed by the same
+fp64 solve (the operator [K | k] is computed once, outside the timing, for both).
 """
 import argparse
 import json
@@ -106,7 +110,8 @@ def ig_compare(args, lib, cfg_name, model, b, device):
 
 def coalition_compare(args, lib, cfg_name, model, b, device):
     """Alternating timing of one feature_ablation / shapley_value_sampling call and of the loop of module forwards."""
-    from raindrop_b200.attribution import (_default_coalitions_per_chunk, feature_ablation, sample_permutations,
+    from raindrop_b200.attribution import (_default_coalitions_per_chunk, feature_ablation, kernel_shap,
+                                           kernel_shap_operator, sample_coalitions, sample_permutations,
                                            shapley_value_sampling, time_window_mask)
     src, static, times, lengths, y = b["src"], b["static"], b["times"], b["lengths"], b["y"]
     B, N = src.shape[1], src.shape[2] // 2
@@ -117,11 +122,21 @@ def coalition_compare(args, lib, cfg_name, model, b, device):
         cell_player = mask.long()                              # id -1 indexes the appended "kept" entry below
     P = G + (1 if static is not None else 0)
     M = args.shapley_samples
+    K = args.kernel_shap_samples
     orders = sample_permutations(P, M, 0).tolist() if M else None
     n_coal = M * (P - 1) if M else P
+    if K:
+        Z, w = sample_coalitions(P, K, 0)
+        n_coal = Z.shape[0]
+        op = torch.tensor(kernel_shap_operator(Z, w), dtype=torch.float64, device=device)
+        keeps = torch.tensor(Z, dtype=torch.bool, device=device)
+        zw = torch.tensor(Z * w[:, None], dtype=torch.float64, device=device)
 
     def batched():
-        if M:
+        if K:
+            kernel_shap(model, src, static, times, lengths, target=y, n_samples=K, seed=0,
+                        internal_batch_size=args.coalition_rows, feature_mask=mask)
+        elif M:
             shapley_value_sampling(model, src, static, times, lengths, target=y, n_samples=M, seed=0,
                                    internal_batch_size=args.coalition_rows, feature_mask=mask)
         else:
@@ -143,6 +158,11 @@ def coalition_compare(args, lib, cfg_name, model, b, device):
     def loop():
         fx = F(ones)
         attr = torch.zeros(B, P, dtype=torch.float64, device=device)
+        if K:
+            fx0 = F(~ones)
+            v = torch.stack([F(k) for k in keeps])                              # [M, B]
+            r = zw.T @ (v - fx0[None, :])                                        # [P, B]
+            return (op[:, :P] @ r + op[:, P:] * (fx - fx0)[None, :]).T
         if not M:
             for g in range(P):
                 keep = ones.clone()
@@ -174,10 +194,12 @@ def coalition_compare(args, lib, cfg_name, model, b, device):
     cc = min(n_coal, max(1, args.coalition_rows // B)) if args.coalition_rows else \
         _default_coalitions_per_chunk(lib, model._plan.dims(B, False), P, n_coal)
     what = "Shapley-value sampling, %d permutations" % M if M else "leave-one-out ablation"
+    if K:
+        what = "KernelSHAP, %d coalitions" % n_coal
     if args.window:
         what += " over (sensor, %g-unit time window) players" % args.window
     res = {"metric": "%s, %d players, samples/s (%s-shape synthetic)" % (what, P, cfg_name), "batch": B,
-           "players": P, "window": args.window, "shapley_samples": M, "coalitions": n_coal, "coalition_rows": args.coalition_rows,
+           "players": P, "window": args.window, "shapley_samples": M, "kernel_shap_samples": K, "coalitions": n_coal, "coalition_rows": args.coalition_rows,
            "coalitions_per_chunk": cc, "steps": args.steps, "card": card()}
     for tag, t, n in (("batched", sb, n_batched), ("loop", sl, n_loop)):
         res[tag] = {"samples_per_s": round(B / (t["median"] * 1e-3), 1), "ms_per_call": round(t["median"], 4),
@@ -197,14 +219,18 @@ def main():
     ap.add_argument("--ablation", action="store_true", help="compare leave-one-out sensor ablation, batched vs loop")
     ap.add_argument("--shapley-samples", type=int, default=0,
                     help="compare M-permutation sensor Shapley-value sampling, batched vs loop")
+    ap.add_argument("--kernel-shap-samples", type=int, default=0,
+                    help="compare KernelSHAP over M sampled coalitions, batched vs loop")
     ap.add_argument("--coalition-rows", type=int, default=None,
                     help="internal_batch_size of the batched ablation / Shapley call ((sample, coalition) rows per "
                          "chunk; default: 1 GiB scratch)")
     ap.add_argument("--window", type=float, default=0.0,
-                    help="with --ablation / --shapley-samples: (sensor, time window) players, windows of W units of times")
+                    help="with --ablation / --shapley-samples / --kernel-shap-samples: (sensor, time window) players, "
+                         "windows of W units of times")
     args = ap.parse_args()
-    if args.window and not (args.ablation or args.shapley_samples > 0):
-        ap.error("--window needs --ablation or --shapley-samples")
+    coalitions = args.ablation or args.shapley_samples > 0 or args.kernel_shap_samples > 0
+    if args.window and not coalitions:
+        ap.error("--window needs --ablation, --shapley-samples or --kernel-shap-samples")
     from raindrop_b200 import lib as L
     lib = L.load()
     device = torch.device("cuda", 0)
@@ -215,7 +241,7 @@ def main():
     if args.ig_steps > 0:
         ig_compare(args, lib, cfg_name, model, b, device)
         return
-    if args.ablation or args.shapley_samples > 0:
+    if coalitions:
         coalition_compare(args, lib, cfg_name, model, b, device)
         return
     src = b["src"].clone().requires_grad_(True)

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Writes IG_density_scores_<name>.npy, the sensor ranking the reference's leave-sensors-out experiment with
 feature_removal_level='set' reads (code/Raindrop.py:227-231), from a trained Raindrop_v2 and a data set (or, with
---method ablation / shapley, Ablation_density_scores_<name>.npy / Shapley_density_scores_<name>.npy):
+--method ablation / shapley / kernelshap, Ablation_density_scores_<name>.npy / Shapley_density_scores_<name>.npy /
+KernelSHAP_density_scores_<name>.npy):
 
     python tools/ig_sensor_ranking.py --checkpoint model.pt --data P19data/processed_data/PTdict_list.npy \\
         --outcomes P19data/processed_data/arr_outcomes.npy --split P19data/splits/phy19_split1_new.npy --part test \\
@@ -21,10 +22,11 @@ is not recorded, so this ranking is not claimed to reproduce them.
 
 --method ablation / shapley rank by the attribution of REMOVING each sensor (zeroing its value columns, as the
 experiment does; the static vector is held fixed): raindrop_b200.attribution.feature_ablation, or
-shapley_value_sampling with --shapley-samples permutations (seed --seed).  A sensor's score is the mean over samples of
-|attribution|; the file has the same [N, 2] layout.
+shapley_value_sampling with --shapley-samples permutations (seed --seed), or kernel_shap with --kernel-shap-samples
+coalitions (default 2P + 2048; seed --seed).  A sensor's score is the mean over samples of |attribution|; the file has
+the same [N, 2] layout.
 
---window W with --method ablation / shapley attributes (sensor, time window) cells instead
+--window W with --method ablation / shapley / kernelshap attributes (sensor, time window) cells instead
 (raindrop_b200.attribution.time_window_mask, windows of W units of `times`, padding rows in no window) and writes
 <Method>_time_sensor_scores_<name>.npy: float64 [n_windows, N], the mean over samples of |attribution| per (window,
 sensor).  n_windows = max(1, ceil(max(times) / W)) over the whole data set, so every batch shares the layout.
@@ -73,21 +75,23 @@ def main():
     ap.add_argument("--part", default="test", choices=["train", "val", "test"])
     ap.add_argument("--n-samples", type=int, default=512, help="--synthetic: number of samples")
     ap.add_argument("--sensor-names", help="text file, one sensor name per line (default: the indices)")
-    ap.add_argument("--method", default="ig", choices=["ig", "ablation", "shapley"])
+    ap.add_argument("--method", default="ig", choices=["ig", "ablation", "shapley", "kernelshap"])
     ap.add_argument("--steps", type=int, default=50, help="--method ig: Gauss-Legendre nodes per attribution")
     ap.add_argument("--shapley-samples", type=int, default=25, help="--method shapley: permutations per batch")
+    ap.add_argument("--kernel-shap-samples", type=int, default=None,
+                    help="--method kernelshap: sampled coalitions per batch (default 2P + 2048)")
     ap.add_argument("--window", type=float, default=0.0,
-                    help="--method ablation / shapley: (sensor, time window) players, windows of W units of times")
+                    help="--method ablation / shapley / kernelshap: (sensor, time window) players, windows of W units of times")
     ap.add_argument("--batch-size", type=int, default=128)
     ap.add_argument("--name", help="file name suffix (default: the synthetic configuration or 'dataset')")
     ap.add_argument("--out-dir", default=".")
     args = ap.parse_args()
     if args.window and args.method == "ig":
-        ap.error("--window needs --method ablation or shapley")
+        ap.error("--window needs --method ablation, shapley or kernelshap")
 
     from raindrop_b200 import data as RD
-    from raindrop_b200.attribution import (feature_ablation, integrated_gradients, sensor_importance, sensor_ranking,
-                                           shapley_value_sampling, time_window_mask)
+    from raindrop_b200.attribution import (feature_ablation, integrated_gradients, kernel_shap, sensor_importance,
+                                           sensor_ranking, shapley_value_sampling, time_window_mask)
     from raindrop_b200.synth import make_batch, model_config
     device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else None
     if device is None:
@@ -151,11 +155,14 @@ def main():
         if args.method == "ablation":
             attr, _ = feature_ablation(model, src, static, times, lengths, target=target, baselines=fixed,
                                        feature_mask=mask)
+        elif args.method == "kernelshap":
+            attr, _ = kernel_shap(model, src, static, times, lengths, target=target, baselines=fixed,
+                                  n_samples=args.kernel_shap_samples, seed=args.seed, feature_mask=mask)
         else:
             attr, _ = shapley_value_sampling(model, src, static, times, lengths, target=target, baselines=fixed,
                                              n_samples=args.shapley_samples, seed=args.seed, feature_mask=mask)
         total[:attr.shape[1]] += attr.double().abs().sum(dim=0)      # a batch may not reach the last windows
-    prefix = {"ig": "IG", "ablation": "Ablation", "shapley": "Shapley"}[args.method]
+    prefix = {"ig": "IG", "ablation": "Ablation", "shapley": "Shapley", "kernelshap": "KernelSHAP"}[args.method]
     if args.window:
         scores = (total / n).view(n_windows, N).cpu().numpy()
         out = os.path.join(args.out_dir, "%s_time_sensor_scores_%s.npy" % (prefix, name))

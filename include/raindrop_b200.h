@@ -357,6 +357,26 @@ int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, con
                                const double* weights, int32_t n_coalitions, const double* solve, int32_t coalitions_per_chunk,
                                void* scratch, float* attr, float* endpoint_logits, void* stream);
 
+/* ---- Monte Carlo dropout predictive uncertainty of Raindrop_v2, in one call ------------------------------------------
+ * Replicate m = 0 .. n_samples-1 is exactly the training-mode forward of the B-row batch with the dropout stream at
+ * {seed, step + m}, rng = {seed, step} (device uint64[2]; read, never written -- the model's own counter is not
+ * advanced).  dims->training is not read: every replicate is a training-mode forward at dims->dropout_p.  With
+ * p_m = softmax(logits_m) in fp64:
+ *   mean_probs [B, C] = mean_m p_m;  variance [B, C] = sample variance over m of p_m (divisor M - 1, 0 when M = 1);
+ *   entropies [3, B]  = (H(mean p), mean_m H(p_m), their difference = the mutual information), natural log, 0 log 0 = 0;
+ *   samples [M, B, C] (optional, may be NULL) = the replicates' logits.
+ * Work: chunks of replicates_per_chunk replicates, each ONE training forward on B*replicates_per_chunk replicate-major
+ * rows (row j = m*B + b) in which every dropout site draws for row j the words the B-row forward at step + m draws for
+ * row b, and one launch that adds the chunk into fp64 sums in replicate order (no atomics: the result is bitwise
+ * independent of the chunking).  dims->obprop_mode 0 is resolved once from B*replicates_per_chunk rows.
+ * scratch: rd_mc_dropout_scratch_bytes(dims, replicates_per_chunk) bytes.  Stream-ordered, allocation- and sync-free,
+ * CUDA-graph capturable. */
+size_t rd_mc_dropout_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk);
+int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                              const float* times, const int64_t* lengths, const float* node_scale, const uint64_t* rng,
+                              int32_t n_samples, int32_t replicates_per_chunk, void* scratch, float* mean_probs,
+                              float* variance, float* entropies, float* samples, void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);

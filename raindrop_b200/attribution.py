@@ -151,7 +151,8 @@ def _check_call(fn, model, src, static, baselines, internal_batch_size):
 
 class _Call:
     """The device-side operands of one attribution call: inputs and baselines as contiguous fp32 / int64 device tensors,
-    the target, and the parameter pointers (rd_params; `keep` holds the tensors they point into)."""
+    the target, and the parameter pointers (rd_params; `keep` holds the tensors they point into).  baselines=False: a
+    call without baselines (x0 and st0 are None)."""
 
     def __init__(self, model, src, static, times, lengths, target, baselines):
         from .models_rd import _device_of
@@ -166,9 +167,12 @@ class _Call:
         self.tm = times.detach().to(**f32).contiguous()
         self.ln = lengths.detach().to(device=device, dtype=torch.int64).contiguous()
         self.st = static.detach().to(**f32).contiguous() if model.static else None
-        b_src, b_st = baselines if baselines is not None else (None, None)
-        self.x0 = _baseline(b_src, self.x)
-        self.st0 = _baseline(b_st, self.st) if self.st is not None else None
+        if baselines is False:
+            self.x0 = self.st0 = None
+        else:
+            b_src, b_st = baselines if baselines is not None else (None, None)
+            self.x0 = _baseline(b_src, self.x)
+            self.st0 = _baseline(b_st, self.st) if self.st is not None else None
 
         params = [p.detach() for p in model.used_parameters()]
         if params[0].device != device:

@@ -26,6 +26,7 @@ struct AttnP {
   int B, H, T, hd, D;
   float scale, drop_p;
   const uint64_t* rng; uint32_t site;
+  DropRep rep;                             // forward only
 };
 
 // One [T x hd] head slice -> shared memory, row-major (rm[t*LDR + d], zero padded to 64 x 96) and/or
@@ -127,13 +128,17 @@ __device__ __forceinline__ void softmax_rows(const AttnP& p, int b, int h, float
     float e0 = (i < T && lane < nv) ? expf(v0 - mx) : 0.f, e1 = (i < T && lane + 32 < nv) ? expf(v1 - mx) : 0.f;
     float sum = warp_sum(e0 + e1);
     float inv = (i < T && nv > 0) ? 1.f / sum : 0.f;
-    const uint64_t base = ((uint64_t)(b * p.H + h) * T + i) * T;     // index space [B, H, T, T]
+    uint64_t base = ((uint64_t)(b * p.H + h) * T + i) * T;     // index space [B, H, T, T]
+    RngKey key;
+    if (p.rep.B && p.drop_p > 0.f) base = rep_remap(p.rng, p.rep, (uint32_t)b, (uint64_t)p.H * T * T, ((uint64_t)h * T + i) * T, &key);
 #pragma unroll
     for (int half = 0; half < 2; ++half) {
       const int j = lane + 32 * half;
       const float pr = (half ? e1 : e0) * inv;
       row[j] = pr;
-      const float m = (p.drop_p > 0.f && i < T && j < T) ? dropout_scale(p.rng, p.site, base + j, p.drop_p, ik) : 1.f;
+      float m = 1.f;
+      if (p.drop_p > 0.f && i < T && j < T)
+        m = p.rep.B ? dropout_scale(key, p.site, base + j, p.drop_p, ik) : dropout_scale(p.rng, p.site, base + j, p.drop_p, ik);
       Pd[i * pd_si + j * pd_sj] = pr * m;
     }
   }
@@ -332,10 +337,10 @@ static int ensure_smem_attrs() {
 }
 
 int attn_small_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p,
-                   const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st) {
+                   const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st, DropRep rep) {
   AttnP p{};
   p.qkv = qkv; p.ctx = ctx; p.lengths = lengths; p.B = B; p.H = H; p.T = T; p.hd = hd; p.D = H * hd;
-  p.scale = 1.f / sqrtf((float)hd); p.drop_p = drop_p; p.rng = rng; p.site = site;
+  p.scale = 1.f / sqrtf((float)hd); p.drop_p = drop_p; p.rng = rng; p.site = site; p.rep = rep;
   RD_TRY(ensure_smem_attrs());
   attn_small_fwd_kernel<<<B * H, 512, fwd_smem(hd), st>>>(p);
   RD_CHECK_LAUNCH("attn_small_fwd_kernel");

@@ -34,6 +34,7 @@ struct AttnTcP {
   int B, H, T, hd, D, ld;
   float scale, drop_p;
   const uint64_t* rng; uint32_t site;
+  DropRep rep;                  // forward only: replicate-major samples (rep_remap)
   unsigned long long* dbg;      // optional start / end timestamps (rd_debug_attention_timing): [CTA][16] of clock64
 };
 
@@ -149,6 +150,8 @@ __device__ __forceinline__ RowStat row_stats(const float (&s)[TR / 8][4], int nv
 // =================================================================================================
 // forward: ctx[t, b, h*hd + d] = sum_j dropout(softmax(scale * Q K^T))[t, j] V[j, d]
 // =================================================================================================
+// REP: attention dropout of replicate-major samples (rep_remap); a separate instance, so the training step's is unchanged
+template <bool REP>
 __global__ void __launch_bounds__(NTHR) attn_tc_fwd_kernel(const float* __restrict__ qkv, const AttnTcP p) {
   extern __shared__ float sm[];
   pdl_launch_dependents();
@@ -162,7 +165,9 @@ __global__ void __launch_bounds__(NTHR) attn_tc_fwd_kernel(const float* __restri
   load_slice(sQ, base, rs, p);
   load_slice(sK, base + p.D, rs, p);
   load_slice(sV, base + 2 * p.D, rs, p);
-  const RngKey key = load_rng_key(p.drop_p > 0.f ? p.rng : nullptr);
+  RngKey key = load_rng_key(p.drop_p > 0.f ? p.rng : nullptr);
+  int bd = b;             // the sample whose dropout words this CTA draws
+  if (REP) bd = (int)(rep_remap(p.rng, p.rep, (uint32_t)b, 1, 0, &key));
   const long long len = p.lengths[b];
   const int nv = (int)(len < p.T ? (len < 0 ? 0 : len) : p.T);
   const int ksd = (p.hd + 7) >> 3;
@@ -185,7 +190,7 @@ __global__ void __launch_bounds__(NTHR) attn_tc_fwd_kernel(const float* __restri
       for (int e = 0; e < 2; ++e) {
         const int c = j * 8 + 2 * t + e;
         const float ex = c < nv ? ex2_approx(fmaf(s[j][2 * i + e], sl2, -st.mxs[i])) : 0.f;
-        o[e] = (ex != 0.f && invk != 0.f) ? ex * invk * keep_at(p, key, b, h, r, c, ik) : 0.f;
+        o[e] = (ex != 0.f && invk != 0.f) ? ex * invk * keep_at(p, key, bd, h, r, c, ik) : 0.f;
       }
       *reinterpret_cast<float2*>(sP + r * LDP + j * 8 + 2 * t) = make_float2(o[0], o[1]);
     }
@@ -293,16 +298,17 @@ bool attn_tc_supported(int T, int hd) {
 }
 
 int attn_tc_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p, const uint64_t* rng,
-                uint32_t site, float* ctx, cudaStream_t st) {
+                uint32_t site, float* ctx, cudaStream_t st, DropRep rep) {
   if (!attn_tc_supported(T, hd) || ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15)) {
     set_error("attn_tc_fwd: unsupported shape / alignment (T=%d hd=%d)", T, hd);
     return -2;
   }
   AttnTcP p{};
   p.ctx = ctx; p.lengths = lengths; p.B = B; p.H = H; p.T = T; p.hd = hd; p.D = H * hd; p.ld = slice_ld(hd);
-  p.scale = 1.f / sqrtf((float)hd); p.drop_p = drop_p; p.rng = rng; p.site = site; p.dbg = g_attn_dbg;
-  RD_TRY(ensure_max_smem((const void*)attn_tc_fwd_kernel, fwd_smem(HD_MAX)));
-  launch_pdl(attn_tc_fwd_kernel, dim3(B * H), dim3(NTHR), fwd_smem(hd), st, qkv, p);
+  p.scale = 1.f / sqrtf((float)hd); p.drop_p = drop_p; p.rng = rng; p.site = site; p.rep = rep; p.dbg = g_attn_dbg;
+  auto kern = drop_p > 0.f && rep.B ? attn_tc_fwd_kernel<true> : attn_tc_fwd_kernel<false>;
+  RD_TRY(ensure_max_smem((const void*)kern, fwd_smem(HD_MAX)));
+  launch_pdl(kern, dim3(B * H), dim3(NTHR), fwd_smem(hd), st, qkv, p);
   RD_CHECK_LAUNCH("attn_tc_fwd_kernel");
   return 0;
 }

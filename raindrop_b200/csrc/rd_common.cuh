@@ -129,6 +129,22 @@ __device__ __forceinline__ float4 dropout_scale4(const RngKey& k, uint32_t site,
                      keep_scale(b.w, p, inv_keep));
 }
 
+// ---- Monte Carlo dropout replicates in one forward ------------------------------------------------------------------
+// A forward over Bc = cc*B rows, replicate-major (row j = m*B + b), in which row j draws exactly the words that the
+// B-row forward at step (step + m) draws for row b.  Every site's index space is [T, Bc, width] (attention: T = 1,
+// width = H*T*T), and rep_remap turns element `col` of row r = t*Bc + j into the key of step + m and the B-row index
+// (t*B + b)*width + col.  A 4-word draw stays valid where width % 4 == 0 and col % 4 == 0 (the row maps to a row of the
+// same width).  B == 0: off, every kernel draws as before.
+struct DropRep { int B = 0, Bc = 0; };
+__device__ __forceinline__ uint64_t rep_remap(const uint64_t* __restrict__ rng, const DropRep& rep, uint32_t r,
+                                              uint64_t width, uint64_t col, RngKey* key) {
+  const uint32_t t = r / (uint32_t)rep.Bc, j = r - t * (uint32_t)rep.Bc;
+  const uint32_t m = j / (uint32_t)rep.B, b = j - m * (uint32_t)rep.B;
+  const uint64_t seed = rng[0], step = rng[1] + m;
+  *key = RngKey{(uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(step >> 32), (uint32_t)step};
+  return ((uint64_t)t * (uint32_t)rep.B + b) * width + col;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -161,6 +177,7 @@ struct GemmP {
   const float* rowscale = nullptr; int rowscale_mod = 1;  // * rowscale[i % mod]
   const float* gate = nullptr; long long gate_ld = 0; float gate_scale = 1.f;  // * (gate[i,j] > 0 ? gate_scale : 0)
   float drop_p = 0.f; const uint64_t* rng = nullptr; uint32_t drop_site = 0;   // dropout, index i*N + j
+  DropRep rep;                                           // replicate rows (i = t*Bc + j): see rep_remap
   uint32_t* drop_mask = nullptr; int drop_mask_ld = 0;   // optional keep bits out: word [i*ld + j/32], bit j%32 (tensor-core path only)
   const float* resid = nullptr; long long resid_ld = 0;  // + resid[i*ld + j]
   // permuted store of the ob-prop output into the encoder input (code/models_rd.py:338-341):

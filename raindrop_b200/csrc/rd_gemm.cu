@@ -18,9 +18,16 @@ __device__ __forceinline__ void epilogue_store(const GemmP& p, float* __restrict
   if (p.relu) v = fmaxf(v, 0.f);
   if (p.rowscale) v *= __ldg(p.rowscale + (i % p.rowscale_mod));
   if (p.gate) v *= (__ldg(p.gate + (long long)i * p.gate_ld + j) > 0.f) ? p.gate_scale : 0.f;
-  if (p.drop_p > 0.f)
-    v *= dropout_scale(p.rng, p.drop_site, (uint64_t)i * (uint64_t)p.N + (uint64_t)j, p.drop_p,
-                       1.f / (1.f - p.drop_p));
+  if (p.drop_p > 0.f) {
+    if (p.rep.B) {
+      RngKey key;
+      const uint64_t idx = rep_remap(p.rng, p.rep, (uint32_t)i, (uint64_t)p.N, (uint64_t)j, &key);
+      v *= dropout_scale(key, p.drop_site, idx, p.drop_p, 1.f / (1.f - p.drop_p));
+    } else {
+      v *= dropout_scale(p.rng, p.drop_site, (uint64_t)i * (uint64_t)p.N + (uint64_t)j, p.drop_p,
+                         1.f / (1.f - p.drop_p));
+    }
+  }
   if (p.resid) v += __ldg(p.resid + (long long)i * p.resid_ld + j);
   if (p.perm) {
     int b = i / p.pN, n = i - b * p.pN;

@@ -219,10 +219,13 @@ struct TS8 { float v[32]; int d_pe; };      // up to 32 timescales (d_pe <= 64)
 //   o <  n_lift : X0[(b*N+n), t*d_ob + 0..d_ob) = dropout(relu(src[t,b,n] * R_u[n*d_ob + k]))   code/models_rd.py:285-296,323-327
 //                 (one thread per (row, t); for d_ob == 4 one 128-bit store and ONE Philox block per thread)
 //   o >= n_lift : positional encoding of token (o - n_lift) / 16 into out[tok*ld + col0 + j]   code/models_rd.py:28-43
+// REP: the dropout of replicate-major rows (rep_remap); a separate instance, so the training step's is unchanged
+template <bool REP>
 __global__ void lift_posenc_kernel(const float* __restrict__ src, const float* __restrict__ R_u, int B, int T, int N,
                                    int d_ob, float drop_p, const uint64_t* __restrict__ rng, int round,
                                    float* __restrict__ X0, long long n_lift, const float* __restrict__ times,
-                                   long long n_tokens, TS8 ts, float* __restrict__ pe_out, long long ld, int col0) {
+                                   long long n_tokens, TS8 ts, float* __restrict__ pe_out, long long ld, int col0,
+                                   DropRep rep) {
   pdl_launch_dependents();
   pdl_wait();
   long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -232,8 +235,26 @@ __global__ void lift_posenc_kernel(const float* __restrict__ src, const float* _
     const int b = (int)(row / N), n = (int)(row - (long long)b * N);
     const float sv = __ldg(src + ((long long)t * B + b) * (2 * N) + n);
     const float ik = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
-    const uint64_t idx0 = ((uint64_t)t * B + b) * (uint64_t)(N * d_ob) + (uint64_t)(n * d_ob);
     float* dst = X0 + row * ((long long)T * d_ob) + (long long)t * d_ob;
+    if (REP) {             // replicate rows: row t*B + b of [T, B, N*d_ob] (N*d_ob % 4 == 0 when d_ob == 4)
+      RngKey key;
+      const uint64_t idx0 = rep_remap(rng, rep, (uint32_t)(t * B + b), (uint64_t)(N * d_ob), (uint64_t)(n * d_ob), &key);
+      if (d_ob == 4) {
+        const float4 r = __ldg(reinterpret_cast<const float4*>(R_u) + n);
+        const float4 m = dropout_scale4(key, SITE_LIFT, idx0, drop_p, ik);
+        float4 v = make_float4(fmaxf(sv * r.x, 0.f) * m.x, fmaxf(sv * r.y, 0.f) * m.y, fmaxf(sv * r.z, 0.f) * m.z,
+                               fmaxf(sv * r.w, 0.f) * m.w);
+        if (round) v = make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
+        *reinterpret_cast<float4*>(dst) = v;
+      } else {
+        for (int k = 0; k < d_ob; ++k) {
+          const float v = fmaxf(sv * __ldg(R_u + n * d_ob + k), 0.f) * dropout_scale(key, SITE_LIFT, idx0 + k, drop_p, ik);
+          dst[k] = round ? to_tf32(v) : v;
+        }
+      }
+      return;
+    }
+    const uint64_t idx0 = ((uint64_t)t * B + b) * (uint64_t)(N * d_ob) + (uint64_t)(n * d_ob);
     if (d_ob == 4) {       // idx0 % 4 == 0: the four channels share one Philox block
       const float4 r = __ldg(reinterpret_cast<const float4*>(R_u) + n);
       float4 v = make_float4(fmaxf(sv * r.x, 0.f), fmaxf(sv * r.y, 0.f), fmaxf(sv * r.z, 0.f), fmaxf(sv * r.w, 0.f));
@@ -655,6 +676,109 @@ __global__ void kernel_shap_solve_kernel(const __grid_constant__ KernelShapSolve
   }
 }
 
+// ---- Monte Carlo dropout --------------------------------------------------------------------------------------------
+// mc_expand_kernel: nc replicate-major copies (row j = m*B + b) of the batch, one thread per output element of
+// src_e [T, B*nc, 2N], then times_e [T, B*nc], statics_e [B*nc, ds] and lengths_e [B*nc].
+struct McExpandArgs {
+  const float* src; const float* statics; const float* times; const int64_t* lengths;
+  float* src_e; float* statics_e; float* times_e; int64_t* lengths_e;
+  int B, nc, T, N, ds;
+};
+__global__ void mc_expand_kernel(const __grid_constant__ McExpandArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long Bc = (long long)a.B * a.nc, W = 2LL * a.N;
+  const long long n_src = a.T * Bc * W, n_times = a.T * Bc, n_stat = a.statics ? Bc * a.ds : 0;
+  long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o < n_src) {
+    const long long k = o % W, r = o / W, t = r / Bc, b = (r - t * Bc) % a.B;
+    a.src_e[o] = __ldg(a.src + (t * a.B + b) * W + k);
+    return;
+  }
+  o -= n_src;
+  if (o < n_times) {
+    const long long t = o / Bc, b = (o - t * Bc) % a.B;
+    a.times_e[o] = __ldg(a.times + t * a.B + b);
+    return;
+  }
+  o -= n_times;
+  if (o < n_stat) {
+    const long long j = o / a.ds, k = o - j * a.ds;
+    a.statics_e[o] = __ldg(a.statics + (j % a.B) * a.ds + k);
+    return;
+  }
+  o -= n_stat;
+  if (o < Bc) a.lengths_e[o] = __ldg(a.lengths + o % a.B);
+}
+
+// mc_accum_kernel, one warp per sample b: for the chunk's replicates m0 .. m0+nc-1 IN ORDER, p = softmax(logits row
+// m*B + b) in fp64 (log p = l - max - log sum exp), then acc[b] = [sum p (C) | sum p^2 (C) | sum H(p)] += ...  Lanes stride
+// over the classes and reduce by a fixed butterfly, and no other thread touches sample b's sums: the result does not
+// depend on how the replicates are chunked.  samples (optional) [M, B, C] receives the fp32 logits.  last: the fp32
+// statistics from the sums: mean [B, C], sample variance [B, C] (divisor M - 1, 0 for M = 1) and ent [3, B] =
+// (H(mean p), mean H(p), their difference).
+struct McAccumArgs {
+  const float* logits; double* acc; float* samples; float* mean; float* var; float* ent;
+  int B, ncls, nc, first, last;
+  long long m0, M;
+};
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__global__ void mc_accum_kernel(const __grid_constant__ McAccumArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= a.B) return;
+  const int C = a.ncls;
+  double* s1 = a.acc + (long long)b * (2 * C + 1);
+  double* s2 = s1 + C;
+  if (a.first) {
+    for (int c = lane; c < 2 * C + 1; c += 32) s1[c] = 0.0;
+    __syncwarp();
+  }
+  for (int m = 0; m < a.nc; ++m) {
+    const float* row = a.logits + ((long long)m * a.B + b) * C;
+    float mx = -INFINITY;
+    for (int c = lane; c < C; c += 32) mx = fmaxf(mx, __ldg(row + c));
+    mx = warp_max(mx);
+    double se = 0.0;
+    for (int c = lane; c < C; c += 32) se += exp((double)__ldg(row + c) - (double)mx);
+    const double lse = log(warp_sum_f64(se));
+    double h = 0.0;
+    for (int c = lane; c < C; c += 32) {
+      const float l = __ldg(row + c);
+      const double lp = ((double)l - (double)mx) - lse, p = exp(lp);
+      h -= p * lp;                      // p = 0 (underflow) adds 0: 0 log 0 = 0
+      s1[c] += p;
+      s2[c] += p * p;
+      if (a.samples) a.samples[((a.m0 + m) * a.B + b) * C + c] = l;
+    }
+    h = warp_sum_f64(h);
+    if (lane == 0) s1[2 * C] += h;
+  }
+  if (!a.last) return;
+  __syncwarp();
+  const double M = (double)a.M;
+  double hp = 0.0;
+  for (int c = lane; c < C; c += 32) {
+    const double mu = s1[c] / M;
+    const double v = a.M > 1 ? fmax(s2[c] - s1[c] * mu, 0.0) / (M - 1.0) : 0.0;
+    a.mean[(long long)b * C + c] = (float)mu;
+    a.var[(long long)b * C + c] = (float)v;
+    if (mu > 0.0) hp -= mu * log(mu);
+  }
+  hp = warp_sum_f64(hp);
+  if (lane == 0) {
+    const double he = s1[2 * C] / M;
+    a.ent[b] = (float)hp;
+    a.ent[a.B + b] = (float)he;
+    a.ent[2LL * a.B + b] = (float)(hp - he);
+  }
+}
+
 // one warp per node: segment max, then sum of exp, then s = sum(exp / (sum + 1e-16))
 __global__ void node_scale_kernel(const int64_t* __restrict__ tgt, const float* __restrict__ w, int E, int N,
                                   float* __restrict__ s) {
@@ -959,9 +1083,11 @@ __global__ void layernorm_bwd_param_kernel(const float* __restrict__ x, const fl
   }
 }
 
+// REP: the dropout of replicate-major samples (rep_remap); a separate instance, so the training step's is unchanged
+template <bool REP>
 __global__ void attn_softmax_fwd_kernel(float* __restrict__ S, const int64_t* __restrict__ lengths, int B, int H,
                                         int T, float drop_p, const uint64_t* __restrict__ rng, uint32_t site,
-                                        float* __restrict__ Pd) {
+                                        float* __restrict__ Pd, DropRep rep) {
   long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   int lane = threadIdx.x & 31;
   long long rows = (long long)B * H * T;
@@ -978,11 +1104,19 @@ __global__ void attn_softmax_fwd_kernel(float* __restrict__ S, const int64_t* __
   sum = warp_sum(sum);
   float inv = nv > 0 ? 1.f / sum : 0.f;
   float ik = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  RngKey key;
+  uint64_t rbase = 0;           // replicate rows: the row's words are those of sample b % rep.B of [B, H*T*T]
+  if (REP) rbase = rep_remap(rng, rep, (uint32_t)b, (uint64_t)H * T * T, (uint64_t)(row - (long long)b * H * T) * T, &key);
   for (int j = lane; j < T; j += 32) {
     float p = j < nv ? expf(sr[j] - mx) * inv : 0.f;
     sr[j] = p;
     if (Pd) {
-      float m = drop_p > 0.f ? dropout_scale(rng, site, (uint64_t)row * T + j, drop_p, ik) : 1.f;
+      float m = 1.f;
+      if (REP) {
+        m = dropout_scale(key, site, rbase + j, drop_p, ik);
+      } else if (drop_p > 0.f) {
+        m = dropout_scale(rng, site, (uint64_t)row * T + j, drop_p, ik);
+      }
       Pd[row * T + j] = p * m;
     }
   }
@@ -1214,7 +1348,7 @@ int gather_batch(const float* src, const int64_t* idx, int64_t T, int64_t n_tota
 
 int lift_posenc(const float* src, const float* R_u, int B, int T, int N, int d_ob, float drop_p, const uint64_t* rng,
                 int round, float* X0, const float* times, int64_t n_tokens, const float* ts_host, int d_pe, float* pe_out,
-                int64_t ld, int col0, cudaStream_t st) {
+                int64_t ld, int col0, cudaStream_t st, DropRep rep) {
   if (times && (d_pe < 2 || d_pe > 64 || (d_pe & 1))) { set_error("positional encoding width must be even and <= 64"); return -2; }
   const int64_t n_lift = src ? (int64_t)B * N * T : 0;      // one thread per (row, t)
   const int64_t n_pe = times ? n_tokens * d_pe : 0;
@@ -1223,8 +1357,9 @@ int lift_posenc(const float* src, const float* R_u, int B, int T, int N, int d_o
   ts.d_pe = times ? d_pe : 2;
   if (times) memcpy(ts.v, ts_host, sizeof(float) * (d_pe / 2));
   if (n_lift + n_pe <= 0) return 0;
-  launch_pdl(lift_posenc_kernel, dim3(blocks_for(n_lift + n_pe)), dim3(TPB), 0, st, src, R_u, B, T, N, d_ob, drop_p, rng, round, X0,
-             (long long)n_lift, times, (long long)(times ? n_tokens : 0), ts, pe_out, (long long)ld, col0);
+  launch_pdl(drop_p > 0.f && rep.B ? lift_posenc_kernel<true> : lift_posenc_kernel<false>, dim3(blocks_for(n_lift + n_pe)),
+             dim3(TPB), 0, st, src, R_u, B, T, N, d_ob, drop_p, rng, round, X0, (long long)n_lift, times,
+             (long long)(times ? n_tokens : 0), ts, pe_out, (long long)ld, col0, rep);
   RD_CHECK_LAUNCH("lift_posenc_kernel");
   return 0;
 }
@@ -1344,6 +1479,29 @@ int kernel_shap_solve(const double* acc, const double* solve, const float* ends,
   return 0;
 }
 
+int mc_expand(const float* src, const float* statics, const float* times, const int64_t* lengths, int B, int nc, int T,
+              int N, int ds, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st) {
+  McExpandArgs a;
+  a.src = src; a.statics = ds > 0 ? statics : nullptr; a.times = times; a.lengths = lengths;
+  a.src_e = src_e; a.statics_e = statics_e; a.times_e = times_e; a.lengths_e = lengths_e;
+  a.B = B; a.nc = nc; a.T = T; a.N = N; a.ds = ds;
+  const int64_t Bc = (int64_t)B * nc;
+  const int64_t n = Bc * T * 2 * N + Bc * T + (ds > 0 ? Bc * ds : 0) + Bc;
+  launch_pdl(mc_expand_kernel, dim3(blocks_for(n)), dim3(TPB), 0, st, a);
+  RD_CHECK_LAUNCH("mc_expand_kernel");
+  return 0;
+}
+
+int mc_accumulate(const float* logits, int nc, int B, int ncls, int64_t m0, int64_t M, double* acc, float* samples,
+                  float* mean, float* var, float* ent, int first, int last, cudaStream_t st) {
+  McAccumArgs a;
+  a.logits = logits; a.acc = acc; a.samples = samples; a.mean = mean; a.var = var; a.ent = ent;
+  a.B = B; a.ncls = ncls; a.nc = nc; a.first = first; a.last = last; a.m0 = m0; a.M = M;
+  launch_pdl(mc_accum_kernel, dim3(blocks_for((int64_t)B * 32, 128)), dim3(128), 0, st, a);
+  RD_CHECK_LAUNCH("mc_accum_kernel");
+  return 0;
+}
+
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st) {
   node_scale_kernel<<<blocks_for((int64_t)N * 32), TPB, 0, st>>>(edge_tgt, edge_w, E, N, s);
   RD_CHECK_LAUNCH("node_scale_kernel");
@@ -1401,9 +1559,12 @@ int layernorm_bwd(const float* x, const float* stats, const float* gamma, const 
 }
 
 int attn_softmax_fwd(float* S, const int64_t* lengths, int B, int H, int T, float drop_p, const uint64_t* rng,
-                     uint32_t site, float* Pd, cudaStream_t st) {
+                     uint32_t site, float* Pd, cudaStream_t st, DropRep rep) {
   int64_t rows = (int64_t)B * H * T;
-  attn_softmax_fwd_kernel<<<blocks_for(rows * 32), TPB, 0, st>>>(S, lengths, B, H, T, drop_p, rng, site, Pd);
+  if (Pd && drop_p > 0.f && rep.B)
+    attn_softmax_fwd_kernel<true><<<blocks_for(rows * 32), TPB, 0, st>>>(S, lengths, B, H, T, drop_p, rng, site, Pd, rep);
+  else
+    attn_softmax_fwd_kernel<false><<<blocks_for(rows * 32), TPB, 0, st>>>(S, lengths, B, H, T, drop_p, rng, site, Pd, rep);
   RD_CHECK_LAUNCH("attn_softmax_fwd_kernel");
   return 0;
 }

@@ -24,9 +24,10 @@ int assemble_batch(const float* P, const float* Pt, const float* Ps, const int64
 // round != 0: values are rounded (RN) to TF32 so the tensor-core layer reads them exactly.
 // The same launch writes the positional encoding of `times` into pe_out[tok*ld + col0 ..+16] (src == nullptr
 // or times == nullptr skips that half).
+// rep.B > 0: the lift dropout of replicate-major rows (rep_remap, rd_common.cuh).
 int lift_posenc(const float* src, const float* R_u, int B, int T, int N, int d_ob, float drop_p, const uint64_t* rng,
                 int round, float* X0, const float* times, int64_t n_tokens, const float* ts_host, int d_pe, float* pe_out,
-                int64_t ld, int col0, cudaStream_t st);
+                int64_t ld, int col0, cudaStream_t st, DropRep rep = {});
 
 // y [cols, rows] = RN_tf32(x [rows, cols])^T
 int transpose_round(const float* x, int rows, int cols, float* y, cudaStream_t st);
@@ -91,6 +92,16 @@ int kernel_shap_accumulate(const float* logits_c, const float* ends, const int64
 int kernel_shap_solve(const double* acc, const double* solve, const float* ends, const int64_t* target, int P, int B,
                       int ncls, float* attr, cudaStream_t st);
 
+// Monte Carlo dropout over chunks of nc replicates on B*nc rows, replicate-major (j = m*B + b).
+// mc_expand: src_e [T, B*nc, 2N], statics_e (ds > 0), times_e, lengths_e = nc copies of the batch.
+int mc_expand(const float* src, const float* statics, const float* times, const int64_t* lengths, int B, int nc, int T,
+              int N, int ds, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
+// mc_accumulate: adds replicates m0 .. m0+nc-1 (logits [B*nc, ncls]) to the fp64 sums acc [B, 2*ncls + 1] in replicate
+// order (first: from 0); samples (optional) [M, B, ncls] gets their logits; last: mean [B, ncls], var [B, ncls] and
+// ent [3, B] = (predictive entropy, expected entropy, mutual information) over all M replicates.
+int mc_accumulate(const float* logits, int nc, int B, int ncls, int64_t m0, int64_t M, double* acc, float* samples,
+                  float* mean, float* var, float* ent, int first, int last, cudaStream_t st);
+
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 
 // y = LN(x) * gamma + beta over the last dim (width D); stats[row] = {mean, rstd}
@@ -108,9 +119,9 @@ int layernorm_bwd(const float* x, const float* stats, const float* gamma, const 
                   const uint32_t* keep_bits = nullptr, int keep_ld = 0);   // keep_bits: decisions stored by the forward (else Philox)
 
 // in-place masked softmax over rows of S [B,H,T,T]; key j masked when j >= lengths[b].
-// If Pd != nullptr also writes the dropped probabilities (training).
+// If Pd != nullptr also writes the dropped probabilities (training; rep.B > 0: of replicate-major rows, rep_remap).
 int attn_softmax_fwd(float* S, const int64_t* lengths, int B, int H, int T, float drop_p,
-                     const uint64_t* rng, uint32_t site, float* Pd, cudaStream_t st);
+                     const uint64_t* rng, uint32_t site, float* Pd, cudaStream_t st, DropRep rep = {});
 // dS = P * (dP - sum_j dP_j P_j), dP = dPd * mask/(1-p); in place on dP
 int attn_softmax_bwd(const float* P, float* dP, int B, int H, int T, float drop_p, const uint64_t* rng,
                      uint32_t site, cudaStream_t st);
@@ -129,8 +140,9 @@ int head_bwd(int B, int T, int D, int N, int ds, int ncls, const int64_t* length
 
 // fused attention for short sequences (rd_attn_small.cu): ctx from qkv in one launch, dqkv in one launch
 bool attn_small_supported(int T, int hd);
+// rep.B > 0 (forwards): attention dropout of replicate-major rows (rep_remap, rd_common.cuh)
 int attn_small_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p,
-                   const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st);
+                   const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st, DropRep rep = {});
 int attn_small_bwd(const float* qkv, const float* dctx, const int64_t* lengths, int B, int H, int T, int hd,
                    float drop_p, const uint64_t* rng, uint32_t site, float* dqkv, cudaStream_t st);
 
@@ -138,7 +150,7 @@ int attn_small_bwd(const float* qkv, const float* dctx, const int64_t* lengths, 
 bool attn_tc_supported(int T, int hd);
 void attn_tc_set_debug(unsigned long long* buf);   // start / end clock64 stamps per CTA: [CTA][16], slots 0 and 12 (debug)
 int attn_tc_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p,
-                const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st);
+                const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st, DropRep rep = {});
 int attn_tc_bwd(const float* qkv, const float* dctx, const int64_t* lengths, int B, int H, int T, int hd,
                 float drop_p, const uint64_t* rng, uint32_t site, float* dqkv, cudaStream_t st);
 

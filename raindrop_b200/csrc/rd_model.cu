@@ -234,6 +234,35 @@ int coalition_layout(const rd_dims* dims, int n_players, int cc, CoalLayout* l) 
   return 0;
 }
 
+// ---- Monte Carlo dropout -------------------------------------------------------------------------------------------
+// A chunk of cc replicates is one training-mode forward on B*cc replicate-major rows.  Its ob-prop arithmetic is pinned
+// from the full chunk's row count, as for integrated gradients, so a ragged tail chunk cannot switch it.
+rd_dims mc_dims(const rd_dims* d, int rows, int cc) {
+  rd_dims e = ig_dims(d, rows, cc);
+  e.training = 1;
+  return e;
+}
+// Scratch of rd_raindrop_v2_mc_dropout: the training forward workspace of B*cc rows, the expanded inputs, the chunk's
+// logits and the fp64 sums [B, 2*n_classes + 1].
+struct McLayout { int64_t ws, src, statics, times, lengths, logits, acc, total; };
+int mc_layout(const rd_dims* dims, int cc, McLayout* l) {
+  if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("replicates_per_chunk = %d out of range", cc); return -2; }
+  const int Bc = dims->B * cc;
+  const rd_dims dc = mc_dims(dims, Bc, cc);
+  Shape sc;
+  RD_TRY(make_shape(&dc, &sc));
+  Arena a;
+  l->ws = a.take(ws_layout(sc).total);
+  l->src = a.take(sc.M2 * 2 * sc.N);
+  l->statics = a.take((int64_t)Bc * sc.ds);
+  l->times = a.take(sc.M2);
+  l->lengths = a.take(2LL * Bc);
+  l->logits = a.take((int64_t)Bc * sc.ncls);
+  l->acc = a.take(2LL * dims->B * (2 * sc.ncls + 1));
+  l->total = a.off;
+  return 0;
+}
+
 // Y[M,N] = epi(X[M,K] . W[N,K]^T)
 GemmP nt(const float* X, int64_t ldx, const float* W, int64_t ldw, float* Y, int64_t ldy, int64_t M, int N, int K) {
   GemmP g;
@@ -302,7 +331,7 @@ static int linear_nt(const GemmP& g, const float* W_lo, cudaStream_t st) {
   a.A = g.A; a.lda = g.sAi; a.B = g.B; a.B_lo = W_lo; a.M = g.M; a.N = g.N; a.K = g.K; a.C = g.C;
   a.bias = g.bias; a.relu = g.relu; a.gate = g.gate; a.gate_ld = g.gate_ld; a.gate_scale = g.gate_scale;
   a.drop_p = g.drop_p; a.rng = g.rng; a.drop_site = g.drop_site; a.resid = g.resid; a.resid_ld = g.resid_ld;
-  a.drop_mask = g.drop_mask; a.drop_mask_ld = g.drop_mask_ld;
+  a.drop_mask = g.drop_mask; a.drop_mask_ld = g.drop_mask_ld; a.rep = g.rep;
   const bool plain = g.ta == 0 && g.tb == 1 && g.sBj == g.K && g.sCi == g.N && g.sCj == 1 && g.nz == 1 && g.nsplit == 1 &&
                      g.alpha == 1.f && !g.rowscale && !g.perm && !g.asum;
   if (plain && W_lo && tc_gemm_supported(a)) return tc_gemm(a, st);
@@ -343,10 +372,13 @@ static int input_grad_dx0(const Shape& s, const rd_params* P, const float* gO1, 
   return gemm(nn(gO1, s.C, P->ob1_value_weight, s.C, dX0, s.C, s.M1, s.C, s.C), st);
 }
 
+// rep_B > 0 (Monte Carlo dropout, training dims): the dims->B rows are replicate-major copies of a rep_B-row batch, row
+// j = m*rep_B + b drawing the dropout words of row b of the rep_B-row forward at step (rng_state[1] + rep_step + m)
+// (rep_remap); rng_state is read, never advanced.
 static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* src, const float* statics,
                         const float* times, const int64_t* lengths, const float* nscale, uint64_t* rng_state,
                         float* ws, float* logits, const int64_t* y, float* loss, float* d_logits, int encoder_only,
-                        cudaStream_t st) {
+                        cudaStream_t st, int rep_B = 0, uint64_t rep_step = 0) {
   Shape s;
   RD_TRY(make_shape(dims, &s));
   if (!encoder_only && (s.dpe != RD_D_PE || s.emb != s.N)) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
@@ -358,7 +390,9 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
   if (y && (!loss || !d_logits)) { set_error("labels given without loss / d_logits outputs"); return -2; }
   // rides along with the first weight-prep launch: dropout-stream capture (+ advance) and the loss ticket reset
   StepPrologue pro;
-  if (s.p > 0.f) { pro.rng_state = rng_state; pro.rng_captured = rng; pro.advance = 1; }
+  if (s.p > 0.f) { pro.rng_state = rng_state; pro.rng_captured = rng; pro.advance = rep_B ? 0 : 1; pro.step_offset = rep_step; }
+  DropRep rep;
+  if (rep_B > 0 && s.B > rep_B && s.p > 0.f) { rep.B = rep_B; rep.Bc = s.B; }   // one replicate: the remap is the identity
   pro.zero_counter = reinterpret_cast<unsigned*>(ws + w.cnt);
   float* X0 = ws + w.X0; float* H1 = ws + w.H1;
   // Fast mode: tensor-core operands are kept exactly TF32-representable by their producers (lift, layer-1 epilogue,
@@ -391,7 +425,7 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
   if (!encoder_only) {
   // lift of the raw observations and the positional encoding (written into Z0[..., 4N:]) in one launch
   RD_TRY(lift_posenc(src, P->R_u, s.B, s.T, s.N, s.dob, s.p, rng, tc && !exact, X0, times, s.M2, dims->pe_timescales, RD_D_PE, Z0,
-                     s.D, s.Dm, st));
+                     s.D, s.Dm, st, rep));
   {
     ObpropTcArgs a;
     a.x = X0; a.W = W1; a.bias = P->ob1_value_bias; a.scale = nscale; a.scale_mod = s.N;
@@ -421,9 +455,9 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
     }
     float* ctx = ws + w.l[l].ctx;
     if (attn_tc_supported(s.T, s.hd)) {
-      RD_TRY(attn_tc_fwd(qkv, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, ctx, st));
+      RD_TRY(attn_tc_fwd(qkv, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, ctx, st, rep));
     } else if (attn_small_supported(s.T, s.hd)) {
-      RD_TRY(attn_small_fwd(qkv, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, ctx, st));
+      RD_TRY(attn_small_fwd(qkv, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, ctx, st, rep));
     } else {
       {  // S[b,h] = scale * Q K^T
         GemmP g;
@@ -433,7 +467,7 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
         g.M = s.T; g.N = s.T; g.K = s.hd; g.nz = s.B * s.H; g.nz_inner = s.H; g.alpha = scale;
         RD_TRY(gemm(g, st));
       }
-      RD_TRY(attn_softmax_fwd(Pm, lengths, s.B, s.H, s.T, s.p, rng, SITE_ATTN + l, Pd, st));
+      RD_TRY(attn_softmax_fwd(Pm, lengths, s.B, s.H, s.T, s.p, rng, SITE_ATTN + l, Pd, st, rep));
       {  // ctx[b,h] = P V
         GemmP g;
         g.A = Pd ? Pd : Pm; g.ta = 0; g.sAi = s.T; g.sAk = 1; g.sAzo = s.H * TT; g.sAzi = TT;
@@ -446,7 +480,7 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
     float* r1 = ws + w.l[l].r1; float* x1 = ws + w.l[l].x1;
     {
       GemmP g = nt(ctx, s.D, E.out_proj_weight, s.D, r1, s.D, s.M2, s.D, s.D);
-      g.bias = E.out_proj_bias; g.drop_p = s.p; g.rng = rng; g.drop_site = SITE_RESID1 + l;
+      g.bias = E.out_proj_bias; g.drop_p = s.p; g.rng = rng; g.drop_site = SITE_RESID1 + l; g.rep = rep;
       g.resid = x; g.resid_ld = s.D;
       if (s.p > 0.f) { g.drop_mask = reinterpret_cast<uint32_t*>(ws + w.l[l].m1); g.drop_mask_ld = (s.D + 31) / 32; }
       RD_TRY(linear_nt(g, ws + w.wsp[l].out_lo, st));
@@ -455,12 +489,12 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
     float* f = ws + w.l[l].f; float* r2 = ws + w.l[l].r2;
     {
       GemmP g = nt(x1, s.D, E.linear1_weight, s.D, f, s.nhid, s.M2, s.nhid, s.D);
-      g.bias = E.linear1_bias; g.relu = 1; g.drop_p = s.p; g.rng = rng; g.drop_site = SITE_FFN + l;
+      g.bias = E.linear1_bias; g.relu = 1; g.drop_p = s.p; g.rng = rng; g.drop_site = SITE_FFN + l; g.rep = rep;
       RD_TRY(linear_nt(g, ws + w.wsp[l].l1_lo, st));
     }
     {
       GemmP g = nt(f, s.nhid, E.linear2_weight, s.nhid, r2, s.D, s.M2, s.D, s.nhid);
-      g.bias = E.linear2_bias; g.drop_p = s.p; g.rng = rng; g.drop_site = SITE_RESID2 + l;
+      g.bias = E.linear2_bias; g.drop_p = s.p; g.rng = rng; g.drop_site = SITE_RESID2 + l; g.rep = rep;
       g.resid = x1; g.resid_ld = s.D;
       if (s.p > 0.f) { g.drop_mask = reinterpret_cast<uint32_t*>(ws + w.l[l].m2); g.drop_mask_ld = (s.D + 31) / 32; }
       RD_TRY(linear_nt(g, ws + w.wsp[l].l2_lo, st));
@@ -1130,6 +1164,56 @@ int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, con
   } while (c0 < M);
   // 3. attr = acc . K^T + (F(x) - F(x')) k^T
   return kernel_shap_solve(r.acc, solve, endpoint_logits, target, P, B, r.s0.ncls, attr, st);
+}
+
+size_t rd_mc_dropout_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk) {
+  if (!dims) return 0;
+  McLayout l;
+  if (mc_layout(dims, replicates_per_chunk, &l) != 0) return 0;
+  return (size_t)l.total * sizeof(float);
+}
+
+// Chunks of cc replicates: the inputs expanded when the chunk size changes (the first and a ragged last chunk), one
+// training forward whose dropout draws replicate m0 + m at step rng[1] + m0 + m (the prologue captures {seed, step + m0},
+// rep_remap adds m), and one launch that adds the chunk to the fp64 sums and, after the last chunk, writes the statistics.
+int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                              const float* times, const int64_t* lengths, const float* node_scale, const uint64_t* rng,
+                              int32_t n_samples, int32_t replicates_per_chunk, void* scratch, float* mean_probs,
+                              float* variance, float* entropies, float* samples, void* stream) {
+  const char* fn = "rd_raindrop_v2_mc_dropout";
+  if (!dims || !params || !src || !times || !lengths || !node_scale || !rng || !scratch || !mean_probs || !variance ||
+      !entropies || !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (n_samples < 1 || replicates_per_chunk < 1) { set_error("%s: n_samples and replicates_per_chunk must be >= 1", fn); return -2; }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s0.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  McLayout l;
+  RD_TRY(mc_layout(dims, replicates_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, cc = replicates_per_chunk;
+  const int64_t M = n_samples;
+  float* S = (float*)scratch;
+  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
+  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  double* acc = reinterpret_cast<double*>(S + l.acc);
+  int expanded = 0;
+  for (int64_t c0 = 0; c0 < M; c0 += cc) {
+    const int nc = (int)(M - c0 < cc ? M - c0 : cc);
+    const rd_dims dc = mc_dims(dims, B * nc, cc);
+    if (nc != expanded) {
+      RD_TRY(mc_expand(src, statics, times, lengths, B, nc, s0.T, s0.N, s0.ds, src_e, stat_e, times_e, len_e, st));
+      expanded = nc;
+    }
+    RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, const_cast<uint64_t*>(rng), S + l.ws,
+                        S + l.logits, nullptr, nullptr, nullptr, 0, st, B, (uint64_t)c0));
+    RD_TRY(mc_accumulate(S + l.logits, nc, B, s0.ncls, c0, M, acc, samples, mean_probs, variance, entropies, c0 == 0,
+                         c0 + nc >= M, st));
+  }
+  return 0;
 }
 
 int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,

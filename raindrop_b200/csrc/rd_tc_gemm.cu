@@ -32,7 +32,8 @@ constexpr int NCH_MAX = 8;                 // 32-column accumulator chunks per t
 constexpr int A_TILE = BM * BK * 4;        // 16 KB
 constexpr int MAX_BN = 160;                // encoder GEMMs: narrower tiles spread the small problems over more SMs
 
-enum : int { F_RELU = 1, F_SCALE = 2, F_GATE = 4, F_DROP = 8, F_RESID = 16, F_ROUND = 32, F_PERM = 64 };
+// F_REP: dropout of replicate-major rows (rep_remap), instantiated only with F_DROP for the Monte Carlo dropout forward
+enum : int { F_RELU = 1, F_SCALE = 2, F_GATE = 4, F_DROP = 8, F_RESID = 16, F_ROUND = 32, F_PERM = 64, F_REP = 128 };
 
 struct NtP {
   long long M; int N, K, BN, nch, n_tiles, m_tiles, k_blocks, nstages;
@@ -40,7 +41,7 @@ struct NtP {
   const float* bias;
   const float* scale; int scale_mod;
   const float* gate; long long gate_ld; float gate_scale;
-  float drop_p; const uint64_t* rng; uint32_t drop_site;
+  float drop_p; const uint64_t* rng; uint32_t drop_site; DropRep rep;
   uint32_t* drop_mask; int drop_mask_ld;
   const float* resid; long long resid_ld;
   int pB, pN, pD;
@@ -189,6 +190,12 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     // ---- epilogue on the accumulator registers: element (row0 + 8i, col0 + 32c + 8j + 2t + {0, 1}) ----
     const long long row0 = (long long)m_t * BM + arow;
     const int col0 = n_t * p.BN;
+    RngKey rkey[2] = {key, key};      // replicate rows: key and B-row index of column 0 of this thread's two rows
+    uint64_t rbase[2] = {0, 0};
+    if (F & F_REP) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) rbase[i] = rep_remap(p.rng, p.rep, (uint32_t)(row0 + 8 * i), (uint64_t)p.N, 0, &rkey[i]);
+    }
     float sc[2] = {1.f, 1.f};
     if (F & F_SCALE) {
 #pragma unroll
@@ -218,8 +225,8 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             v1 = gv.y > 0.f ? v1 * p.gate_scale : 0.f;
           }
           if (F & F_DROP) {   // element index row*N + col; N % 4 == 0, so the pair shares one Philox block
-            const uint64_t idx = (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
-            const uint4 u = dropout_block(key, p.drop_site, idx);
+            const uint64_t idx = (F & F_REP) ? rbase[i] + (uint64_t)col : (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
+            const uint4 u = dropout_block((F & F_REP) ? rkey[i] : key, p.drop_site, idx);
             const bool lo_half = (idx & 3u) == 0;
             const float m0 = keep_scale(lo_half ? u.x : u.z, p.drop_p, ik), m1 = keep_scale(lo_half ? u.y : u.w, p.drop_p, ik);
             v0 *= m0; v1 *= m1;
@@ -484,7 +491,7 @@ __global__ void split_weights_kernel(const __grid_constant__ SplitItems s) {
   if (i == 0) {     // step prologue riding along: dropout counter capture (+ advance) and ticket reset
     if (s.pro.rng_state) {
       s.pro.rng_captured[0] = s.pro.rng_state[0];
-      s.pro.rng_captured[1] = s.pro.rng_state[1];
+      s.pro.rng_captured[1] = s.pro.rng_state[1] + s.pro.step_offset;
       if (s.pro.advance) s.pro.rng_state[1] = s.pro.rng_state[1] + 1;
     }
     if (s.pro.zero_counter) *s.pro.zero_counter = 0u;
@@ -546,6 +553,7 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
   p.bias = a.bias; p.scale = a.scale; p.scale_mod = a.scale_mod > 0 ? a.scale_mod : 1;
   p.gate = a.gate; p.gate_ld = a.gate_ld; p.gate_scale = a.gate_scale;
   p.drop_p = a.drop_p; p.rng = a.rng; p.drop_site = a.drop_site; p.drop_mask = a.drop_mask; p.drop_mask_ld = a.drop_mask_ld;
+  p.rep = a.rep;
   p.resid = a.resid; p.resid_ld = a.resid_ld;
   p.pB = a.pB; p.pN = a.pN; p.pD = a.pD;
   p.dbg = g_gemm_dbg;
@@ -568,7 +576,8 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < num_sms() ? total : num_sms();
   const int f = (a.relu ? F_RELU : 0) | (a.scale ? F_SCALE : 0) | (a.gate ? F_GATE : 0) | (a.drop_p > 0.f ? F_DROP : 0) |
-                (a.resid ? F_RESID : 0) | (a.round_out ? F_ROUND : 0) | (a.perm ? F_PERM : 0);
+                (a.resid ? F_RESID : 0) | (a.round_out ? F_ROUND : 0) | (a.perm ? F_PERM : 0) |
+                (a.drop_p > 0.f && a.rep.B ? F_REP : 0);
   auto launch = [&](auto kern) -> int {
     RD_TRY(ensure_max_smem((const void*)kern, SMEM_LIMIT));   // once per (instantiation, device)
     launch_pdl(kern, dim3(grid), dim3(NT_THREADS), smem_bytes, st, tmA, tmB, tmBlo, p);
@@ -593,6 +602,8 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
   RD_NT_CASE(F_GATE, true)
   RD_NT_CASE(F_RELU, true)
   RD_NT_CASE(F_RELU | F_DROP, true)
+  RD_NT_CASE(F_DROP | F_RESID | F_REP, true)       // Monte Carlo dropout replicates: dropout1, dropout2, the FFN
+  RD_NT_CASE(F_RELU | F_DROP | F_REP, true)
   { set_error("tc_nt: epilogue combination %d (exact=%d) not instantiated", f, (int)exact); return -2; }
 #undef RD_NT_CASE
   if (rc != 0) return rc;
@@ -619,7 +630,7 @@ int tc_gemm(const TcGemmArgs& a, cudaStream_t st) {
   n.A = a.A; n.lda = a.lda; n.B = a.B; n.B_lo = a.B_lo; n.M = a.M; n.N = a.N; n.K = a.K; n.C = a.C;
   plan(a.M, a.N, &n.BN, &n.n_tiles);
   n.bias = a.bias; n.relu = a.relu; n.gate = a.gate; n.gate_ld = a.gate_ld; n.gate_scale = a.gate_scale;
-  n.drop_p = a.drop_p; n.rng = a.rng; n.drop_site = a.drop_site; n.drop_mask = a.drop_mask; n.drop_mask_ld = a.drop_mask_ld;
+  n.drop_p = a.drop_p; n.rng = a.rng; n.drop_site = a.drop_site; n.rep = a.rep; n.drop_mask = a.drop_mask; n.drop_mask_ld = a.drop_mask_ld;
   n.resid = a.resid; n.resid_ld = a.resid_ld;
   return tc_nt(n, st);
 }

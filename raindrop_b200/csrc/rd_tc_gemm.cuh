@@ -18,7 +18,7 @@ struct TcNtArgs {
   const float* bias = nullptr; int relu = 0;
   const float* scale = nullptr; int scale_mod = 1;
   const float* gate = nullptr; long long gate_ld = 0; float gate_scale = 1.f;
-  float drop_p = 0.f; const uint64_t* rng = nullptr; uint32_t drop_site = 0;
+  float drop_p = 0.f; const uint64_t* rng = nullptr; uint32_t drop_site = 0; DropRep rep;
   uint32_t* drop_mask = nullptr; int drop_mask_ld = 0;
   const float* resid = nullptr; long long resid_ld = 0;
   int round_out = 0;
@@ -39,6 +39,7 @@ struct TcGemmArgs {
   const float* bias = nullptr; int relu = 0;
   const float* gate = nullptr; long long gate_ld = 0; float gate_scale = 1.f;
   float drop_p = 0.f; const uint64_t* rng = nullptr; uint32_t drop_site = 0;
+  DropRep rep;                                               // replicate rows: dropout drawn through rep_remap
   uint32_t* drop_mask = nullptr; int drop_mask_ld = 0;      // optional: keep bits of the dropout decisions, word [row*ld + col/32]
   const float* resid = nullptr; long long resid_ld = 0;
 };
@@ -66,9 +67,10 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
 // One launch for all weights of a step: lo = W - trunc19(W); t = W^T; t_lo = W^T - trunc19(W^T).
 // optional extras for the single-pass-TF32 layers: rn = RN_tf32(W), rn_t = RN_tf32(W)^T
 struct WeightSplit { const float* w; int rows, cols; float* lo; float* t; float* t_lo; float* rn = nullptr; float* rn_t = nullptr; };
-// Optional step prologue done by thread 0 of the same launch: capture {seed, counter} of the dropout stream into
-// rng_captured (advance != 0: counter += 1 afterwards) and zero one ticket word.
-struct StepPrologue { uint64_t* rng_state = nullptr; uint64_t* rng_captured = nullptr; int advance = 0; unsigned* zero_counter = nullptr; };
+// Optional step prologue done by thread 0 of the same launch: capture {seed, counter + step_offset} of the dropout stream
+// into rng_captured (advance != 0: counter += 1 afterwards) and zero one ticket word.
+struct StepPrologue { uint64_t* rng_state = nullptr; uint64_t* rng_captured = nullptr; int advance = 0; unsigned* zero_counter = nullptr;
+                      uint64_t step_offset = 0; };
 int split_weights(const WeightSplit* items, int n, cudaStream_t st, const StepPrologue* pro = nullptr);   // n <= 16
 
 }  // namespace rd

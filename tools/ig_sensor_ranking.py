@@ -42,8 +42,9 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 
-def model_from_state_dict(sd, nhead, seed, device):
-    """Raindrop_v2 with the hyper-parameters the state dict's shapes give (code/Raindrop.py:245-251), weights loaded."""
+def model_from_state_dict(sd, nhead, seed, device, dropout=0.0):
+    """Raindrop_v2 with the hyper-parameters the state dict's shapes give (code/Raindrop.py:245-251), weights loaded.
+    The dropout probability is not in the state dict; it only matters for training-mode forwards."""
     from raindrop_b200.models_rd import Raindrop_v2
     static = "emb.weight" in sd
     d_inp, C = sd["ob_propagation.nodewise_weights"].shape          # [n_nodes, T * d_ob]
@@ -55,7 +56,7 @@ def model_from_state_dict(sd, nhead, seed, device):
     n_classes = sd["mlp_static.2.weight"].shape[0]
     torch.manual_seed(seed)
     kw = {} if static else {"static": False}
-    m = Raindrop_v2(d_inp, d_model, nhead, nhid, nlayers, 0.0, C // d_ob, d_static, 100, 0.5, "mean", n_classes,
+    m = Raindrop_v2(d_inp, d_model, nhead, nhid, nlayers, dropout, C // d_ob, d_static, 100, 0.5, "mean", n_classes,
                     torch.ones(d_inp, d_inp), **kw)
     m.load_state_dict(sd)
     return m.to(device).eval()

@@ -20,21 +20,6 @@
 
 namespace rd {
 using namespace tc;
-namespace {
-
-// max_bn: widest n-tile (256 for the single-pass kernel; the error-compensated kernel does 3x the MMAs per tile and
-// takes 128, so that more CTAs share the work of the latency-bound sizes it runs at)
-void plan_n(int C, int max_bn, int* BN, int* n_tiles) {
-  if (C <= max_bn) { *n_tiles = 1; *BN = (int)round_up(C, 32); return; }
-  int best_bn = max_bn, best_nt = (int)ceil_div(C, max_bn), best_pad = best_nt * max_bn;
-  for (int bn = max_bn; bn >= max_bn / 2; bn -= 32) {   // BN % 32 == 0: whole 32-column MMA chunks
-    int nt = (int)ceil_div(C, bn);
-    if (nt * bn < best_pad) { best_pad = nt * bn; best_bn = bn; best_nt = nt; }
-  }
-  *BN = best_bn; *n_tiles = best_nt;
-}
-
-}  // namespace
 
 bool obprop_tc_supported(int C) {
   static int env = -1;
@@ -75,7 +60,7 @@ int obprop_tc_fwd(const ObpropTcArgs& a, cudaStream_t st) {
   if (exact && a.round_out) { set_error("obprop_tc_fwd: the error-compensated mode does not round its output"); return -2; }
   TcNtArgs n;
   n.A = a.x; n.lda = a.C; n.B = a.W; n.B_lo = a.W_lo; n.M = a.rows; n.N = a.C; n.K = a.C; n.C = a.out;
-  plan_n(a.C, exact ? 128 : 256, &n.BN, &n.n_tiles);
+  tc_nt_plan(a.rows, a.C, exact, &n.BN, &n.n_tiles);
   n.bias = a.bias; n.relu = a.relu; n.scale = a.scale; n.scale_mod = a.scale_mod;
   n.gate = a.gate; n.gate_ld = a.C; n.round_out = a.round_out;
   n.perm = a.perm; n.pB = a.pB; n.pN = a.pN; n.pD = a.pD;

@@ -79,24 +79,13 @@ __device__ __forceinline__ void mma_tf32x3(float (&d)[4], const uint32_t (&ah)[4
   mma_tf32(d, ah, bh0, bh1);
 }
 
-// ---- warpgroup MMA (wgmma): D[64 x 32] += A[64 x 8] (registers) . B[32 x 8]^T (shared memory, K-major) ----------------
+// ---- warpgroup MMA (wgmma) synchronisation; the TF32 MMA itself, wgmma_tf32<N>, is in rd_wgmma_tf32.cuh -------------
 // A fragment of warp w of the warpgroup: rows 16w .. 16w+15, same (g, t) layout as mma_tf32 above.
-// Accumulator: d[4j + 0/1] = (16w + g, 8j + 2t + 0/1), d[4j + 2/3] = (16w + g + 8, 8j + 2t + 0/1), j < 4.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
-
-__device__ __forceinline__ void wgmma_n32_tf32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
-  asm volatile(
-      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1;"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
-      : "memory");
-}
 
 // shared-memory matrix descriptor of a K-major tile written by TMA with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128 bytes
 // (32 fp32 of K), 8-row groups 1024 bytes apart (SBO), layout type 1 = 128-byte swizzle.  Moving along K inside the

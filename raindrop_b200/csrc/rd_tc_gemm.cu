@@ -6,10 +6,12 @@
 //   warpgroup 2   TMA producer (one thread): A tile [128 x 32] and B tile [BN x 32] (+ its precomputed remainder B_lo)
 //                 per k-block into a <= 4-stage ring of 128B-swizzled shared memory, one mbarrier per stage and
 //                 direction.  It hands its registers to the MMA warpgroups (setmaxnreg 40 / 232).
-//   warpgroups    0 and 1, rows 0-63 and 64-127 of the tile: wgmma.m64n32k8 TF32 with A from REGISTERS and B from
-//                 shared memory, fp32 accumulators in registers (BN <= 256 -> <= 128 per thread).  A is split into
-//                 hi = top 19 bits and lo = the exact remainder in registers, so the error-compensated mode needs no
-//                 remainder image of the activations: every k-step issues lo.hi + hi.lo + hi.hi.  The epilogue (bias,
+//   warpgroups    0 and 1, rows 0-63 and 64-127 of the tile: one wgmma.m64nBNk8 TF32 per k-step and term across the
+//                 whole tile width (BN a template parameter), A from REGISTERS and B from shared memory, fp32
+//                 accumulators in registers (BN / 2 per thread).  A is split into hi = top 19 bits and lo = the exact
+//                 remainder in registers, so the error-compensated mode needs no remainder image of the activations:
+//                 every k-step issues lo.hi + hi.lo + hi.hi.  One wgmma group stays in flight while the A fragments of
+//                 the next k-block are loaded into a second register buffer.  The epilogue (bias,
 //                 relu, row scale, gate, dropout + keep bits, residual, TF32 rounding, permuted store) runs on the
 //                 accumulator registers and stores straight to global memory; meanwhile the producer already fills
 //                 the ring for the next tile.
@@ -21,6 +23,7 @@
 
 #include "rd_tc_common.cuh"
 #include "rd_tc_gemm.cuh"
+#include "rd_wgmma_tf32.cuh"
 
 namespace rd {
 using namespace tc;
@@ -28,15 +31,14 @@ namespace {
 
 constexpr int BM = 128, BK = 32, MAX_STAGES = 4;
 constexpr int NT_THREADS = 384;            // warpgroups 0, 1: MMA + epilogue; warpgroup 2: TMA producer
-constexpr int NCH_MAX = 8;                 // 32-column accumulator chunks per tile: BN <= 256
 constexpr int A_TILE = BM * BK * 4;        // 16 KB
-constexpr int MAX_BN = 160;                // encoder GEMMs: narrower tiles spread the small problems over more SMs
+constexpr int MAX_BN = 160;                // weight gradients: widest n tile
 
 // F_REP: dropout of replicate-major rows (rep_remap), instantiated only with F_DROP for the Monte Carlo dropout forward
 enum : int { F_RELU = 1, F_SCALE = 2, F_GATE = 4, F_DROP = 8, F_RESID = 16, F_ROUND = 32, F_PERM = 64, F_REP = 128 };
 
 struct NtP {
-  long long M; int N, K, BN, nch, n_tiles, m_tiles, k_blocks, nstages;
+  long long M; int N, K, n_tiles, m_tiles, k_blocks, nstages;
   float* C; long long ldc;
   const float* bias;
   const float* scale; int scale_mod;
@@ -62,27 +64,45 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
   return v;
 }
 
-template <int NCH, bool EXACT>
-__device__ __forceinline__ void issue_kblock(float (&acc)[NCH_MAX][16], const uint32_t (&ah)[BK / 8][4],
+// one k-block: per 8-wide k-step one wgmma across the whole tile width per term, small terms first (lo.hi, hi.lo, hi.hi)
+template <int BN, bool EXACT>
+__device__ __forceinline__ void issue_kblock(float (&acc)[BN / 2], const uint32_t (&ah)[BK / 8][4],
                                              const uint32_t (&al)[BK / 8][4], uint32_t sb, uint32_t b_tile) {
+#pragma unroll
+  for (int e = 0; e < BN / 2; ++e) fence_operand(acc[e]);
   wgmma_fence();
 #pragma unroll
   for (int ks = 0; ks < BK / 8; ++ks) {
+    const uint32_t bo = sb + (uint32_t)ks * 32u;
+    const uint64_t bh = wgmma_desc_sw128(bo);
+    if (EXACT) {
+      wgmma_tf32<BN>(acc, al[ks], bh);
+      wgmma_tf32<BN>(acc, ah[ks], wgmma_desc_sw128(bo + b_tile));
+    }
+    wgmma_tf32<BN>(acc, ah[ks], bh);
+  }
+  wgmma_commit();
+}
+
+// A fragments of one k-block from the swizzled stage, split into hi / lo in the error-compensated mode
+template <bool EXACT>
+__device__ __forceinline__ void load_afrag(uint32_t sa, int arow, int t, uint32_t (&ah)[BK / 8][4], uint32_t (&al)[BK / 8][4]) {
 #pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const uint32_t bo = sb + (uint32_t)c * 4096u + (uint32_t)ks * 32u;
-      const uint64_t bh = wgmma_desc_sw128(bo);
-      if (EXACT) {
-        const uint64_t bl = wgmma_desc_sw128(bo + b_tile);
-        wgmma_n32_tf32(acc[c], al[ks], bh);       // small terms first
-        wgmma_n32_tf32(acc[c], ah[ks], bl);
-      }
-      wgmma_n32_tf32(acc[c], ah[ks], bh);
+  for (int ks = 0; ks < BK / 8; ++ks) {
+    const int col = ks * 8 + t;
+    const float x0 = lds_f32(sa + sw128_offset(arow, col)), x1 = lds_f32(sa + sw128_offset(arow + 8, col));
+    const float x2 = lds_f32(sa + sw128_offset(arow, col + 4)), x3 = lds_f32(sa + sw128_offset(arow + 8, col + 4));
+    if (EXACT) {
+      ah[ks][0] = tf32_hi(x0); ah[ks][1] = tf32_hi(x1); ah[ks][2] = tf32_hi(x2); ah[ks][3] = tf32_hi(x3);
+      al[ks][0] = tf32_lo(x0); al[ks][1] = tf32_lo(x1); al[ks][2] = tf32_lo(x2); al[ks][3] = tf32_lo(x3);
+    } else {   // single pass: the producers keep these operands TF32-representable
+      ah[ks][0] = __float_as_uint(x0); ah[ks][1] = __float_as_uint(x1);
+      ah[ks][2] = __float_as_uint(x2); ah[ks][3] = __float_as_uint(x3);
     }
   }
 }
 
-template <int F, bool EXACT>
+template <int F, bool EXACT, int BN>
 __global__ void __launch_bounds__(NT_THREADS, 1)
 tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmBlo, const NtP p) {
@@ -90,8 +110,8 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   pdl_launch_dependents();
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t b_tile = (uint32_t)p.BN * 128u;
-  const uint32_t stage_bytes = (uint32_t)A_TILE + (EXACT ? 2u : 1u) * b_tile;     // A | B hi [| B lo]
+  constexpr uint32_t b_tile = (uint32_t)BN * 128u;
+  constexpr uint32_t stage_bytes = (uint32_t)A_TILE + (EXACT ? 2u : 1u) * b_tile;     // A | B hi [| B lo]
   const uint32_t bar_base = base + (uint32_t)p.nstages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (MAX_STAGES + s); };
@@ -120,8 +140,8 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           mbar_expect_tx(full_bar(stage), stage_bytes);
           const uint32_t sa = base + (uint32_t)stage * stage_bytes;
           tma_load_2d(&tmA, full_bar(stage), sa, kb * BK, m_t * BM);
-          tma_load_2d(&tmB, full_bar(stage), sa + A_TILE, kb * BK, n_t * p.BN);
-          if (EXACT) tma_load_2d(&tmBlo, full_bar(stage), sa + A_TILE + b_tile, kb * BK, n_t * p.BN);
+          tma_load_2d(&tmB, full_bar(stage), sa + A_TILE, kb * BK, n_t * BN);
+          if (EXACT) tma_load_2d(&tmBlo, full_bar(stage), sa + A_TILE + b_tile, kb * BK, n_t * BN);
           if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -135,61 +155,49 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int arow = wg * 64 + wq * 16 + g;              // tile-local row of fragment elements a0 / a2
   const float ik = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
   const RngKey key = load_rng_key((F & F_DROP) ? p.rng : nullptr);
-  int stage = 0; uint32_t phase = 0;
+  int stage = 0, rstage = 0; uint32_t phase = 0;
+  // the next full stage -> A fragments; returns the stage's B tile address
+  auto acquire = [&](uint32_t (&ah)[BK / 8][4], uint32_t (&al)[BK / 8][4]) {
+    mbar_wait(full_bar(stage), phase);
+    const uint32_t sa = base + (uint32_t)stage * stage_bytes;
+    load_afrag<EXACT>(sa, arow, t, ah, al);
+    if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
+    return sa + (uint32_t)A_TILE;
+  };
+  // the oldest stage still held: every wgmma that read it has retired
+  auto release = [&]() {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_bar(rstage));
+    if (++rstage == p.nstages) rstage = 0;
+  };
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int m_t = tile / p.n_tiles, n_t = tile - m_t * p.n_tiles;
-    float acc[NCH_MAX][16];
+    float acc[BN / 2];
 #pragma unroll
-    for (int c = 0; c < NCH_MAX; ++c)
-#pragma unroll
-      for (int e = 0; e < 16; ++e) acc[c][e] = 0.f;
-    for (int kb = 0; kb < p.k_blocks; ++kb) {
-      mbar_wait(full_bar(stage), phase);
-      const uint32_t sa = base + (uint32_t)stage * stage_bytes, sb = sa + A_TILE;
-      uint32_t ah[BK / 8][4], al[BK / 8][4];
-#pragma unroll
-      for (int ks = 0; ks < BK / 8; ++ks) {
-        const int col = ks * 8 + t;
-        const float x0 = lds_f32(sa + sw128_offset(arow, col)), x1 = lds_f32(sa + sw128_offset(arow + 8, col));
-        const float x2 = lds_f32(sa + sw128_offset(arow, col + 4)), x3 = lds_f32(sa + sw128_offset(arow + 8, col + 4));
-        if (EXACT) {
-          ah[ks][0] = tf32_hi(x0); ah[ks][1] = tf32_hi(x1); ah[ks][2] = tf32_hi(x2); ah[ks][3] = tf32_hi(x3);
-          al[ks][0] = tf32_lo(x0); al[ks][1] = tf32_lo(x1); al[ks][2] = tf32_lo(x2); al[ks][3] = tf32_lo(x3);
-        } else {   // single pass: the producers keep these operands TF32-representable
-          ah[ks][0] = __float_as_uint(x0); ah[ks][1] = __float_as_uint(x1);
-          ah[ks][2] = __float_as_uint(x2); ah[ks][3] = __float_as_uint(x3);
-        }
-      }
-#pragma unroll
-      for (int c = 0; c < NCH_MAX; ++c)
-#pragma unroll
-        for (int e = 0; e < 16; ++e) fence_operand(acc[c][e]);
-      // the chunk count is a compile-time constant of each issue sequence: a runtime guard between the wgmma
-      // instructions makes ptxas fence (serialise) them
-      switch (p.nch) {
-        case 1: issue_kblock<1, EXACT>(acc, ah, al, sb, b_tile); break;
-        case 2: issue_kblock<2, EXACT>(acc, ah, al, sb, b_tile); break;
-        case 3: issue_kblock<3, EXACT>(acc, ah, al, sb, b_tile); break;
-        case 4: issue_kblock<4, EXACT>(acc, ah, al, sb, b_tile); break;
-        case 5: issue_kblock<5, EXACT>(acc, ah, al, sb, b_tile); break;
-        case 6: issue_kblock<6, EXACT>(acc, ah, al, sb, b_tile); break;
-        case 7: issue_kblock<7, EXACT>(acc, ah, al, sb, b_tile); break;
-        default: issue_kblock<8, EXACT>(acc, ah, al, sb, b_tile); break;
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int c = 0; c < NCH_MAX; ++c)
-#pragma unroll
-        for (int e = 0; e < 16; ++e) fence_operand(acc[c][e]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(stage));    // this warp's reads of the stage are complete
-      if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
+    for (int e = 0; e < BN / 2; ++e) acc[e] = 0.f;
+    // k-blocks in pairs over two register buffers of A fragments: while the group of k-block kb runs, the fragments of
+    // kb + 1 are loaded and split into the other buffer (its previous group retired at the wait<1> before)
+    uint32_t ah0[BK / 8][4], al0[BK / 8][4], ah1[BK / 8][4], al1[BK / 8][4];
+    uint32_t sb0 = acquire(ah0, al0), sb1 = 0;
+    for (int kb = 0; kb < p.k_blocks; kb += 2) {
+      issue_kblock<BN, EXACT>(acc, ah0, al0, sb0, b_tile);
+      wgmma_wait<1>();
+      if (kb > 0) release();
+      if (kb + 1 >= p.k_blocks) break;
+      sb1 = acquire(ah1, al1);
+      issue_kblock<BN, EXACT>(acc, ah1, al1, sb1, b_tile);
+      wgmma_wait<1>();
+      release();
+      if (kb + 2 < p.k_blocks) sb0 = acquire(ah0, al0);
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int e = 0; e < BN / 2; ++e) fence_operand(acc[e]);
+    release();
 
-    // ---- epilogue on the accumulator registers: element (row0 + 8i, col0 + 32c + 8j + 2t + {0, 1}) ----
+    // ---- epilogue on the accumulator registers: element (row0 + 8i, col0 + 8j + 2t + {0, 1}) ----
     const long long row0 = (long long)m_t * BM + arow;
-    const int col0 = n_t * p.BN;
+    const int col0 = n_t * BN;
     RngKey rkey[2] = {key, key};      // replicate rows: key and B-row index of column 0 of this thread's two rows
     uint64_t rbase[2] = {0, 0};
     if (F & F_REP) {
@@ -202,60 +210,65 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       for (int i = 0; i < 2; ++i) sc[i] = row0 + 8 * i < p.M ? __ldg(p.scale + ((row0 + 8 * i) % p.scale_mod)) : 0.f;
     }
 #pragma unroll
-    for (int c = 0; c < NCH_MAX; ++c) {
-      if (c >= p.nch) continue;
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = col0 + 8 * j + 2 * t;
+      const bool col_ok = col < p.N;                 // N even, col even: the pair is all in or all out
+      float b0 = 0.f, b1 = 0.f;
+      if (p.bias && col_ok) { b0 = __ldg(p.bias + col); b1 = __ldg(p.bias + col + 1); }
       uint32_t bits[2] = {0u, 0u};
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int col = col0 + c * 32 + 8 * j + 2 * t;
-        const bool col_ok = col < p.N;                 // N even, col even: the pair is all in or all out
-        float b0 = 0.f, b1 = 0.f;
-        if (p.bias && col_ok) { b0 = __ldg(p.bias + col); b1 = __ldg(p.bias + col + 1); }
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const long long row = row0 + 8 * i;
-          const bool ok = col_ok && row < p.M;
-          float v0 = acc[c][4 * j + 2 * i] + b0, v1 = acc[c][4 * j + 2 * i + 1] + b1;
-          if (F & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-          if (F & F_SCALE) { v0 *= sc[i]; v1 *= sc[i]; }
-          if (!ok) continue;
-          if (F & F_GATE) {   // backward: pass the gradient only where the forward output was positive
-            const float2 gv = __ldg(reinterpret_cast<const float2*>(p.gate + row * p.gate_ld + col));
-            v0 = gv.x > 0.f ? v0 * p.gate_scale : 0.f;
-            v1 = gv.y > 0.f ? v1 * p.gate_scale : 0.f;
-          }
-          if (F & F_DROP) {   // element index row*N + col; N % 4 == 0, so the pair shares one Philox block
-            const uint64_t idx = (F & F_REP) ? rbase[i] + (uint64_t)col : (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
-            const uint4 u = dropout_block((F & F_REP) ? rkey[i] : key, p.drop_site, idx);
-            const bool lo_half = (idx & 3u) == 0;
-            const float m0 = keep_scale(lo_half ? u.x : u.z, p.drop_p, ik), m1 = keep_scale(lo_half ? u.y : u.w, p.drop_p, ik);
-            v0 *= m0; v1 *= m1;
-            bits[i] |= ((m0 > 0.f ? 1u : 0u) | (m1 > 0.f ? 2u : 0u)) << (8 * j + 2 * t);
-          }
-          if (F & F_RESID) {
-            const float2 r = __ldg(reinterpret_cast<const float2*>(p.resid + row * p.resid_ld + col));
-            v0 += r.x; v1 += r.y;
-          }
-          if (F & F_ROUND) { v0 = rn_tf32(v0); v1 = rn_tf32(v1); }
-          float* dst;
-          if (F & F_PERM) {   // row = b*pN + n, col = tt*4 + k  ->  encoder input [T, B, D] (code/models_rd.py:338-341)
-            const long long b = row / p.pN, n = row - b * p.pN;
-            dst = p.C + ((long long)(col >> 2) * p.pB + b) * p.pD + n * 4 + (col & 3);
-          } else {
-            dst = p.C + row * p.ldc + col;
-          }
-          *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+      for (int i = 0; i < 2; ++i) {
+        const long long row = row0 + 8 * i;
+        const bool ok = col_ok && row < p.M;
+        float v0 = acc[4 * j + 2 * i] + b0, v1 = acc[4 * j + 2 * i + 1] + b1;
+        if (F & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (F & F_SCALE) { v0 *= sc[i]; v1 *= sc[i]; }
+        if (!ok) continue;
+        if (F & F_GATE) {   // backward: pass the gradient only where the forward output was positive
+          const float2 gv = __ldg(reinterpret_cast<const float2*>(p.gate + row * p.gate_ld + col));
+          v0 = gv.x > 0.f ? v0 * p.gate_scale : 0.f;
+          v1 = gv.y > 0.f ? v1 * p.gate_scale : 0.f;
         }
+        if (F & F_DROP) {   // element index row*N + col; N % 4 == 0, so the pair shares one Philox block
+          const uint64_t idx = (F & F_REP) ? rbase[i] + (uint64_t)col : (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
+          const uint4 u = dropout_block((F & F_REP) ? rkey[i] : key, p.drop_site, idx);
+          const bool lo_half = (idx & 3u) == 0;
+          const float m0 = keep_scale(lo_half ? u.x : u.z, p.drop_p, ik), m1 = keep_scale(lo_half ? u.y : u.w, p.drop_p, ik);
+          v0 *= m0; v1 *= m1;
+          bits[i] = (m0 > 0.f ? 1u : 0u) | (m1 > 0.f ? 2u : 0u);
+        }
+        if (F & F_RESID) {
+          const float2 r = __ldg(reinterpret_cast<const float2*>(p.resid + row * p.resid_ld + col));
+          v0 += r.x; v1 += r.y;
+        }
+        if (F & F_ROUND) { v0 = rn_tf32(v0); v1 = rn_tf32(v1); }
+        float* dst;
+        if (F & F_PERM) {   // row = b*pN + n, col = tt*4 + k  ->  encoder input [T, B, D] (code/models_rd.py:338-341)
+          const long long b = row / p.pN, n = row - b * p.pN;
+          dst = p.C + ((long long)(col >> 2) * p.pB + b) * p.pD + n * 4 + (col & 3);
+        } else {
+          dst = p.C + row * p.ldc + col;
+        }
+        *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
       }
       if ((F & F_DROP) && p.drop_mask) {
-        // the backward of the consumer (LayerNorm) reads these bits instead of regenerating the Philox stream
+        // the backward of the consumer (LayerNorm) reads these bits instead of regenerating the Philox stream.  Columns
+        // 8j .. 8j+7 are one byte of the row's bit words (col0 % 8 == 0) and belong to this tile alone, so tiles that
+        // share a word never write the same byte.  Bytes past N up to the word's end are written as zeros by the tile
+        // holding column N - 1.
+        const int cb = col0 + 8 * j;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-          bits[i] |= __shfl_xor_sync(0xffffffffu, bits[i], 1);
-          bits[i] |= __shfl_xor_sync(0xffffffffu, bits[i], 2);
+          uint32_t b8 = bits[i] << (2 * t);
+          b8 |= __shfl_xor_sync(0xffffffffu, b8, 1);
+          b8 |= __shfl_xor_sync(0xffffffffu, b8, 2);
           const long long row = row0 + 8 * i;
-          const int cw = col0 + c * 32;
-          if (t == 0 && row < p.M && cw < p.N) p.drop_mask[row * p.drop_mask_ld + (cw >> 5)] = bits[i];
+          if (t == 0 && row < p.M && cb < p.N) {
+            uint8_t* w = reinterpret_cast<uint8_t*>(p.drop_mask + row * p.drop_mask_ld);
+            w[cb >> 3] = (uint8_t)b8;
+            if (cb + 8 >= p.N)
+              for (int z = (cb >> 3) + 1; z < 4 * p.drop_mask_ld && z < 4 * ((p.N + 31) >> 5); ++z) w[z] = 0;
+          }
         }
       }
     }
@@ -513,23 +526,77 @@ __global__ void split_weights_kernel(const __grid_constant__ SplitItems s) {
   }
 }
 
-void plan(long long M, int N, int* BN, int* n_tiles) {
-  const long long m_tiles = ceil_div(M, BM);
-  int nt = (int)ceil_div(N, MAX_BN);
-  while (m_tiles * nt < 120 && round_up(ceil_div(N, nt + 1), 32) >= 64) ++nt;   // spread over the SMs
-  *n_tiles = nt;
-  *BN = (int)round_up(ceil_div(N, nt), 32);     // whole 32-column MMA chunks
+}  // namespace
+
+// Tile widths tc_nt_kernel is instantiated for, each with every epilogue combination of its mode (RD_NT_WIDTHS_* below
+// must list the same).  Error-compensated (encoder GEMMs, small ob-prop layers): fine steps around the P19 shapes
+// (on 132 SMs tc_nt_plan picks 152 -> 2 x 80, 272 -> 2 x 136, 456 -> 2 x 232 at 7,680 rows, 240 -> 3 x 80 at 4,352);
+// it stops at 232, where the accumulators and two A-fragment buffers still fit in registers.  Single pass (the
+// HBM-bound ob-prop layers): the multiples of 32 from 64 up and 240, which serves C = 240 in one tile (the roofline
+// size); PAM's C = 2400 at 4,352 rows gets 11 x 224.
+#define RD_NT_WIDTHS_EXACT(X) X(48) X(80) X(96) X(120) X(136) X(152) X(184) X(232)
+#define RD_NT_WIDTHS_FAST(X) X(64) X(96) X(128) X(160) X(192) X(224) X(240) X(256)
+#define RD_NT_LIST(W) W,
+static const int kNtWidthsExact[] = {RD_NT_WIDTHS_EXACT(RD_NT_LIST)};
+static const int kNtWidthsFast[] = {RD_NT_WIDTHS_FAST(RD_NT_LIST)};
+#undef RD_NT_LIST
+template <typename Fn>
+static int nt_first_width(bool exact, Fn&& pred) {
+  if (exact) { for (int w : kNtWidthsExact) if (pred(w)) return w; }
+  else { for (int w : kNtWidthsFast) if (pred(w)) return w; }
+  return 0;
+}
+static bool nt_width_ok(int bn, bool exact) { return nt_first_width(exact, [&](int w) { return w == bn; }) != 0; }
+
+void tc_nt_plan(long long M, int N, bool exact, int* BN, int* n_tiles) {
+  // RD_TC_NT_BN=<width> forces the tile width (a listed one that covers N in at most 64 tiles; tests use it to run
+  // every plan on the same problem)
+  if (const char* e = getenv("RD_TC_NT_BN")) {
+    const int bn = atoi(e);
+    if (nt_width_ok(bn, exact) && ceil_div(N, bn) <= 64) { *BN = bn; *n_tiles = (int)ceil_div(N, bn); return; }
+  }
+  // Per-SM cost of a plan: the tiles of the busiest SM times their width plus a fixed per-tile overhead (pipeline
+  // fill and epilogue), in columns.  Smallest cost wins; ties go to fewer n tiles (A is read once per n tile).  The
+  // overhead of 32 columns is an estimate, not a measurement; the P19 plans above come out the same for any value
+  // from 0 to 256.  BM stays 128: a 64-row tile would need its own producer schedule (or the two MMA warpgroups
+  // working on different tiles, "ping-pong"), which this kernel does not have.
+  const long long m_tiles = ceil_div(M, BM), sms = num_sms();
+  constexpr long long TILE_OVERHEAD = 32;
+  long long best = -1;
+  for (int nt = 1; nt <= 64; ++nt) {
+    const long long need = ceil_div(N, nt);
+    const int bn = nt_first_width(exact, [&](int w) { return w >= need; });
+    if (bn == 0 || ceil_div(N, bn) < nt) continue;     // too narrow, or a wider plan with empty tiles
+    const long long cost = ceil_div(m_tiles * nt, sms) * (bn + TILE_OVERHEAD);
+    if (best < 0 || cost < best) { best = cost; *BN = bn; *n_tiles = nt; }
+  }
+  if (best < 0) {      // wider than 64 of the widest tiles
+    *BN = exact ? kNtWidthsExact[sizeof(kNtWidthsExact) / sizeof(int) - 1] : kNtWidthsFast[sizeof(kNtWidthsFast) / sizeof(int) - 1];
+    *n_tiles = (int)ceil_div(N, *BN);
+  }
 }
 
-
-}  // namespace
+// the instantiation of tile width `bn` (one of the mode's listed widths; tc_nt checked it)
+template <int F, bool EX, typename L>
+static int nt_launch(int bn, L&& launch) {
+#define RD_NT_WIDTH(W) case W: return launch(tc_nt_kernel<F, EX, W>);
+  if constexpr (EX) {
+    switch (bn) { RD_NT_WIDTHS_EXACT(RD_NT_WIDTH) default: break; }
+  } else {
+    switch (bn) { RD_NT_WIDTHS_FAST(RD_NT_WIDTH) default: break; }
+  }
+#undef RD_NT_WIDTH
+  set_error("tc_nt: tile width %d not instantiated", bn);
+  return -2;
+}
 
 static unsigned long long* g_gemm_dbg = nullptr;
 void tc_gemm_set_debug(unsigned long long* buf) { g_gemm_dbg = buf; }
 
 int tc_nt(const TcNtArgs& a, cudaStream_t st) {
-  if (a.BN < 32 || a.BN > 32 * NCH_MAX || a.BN % 32 || a.n_tiles < 1 || a.M < 1 || a.M > 0x7fffffffLL || a.K % 4 ||
-      a.N % 4 || a.lda % 4) {
+  const bool exact = a.B_lo != nullptr;
+  if (!nt_width_ok(a.BN, exact) || a.n_tiles < 1 || (long long)a.BN * a.n_tiles < a.N || a.M < 1 || a.M > 0x7fffffffLL ||
+      a.K % 4 || a.N % 4 || a.lda % 4) {
     set_error("tc_nt: unsupported tiling / shape (M=%lld N=%d K=%d BN=%d)", a.M, a.N, a.K, a.BN);
     return -2;
   }
@@ -538,9 +605,8 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
     set_error("tc_nt: pointers must be 16-byte aligned");
     return -2;
   }
-  const bool exact = a.B_lo != nullptr;
   NtP p;
-  p.M = a.M; p.N = a.N; p.K = a.K; p.BN = a.BN; p.nch = a.BN / 32; p.n_tiles = a.n_tiles;
+  p.M = a.M; p.N = a.N; p.K = a.K; p.n_tiles = a.n_tiles;
   p.m_tiles = (int)ceil_div(a.M, BM);
   p.k_blocks = (int)ceil_div(a.K, BK);
   const int stage_bytes = A_TILE + (exact ? 2 : 1) * a.BN * 128;
@@ -585,7 +651,7 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
   };
   int rc = -2;
 #define RD_NT_CASE(FLAGS, EX) \
-  if (f == (FLAGS) && exact == (EX)) rc = launch(tc_nt_kernel<(FLAGS), (EX)>); else
+  if (f == (FLAGS) && exact == (EX)) rc = nt_launch<(FLAGS), (EX)>(a.BN, launch); else
   // observation propagation: layer 2 -> encoder input, layer 1 (rounded for the next single-pass layer), the plain
   // operator, backward d(input); encoder: bias[,relu][,dropout][,residual] forward, [gate][,residual] backward
   RD_NT_CASE(F_PERM | F_RELU | F_SCALE, false)
@@ -628,7 +694,7 @@ int tc_gemm(const TcGemmArgs& a, cudaStream_t st) {
   if (!tc_gemm_supported(a)) { set_error("tc_gemm: unsupported shape/alignment (M=%lld N=%d K=%d)", a.M, a.N, a.K); return -2; }
   TcNtArgs n;
   n.A = a.A; n.lda = a.lda; n.B = a.B; n.B_lo = a.B_lo; n.M = a.M; n.N = a.N; n.K = a.K; n.C = a.C;
-  plan(a.M, a.N, &n.BN, &n.n_tiles);
+  tc_nt_plan(a.M, a.N, true, &n.BN, &n.n_tiles);
   n.bias = a.bias; n.relu = a.relu; n.gate = a.gate; n.gate_ld = a.gate_ld; n.gate_scale = a.gate_scale;
   n.drop_p = a.drop_p; n.rng = a.rng; n.drop_site = a.drop_site; n.rep = a.rep; n.drop_mask = a.drop_mask; n.drop_mask_ld = a.drop_mask_ld;
   n.resid = a.resid; n.resid_ld = a.resid_ld;

@@ -9,7 +9,8 @@ namespace rd {
 // (3xTF32: A is split in registers, B_lo = B - trunc19(B) is precomputed), else single-pass TF32 on operands the caller
 // keeps TF32-representable.  epi = +bias[col] -> relu -> *scale[row % scale_mod] -> *(gate > 0 ? gate_scale : 0) ->
 // dropout (+ keep bits) -> +resid -> RN to TF32 (round_out); perm != 0 stores row b*pN + n, col t*4 + k into
-// C[(t*pB + b)*pD + n*4 + k].  BN (a multiple of 32, <= 256) and n_tiles are the caller's tiling of N.
+// C[(t*pB + b)*pD + n*4 + k].  BN and n_tiles (BN * n_tiles >= N) are the caller's tiling of N, normally from
+// tc_nt_plan; BN must be one of the widths the kernel is instantiated for in the chosen mode.
 struct TcNtArgs {
   const float* A = nullptr; long long lda = 0;
   const float* B = nullptr; const float* B_lo = nullptr;
@@ -25,6 +26,10 @@ struct TcNtArgs {
   int perm = 0, pB = 0, pN = 0, pD = 0;
 };
 int tc_nt(const TcNtArgs& a, cudaStream_t st);
+// Tiling of N for an M x N tc_nt problem (exact: error-compensated mode): the instantiated width and n-tile count that
+// minimise the busiest SM's work over the device's SMs.  Deterministic for a given (M, N, mode, SM count);
+// the environment variable RD_TC_NT_BN=<width> forces a width (debugging, and tests that compare plans).
+void tc_nt_plan(long long M, int N, bool exact, int* BN, int* n_tiles);
 
 // C[M,N] = epi( A[M,K] . B[N,K]^T ) with fp32-level accuracy on the TF32 tensor cores ("3xTF32"):
 //   A = A_hi + A_lo, B = B_hi + B_lo (hi = top 19 bits, what the MMA reads; lo = exact remainder)

@@ -496,6 +496,50 @@ int rd_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg
                  float lr, const float* lr_dev, float beta1, float beta2, float eps, float grad_scale,
                  int64_t* step, void* stream);
 
+/* ---- differentially private training (DP-SGD, Abadi et al. 2016) ---------------------------------------------------
+ * theta = the trained tensors of Raindrop_v2 in flat-bucket order (raindrop_b200.functional.used_param_fields): the
+ * head (emb weight and bias when d_static > 0, mlp_static.0 weight and bias, mlp_static.2 weight and bias), 12 per
+ * encoder layer (in_proj weight, bias, out_proj weight, bias, linear1 weight, bias, linear2 weight, bias, norm1 weight,
+ * bias, norm2 weight, bias), then ob_propagation.lin_value weight, bias and ob_propagation_layer2.lin_value weight,
+ * bias: n_fields = (d_static > 0 ? 6 : 4) + 12 nlayers + 4.  l_b = CrossEntropy(logits_b, y_b) of the forward in the
+ * workspace (training mode: with its dropout masks), g_b = grad_theta l_b.  A DP step:
+ *   1. rd_raindrop_v2_fwd with labels: d_logits = (softmax - onehot) / B;
+ *   2. rd_raindrop_v2_per_sample_grad_sqnorms: the per-sample squared norms of the gradient of l_b / B;
+ *   3. rd_dp_clip_scale: d_logits row b *= w_b c_b B / L with c_b = min(1, C / (||g_b|| + 1e-6));
+ *   4. rd_raindrop_v2_bwd(RD_BWD_ALL) on the same workspace: grads = sum_b w_b c_b g_b / L;
+ *   5. rd_dp_add_noise: grads += (sigma C / L) xi, xi ~ N(0, I) over the used elements of the bucket;
+ *   6. rd_adam_step. */
+
+/* Scratch of rd_raindrop_v2_per_sample_grad_sqnorms: a backward scratch and the norm pass's partial sums. */
+size_t rd_dp_scratch_bytes(const rd_dims* dims);
+/* sqnorms [B, n_fields] (fp64, device) = the squared L2 norm of each sample's gradient per trained tensor, for the
+ * gradient the backward would compute from d_logits (after step 1: of l_b / B).  Runs the data-gradient chain of the
+ * backward (grads == NULL, as rd_raindrop_v2_bwd); per linear layer the sample's rows (encoder: t*B + b, ob-prop:
+ * b*N + n) give the norm in the cheaper of the ghost form sum_{r,r'} (y_r.y_r')(x_r.x_r' + 1) and the explicit form
+ * ||sum_r y_r [x_r, 1]^T||^2 (chosen from the shape alone); LayerNorm gamma / beta from the recomputed normalised input;
+ * the head from its one row per sample.  Every entry is written by one thread in a fixed order, without atomics: the
+ * result is bitwise reproducible.  The workspace and the backward's arithmetic mode are those of the forward (dims as
+ * passed to it).  scratch: rd_dp_scratch_bytes(dims) bytes.  Stream-ordered, sync-free, CUDA-graph capturable. */
+int rd_raindrop_v2_per_sample_grad_sqnorms(const rd_dims* dims, const rd_params* params, const float* statics,
+                                           const int64_t* lengths, const float* node_scale, const void* workspace,
+                                           const float* d_logits, void* scratch, double* sqnorms, void* stream);
+/* Clipping, in place on d_logits [B, n_classes] of step 1: n_b = B sqrt(sum_f sqnorms[b, f]) (fp64),
+ * c_b = min(1, max_grad_norm / (n_b + 1e-6)) -> clip_factors[b]; row b *= w_b c_b B / expected_batch_size, weight [B]
+ * in {0, 1}; loss = sum_b w_b l_b / sum_b w_b (0 when every weight is 0) from the forward's per-sample losses in the
+ * workspace.  One launch. */
+int rd_dp_clip_scale(const rd_dims* dims, const void* workspace, const double* sqnorms, const float* weight,
+                     float max_grad_norm, float expected_batch_size, float* d_logits, float* clip_factors, float* loss,
+                     void* stream);
+/* grad[i] += noise_std * xi_i for i in the used ranges [field_offsets[f], + field_numel[f]) of the flat bucket grad [n]
+ * (host arrays, ascending, offsets % 4 == 0, n % 4 == 0, 1 <= n_fields <= 128); padding is not touched.  xi_i is drawn
+ * from the Philox4x32-10 stream of the dropout masks with key {seed, step} = key[0], key[1] (device uint64[3]; key[2]
+ * is a ticket word, 0 on entry), site 96, counter i >> 2, and Box-Muller on the block's word pairs:
+ * u1 = ((w0 >> 8) + 1) 2^-24, u2 = (w1 >> 8) 2^-24, xi = sqrt(-2 ln u1) (cos, sin)(2 pi u2) in fp64, rounded to fp32.
+ * The launch advances key[1] by one, so CUDA-graph replays draw fresh noise.  Philox is not a cryptographically secure
+ * generator.  One 128-bit grid-stride launch. */
+int rd_dp_add_noise(float* grad, int64_t n, const int64_t* field_offsets, const int64_t* field_numel, int32_t n_fields,
+                    float noise_std, uint64_t* key, void* stream);
+
 /* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);

@@ -173,4 +173,35 @@ int cross_entropy(const float* logits, const int64_t* y, int B, int ncls, float*
 int adam(float* p, const float* g, float* m, float* v, int64_t n, float lr, const float* lr_dev, float b1, float b2,
          float eps, float gscale, int64_t* step, cudaStream_t st);
 
+// ---- differentially private training (rd_dp.cu) ---------------------------------------------------------------------
+// Per-sample squared gradient norms of the linear layers.  Item = one (dY, X) operand pair of a weight gradient; sample
+// b's rows are r = b*sstride + t*rstride, t < R (encoder: sstride 1, rstride B, R = T; ob-prop: sstride N, rstride 1,
+// R = N).  Its weight and bias sums land in sqnorms[b*nf + fw] and [b*nf + fb].  ghost / tm / tn / ntiles come from
+// dp_norm_tiles; blk0 = the item's first CTA in the group launch (items in order, B*ntiles CTAs each).
+constexpr uint32_t SITE_DP_NOISE = 96;      // Philox site of the DP-SGD noise (its key is the noise key, not the dropout key)
+constexpr int DP_MAX_ITEMS = 4 * RD_MAX_LAYERS;
+constexpr int DP_MAX_FIELDS = 128;
+struct DpNormItem {
+  const float* Y; const float* X;
+  long long ldy, ldx, sstride, rstride, blk0;
+  int Nout, Kin, R, ghost, tm, tn, ntiles, fw, fb;
+};
+struct DpNormGroup { DpNormItem it[DP_MAX_ITEMS]; int n; };
+// ghost iff R (Nout + Kin + 1) < Nout (Kin + 1): the form with fewer multiply-adds
+bool dp_ghost(int R, int Nout, int Kin);
+int dp_norm_tiles(int R, int Nout, int Kin, int* tm, int* tn);     // tiles per sample; sets tm, tn
+// one launch over every item's tiles (partial: 2 doubles per CTA), one launch adding them into sqnorms
+int dp_norm_group(const DpNormGroup& g, int B, double* partial, double* sqnorms, int nf, cudaStream_t st);
+// LayerNorm gamma / beta of each sample (rows t*B + b, t < T) from its input x, stats {mean, rstd} and output gradient dy
+int dp_ln_sqnorm(const float* x, const float* stats, const float* dy, int T, int B, int D, double* sqnorms, int nf, int fw,
+                 int fb, cudaStream_t st);
+// emb (ds > 0), mlp_static.0, mlp_static.2 weight and bias, in that order from field 0
+int dp_head_sqnorm(int B, int D, int Df, int ds, int ncls, const float* dlogits, const float* hpre, const float* dh,
+                   const float* feat, const float* dfeat, const float* statics, double* sqnorms, int nf, cudaStream_t st);
+int dp_clip(const double* sqnorms, int B, int nf, int ncls, const float* weight, double max_norm, double L,
+            const float* loss_ps, float* dlogits, float* clip, float* loss, cudaStream_t st);
+// the used ranges [off, off + numel) of the flat bucket, ascending, off % 4 == 0
+struct DpFields { long long off[DP_MAX_FIELDS]; long long numel[DP_MAX_FIELDS]; int n; };
+int dp_noise(float* g, int64_t n, const DpFields& fields, float stdv, uint64_t* key, cudaStream_t st);
+
 }  // namespace rd

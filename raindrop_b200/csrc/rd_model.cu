@@ -155,6 +155,58 @@ BwLayout bw_layout(const Shape& s) {
   return b;
 }
 
+// ---- DP-SGD per-sample norm pass -----------------------------------------------------------------------------------
+// Trained tensors, in used_param_fields order: the head (emb weight / bias when d_static > 0, mlp_static.0, mlp_static.2),
+// 12 per encoder layer, the two lin_value pairs.
+int dp_head_fields(const Shape& s) { return s.ds > 0 ? 6 : 4; }
+int dp_n_fields(const Shape& s) { return dp_head_fields(s) + 12 * s.L + 4; }
+
+// Norm items of one backward phase, queued where the training path queues the weight-gradient items of the same
+// (dY, X) pairs, and flushed as one group launch (dp_norm_group).  The partial sums of a phase start at `partial` again:
+// the previous phase's launches have completed by then (stream order).
+struct DpQueue {
+  DpNormGroup g;
+  long long blk = 0;
+  int B = 0, nf = 0;
+  double* sqnorms = nullptr; double* partial = nullptr;
+  DpQueue() { g.n = 0; }
+  void add(const float* Y, int64_t ldy, const float* X, int64_t ldx, int Nout, int Kin, int R, int64_t sstride,
+           int64_t rstride, int fw) {
+    DpNormItem& o = g.it[g.n++];
+    o.Y = Y; o.X = X; o.ldy = ldy; o.ldx = ldx; o.sstride = sstride; o.rstride = rstride; o.blk0 = blk;
+    o.Nout = Nout; o.Kin = Kin; o.R = R; o.ghost = dp_ghost(R, Nout, Kin) ? 1 : 0;
+    o.ntiles = dp_norm_tiles(R, Nout, Kin, &o.tm, &o.tn);
+    o.fw = fw; o.fb = fw + 1;
+    blk += (long long)B * o.ntiles;
+  }
+  int flush(cudaStream_t st) {
+    int rc = dp_norm_group(g, B, partial, sqnorms, nf, st);
+    g.n = 0; blk = 0;
+    return rc;
+  }
+};
+
+// CTAs (= partial pairs) of the larger of the two phases' group launches
+int64_t dp_partial_blocks(const Shape& s) {
+  int tm, tn;
+  int64_t enc = (int64_t)s.L * (dp_norm_tiles(s.T, s.D, s.nhid, &tm, &tn) + dp_norm_tiles(s.T, s.nhid, s.D, &tm, &tn) +
+                                dp_norm_tiles(s.T, s.D, s.D, &tm, &tn) + dp_norm_tiles(s.T, 3 * s.D, s.D, &tm, &tn));
+  int64_t ob = 2LL * dp_norm_tiles(s.N, s.C, s.C, &tm, &tn);
+  return (int64_t)s.B * (enc > ob ? enc : ob);
+}
+
+// Scratch of rd_raindrop_v2_per_sample_grad_sqnorms: the backward scratch of the data-gradient chain, then the partial
+// sums (2 doubles per CTA of a group launch)
+struct DpLayout { int64_t bw, partial, total; };
+DpLayout dp_layout(const Shape& s) {
+  DpLayout l;
+  Arena a;
+  l.bw = a.take(bw_layout(s).total);
+  l.partial = a.take(4 * dp_partial_blocks(s));
+  l.total = a.off;
+  return l;
+}
+
 // Scratch of rd_raindrop_v2_input_grad: W1^T with its error-compensation remainder, and dX0 = d(loss)/d(X0) [B*N, C]
 struct IgLayout { int64_t W1t, W1tlo, dX0, total; };
 IgLayout input_grad_layout(const Shape& s) {
@@ -510,7 +562,7 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
 
 static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* statics, const int64_t* lengths,
                         const float* nscale, const float* ws, const float* dlogits, const rd_grads* G, float* sc,
-                        int phases, float* d_z0_out, cudaStream_t st) {
+                        int phases, float* d_z0_out, cudaStream_t st, DpQueue* dp = nullptr) {
   Shape s;
   RD_TRY(make_shape(dims, &s));
   if ((phases & ~3) || phases == 0) { set_error("rd_raindrop_v2_bwd: phases must be 1, 2 or 3"); return -2; }
@@ -533,6 +585,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   float* dfeat = sc + b.dfeat; float* dhpre = sc + b.dhpre;
   RD_TRY(head_bwd(s.B, s.T, s.D, s.emb, s.ds, s.ncls, lengths, statics, P->mlp0_weight, P->mlp2_weight, feat, hpre, dlogits,
                   dhpre, dfeat, gA, G->mlp0_weight, G->mlp0_bias, G->mlp2_weight, G->mlp2_bias, G->emb_weight, G->emb_bias, st));
+  if (dp) RD_TRY(dp_head_sqnorm(s.B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dhpre, feat, dfeat, statics, dp->sqnorms, dp->nf, st));
 
   const float scale = 1.f / sqrtf((float)s.hd);
   const int64_t row3 = (int64_t)s.B * 3 * s.D;
@@ -540,6 +593,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   for (int l = s.L - 1; l >= 0; --l) {
     const rd_encoder_layer_params& E = P->layer[l];
     const rd_encoder_layer_grads& GE = G->layer[l];
+    const int fl = dp ? dp_head_fields(s) + 12 * l : 0;     // this layer's first field (in_proj_weight)
     const float* x = ws + w.Z[l];
     const float* qkv = ws + w.l[l].qkv; const float* Pm = ws + w.l[l].P;
     const float* Pd = s.p > 0.f ? ws + w.l[l].Pd : Pm;
@@ -563,15 +617,18 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     }
     RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, GE.norm2_weight, GE.norm2_bias,
                          sc + b.l[l].ln[0], K2, s.p, rng, SITE_RESID2 + l, &chunks, st, m2, mld));
+    if (dp) RD_TRY(dp_ln_sqnorm(r2, ws + w.l[l].st2, gA, s.T, s.B, s.D, dp->sqnorms, dp->nf, fl + 10, fl + 11, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0], 2 * s.D, chunks, s.D, GE.norm2_weight, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0] + s.D, 2 * s.D, chunks, s.D, GE.norm2_bias, st));
     if (wg) RD_TRY(tn(&wq, K2, s.D, f, s.nhid, GE.linear2_weight, GE.linear2_bias, s.D, s.nhid, s.M2, sc + b.l[l].wp[0], partial, st));
+    if (dp) dp->add(K2, s.D, f, s.nhid, s.D, s.nhid, s.T, 1, s.B, fl + 6);
     {   // gF = (K2 . W2) * [f > 0] / (1-p)   ("NT" against W2^T so that the tensor-core kernel applies)
       GemmP g = nt(K2, s.D, ws + w.wsp[l].l2_t, s.D, gF, s.nhid, s.M2, s.nhid, s.D);
       g.gate = f; g.gate_ld = s.nhid; g.gate_scale = ik;  // relu' and the FFN dropout mask in one
       RD_TRY(linear_nt(g, ws + w.wsp[l].l2_tlo, st));
     }
     if (wg) RD_TRY(tn(&wq, gF, s.nhid, x1, s.D, GE.linear1_weight, GE.linear1_bias, s.nhid, s.D, s.M2, sc + b.l[l].wp[1], partial, st));
+    if (dp) dp->add(gF, s.nhid, x1, s.D, s.nhid, s.D, s.T, 1, s.B, fl + 4);
     {
       GemmP g = nt(gF, s.nhid, ws + w.wsp[l].l1_t, s.nhid, gA, s.D, s.M2, s.D, s.nhid);
       g.resid = res; g.resid_ld = s.D;
@@ -581,9 +638,11 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     res = s.p > 0.f ? gB : K1;
     RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, GE.norm1_weight, GE.norm1_bias,
                          sc + b.l[l].ln[1], K1, s.p, rng, SITE_RESID1 + l, &chunks, st, m1, mld));
+    if (dp) RD_TRY(dp_ln_sqnorm(r1, ws + w.l[l].st1, gA, s.T, s.B, s.D, dp->sqnorms, dp->nf, fl + 8, fl + 9, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1], 2 * s.D, chunks, s.D, GE.norm1_weight, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1] + s.D, 2 * s.D, chunks, s.D, GE.norm1_bias, st));
     if (wg) RD_TRY(tn(&wq, K1, s.D, ctx, s.D, GE.out_proj_weight, GE.out_proj_bias, s.D, s.D, s.M2, sc + b.l[l].wp[2], partial, st));
+    if (dp) dp->add(K1, s.D, ctx, s.D, s.D, s.D, s.T, 1, s.B, fl + 2);
     RD_TRY(linear_nt(nt(K1, s.D, ws + w.wsp[l].out_t, s.D, gD, s.D, s.M2, s.D, s.D), ws + w.wsp[l].out_tlo, st));
     if (attn_tc_supported(s.T, s.hd)) {
       RD_TRY(attn_tc_bwd(qkv, gD, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, dqkv, st));
@@ -625,6 +684,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
       }
     }
     if (wg) RD_TRY(tn(&wq, dqkv, 3 * s.D, x, s.D, GE.in_proj_weight, GE.in_proj_bias, 3 * s.D, s.D, s.M2, sc + b.l[l].wp[3], partial, st));
+    if (dp) dp->add(dqkv, 3 * s.D, x, s.D, 3 * s.D, s.D, s.T, 1, s.B, fl);
     {
       // the first layer's input gradient is d(loss)/d(encoder input): optionally delivered straight to the caller
       GemmP g = nt(dqkv, 3 * s.D, ws + w.wsp[l].in_t, 3 * s.D, (l == 0 && d_z0_out) ? d_z0_out : gA, s.D, s.M2, s.D, 3 * s.D);
@@ -633,6 +693,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     }
   }
   if (!(phases & RD_BWD_OBPROP)) RD_TRY(wq.flush(st));   // encoder + head gradients complete: the caller may reduce them now
+  if (dp) RD_TRY(dp->flush(st));
   }
 
   if (phases & RD_BWD_OBPROP) {
@@ -642,6 +703,8 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   const int tc = s.tc;
   RD_TRY(obprop_out_grad(gA, ws + w.Z[0], nscale, s.B, s.T, s.N, s.dob, s.D, tc && !s.exact, gO2, st));
   if (wg) RD_TRY(tn(&wq, gO2, s.C, H1, s.C, G->ob2_value_weight, G->ob2_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[0], partial, st));
+  const int fob = dp ? dp_head_fields(s) + 12 * s.L : 0;    // ob1 weight, ob1 bias, ob2 weight, ob2 bias
+  if (dp) dp->add(gO2, s.C, H1, s.C, s.C, s.C, s.N, s.N, 1, fob + 2);
   if (tc) {
     // dZ1 = (dZ2 . W2) * s * [H1 > 0] on the tensor cores: "NT" form against a transposed, TF32-rounded W2
     const float* W2t = ws + w.W2t;      // written by the forward's weight-prep launch
@@ -656,7 +719,9 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     RD_TRY(gemm(g, st));
   }
   if (wg) RD_TRY(tn(&wq, gO1, s.C, X0, s.C, G->ob1_value_weight, G->ob1_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[1], partial, st));
+  if (dp) dp->add(gO1, s.C, X0, s.C, s.C, s.C, s.N, s.N, 1, fob);
   RD_TRY(wq.flush(st));
+  if (dp) RD_TRY(dp->flush(st));
   }
   return 0;
 }
@@ -1214,6 +1279,73 @@ int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, cons
                          c0 + nc >= M, st));
   }
   return 0;
+}
+
+size_t rd_dp_scratch_bytes(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return (size_t)dp_layout(s).total * sizeof(float);
+}
+
+int rd_raindrop_v2_per_sample_grad_sqnorms(const rd_dims* dims, const rd_params* params, const float* statics,
+                                           const int64_t* lengths, const float* node_scale, const void* workspace,
+                                           const float* d_logits, void* scratch, double* sqnorms, void* stream) {
+  const char* fn = "rd_raindrop_v2_per_sample_grad_sqnorms";
+  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch || !sqnorms) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  const DpLayout l = dp_layout(s);
+  DpQueue q;
+  q.B = s.B; q.nf = dp_n_fields(s); q.sqnorms = sqnorms;
+  q.partial = reinterpret_cast<double*>((float*)scratch + l.partial);
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr,
+                      (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, &q);
+}
+
+int rd_dp_clip_scale(const rd_dims* dims, const void* workspace, const double* sqnorms, const float* weight,
+                     float max_grad_norm, float expected_batch_size, float* d_logits, float* clip_factors, float* loss,
+                     void* stream) {
+  if (!dims || !workspace || !sqnorms || !weight || !d_logits || !clip_factors || !loss) {
+    set_error("rd_dp_clip_scale: NULL argument");
+    return -2;
+  }
+  if (!(max_grad_norm > 0.f) || !(expected_batch_size > 0.f)) {
+    set_error("rd_dp_clip_scale: max_grad_norm and expected_batch_size must be > 0");
+    return -2;
+  }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  const WsLayout w = ws_layout(s);
+  return dp_clip(sqnorms, s.B, dp_n_fields(s), s.ncls, weight, (double)max_grad_norm, (double)expected_batch_size,
+                 (const float*)workspace + w.loss_ps, d_logits, clip_factors, loss, (cudaStream_t)stream);
+}
+
+int rd_dp_add_noise(float* grad, int64_t n, const int64_t* field_offsets, const int64_t* field_numel, int32_t n_fields,
+                    float noise_std, uint64_t* key, void* stream) {
+  if (!grad || !field_offsets || !field_numel || !key || n < 0 || (n & 3) || n_fields < 1 || n_fields > DP_MAX_FIELDS ||
+      !(noise_std >= 0.f)) {
+    set_error("rd_dp_add_noise: bad arguments");
+    return -2;
+  }
+  DpFields f;
+  f.n = n_fields;
+  int64_t prev_end = 0;
+  for (int i = 0; i < n_fields; ++i) {
+    f.off[i] = field_offsets[i]; f.numel[i] = field_numel[i];
+    if (f.off[i] < prev_end || (f.off[i] & 3) || f.numel[i] < 0 || f.off[i] + f.numel[i] > n) {
+      set_error("rd_dp_add_noise: field %d [%lld, +%lld) is not ascending, 4-aligned and inside the bucket", i,
+                (long long)f.off[i], (long long)f.numel[i]);
+      return -2;
+    }
+    prev_end = f.off[i] + f.numel[i];
+  }
+  if (n == 0) return 0;
+  return dp_noise(grad, n, f, noise_std, key, (cudaStream_t)stream);
 }
 
 int rd_positional_encoding_bwd(const float* times, const float* d_pe, int64_t n_tokens, const float* timescales_host,

@@ -144,6 +144,12 @@ SIGNATURES = {
                                            C.c_void_p, C.c_void_p]),
     "rd_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_void_p,
                                C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
+    "rd_dp_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
+    "rd_raindrop_v2_per_sample_grad_sqnorms": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 8),
+    "rd_dp_clip_scale": (C.c_int, [C.POINTER(RdDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float] +
+                         [C.c_void_p] * 4),
+    "rd_dp_add_noise": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32, C.c_float,
+                                  C.c_void_p, C.c_void_p]),
     "rd_debug_attention_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_gemm_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_dropout_mask": (C.c_int, [C.c_void_p, C.c_uint32, C.c_int64, C.c_float, C.c_void_p,

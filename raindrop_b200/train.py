@@ -165,14 +165,24 @@ class TrainStep:
                                             self.plan.node_scale.data_ptr(), self.ws.data_ptr(), self.d_logits.data_ptr(),
                                             C.byref(self.G), self.scratch.data_ptr(), phases, st), "rd_raindrop_v2_bwd")
 
-    def _enqueue(self):
-        lib, st = self.lib, L.stream_ptr(self.device)
-        # forward incl. CrossEntropyLoss + d(loss)/d(logits) (fused into the head kernel)
-        L.check(lib.rd_raindrop_v2_fwd(C.byref(self.dims), C.byref(self.P), self.src.data_ptr(), L.ptr(self.static),
-                                       self.times.data_ptr(), self.lengths.data_ptr(), self.plan.node_scale.data_ptr(),
-                                       self.plan.rng_state.data_ptr(), self.ws.data_ptr(), self.logits.data_ptr(),
-                                       self.y.data_ptr(), self.loss.data_ptr(), self.d_logits.data_ptr(), st),
+    def _forward(self, st):
+        """forward incl. CrossEntropyLoss + d(loss)/d(logits) (fused into the head kernel)"""
+        L.check(self.lib.rd_raindrop_v2_fwd(C.byref(self.dims), C.byref(self.P), self.src.data_ptr(), L.ptr(self.static),
+                                            self.times.data_ptr(), self.lengths.data_ptr(), self.plan.node_scale.data_ptr(),
+                                            self.plan.rng_state.data_ptr(), self.ws.data_ptr(), self.logits.data_ptr(),
+                                            self.y.data_ptr(), self.loss.data_ptr(), self.d_logits.data_ptr(), st),
                 "rd_raindrop_v2_fwd")
+
+    def _adam(self, st):
+        L.check(self.lib.rd_adam_step(self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
+                                      self.exp_avg_sq.data_ptr(), self.flat_p.numel(), self._lr, self.lr_dev.data_ptr(),
+                                      self.betas[0], self.betas[1], self.eps, 1.0 / self.world, self.step_count.data_ptr(),
+                                      st),
+                "rd_adam_step")
+
+    def _enqueue(self):
+        st = L.stream_ptr(self.device)
+        self._forward(st)
         if self.world > 1:
             cur = torch.cuda.current_stream(self.device)
             self._bwd(L.BWD_ENCODER, st)
@@ -184,18 +194,17 @@ class TrainStep:
             cur.wait_stream(self.side)
         else:
             self._bwd(L.BWD_ALL, st)
-        L.check(lib.rd_adam_step(self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(),
-                                 self.exp_avg_sq.data_ptr(), self.flat_p.numel(), self._lr, self.lr_dev.data_ptr(),
-                                 self.betas[0], self.betas[1], self.eps, 1.0 / self.world, self.step_count.data_ptr(), st),
-                "rd_adam_step")
+        self._adam(st)
+
+    def _state(self):
+        """What a step changes besides its scratch: snapshotted around capture()'s warm-up steps."""
+        return (self.flat_p, self.exp_avg, self.exp_avg_sq, self.step_count, self.plan.rng_state, self.loss, self.logits)
 
     def _snapshot(self):
-        return [t.clone() for t in (self.flat_p, self.exp_avg, self.exp_avg_sq, self.step_count, self.plan.rng_state,
-                                    self.loss, self.logits)]
+        return [t.clone() for t in self._state()]
 
     def _restore(self, snap):
-        for t, s_ in zip((self.flat_p, self.exp_avg, self.exp_avg_sq, self.step_count, self.plan.rng_state,
-                          self.loss, self.logits), snap):
+        for t, s_ in zip(self._state(), snap):
             t.copy_(s_)
 
     def capture(self, warmup=3):

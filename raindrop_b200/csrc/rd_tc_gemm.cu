@@ -17,8 +17,9 @@
 //                 the ring for the next tile.
 //
 // tc_wgrad_group: dW = dY^T X (+ db) for up to WG_MAX problems in one launch.  Both operands are activations whose
-// contraction index runs over their ROWS; wgmma's TF32 form only reads K-major operands from shared memory, so these
-// tiles are staged row-major (cp.async, padded rows) and fed to mma.sync.m16n8k8 from fragments gathered per thread.
+// contraction index runs over their ROWS; wgmma's TF32 form only reads K-major operands from shared memory, so dY^T is
+// gathered into registers from a row-major stage and X is transposed by a producer warpgroup into the K-major swizzled
+// image wgmma reads (tc_wgrad_kernel below), followed by a fixed-order split-K reduce.
 #include <stdlib.h>
 
 #include "rd_tc_common.cuh"
@@ -278,27 +279,49 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 
 // =================================================================================================
 // weight-gradient kernel ("TN"), GROUPED: one launch serves up to WG_MAX independent problems
-//   D_k[m, n] = sum_r A_k[r, m] * B_k[r, n]   over this CTA's row range of problem k
-// A training step has ten of these (8 encoder weights + 2 lin_value); grouped, the launch latency is paid once.
-// One CTA per work item (problem, m tile, n tile, row split): 8 warps, 4 (m: 32 rows) x 2 (n: BN/2 columns), row
-// blocks of 32 staged by cp.async into a two-stage ring.  Row strides of the staged tiles are 8 floats more than a
-// multiple of 32, so the fragment gathers (lanes g along M/N, lanes t along K) hit 32 distinct banks.  The bias
-// gradient falls out of the same MMAs as one extra "ones" column of X (column N).
+//   D_k[m, n] = sum_r A_k[r, m] * B_k[r, n]   (A = dY, B = X plus a "ones" column N for the bias gradient)
+// over one row split of problem k per work item (problem, m tile, n tile, split).  A training step has ten of these
+// (8 encoder weights + 2 lin_value).  Persistent: one CTA per SM walks the items blockIdx.x, + gridDim.x, ...
+//   warpgroup 2   producer, 128 threads.  Per 32-row k-block: the dY tile [32 x 128] by cp.async into a row-major
+//                 stage (column XOR-ed with 8 (r % 4), see wa_offset), completion tracked on the stage's mbarrier; the
+//                 X tile [32 x BN] through registers (loaded one k-block ahead), TRANSPOSED into the K-major 128B-swizzled
+//                 image wgmma reads (sw128_offset(n, r)) as hi = top 19 bits and lo = exact remainder, with the ones
+//                 column written here (TMA cannot synthesise it).  Lane = row r and a warp's 32 stores share n, so
+//                 (((r >> 2) ^ n) & 7) * 4 + r % 4 hits 32 distinct banks.  fence.proxy.async, then arrive.
+//   warpgroups    0 and 1: dW rows 0-63 and 64-127 of the tile, one wgmma.m64nBNk8 per k-step and term (lo.hi, hi.lo,
+//                 hi.hi) with A = dY^T gathered from the row-major stage (a transposed gather is addressing) and split in
+//                 registers, exactly the tc_nt_kernel pipeline (one group in flight, two A-fragment buffers, a stage is
+//                 released only after the group that read it retired).  A warpgroup whose 64 rows lie past M waits and
+//                 releases the stages without MMAs.  Partial tiles go to slab [split][M][Nld] (Nld = N + 1 rounded up to 4).
+// The tile width BN is a template parameter, one per launch (wgrad_plan picks it for the whole group): with several
+// widths dispatched per item inside one kernel, ptxas serialises the wgmma for lack of registers (C7512).
 // =================================================================================================
 struct WP {
   const float* dY; const float* X; long long ldy, ldx;
-  float* partial;                    // [nsplit][Mpad][Nld]
-  long long rows; int M, N, BN, n_tiles, m_tiles, nsplit, rows_per_split, Mpad, Nld;
+  float* partial;                    // [nsplit][M][Nld]
+  int rows, M, N, Nld, n_tiles, m_tiles, nsplit, rows_per_split;
   int item0;                         // first work item of this problem inside the grouped list
 };
 struct WGroup { WP it[WG_MAX]; int n, total_items; };
 
-constexpr int W_THREADS = 256;
-constexpr int WBK = 32;              // contraction rows per block
-constexpr int LDA_W = BM + 8;        // staged dY tile [32][BM + 8]
-constexpr int NJ_MAX = MAX_BN / 16;  // n8 tiles per warp
+constexpr int W_THREADS = 384;            // warpgroups 0, 1: MMA; warpgroup 2: producer
+constexpr int WA_TILE = BK * BM * 4;      // 16 KB: 32 rows of dY x 128 columns
+// ring stage: dY tile | X^T hi | X^T lo; as many stages (<= MAX_STAGES) as fit next to the barriers and the alignment slack
+__host__ __device__ constexpr int w_stage_bytes(int bn) { return WA_TILE + 2 * bn * 128; }
+__host__ __device__ constexpr int w_nstages(int bn) { return (SMEM_LIMIT - 1280) / w_stage_bytes(bn) < MAX_STAGES ? (SMEM_LIMIT - 1280) / w_stage_bytes(bn) : MAX_STAGES; }
 
-struct WItem { int pi, n_t, m_t, split, k_blocks; long long r_begin, r_end; };
+// Tile widths the weight-gradient kernel is instantiated for (multiples of 8 up to MAX_BN)
+#define RD_WG_WIDTHS(X) X(32) X(64) X(96) X(128) X(144) X(160)
+
+// byte offset of element (r, m) of the staged dY tile: the fragment gathers read (r = 8ks + t (+4), m = arow + g (+8)),
+// so XOR-ing m with 8 (r % 4) = 8t spreads lanes (g, t) over 32 banks; 16-byte chunks stay contiguous for cp.async
+__device__ __forceinline__ uint32_t wa_offset(int r, int m) { return (uint32_t)(r * BM + (m ^ ((r & 3) << 3))) * 4u; }
+
+__device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+
+struct WItem { int pi, n_t, m_t, split, k_blocks, r_begin, r_end; };
 __device__ __forceinline__ WItem wgrad_item(const WGroup& g, int w) {
   WItem it;
   it.pi = 0;
@@ -307,107 +330,189 @@ __device__ __forceinline__ WItem wgrad_item(const WGroup& g, int w) {
   const WP& p = g.it[it.pi];
   const int item = w - p.item0;
   it.n_t = item % p.n_tiles; it.m_t = (item / p.n_tiles) % p.m_tiles; it.split = item / (p.n_tiles * p.m_tiles);
-  it.r_begin = (long long)it.split * p.rows_per_split;
+  it.r_begin = it.split * p.rows_per_split;
   it.r_end = min(p.rows, it.r_begin + p.rows_per_split);
-  it.k_blocks = (int)((it.r_end - it.r_begin + WBK - 1) / WBK);
+  it.k_blocks = (it.r_end - it.r_begin + BK - 1) / BK;
   return it;
 }
 
-__global__ void __launch_bounds__(W_THREADS)
-tc_wgrad_kernel(const __grid_constant__ WGroup g) {
-  extern __shared__ float wsm[];
-  pdl_launch_dependents();
-  pdl_wait();
-  const WItem it = wgrad_item(g, blockIdx.x);
-  const WP& p = g.it[it.pi];
-  const int ldb = p.BN + 8;
-  const int stage_floats = WBK * LDA_W + WBK * ldb;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq = lane >> 2, t = lane & 3;
-  const int wm = warp & 3, wn = warp >> 2;
-  const int nj = p.BN >> 4;                      // n8 tiles of this warp (BN / 2 columns)
-  const int mcol0 = it.m_t * BM, ncol0 = it.n_t * p.BN;
+struct WRing {
+  uint32_t base, stage_bytes, bar_base, phase = 0;
+  int nstages, stage = 0, rstage = 0;
+  __device__ uint32_t full(int s) const { return bar_base + 8u * s; }
+  __device__ uint32_t empty(int s) const { return bar_base + 8u * (MAX_STAGES + s); }
+  __device__ uint32_t addr(int s) const { return base + (uint32_t)s * stage_bytes; }
+};
 
-  auto load = [&](int kb, int s) {
-    float* sA = wsm + s * stage_floats;
-    float* sB = sA + WBK * LDA_W;
-    const long long r0 = it.r_begin + (long long)kb * WBK;
-    for (int v = threadIdx.x; v < WBK * (BM / 4); v += W_THREADS) {
-      const int r = v / (BM / 4), c = 4 * (v % (BM / 4));
-      const long long gr = r0 + r;
-      const bool ok = gr < it.r_end && mcol0 + c < p.M;
-      const float* src = ok ? p.dY + gr * p.ldy + mcol0 + c : p.dY;
-      cp_async16(smem_u32(sA + r * LDA_W + c), src, ok ? 16u : 0u);
-    }
-    const int bq = p.BN / 4;
-    for (int v = threadIdx.x; v < WBK * bq; v += W_THREADS) {
-      const int r = v / bq, c = 4 * (v % bq);
-      const long long gr = r0 + r;
-      const int gc = ncol0 + c;
-      float* dst = sB + r * ldb + c;
-      if (gc == p.N) {                          // X[r, N] := 1 for the valid rows: the bias gradient column
-        *reinterpret_cast<float4*>(dst) = make_float4(gr < it.r_end ? 1.f : 0.f, 0.f, 0.f, 0.f);
-      } else {
-        const bool ok = gr < it.r_end && gc < p.N;
-        cp_async16(smem_u32(dst), ok ? p.X + gr * p.ldx + gc : p.X, ok ? 16u : 0u);
-      }
-    }
-    cp_async_commit();
+// one item on MMA warpgroup `wg`: k-blocks -> accumulators -> this split's slab
+template <int BN>
+__device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRing& q, int wg, int arow, int t) {
+  constexpr uint32_t b_tile = (uint32_t)BN * 128u;
+  auto release = [&]() {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(q.empty(q.rstage));
+    if (++q.rstage == q.nstages) q.rstage = 0;
   };
+  if (it.m_t * BM + wg * 64 >= p.M) {      // this warpgroup's rows are all padding: pass the stages through
+    for (int kb = 0; kb < it.k_blocks; ++kb) {
+      mbar_wait(q.full(q.stage), q.phase);
+      if (++q.stage == q.nstages) { q.stage = 0; q.phase ^= 1u; }
+      release();
+    }
+    return;
+  }
+  const int m0 = arow ^ (t << 3), m1 = (arow + 8) ^ (t << 3);     // the rows r of this thread's elements are = t (mod 4)
+  auto acquire = [&](uint32_t (&ah)[BK / 8][4], uint32_t (&al)[BK / 8][4]) {
+    mbar_wait(q.full(q.stage), q.phase);
+    const uint32_t sa = q.addr(q.stage);
+#pragma unroll
+    for (int ks = 0; ks < BK / 8; ++ks) {
+      const int r = ks * 8 + t;
+      const float x0 = lds_f32(sa + (uint32_t)(r * BM + m0) * 4u), x1 = lds_f32(sa + (uint32_t)(r * BM + m1) * 4u);
+      const float x2 = lds_f32(sa + (uint32_t)((r + 4) * BM + m0) * 4u), x3 = lds_f32(sa + (uint32_t)((r + 4) * BM + m1) * 4u);
+      ah[ks][0] = tf32_hi(x0); ah[ks][1] = tf32_hi(x1); ah[ks][2] = tf32_hi(x2); ah[ks][3] = tf32_hi(x3);
+      al[ks][0] = tf32_lo(x0); al[ks][1] = tf32_lo(x1); al[ks][2] = tf32_lo(x2); al[ks][3] = tf32_lo(x3);
+    }
+    if (++q.stage == q.nstages) { q.stage = 0; q.phase ^= 1u; }
+    return sa + (uint32_t)WA_TILE;
+  };
+  float acc[BN / 2];
+#pragma unroll
+  for (int e = 0; e < BN / 2; ++e) acc[e] = 0.f;
+  uint32_t ah0[BK / 8][4], al0[BK / 8][4], ah1[BK / 8][4], al1[BK / 8][4];
+  uint32_t sb0 = acquire(ah0, al0), sb1 = 0;
+  for (int kb = 0; kb < it.k_blocks; kb += 2) {
+    issue_kblock<BN, true>(acc, ah0, al0, sb0, b_tile);
+    wgmma_wait<1>();
+    if (kb > 0) release();
+    if (kb + 1 >= it.k_blocks) break;
+    sb1 = acquire(ah1, al1);
+    issue_kblock<BN, true>(acc, ah1, al1, sb1, b_tile);
+    wgmma_wait<1>();
+    release();
+    if (kb + 2 < it.k_blocks) sb0 = acquire(ah0, al0);
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int e = 0; e < BN / 2; ++e) fence_operand(acc[e]);
+  release();
 
-  float acc[2][NJ_MAX][4];
+  // element (row0 + 8i, col0 + 8j + {0, 1}); Nld % 4 == 0 and the column even: a pair is all in or all out
+  const int row0 = it.m_t * BM + arow, col0 = it.n_t * BN + 2 * t;
+  float* slab = p.partial + (long long)it.split * p.M * p.Nld;
 #pragma unroll
-  for (int mi = 0; mi < 2; ++mi)
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = col0 + 8 * j;
 #pragma unroll
-    for (int j = 0; j < NJ_MAX; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) acc[mi][j][e] = 0.f;
+    for (int i = 0; i < 2; ++i) {
+      const int row = row0 + 8 * i;
+      if (col < p.Nld && row < p.M)
+        *reinterpret_cast<float2*>(slab + (long long)row * p.Nld + col) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+    }
+  }
+}
 
-  if (it.k_blocks > 0) load(0, 0);
-  for (int kb = 0; kb < it.k_blocks; ++kb) {
-    if (kb + 1 < it.k_blocks) { load(kb + 1, (kb + 1) & 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
-    __syncthreads();
-    const float* sA = wsm + (kb & 1) * stage_floats;
-    const float* sB = sA + WBK * LDA_W;
+template <int BN>
+__global__ void __launch_bounds__(W_THREADS, 1)
+tc_wgrad_kernel(const __grid_constant__ WGroup g) {
+  constexpr int NQ = (BN / 4 + 3) / 4;      // X quads (4 columns) per producer thread and k-block
+  extern __shared__ uint8_t smem_raw[];
+  pdl_launch_dependents();
+  WRing q;
+  q.base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  q.stage_bytes = (uint32_t)w_stage_bytes(BN);
+  q.nstages = w_nstages(BN);
+  q.bar_base = q.base + (uint32_t)(w_nstages(BN) * w_stage_bytes(BN));
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(q.full(s), 128); mbar_init(q.empty(s), 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  pdl_wait();          // everything above is private to this CTA; the previous kernel's output is first touched below
+
+  if (warp >= 8) {
+    // ===== producer warpgroup ======================================================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 120;" ::: "memory");
+    const int pt = threadIdx.x - 256, pw = warp - 8;
+    // X row (r_begin + 32 kb + lane), quads pw, pw + 4, ... of the item's n tile -> registers
+    auto load_x = [&](const WItem& it, int kb, float4 (&xv)[NQ]) {
+      const WP& p = g.it[it.pi];
+      const int r = it.r_begin + kb * BK + lane, nq = BN / 4, c0 = it.n_t * BN;
+      const float* src = p.X + (long long)r * p.ldx;
 #pragma unroll
-    for (int ks = 0; ks < WBK / 8; ++ks) {
-      const int k0 = ks * 8 + t;
-      uint32_t ah[2][4], al[2][4];
-#pragma unroll
-      for (int mi = 0; mi < 2; ++mi) {
-        const int m = wm * 32 + mi * 16 + gq;
-        const float x0 = sA[k0 * LDA_W + m], x1 = sA[k0 * LDA_W + m + 8];
-        const float x2 = sA[(k0 + 4) * LDA_W + m], x3 = sA[(k0 + 4) * LDA_W + m + 8];
-        ah[mi][0] = tf32_hi(x0); ah[mi][1] = tf32_hi(x1); ah[mi][2] = tf32_hi(x2); ah[mi][3] = tf32_hi(x3);
-        al[mi][0] = tf32_lo(x0); al[mi][1] = tf32_lo(x1); al[mi][2] = tf32_lo(x2); al[mi][3] = tf32_lo(x3);
+      for (int i = 0; i < NQ; ++i) {
+        const int qd = pw + 4 * i, c = c0 + 4 * qd;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (qd < nq && r < it.r_end) {
+          if (c < p.N) v = __ldg(reinterpret_cast<const float4*>(src + c));
+          else if (c == p.N) v.x = 1.f;
+        }
+        xv[i] = v;
       }
+    };
+    auto produce = [&](const WItem& it, int kb, const float4 (&xv)[NQ]) {
+      const WP& p = g.it[it.pi];
+      mbar_wait(q.empty(q.stage), q.phase ^ 1u);
+      const uint32_t sa = q.addr(q.stage), full = q.full(q.stage);
+      const int r0 = it.r_begin + kb * BK, mc0 = it.m_t * BM;
 #pragma unroll
-      for (int j = 0; j < NJ_MAX; ++j) {
-        if (j < nj) {
-          const int n = wn * (p.BN >> 1) + j * 8 + gq;
-          const float y0 = sB[k0 * ldb + n], y1 = sB[(k0 + 4) * ldb + n];
-          const uint32_t bh0 = tf32_hi(y0), bh1 = tf32_hi(y1), bl0 = tf32_lo(y0), bl1 = tf32_lo(y1);
-          mma_tf32x3(acc[0][j], ah[0], al[0], bh0, bh1, bl0, bl1);
-          mma_tf32x3(acc[1][j], ah[1], al[1], bh0, bh1, bl0, bl1);
+      for (int j = 0; j < BK * BM / 4 / 128; ++j) {
+        const int v = pt + 128 * j, r = v >> 5, c = (v & 31) * 4;
+        const bool ok = r0 + r < it.r_end && mc0 + c < p.M;
+        cp_async16(sa + wa_offset(r, c), ok ? p.dY + (long long)(r0 + r) * p.ldy + mc0 + c : p.dY, ok ? 16u : 0u);
+      }
+      asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(full) : "memory");
+      const uint32_t sb = sa + (uint32_t)WA_TILE, sl = sb + (uint32_t)BN * 128u;
+      const int nq = BN / 4;
+#pragma unroll
+      for (int i = 0; i < NQ; ++i) {
+        const int qd = pw + 4 * i;
+        if (qd < nq) {
+          const float e[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const uint32_t off = sw128_offset(4 * qd + k, lane);
+            sts_f32(sb + off, __uint_as_float(tf32_hi(e[k])));
+            sts_f32(sl + off, __uint_as_float(tf32_lo(e[k])));
+          }
         }
       }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> wgmma's reads
+      mbar_arrive(full);
+      if (++q.stage == q.nstages) { q.stage = 0; q.phase ^= 1u; }
+    };
+    // (item, k-block) walk.  The X rows of the next k-block are prefetched into L2 while the current one is written,
+    // so the loads at the top of the next step see L2 latency (a second register buffer would not fit next to BN = 160).
+    const int total = g.total_items;
+    int w = blockIdx.x, kb = 0;
+    while (w < total) {
+      const WItem it = wgrad_item(g, w);
+      int nw = w, nkb = kb + 1;
+      if (nkb == it.k_blocks) { nw += gridDim.x; nkb = 0; }
+      float4 xv[NQ];
+      load_x(it, kb, xv);
+      if (nw < total) {
+        const WItem nt = wgrad_item(g, nw);
+        const WP& p = g.it[nt.pi];
+        const int r = nt.r_begin + nkb * BK + lane;
+        if (r < nt.r_end)
+          for (int c = 32 * pw; c < BN; c += 128)       // one prefetch per 128-byte line of this row's tile segment
+            if (nt.n_t * BN + c < p.N) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.X + (long long)r * p.ldx + nt.n_t * BN + c));
+      }
+      produce(it, kb, xv);
+      w = nw; kb = nkb;
     }
-    __syncthreads();
+    return;
   }
 
-  // ---- partial tile -> slab [split][Mpad][Nld] ------------------------------------------------------
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi) {
-#pragma unroll
-    for (int j = 0; j < NJ_MAX; ++j) {
-      if (j < nj) {
-        const int n = ncol0 + wn * (p.BN >> 1) + j * 8 + 2 * t;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const long long m = (long long)it.split * p.Mpad + mcol0 + wm * 32 + mi * 16 + gq + 8 * i;
-          *reinterpret_cast<float2*>(p.partial + m * p.Nld + n) = make_float2(acc[mi][j][2 * i], acc[mi][j][2 * i + 1]);
-        }
-      }
-    }
+  // ===== warpgroups 0, 1: MMA ======================================================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 192;" ::: "memory");
+  const int wg = warp >> 2, wq = warp & 3, gq = lane >> 2, t = lane & 3;
+  const int arow = wg * 64 + wq * 16 + gq;
+  for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
+    const WItem it = wgrad_item(g, w);
+    wgrad_consume<BN>(g.it[it.pi], it, q, wg, arow, t);
   }
 }
 
@@ -471,21 +576,22 @@ __global__ void wgrad_reduce_kernel(const __grid_constant__ RGroup g) {
   }
 }
 
-struct WPlan { int BN, n_tiles, m_tiles, nsplit, rows_per_split, Mpad, Nld; };
-// `rows_target`: contraction rows per work item.  512 sizes the partial buffers (the CAPACITY in row splits); the grouped
-// launch may raise it so that the item count of the whole group fills whole waves (one CTA per work item; at ~170
-// registers x 256 threads one CTA is resident per SM, so a wave is num_sms() items).
-WPlan wgrad_plan(int M, int N, long long rows, int rows_target = 512) {
-  WPlan w;
-  w.m_tiles = (int)ceil_div(M, BM);
-  w.Mpad = w.m_tiles * BM;
-  const int Ncols = N + 1;                                  // + the ones column
-  w.n_tiles = (int)ceil_div(Ncols, MAX_BN);
-  w.BN = (int)round_up(ceil_div(Ncols, w.n_tiles), 32);     // whole 32-column TMA boxes
-  w.Nld = (int)round_up(w.n_tiles * w.BN, 4);
-  // row splits: ~512 rows (16 k-blocks) per item so the pipeline amortises its fill, but never more than
-  // ~2 rounds of items per problem (bounds the partial buffer for the big configurations)
-  const int mn = w.m_tiles * w.n_tiles;
+static const int kWgWidths[] = {
+#define RD_WG_LIST(W) W,
+    RD_WG_WIDTHS(RD_WG_LIST)
+#undef RD_WG_LIST
+};
+
+// Row splits of one problem for a target of `rows_target` rows per split.  They depend on the shapes alone, never on the
+// tile width, so every width computes each element of a split as the same product sequence (bitwise equal results).
+// ~512 rows (16 k-blocks) per item so the pipeline amortises its fill, but never more than ~2 rounds of items per
+// problem in 128 x 160 tiles (bounds the partial buffer for the big configurations).  512 sizes the partial buffers
+// (the CAPACITY in row splits); wgrad_rows_target may raise it for a group, which only lowers the split count.
+struct WSplit { int nsplit, rows_per_split, Nld; };
+WSplit wgrad_split(int M, int N, long long rows, int rows_target = 512) {
+  WSplit w;
+  w.Nld = (int)round_up(N + 1, 4);                          // + the ones column
+  const long long mn = ceil_div(M, BM) * ceil_div(N + 1, MAX_BN);
   long long ns = ceil_div(rows, rows_target);
   const long long cap = (2 * num_sms()) / mn > 1 ? (2 * num_sms()) / mn : 1;
   if (ns > cap) ns = cap;
@@ -493,6 +599,47 @@ WPlan wgrad_plan(int M, int N, long long rows, int rows_target = 512) {
   w.rows_per_split = (int)round_up(ceil_div(rows, ns), BK);
   w.nsplit = (int)ceil_div(rows, w.rows_per_split);
   return w;
+}
+
+// Rows per split of a group: the smallest target >= 512 (in steps of 32, up to 1024) for which the group's count of
+// 128 x 160 work items fills whole waves of the SMs.  With the same splits (and per split the same k-block and k-step
+// order of lo.hi, hi.lo, hi.hi) every weight gradient is bitwise the one the mma.sync kernel this one replaced gave.
+int wgrad_rows_target(const WgradItem* items, int n) {
+  auto count_items = [&](int target) {
+    long long t = 0;
+    for (int i = 0; i < n; ++i) {
+      const WgradItem& a = items[i];
+      t += (long long)wgrad_split(a.Nout, a.Kin, a.rows, target).nsplit * ceil_div(a.Nout, BM) * ceil_div(a.Kin + 1, MAX_BN);
+    }
+    return t;
+  };
+  const long long sms = num_sms(), t0 = count_items(512);
+  if (t0 > sms && t0 % sms) {
+    const long long goal = (t0 / sms) * sms;
+    for (int t = 544; t <= 1024; t += 32)
+      if (count_items(t) <= goal) return t;
+  }
+  return 512;
+}
+
+// Tile width of a group: the instantiated width that minimises the MMA work of the group's items, sum over items of
+// rows x (width + a per-tile overhead of 32 columns: the dY tile is staged and gathered once per n tile), computed and
+// padded columns alike; ties go to the wider tile (fewer n tiles).  RD_TC_WGRAD_BN=<width> forces a listed width
+// (tests compare widths on the same problems).
+int wgrad_width(const WgradItem* items, int n) {
+  if (const char* e = getenv("RD_TC_WGRAD_BN")) {
+    const int f = atoi(e);
+    for (int bn : kWgWidths) if (bn == f) return f;         // not a listed width: ignored
+  }
+  int best_bn = MAX_BN;
+  long long best = -1;
+  for (int bn : kWgWidths) {
+    long long cost = 0;
+    for (int i = 0; i < n; ++i)
+      cost += ceil_div(items[i].Nout, BM) * ceil_div(items[i].Kin + 1, bn) * items[i].rows * (bn + 32);
+    if (best < 0 || cost <= best) { best = cost; best_bn = bn; }
+  }
+  return best_bn;
 }
 
 struct SplitItems { WeightSplit it[16]; long long start[17]; int n; StepPrologue pro; };
@@ -710,8 +857,8 @@ bool tc_wgrad_supported(int Nout, int Kin, long long ldy, long long ldx, const v
 }
 
 long long tc_wgrad_partial_floats(int Nout, int Kin, long long rows) {
-  WPlan w = wgrad_plan(Nout, Kin, rows);
-  return round_up((long long)w.nsplit * w.Mpad * w.Nld, 64);
+  const WSplit w = wgrad_split(Nout, Kin, rows);
+  return round_up((long long)w.nsplit * Nout * w.Nld, 64);
 }
 
 int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st) {
@@ -720,22 +867,9 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
   WGroup g;
   RGroup r;
   g.n = n; r.n = n + (ncs > 0 ? ncs : 0);
-  // rows per work item: the smallest target >= 512 for which the group's item count fills whole waves of the grid
-  auto count_items = [&](int target) {
-    long long t = 0;
-    for (int i = 0; i < n; ++i) { const WPlan w = wgrad_plan(items[i].Nout, items[i].Kin, items[i].rows, target); t += (long long)w.nsplit * w.m_tiles * w.n_tiles; }
-    return t;
-  };
-  int target = 512;
-  if (n > 0) {
-    const long long sms = num_sms(), t0 = count_items(512);
-    if (t0 > sms && t0 % sms) {
-      const long long goal = (t0 / sms) * sms;
-      for (int t = 544; t <= 1024; t += 32)
-        if (count_items(t) <= goal) { target = t; break; }
-    }
-  }
-  int item = 0, max_bn = 32;
+  WSplit sp[WG_MAX];
+  const int target = n > 0 ? wgrad_rows_target(items, n) : 512;
+  int order[WG_MAX];
   long long tot = 0;
   for (int i = 0; i < n; ++i) {
     const WgradItem& a = items[i];
@@ -744,25 +878,36 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
       set_error("tc_wgrad_group: problem %d has an unsupported shape/alignment", i);
       return -2;
     }
-    const WPlan w = wgrad_plan(a.Nout, a.Kin, a.rows, target);
-    WP& p = g.it[i];
-    p.partial = a.partial;
-    p.rows = a.rows; p.M = a.Nout; p.N = a.Kin;
-    p.dY = a.dY; p.X = a.X; p.ldy = a.ldy; p.ldx = a.ldx;
-    p.BN = w.BN; p.n_tiles = w.n_tiles; p.m_tiles = w.m_tiles; p.nsplit = w.nsplit; p.rows_per_split = w.rows_per_split;
-    p.Mpad = w.Mpad; p.Nld = w.Nld;
-    if (p.BN > max_bn) max_bn = p.BN;
     if (a.rows > 0x7fffffffLL) { set_error("tc_wgrad_group: too many rows"); return -2; }
-    p.item0 = item;
-    item += w.nsplit * w.m_tiles * w.n_tiles;
+    const WSplit& w = sp[i] = wgrad_split(a.Nout, a.Kin, a.rows, target);
+    order[i] = i;
     RItem& q = r.it[i];
-    q.partial = a.partial; q.dW = a.dW; q.db = a.db; q.nsplit = w.nsplit; q.M = a.Nout; q.N = a.Kin; q.Mpad = w.Mpad; q.Nld = w.Nld;
+    q.partial = a.partial; q.dW = a.dW; q.db = a.db; q.nsplit = w.nsplit; q.M = a.Nout; q.N = a.Kin; q.Mpad = a.Nout; q.Nld = w.Nld;
     q.kind = 0; q.stride = 0;
     q.start = tot;
     tot += (long long)a.Nout * (a.Kin / 4 + 1);
   }
+  const int BN = n > 0 ? wgrad_width(items, n) : MAX_BN;
+  // the persistent grid deals the items round robin: problems with the longest items (rows per split) go first
+  for (int i = 1; i < n; ++i)
+    for (int j = i; j > 0 && sp[order[j]].rows_per_split > sp[order[j - 1]].rows_per_split; --j) {
+      const int t = order[j]; order[j] = order[j - 1]; order[j - 1] = t;
+    }
+  int item = 0;
+  for (int k = 0; k < n; ++k) {
+    const WgradItem& a = items[order[k]];
+    const WSplit& w = sp[order[k]];
+    WP& p = g.it[k];
+    p.partial = a.partial;
+    p.rows = (int)a.rows; p.M = a.Nout; p.N = a.Kin; p.Nld = w.Nld;
+    p.dY = a.dY; p.X = a.X; p.ldy = a.ldy; p.ldx = a.ldx;
+    p.n_tiles = (int)ceil_div(a.Kin + 1, BN); p.m_tiles = (int)ceil_div(a.Nout, BM);
+    p.nsplit = w.nsplit; p.rows_per_split = w.rows_per_split;
+    p.item0 = item;
+    item += w.nsplit * p.m_tiles * p.n_tiles;
+  }
   g.total_items = item;
-  const int smem_bytes = 2 * (WBK * LDA_W + WBK * (max_bn + 8)) * (int)sizeof(float);
+  const int smem_bytes = 1280 + w_nstages(BN) * w_stage_bytes(BN);
   for (int i = 0; i < ncs; ++i) {
     RItem& q = r.it[n + i];
     q.partial = cs[i].partial; q.dW = cs[i].out; q.db = nullptr; q.nsplit = cs[i].nsplit; q.M = 1; q.N = cs[i].ncols;
@@ -773,8 +918,20 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
   }
   r.total = tot;
   if (n > 0) {
-    RD_TRY(ensure_max_smem((const void*)tc_wgrad_kernel, smem_bytes));
-    launch_pdl(tc_wgrad_kernel, dim3(item), dim3(W_THREADS), smem_bytes, st, g);
+    const int grid = item < num_sms() ? item : num_sms();
+    auto launch = [&](auto kern) -> int {
+      RD_TRY(ensure_max_smem((const void*)kern, SMEM_LIMIT));
+      launch_pdl(kern, dim3(grid), dim3(W_THREADS), smem_bytes, st, g);
+      return 0;
+    };
+    int rc = -2;
+    switch (BN) {
+#define RD_WG_CASE(W) case W: rc = launch(tc_wgrad_kernel<W>); break;
+      RD_WG_WIDTHS(RD_WG_CASE)
+#undef RD_WG_CASE
+      default: break;
+    }
+    if (rc != 0) { set_error("tc_wgrad_group: tile width %d not instantiated", BN); return -2; }
     RD_CHECK_LAUNCH("tc_wgrad_kernel");
   }
   launch_pdl(wgrad_reduce_kernel, dim3((unsigned)ceil_div(tot, 256)), dim3(256), 0, st, r);

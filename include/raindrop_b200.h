@@ -546,6 +546,12 @@ int rd_debug_attention_timing(uint64_t* buffer);
 /* same for the tensor-core GEMM kernel (rd_linear_fwd, the encoder and ob-prop GEMMs): [n_ctas][8] uint64,
  * %globaltimer at the CTA's start (slot 0) and end (slot 7) */
 int rd_debug_gemm_timing(uint64_t* buffer);
+/* same for the grouped weight-gradient kernel (rd_linear_wgrad_group and the training backward): [n_ctas][16] uint64
+ * per launch CTA (at most one per SM), clock64 at the CTA's start (slot 0) and end (1); summed cycles of the producer
+ * waiting for an empty stage (2), for its X tile (3), transposing and storing it (4); of MMA thread 0 waiting for a full
+ * stage (5) and in its epilogue (6); %globaltimer ns from start to end (7); k-blocks produced (8); the producer's end
+ * (9); the producer's cycles issuing the loads of a released stage (10).  Each launch overwrites the buffer. */
+int rd_debug_wgrad_timing(uint64_t* buffer);
 
 /* debug: materialise the dropout keep/scale mask (0 or 1/(1-p)) of one dropout site, so tests can
  * replay train-mode forward/backward in the oracle with identical masks.  `site` ids in DESIGN.md. */

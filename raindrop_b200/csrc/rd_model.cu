@@ -817,6 +817,7 @@ int rd_linear_fwd(const float* x, const float* weight, const float* bias, int64_
 
 int rd_debug_attention_timing(uint64_t* buffer) { attn_tc_set_debug((unsigned long long*)buffer); return 0; }
 int rd_debug_gemm_timing(uint64_t* buffer) { tc_gemm_set_debug((unsigned long long*)buffer); return 0; }
+int rd_debug_wgrad_timing(uint64_t* buffer) { tc_wgrad_set_debug((unsigned long long*)buffer); return 0; }
 
 int rd_temporal_attention_fwd(const float* qkv, const int64_t* lengths, int32_t B, int32_t H, int32_t T, int32_t hd,
                               float drop_p, const uint64_t* rng_captured, uint32_t site, int32_t impl, float* ctx,

@@ -18,8 +18,9 @@
 //
 // tc_wgrad_group: dW = dY^T X (+ db) for up to WG_MAX problems in one launch.  Both operands are activations whose
 // contraction index runs over their ROWS; wgmma's TF32 form only reads K-major operands from shared memory, so dY^T is
-// gathered into registers from a row-major stage and X is transposed by a producer warpgroup into the K-major swizzled
-// image wgmma reads (tc_wgrad_kernel below), followed by a fixed-order split-K reduce.
+// gathered into registers from a row-major stage and X, delivered by TMA several k-blocks ahead, is transposed in shared
+// memory by a producer warpgroup into the K-major swizzled image wgmma reads (tc_wgrad_kernel below), followed by a
+// fixed-order split-K reduce.
 #include <stdlib.h>
 
 #include "rd_tc_common.cuh"
@@ -282,10 +283,12 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 //   D_k[m, n] = sum_r A_k[r, m] * B_k[r, n]   (A = dY, B = X plus a "ones" column N for the bias gradient)
 // over one row split of problem k per work item (problem, m tile, n tile, split).  A training step has ten of these
 // (8 encoder weights + 2 lin_value).  Persistent: one CTA per SM walks the items blockIdx.x, + gridDim.x, ...
-//   warpgroup 2   producer, 128 threads.  Per 32-row k-block: the dY tile [32 x 128] by cp.async into a row-major
-//                 stage (column XOR-ed with 8 (r % 4), see wa_offset), completion tracked on the stage's mbarrier; the
-//                 X tile [32 x BN] through registers (loaded one k-block ahead), TRANSPOSED into the K-major 128B-swizzled
-//                 image wgmma reads (sw128_offset(n, r)) as hi = top 19 bits and lo = exact remainder, with the ones
+//   warpgroup 2   producer, 128 threads.  Per 32-row k-block, issued nstages - 2 k-blocks ahead as soon as the stage
+//                 is released: the dY tile [32 x 128] by cp.async into a row-major stage (column XOR-ed with 8 (r % 4),
+//                 see wa_offset), completion tracked on the stage's full mbarrier; the raw X tile [32 x BN] by TMA
+//                 (32 x 32 boxes, 128B swizzle) into the stage's hi | lo region, on its own mbarrier.  When the
+//                 k-block's turn comes, the X tile is read into registers and TRANSPOSED into the K-major 128B-swizzled
+//                 images wgmma reads (sw128_offset(n, r)) as hi = top 19 bits and lo = exact remainder, with the ones
 //                 column written here (TMA cannot synthesise it).  Lane = row r and a warp's 32 stores share n, so
 //                 (((r >> 2) ^ n) & 7) * 4 + r % 4 hits 32 distinct banks.  fence.proxy.async, then arrive.
 //   warpgroups    0 and 1: dW rows 0-63 and 64-127 of the tile, one wgmma.m64nBNk8 per k-step and term (lo.hi, hi.lo,
@@ -297,12 +300,28 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 // widths dispatched per item inside one kernel, ptxas serialises the wgmma for lack of registers (C7512).
 // =================================================================================================
 struct WP {
-  const float* dY; const float* X; long long ldy, ldx;
+  const float* dY; long long ldy;    // X arrives through WGroup::tmX
   float* partial;                    // [nsplit][M][Nld]
   int rows, M, N, Nld, n_tiles, m_tiles, nsplit, rows_per_split;
   int item0;                         // first work item of this problem inside the grouped list
 };
-struct WGroup { WP it[WG_MAX]; int n, total_items; };
+struct WGroup {
+  CUtensorMap tmX[WG_MAX];           // X of problem k: dims {Kin, rows}, boxes of 32 columns x 32 rows, 128B swizzle
+  WP it[WG_MAX]; int n, total_items;
+  unsigned long long* dbg;           // optional per-CTA phase cycles [CTA][16] (rd_debug_wgrad_timing)
+};
+
+// Phase timing of one CTA, clock64 deltas summed in registers and written once at the end when WGroup::dbg is set.
+// Slots: 0 / 1 clock64 at the start (after the grid dependency wait) / end of MMA thread 0; 2 / 3 / 4 the producer's
+// (thread 256) cycles waiting for an empty stage / for its X tile / transposing and storing; 5 / 6 MMA thread 0's cycles
+// waiting for a full stage / in the slab-store epilogue; 7 %globaltimer ns from start to end (the clock rate); 8 the
+// k-blocks the CTA produced; 9 clock64 at the producer's end; 10 the producer's cycles issuing the loads of a released
+// stage.
+__device__ __forceinline__ unsigned long long gtimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
 
 constexpr int W_THREADS = 384;            // warpgroups 0, 1: MMA; warpgroup 2: producer
 constexpr int WA_TILE = BK * BM * 4;      // 16 KB: 32 rows of dY x 128 columns
@@ -319,6 +338,11 @@ __device__ __forceinline__ uint32_t wa_offset(int r, int m) { return (uint32_t)(
 
 __device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+__device__ __forceinline__ float4 lds_v4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
 }
 
 struct WItem { int pi, n_t, m_t, split, k_blocks, r_begin, r_end; };
@@ -341,12 +365,15 @@ struct WRing {
   int nstages, stage = 0, rstage = 0;
   __device__ uint32_t full(int s) const { return bar_base + 8u * s; }
   __device__ uint32_t empty(int s) const { return bar_base + 8u * (MAX_STAGES + s); }
+  __device__ uint32_t xfull(int s) const { return bar_base + 8u * (2 * MAX_STAGES + s); }    // the stage's raw X tile
   __device__ uint32_t addr(int s) const { return base + (uint32_t)s * stage_bytes; }
 };
 
-// one item on MMA warpgroup `wg`: k-blocks -> accumulators -> this split's slab
+// one item on MMA warpgroup `wg`: k-blocks -> accumulators -> this split's slab; adds its cycles waiting for full stages
+// to t_full and in the epilogue to t_epi
 template <int BN>
-__device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRing& q, int wg, int arow, int t) {
+__device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRing& q, int wg, int arow, int t,
+                                              long long& t_full, long long& t_epi) {
   constexpr uint32_t b_tile = (uint32_t)BN * 128u;
   auto release = [&]() {
     __syncwarp();
@@ -363,7 +390,9 @@ __device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRin
   }
   const int m0 = arow ^ (t << 3), m1 = (arow + 8) ^ (t << 3);     // the rows r of this thread's elements are = t (mod 4)
   auto acquire = [&](uint32_t (&ah)[BK / 8][4], uint32_t (&al)[BK / 8][4]) {
+    const long long c0 = clock64();
     mbar_wait(q.full(q.stage), q.phase);
+    t_full += clock64() - c0;
     const uint32_t sa = q.addr(q.stage);
 #pragma unroll
     for (int ks = 0; ks < BK / 8; ++ks) {
@@ -398,6 +427,7 @@ __device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRin
   release();
 
   // element (row0 + 8i, col0 + 8j + {0, 1}); Nld % 4 == 0 and the column even: a pair is all in or all out
+  const long long c0 = clock64();
   const int row0 = it.m_t * BM + arow, col0 = it.n_t * BN + 2 * t;
   float* slab = p.partial + (long long)it.split * p.M * p.Nld;
 #pragma unroll
@@ -410,12 +440,16 @@ __device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRin
         *reinterpret_cast<float2*>(slab + (long long)row * p.Nld + col) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
     }
   }
+  t_epi += clock64() - c0;
 }
 
 template <int BN>
 __global__ void __launch_bounds__(W_THREADS, 1)
 tc_wgrad_kernel(const __grid_constant__ WGroup g) {
   constexpr int NQ = (BN / 4 + 3) / 4;      // X quads (4 columns) per producer thread and k-block
+  constexpr int NBOX = (BN + 31) / 32;      // 32-column TMA boxes of X per k-block
+  static_assert(NBOX * 4096 <= 2 * BN * 128, "the raw X boxes land in the stage's hi | lo images");
+  static_assert(w_nstages(BN) >= 3, "the producer issues nstages - 2 k-blocks ahead of the one it transposes");
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();
   WRing q;
@@ -425,46 +459,88 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
   q.bar_base = q.base + (uint32_t)(w_nstages(BN) * w_stage_bytes(BN));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(q.full(s), 128); mbar_init(q.empty(s), 8); }
+    for (int k = 0; k < g.n; ++k) asm volatile("prefetch.tensormap [%0];" ::"l"(&g.tmX[k]) : "memory");
+    for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(q.full(s), 128); mbar_init(q.empty(s), 8); mbar_init(q.xfull(s), 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();          // everything above is private to this CTA; the previous kernel's output is first touched below
+  const long long clk0 = clock64();
+  const unsigned long long gt0 = gtimer();
+  unsigned long long* const dbg = g.dbg ? g.dbg + (size_t)blockIdx.x * 16 : nullptr;
 
   if (warp >= 8) {
     // ===== producer warpgroup ======================================================================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 120;" ::: "memory");
     const int pt = threadIdx.x - 256, pw = warp - 8;
-    // X row (r_begin + 32 kb + lane), quads pw, pw + 4, ... of the item's n tile -> registers
-    auto load_x = [&](const WItem& it, int kb, float4 (&xv)[NQ]) {
-      const WP& p = g.it[it.pi];
-      const int r = it.r_begin + kb * BK + lane, nq = BN / 4, c0 = it.n_t * BN;
-      const float* src = p.X + (long long)r * p.ldx;
+    const int total = g.total_items;
+    long long t_empty = 0, t_x = 0, t_store = 0, t_issue = 0, n_kb = 0;
+    // Two cursors walk the same (item, k-block) sequence.  The issue cursor sends a k-block's loads into its stage as
+    // soon as the MMA warpgroups release it: dY by cp.async (completion on the stage's full barrier), X by TMA (on the
+    // stage's xfull barrier).  It runs nstages - 2 k-blocks ahead of the transpose cursor: the stage one further ahead
+    // is released only after the consumers acquired the k-block being transposed.  The work item of each cursor is
+    // computed once per item: the walk over the group's problems reads kernel parameters at a register index.
+    int iw = blockIdx.x, ikb = 0, istage = 0, ahead = 0;
+    uint32_t iphase = 0;
+    WItem iit = wgrad_item(g, iw);
+    auto issue = [&]() {
+      const WP& p = g.it[iit.pi];
+      const long long c0 = clock64();
+      mbar_wait(q.empty(istage), iphase ^ 1u);
+      const long long c1 = clock64();
+      t_empty += c1 - c0;
+      const uint32_t sa = q.addr(istage);
+      const int r0 = iit.r_begin + ikb * BK, mc0 = iit.m_t * BM;
+      if (pt == 0) {      // rows past `rows` and columns past Kin arrive as zeros
+        mbar_expect_tx(q.xfull(istage), NBOX * 4096u);
 #pragma unroll
-      for (int i = 0; i < NQ; ++i) {
-        const int qd = pw + 4 * i, c = c0 + 4 * qd;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (qd < nq && r < it.r_end) {
-          if (c < p.N) v = __ldg(reinterpret_cast<const float4*>(src + c));
-          else if (c == p.N) v.x = 1.f;
-        }
-        xv[i] = v;
+        for (int b = 0; b < NBOX; ++b)
+          tma_load_2d(&g.tmX[iit.pi], q.xfull(istage), sa + (uint32_t)WA_TILE + 4096u * b, iit.n_t * BN + 32 * b, r0);
       }
-    };
-    auto produce = [&](const WItem& it, int kb, const float4 (&xv)[NQ]) {
-      const WP& p = g.it[it.pi];
-      mbar_wait(q.empty(q.stage), q.phase ^ 1u);
-      const uint32_t sa = q.addr(q.stage), full = q.full(q.stage);
-      const int r0 = it.r_begin + kb * BK, mc0 = it.m_t * BM;
 #pragma unroll
       for (int j = 0; j < BK * BM / 4 / 128; ++j) {
         const int v = pt + 128 * j, r = v >> 5, c = (v & 31) * 4;
-        const bool ok = r0 + r < it.r_end && mc0 + c < p.M;
+        const bool ok = r0 + r < iit.r_end && mc0 + c < p.M;
         cp_async16(sa + wa_offset(r, c), ok ? p.dY + (long long)(r0 + r) * p.ldy + mc0 + c : p.dY, ok ? 16u : 0u);
       }
-      asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(full) : "memory");
-      const uint32_t sb = sa + (uint32_t)WA_TILE, sl = sb + (uint32_t)BN * 128u;
-      const int nq = BN / 4;
+      asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(q.full(istage)) : "memory");
+      if (++istage == q.nstages) { istage = 0; iphase ^= 1u; }
+      t_issue += clock64() - c1;
+      if (++ikb == iit.k_blocks) {
+        ikb = 0; iw += gridDim.x;
+        if (iw < total) iit = wgrad_item(g, iw);
+      }
+    };
+    // The transpose cursor: the raw X tile (NBOX boxes of 32 rows x 32 columns, 128B-swizzled, at the start of the
+    // stage's hi image) -> registers, row r = lane and quads pw, pw + 4, ... of the n tile (a quarter warp's 16-byte
+    // loads hit 8 distinct chunks of 8 rows: conflict-free), with the ones column N of the bias gradient set here ->
+    // hi / lo images.
+    int w = blockIdx.x, kb = 0;
+    WItem it = iit;
+    while (w < total) {
+      for (; ahead < q.nstages - 1 && iw < total; ++ahead) issue();
+      const WP& p = g.it[it.pi];
+      const long long c0 = clock64();
+      mbar_wait(q.xfull(q.stage), q.phase);
+      const long long c1 = clock64();
+      const uint32_t sb = q.addr(q.stage) + (uint32_t)WA_TILE, sl = sb + (uint32_t)BN * 128u;
+      const int r = it.r_begin + kb * BK + lane, nq = BN / 4, c0n = it.n_t * BN;
+      float4 xv[NQ];
+#pragma unroll
+      for (int i = 0; i < NQ; ++i) {
+        const int qd = pw + 4 * i;
+        xv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (qd < nq) {
+          xv[i] = lds_v4(sb + 4096u * (uint32_t)(qd >> 3) + sw128_offset(lane, 4 * (qd & 7)));
+          if (c0n + 4 * qd == p.N && r < it.r_end) xv[i].x = 1.f;
+        }
+      }
+      asm volatile("bar.sync 1, 128;" ::: "memory");        // every raw read is done before the images overwrite it
+      // image row n = 4 qd + k = 4 pw + k + 16 i: the swizzle term depends on n % 8 only, so the offsets of quad i are
+      // those of quad 0 plus 16 i rows (keeps 4 address registers live instead of 4 NQ)
+      uint32_t off[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) off[k] = sw128_offset(4 * pw + k, lane);
 #pragma unroll
       for (int i = 0; i < NQ; ++i) {
         const int qd = pw + 4 * i;
@@ -472,36 +548,23 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
           const float e[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
-            const uint32_t off = sw128_offset(4 * qd + k, lane);
-            sts_f32(sb + off, __uint_as_float(tf32_hi(e[k])));
-            sts_f32(sl + off, __uint_as_float(tf32_lo(e[k])));
+            sts_f32(sb + off[k] + 2048u * i, __uint_as_float(tf32_hi(e[k])));
+            sts_f32(sl + off[k] + 2048u * i, __uint_as_float(tf32_lo(e[k])));
           }
         }
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> wgmma's reads
-      mbar_arrive(full);
+      mbar_arrive(q.full(q.stage));
       if (++q.stage == q.nstages) { q.stage = 0; q.phase ^= 1u; }
-    };
-    // (item, k-block) walk.  The X rows of the next k-block are prefetched into L2 while the current one is written,
-    // so the loads at the top of the next step see L2 latency (a second register buffer would not fit next to BN = 160).
-    const int total = g.total_items;
-    int w = blockIdx.x, kb = 0;
-    while (w < total) {
-      const WItem it = wgrad_item(g, w);
-      int nw = w, nkb = kb + 1;
-      if (nkb == it.k_blocks) { nw += gridDim.x; nkb = 0; }
-      float4 xv[NQ];
-      load_x(it, kb, xv);
-      if (nw < total) {
-        const WItem nt = wgrad_item(g, nw);
-        const WP& p = g.it[nt.pi];
-        const int r = nt.r_begin + nkb * BK + lane;
-        if (r < nt.r_end)
-          for (int c = 32 * pw; c < BN; c += 128)       // one prefetch per 128-byte line of this row's tile segment
-            if (nt.n_t * BN + c < p.N) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.X + (long long)r * p.ldx + nt.n_t * BN + c));
+      --ahead;
+      t_x += c1 - c0; t_store += clock64() - c1; ++n_kb;
+      if (++kb == it.k_blocks) {
+        kb = 0; w += gridDim.x;
+        if (w < total) it = wgrad_item(g, w);
       }
-      produce(it, kb, xv);
-      w = nw; kb = nkb;
+    }
+    if (dbg && pt == 0) {
+      dbg[2] = t_empty; dbg[3] = t_x; dbg[4] = t_store; dbg[8] = n_kb; dbg[9] = clock64(); dbg[10] = t_issue;
     }
     return;
   }
@@ -510,9 +573,13 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
   asm volatile("setmaxnreg.inc.sync.aligned.u32 192;" ::: "memory");
   const int wg = warp >> 2, wq = warp & 3, gq = lane >> 2, t = lane & 3;
   const int arow = wg * 64 + wq * 16 + gq;
+  long long t_full = 0, t_epi = 0;
   for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
     const WItem it = wgrad_item(g, w);
-    wgrad_consume<BN>(g.it[it.pi], it, q, wg, arow, t);
+    wgrad_consume<BN>(g.it[it.pi], it, q, wg, arow, t, t_full, t_epi);
+  }
+  if (dbg && threadIdx.x == 0) {
+    dbg[0] = clk0; dbg[1] = clock64(); dbg[5] = t_full; dbg[6] = t_epi; dbg[7] = gtimer() - gt0;
   }
 }
 
@@ -861,12 +928,16 @@ long long tc_wgrad_partial_floats(int Nout, int Kin, long long rows) {
   return round_up((long long)w.nsplit * Nout * w.Nld, 64);
 }
 
+static unsigned long long* g_wgrad_dbg = nullptr;
+void tc_wgrad_set_debug(unsigned long long* buf) { g_wgrad_dbg = buf; }
+
 int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st) {
   if (n <= 0 && ncs <= 0) return 0;
   if (n > WG_MAX || ncs > CS_MAX) { set_error("tc_wgrad_group: at most %d problems (+ %d column sums) per launch", WG_MAX, CS_MAX); return -2; }
   WGroup g;
   RGroup r;
   g.n = n; r.n = n + (ncs > 0 ? ncs : 0);
+  g.dbg = g_wgrad_dbg;
   WSplit sp[WG_MAX];
   const int target = n > 0 ? wgrad_rows_target(items, n) : 512;
   int order[WG_MAX];
@@ -900,7 +971,13 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
     WP& p = g.it[k];
     p.partial = a.partial;
     p.rows = (int)a.rows; p.M = a.Nout; p.N = a.Kin; p.Nld = w.Nld;
-    p.dY = a.dY; p.X = a.X; p.ldy = a.ldy; p.ldx = a.ldx;
+    p.dY = a.dY; p.ldy = a.ldy;
+    {
+      cuuint64_t d[2] = {(cuuint64_t)a.Kin, (cuuint64_t)a.rows};
+      cuuint64_t s[1] = {(cuuint64_t)a.ldx * 4};
+      cuuint32_t b[2] = {BK, BK};
+      RD_TRY(encode(&g.tmX[k], a.X, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "X"));
+    }
     p.n_tiles = (int)ceil_div(a.Kin + 1, BN); p.m_tiles = (int)ceil_div(a.Nout, BM);
     p.nsplit = w.nsplit; p.rows_per_split = w.rows_per_split;
     p.item0 = item;

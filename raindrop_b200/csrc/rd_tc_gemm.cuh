@@ -68,6 +68,7 @@ struct WgradItem { const float* dY; long long ldy; const float* X; long long ldx
 constexpr int CS_MAX = 36;
 struct ColsumItem { const float* partial; long long stride; int nsplit, ncols; float* out; };
 int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st);
+void tc_wgrad_set_debug(unsigned long long* buf);    // per-CTA phase cycles [CTA][16] of tc_wgrad_kernel (debug)
 
 // One launch for all weights of a step: lo = W - trunc19(W); t = W^T; t_lo = W^T - trunc19(W^T).
 // optional extras for the single-pass-TF32 layers: rn = RN_tf32(W), rn_t = RN_tf32(W)^T

@@ -152,6 +152,7 @@ SIGNATURES = {
                                   C.c_void_p, C.c_void_p]),
     "rd_debug_attention_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_gemm_timing": (C.c_int, [C.c_void_p]),
+    "rd_debug_wgrad_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_dropout_mask": (C.c_int, [C.c_void_p, C.c_uint32, C.c_int64, C.c_float, C.c_void_p,
                                         C.c_void_p]),
 }

@@ -12,6 +12,10 @@ by an L2 flush (256 MiB write) outside the CUDA-event pair.  Reported, medians o
 floor = 3 * sum(rows * Nout * (Kin + 1)) MACs (3xTF32 counted as three products, the bias column included) at 1,024 TF32
 MAC per clock per SM on all SMs at the card's maximum SM clock (the data-sheet rate).  Prints a table and one JSON line,
 with the card's name, power limit and clocks read in the same run.
+
+--stamps adds the kernel's per-CTA phase breakdown (rd_debug_wgrad_timing) from 5 more calls, each after an L2 flush:
+for the busiest CTA (longest start-to-end) and the mean over CTAs, in us at the CTA's own clock rate, of the call whose
+busiest CTA is the median.
 """
 import argparse
 import json
@@ -50,11 +54,48 @@ def problems(config, batch):
     return enc + enc + [("ob-prop lin_value", m1, C, C)] * 2
 
 
+STAMP_PHASES = [("total", None), ("producer: wait empty stage", 2), ("producer: wait X", 3),
+                ("producer: transpose + store", 4), ("producer: issue loads", 10), ("producer: other", None),
+                ("MMA: wait full stage", 5), ("MMA: epilogue", 6)]
+
+
+def stamp_breakdown(lib, call, flush, sms, dev, reps=5):
+    """per-phase us of the busiest and the mean CTA (rd_debug_wgrad_timing), from the median of `reps` calls"""
+    import ctypes as C
+    buf = torch.zeros(sms, 16, dtype=torch.int64, device=dev)
+    runs = []
+    for _ in range(reps):
+        buf.zero_()
+        flush.zero_()
+        lib.rd_debug_wgrad_timing(C.c_void_p(buf.data_ptr()))
+        try:
+            call()
+            torch.cuda.synchronize()
+        finally:
+            lib.rd_debug_wgrad_timing(None)
+        s = buf.cpu().double()
+        s = s[s[:, 7] > 0]                                   # launched CTAs
+        mhz = (s[:, 1] - s[:, 0]) / s[:, 7] * 1000.0          # cycles per ns -> MHz, per CTA
+        us = {name: s[:, slot] / mhz for name, slot in STAMP_PHASES if slot is not None}
+        us["total"] = (s[:, 1] - s[:, 0]) / mhz
+        # the producer's time outside the measured phases (its item walk and loop), start to its own end
+        us["producer: other"] = (s[:, 9] - s[:, 0] - s[:, 2] - s[:, 3] - s[:, 4] - s[:, 10]) / mhz
+        us = {name: us[name] for name, _ in STAMP_PHASES}
+        us["k-blocks"] = s[:, 8]
+        busiest = int(torch.argmax(us["total"]))
+        runs.append({"busiest": {k: float(v[busiest]) for k, v in us.items()},
+                     "mean": {k: float(v.mean()) for k, v in us.items()}, "ctas": int(s.shape[0]),
+                     "mhz": float(mhz.mean())})
+    runs.sort(key=lambda r: r["busiest"]["total"])
+    return runs[len(runs) // 2]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="P19", choices=sorted(BATCH))
     ap.add_argument("--batch", type=int, default=None)
     ap.add_argument("--reps", type=int, default=50)
+    ap.add_argument("--stamps", action="store_true", help="also print the per-CTA phase breakdown")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_wgrad.py needs a GPU")
@@ -119,9 +160,17 @@ def main():
     print("useful 3xTF32 MACs %.3f G, floor %.1f us" % (3.0 * useful / 1e9, floor_us))
     print("call %.1f us (range %.1f - %.1f); tc_wgrad_kernel %.1f us (floor fraction %.3f); wgrad_reduce_kernel %.1f us" %
           (tc, min(t_call), max(t_call), tk["tc_wgrad_kernel"], floor_us / tk["tc_wgrad_kernel"], tk["wgrad_reduce_kernel"]))
-    print(json.dumps({"card": info, "sms": sms, "config": args.config, "problems": probs, "floor_us": floor_us,
-                      "call_us": tc, "call_us_range": [min(t_call), max(t_call)], "kernel_us": tk,
-                      "floor_frac_kernel": floor_us / tk["tc_wgrad_kernel"]}))
+    out = {"card": info, "sms": sms, "config": args.config, "problems": probs, "floor_us": floor_us,
+           "call_us": tc, "call_us_range": [min(t_call), max(t_call)], "kernel_us": tk,
+           "floor_frac_kernel": floor_us / tk["tc_wgrad_kernel"]}
+    if args.stamps:
+        st = stamp_breakdown(lib, call, flush, sms, dev)
+        print("phase breakdown, us (%d CTAs, mean clock %.0f MHz)" % (st["ctas"], st["mhz"]))
+        print("%-30s %10s %10s" % ("phase", "busiest", "mean"))
+        for k in st["busiest"]:
+            print("%-30s %10.1f %10.1f" % (k, st["busiest"][k], st["mean"][k]))
+        out["stamps"] = st
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":

@@ -100,6 +100,62 @@ def run_case(name, cfg_name, B, dseed, wseed, opt):
     print("%-18s logits[0]=%s loss=%.6f  %d arrays" % (name, logits[0].tolist(), loss.item(), len(out)))
 
 
+# Raindrop_v2 away from the defaults of synth.model_config (d_ob = 4, nhead = 2, nhid = 2 d_model, 2 layers): name ->
+# (hyper-parameters, batch, data seed, weight seed).  D = N d_ob + 16; tests/test_hparams.py builds the same models.
+HPARAM_CASES = {
+    # D = 52, hd = 13, nhid % 4 != 0, d_ob = 3, five layers
+    "A": (dict(d_inp=12, d_ob=3, nhead=4, nhid=50, nlayers=5, max_len=40, d_static=4, n_classes=3), 9, 411, 41),
+    # D = 32, hd = 4, eight layers, no statics
+    "B": (dict(d_inp=8, d_ob=2, nhead=8, nhid=64, nlayers=8, max_len=48, d_static=0, n_classes=2), 6, 252, 42),
+    # D = 26 (D % 4 != 0), d_ob = 1, C = T = 130
+    "C": (dict(d_inp=10, d_ob=1, nhead=2, nhid=37, nlayers=3, max_len=130, d_static=2, n_classes=4), 3, 53, 43),
+}
+HPARAM_FULL_MAX = 4096      # tensors up to this many elements are stored in full, larger ones as fingerprints
+
+
+def hparam_config(name, hp):
+    """synth-style cfg of a HPARAM_CASES entry (dropout 0.2 as everywhere; fixtures are taken in eval mode)."""
+    cfg = dict(hp, name="HP_" + name, static=hp["d_static"] > 0, p_obs=0.5, dropout=0.2, MAX=100)
+    cfg["d_model"] = cfg["d_inp"] * cfg["d_ob"]
+    return cfg
+
+
+def hparam_cases():
+    """The reference's own Raindrop_v2 (eval mode) at HPARAM_CASES -> hparams_<case>.npz: logits, loss, the obs / pe /
+    enc stages and the gradient of every parameter that gets one.  `meta` carries the full cfg."""
+    for name, (hp, B, dseed, wseed) in HPARAM_CASES.items():
+        cfg = hparam_config(name, hp)
+        model = ref_harness.build_reference_model(cfg).eval()
+        synth_weights(model, cfg, seed=wseed)
+        batch = make_batch(cfg, B, seed=dseed)
+        grabbed = {}
+        h = model.transformer_encoder.register_forward_hook(lambda m, i, o: grabbed.update(enc=o, obs=i[0]))
+        logits, distance, _ = model.forward(batch["src"], batch["static"], batch["times"], batch["lengths"])
+        h.remove()
+        loss = F.cross_entropy(logits, batch["y"])
+        model.zero_grad()
+        loss.backward()
+        D4 = cfg["d_inp"] * cfg["d_ob"]
+        tensors = dict(obs=grabbed["obs"][:, :, :D4], pe=grabbed["obs"][:, :, D4:], enc=grabbed["enc"])
+        params = dict(model.named_parameters())
+        with_grad = sorted(k for k, p in params.items() if p.grad is not None)
+        assert with_grad == sorted(used_param_keys(cfg)), set(with_grad) ^ set(used_param_keys(cfg))
+        tensors.update({"grad." + k: params[k].grad for k in with_grad})
+        out = dict(logits=logits.detach().numpy(), distance=np.float32(distance.item()), loss=np.float32(loss.item()))
+        for k, t in tensors.items():
+            if t.numel() <= HPARAM_FULL_MAX:
+                out[k] = t.detach().numpy()
+            else:
+                fp = fingerprint(t)
+                out[k + "#sample"] = fp["sample"]
+                out[k + "#stats"] = np.array([fp["sum"], fp["asum"], fp["l2"]], dtype=np.float64)
+        meta = dict(case="hparams_" + name, cfg=cfg, batch=B, data_seed=dseed, weight_seed=wseed, torch=torch.__version__,
+                    reference_commit="892eb57", generator="oracle/make_golden.py hparams")
+        out["meta"] = np.frombuffer(json.dumps(meta).encode(), dtype=np.uint8)
+        np.savez_compressed(os.path.join(GOLDEN, "hparams_%s.npz" % name), **out)
+        print("hparams_%s  logits[0]=%s loss=%.6f  %d arrays" % (name, logits[0].tolist(), loss.item(), len(out)))
+
+
 def operator_cases():
     """Operator-level fixtures: `Observation_progation` with use_beta both ways on a sparse
     weighted graph, and `TransformerConv` with and without supplied edge weights."""
@@ -282,6 +338,9 @@ if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "v1":
         v1_case()
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "hparams":
+        hparam_cases()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "live":
         data_utils_case()
         live_tiny_case()
@@ -293,3 +352,4 @@ if __name__ == "__main__":
     v1_case()
     data_utils_case()
     live_tiny_case()
+    hparam_cases()

@@ -203,14 +203,15 @@ def positional_encoding(times, max_len, d_pe=16):
 # --------------------------------------------------------------------------------------------
 # Transformer encoder layer written out (torch.nn.TransformerEncoderLayer, post-LN, relu)
 # --------------------------------------------------------------------------------------------
-def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None):
+def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None, ffn_pre=None):
     """x [T, B, D]; pad [B, T] bool (True = padded key); p = dict of the layer's tensors with the
     state-dict suffixes as keys.  Eval-mode math of the module called at code/models_rd.py:358.
 
     `masks` (optional) = dict of dropout multipliers (0 or 1/(1-p)), each optional, applied where the module's
     dropouts sit in training: "attn" [B, H, T, T] (query, key) on the attention weights after the softmax,
     "resid1" [T*B, D] on the out-projection (dropout1), "ffn" [T*B, nhid] on relu(linear1) (dropout) and
-    "resid2" [T*B, D] on linear2 (dropout2).  Train-mode math with those masks instead of torch's RNG."""
+    "resid2" [T*B, D] on linear2 (dropout2).  Train-mode math with those masks instead of torch's RNG.
+    `ffn_pre` (optional list): the linear1 pre-activation [T, B, nhid] (the FFN's ReLU input) is appended to it."""
     T, B, D = x.shape
     hd = D // nhead
     m = masks or {}
@@ -231,7 +232,10 @@ def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None):
     o = (a @ heads(v)).permute(2, 0, 1, 3).reshape(T, B, D)
     y = drop(o @ p["self_attn.out_proj.weight"].T + p["self_attn.out_proj.bias"], "resid1")
     x1 = F.layer_norm(x + y, (D,), p["norm1.weight"], p["norm1.bias"], eps)
-    f = drop(F.relu(x1 @ p["linear1.weight"].T + p["linear1.bias"]), "ffn")
+    f_pre = x1 @ p["linear1.weight"].T + p["linear1.bias"]
+    if ffn_pre is not None:
+        ffn_pre.append(f_pre.detach())
+    f = drop(F.relu(f_pre), "ffn")
     g = drop(f @ p["linear2.weight"].T + p["linear2.bias"], "resid2")
     return F.layer_norm(x1 + g, (D,), p["norm2.weight"], p["norm2.bias"], eps)
 
@@ -290,9 +294,10 @@ class RaindropV2Oracle(nn.Module):
             gs = torch.ones(self.d_inp, self.d_inp)
         return graph_from_adjacency(gs.float())
 
-    def _tail(self, obs, pe, static, lengths, pad, layer_masks=None):
+    def _tail(self, obs, pe, static, lengths, pad, layer_masks=None, ffn_pre=None):
         """code/models_rd.py:354-385: concat PE, temporal self-attention, masked mean, head.  With `layer_masks`
-        (one encoder_layer_explicit mask dict per layer) the layers run written out, with those dropout masks."""
+        (one encoder_layer_explicit mask dict per layer) the layers run written out, with those dropout masks, and
+        append their FFN pre-activations to `ffn_pre` (a list) when one is given."""
         z = torch.cat([obs, pe], dim=2)
         if layer_masks is None:
             r = self.transformer_encoder(z, src_key_padding_mask=pad)
@@ -300,7 +305,8 @@ class RaindropV2Oracle(nn.Module):
             assert len(layer_masks) == self.nlayers, (len(layer_masks), self.nlayers)
             r = z
             for layer, lm in zip(self.transformer_encoder.layers, layer_masks):
-                r = encoder_layer_explicit(r, pad, dict(layer.named_parameters()), self.nhead, layer.norm1.eps, lm)
+                r = encoder_layer_explicit(r, pad, dict(layer.named_parameters()), self.nhead, layer.norm1.eps, lm,
+                                           ffn_pre)
         keep = (~pad).T[:, :, None].to(r.dtype)                          # [T, B, 1]
         pooled = (r * keep).sum(0) / (lengths[:, None] + 1)
         if static is not None:
@@ -337,7 +343,10 @@ class RaindropV2Oracle(nn.Module):
         """`masks` (optional, oracle/dropout_masks.model_masks layout): {"lift": [T, B, N*d_ob], "layers": [one
         encoder_layer_explicit mask dict per layer]} replace every dropout of the training forward, so that the
         train-mode output and its autograd gradient are those of the given masks (run in float64 for an exact
-        reference).  Without masks the modules' own dropout applies (identity in eval)."""
+        reference).  Without masks the modules' own dropout applies (identity in eval).
+
+        `stages` also receives the ReLU inputs a rounding error can flip: "obprop_pre" (the two ob-prop layers'
+        lin_value outputs [B, N, C]) and, with masks, "ffn_pre" (one [T, B, nhid] linear1 output per encoder layer)."""
         T, B = src.shape[0], src.shape[1]
         N, d_ob = self.d_inp, self.d_ob
         h = self._lift(src, None if masks is None else masks["lift"])
@@ -355,9 +364,14 @@ class RaindropV2Oracle(nn.Module):
             h1 = self.ob_propagation.forward_dense(x, s)
             h2 = self.ob_propagation_layer2.forward_dense(h1, s)
         obs = h2.view(B, N, T, d_ob).permute(2, 0, 1, 3).reshape(T, B, N * d_ob)
-        logits, r = self._tail(obs, pe, static, lengths, pad, None if masks is None else masks["layers"])
+        ffn_pre = [] if stages is not None and masks is not None else None
+        logits, r = self._tail(obs, pe, static, lengths, pad, None if masks is None else masks["layers"], ffn_pre)
         if stages is not None:
-            stages.update(lift=h, pe=pe, x0=x, h1=h1, obs=obs, enc=r)
+            with torch.no_grad():
+                obprop_pre = [self.ob_propagation.lin_value(x), self.ob_propagation_layer2.lin_value(h1)]
+            stages.update(lift=h, pe=pe, x0=x, h1=h1, obs=obs, enc=r, obprop_pre=obprop_pre)
+            if ffn_pre is not None:
+                stages["ffn_pre"] = ffn_pre
         return logits, torch.zeros((), dtype=src.dtype), None
 
 

@@ -21,7 +21,9 @@ struct HeadP {
   const int64_t* lengths;
 };
 
-// grid = B, block = HT.  x = encoder output [T, B, D].
+// grid = B, block = HT.  x = encoder output [T, B, D].  VEC: D % 4 == 0, the masked mean reads and writes float4;
+// otherwise one column at a time (same time groups, same summation order).
+template <bool VEC>
 __global__ void __launch_bounds__(HT) head_fwd_kernel(HeadP p, const float* __restrict__ x, float* __restrict__ feat,
                                                       float* __restrict__ hpre, float* __restrict__ logits,
                                                       const int64_t* __restrict__ y, float* __restrict__ loss_ps,
@@ -39,14 +41,23 @@ __global__ void __launch_bounds__(HT) head_fwd_kernel(HeadP p, const float* __re
     const long long len = p.lengths[b];
     const int nv = (int)(len < p.T ? (len < 0 ? 0 : len) : p.T);
     const int tg = tid >> 6, dq0 = tid & 63, nq = p.D >> 2;
-    for (int dq = dq0; dq < nq; dq += 64) {
-      float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (VEC) {
+      for (int dq = dq0; dq < nq; dq += 64) {
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 8
-      for (int t = tg; t < nv; t += 8) {
-        const float4 v = __ldg(reinterpret_cast<const float4*>(x + ((long long)t * p.B + b) * p.D) + dq);
-        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+        for (int t = tg; t < nv; t += 8) {
+          const float4 v = __ldg(reinterpret_cast<const float4*>(x + ((long long)t * p.B + b) * p.D) + dq);
+          s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+        }
+        *reinterpret_cast<float4*>(red + tg * p.D + 4 * dq) = s;
       }
-      *reinterpret_cast<float4*>(red + tg * p.D + 4 * dq) = s;
+    } else {
+      for (int d = dq0; d < p.D; d += 64) {
+        float s = 0.f;
+#pragma unroll 8
+        for (int t = tg; t < nv; t += 8) s += __ldg(x + ((long long)t * p.B + b) * p.D + d);
+        red[tg * p.D + d] = s;
+      }
     }
     __syncthreads();
     const float inv = 1.f / (float)(len + 1);
@@ -147,6 +158,8 @@ __global__ void __launch_bounds__(HT) head_fwd_kernel(HeadP p, const float* __re
 }
 
 // grid = B: dh = (dlogits . W2) * [h > 0];  dfeat = dh . W0;  d(encoder output)[t, b, :] = dfeat[:D] / (len+1) for t < len
+// VEC: D % 4 == 0, the encoder-output gradient is written in float4; otherwise one column at a time.
+template <bool VEC>
 __global__ void __launch_bounds__(HT) head_bwd_sample_kernel(HeadP p, const float* __restrict__ hpre,
                                                              const float* __restrict__ dlogits, float* __restrict__ dh,
                                                              float* __restrict__ dfeat, float* __restrict__ dx) {
@@ -208,12 +221,19 @@ __global__ void __launch_bounds__(HT) head_bwd_sample_kernel(HeadP p, const floa
   // masked-mean backward (code/models_rd.py:366-379)
   const long long len = p.lengths[b];
   const float inv = 1.f / (float)(len + 1);
-  const int nq = p.D >> 2;
-  for (int i = tid; i < p.T * nq; i += HT) {
-    const int t = i / nq, dq = i - t * nq;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t < len) v = make_float4(df[4 * dq] * inv, df[4 * dq + 1] * inv, df[4 * dq + 2] * inv, df[4 * dq + 3] * inv);
-    *(reinterpret_cast<float4*>(dx + ((long long)t * p.B + b) * p.D) + dq) = v;
+  if (VEC) {
+    const int nq = p.D >> 2;
+    for (int i = tid; i < p.T * nq; i += HT) {
+      const int t = i / nq, dq = i - t * nq;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (t < len) v = make_float4(df[4 * dq] * inv, df[4 * dq + 1] * inv, df[4 * dq + 2] * inv, df[4 * dq + 3] * inv);
+      *(reinterpret_cast<float4*>(dx + ((long long)t * p.B + b) * p.D) + dq) = v;
+    }
+  } else {
+    for (int i = tid; i < p.T * p.D; i += HT) {
+      const int t = i / p.D, d = i - t * p.D;
+      dx[((long long)t * p.B + b) * p.D + d] = t < len ? df[d] * inv : 0.f;
+    }
   }
 }
 
@@ -282,20 +302,25 @@ int head_fwd(int B, int T, int D, int N, int ds, int ncls, const float* x, const
   HeadP p = make(B, T, D, N, ds, ncls, statics, emb_w, emb_b, w0, b0, w2, b2, lengths);
   const int red = 8 * D > ncls ? 8 * D : ncls;
   const size_t smem = (size_t)(((2 * p.Df + 3) & ~3) + red) * sizeof(float);
-  if (smem > 48 * 1024 || (D & 3)) { set_error("head_fwd: feature width %d not supported", p.Df); return -2; }
+  if (smem > 48 * 1024) { set_error("head_fwd: feature width %d not supported", p.Df); return -2; }
   if (y && (!loss_ps || !dlogits || !loss || !counter)) { set_error("head_fwd: labels given without loss outputs"); return -2; }
-  launch_pdl(head_fwd_kernel, dim3(B), dim3(HT), smem, st, p, x, feat, hpre, logits, y, loss_ps, dlogits, loss, counter);
+  launch_pdl((D & 3) ? head_fwd_kernel<false> : head_fwd_kernel<true>, dim3(B), dim3(HT), smem, st, p, x, feat, hpre, logits, y,
+             loss_ps, dlogits, loss, counter);
   RD_CHECK_LAUNCH("head_fwd_kernel");
   return 0;
 }
+
+// the backward keeps dh and one partial dfeat row per warp in shared memory: Df <= 722
+bool head_bwd_supported(int Df) { return (size_t)(1 + HT / 32) * Df * sizeof(float) <= 48 * 1024; }
 
 int head_bwd(int B, int T, int D, int N, int ds, int ncls, const int64_t* lengths, const float* statics, const float* w0,
              const float* w2, const float* feat, const float* hpre, const float* dlogits, float* dh, float* dfeat, float* dx,
              float* g_w0, float* g_b0, float* g_w2, float* g_b2, float* g_emb_w, float* g_emb_b, cudaStream_t st) {
   HeadP p = make(B, T, D, N, ds, ncls, statics, nullptr, nullptr, w0, nullptr, w2, nullptr, lengths);
   const size_t smem = (size_t)(1 + HT / 32) * p.Df * sizeof(float);       // dh + one partial dfeat row per warp
-  if (smem > 48 * 1024) { set_error("head_bwd: feature width %d too large", p.Df); return -2; }
-  launch_pdl(head_bwd_sample_kernel, dim3(B), dim3(HT), smem, st, p, hpre, dlogits, dh, dfeat, dx);
+  if (!head_bwd_supported(p.Df)) { set_error("head_bwd: feature width %d too large", p.Df); return -2; }
+  launch_pdl((D & 3) ? head_bwd_sample_kernel<false> : head_bwd_sample_kernel<true>, dim3(B), dim3(HT), smem, st, p, hpre,
+             dlogits, dh, dfeat, dx);
   RD_CHECK_LAUNCH("head_bwd_sample_kernel");
   if (!g_w0) return 0;      // frozen parameters: data gradients only
   OuterGroup g;

@@ -134,6 +134,7 @@ int head_fwd(int B, int T, int D, int N, int ds, int ncls, const float* x, const
              float* feat, float* hpre, float* logits, const int64_t* y, float* loss_ps, float* dlogits, float* loss,
              unsigned* counter, cudaStream_t st);
 // dx = d(loss)/d(encoder output) [T, B, D] (masked-mean backward); g_w0 == nullptr skips the weight gradients
+bool head_bwd_supported(int Df);
 int head_bwd(int B, int T, int D, int N, int ds, int ncls, const int64_t* lengths, const float* statics, const float* w0,
              const float* w2, const float* feat, const float* hpre, const float* dlogits, float* dh, float* dfeat, float* dx,
              float* g_w0, float* g_b0, float* g_w2, float* g_b2, float* g_emb_w, float* g_emb_b, cudaStream_t st);

@@ -907,6 +907,11 @@ int rd_raindrop_v2_fwd(const rd_dims* dims, const rd_params* params, const float
     set_error("rd_raindrop_v2_fwd: NULL argument");
     return -2;
   }
+  if (dims->training) {       // a training forward is followed by a backward: refuse before any output is written
+    Shape s;
+    RD_TRY(make_shape(dims, &s));
+    if (!head_bwd_supported(s.Df)) { set_error("rd_raindrop_v2_fwd: training needs the head backward, feature width %d > 722", s.Df); return -2; }
+  }
   return raindrop_fwd(dims, params, src, statics, times, lengths, node_scale, rng_state, (float*)workspace, logits,
                       y, loss, d_logits, 0, (cudaStream_t)stream);
 }

@@ -111,7 +111,10 @@ enum rd_ws_buffer {
   RD_WS_ENC_IN = 2,/* cat(obs, pe)   [T, B, D] (code/models_rd.py:341,354)                  */
   RD_WS_ENC_OUT = 3,/* r_out         [T, B, D] (code/models_rd.py:358)                      */
   RD_WS_FEAT = 4,  /* cat(pooled, emb) [B, Df] (code/models_rd.py:379,384)                  */
-  RD_WS_RNG = 5    /* 2 x uint64 (seed, step counter) captured by this forward              */
+  RD_WS_RNG = 5,   /* 2 x uint64 (seed, step counter) captured by this forward              */
+  RD_WS_HEAD_HIDDEN = 6,/* relu(mlp_static.0(feat)) [B, Df] (code/models_rd.py:385)         */
+  RD_WS_FFN = 7    /* RD_WS_FFN + l, l < nlayers: dropout(relu(linear1)) of encoder layer l
+                      [T*B, nhid], token-major rows t*B + b                                 */
 };
 
 int rd_abi_version(void);

@@ -51,12 +51,35 @@ def dropout_words(seed, step, site, n):
     return philox4x32_10(ctr, key).reshape(-1)[: int(n)]
 
 
-def dropout_mask(seed, step, site, n, p):
-    """float32 [n]: 1/(1-p) where element idx is kept, 0 where it is dropped (bitwise what the kernels multiply by)."""
+def dropout_words_at(seed, step, site, idx):
+    """The 32-bit Philox word of the given element indices (any integer array) of `site` under (seed, step): the same
+    values as dropout_words(...)[idx], without generating the indices below them."""
+    seed, step = int(seed) & 0xFFFFFFFFFFFFFFFF, int(step) & 0xFFFFFFFFFFFFFFFF
+    idx = np.asarray(idx, dtype=np.uint64)
+    blk = idx >> np.uint64(2)
+    ctr = np.empty(idx.shape + (4,), dtype=np.uint64)
+    ctr[..., 0], ctr[..., 1] = blk & _LO, blk >> _S32
+    ctr[..., 2], ctr[..., 3] = site, step & 0xFFFFFFFF
+    key = np.array([seed & 0xFFFFFFFF, (seed >> 32) ^ (step >> 32)], dtype=np.uint64)
+    words = philox4x32_10(ctr, key)
+    return np.take_along_axis(words, (idx & np.uint64(3)).astype(np.int64)[..., None], -1)[..., 0]
+
+
+def _keep_scale(words, p):
     p32 = np.float32(p)
     inv_keep = np.float32(1.0) / (np.float32(1.0) - p32)
-    u = (dropout_words(seed, step, site, n) >> np.uint32(8)).astype(np.float64) * 2.0 ** -24   # exact
+    u = (words >> np.uint32(8)).astype(np.float64) * 2.0 ** -24   # exact
     return np.where(u >= np.float64(p32), inv_keep, np.float32(0.0)).astype(np.float32)
+
+
+def dropout_mask(seed, step, site, n, p):
+    """float32 [n]: 1/(1-p) where element idx is kept, 0 where it is dropped (bitwise what the kernels multiply by)."""
+    return _keep_scale(dropout_words(seed, step, site, n), p)
+
+
+def dropout_mask_at(seed, step, site, idx, p):
+    """dropout_mask(seed, step, site, max(idx) + 1, p)[idx], evaluated at the given element indices only."""
+    return _keep_scale(dropout_words_at(seed, step, site, idx), p)
 
 
 def lift_mask(rng, p, T, B, width):
@@ -92,6 +115,18 @@ def model_masks(rng, p, cfg, B):
                    ffn=ffn_mask(rng, p, l, rows, nhid), resid2=resid2_mask(rng, p, l, rows, D))
               for l in range(cfg["nlayers"])]
     return dict(lift=lift_mask(rng, p, T, B, N * d_ob), layers=layers)
+
+
+def slice_masks(masks, sl, T, B):
+    """The masks of samples `sl` (a slice) of a batch of B, in the model_masks layout; numpy arrays or tensors.  A mask
+    that is None or absent stays so (no dropout there)."""
+    def cut(key, m):
+        if key == "attn":                # [B, H, T, T]
+            return m[sl]
+        return m.reshape(T, B, -1)[:, sl].reshape(-1, m.shape[-1])     # token-major [T*B, width] -> [T*Bc, width]
+    lift = masks.get("lift")
+    return dict(lift=None if lift is None else lift[:, sl],
+                layers=[{k: cut(k, m) for k, m in l.items() if m is not None} for l in masks["layers"]])
 
 
 def ones_masks(cfg, B):

@@ -149,9 +149,9 @@ class ObPropOracle(nn.Module):
         out = scatter_rows(msg, seg, n)                       # :226-228
         return out, (edge_index, alpha_ret)
 
-    def forward_dense(self, x, node_scale):
-        """Live path (use_beta=False) closed form for a batch of node rows x [..., C]."""
-        return F.relu(self.lin_value(x)) * node_scale
+    def forward_dense(self, x, node_scale, gate=None):
+        """Live path (use_beta=False) closed form for a batch of node rows x [..., C]; `gate`: relu_or_gate."""
+        return relu_or_gate(self.lin_value(x), gate) * node_scale
 
 
 # --------------------------------------------------------------------------------------------
@@ -195,7 +195,7 @@ def pe_timescales(max_len, d_pe=16):
 
 
 def positional_encoding(times, max_len, d_pe=16):
-    ts = torch.from_numpy(pe_timescales(max_len, d_pe)).to(times.dtype)
+    ts = torch.from_numpy(pe_timescales(max_len, d_pe)).to(times)
     scaled = times[:, :, None] / ts[None, None, :]
     return torch.cat([torch.sin(scaled), torch.cos(scaled)], -1)
 
@@ -203,7 +203,15 @@ def positional_encoding(times, max_len, d_pe=16):
 # --------------------------------------------------------------------------------------------
 # Transformer encoder layer written out (torch.nn.TransformerEncoderLayer, post-LN, relu)
 # --------------------------------------------------------------------------------------------
-def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None, ffn_pre=None):
+def relu_or_gate(x, gate=None):
+    """relu(x), or with `gate` (bool, x's shape) the ReLU whose on/off decisions are given: x where gate, else 0.  With
+    gate = x > 0 this is relu bitwise, forward and backward."""
+    if gate is None:
+        return F.relu(x)
+    return torch.where(torch.as_tensor(gate, device=x.device).reshape(x.shape), x, x.new_zeros(()))
+
+
+def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None, ffn_pre=None, ffn_gate=None):
     """x [T, B, D]; pad [B, T] bool (True = padded key); p = dict of the layer's tensors with the
     state-dict suffixes as keys.  Eval-mode math of the module called at code/models_rd.py:358.
 
@@ -211,14 +219,15 @@ def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None, ffn_pre=None)
     dropouts sit in training: "attn" [B, H, T, T] (query, key) on the attention weights after the softmax,
     "resid1" [T*B, D] on the out-projection (dropout1), "ffn" [T*B, nhid] on relu(linear1) (dropout) and
     "resid2" [T*B, D] on linear2 (dropout2).  Train-mode math with those masks instead of torch's RNG.
-    `ffn_pre` (optional list): the linear1 pre-activation [T, B, nhid] (the FFN's ReLU input) is appended to it."""
+    `ffn_pre` (optional list): the linear1 pre-activation [T, B, nhid] (the FFN's ReLU input) is appended to it.
+    `ffn_gate` (optional, bool [T*B, nhid]): the FFN ReLU's decisions (relu_or_gate)."""
     T, B, D = x.shape
     hd = D // nhead
     m = masks or {}
 
     def drop(t, key):
         mk = m.get(key)
-        return t if mk is None else t * torch.as_tensor(mk, dtype=t.dtype).reshape(t.shape)
+        return t if mk is None else t * torch.as_tensor(mk, dtype=t.dtype, device=t.device).reshape(t.shape)
 
     qkv = x @ p["self_attn.in_proj_weight"].T + p["self_attn.in_proj_bias"]
     q, k, v = qkv.split(D, dim=-1)
@@ -235,7 +244,7 @@ def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None, ffn_pre=None)
     f_pre = x1 @ p["linear1.weight"].T + p["linear1.bias"]
     if ffn_pre is not None:
         ffn_pre.append(f_pre.detach())
-    f = drop(F.relu(f_pre), "ffn")
+    f = drop(relu_or_gate(f_pre, ffn_gate), "ffn")
     g = drop(f @ p["linear2.weight"].T + p["linear2.bias"], "resid2")
     return F.layer_norm(x1 + g, (D,), p["norm2.weight"], p["norm2.bias"], eps)
 
@@ -283,9 +292,9 @@ class RaindropV2Oracle(nn.Module):
         """code/models_rd.py:285-296: drop the mask half, repeat each sensor d_ob times, scale by
         R_u, relu, dropout (or the given [T, B, N*d_ob] dropout multipliers in its place)."""
         vals = src[:, :, : src.shape[2] // 2]
-        h = F.relu(torch.repeat_interleave(vals, self.d_ob, dim=-1) * self.R_u.to(src.dtype))
+        h = F.relu(torch.repeat_interleave(vals, self.d_ob, dim=-1) * self.R_u.to(src))   # R_u: not moved by .to()
         if mask is not None:
-            return h * torch.as_tensor(mask, dtype=h.dtype).reshape(h.shape)
+            return h * torch.as_tensor(mask, dtype=h.dtype, device=h.device).reshape(h.shape)
         return self.dropout(h)
 
     def _graph(self):
@@ -294,24 +303,34 @@ class RaindropV2Oracle(nn.Module):
             gs = torch.ones(self.d_inp, self.d_inp)
         return graph_from_adjacency(gs.float())
 
-    def _tail(self, obs, pe, static, lengths, pad, layer_masks=None, ffn_pre=None):
+    def _tail(self, obs, pe, static, lengths, pad, layer_masks=None, ffn_pre=None, gates=None, head_pre=None):
         """code/models_rd.py:354-385: concat PE, temporal self-attention, masked mean, head.  With `layer_masks`
         (one encoder_layer_explicit mask dict per layer) the layers run written out, with those dropout masks, and
-        append their FFN pre-activations to `ffn_pre` (a list) when one is given."""
+        append their FFN pre-activations to `ffn_pre` (a list) when one is given.  `gates` (forward_dense) gives the
+        decisions of the FFN ("ffn", written-out layers only) and head ("head") ReLUs; the head's pre-activation is
+        appended to `head_pre` (a list) when one is given."""
         z = torch.cat([obs, pe], dim=2)
+        g = gates or {}
         if layer_masks is None:
+            assert g.get("ffn") is None, "FFN gates need the written-out layers (masks)"
             r = self.transformer_encoder(z, src_key_padding_mask=pad)
         else:
             assert len(layer_masks) == self.nlayers, (len(layer_masks), self.nlayers)
+            ffn_gates = g.get("ffn") or [None] * self.nlayers
             r = z
-            for layer, lm in zip(self.transformer_encoder.layers, layer_masks):
+            for layer, lm, fg in zip(self.transformer_encoder.layers, layer_masks, ffn_gates):
                 r = encoder_layer_explicit(r, pad, dict(layer.named_parameters()), self.nhead, layer.norm1.eps, lm,
-                                           ffn_pre)
+                                           ffn_pre, fg)
         keep = (~pad).T[:, :, None].to(r.dtype)                          # [T, B, 1]
         pooled = (r * keep).sum(0) / (lengths[:, None] + 1)
         if static is not None:
             pooled = torch.cat([pooled, self.emb(static)], dim=1)
-        return self.mlp_static(pooled), r
+        # mlp_static written out (Linear, ReLU, Linear: the same calls nn.Sequential makes) so that its ReLU can be gated
+        lin0, lin2 = self.mlp_static[0], self.mlp_static[2]
+        h = F.linear(pooled, lin0.weight, lin0.bias)
+        if head_pre is not None:
+            head_pre.append(h.detach())
+        return F.linear(relu_or_gate(h, g.get("head")), lin2.weight, lin2.bias), r
 
     # -- the reference's own structure (what cpu_baseline times) ---------------------------------
     def forward(self, src, static, times, lengths, use_beta=False, stages=None):
@@ -339,40 +358,72 @@ class RaindropV2Oracle(nn.Module):
         return logits, distance, None
 
     # -- independent closed form -----------------------------------------------------------------
-    def forward_dense(self, src, static, times, lengths, stages=None, tf32_model=False, masks=None):
+    def forward_dense(self, src, static, times, lengths, stages=None, tf32_model=False, masks=None, gates=None,
+                      h1_value=None):
         """`masks` (optional, oracle/dropout_masks.model_masks layout): {"lift": [T, B, N*d_ob], "layers": [one
         encoder_layer_explicit mask dict per layer]} replace every dropout of the training forward, so that the
         train-mode output and its autograd gradient are those of the given masks (run in float64 for an exact
         reference).  Without masks the modules' own dropout applies (identity in eval).
 
-        `stages` also receives the ReLU inputs a rounding error can flip: "obprop_pre" (the two ob-prop layers'
-        lin_value outputs [B, N, C]) and, with masks, "ffn_pre" (one [T, B, nhid] linear1 output per encoder layer)."""
+        `gates` (optional dict, every entry optional, bool) replaces the on/off decisions of the ReLUs a rounding error
+        can flip by given ones (relu_or_gate), so that the output is a smooth function of the inputs and parameters
+        around the decisions another implementation took:
+          "h1"   [B, N, C]            ob-prop layer 1
+          "obs"  [T, B, N*d_ob]       ob-prop layer 2, in the layout of its output `obs`
+          "ffn"  [[T*B, nhid]] * nlayers, the FFN of each encoder layer (needs masks: the written-out layers)
+          "head" [B, Df]              mlp_static.0
+        The lift's ReLU has none: the sign of src * R_u is exact in fp32.
+
+        `h1_value` (tf32_model only, [B, N, C]): the TF32-rounded layer-1 output another implementation computed.  Layer
+        2 takes its value; the gradient flows on into layer 1 as if it were the model's own.  A rounding that lands on
+        the other side of a TF32 rounding boundary then cannot move layer 2.  `stages["h1_own"]` keeps the model's own
+        layer-1 output, so that the value fed in can itself be checked.
+
+        `stages` also receives the ReLU inputs: "obprop_pre" (the two ob-prop layers' lin_value outputs [B, N, C]),
+        "head_pre" [B, Df] and, with masks, "ffn_pre" (one [T, B, nhid] linear1 output per encoder layer).
+
+        Runs on the device and in the dtype of `src` (the model's parameters must be there too)."""
         T, B = src.shape[0], src.shape[1]
         N, d_ob = self.d_inp, self.d_ob
+        g = gates or {}
         h = self._lift(src, None if masks is None else masks["lift"])
         pe = positional_encoding(times, self.max_len).to(src.dtype)
-        pad = torch.arange(T)[None, :] >= lengths[:, None]
+        lengths = lengths.to(src.device)
+        pad = torch.arange(T, device=src.device)[None, :] >= lengths[:, None]
         edge_index, edge_w = self._graph()
-        s = node_scale_from_graph(edge_index, edge_w, N, src.dtype)[None, :, None]   # [1, N, 1]
+        s = node_scale_from_graph(edge_index, edge_w, N, src.dtype).to(src.device)[None, :, None]   # [1, N, 1]
         x = h.reshape(T, B, N, d_ob).permute(1, 2, 0, 3).reshape(B, N, T * d_ob)
+        gate2 = g.get("obs")
+        if gate2 is not None:       # obs layout [T, B, N*d_ob] -> ob-prop rows [B, N, C]
+            gate2 = torch.as_tensor(gate2, device=src.device).reshape(T, B, N, d_ob).permute(1, 2, 0, 3).reshape(B, N, -1)
+        l1, l2 = self.ob_propagation.lin_value, self.ob_propagation_layer2.lin_value
         if tf32_model:
             rows = x.reshape(B * N, T * d_ob)
-            h1, h2 = obprop_two_layers_tf32(rows, self.ob_propagation, self.ob_propagation_layer2,
-                                            s.expand(B, N, 1).reshape(B * N, 1))
-            h1, h2 = h1.view(B, N, -1), h2.view(B, N, -1)
+            gr = lambda t: None if t is None else torch.as_tensor(t, device=src.device).reshape(B * N, -1)
+            h1, h2, h1_own = obprop_two_layers_tf32(rows, self.ob_propagation, self.ob_propagation_layer2,
+                                            s.expand(B, N, 1).reshape(B * N, 1), gr(g.get("h1")), gr(gate2),
+                                            None if h1_value is None else h1_value.to(src).reshape(B * N, -1))
+            h1, h2, h1_own = h1.view(B, N, -1), h2.view(B, N, -1), h1_own.view(B, N, -1)
+            # ReLU inputs as the rounding model computes them
+            pre = lambda lin, t: round_tf32(t) @ round_tf32(lin.weight).T + lin.bias
+            l1, l2 = (lambda t: pre(self.ob_propagation.lin_value, t)), (lambda t: pre(self.ob_propagation_layer2.lin_value, t))
         else:
-            h1 = self.ob_propagation.forward_dense(x, s)
-            h2 = self.ob_propagation_layer2.forward_dense(h1, s)
+            h1 = self.ob_propagation.forward_dense(x, s, g.get("h1"))
+            h2 = self.ob_propagation_layer2.forward_dense(h1, s, gate2)
+            h1_own = h1
         obs = h2.view(B, N, T, d_ob).permute(2, 0, 1, 3).reshape(T, B, N * d_ob)
         ffn_pre = [] if stages is not None and masks is not None else None
-        logits, r = self._tail(obs, pe, static, lengths, pad, None if masks is None else masks["layers"], ffn_pre)
+        head_pre = [] if stages is not None else None
+        logits, r = self._tail(obs, pe, static, lengths, pad, None if masks is None else masks["layers"], ffn_pre, g,
+                               head_pre)
         if stages is not None:
             with torch.no_grad():
-                obprop_pre = [self.ob_propagation.lin_value(x), self.ob_propagation_layer2.lin_value(h1)]
-            stages.update(lift=h, pe=pe, x0=x, h1=h1, obs=obs, enc=r, obprop_pre=obprop_pre)
+                obprop_pre = [l1(x), l2(h1)]
+            stages.update(lift=h, pe=pe, x0=x, h1=h1, h1_own=h1_own.detach(), obs=obs, enc=r, obprop_pre=obprop_pre,
+                          head_pre=head_pre[0])
             if ffn_pre is not None:
                 stages["ffn_pre"] = ffn_pre
-        return logits, torch.zeros((), dtype=src.dtype), None
+        return logits, torch.zeros((), dtype=src.dtype, device=src.device), None
 
 
 # --------------------------------------------------------------------------------------------
@@ -383,9 +434,10 @@ class RaindropV2Oracle(nn.Module):
 # checked tightly even though a ReLU network's gradient is discontinuous in forward perturbations.
 # --------------------------------------------------------------------------------------------
 def round_tf32(t):
-    """Round-to-nearest (ties away) to 10 explicit mantissa bits, like cvt.rna.tf32.f32."""
-    i = t.detach().contiguous().view(torch.int32)
-    return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
+    """Round-to-nearest (ties away) to 10 explicit mantissa bits, like cvt.rna.tf32.f32.  A float64 value is first
+    rounded to fp32, as the kernels hold it, and the result is returned in t's dtype."""
+    i = t.detach().float().contiguous().view(torch.int32)
+    return ((i + 0x1000) & ~0x1FFF).view(torch.float32).to(t.dtype)
 
 
 class _RoundSTE(torch.autograd.Function):
@@ -415,12 +467,74 @@ class _LinearTF32(torch.autograd.Function):
         return dyr @ Wr, dyr.T @ x, dyr.sum(0), None
 
 
-def obprop_two_layers_tf32(x, layer1, layer2, s):
-    """x [rows, C] fp32 -> (h1, h2) with the kernels' rounding points (see above)."""
+def obprop_two_layers_tf32(x, layer1, layer2, s, gate1=None, gate2=None, h1_value=None):
+    """x [rows, C] -> (h1, h2, h1_own) with the kernels' rounding points (see above); fp32 or float64 between them.
+    gate1 / gate2 (bool [rows, C], optional): the two ReLUs' decisions (relu_or_gate); h1_value: see forward_dense.
+    h1_own is the model's own layer-1 output, h1 the one layer 2 took."""
     x = _RoundSTE.apply(x)
-    h1 = _RoundSTE.apply(F.relu(_LinearTF32.apply(x, layer1.lin_value.weight, layer1.lin_value.bias, False)) * s)
-    h2 = F.relu(_LinearTF32.apply(h1, layer2.lin_value.weight, layer2.lin_value.bias, True)) * s
-    return h1, h2
+    h1 = h1_own = _RoundSTE.apply(relu_or_gate(_LinearTF32.apply(x, layer1.lin_value.weight, layer1.lin_value.bias, False),
+                                               gate1) * s)
+    if h1_value is not None:
+        h1 = h1 + (h1_value - h1).detach()
+    h2 = relu_or_gate(_LinearTF32.apply(h1, layer2.lin_value.weight, layer2.lin_value.bias, True), gate2) * s
+    return h1, h2, h1_own
+
+
+def dense_train_chunked(model, batch, masks=None, gates=None, chunk=None, tf32_model=False, input_grads=False,
+                        on_chunk=None, h1_value=None):
+    """Cross-entropy (mean over the batch) and its gradients through `forward_dense`, evaluated `chunk` samples at a
+    time on the device and in the dtype of the model's parameters, so that a full-size batch fits in a bounded amount
+    of memory.  Each chunk contributes sum(CE) / B; the parameter gradients accumulate in the parameters' .grad (their
+    dtype).  `masks` (dropout_masks.model_masks layout) and `gates` (forward_dense layout) cover the whole batch and are
+    sliced per chunk, as is `h1_value` [B, N, C] (forward_dense).  on_chunk(sl, stages, logits) sees each chunk's
+    stages before they are dropped.
+
+    Returns {"logits" [B, classes], "loss", and with input_grads "d_src", "d_times", "d_static"}."""
+    from oracle.dropout_masks import slice_masks
+    p0 = next(model.parameters())
+    dev, dt = p0.device, p0.dtype
+    T, B = batch["src"].shape[0], batch["src"].shape[1]
+    chunk = B if chunk is None else int(chunk)
+    model.zero_grad(set_to_none=True)
+    logits_all, loss, grads_in = [], 0.0, {"d_src": [], "d_times": [], "d_static": []}
+    for b0 in range(0, B, chunk):
+        sl = slice(b0, min(B, b0 + chunk))
+        Bc = sl.stop - sl.start
+        src = batch["src"][:, sl].to(dev, dt).requires_grad_(input_grads)
+        times = batch["times"][:, sl].to(dev, dt).requires_grad_(input_grads)
+        static = None if batch["static"] is None else batch["static"][sl].to(dev, dt).requires_grad_(input_grads)
+        g = None
+        if gates is not None:
+            g = {}
+            for k, v in gates.items():
+                if v is None:
+                    continue
+                if k == "ffn":
+                    g[k] = [f.reshape(T, B, -1)[:, sl].reshape(T * Bc, -1) for f in v]
+                elif k == "obs":
+                    g[k] = v[:, sl]
+                else:
+                    g[k] = v[sl]
+        stages = {} if on_chunk is not None else None
+        logits, _, _ = model.forward_dense(src, static, times, batch["lengths"][sl], stages=stages, tf32_model=tf32_model,
+                                           masks=None if masks is None else slice_masks(masks, sl, T, B), gates=g,
+                                           h1_value=None if h1_value is None else h1_value[sl])
+        part = F.cross_entropy(logits, batch["y"][sl].to(dev), reduction="sum") / B
+        part.backward()
+        loss += part.item()
+        logits_all.append(logits.detach())
+        if input_grads:
+            grads_in["d_src"].append(src.grad)
+            grads_in["d_times"].append(times.grad)
+            grads_in["d_static"].append(None if static is None else static.grad)
+        if on_chunk is not None:
+            on_chunk(sl, stages, logits.detach())
+        del logits, part, stages
+    out = dict(logits=torch.cat(logits_all), loss=loss)
+    if input_grads:
+        out.update(d_src=torch.cat(grads_in["d_src"], 1), d_times=torch.cat(grads_in["d_times"], 1),
+                   d_static=None if batch["static"] is None else torch.cat(grads_in["d_static"]))
+    return out
 
 
 def build_oracle_model(cfg, seed=1):

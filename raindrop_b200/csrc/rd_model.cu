@@ -894,7 +894,10 @@ int64_t rd_workspace_offset(const rd_dims* dims, int32_t which, int64_t* n_float
     case RD_WS_ENC_OUT: off = w.Z[s.L]; n = s.M2 * s.D; break;
     case RD_WS_FEAT: off = w.feat; n = (int64_t)s.B * s.Df; break;
     case RD_WS_RNG: off = w.rng; n = 4; break;
-    default: set_error("rd_workspace_offset: unknown buffer %d", which); return -1;
+    case RD_WS_HEAD_HIDDEN: off = w.hpre; n = (int64_t)s.B * s.Df; break;
+    default:
+      if (which >= RD_WS_FFN && which < RD_WS_FFN + s.L) { off = w.l[which - RD_WS_FFN].f; n = s.M2 * s.nhid; break; }
+      set_error("rd_workspace_offset: unknown buffer %d", which); return -1;
   }
   if (n_floats) *n_floats = n;
   return off * (int64_t)sizeof(float);

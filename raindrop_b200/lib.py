@@ -15,7 +15,8 @@ BWD_ENCODER, BWD_OBPROP, BWD_ALL = 1, 2, 3
 RD_D_PE = 16
 
 # enum rd_ws_buffer
-WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG = range(6)
+WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
+WS_FFN = 7                  # + layer index: one view per encoder layer
 
 # dropout site ids (rd_common.cuh: DropSite)
 SITE_LIFT, SITE_ATTN, SITE_RESID1, SITE_FFN, SITE_RESID2 = 1, 16, 32, 48, 64

@@ -100,3 +100,78 @@ def build_dropin(cfg, weight_seed, device="cuda"):
 
 def to_dev(batch, device="cuda"):
     return {k: (v.to(device) if v is not None else None) for k, v in batch.items()}
+
+
+# ---- the GPU's ReLU decisions, for the gate-replaying oracle (RaindropV2Oracle.forward_dense(gates=...)) -------------
+GATE_SITES = ("h1", "obs", "ffn", "head")
+
+
+def ws_view(dims, ws, which):
+    """Named buffer `which` (rd_ws_buffer) of a forward's workspace."""
+    import ctypes as C
+    from raindrop_b200 import lib as L
+    n = C.c_int64(0)
+    off = L.load().rd_workspace_offset(C.byref(dims), which, C.byref(n))
+    assert off >= 0, which
+    return ws[off // 4: off // 4 + n.value]
+
+
+def read_gpu(cfg, dims, ws):
+    """What a forward left in its workspace: the gates of the four ReLU sites in forward_dense's layout (H1 > 0; the obs
+    columns of the encoder input > 0; each layer's FFN activation > 0, whatever its gate where the mask dropped; the
+    head's hidden activation > 0), the (rounded) layer-1 output and the encoder input and output."""
+    from raindrop_b200 import lib as L
+    T, B, N, d_ob = dims.T, dims.B, cfg["d_inp"], cfg["d_ob"]
+    D = N * d_ob + 16
+    h1 = ws_view(dims, ws, L.WS_H1).view(B, N, -1)
+    enc_in = ws_view(dims, ws, L.WS_ENC_IN).view(T, B, D)
+    ffn = [ws_view(dims, ws, L.WS_FFN + l).view(T * B, -1) for l in range(cfg["nlayers"])]
+    gates = dict(h1=h1 > 0, obs=enc_in[:, :, :N * d_ob] > 0, ffn=[f > 0 for f in ffn],
+                 head=ws_view(dims, ws, L.WS_HEAD_HIDDEN).view(B, -1) > 0)
+    return dict(gates=gates, h1=h1.clone(), enc_in=enc_in.clone(),
+                enc_out=ws_view(dims, ws, L.WS_ENC_OUT).view(T, B, D).clone())
+
+
+def gate_disagreements(cfg, gates, stages, masks, sl, B, counts):
+    """Adds to counts[site] = [disagreeing, gates] the gates of samples `sl` (a slice of a batch of B) where the GPU's
+    decision differs from the sign of the oracle's own ReLU input (`stages` of forward_dense on those samples).  FFN
+    gates count only where the mask kept the element (all of them without an FFN mask: eval)."""
+    T, N, d_ob = cfg["max_len"], cfg["d_inp"], cfg["d_ob"]
+    Bc = sl.stop - sl.start
+    dev = stages["obs"].device
+    pre2 = stages["obprop_pre"][1].reshape(Bc, N, T, d_ob).permute(2, 0, 1, 3).reshape(T, Bc, N * d_ob)
+    for site, mine, own in (("h1", gates["h1"][sl], stages["obprop_pre"][0] > 0), ("obs", gates["obs"][:, sl], pre2 > 0),
+                            ("head", gates["head"][sl], stages["head_pre"] > 0)):
+        counts[site][0] += int((mine.to(dev) != own).sum())
+        counts[site][1] += mine.numel()
+    for l, f in enumerate(stages.get("ffn_pre", [])):
+        mk = None if masks is None else masks["layers"][l].get("ffn")
+        kept = torch.ones_like(f, dtype=torch.bool) if mk is None else \
+            torch.as_tensor(mk, device=dev).reshape(T, B, -1)[:, sl] > 0
+        mine = gates["ffn"][l].reshape(T, B, -1)[:, sl].to(dev)
+        counts["ffn"][0] += int(((mine != (f > 0)) & kept).sum())
+        counts["ffn"][1] += int(kept.sum())
+    return counts
+
+
+def tf32_ulp_distance(gpu_h1, own_h1, counts):
+    """Adds to counts = [elements, 1 TF32 ulp apart, more than 1 ulp apart, GPU values not TF32-representable] the
+    comparison of the GPU's TF32-rounded layer-1 output with the rounding model's own (stages["h1_own"]), over the
+    elements where both are positive (where one is not, the gate disagreement counts see it).  Both should hold TF32
+    values, so their fp32 bit patterns differ by a multiple of 2^13 and, for positive values, the pattern difference
+    >> 13 is their distance in TF32 ulps."""
+    a, b = gpu_h1.float(), own_h1.to(gpu_h1.device).float()
+    ia = a.view(torch.int32)
+    both = (a > 0) & (b > 0)
+    d = ((ia - b.view(torch.int32)).abs() >> 13)[both]
+    counts[0] += int(both.sum())
+    counts[1] += int((d == 1).sum())
+    counts[2] += int((d > 1).sum())
+    counts[3] += int(((ia & 0x1FFF) != 0).sum())
+    return counts
+
+
+def h1_ulp_ok(counts, rates):
+    """counts of tf32_ulp_distance within rates = (1-ulp rate, more-than-1-ulp rate); every GPU value TF32."""
+    n, one, more, unrounded = counts
+    return n > 0 and unrounded == 0 and one <= rates[0] * n and more <= rates[1] * n

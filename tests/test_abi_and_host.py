@@ -55,6 +55,38 @@ def test_workspace_queries_are_pure_host_code():
     assert b"divisible" in lib.rd_last_error_string()
 
 
+# (N, d_ob, nhead, nhid, nlayers, d_static, T, B, training): P19, PAM, a model with D, nhid and Df not multiples of 4
+@pytest.mark.parametrize("dims", [(34, 4, 2, 272, 2, 6, 60, 128, True), (17, 4, 2, 136, 2, 0, 600, 3, False),
+                                  (10, 1, 2, 37, 3, 2, 130, 5, True), (8, 2, 8, 64, 8, 0, 48, 1, True)])
+def test_workspace_views_are_disjoint_and_sized(dims):
+    """Every named workspace view (rd_ws_buffer, the per-layer FFN activations included) lies inside the workspace, has
+    its documented size, and overlaps no other view; RD_WS_FFN + nlayers and a negative id are rejected."""
+    _ensure_built()
+    import ctypes as C
+    lib = L.load()
+    N, d_ob, H, nhid, nl, ds, T, B, training = dims
+    d = RF.Plan(N, d_ob, H, nhid, nl, ds, 2, T, 0.2, ds > 0).dims(B, training)
+    total = lib.rd_workspace_bytes(C.byref(d))
+    D = N * d_ob + 16
+    Df = D + (N if ds > 0 else 0)
+    want = {L.WS_X0: B * N * T * d_ob, L.WS_H1: B * N * T * d_ob, L.WS_ENC_IN: T * B * D, L.WS_ENC_OUT: T * B * D,
+            L.WS_FEAT: B * Df, L.WS_RNG: 4, L.WS_HEAD_HIDDEN: B * Df}
+    want.update({L.WS_FFN + l: T * B * nhid for l in range(nl)})
+    spans = []
+    for which, n_want in want.items():
+        n = C.c_int64(0)
+        off = lib.rd_workspace_offset(C.byref(d), which, C.byref(n))
+        assert n.value == n_want, (which, n.value, n_want)
+        assert off >= 0 and off % 256 == 0 and off + 4 * n.value <= total, (which, off, total)
+        spans.append((off, off + 4 * n.value, which))
+    spans.sort()
+    for (a0, a1, wa), (b0, b1, wb) in zip(spans, spans[1:]):
+        assert a1 <= b0, (wa, wb)
+    for bad in (L.WS_FFN + nl, -1):
+        assert lib.rd_workspace_offset(C.byref(d), bad, None) == -1
+        assert b"unknown buffer" in lib.rd_last_error_string()
+
+
 @pytest.mark.parametrize("name", ["P19", "PAM", "TINY"])
 def test_dropin_state_dict_contract(name):
     """Same keys/shapes as the reference (via the oracle, which is key-identical to it), R_u absent."""

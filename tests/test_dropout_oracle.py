@@ -163,3 +163,108 @@ def test_forward_dense_with_unit_masks_equals_forward_dense():
         assert normwise(g1[k], g0[k]) < 1e-12, k
     l2, _, _ = run(DM.model_masks((5, 1), 0.2, cfg, B))
     assert normwise(l2, l0) > 1e-3            # real masks change the function
+
+
+def test_dropout_words_at_arbitrary_indices():
+    """dropout_words_at / dropout_mask_at (used to spot-check full-size masks) equal the sequential stream."""
+    seed, step, site = 0x0123456789ABCDEF, (5 << 32) | 17, 16 + 1
+    n = 4 * 777 + 2
+    words = DM.dropout_words(seed, step, site, n)
+    idx = np.random.default_rng(0).integers(0, n, 500)
+    idx = np.concatenate([[0, 1, 2, 3, n - 1], idx])
+    assert np.array_equal(DM.dropout_words_at(seed, step, site, idx), words[idx])
+    assert np.array_equal(DM.dropout_mask_at(seed, step, site, idx, 0.2), DM.dropout_mask(seed, step, site, n, 0.2)[idx])
+    # indices past 2^32 / 4 blocks carry into the counter's second word
+    big = np.array([(1 << 34) + 5, (1 << 40) + 2], dtype=np.uint64)
+    for i in big:
+        blk = DM.philox4x32_10(np.array([int(i >> 2) & 0xFFFFFFFF, int(i >> 2) >> 32, site, step & 0xFFFFFFFF]),
+                               np.array([seed & 0xFFFFFFFF, (seed >> 32) ^ (step >> 32)]))
+        assert DM.dropout_words_at(seed, step, site, [i])[0] == blk[int(i) & 3]
+
+
+def _dense_run(cfg, batch, masks, gates=None, stages=None, tf32_model=False):
+    oracle = build_oracle_model(cfg).eval()
+    synth_weights(oracle, cfg, seed=11)
+    oracle.double()
+    src = batch["src"].double().requires_grad_(True)
+    times = batch["times"].double().requires_grad_(True)
+    static = None if batch["static"] is None else batch["static"].double().requires_grad_(True)
+    logits, _, _ = oracle.forward_dense(src, static, times, batch["lengths"], stages=stages, masks=masks, gates=gates,
+                                        tf32_model=tf32_model)
+    F.cross_entropy(logits, batch["y"]).backward()
+    g = dict(oracle.named_parameters())
+    out = dict(logits=logits.detach(), d_src=src.grad, d_times=times.grad)
+    if static is not None:
+        out["d_static"] = static.grad
+    out.update({k: g[k].grad for k in used_param_keys(cfg)})
+    return out
+
+
+def own_gates(cfg, stages):
+    """The gates of every site (forward_dense layout) that the oracle's own ReLU inputs in `stages` imply."""
+    T, B = stages["obs"].shape[0], stages["obs"].shape[1]
+    N, d_ob = cfg["d_inp"], cfg["d_ob"]
+    pre2 = stages["obprop_pre"][1]                                   # [B, N, C] -> obs layout [T, B, N*d_ob]
+    return dict(h1=stages["obprop_pre"][0] > 0,
+                obs=(pre2 > 0).reshape(B, N, T, d_ob).permute(2, 0, 1, 3).reshape(T, B, N * d_ob),
+                ffn=[(f > 0).reshape(T * B, -1) for f in stages["ffn_pre"]], head=stages["head_pre"] > 0)
+
+
+@pytest.mark.parametrize("tf32_model", [False, True], ids=["plain", "tf32_model"])
+@pytest.mark.parametrize("name", ["TINY", "TINY8"])
+def test_gate_replay_with_own_gates_is_bitwise(name, tf32_model):
+    """forward_dense(gates=...) with the gates the oracle's own ReLU inputs imply is the run without gates, bitwise, in
+    the logits, every parameter gradient and the input gradients (float64, CPU); and a flipped gate at each site
+    changes the result, so every site is wired."""
+    cfg = model_config(name, dropout=0.2)
+    B = 5
+    batch = make_batch(cfg, B, seed=8)
+    masks = DM.model_masks((3, 4), 0.2, cfg, B)
+    stages = {}
+    ref = _dense_run(cfg, batch, masks, stages=stages, tf32_model=tf32_model)
+    gates = own_gates(cfg, stages)
+    Df = cfg["d_inp"] * (cfg["d_ob"] + (1 if cfg["static"] else 0)) + 16
+    assert len(gates["ffn"]) == cfg["nlayers"] and gates["head"].shape == (B, Df)
+    got = _dense_run(cfg, batch, masks, gates=gates, tf32_model=tf32_model)
+    assert got.keys() == ref.keys()
+    for k in ref:
+        assert torch.equal(got[k], ref[k]), k
+        assert got[k].view(torch.int64).equal(ref[k].view(torch.int64)), k
+    for site in ("h1", "obs", "ffn", "head"):
+        flipped = dict(gates)
+        if site == "ffn":
+            f = gates["ffn"][0].clone()
+            f[: f.shape[0] // 2] = ~f[: f.shape[0] // 2]
+            flipped["ffn"] = [f] + gates["ffn"][1:]
+        else:
+            flipped[site] = ~gates[site]
+        other = _dense_run(cfg, batch, masks, gates=flipped, tf32_model=tf32_model)
+        assert not torch.equal(other["logits"], ref["logits"]), site
+
+
+def test_chunked_training_reference_equals_one_batch():
+    """dense_train_chunked: chunks of 2 samples (masks and gates sliced per chunk) give the one-batch loss, logits and
+    gradients up to float64 summation order."""
+    from oracle.raindrop_oracle import dense_train_chunked
+    cfg = model_config("TINY", dropout=0.2)
+    B = 5
+    batch = make_batch(cfg, B, seed=9)
+    masks = DM.model_masks((3, 5), 0.2, cfg, B)
+    stages = {}
+    ref = _dense_run(cfg, batch, masks, stages=stages)
+    gates = own_gates(cfg, stages)
+    oracle = build_oracle_model(cfg).eval()
+    synth_weights(oracle, cfg, seed=11)
+    oracle.double()
+    seen = []
+    out = dense_train_chunked(oracle, batch, masks=masks, gates=gates, chunk=2, input_grads=True,
+                              on_chunk=lambda sl, st, lg: seen.append((sl.start, sl.stop, st["enc"].shape[1])))
+    assert seen == [(0, 2, 2), (2, 4, 2), (4, 5, 1)]
+    loss = F.cross_entropy(ref["logits"], batch["y"]).item()
+    assert abs(out["loss"] - loss) < 1e-14 * abs(loss)
+    assert normwise(out["logits"], ref["logits"]) < 1e-14
+    for k in ("d_src", "d_times", "d_static"):
+        assert normwise(out[k], ref[k]) < 1e-13, k
+    g = dict(oracle.named_parameters())
+    for k in used_param_keys(cfg):
+        assert normwise(g[k].grad, ref[k]) < 1e-13, k

@@ -23,10 +23,8 @@ cases below each reach a distinct set of kernels; `test_kernel_coverage` asserts
 
 A, B and C are also pinned to the reference's own outputs (tests/golden/hparams_<case>.npz, oracle/make_golden.py).
 
-Bounds are those of test_gpu_parity.test_against_oracle (eval) and test_train_parity.compare (train, replayed masks).
-On top of those, a training step in error-compensated mode whose float64 oracle has no ob-prop and no FFN ReLU input
-within 1e-5 (relative to its tensor's largest) of zero is held to 1e-4 normwise in the logits and every parameter and
-input gradient: no gate can flip there, so the fp32 path has nothing to be further off than its own rounding.
+Bounds are those of test_gpu_parity.test_against_oracle (eval) and test_train_parity.compare (train): a training step
+replays the kernels' dropout masks and ReLU decisions, so every tensor is held to test_train_parity.TIGHT.
 """
 import collections
 import ctypes as C
@@ -44,8 +42,6 @@ from raindrop_b200.synth import make_batch, synth_weights, used_param_keys
 EXACT, FAST = 2, 1
 P = 0.2
 FWD_TOL, GRAD_TOL_EXACT, GRAD_TOL, OBPROP_GRAD_L2, MODEL_TOL = 1e-3, 2e-3, 2e-2, 5e-2, 5e-3
-TIGHT_TOL = 1e-4            # error-compensated training step, no ReLU input of the oracle near zero
-MARGIN = 1e-5               # "near zero": |pre-activation| < MARGIN * max |pre-activation of that tensor|
 HEAD_BWD_MAX_DF = 722       # (1 + 16 warps) * Df floats of shared memory <= 48 KB (rd_head.cu)
 
 # name -> (hyper-parameters, B, data seed, weight seed)
@@ -56,10 +52,6 @@ CASES.update({
     "F": (dict(d_inp=11, d_ob=4, nhead=3, nhid=30, nlayers=2, max_len=65, d_static=0, n_classes=7), 4, 96, 46),
 })
 FIXTURE_CASES = sorted(HPARAM_CASES)
-# cases whose data seed keeps every ReLU input of the masked float64 training forward clear of zero (see
-# relu_margin_ok): their training step is always held to the tight bound.  D and E have 50k+ ob-prop gates, and some
-# of them lie within the margin at any seed.
-TIGHT_CASES = ("A", "B", "C", "F")
 
 
 def case_setup(name):
@@ -360,83 +352,17 @@ def test_eval_against_reference_fixture(golden_dir, name, mode):
     print(name, mode, "worst", max(errs.items(), key=lambda kv: kv[1]))
 
 
-def relu_margin_ok(cfg, batch, ref_stages):
-    """True when no ReLU input of the float64 oracle (both ob-prop layers; the FFN of every encoder layer at valid
-    positions) lies within MARGIN of zero, relative to the largest of its tensor."""
-    valid = (torch.arange(cfg["max_len"])[:, None] < batch["lengths"][None, :])
-    pre = list(ref_stages["obprop_pre"]) + [f[valid] for f in ref_stages["ffn_pre"]]
-    return all(bool((t.abs() >= MARGIN * t.abs().max()).all()) for t in pre)
-
-
 def check_train(name, modes=(EXACT, FAST)):
-    """One training step with replayed masks against the float64 oracle (test_train_parity.compare), input gradients
-    included; in exact mode also the tight bound where relu_margin_ok.  Returns whether the tight bound applied."""
-    from test_train_parity import RNG0, check_masks, compare, gpu_train, oracle_tf32_grads
-    from oracle import dropout_masks as DM
-    from oracle.raindrop_oracle import build_oracle_model
-    cfg, batch, wseed = case_setup(name)
-    B = batch["src"].shape[1]
-    masks = DM.model_masks(RNG0, P, cfg, B)
-    check_masks(masks, P)
-    oracle = build_oracle_model(cfg).eval()
-    synth_weights(oracle, cfg, seed=wseed)
-    oracle.double()
-    src = batch["src"].double().requires_grad_(True)
-    times = batch["times"].double().requires_grad_(True)
-    static = None if batch["static"] is None else batch["static"].double().requires_grad_(True)
-    stages = {}
-    logits, _, _ = oracle.forward_dense(src, static, times, batch["lengths"], stages=stages, masks=masks)
-    loss = F.cross_entropy(logits, batch["y"])
-    loss.backward()
-    go = dict(oracle.named_parameters())
-    ref = dict(logits=logits.detach(), loss=loss.item(), obs=stages["obs"].detach(), pe=stages["pe"].detach(),
-               h1=stages["h1"].detach(), grads={k: go[k].grad for k in used_param_keys(cfg)}, d_src=src.grad,
-               d_times=times.grad, d_static=None if static is None else static.grad)
-    tight = relu_margin_ok(cfg, batch, stages)
-    ref_tf32 = oracle_tf32_grads(cfg, batch, wseed, masks) if FAST in modes else None
-    bad = []
-    N = cfg["d_inp"]
-    for mode in modes:
-        got = gpu_train(cfg, batch, wseed, mode)
-        errs, b = compare(cfg, batch, got, ref, mode, ref_tf32)
-        bad += [(mode,) + x for x in b]
-        if mode == EXACT and tight:
-            valid = (torch.arange(cfg["max_len"])[:, None] < batch["lengths"][None, :]).to(got["d_times"].device)
-            te = {"logits": normwise(got["logits"], ref["logits"]),
-                  "d_src": normwise(got["d_src"][:, :, :N], ref["d_src"][:, :, :N]),
-                  "d_times": normwise(got["d_times"] * valid, ref["d_times"] * valid.cpu())}
-            if ref["d_static"] is not None:
-                te["d_static"] = normwise(got["d_static"], ref["d_static"])
-            te.update({k: normwise(got["grads"][k], ref["grads"][k]) for k in used_param_keys(cfg)})
-            bad += [("tight", k, e, TIGHT_TOL) for k, e in te.items() if not e < TIGHT_TOL]
-            errs = te
-        print("train parity %-6s mode=%s tight=%s worst %s" % (name, "exact" if mode == EXACT else "fast", tight,
-                                                               max(errs.items(), key=lambda kv: kv[1])))
-    assert not bad, (name, bad)
-    return tight
-
-
-def test_named_cases_qualify_for_the_tight_bound():
-    """CPU: at the TIGHT_CASES the float64 training forward keeps all ReLU inputs away from zero, so the GPU training
-    test holds each of them to the tight bound rather than the gate-flip-tolerant one."""
-    from test_train_parity import RNG0
-    from oracle import dropout_masks as DM
-    for name in TIGHT_CASES:
-        cfg, batch, wseed = case_setup(name)
-        oracle = _oracle(cfg, wseed, torch.float64)
-        st = None if batch["static"] is None else batch["static"].double()
-        stages = {}
-        with torch.no_grad():
-            oracle.forward_dense(batch["src"].double(), st, batch["times"].double(), batch["lengths"], stages=stages,
-                                 masks=DM.model_masks(RNG0, P, cfg, batch["src"].shape[1]))
-        assert relu_margin_ok(cfg, batch, stages), name
+    """One training step with replayed masks and gates against the float64 oracle, input gradients included
+    (test_train_parity.check_train_case)."""
+    from test_train_parity import check_train_case
+    check_train_case(name, modes, setup=case_setup(name))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_train_against_masked_oracle(name):
-    tight = check_train(name)
-    assert tight or name not in TIGHT_CASES
+    check_train(name)
 
 
 @pytest.mark.gpu
@@ -452,21 +378,20 @@ def test_dp_sqnorms_against_oracle(name):
     the same masks (bounds of test_dp_sgd.test_sqnorms_train_match_oracle_under_replayed_masks)."""
     from oracle import dropout_masks as DM
     from raindrop_b200 import privacy as PV
-    from test_dp_sgd import RNG0, _close, _gate_flips, _oracle_per_sample
+    from test_dp_sgd import RNG0, _check_gates, _close, _gpu_gates, _oracle_per_sample
     cfg, batch, _ = case_setup(name)
     model = build_dropin(cfg, 21).train()        # _oracle_per_sample builds weight seed 21
     plan = model._prepare(torch.device("cuda"))
     plan.obprop_mode = EXACT
-    plan.rng_state.copy_(torch.tensor(RNG0, dtype=torch.int64))
     d = to_dev(batch)
+    gates = _gpu_gates(model, cfg, d)
     sq = PV.per_sample_grad_sqnorms(model, d["src"], d["static"], d["times"], d["lengths"], d["y"]).cpu().numpy()
     keys = PV.sqnorm_fields(model)
     assert sorted(keys) == sorted(used_param_keys(cfg))
-    ref, _, stages = _oracle_per_sample(cfg, batch, DM.model_masks(RNG0, P, cfg, batch["src"].shape[1]), keys)
+    masks = DM.model_masks(RNG0, P, cfg, batch["src"].shape[1])
+    ref, _, stages = _oracle_per_sample(cfg, batch, masks, keys, gates)
+    _check_gates(cfg, gates, stages, masks, batch["src"].shape[1])
     ok = _close(sq, ref, 1e-4)
-    if _gate_flips(model, cfg, d, stages) > 0:
-        lin = np.array(["lin_value" in k for k in keys])
-        ok |= lin[None, :] & _close(sq, ref, 1e-2)
     assert ok.all(), [(b, keys[f], sq[b, f], ref[b, f]) for b, f in zip(*np.nonzero(~ok))][:10]
 
 
@@ -555,9 +480,10 @@ def test_integrated_gradients_at_d_mod_4():
 @pytest.mark.gpu
 def test_train_step_graph_replay_at_eight_layers():
     """TrainStep (CUDA graph) on B: two steps, each against the float64 oracle at the pre-step parameters under that
-    step's masks (test_train_parity.test_train_step_graph_replay_against_masked_oracle)."""
+    step's masks and gates (test_train_parity.test_train_step_graph_replay_against_masked_oracle)."""
+    from helpers import read_gpu
     from raindrop_b200.train import TrainStep
-    from test_train_parity import GRAD_TOL_EXACT as TOL, LOGIT_TOL_EXACT, _ws_rng, check_masks, oracle_train
+    from test_train_parity import TIGHT, _ws_rng, check_masks, oracle_train
     cfg, batch, wseed = case_setup("B")
     B = batch["src"].shape[1]
     model = build_dropin(cfg, wseed).train()
@@ -573,12 +499,13 @@ def test_train_step_graph_replay_at_eight_layers():
         torch.cuda.synchronize()
         assert ts.graph is not None and _ws_rng(ts.dims, ts.ws) == rng
         sd = {k: p_before[off:off + p.numel()].view(p.shape).cpu() for k, p, off in zip(keys, params, ts.offsets)}
-        ref, masks = oracle_train(cfg, b, wseed, rng, params=sd)
+        ref, masks = oracle_train(cfg, b, wseed, rng, params=sd, gates=read_gpu(cfg, ts.dims, ts.ws)["gates"])
         check_masks(masks, P)
-        assert abs(ts.loss.item() - ref["loss"]) / max(1.0, abs(ref["loss"])) < LOGIT_TOL_EXACT
+        assert all(n <= max(1, 1e-4 * g) for n, g in ref["gate_dis"].values()), ref["gate_dis"]
+        assert abs(ts.loss.item() - ref["loss"]) / max(1.0, abs(ref["loss"])) < TIGHT
         errs = {k: normwise(ts.flat_g[off:off + p.numel()].view(p.shape), ref["grads"][k])
                 for k, p, off in zip(keys, params, ts.offsets)}
-        assert all(e < TOL for e in errs.values()), errs
+        assert all(e < TIGHT for e in errs.values()), errs
         print("TrainStep B step", it, "worst", max(errs.items(), key=lambda kv: kv[1]))
 
 

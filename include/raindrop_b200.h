@@ -543,6 +543,44 @@ int rd_dp_clip_scale(const rd_dims* dims, const void* workspace, const double* s
 int rd_dp_add_noise(float* grad, int64_t n, const int64_t* field_offsets, const int64_t* field_numel, int32_t n_fields,
                     float noise_std, uint64_t* key, void* stream);
 
+/* ---- training-data influence (TracIn, Pruthi et al. 2020) -----------------------------------------------------------
+ * influence(z_q, z_t) = sum_c lr_c < g_q(theta_c), g_t(theta_c) >, g = the per-sample gradients of the DP-SGD section
+ * above, materialised as rows of the flat bucket and contracted on the tensor cores. */
+
+/* Scratch of rd_raindrop_v2_per_sample_grads: a backward scratch. */
+size_t rd_per_sample_grads_scratch_bytes(const rd_dims* dims);
+/* G [B, ldg] (fp32, device, 16-byte aligned): row b = g_b = grad_theta CrossEntropy(logits_b, y_b), the gradient of l_b
+ * (not of l_b / B), in the layout of TrainStep's flat gradient bucket: the trained tensors in the order of the DP-SGD
+ * section, each at an offset rounded up to 4 floats, padding columns written as 0, ldg = the bucket length (anything
+ * else is refused).  d_logits: as rd_raindrop_v2_fwd writes it with labels (the gradient of l_b / B; every row is
+ * scaled by B).  Runs the data-gradient chain of the backward (grads == NULL) and, where the training path queues a
+ * weight-gradient item, writes sample b's [Nout, Kin + 1] tile of dY_b^T [X_b | 1] (the bias as the ones column;
+ * encoder rows t*B + b, ob-prop rows b*N + n) on the CUDA cores, fp32 slices of 16 rows summed in fp64; LayerNorm
+ * gamma / beta from the recomputed normalised input; the head from its one row per sample.  Every value is scaled and
+ * rounded to fp32 once, written by one thread, without atomics: bitwise reproducible.  scratch:
+ * rd_per_sample_grads_scratch_bytes(dims) bytes.  Stream-ordered, sync-free, CUDA-graph capturable. */
+int rd_raindrop_v2_per_sample_grads(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
+                                    const float* node_scale, const void* workspace, const float* d_logits, void* scratch,
+                                    float* G, int64_t ldg, void* stream);
+
+/* Longest segment of rd_per_sample_grad_dot, in columns: each segment's inner product is one fp32 sum of at most this
+ * many error-compensated products. */
+#define RD_GRAD_DOT_SEGMENT 4096
+/* Scratch of rd_per_sample_grad_dot: the remainder image of Gq [Bq, ldg], the segment table and fp32 partial sums
+ * [n_seg, Bq, Bt]. */
+size_t rd_per_sample_grad_dot_scratch_bytes(int32_t Bq, int32_t Bt, int64_t ldg, int32_t n_seg);
+/* scores[q * lds + t] += alpha * sum_s < Gq[q, seg_s], Gt[t, seg_s] > for q < Bq, t < Bt (fp64, device).  Gq [Bq, ldg]
+ * and Gt [Bt, ldg]: fp32 rows, device, 16-byte aligned, ldg % 4 == 0.  Segment s = columns [seg_off[s], + seg_len[s])
+ * (host arrays, n_seg <= 65535, offsets % 4 == 0, 1 <= length <= RD_GRAD_DOT_SEGMENT, inside the row).  A segment's
+ * last 32-column block may reach past its end: those columns of Gq are read and multiplied by 0, so the rows must be
+ * finite.  One psg_lo launch (the remainder image), one launch of wgmma 3xTF32 tiles over (64 queries, 128 train rows, segment), each segment summed in
+ * fp32, and one reduce launch adding the segments in order in fp64: every score is the same product sequence whatever
+ * Bq, Bt and the segment count, hence bitwise reproducible across query blockings and train chunkings.  Stream-ordered;
+ * the segment table is copied from the host (not CUDA-graph capturable). */
+int rd_per_sample_grad_dot(const float* Gq, int32_t Bq, const float* Gt, int32_t Bt, int64_t ldg, const int64_t* seg_off,
+                           const int64_t* seg_len, int32_t n_seg, double alpha, double* scores, int64_t lds, void* scratch,
+                           void* stream);
+
 /* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);

@@ -309,7 +309,156 @@ __global__ void __launch_bounds__(DP_THREADS) dp_noise_kernel(float* __restrict_
   }
 }
 
+// ---- per-sample gradients, materialised ---------------------------------------------------------------------------
+// The explicit form of dp_norm_tile_kernel, written out instead of squared: tile (m0, n0) of sample b's [Nout, Kin + 1]
+// product dY_b^T [X_b | 1], 16-row fp32 slices summed in fp64, each value scaled and rounded to fp32 once.
+__global__ void __launch_bounds__(DP_THREADS) psg_tile_kernel(const __grid_constant__ PsgGroup g, float* __restrict__ G,
+                                                              long long ldg, float scale) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ __align__(16) float As[DP_BK][DP_SMEM_LD];
+  __shared__ __align__(16) float Bs[DP_BK][DP_SMEM_LD];
+  int ii = 0;
+  for (int k = 1; k < g.n; ++k)
+    if ((long long)blockIdx.x >= g.it[k].blk0) ii = k;
+  const PsgItem& o = g.it[ii];
+  const long long local = (long long)blockIdx.x - o.blk0;
+  const int b = (int)(local / o.ntiles), tile = (int)(local % o.ntiles);
+  const float* Yb = o.Y + (long long)b * o.sstride * o.ldy;
+  const float* Xb = o.X + (long long)b * o.sstride * o.ldx;
+  const long long ys = o.rstride * o.ldy, xs = o.rstride * o.ldx;
+  const int m0 = (tile / o.tn) * DP_TILE, n0 = (tile % o.tn) * DP_TILE;
+  double e[4][4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u)
+#pragma unroll
+    for (int v = 0; v < 4; ++v) e[u][v] = 0.0;
+  for (int r0 = 0; r0 < o.R; r0 += DP_BK) {
+    __syncthreads();
+    load_cols(As, Yb, ys, r0, o.R, m0, o.Nout, -1);
+    load_cols(Bs, Xb, xs, r0, o.R, n0, o.Kin, o.Kin);
+    __syncthreads();
+    mma_slice(As, Bs, e);
+  }
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  float* Gb = G + (long long)b * ldg;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int m = m0 + ty * 4 + u;
+    if (m >= o.Nout) continue;
+#pragma unroll
+    for (int v = 0; v < 4; ++v) {
+      const int n = n0 + tx * 4 + v;
+      const float val = (float)(e[u][v] * (double)scale);
+      if (n < o.Kin) Gb[o.gw + (long long)m * o.Kin + n] = val;
+      else if (n == o.Kin) Gb[o.gb + m] = val;
+    }
+  }
+}
+
+// LayerNorm gamma / beta of sample b, written out (dp_ln_sqnorm_kernel's per-column sums)
+__global__ void __launch_bounds__(DP_THREADS) psg_ln_kernel(const float* __restrict__ x, const float* __restrict__ stats,
+                                                            const float* __restrict__ dy, int T, int B, int D,
+                                                            float* __restrict__ G, long long ldg, long long gw, long long gb,
+                                                            float scale) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x;
+  float* Gb = G + (long long)b * ldg;
+  for (int d = threadIdx.x; d < D; d += DP_THREADS) {
+    double sw = 0.0, sb = 0.0;
+    for (int t = 0; t < T; ++t) {
+      const long long r = (long long)t * B + b;
+      const float mean = stats[2 * r], rstd = stats[2 * r + 1];
+      const float g = dy[r * D + d];
+      sw += (double)(g * ((x[r * D + d] - mean) * rstd));
+      sb += (double)g;
+    }
+    Gb[gw + d] = (float)(sw * (double)scale);
+    Gb[gb + d] = (float)(sb * (double)scale);
+  }
+}
+
+// a [n] (x) [x | 1] [m + 1] -> weight [n, m] at Gb + ow, bias [n] at Gb + ob; products in fp64, scaled, rounded once
+__device__ void psg_outer(const float* __restrict__ a, int n, const float* __restrict__ x, int m, float* Gb, long long ow,
+                          long long ob, double scale) {
+  const long long nm = (long long)n * m;
+  for (long long i = threadIdx.x; i < nm; i += DP_THREADS) {
+    const int r = (int)(i / m), c = (int)(i - (long long)r * m);
+    Gb[ow + i] = (float)((double)a[r] * (double)x[c] * scale);
+  }
+  for (int r = threadIdx.x; r < n; r += DP_THREADS) Gb[ob + r] = (float)((double)a[r] * scale);
+}
+
+// the head's one row per sample: mlp_static.2 (d_logits, h), mlp_static.0 (dh, feat), emb (dfeat[:, D:], static)
+__global__ void __launch_bounds__(DP_THREADS) psg_head_kernel(int D, int Df, int ds, int ncls, const float* __restrict__ dlogits,
+                                                              const float* __restrict__ hpre, const float* __restrict__ dh,
+                                                              const float* __restrict__ feat, const float* __restrict__ dfeat,
+                                                              const float* __restrict__ statics, float* __restrict__ G,
+                                                              long long ldg, long long o0, long long o1, long long o2,
+                                                              long long o3, long long o4, long long o5, float scale) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x;
+  const long long rf = (long long)b * Df;
+  float* Gb = G + (long long)b * ldg;
+  if (ds > 0) psg_outer(dfeat + rf + D, Df - D, statics + (long long)b * ds, ds, Gb, o0, o1, scale);
+  psg_outer(dh + rf, Df, feat + rf, Df, Gb, o2, o3, scale);
+  psg_outer(dlogits + (long long)b * ncls, ncls, hpre + rf, Df, Gb, o4, o5, scale);
+}
+
+__global__ void psg_pad_kernel(const __grid_constant__ DpFields fl, int B, float* __restrict__ G, long long ldg) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)fl.n * B) return;
+  const int f = (int)(idx % fl.n), b = (int)(idx / fl.n);
+  const long long end = f + 1 < fl.n ? fl.off[f + 1] : ldg;
+  float* Gb = G + (long long)b * ldg;
+  for (long long i = fl.off[f] + fl.numel[f]; i < end; ++i) Gb[i] = 0.f;
+}
+
 }  // namespace
+
+int psg_tiles(int Nout, int Kin, int* tn) {
+  *tn = (int)ceil_div(Kin + 1, DP_TILE);
+  return (int)ceil_div(Nout, DP_TILE) * *tn;
+}
+
+int psg_group(const PsgGroup& g, int B, float* G, long long ldg, float scale, cudaStream_t st) {
+  if (g.n == 0) return 0;
+  const PsgItem& last = g.it[g.n - 1];
+  const long long blocks = last.blk0 + (long long)B * last.ntiles;
+  if (blocks > 0x7FFFFFFFLL) { set_error("psg_group: %lld tiles, too many for one launch", blocks); return -2; }
+  launch_pdl(psg_tile_kernel, dim3((unsigned)blocks), dim3(DP_THREADS), 0, st, g, G, ldg, scale);
+  RD_CHECK_LAUNCH("psg_tile_kernel");
+  return 0;
+}
+
+int psg_ln(const float* x, const float* stats, const float* dy, int T, int B, int D, float* G, long long ldg, long long gw,
+           long long gb, float scale, cudaStream_t st) {
+  launch_pdl(psg_ln_kernel, dim3(B), dim3(DP_THREADS), 0, st, x, stats, dy, T, B, D, G, ldg, gw, gb, scale);
+  RD_CHECK_LAUNCH("psg_ln_kernel");
+  return 0;
+}
+
+int psg_head(int B, int D, int Df, int ds, int ncls, const float* dlogits, const float* hpre, const float* dh, const float* feat,
+             const float* dfeat, const float* statics, float* G, long long ldg, const long long* off, float scale,
+             cudaStream_t st) {
+  const int h = ds > 0 ? 2 : 0;     // the first field past the static embedding
+  const long long o0 = ds > 0 ? off[0] : 0, o1 = ds > 0 ? off[1] : 0;
+  launch_pdl(psg_head_kernel, dim3(B), dim3(DP_THREADS), 0, st, D, Df, ds, ncls, dlogits, hpre, dh, feat, dfeat, statics, G,
+             ldg, o0, o1, off[h], off[h + 1], off[h + 2], off[h + 3], scale);
+  RD_CHECK_LAUNCH("psg_head_kernel");
+  return 0;
+}
+
+int psg_pad(const DpFields& fields, int B, float* G, long long ldg, cudaStream_t st) {
+  const long long n = (long long)fields.n * B;
+  launch_pdl(psg_pad_kernel, dim3((unsigned)ceil_div(n, 128)), dim3(128), 0, st, fields, B, G, ldg);
+  RD_CHECK_LAUNCH("psg_pad_kernel");
+  return 0;
+}
 
 bool dp_ghost(int R, int Nout, int Kin) {
   return (int64_t)R * (Nout + Kin + 1) < (int64_t)Nout * (Kin + 1);

@@ -205,4 +205,27 @@ int dp_clip(const double* sqnorms, int B, int nf, int ncls, const float* weight,
 struct DpFields { long long off[DP_MAX_FIELDS]; long long numel[DP_MAX_FIELDS]; int n; };
 int dp_noise(float* g, int64_t n, const DpFields& fields, float stdv, uint64_t* key, cudaStream_t st);
 
+// ---- per-sample gradients, materialised (rd_dp.cu; TracIn influence) -------------------------------------------------
+// Sample b's gradient row G[b, :] (ldg floats) in flat-bucket layout, every value scale * (its fp64 sum) rounded once.
+// Item = one (dY, X) pair as in DpNormItem; the sample's [Nout, Kin + 1] product dY_b^T [X_b | 1] goes to the weight
+// field at column gw (row-major [Nout, Kin]) and the bias field at gb.  tn = ceil((Kin + 1) / 64), ntiles = tn *
+// ceil(Nout / 64), blk0 as in DpNormGroup.
+struct PsgItem {
+  const float* Y; const float* X;
+  long long ldy, ldx, sstride, rstride, blk0, gw, gb;
+  int Nout, Kin, R, tn, ntiles;
+};
+struct PsgGroup { PsgItem it[DP_MAX_ITEMS]; int n; };
+int psg_tiles(int Nout, int Kin, int* tn);
+int psg_group(const PsgGroup& g, int B, float* G, long long ldg, float scale, cudaStream_t st);
+// LayerNorm gamma -> G[b, gw + d], beta -> G[b, gb + d] (sums over the rows t*B + b, t < T)
+int psg_ln(const float* x, const float* stats, const float* dy, int T, int B, int D, float* G, long long ldg, long long gw,
+           long long gb, float scale, cudaStream_t st);
+// the head's fields: off[0..5] = emb weight, bias (ds > 0), mlp_static.0 weight, bias, mlp_static.2 weight, bias
+int psg_head(int B, int D, int Df, int ds, int ncls, const float* dlogits, const float* hpre, const float* dh, const float* feat,
+             const float* dfeat, const float* statics, float* G, long long ldg, const long long* off, float scale,
+             cudaStream_t st);
+// zeroes G[b, off[f] + numel[f] .. next field's offset) and the tail up to ldg: the bucket's padding columns
+int psg_pad(const DpFields& fields, int B, float* G, long long ldg, cudaStream_t st);
+
 }  // namespace rd

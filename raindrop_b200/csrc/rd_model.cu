@@ -161,17 +161,47 @@ BwLayout bw_layout(const Shape& s) {
 int dp_head_fields(const Shape& s) { return s.ds > 0 ? 6 : 4; }
 int dp_n_fields(const Shape& s) { return dp_head_fields(s) + 12 * s.L + 4; }
 
-// Norm items of one backward phase, queued where the training path queues the weight-gradient items of the same
-// (dY, X) pairs, and flushed as one group launch (dp_norm_group).  The partial sums of a phase start at `partial` again:
-// the previous phase's launches have completed by then (stream order).
+// Field table of the flat gradient bucket (TrainStep's layout): each trained tensor at a 4-aligned offset, in the order
+// above.  Returns the bucket length.
+int64_t bucket_fields(const Shape& s, DpFields* f) {
+  int64_t n[DP_MAX_FIELDS];
+  int k = 0;
+  if (s.ds > 0) { n[k++] = (int64_t)s.emb * s.ds; n[k++] = s.emb; }
+  n[k++] = (int64_t)s.Df * s.Df; n[k++] = s.Df; n[k++] = (int64_t)s.ncls * s.Df; n[k++] = s.ncls;
+  for (int l = 0; l < s.L; ++l) {
+    const int64_t D = s.D, H = s.nhid;
+    const int64_t v[12] = {3 * D * D, 3 * D, D * D, D, H * D, H, D * H, D, D, D, D, D};
+    for (int i = 0; i < 12; ++i) n[k++] = v[i];
+  }
+  for (int i = 0; i < 2; ++i) { n[k++] = (int64_t)s.C * s.C; n[k++] = s.C; }
+  int64_t off = 0;
+  for (int i = 0; i < k; ++i) { f->off[i] = off; f->numel[i] = n[i]; off += round_up(n[i], 4); }
+  f->n = k;
+  return off;
+}
+
+// Per-sample items of one backward phase, queued where the training path queues the weight-gradient items of the same
+// (dY, X) pairs, and flushed as one group launch.  Two modes: squared norms into `sqnorms` (dp_norm_group; the partial
+// sums of a phase start at `partial` again: the previous phase's launches have completed by then, stream order), or,
+// with G set, the per-sample gradient rows themselves (psg_group), scaled by `scale`.
 struct DpQueue {
   DpNormGroup g;
+  PsgGroup pg;
   long long blk = 0;
   int B = 0, nf = 0;
   double* sqnorms = nullptr; double* partial = nullptr;
-  DpQueue() { g.n = 0; }
+  float* G = nullptr; long long ldg = 0; float scale = 1.f; DpFields fields;     // rows mode
+  DpQueue() { g.n = 0; pg.n = 0; }
   void add(const float* Y, int64_t ldy, const float* X, int64_t ldx, int Nout, int Kin, int R, int64_t sstride,
            int64_t rstride, int fw) {
+    if (G) {
+      PsgItem& o = pg.it[pg.n++];
+      o.Y = Y; o.X = X; o.ldy = ldy; o.ldx = ldx; o.sstride = sstride; o.rstride = rstride; o.blk0 = blk;
+      o.gw = fields.off[fw]; o.gb = fields.off[fw + 1];
+      o.Nout = Nout; o.Kin = Kin; o.R = R; o.ntiles = psg_tiles(Nout, Kin, &o.tn);
+      blk += (long long)B * o.ntiles;
+      return;
+    }
     DpNormItem& o = g.it[g.n++];
     o.Y = Y; o.X = X; o.ldy = ldy; o.ldx = ldx; o.sstride = sstride; o.rstride = rstride; o.blk0 = blk;
     o.Nout = Nout; o.Kin = Kin; o.R = R; o.ghost = dp_ghost(R, Nout, Kin) ? 1 : 0;
@@ -179,9 +209,18 @@ struct DpQueue {
     o.fw = fw; o.fb = fw + 1;
     blk += (long long)B * o.ntiles;
   }
+  int ln(const float* x, const float* stats, const float* dy, int T, int D, int fw, int fb, cudaStream_t st) {
+    if (G) return psg_ln(x, stats, dy, T, B, D, G, ldg, fields.off[fw], fields.off[fb], scale, st);
+    return dp_ln_sqnorm(x, stats, dy, T, B, D, sqnorms, nf, fw, fb, st);
+  }
+  int head(const Shape& s, const float* dlogits, const float* hpre, const float* dh, const float* feat, const float* dfeat,
+           const float* statics, cudaStream_t st) {
+    if (G) return psg_head(B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dh, feat, dfeat, statics, G, ldg, fields.off, scale, st);
+    return dp_head_sqnorm(B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dh, feat, dfeat, statics, sqnorms, nf, st);
+  }
   int flush(cudaStream_t st) {
-    int rc = dp_norm_group(g, B, partial, sqnorms, nf, st);
-    g.n = 0; blk = 0;
+    int rc = G ? psg_group(pg, B, G, ldg, scale, st) : dp_norm_group(g, B, partial, sqnorms, nf, st);
+    g.n = 0; pg.n = 0; blk = 0;
     return rc;
   }
 };
@@ -585,7 +624,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   float* dfeat = sc + b.dfeat; float* dhpre = sc + b.dhpre;
   RD_TRY(head_bwd(s.B, s.T, s.D, s.emb, s.ds, s.ncls, lengths, statics, P->mlp0_weight, P->mlp2_weight, feat, hpre, dlogits,
                   dhpre, dfeat, gA, G->mlp0_weight, G->mlp0_bias, G->mlp2_weight, G->mlp2_bias, G->emb_weight, G->emb_bias, st));
-  if (dp) RD_TRY(dp_head_sqnorm(s.B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dhpre, feat, dfeat, statics, dp->sqnorms, dp->nf, st));
+  if (dp) RD_TRY(dp->head(s, dlogits, hpre, dhpre, feat, dfeat, statics, st));
 
   const float scale = 1.f / sqrtf((float)s.hd);
   const int64_t row3 = (int64_t)s.B * 3 * s.D;
@@ -617,7 +656,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     }
     RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, GE.norm2_weight, GE.norm2_bias,
                          sc + b.l[l].ln[0], K2, s.p, rng, SITE_RESID2 + l, &chunks, st, m2, mld));
-    if (dp) RD_TRY(dp_ln_sqnorm(r2, ws + w.l[l].st2, gA, s.T, s.B, s.D, dp->sqnorms, dp->nf, fl + 10, fl + 11, st));
+    if (dp) RD_TRY(dp->ln(r2, ws + w.l[l].st2, gA, s.T, s.D, fl + 10, fl + 11, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0], 2 * s.D, chunks, s.D, GE.norm2_weight, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0] + s.D, 2 * s.D, chunks, s.D, GE.norm2_bias, st));
     if (wg) RD_TRY(tn(&wq, K2, s.D, f, s.nhid, GE.linear2_weight, GE.linear2_bias, s.D, s.nhid, s.M2, sc + b.l[l].wp[0], partial, st));
@@ -638,7 +677,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     res = s.p > 0.f ? gB : K1;
     RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, GE.norm1_weight, GE.norm1_bias,
                          sc + b.l[l].ln[1], K1, s.p, rng, SITE_RESID1 + l, &chunks, st, m1, mld));
-    if (dp) RD_TRY(dp_ln_sqnorm(r1, ws + w.l[l].st1, gA, s.T, s.B, s.D, dp->sqnorms, dp->nf, fl + 8, fl + 9, st));
+    if (dp) RD_TRY(dp->ln(r1, ws + w.l[l].st1, gA, s.T, s.D, fl + 8, fl + 9, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1], 2 * s.D, chunks, s.D, GE.norm1_weight, st));
     if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1] + s.D, 2 * s.D, chunks, s.D, GE.norm1_bias, st));
     if (wg) RD_TRY(tn(&wq, K1, s.D, ctx, s.D, GE.out_proj_weight, GE.out_proj_bias, s.D, s.D, s.M2, sc + b.l[l].wp[2], partial, st));
@@ -1314,6 +1353,36 @@ int rd_raindrop_v2_per_sample_grad_sqnorms(const rd_dims* dims, const rd_params*
   q.partial = reinterpret_cast<double*>((float*)scratch + l.partial);
   return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr,
                       (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, &q);
+}
+
+size_t rd_per_sample_grads_scratch_bytes(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return (size_t)bw_layout(s).total * sizeof(float);
+}
+
+int rd_raindrop_v2_per_sample_grads(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
+                                    const float* node_scale, const void* workspace, const float* d_logits, void* scratch,
+                                    float* G, int64_t ldg, void* stream) {
+  const char* fn = "rd_raindrop_v2_per_sample_grads";
+  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch || !G) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  DpQueue q;
+  const int64_t bucket = bucket_fields(s, &q.fields);
+  if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
+  if (reinterpret_cast<uintptr_t>(G) & 15) { set_error("%s: G must be 16-byte aligned", fn); return -2; }
+  q.B = s.B; q.nf = q.fields.n; q.G = G; q.ldg = ldg;
+  q.scale = (float)s.B;      // d_logits holds the gradient of l_b / B (the forward's batch mean): rows are of l_b
+  cudaStream_t st = (cudaStream_t)stream;
+  RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, (float*)scratch,
+                      RD_BWD_ALL, nullptr, st, &q);
 }
 
 int rd_dp_clip_scale(const rd_dims* dims, const void* workspace, const double* sqnorms, const float* weight,

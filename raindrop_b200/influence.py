@@ -1,0 +1,450 @@
+"""Training-data influence of Raindrop_v2: TracIn (Pruthi et al. 2020; Captum's TracInCP) with the per-sample gradients
+and their inner products computed on the device.
+
+    influence(z_q, z_t) = sum_c lr_c < grad_theta l(z_q; theta_c), grad_theta l(z_t; theta_c) >
+
+l = CrossEntropy of one sample, theta_c = the trained tensors at checkpoint c.  A large positive score marks a training
+sample that pushed the query's prediction ("proponent"), a large negative one an "opponent"; a large self-influence
+sum_c lr_c ||g_t||^2 marks training samples the model found hard, often mislabelled ones.
+
+    scores = tracin(model, {"src": X, "static": S, "times": t, "lengths": n, "y": None},     # y None: predicted class
+                    DeviceDataset(P, Pstatic, Ptime, y), checkpoints=[(sd1, 1e-4), (sd2, 1e-4)])
+
+The gradient rows come from rd_raindrop_v2_per_sample_grads (a data-gradient backward that writes each sample's gradient
+in the layout of TrainStep's flat bucket) and are contracted by rd_per_sample_grad_dot (wgmma 3xTF32, fp32 within
+segments of at most RD_GRAD_DOT_SEGMENT columns, fp64 across them), so a score is bitwise the same for any chunking.
+The model runs in eval arithmetic; the ob-prop layers run in their error-compensated mode unless the model pins the
+single-pass mode (obprop_mode 1).  One GPU per call.
+"""
+import ctypes as C
+import math
+
+import numpy as np
+import torch
+
+from . import lib as L
+from .attribution import DEFAULT_SCRATCH_BYTES, _Call, _check_call, _largest_chunk
+
+SEGMENT = L.GRAD_DOT_SEGMENT
+
+
+def grad_layout(model):
+    """[(state-dict key, offset, shape)] of the trained tensors in a gradient row (TrainStep's flat bucket: each tensor
+    at an offset rounded up to 4 floats)."""
+    out, off = [], 0
+    for (key, _), p in zip(model._plan.fields, model.used_parameters()):
+        out.append((key, off, tuple(p.shape)))
+        off += (p.numel() + 3) // 4 * 4
+    return out
+
+
+def _bucket_length(layout):
+    key, off, shape = layout[-1]
+    return off + (math.prod(shape) + 3) // 4 * 4
+
+
+def _selected(layout, fields):
+    keys = [k for k, _, _ in layout]
+    if fields is None:
+        return set(keys)
+    if isinstance(fields, str):
+        raise ValueError("fields must be a list of state-dict keys, not a string")
+    sel = list(fields)
+    unknown = [k for k in sel if k not in keys]
+    if unknown:
+        raise ValueError("unknown fields %s: pick from privacy.sqnorm_fields(model)" % unknown)
+    if not sel or len(set(sel)) != len(sel):
+        raise ValueError("fields must be a non-empty list without repeats")
+    return set(sel)
+
+
+def plan_segments(layout, fields=None):
+    """(seg_off, seg_len) int64 arrays: the columns of the selected fields, each field cut into pieces of at most SEGMENT
+    columns (every piece starts 4-aligned, since fields and SEGMENT are; no piece crosses a field)."""
+    sel = _selected(layout, fields)
+    offs, lens = [], []
+    for key, off, shape in layout:
+        if key not in sel:
+            continue
+        n = math.prod(shape)
+        for s in range(0, n, SEGMENT):
+            offs.append(off + s)
+            lens.append(min(SEGMENT, n - s))
+    return np.asarray(offs, dtype=np.int64), np.asarray(lens, dtype=np.int64)
+
+
+def _dims(plan, B):
+    """Eval dims of B rows with the ob-prop arithmetic pinned (auto -> error-compensated), so it cannot follow B."""
+    cache = plan.__dict__.setdefault("_influence_dims", {})
+    key = (B, plan.obprop_mode)
+    d = cache.get(key)
+    if d is None:
+        src = plan.dims(B, False)
+        d = L.RdDims()
+        C.memmove(C.byref(d), C.byref(src), C.sizeof(src))
+        if d.obprop_mode == 0:
+            d.obprop_mode = 2
+        d = cache[key] = d
+    return d
+
+
+def _rows_bytes(lib, plan, B, ldg):
+    d = _dims(plan, B)
+    return lib.rd_workspace_bytes(C.byref(d)) + lib.rd_per_sample_grads_scratch_bytes(C.byref(d)) + 4 * B * ldg
+
+
+def _row_batch(lib, plan, ldg, cap=DEFAULT_SCRATCH_BYTES):
+    """Samples per forward / backward of the row computation: a power of two <= 128 whose buffers fit in half the cap.
+    It depends on the model alone, and rows are computed in batches aligned to its multiples, so every sample's row comes
+    from the same batch whatever the chunking (the forward's arithmetic depends on the batch it runs in)."""
+    r = 128
+    while r > 1 and _rows_bytes(lib, plan, r, ldg) > cap // 2:
+        r //= 2
+    return r
+
+
+def _rows_aligned(model, fetch, i0, i1, R, ldg):
+    """Rows of samples [i0, i1) (i0 a multiple of R), computed in batches [k R, (k + 1) R)."""
+    G = None
+    for s0 in range(i0, i1, R):
+        s1 = min(i1, s0 + R)
+        g = _rows(model, *fetch(s0, s1), ldg)
+        if G is None:
+            if s1 == i1:
+                return g
+            G = torch.empty(i1 - i0, ldg, dtype=torch.float32, device=g.device)
+        G[s0 - i0:s1 - i0] = g
+        del g
+    return G
+
+
+def _rows(model, src, static, times, lengths, y, ldg):
+    """[B, ldg] float32 gradient rows of CrossEntropy(logits_b, y_b); y None: the predicted class (argmax of the logits)."""
+    cl = _Call(model, src, static, times, lengths, None, False)
+    lib, plan, dev = cl.lib, cl.plan, cl.device
+    B = cl.x.shape[1]
+    dims = _dims(plan, B)
+    key = (B, dims.obprop_mode, dev.index)
+    ws = cl.scratch("_psg_workspace", key, lib.rd_workspace_bytes(C.byref(dims)))
+    f32 = dict(device=dev, dtype=torch.float32)
+    logits, dlog, loss = torch.empty(B, plan.n_classes, **f32), torch.empty(B, plan.n_classes, **f32), torch.empty(1, **f32)
+    st = L.stream_ptr(dev)
+
+    def fwd(yv):
+        L.check(lib.rd_raindrop_v2_fwd(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st), cl.tm.data_ptr(),
+                                       cl.ln.data_ptr(), plan.node_scale.data_ptr(), L.ptr(plan.rng_state), ws.data_ptr(),
+                                       logits.data_ptr(), L.ptr(yv), L.ptr(None if yv is None else loss),
+                                       L.ptr(None if yv is None else dlog), st), "rd_raindrop_v2_fwd")
+
+    if y is None:
+        fwd(None)
+        y = logits.argmax(dim=1)
+    fwd(y.to(device=dev, dtype=torch.int64).contiguous())
+    G = torch.empty(B, ldg, **f32)
+    scratch = cl.scratch("_psg_scratch", key, lib.rd_per_sample_grads_scratch_bytes(C.byref(dims)))
+    L.check(lib.rd_raindrop_v2_per_sample_grads(C.byref(dims), C.byref(cl.params), L.ptr(cl.st), cl.ln.data_ptr(),
+                                                plan.node_scale.data_ptr(), ws.data_ptr(), dlog.data_ptr(), scratch.data_ptr(),
+                                                G.data_ptr(), ldg, st), "rd_raindrop_v2_per_sample_grads")
+    return G
+
+
+def _check_labels(y, B, n_classes, allow_none=False):
+    if y is None:
+        if allow_none:
+            return None
+        raise ValueError("y (labels [B]) is required")
+    t = torch.as_tensor(y)
+    if t.is_floating_point() or t.is_complex() or t.dtype == torch.bool:
+        raise ValueError("y must hold integer class indices")
+    if tuple(t.shape) != (B,):
+        raise ValueError("y must be [B=%d], got %s" % (B, tuple(t.shape)))
+    if B:
+        lo, hi = torch.stack(torch.aminmax(t)).tolist()
+        if lo < 0 or hi >= n_classes:
+            raise ValueError("y values must lie in [0, %d), got [%d, %d]" % (n_classes, lo, hi))
+    return t
+
+
+def per_sample_grads(model, src, static, times, lengths, y):
+    """[B, bucket] float32 on the device: row b = the gradient of CrossEntropy(logits_b, y_b) (not divided by B) with
+    respect to every trained tensor, laid out as grad_layout(model) (padding columns 0).  Eval mode only; parameters and
+    their .grad are left unchanged.  Raises RaindropB200Error without CUDA or without the built library."""
+    _check_call("per_sample_grads", model, src, static, None, None)
+    y = _check_labels(y, src.shape[1], model._plan.n_classes)
+    with torch.no_grad():
+        return _rows(model, src, static, times, lengths, y, _bucket_length(grad_layout(model)))
+
+
+# ---- data sources: a dict of tensors, or a DeviceDataset (optionally with an index subset) ----------------------------
+def _source(data, what):
+    """-> (n, fetch(i0, i1) -> (src, static, times, lengths, y)).  data: dict(src, static, times, lengths, y),
+    a data.DeviceDataset, or a pair (DeviceDataset, indices)."""
+    from .data import BatchBuffers, DeviceDataset
+    idx = None
+    if isinstance(data, tuple) and len(data) == 2 and isinstance(data[0], DeviceDataset):
+        data, idx = data
+    if isinstance(data, DeviceDataset):
+        ds = data
+        idx = torch.arange(ds.n, dtype=torch.int64) if idx is None else torch.as_tensor(idx, dtype=torch.int64).reshape(-1)
+        if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= ds.n):
+            raise ValueError("%s indices must lie in [0, %d)" % (what, ds.n))
+        if ds.y is None:
+            raise ValueError("%s DeviceDataset has no labels" % what)
+        idx = idx.to(ds.P.device)
+
+        def fetch(i0, i1):
+            buf = BatchBuffers(ds.T, i1 - i0, ds.width, 0 if ds.Pstatic is None else ds.Pstatic.shape[1], device=ds.P.device)
+            ds.fill(buf, idx[i0:i1])
+            return buf.src, buf.static, buf.times, buf.lengths, buf.y
+        return idx.numel(), fetch
+    if not isinstance(data, dict):
+        raise TypeError("%s must be a dict (src, static, times, lengths, y) or a DeviceDataset" % what)
+    missing = [k for k in ("src", "times", "lengths") if data.get(k) is None]
+    if missing:
+        raise ValueError("%s is missing %s" % (what, missing))
+    src, static, times, lengths, y = (data["src"], data.get("static"), data["times"], data["lengths"], data.get("y"))
+
+    def fetch(i0, i1):
+        return (src[:, i0:i1], None if static is None else static[i0:i1], times[:, i0:i1], lengths[i0:i1],
+                None if y is None else y[i0:i1])
+    return src.shape[1], fetch
+
+
+def _check_data(model, data, what, allow_none_y):
+    """Host-side checks of a data argument against the model, before anything touches the device: a dict's tensor
+    shapes and labels, or a DeviceDataset's T, width, static width, indices and the labels it will serve."""
+    from .data import DeviceDataset
+    from .models_rd import Raindrop_v2
+    plan = model._plan
+    if isinstance(data, tuple) and len(data) == 2 and isinstance(data[0], DeviceDataset):
+        ds, idx = data
+    else:
+        ds, idx = data, None
+    if isinstance(ds, DeviceDataset):
+        if not isinstance(model, Raindrop_v2):
+            raise TypeError("%s takes a raindrop_b200 Raindrop_v2 model, got %s" % (what, type(model).__name__))
+        if model.training:
+            raise ValueError("%s runs the model in eval arithmetic: call model.eval() first" % what)
+        ds_static = 0 if ds.Pstatic is None else ds.Pstatic.shape[1]
+        if ds.T != plan.T or ds.width != 2 * plan.N or (model.static and ds_static != plan.d_static):
+            raise ValueError("%s DeviceDataset holds [T=%d, n, %d] with %d static columns; the model needs [T=%d, n, %d] "
+                             "with %d" % (what, ds.T, ds.width, ds_static, plan.T, 2 * plan.N,
+                                          plan.d_static if model.static else 0))
+        if tuple(ds.Ptime.shape) != (ds.T, ds.n):
+            raise ValueError("%s DeviceDataset times must be [T, n]" % what)
+        if ds.y is None:
+            raise ValueError("%s DeviceDataset has no labels" % what)
+        if tuple(ds.y.shape) != (ds.n,):
+            raise ValueError("%s DeviceDataset labels must be [n]" % what)
+        sel = torch.arange(ds.n, dtype=torch.int64) if idx is None else torch.as_tensor(idx).reshape(-1)
+        if sel.is_floating_point() or sel.dtype == torch.bool:
+            raise ValueError("%s indices must be integers" % what)
+        if sel.numel():
+            lo, hi = torch.stack(torch.aminmax(sel.to(torch.int64))).tolist()
+            if lo < 0 or hi >= ds.n:
+                raise ValueError("%s indices must lie in [0, %d)" % (what, ds.n))
+            ys = ds.y[sel.to(ds.y.device)] if idx is not None else ds.y
+            lo, hi = torch.stack(torch.aminmax(ys)).tolist()         # one host sync
+            if lo < 0 or hi >= plan.n_classes:
+                raise ValueError("%s labels must lie in [0, %d), got [%d, %d]" % (what, plan.n_classes, lo, hi))
+        return
+    if not isinstance(data, dict):
+        raise TypeError("%s must be a dict (src, static, times, lengths, y), a DeviceDataset or (DeviceDataset, indices)"
+                        % what)
+    src = data.get("src")
+    if src is None:
+        raise ValueError("%s is missing ['src']" % what)
+    _check_call(what, model, src, data.get("static"), None, None)
+    B = src.shape[1]
+    shapes = [("times", (plan.T, B)), ("lengths", (B,))]
+    if model.static:
+        shapes.append(("static", (B, plan.d_static)))
+    for k, shape in shapes:
+        v = data.get(k)
+        if v is None or tuple(v.shape) != shape:
+            raise ValueError("%s[%r] must be %s" % (what, k, shape))
+    _check_labels(data.get("y"), B, plan.n_classes, allow_none=allow_none_y)
+
+
+def _checkpoints(model, checkpoints):
+    """[(state_dict or None, lr)]; None = the current weights with lr 1."""
+    if checkpoints is None:
+        return [(None, 1.0)]
+    out = []
+    keys = [k for k, _ in model._plan.fields]
+    shapes = {k: tuple(p.shape) for k, p in zip(keys, model.used_parameters())}
+    for c in checkpoints:
+        if not isinstance(c, (tuple, list)) or len(c) != 2:
+            raise ValueError("each checkpoint must be a pair (state_dict, lr)")
+        sd, lr = c
+        lr = float(lr)
+        if not math.isfinite(lr):
+            raise ValueError("checkpoint lr must be finite")
+        missing = [k for k in keys if k not in sd]
+        if missing:
+            raise ValueError("checkpoint state_dict is missing %s" % missing[:4])
+        bad = [k for k in keys if tuple(sd[k].shape) != shapes[k]]
+        if bad:
+            raise ValueError("checkpoint tensors of the wrong shape: %s" % bad[:4])
+        out.append((sd, lr))
+    if not out:
+        raise ValueError("checkpoints must not be empty")
+    return out
+
+
+class _Weights:
+    """Loads checkpoints into the trained tensors in place; restores the original values, the mode and the dropout
+    counter on exit."""
+
+    def __init__(self, model):
+        self.model = model
+
+    def __enter__(self):
+        m = self.model
+        self.params = m.used_parameters()
+        self.saved = [p.detach().clone() for p in self.params]
+        self.training = m.training
+        rs = m._plan.rng_state
+        self.rng = None if rs is None else rs.clone()
+        return self
+
+    def load(self, sd):
+        with torch.no_grad():
+            for (key, _), p in zip(self.model._plan.fields, self.params):
+                p.copy_(sd[key])
+
+    def __exit__(self, *exc):
+        with torch.no_grad():
+            for p, s in zip(self.params, self.saved):
+                p.copy_(s)
+            if self.rng is not None:
+                self.model._plan.rng_state.copy_(self.rng)
+        self.model.train(self.training)
+        return False
+
+
+def _check_batch_size(internal_batch_size):
+    if internal_batch_size is not None and int(internal_batch_size) < 1:
+        raise ValueError("internal_batch_size must be >= 1")
+
+
+def _blocks(lib, plan, ldg, n_seg, nq, nt, internal_batch_size, cap=DEFAULT_SCRATCH_BYTES):
+    """(query block, train chunk, row batch R): blocks are multiples of R (internal_batch_size is rounded up to one).
+    By default the query block is the largest whose rows, their remainder image (the dot's scratch) and one row batch's
+    buffers fit in `cap`, and the train chunk the largest whose rows, one row batch's buffers and the dot's partial sums
+    do; both are resident during a dot, so a call holds at most about 2 `cap` (2 GiB) besides the scores."""
+    R = _row_batch(lib, plan, ldg, cap)
+    up = lambda b: max(R, (b + R - 1) // R * R)
+    down = lambda b: max(R, b // R * R)
+    qb = down(_largest_chunk(lambda b: 8 * b * ldg + _rows_bytes(lib, plan, min(b, R), ldg), nq, cap))
+    tc = down(_largest_chunk(lambda b: 4 * b * ldg + _rows_bytes(lib, plan, min(b, R), ldg) + 4 * n_seg * qb * b, nt, cap))
+    if internal_batch_size is not None:
+        qb = tc = up(int(internal_batch_size))
+    return qb, tc, R
+
+
+def tracin(model, query, train, checkpoints=None, fields=None, internal_batch_size=None):
+    """TracIn scores [n_query, n_train] float64 on the device: sum_c lr_c <g_q(theta_c), g_t(theta_c)> over the selected
+    fields (default: all trained tensors; a subset of privacy.sqnorm_fields(model), Captum's `layers`).
+
+    query: dict(src, static, times, lengths, y); y None = each query's predicted class.  train: such a dict with y, a
+    data.DeviceDataset, or a pair (DeviceDataset, indices).  checkpoints: [(state_dict, lr)] holding the trained tensors
+    (default: the current weights, lr 1); the weights, the mode and the dropout counter are restored afterwards.
+    internal_batch_size: rows per train chunk and per query block, rounded up to a multiple of the row batch (at most
+    128 samples per forward; default: the largest whose buffers fit in 1 GiB each, so a call holds about 2 GiB).
+    The query rows are computed once per checkpoint and query block, the train rows once per checkpoint, query
+    block and chunk.  Eval mode only."""
+    from .models_rd import _device_of
+    if not isinstance(query, dict):
+        raise TypeError("query must be a dict (src, static, times, lengths, y)")
+    _check_data(model, query, "query", allow_none_y=True)
+    _check_data(model, train, "train", allow_none_y=False)
+    _check_batch_size(internal_batch_size)
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    seg_off, seg_len = plan_segments(layout, fields)
+    ckpts = _checkpoints(model, checkpoints)
+    dev = _device_of(query["src"])
+    lib = L.load()
+    plan = model._prepare(dev)
+    nq, q_fetch = _source(query, "query")
+    nt, t_fetch = _source(train, "train")
+    n_seg = len(seg_off)
+    scores = torch.zeros(nq, nt, dtype=torch.float64, device=dev)
+    if nq == 0 or nt == 0:
+        return scores
+    qb, tc, R = _blocks(lib, plan, ldg, n_seg, nq, nt, internal_batch_size)
+    offs = (C.c_int64 * n_seg)(*seg_off.tolist())
+    lens = (C.c_int64 * n_seg)(*seg_len.tolist())
+    st = L.stream_ptr(dev)
+    with torch.no_grad(), _Weights(model) as w:
+        for sd, lr in ckpts:
+            if sd is not None:
+                w.load(sd)
+            for q0 in range(0, nq, qb):
+                q1 = min(nq, q0 + qb)
+                Gq = _rows_aligned(model, q_fetch, q0, q1, R, ldg)
+                for t0 in range(0, nt, tc):
+                    t1 = min(nt, t0 + tc)
+                    Gt = _rows_aligned(model, t_fetch, t0, t1, R, ldg)
+                    nb = lib.rd_per_sample_grad_dot_scratch_bytes(q1 - q0, t1 - t0, ldg, n_seg)
+                    sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
+                    L.check(lib.rd_per_sample_grad_dot(Gq.data_ptr(), q1 - q0, Gt.data_ptr(), t1 - t0, ldg, offs, lens, n_seg,
+                                                       lr, scores.data_ptr() + 8 * (q0 * nt + t0), nt, sc.data_ptr(), st),
+                            "rd_per_sample_grad_dot")
+                    del Gt, sc
+                del Gq
+    return scores
+
+
+def self_influence(model, data, checkpoints=None, fields=None, internal_batch_size=None):
+    """[n] float64 on the device: sum_c lr_c ||g(theta_c)||^2 over the selected fields, from per_sample_grad_sqnorms
+    (raindrop_b200.privacy; no gradient rows are materialised).  data: as tracin's train argument.  Chunks of tracin's
+    row batch (internal_batch_size rounds up to a multiple of it), in tracin's ob-prop arithmetic."""
+    from .models_rd import _device_of
+    from .privacy import per_sample_grad_sqnorms, sqnorm_fields
+    _check_data(model, data, "data", allow_none_y=False)
+    _check_batch_size(internal_batch_size)
+    if model.training:
+        raise ValueError("self_influence runs the model in eval arithmetic: call model.eval() first")
+    keys = sqnorm_fields(model)
+    sel = _selected(grad_layout(model), fields)
+    cols = torch.tensor([i for i, k in enumerate(keys) if k in sel], dtype=torch.int64)
+    ckpts = _checkpoints(model, checkpoints)
+    n, fetch = _source(data, "data")
+    dev = _device_of(data["src"]) if isinstance(data, dict) else (data[0] if isinstance(data, tuple) else data).P.device
+    out = torch.zeros(n, dtype=torch.float64, device=dev)
+    lib = L.load()
+    plan = model._prepare(dev)
+    # chunks of tracin's row batch (so each chunk's buffers fit the cap), in tracin's ob-prop arithmetic: auto is pinned
+    # to the error-compensated mode for the call, so the diagonal of tracin(X, X) and this agree
+    R = _row_batch(lib, plan, _bucket_length(grad_layout(model)))
+    chunk = R if internal_batch_size is None else max(R, (int(internal_batch_size) + R - 1) // R * R)
+    mode = plan.obprop_mode
+    try:
+        if mode == 0:
+            plan.obprop_mode = 2
+        with torch.no_grad(), _Weights(model) as w:
+            for sd, lr in ckpts:
+                if sd is not None:
+                    w.load(sd)
+                for i0 in range(0, n, chunk):
+                    i1 = min(n, i0 + chunk)
+                    sq = per_sample_grad_sqnorms(model, *fetch(i0, i1))
+                    out[i0:i1] += lr * sq[:, cols.to(dev)].sum(dim=1)
+    finally:
+        plan.obprop_mode = mode
+    return out
+
+
+def tracin_from_grads(Gq, Gt, lrs):
+    """Host restatement of tracin in float64: Gq [n_ckpt, n_query, K] and Gt [n_ckpt, n_train, K] gradient rows (any
+    array-likes; a 2-D pair is one checkpoint), lrs [n_ckpt] -> sum_c lrs[c] Gq[c] Gt[c]^T [n_query, n_train]."""
+    Gq = np.asarray(Gq, dtype=np.float64)
+    Gt = np.asarray(Gt, dtype=np.float64)
+    if Gq.ndim == 2:
+        Gq, Gt = Gq[None], Gt[None]
+    lrs = np.atleast_1d(np.asarray(lrs, dtype=np.float64))
+    if Gq.ndim != 3 or Gt.ndim != 3 or Gq.shape[0] != Gt.shape[0] or Gq.shape[2] != Gt.shape[2] or lrs.shape != (Gq.shape[0],):
+        raise ValueError("Gq [c, q, K], Gt [c, t, K] and lrs [c] do not match: %s, %s, %s" % (Gq.shape, Gt.shape, lrs.shape))
+    return np.einsum("c,cqk,ctk->qt", lrs, Gq, Gt)

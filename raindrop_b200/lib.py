@@ -13,6 +13,7 @@ RD_MAX_LAYERS = 8
 ABI_VERSION = 2
 BWD_ENCODER, BWD_OBPROP, BWD_ALL = 1, 2, 3
 RD_D_PE = 16
+GRAD_DOT_SEGMENT = 4096     # RD_GRAD_DOT_SEGMENT
 
 # enum rd_ws_buffer
 WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
@@ -151,6 +152,13 @@ SIGNATURES = {
                          [C.c_void_p] * 4),
     "rd_dp_add_noise": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int32, C.c_float,
                                   C.c_void_p, C.c_void_p]),
+    "rd_per_sample_grads_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
+    "rd_raindrop_v2_per_sample_grads": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 7 +
+                                        [C.c_int64, C.c_void_p]),
+    "rd_per_sample_grad_dot_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int64, C.c_int32]),
+    "rd_per_sample_grad_dot": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int64), C.c_int32, C.c_double, C.c_void_p, C.c_int64, C.c_void_p,
+                                         C.c_void_p]),
     "rd_debug_attention_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_gemm_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_wgrad_timing": (C.c_int, [C.c_void_p]),

@@ -581,6 +581,27 @@ int rd_per_sample_grad_dot(const float* Gq, int32_t Bq, const float* Gt, int32_t
                            const int64_t* seg_len, int32_t n_seg, double alpha, double* scores, int64_t lds, void* scratch,
                            void* stream);
 
+/* Random projection of gradient rows (TracIn-RP, Pruthi et al. 2020): phi = g Omega / sqrt(dim), E[phi_q . phi_t] =
+ * g_q . g_t.  Omega [ldg, dim] is +-1 and never stored: Omega(seed, j, m) for absolute column j and dimension m is
+ * bit (j & 31) of word ((j >> 5) & 3) of Philox4x32-10 with key (seed & 0xffffffff, seed >> 32) and counter
+ * (jb & 0xffffffff, jb >> 32, m, 0), jb = j >> 7 (words and bits numbered from 0, bits from the least significant);
+ * bit 0 -> +1, bit 1 -> -1.  A column has the same signs whatever the fields, the segments or the rows.  dim: a multiple
+ * of 128 in [128, 32768]. */
+/* Scratch of rd_grad_projection: the remainder image of G [rows, ldg], the segment table and fp32 partial sums
+ * [n_seg, rows, dim]; 0 for sizes rd_grad_projection refuses. */
+size_t rd_grad_projection_scratch_bytes(int32_t rows, int64_t ldg, int32_t dim, int32_t n_seg);
+/* out[r * ldo + m] = (1/sqrt(dim)) sum_s sum_{j in seg_s} G[r, j] Omega(seed, j, m) for r < rows, m < dim (fp32,
+ * device).  G [rows, ldg]: fp32 rows, device, 16-byte aligned, ldg % 4 == 0.  Segments as for rd_per_sample_grad_dot
+ * (host arrays, n_seg <= 65535, offsets % 4 == 0, 1 <= length <= RD_GRAD_DOT_SEGMENT, inside the row); the k-blocks
+ * run over whole 32-column blocks, so columns next to a segment are read and multiplied by 0 and the rows must be
+ * finite.  One psg_lo launch (the remainder image), one launch of wgmma TF32 tiles over (128 dimensions, 64 rows,
+ * segment) with Omega drawn in registers and two passes (Omega.G_lo, Omega.G_hi; Omega is exact in TF32), each segment
+ * summed in fp32, and one reduce launch adding the segments in order in fp64 and rounding to fp32 once.  A row's output
+ * is bitwise the same whatever the other rows of the launch and `rows`.  Stream-ordered, sync-free; the segment table
+ * is copied from the host (not CUDA-graph capturable). */
+int rd_grad_projection(const float* G, int32_t rows, int64_t ldg, const int64_t* seg_off, const int64_t* seg_len,
+                       int32_t n_seg, int32_t dim, uint64_t seed, float* out, int64_t ldo, void* scratch, void* stream);
+
 /* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);
@@ -598,6 +619,10 @@ int rd_debug_wgrad_timing(uint64_t* buffer);
  * replay train-mode forward/backward in the oracle with identical masks.  `site` ids in DESIGN.md. */
 int rd_debug_dropout_mask(const uint64_t* rng_captured, uint32_t site, int64_t n, float p, float* out,
                           void* stream);
+
+/* debug: materialise the block out[c * dim + m] = Omega(seed, col0 + c, m) (+1.0f / -1.0f) of rd_grad_projection's
+ * projection, c < n_cols, m < dim, so tests can compare it with a host restatement of the mapping. */
+int rd_debug_projection_signs(uint64_t seed, int64_t col0, int32_t n_cols, int32_t dim, float* out, void* stream);
 
 #ifdef __cplusplus
 }

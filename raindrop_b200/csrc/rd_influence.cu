@@ -16,6 +16,7 @@
 // Every score is the same sequence of products and additions whatever the tile plan, the query blocking or the train
 // chunking, so results are bitwise reproducible across them.
 #include "rd_tc_common.cuh"
+#include "rd_influence.cuh"
 #include "rd_wgmma_tf32.cuh"
 
 namespace rd {
@@ -73,17 +74,14 @@ psg_dot_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_launch_dependents();
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t bar_base = base + (uint32_t)GD_STAGES * GD_STAGE;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (GD_STAGES + s); };
+  const TmaRing<GD_STAGES> ring{base + (uint32_t)GD_STAGES * GD_STAGE};
   const int q_t = blockIdx.x, t_t = blockIdx.y, z = blockIdx.z;
 
   if (warp == 8 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBlo) : "memory");
-    for (int s = 0; s < GD_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    ring.init(8);
   }
   __syncthreads();
   pdl_wait();
@@ -95,16 +93,14 @@ psg_dot_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // ===== TMA producer ==========================================================================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 8 && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+      RingPos<GD_STAGES> p;
       for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1u);
-        mbar_expect_tx(full_bar(stage), GD_STAGE);
+        const int stage = ring.produce(p, GD_STAGE);
         const uint32_t sa = base + (uint32_t)stage * GD_STAGE;
         const int col = (int)(off + (long long)kb * GD_BK);
-        tma_load_2d(&tmA, full_bar(stage), sa, col, t_t * GD_BM);
-        tma_load_2d(&tmB, full_bar(stage), sa + GD_A_TILE, col, q_t * GD_BN);
-        tma_load_2d(&tmBlo, full_bar(stage), sa + GD_A_TILE + GD_B_TILE, col, q_t * GD_BN);
-        if (++stage == GD_STAGES) { stage = 0; phase ^= 1u; }
+        tma_load_2d(&tmA, ring.full(stage), sa, col, t_t * GD_BM);
+        tma_load_2d(&tmB, ring.full(stage), sa + GD_A_TILE, col, q_t * GD_BN);
+        tma_load_2d(&tmBlo, ring.full(stage), sa + GD_A_TILE + GD_B_TILE, col, q_t * GD_BN);
       }
     }
     return;
@@ -114,20 +110,15 @@ psg_dot_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   const int wg = warp >> 2, wq = warp & 3, g = lane >> 2, t = lane & 3;
   const int arow = wg * 64 + wq * 16 + g;
-  int stage = 0, rstage = 0, next = 0; uint32_t phase = 0;
+  RingPos<GD_STAGES> cpos, rpos;
+  int next = 0;
   auto acquire = [&](uint32_t (&ah)[GD_BK / 8][4], uint32_t (&al)[GD_BK / 8][4]) {
-    mbar_wait(full_bar(stage), phase);
-    const uint32_t sa = base + (uint32_t)stage * GD_STAGE;
+    const uint32_t sa = base + (uint32_t)ring.consume(cpos) * GD_STAGE;
     gd_afrag(sa, arow, t, len - next * GD_BK, ah, al);
     ++next;
-    if (++stage == GD_STAGES) { stage = 0; phase ^= 1u; }
     return sa + (uint32_t)GD_A_TILE;
   };
-  auto release = [&]() {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(empty_bar(rstage));
-    if (++rstage == GD_STAGES) rstage = 0;
-  };
+  auto release = [&]() { ring.release(rpos, lane); };
   // The tensor cores' fp32 accumulation is not round-to-nearest: summed over thousands of k-steps, same-sign products lose
   // magnitude systematically (measured 4.5e-5 relative at 4,096 columns).  So each k-block's 12 wgmma go to fresh
   // accumulators (k-blocks alternate between a0 and a1), and the k-block sums are added on the CUDA cores, in order.
@@ -201,6 +192,17 @@ DotLayout dot_layout(int Bq, int Bt, int64_t ldg, int n_seg) {
 }
 
 }  // namespace
+
+int grad_lo_image(const float* G, long long n, float* lo, cudaStream_t st) {
+  const long long n4 = n / 4;
+  long long blocks = ceil_div(n4, 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  launch_pdl(psg_lo_kernel, dim3((unsigned)blocks), dim3(256), 0, st, reinterpret_cast<const float4*>(G),
+             reinterpret_cast<float4*>(lo), n4);
+  RD_CHECK_LAUNCH("psg_lo_kernel");
+  return 0;
+}
+
 }  // namespace rd
 
 using namespace rd;
@@ -247,12 +249,7 @@ int rd_per_sample_grad_dot(const float* Gq, int32_t Bq, const float* Gt, int32_t
   if (ce != cudaSuccess) { set_error("%s: segment table copy: %s", fn, cudaGetErrorString(ce)); return -1; }
 
   float* lo = S + l.lo;
-  const long long n4 = (long long)Bq * ldg / 4;
-  long long blocks = ceil_div(n4, 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  launch_pdl(psg_lo_kernel, dim3((unsigned)blocks), dim3(256), 0, st, reinterpret_cast<const float4*>(Gq),
-             reinterpret_cast<float4*>(lo), n4);
-  RD_CHECK_LAUNCH("psg_lo_kernel");
+  RD_TRY(grad_lo_image(Gq, (long long)Bq * ldg, lo, st));
 
   CUtensorMap tmA, tmB, tmBlo;
   {

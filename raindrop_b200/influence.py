@@ -15,9 +15,15 @@ in the layout of TrainStep's flat bucket) and are contracted by rd_per_sample_gr
 segments of at most RD_GRAD_DOT_SEGMENT columns, fp64 across them), so a score is bitwise the same for any chunking.
 The model runs in eval arithmetic; the ob-prop layers run in their error-compensated mode unless the model pins the
 single-pass mode (obprop_mode 1).  One GPU per call.
+
+TracIn-RP (same paper): project() computes a GradientSketch of a data set once, its rows projected onto `dim` random +-1
+directions on the tensor cores (rd_grad_projection, Omega drawn from Philox and never stored); tracin_sketch() scores two
+sketches, an unbiased estimate of tracin's scores whose variance falls as 1 / dim.
 """
 import ctypes as C
+import hashlib
 import math
+from dataclasses import dataclass
 
 import numpy as np
 import torch
@@ -448,3 +454,157 @@ def tracin_from_grads(Gq, Gt, lrs):
     if Gq.ndim != 3 or Gt.ndim != 3 or Gq.shape[0] != Gt.shape[0] or Gq.shape[2] != Gt.shape[2] or lrs.shape != (Gq.shape[0],):
         raise ValueError("Gq [c, q, K], Gt [c, t, K] and lrs [c] do not match: %s, %s, %s" % (Gq.shape, Gt.shape, lrs.shape))
     return np.einsum("c,cqk,ctk->qt", lrs, Gq, Gt)
+
+
+# ---- TracIn-RP: random projections of the gradient rows (Pruthi et al. 2020, section 3.2) ------------------------------
+PROJECTION_DIM_MULTIPLE, PROJECTION_DIM_MAX = 128, 32768
+
+
+@dataclass
+class GradientSketch:
+    """Random projections phi = g Omega / sqrt(dim) of a data set's gradient rows, one block per checkpoint (project).
+    features [n_ckpt, n, dim] float32; E[phi_q . phi_t] = g_q . g_t, with a variance that falls as 1 / dim.  Omega is
+    the +-1 matrix of rd_grad_projection, fixed by `seed`; two sketches score against each other (tracin_sketch) only when
+    dim, seed, fields, layout, lrs and the checkpoints' fingerprints (sha256 of their trained tensors) all agree."""
+    features: torch.Tensor
+    lrs: tuple
+    dim: int
+    seed: int
+    fields: tuple            # None: every trained tensor
+    layout: tuple            # ((state-dict key, shape), ...) of the gradient rows
+    fingerprints: tuple      # sha256 hex digest per checkpoint
+
+    def save(self, path):
+        torch.save(dict(features=self.features.detach().cpu(), lrs=list(self.lrs), dim=self.dim, seed=self.seed,
+                        fields=None if self.fields is None else list(self.fields),
+                        layout=[[k, list(s)] for k, s in self.layout], fingerprints=list(self.fingerprints)), path)
+
+    @classmethod
+    def load(cls, path, map_location=None):
+        d = torch.load(path, map_location=map_location, weights_only=True)
+        return cls(features=d["features"], lrs=tuple(float(x) for x in d["lrs"]), dim=int(d["dim"]), seed=int(d["seed"]),
+                   fields=None if d["fields"] is None else tuple(d["fields"]),
+                   layout=tuple((k, tuple(int(x) for x in s)) for k, s in d["layout"]),
+                   fingerprints=tuple(d["fingerprints"]))
+
+
+def _check_projection(dim, seed):
+    if isinstance(dim, bool) or not isinstance(dim, (int, np.integer)):
+        raise ValueError("dim must be an integer")
+    if dim % PROJECTION_DIM_MULTIPLE or not PROJECTION_DIM_MULTIPLE <= dim <= PROJECTION_DIM_MAX:
+        raise ValueError("dim must be a multiple of %d in [%d, %d], got %d"
+                         % (PROJECTION_DIM_MULTIPLE, PROJECTION_DIM_MULTIPLE, PROJECTION_DIM_MAX, dim))
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 1 << 64:
+        raise ValueError("seed must be an integer in [0, 2**64)")
+
+
+def _fingerprint(params):
+    h = hashlib.sha256()
+    for p in params:
+        h.update(p.detach().to(torch.float32).contiguous().cpu().numpy().tobytes())
+    return h.hexdigest()
+
+
+def project(model, data, checkpoints=None, dim=4096, seed=0, fields=None, internal_batch_size=None):
+    """GradientSketch of `data` (tracin's train argument, or a query dict whose y is None: the predicted class): the
+    gradient rows of every sample at every checkpoint, projected onto `dim` random +-1 directions by rd_grad_projection
+    (wgmma TF32 with Omega drawn in registers; fp32 within segments, fp64 across them).  The rows are computed as for
+    tracin (eval arithmetic, ob-prop auto pinned to the error-compensated mode) chunk by chunk, and the full rows of the
+    set are never held.  checkpoints, fields: as for tracin.  internal_batch_size: rows per chunk, rounded up to a
+    multiple of the row batch (default: the largest whose rows and projection scratch fit in 1 GiB).  Features are
+    bitwise the same for any internal_batch_size, data source or run.  The weights, the mode and the dropout counter are
+    restored afterwards."""
+    from .models_rd import _device_of
+    _check_projection(dim, seed)
+    _check_data(model, data, "data", allow_none_y=True)
+    _check_batch_size(internal_batch_size)
+    if model.training:
+        raise ValueError("project runs the model in eval arithmetic: call model.eval() first")
+    dim, seed = int(dim), int(seed)
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    seg_off, seg_len = plan_segments(layout, fields)
+    sel_fields = None if fields is None else tuple(fields)
+    ckpts = _checkpoints(model, checkpoints)
+    dev = _device_of(data["src"]) if isinstance(data, dict) else (data[0] if isinstance(data, tuple) else data).P.device
+    lib = L.load()
+    plan = model._prepare(dev)
+    n, fetch = _source(data, "data")
+    n_seg = len(seg_off)
+    features = torch.zeros(len(ckpts), n, dim, dtype=torch.float32, device=dev)
+    R = _row_batch(lib, plan, ldg)
+    if internal_batch_size is not None:
+        chunk = max(R, (int(internal_batch_size) + R - 1) // R * R)
+    else:
+        chunk = max(R, _largest_chunk(lambda b: 4 * b * ldg + _rows_bytes(lib, plan, min(b, R), ldg) +
+                                      lib.rd_grad_projection_scratch_bytes(b, ldg, dim, n_seg), max(n, 1)) // R * R)
+    offs = (C.c_int64 * n_seg)(*seg_off.tolist())
+    lens = (C.c_int64 * n_seg)(*seg_len.tolist())
+    st = L.stream_ptr(dev)
+    prints = []
+    with torch.no_grad(), _Weights(model) as w:
+        for c, (sd, lr) in enumerate(ckpts):
+            if sd is not None:
+                w.load(sd)
+            prints.append(_fingerprint(w.params))
+            for i0 in range(0, n, chunk):
+                i1 = min(n, i0 + chunk)
+                G = _rows_aligned(model, fetch, i0, i1, R, ldg)
+                nb = lib.rd_grad_projection_scratch_bytes(i1 - i0, ldg, dim, n_seg)
+                sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
+                L.check(lib.rd_grad_projection(G.data_ptr(), i1 - i0, ldg, offs, lens, n_seg, dim, seed,
+                                               features[c, i0:i1].data_ptr(), dim, sc.data_ptr(), st), "rd_grad_projection")
+                del G, sc
+    return GradientSketch(features=features, lrs=tuple(lr for _, lr in ckpts), dim=dim, seed=seed, fields=sel_fields,
+                          layout=tuple((k, tuple(s)) for k, _, s in layout), fingerprints=tuple(prints))
+
+
+def _check_sketches(q, t):
+    for name in ("dim", "seed", "fields", "layout", "lrs", "fingerprints"):
+        a, b = getattr(q, name), getattr(t, name)
+        if a != b:
+            raise ValueError("the sketches differ in %s: %s against %s" % (name, str(a)[:120], str(b)[:120]))
+    if q.features.dim() != 3 or t.features.dim() != 3 or q.features.shape[0] != len(q.lrs) or \
+            t.features.shape[0] != len(t.lrs) or q.features.shape[2] != q.dim or t.features.shape[2] != t.dim:
+        raise ValueError("sketch features must be [n_ckpt, n, dim]: %s, %s"
+                         % (tuple(q.features.shape), tuple(t.features.shape)))
+    if q.features.device != t.features.device:
+        raise ValueError("the sketches are on different devices: %s, %s" % (q.features.device, t.features.device))
+
+
+def tracin_sketch(query_sketch, train_sketch, cap=DEFAULT_SCRATCH_BYTES):
+    """TracIn-RP scores [n_query, n_train] float64 on the device: sum_c lr_c phi_q,c . phi_t,c, through
+    rd_per_sample_grad_dot (ldg = dim, segments of RD_GRAD_DOT_SEGMENT columns), an unbiased estimate of tracin's
+    scores.  Raises ValueError on the host when the sketches do not match (dim, seed, fields, layout, lrs, checkpoint
+    fingerprints)."""
+    _check_sketches(query_sketch, train_sketch)
+    Fq, Ft = query_sketch.features, train_sketch.features
+    nq, nt, dim = Fq.shape[1], Ft.shape[1], query_sketch.dim
+    if Fq.device.type != "cuda":
+        raise L.RaindropB200Error("tracin_sketch runs on a CUDA device; the sketches are on %s" % Fq.device)
+    dev = Fq.device
+    lib = L.load()
+    scores = torch.zeros(nq, nt, dtype=torch.float64, device=dev)
+    if nq == 0 or nt == 0:
+        return scores
+    Fq, Ft = Fq.to(torch.float32).contiguous(), Ft.to(torch.float32).contiguous()
+    seg_off = np.arange(0, dim, SEGMENT, dtype=np.int64)
+    seg_len = np.minimum(SEGMENT, dim - seg_off)
+    n_seg = len(seg_off)
+    offs = (C.c_int64 * n_seg)(*seg_off.tolist())
+    lens = (C.c_int64 * n_seg)(*seg_len.tolist())
+    qb = min(nq, 4096)
+    tc = _largest_chunk(lambda b: lib.rd_per_sample_grad_dot_scratch_bytes(qb, b, dim, n_seg), nt, cap)
+    st = L.stream_ptr(dev)
+    for c, lr in enumerate(query_sketch.lrs):
+        for q0 in range(0, nq, qb):
+            q1 = min(nq, q0 + qb)
+            for t0 in range(0, nt, tc):
+                t1 = min(nt, t0 + tc)
+                nb = lib.rd_per_sample_grad_dot_scratch_bytes(q1 - q0, t1 - t0, dim, n_seg)
+                sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
+                L.check(lib.rd_per_sample_grad_dot(Fq[c, q0].data_ptr(), q1 - q0, Ft[c, t0].data_ptr(), t1 - t0, dim, offs,
+                                                   lens, n_seg, lr, scores.data_ptr() + 8 * (q0 * nt + t0), nt,
+                                                   sc.data_ptr(), st), "rd_per_sample_grad_dot")
+                del sc
+    return scores

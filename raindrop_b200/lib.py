@@ -159,11 +159,15 @@ SIGNATURES = {
     "rd_per_sample_grad_dot": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64), C.c_int32, C.c_double, C.c_void_p, C.c_int64, C.c_void_p,
                                          C.c_void_p]),
+    "rd_grad_projection_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
+    "rd_grad_projection": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                     C.c_int32, C.c_int32, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rd_debug_attention_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_gemm_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_wgrad_timing": (C.c_int, [C.c_void_p]),
     "rd_debug_dropout_mask": (C.c_int, [C.c_void_p, C.c_uint32, C.c_int64, C.c_float, C.c_void_p,
                                         C.c_void_p]),
+    "rd_debug_projection_signs": (C.c_int, [C.c_uint64, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

@@ -8,6 +8,13 @@ paper bound of writing each train row once and reading it once per query block, 
 `--loop` samples and extrapolated to n_train.  The card's name and power limit are printed with the numbers.
 
     python tools/bench_tracin.py --shape P19 --n-query 128 --n-train 31000
+
+--projection DIM times TracIn-RP instead (influence.project / tracin_sketch): the train set's sketch, split into rows
+and the projection launches (CUDA events, in project's chunk plan), the projection kernel's TF32 rate counting both
+passes (2 x 2 x rows x columns x dim) against the 495 TFLOP/s data sheet, the query sketch and scoring times, and the
+whole-set exact time, extrapolated from tracin timed on --exact-train training samples (labelled as extrapolated).
+
+    python tools/bench_tracin.py --shape PAM --n-query 533 --n-train 4266 --projection 4096
 """
 import argparse
 import ctypes as C
@@ -158,13 +165,96 @@ def run(shape, nq, nt, loop_n):
                 one_sample_loop_s_extrapolated=loop, loop_samples_timed=loop_n)
 
 
+def run_projection(shape, nq, nt, dim, exact_nt):
+    cfg = model_config(shape, dropout=0.2)
+    model = build_dropin(cfg, 21)
+    model.eval()
+    dq = to_dev(make_batch(cfg, nq, seed=1))
+    dt = make_batch(cfg, nt, seed=2)
+    ds = DeviceDataset(dt["src"], dt["static"], dt["times"], dt["y"])
+    q = dict(src=dq["src"], static=dq["static"], times=dq["times"], lengths=dq["lengths"], y=None)
+    IF.tracin_sketch(IF.project(model, q, dim=dim), IF.project(model, (ds, torch.arange(min(nt, 64))), dim=dim))  # warm-up
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    st = IF.project(model, ds, dim=dim)
+    torch.cuda.synchronize()
+    t_train = time.perf_counter() - t0
+    t0 = time.perf_counter()
+    sq = IF.project(model, q, dim=dim)
+    torch.cuda.synchronize()
+    t_query = time.perf_counter() - t0
+    t0 = time.perf_counter()
+    S = IF.tracin_sketch(sq, st)
+    torch.cuda.synchronize()
+    t_score = time.perf_counter() - t0
+
+    # the split of the train sketch, with CUDA events, over project's chunk plan
+    lib, plan = L.load(), model._plan
+    layout = IF.grad_layout(model)
+    ldg = IF._bucket_length(layout)
+    off, ln = IF.plan_segments(layout)
+    n_seg = len(off)
+    offs, lens = (C.c_int64 * n_seg)(*off.tolist()), (C.c_int64 * n_seg)(*ln.tolist())
+    R = IF._row_batch(lib, plan, ldg)
+    chunk = max(R, IF._largest_chunk(lambda b: 4 * b * ldg + IF._rows_bytes(lib, plan, min(b, R), ldg) +
+                                     lib.rd_grad_projection_scratch_bytes(b, ldg, dim, n_seg), nt) // R * R)
+    ev = lambda: torch.cuda.Event(enable_timing=True)
+    feats = torch.empty(nt, dim, dtype=torch.float32, device="cuda")
+    idx = torch.arange(nt, device="cuda")
+    st_w = 0 if ds.Pstatic is None else ds.Pstatic.shape[1]
+
+    def fetch(a, b):
+        buf = BatchBuffers(ds.T, b - a, ds.width, st_w)
+        ds.fill(buf, idx[a:b])
+        return buf.src, buf.static, buf.times, buf.lengths, buf.y
+    t_rows = t_proj = 0.0
+    with torch.no_grad():
+        for i0 in range(0, nt, chunk):
+            i1 = min(nt, i0 + chunk)
+            e = [ev() for _ in range(3)]
+            e[0].record()
+            G = IF._rows_aligned(model, fetch, i0, i1, R, ldg)
+            nb = lib.rd_grad_projection_scratch_bytes(i1 - i0, ldg, dim, n_seg)
+            sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device="cuda")
+            e[1].record()
+            L.check(lib.rd_grad_projection(G.data_ptr(), i1 - i0, ldg, offs, lens, n_seg, dim, 0, feats[i0:i1].data_ptr(),
+                                           dim, sc.data_ptr(), L.stream_ptr()), "rd_grad_projection")
+            e[2].record()
+            torch.cuda.synchronize()
+            t_rows += e[0].elapsed_time(e[1]) / 1e3
+            t_proj += e[1].elapsed_time(e[2]) / 1e3
+            del G, sc
+    assert torch.equal(feats, st.features[0]), "the split run must reproduce project bitwise"
+    K = int(ln.sum())
+    proj_flop = 2 * 2.0 * nt * K * dim           # two TF32 passes (Omega.G_lo, Omega.G_hi)
+    # exact TracIn on a subset of the train set, extrapolated linearly in n_train
+    ne = min(nt, exact_nt)
+    IF.tracin(model, q, (ds, torch.arange(min(ne, 64))))
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    IF.tracin(model, q, (ds, torch.arange(ne)))
+    torch.cuda.synchronize()
+    t_exact = (time.perf_counter() - t0) * nt / ne
+    return dict(shape=shape, card=card(), projection_dim=dim, n_query=nq, n_train=nt, bucket=ldg, chunk=chunk,
+                train_sketch_s=t_train, train_sketch_split_s=dict(rows=t_rows, projection=t_proj),
+                projection_tflops_tf32=proj_flop / t_proj / 1e12, projection_tf32_fraction=proj_flop / t_proj / 495e12,
+                query_sketch_s=t_query, scoring_s=t_score, scores_finite=bool(torch.isfinite(S).all()),
+                sketch_total_s=t_train + t_query + t_score, exact_timed_train_samples=ne,
+                exact_s_extrapolated=t_exact, sketch_bytes=4 * (nt + nq) * dim)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shape", default="P19")
     ap.add_argument("--n-query", type=int, default=128)
     ap.add_argument("--n-train", type=int, default=31000)
     ap.add_argument("--loop", type=int, default=64)
+    ap.add_argument("--projection", type=int, help="time TracIn-RP with this many projection dimensions")
+    ap.add_argument("--exact-train", type=int, default=1024, help="--projection: train samples of the timed exact call")
     a = ap.parse_args()
+    if a.projection:
+        print(json.dumps(run_projection(a.shape, a.n_query, a.n_train, a.projection, a.exact_train)), flush=True)
+        return
     print(json.dumps(run(a.shape, a.n_query, a.n_train, a.loop)), flush=True)
 
 

@@ -13,6 +13,11 @@ class.  Files, under --out-dir with suffix _<name>.npy:
   tracin_proponent_scores, tracin_opponents, tracin_opponent_scores: the scores, and the k most negative
   tracin_self_influence_order  int64 [n_train]: training indices by decreasing self-influence (candidate mislabels)
   tracin_self_influence  float64 [n_train]: sum_c lr_c ||g||^2 per training sample
+
+--projection DIM scores through TracIn-RP sketches instead (influence.project / tracin_sketch: each gradient row projected
+onto DIM random +-1 directions fixed by --projection-seed); --save-sketch PATH writes the training set's sketch and
+--load-sketch PATH reuses one (it must match the checkpoints, fields, DIM and seed).  The files are the same; the
+self-influence stays exact.
 """
 import argparse
 import os
@@ -52,15 +57,21 @@ def main():
     ap.add_argument("--n-test", type=int, default=32, help="--synthetic: number of test samples")
     ap.add_argument("--top-k", type=int, default=10)
     ap.add_argument("--fields", nargs="*", help="restrict to these state-dict keys (privacy.sqnorm_fields)")
+    ap.add_argument("--projection", type=int, metavar="DIM", help="score through random-projection sketches of DIM dims")
+    ap.add_argument("--projection-seed", type=int, default=0, help="seed of the projection's +-1 directions")
+    ap.add_argument("--save-sketch", metavar="PATH", help="--projection: write the training set's sketch here")
+    ap.add_argument("--load-sketch", metavar="PATH", help="--projection: reuse this training-set sketch")
     ap.add_argument("--name", help="file name suffix (default: the synthetic configuration or 'dataset')")
     ap.add_argument("--out-dir", default=".")
     args = ap.parse_args()
 
     from raindrop_b200 import data as RD
-    from raindrop_b200.influence import self_influence, tracin
+    from raindrop_b200.influence import GradientSketch, project, self_influence, tracin, tracin_sketch
     from raindrop_b200.synth import make_batch, model_config
     if not torch.cuda.is_available():
         raise SystemExit("tracin runs on a CUDA device")
+    if (args.save_sketch or args.load_sketch) and not args.projection:
+        raise SystemExit("--save-sketch and --load-sketch need --projection")
     lrs = args.lr or [1.0] * len(args.checkpoint)
     if len(lrs) != len(args.checkpoint):
         raise SystemExit("give one --lr per --checkpoint")
@@ -104,7 +115,17 @@ def main():
         test = dict(src=P, static=Ps, times=Pt, lengths=torch.sum(Pt > 0, dim=0), y=None)
         name = args.name or "dataset"
 
-    scores = tracin(model, test, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
+    if args.projection:
+        kw = dict(checkpoints=ckpts, dim=args.projection, seed=args.projection_seed, fields=args.fields)
+        if args.load_sketch:
+            train_sketch = GradientSketch.load(args.load_sketch, map_location=device)
+        else:
+            train_sketch = project(model, train, **kw)
+        if args.save_sketch:
+            train_sketch.save(args.save_sketch)
+        scores = tracin_sketch(project(model, test, **kw), train_sketch).cpu().numpy()
+    else:
+        scores = tracin(model, test, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
     si = self_influence(model, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
     pro, pro_s, opp, opp_s = top_k(scores, args.top_k)
     out = dict(tracin_proponents=pro, tracin_proponent_scores=pro_s, tracin_opponents=opp, tracin_opponent_scores=opp_s,

@@ -602,6 +602,56 @@ size_t rd_grad_projection_scratch_bytes(int32_t rows, int64_t ldg, int32_t dim, 
 int rd_grad_projection(const float* G, int32_t rows, int64_t ldg, const int64_t* seg_off, const int64_t* seg_len,
                        int32_t n_seg, int32_t dim, uint64_t seed, float* out, int64_t ldo, void* scratch, void* stream);
 
+/* ---- EK-FAC influence functions (George et al. 2018; Grosse et al. 2023) ----------------------------------------------
+ * score(q, t) = sum_j G~_q[j] G~_t[j] / (Lambda_j + lambda), G~ = the gradient rows rotated into the Kronecker eigenbasis
+ * of each linear layer's Fisher block A (x) S:  G~_b = Q_S^T G_b Q_A = sum_r (Q_S^T dy_r)(Q_A^T x~_r)^T, x~ = [x | 1].
+ * Blocks, in bucket order: per encoder layer in_proj [3D, D], out_proj [D, D], linear1 [nhid, D], linear2 [D, nhid],
+ * then the lin_value of ob-prop layers 1 and 2 [C, C] ([Nout, Kin] each).  Every block covers its weight and bias.
+ * factors (fp64): per block A [(Kin + 1)^2] then S [Nout^2], row-major, packed (rd_kfac_factors_doubles(dims) in all).
+ * bases (fp32): per block Q_S^T [Nout, Nout] (padded to 4 floats), Q_A[:Kin]^T [Np, Kin] and Q_A[Kin] [Np], Np = Kin + 1
+ * rounded up to 4, rows / entries past Kin + 1 zero (rd_ekfac_bases_floats(dims) in all). */
+int64_t rd_kfac_factors_doubles(const rd_dims* dims);
+int64_t rd_ekfac_bases_floats(const rd_dims* dims);
+/* Scratch of rd_raindrop_v2_kfac_factors: a backward scratch, the fp32 factor sums of every block and their partial
+ * buffers. */
+size_t rd_kfac_factors_scratch_bytes(const rd_dims* dims);
+/* factors += this batch's K-FAC sums, per block A += sum_rows x~ x~^T over [X | 1] and S += sum_rows (B dy)(B dy)^T
+ * (d_logits as rd_raindrop_v2_fwd writes it with labels, the gradient of l_b / B; scaled to l_b as the rows are), over
+ * the rows of each queued item (encoder t*B + b for all T, ob-prop b*N + n).  Runs the data-gradient chain of the backward
+ * (grads == NULL); each item becomes two weight-gradient problems (X, X) and (dY, dY) of the grouped tensor-core launch
+ * (CUDA cores for shapes it does not take), flushed with the phase; one small launch per block then adds the fp32 sums
+ * into the fp64 factors (the last row and column of A from the bias column and the row count).  No atomics: bitwise
+ * reproducible.  The caller divides by the sample count.  Stream-ordered, sync-free. */
+int rd_raindrop_v2_kfac_factors(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
+                                const float* node_scale, const void* workspace, const float* d_logits, void* scratch,
+                                double* factors, void* stream);
+/* Scratch of rd_raindrop_v2_ekfac_rows: a backward scratch, the remainder image of the bases and the rotated operands
+ * of the larger backward phase. */
+size_t rd_ekfac_rows_scratch_bytes(const rd_dims* dims);
+/* As rd_raindrop_v2_per_sample_grads, but the linear layers' fields hold the rotated G~_b: each queued item's operands
+ * are first rotated, Y^ = dY Q_S and X^ = [X | 1] Q_A (the error-compensated tensor-core GEMM of rd_linear_fwd, the
+ * last row of Q_A as its bias), and sample b's tile Y^_b^T X^_b goes to the weight field (columns < Kin) and the bias
+ * field (column Kin).  LayerNorm and head fields are the plain gradient (identity basis).  bases: 16-byte aligned. */
+int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
+                              const float* node_scale, const void* workspace, const float* d_logits, const float* bases,
+                              void* scratch, float* G, int64_t ldg, void* stream);
+/* lam[j] += sum_{r < rows} G[r * ldg + j]^2 (fp64, rows in order, one thread per column, no atomics) for the columns of
+ * the segments (host arrays; segments separated by bucket padding only are launched as one run). */
+int rd_ekfac_accumulate_sq(const float* G, int32_t rows, int64_t ldg, const int64_t* seg_off, const int64_t* seg_len,
+                           int32_t n_seg, double* lam, void* stream);
+/* G[r * ldg + j] *= w[j] (fp32) for r < rows and the columns of the segments. */
+int rd_ekfac_scale_rows(float* G, int32_t rows, int64_t ldg, const int64_t* seg_off, const int64_t* seg_len,
+                        int32_t n_seg, const float* w, void* stream);
+/* Labels of the true Fisher: y[b] = the first class c with u_b sum_c' p_c' < sum_{c'' <= c} p_c'' (fp64, p_c =
+ * exp(logits[b, c] - max_c logits[b, c]), classes in order; the last class if none), u_b = U(seed, index0 + b).
+ * U(seed, i) = ((w0 >> 5) 2^26 + (w1 >> 6)) / 2^53 with (w0, w1, w2, w3) = Philox4x32-10 with key (seed & 0xffffffff,
+ * seed >> 32) and counter (i & 0xffffffff, i >> 32, 97, 0): site 97, past the dropout sites 1-96.  A sample's label
+ * depends on (seed, its global index, its logits) alone. */
+int rd_fisher_labels(const float* logits, int32_t B, int32_t n_classes, uint64_t seed, uint64_t index0, int64_t* y,
+                     void* stream);
+/* debug: out[i] = U(seed, index0 + i) (fp64, device) for i < n. */
+int rd_debug_fisher_uniforms(uint64_t seed, uint64_t index0, int32_t n, double* out, void* stream);
+
 /* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);

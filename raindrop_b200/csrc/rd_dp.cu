@@ -311,7 +311,9 @@ __global__ void __launch_bounds__(DP_THREADS) dp_noise_kernel(float* __restrict_
 
 // ---- per-sample gradients, materialised ---------------------------------------------------------------------------
 // The explicit form of dp_norm_tile_kernel, written out instead of squared: tile (m0, n0) of sample b's [Nout, Kin + 1]
-// product dY_b^T [X_b | 1], 16-row fp32 slices summed in fp64, each value scaled and rounded to fp32 once.
+// product dY_b^T [X_b | 1], 16-row fp32 slices summed in fp64, each value scaled and rounded to fp32 once.  kRotated
+// (EK-FAC rows): X already holds Kin + 1 columns (the rotated [X | 1] Q_A), so no ones column is appended.
+template <bool kRotated>
 __global__ void __launch_bounds__(DP_THREADS) psg_tile_kernel(const __grid_constant__ PsgGroup g, float* __restrict__ G,
                                                               long long ldg, float scale) {
   pdl_launch_dependents();
@@ -336,7 +338,8 @@ __global__ void __launch_bounds__(DP_THREADS) psg_tile_kernel(const __grid_const
   for (int r0 = 0; r0 < o.R; r0 += DP_BK) {
     __syncthreads();
     load_cols(As, Yb, ys, r0, o.R, m0, o.Nout, -1);
-    load_cols(Bs, Xb, xs, r0, o.R, n0, o.Kin, o.Kin);
+    if (kRotated) load_cols(Bs, Xb, xs, r0, o.R, n0, o.Kin + 1, -1);
+    else load_cols(Bs, Xb, xs, r0, o.R, n0, o.Kin, o.Kin);
     __syncthreads();
     mma_slice(As, Bs, e);
   }
@@ -425,12 +428,13 @@ int psg_tiles(int Nout, int Kin, int* tn) {
   return (int)ceil_div(Nout, DP_TILE) * *tn;
 }
 
-int psg_group(const PsgGroup& g, int B, float* G, long long ldg, float scale, cudaStream_t st) {
+int psg_group(const PsgGroup& g, int B, float* G, long long ldg, float scale, cudaStream_t st, bool rotated) {
   if (g.n == 0) return 0;
   const PsgItem& last = g.it[g.n - 1];
   const long long blocks = last.blk0 + (long long)B * last.ntiles;
   if (blocks > 0x7FFFFFFFLL) { set_error("psg_group: %lld tiles, too many for one launch", blocks); return -2; }
-  launch_pdl(psg_tile_kernel, dim3((unsigned)blocks), dim3(DP_THREADS), 0, st, g, G, ldg, scale);
+  if (rotated) launch_pdl(psg_tile_kernel<true>, dim3((unsigned)blocks), dim3(DP_THREADS), 0, st, g, G, ldg, scale);
+  else launch_pdl(psg_tile_kernel<false>, dim3((unsigned)blocks), dim3(DP_THREADS), 0, st, g, G, ldg, scale);
   RD_CHECK_LAUNCH("psg_tile_kernel");
   return 0;
 }

@@ -217,7 +217,8 @@ struct PsgItem {
 };
 struct PsgGroup { PsgItem it[DP_MAX_ITEMS]; int n; };
 int psg_tiles(int Nout, int Kin, int* tn);
-int psg_group(const PsgGroup& g, int B, float* G, long long ldg, float scale, cudaStream_t st);
+// rotated (EK-FAC): X holds Kin + 1 columns of [X | 1] Q_A (ldx >= Kin + 1) and no ones column is appended
+int psg_group(const PsgGroup& g, int B, float* G, long long ldg, float scale, cudaStream_t st, bool rotated = false);
 // LayerNorm gamma -> G[b, gw + d], beta -> G[b, gb + d] (sums over the rows t*B + b, t < T)
 int psg_ln(const float* x, const float* stats, const float* dy, int T, int B, int D, float* G, long long ldg, long long gw,
            long long gb, float scale, cudaStream_t st);
@@ -225,6 +226,9 @@ int psg_ln(const float* x, const float* stats, const float* dy, int T, int B, in
 int psg_head(int B, int D, int Df, int ds, int ncls, const float* dlogits, const float* hpre, const float* dh, const float* feat,
              const float* dfeat, const float* statics, float* G, long long ldg, const long long* off, float scale,
              cudaStream_t st);
+// EK-FAC factors (rd_ekfac.cu): A [(Kin + 1)^2] += [[Aw, Ab], [Ab^T, rows]], S [Nout^2] += sscale * Sw (fp64)
+int kfac_accumulate(const float* Aw, const float* Ab, const float* Sw, int Kin, int Nout, long long rows, double sscale,
+                    double* A, double* S, cudaStream_t st);
 // zeroes G[b, off[f] + numel[f] .. next field's offset) and the tail up to ldg: the bucket's padding columns
 int psg_pad(const DpFields& fields, int B, float* G, long long ldg, cudaStream_t st);
 

@@ -14,6 +14,7 @@
 #include "rd_tc_gemm.cuh"
 
 namespace rd {
+int grad_lo_image(const float* G, long long n, float* lo, cudaStream_t st);     // rd_influence.cu
 namespace {
 
 struct Shape {
@@ -180,10 +181,44 @@ int64_t bucket_fields(const Shape& s, DpFields* f) {
   return off;
 }
 
+// EK-FAC blocks: one per queued linear layer, in bucket order (per encoder layer in_proj, out_proj, linear1, linear2;
+// then lin_value of ob-prop layers 1 and 2).  a, s: offsets (doubles) of A [(Kin + 1)^2] and S [Nout^2] in the caller's
+// factors; qs, qa, qb: offsets (floats) of Q_S^T [Nout, Nout], Q_A[:Kin]^T [Np, Kin] and Q_A[Kin] [Np] in the caller's
+// bases, Np = Kin + 1 rounded up to 4 (rows past Kin + 1 are 0); each piece starts 4-aligned.
+struct KfacBlock { int Nout, Kin, Np; int64_t a, s, qs, qa, qb; };
+struct KfacBlocks { KfacBlock b[4 * RD_MAX_LAYERS + 2]; int n; int64_t factor_doubles, base_floats; };
+KfacBlocks kfac_blocks(const Shape& s) {
+  KfacBlocks k;
+  k.n = 0;
+  int64_t a = 0, q = 0;
+  auto add = [&](int Nout, int Kin) {
+    KfacBlock& o = k.b[k.n++];
+    o.Nout = Nout; o.Kin = Kin; o.Np = (int)round_up(Kin + 1, 4);
+    o.a = a; a += (int64_t)(Kin + 1) * (Kin + 1);
+    o.s = a; a += (int64_t)Nout * Nout;
+    o.qs = q; q += round_up((int64_t)Nout * Nout, 4);
+    o.qa = q; q += (int64_t)o.Np * Kin;
+    o.qb = q; q += o.Np;
+  };
+  for (int l = 0; l < s.L; ++l) { add(3 * s.D, s.D); add(s.D, s.D); add(s.nhid, s.D); add(s.D, s.nhid); }
+  add(s.C, s.C); add(s.C, s.C);
+  k.factor_doubles = a; k.base_floats = q;
+  return k;
+}
+// the block of the weight field fw (a queued item's)
+int kfac_block_of(const Shape& s, int fw) {
+  const int f = fw - dp_head_fields(s);
+  return f < 12 * s.L ? 4 * (f / 12) + (f % 12) / 2 : 4 * s.L + (f - 12 * s.L) / 2;
+}
+
 // Per-sample items of one backward phase, queued where the training path queues the weight-gradient items of the same
-// (dY, X) pairs, and flushed as one group launch.  Two modes: squared norms into `sqnorms` (dp_norm_group; the partial
-// sums of a phase start at `partial` again: the previous phase's launches have completed by then, stream order), or,
-// with G set, the per-sample gradient rows themselves (psg_group), scaled by `scale`.
+// (dY, X) pairs, and flushed as one group launch.  Modes: squared norms into `sqnorms` (dp_norm_group; the partial
+// sums of a phase start at `partial` again: the previous phase's launches have completed by then, stream order); with
+// G set, the per-sample gradient rows themselves (psg_group), scaled by `scale`, and with `bases` also set, the EK-FAC
+// rows: each item's operands rotated into `rot` first (kfac_flush); with `factors` set, the EK-FAC factor sums of
+// every item (kfac_flush).
+struct DpQueue;
+int kfac_flush(DpQueue& q, cudaStream_t st);
 struct DpQueue {
   DpNormGroup g;
   PsgGroup pg;
@@ -191,13 +226,17 @@ struct DpQueue {
   int B = 0, nf = 0;
   double* sqnorms = nullptr; double* partial = nullptr;
   float* G = nullptr; long long ldg = 0; float scale = 1.f; DpFields fields;     // rows mode
+  const Shape* shape = nullptr; const KfacBlocks* kb = nullptr; int blk_of[DP_MAX_ITEMS];   // EK-FAC modes
+  const float* bases = nullptr; const float* bases_lo = nullptr; float* rot = nullptr;     // rotated rows
+  double* factors = nullptr; float* kws = nullptr; float* kpartial = nullptr;             // factors
   DpQueue() { g.n = 0; pg.n = 0; }
   void add(const float* Y, int64_t ldy, const float* X, int64_t ldx, int Nout, int Kin, int R, int64_t sstride,
            int64_t rstride, int fw) {
-    if (G) {
+    if (G || factors) {
+      if (kb) blk_of[pg.n] = kfac_block_of(*shape, fw);
       PsgItem& o = pg.it[pg.n++];
       o.Y = Y; o.X = X; o.ldy = ldy; o.ldx = ldx; o.sstride = sstride; o.rstride = rstride; o.blk0 = blk;
-      o.gw = fields.off[fw]; o.gb = fields.off[fw + 1];
+      o.gw = G ? fields.off[fw] : 0; o.gb = G ? fields.off[fw + 1] : 0;
       o.Nout = Nout; o.Kin = Kin; o.R = R; o.ntiles = psg_tiles(Nout, Kin, &o.tn);
       blk += (long long)B * o.ntiles;
       return;
@@ -210,16 +249,18 @@ struct DpQueue {
     blk += (long long)B * o.ntiles;
   }
   int ln(const float* x, const float* stats, const float* dy, int T, int D, int fw, int fb, cudaStream_t st) {
+    if (factors) return 0;
     if (G) return psg_ln(x, stats, dy, T, B, D, G, ldg, fields.off[fw], fields.off[fb], scale, st);
     return dp_ln_sqnorm(x, stats, dy, T, B, D, sqnorms, nf, fw, fb, st);
   }
   int head(const Shape& s, const float* dlogits, const float* hpre, const float* dh, const float* feat, const float* dfeat,
            const float* statics, cudaStream_t st) {
+    if (factors) return 0;
     if (G) return psg_head(B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dh, feat, dfeat, statics, G, ldg, fields.off, scale, st);
     return dp_head_sqnorm(B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dh, feat, dfeat, statics, sqnorms, nf, st);
   }
   int flush(cudaStream_t st) {
-    int rc = G ? psg_group(pg, B, G, ldg, scale, st) : dp_norm_group(g, B, partial, sqnorms, nf, st);
+    int rc = kb ? kfac_flush(*this, st) : G ? psg_group(pg, B, G, ldg, scale, st) : dp_norm_group(g, B, partial, sqnorms, nf, st);
     g.n = 0; pg.n = 0; blk = 0;
     return rc;
   }
@@ -438,6 +479,105 @@ static bool linear_nt_is_tc(const GemmP& g, const float* W_lo) {
   a.drop_p = g.drop_p; a.rng = g.rng; a.drop_site = g.drop_site; a.resid = g.resid; a.resid_ld = g.resid_ld;
   return W_lo && tc_gemm_supported(a);
 }
+
+// ---- EK-FAC: the factor pass and the rotated rows (DpQueue's kfac modes) ------------------------------------------
+namespace {
+// Factors: per item, dW = X^T X with db = column sums of X, and dW = dY^T dY (tn: queued for one grouped tensor-core
+// launch when the shape fits, else CUDA cores), then each block's sums are added into the fp64 factors (dY carries
+// the gradient of l_b / B, so S is scaled by B^2).  Rotated rows: Y^ = dY Q_S and X^ = [X | 1] Q_A on the error-compensated
+// tensor-core GEMM (linear_nt, bias = the last row of Q_A), then psg_group on the rotated operands without a ones column.
+int kfac_flush(DpQueue& q, cudaStream_t st) {
+  if (q.pg.n == 0) return 0;
+  const KfacBlocks& K = *q.kb;
+  if (q.factors) {
+    WgradQueue wq;
+    int64_t off = 0;
+    float* ws = q.kws;
+    const float* Aw[DP_MAX_ITEMS]; const float* Ab[DP_MAX_ITEMS]; const float* Sw[DP_MAX_ITEMS];
+    for (int i = 0; i < q.pg.n; ++i) {
+      const PsgItem& o = q.pg.it[i];
+      const int64_t rows = (int64_t)q.B * o.R;
+      float* aw = ws + off; off += round_up((int64_t)o.Kin * o.Kin, 64);
+      float* ab = ws + off; off += round_up(o.Kin, 64);
+      float* sw = ws + off; off += round_up((int64_t)o.Nout * o.Nout, 64);
+      float* sb = ws + off; off += round_up(o.Nout, 64);
+      float* pa = ws + off; off += round_up(tc_wgrad_partial_floats(o.Kin, o.Kin, rows), 64);
+      float* ps = ws + off; off += round_up(tc_wgrad_partial_floats(o.Nout, o.Nout, rows), 64);
+      RD_TRY(tn(&wq, o.X, o.ldx, o.X, o.ldx, aw, ab, o.Kin, o.Kin, rows, pa, q.kpartial, st));
+      RD_TRY(tn(&wq, o.Y, o.ldy, o.Y, o.ldy, sw, sb, o.Nout, o.Nout, rows, ps, q.kpartial, st));
+      Aw[i] = aw; Ab[i] = ab; Sw[i] = sw;
+    }
+    RD_TRY(wq.flush(st));
+    for (int i = 0; i < q.pg.n; ++i) {
+      const PsgItem& o = q.pg.it[i];
+      const KfacBlock& b = K.b[q.blk_of[i]];
+      RD_TRY(kfac_accumulate(Aw[i], Ab[i], Sw[i], o.Kin, o.Nout, (long long)q.B * o.R, (double)q.B * (double)q.B,
+                             q.factors + b.a, q.factors + b.s, st));
+    }
+    return 0;
+  }
+  int64_t off = 0;
+  for (int i = 0; i < q.pg.n; ++i) {
+    PsgItem& o = q.pg.it[i];
+    const KfacBlock& b = K.b[q.blk_of[i]];
+    const int64_t rows = (int64_t)q.B * o.R;
+    float* yh = q.rot + off; off += round_up(rows * o.Nout, 64);
+    float* xh = q.rot + off; off += round_up(rows * b.Np, 64);
+    RD_TRY(linear_nt(nt(o.Y, o.ldy, q.bases + b.qs, o.Nout, yh, o.Nout, rows, o.Nout, o.Nout), q.bases_lo + b.qs, st));
+    GemmP g = nt(o.X, o.ldx, q.bases + b.qa, o.Kin, xh, b.Np, rows, b.Np, o.Kin);
+    g.bias = q.bases + b.qb;
+    RD_TRY(linear_nt(g, q.bases_lo + b.qa, st));
+    o.Y = yh; o.ldy = o.Nout; o.X = xh; o.ldx = b.Np;
+  }
+  return psg_group(q.pg, q.B, q.G, q.ldg, q.scale, st, true);
+}
+
+// Scratch of the factor pass: the backward scratch, then per block the fp32 sums X^T X, x, dY^T dY, dY colsums and two
+// tensor-core partial buffers (kfac_flush lays a phase's items out from the start of that region, in queue order), and
+// the CUDA-core fallback's split-K partial buffer.
+struct KfacLayout { int64_t bw, kws, kpartial, total; };
+KfacLayout kfac_layout(const Shape& s) {
+  KfacLayout l;
+  Arena a;
+  l.bw = a.take(bw_layout(s).total);
+  const KfacBlocks K = kfac_blocks(s);
+  int64_t ws = 0, pf = 0;
+  for (int i = 0; i < K.n; ++i) {
+    const KfacBlock& b = K.b[i];
+    const int64_t rows = i < 4 * s.L ? s.M2 : s.M1;
+    ws += round_up((int64_t)b.Kin * b.Kin, 64) + round_up(b.Kin, 64) + round_up((int64_t)b.Nout * b.Nout, 64) +
+          round_up(b.Nout, 64) + round_up(tc_wgrad_partial_floats(b.Kin, b.Kin, rows), 64) +
+          round_up(tc_wgrad_partial_floats(b.Nout, b.Nout, rows), 64);
+    const int64_t p1 = splitk_partial_floats(b.Kin, b.Kin, rows), p2 = splitk_partial_floats(b.Nout, b.Nout, rows);
+    if (p1 > pf) pf = p1;
+    if (p2 > pf) pf = p2;
+  }
+  l.kws = a.take(ws);
+  l.kpartial = a.take(pf);
+  l.total = a.off;
+  return l;
+}
+
+// Scratch of the rotated rows: the backward scratch, the remainder image of the bases, and the rotated operands of the
+// larger phase (every item of a phase is resident until its group launch).
+struct EkfacLayout { int64_t bw, lo, rot, total; };
+EkfacLayout ekfac_layout(const Shape& s) {
+  EkfacLayout l;
+  Arena a;
+  l.bw = a.take(bw_layout(s).total);
+  const KfacBlocks K = kfac_blocks(s);
+  l.lo = a.take(K.base_floats);
+  int64_t enc = 0, ob = 0;
+  for (int i = 0; i < K.n; ++i) {
+    const KfacBlock& b = K.b[i];
+    const int64_t rows = i < 4 * s.L ? s.M2 : s.M1;
+    (i < 4 * s.L ? enc : ob) += round_up(rows * b.Nout, 64) + round_up(rows * b.Np, 64);
+  }
+  l.rot = a.take(enc > ob ? enc : ob);
+  l.total = a.off;
+  return l;
+}
+}  // namespace
 
 // ---- observation propagation layer (operator level) ---------------------------------------------
 // Forward goes to the tensor-core kernel when the shape fits its tiling, otherwise to the generic
@@ -1382,6 +1522,84 @@ int rd_raindrop_v2_per_sample_grads(const rd_dims* dims, const rd_params* params
   cudaStream_t st = (cudaStream_t)stream;
   RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
   return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, (float*)scratch,
+                      RD_BWD_ALL, nullptr, st, &q);
+}
+
+int64_t rd_kfac_factors_doubles(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return kfac_blocks(s).factor_doubles;
+}
+
+int64_t rd_ekfac_bases_floats(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return kfac_blocks(s).base_floats;
+}
+
+size_t rd_kfac_factors_scratch_bytes(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return (size_t)kfac_layout(s).total * sizeof(float);
+}
+
+int rd_raindrop_v2_kfac_factors(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
+                                const float* node_scale, const void* workspace, const float* d_logits, void* scratch,
+                                double* factors, void* stream) {
+  const char* fn = "rd_raindrop_v2_kfac_factors";
+  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch || !factors) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  if (reinterpret_cast<uintptr_t>(scratch) & 15) { set_error("%s: scratch must be 16-byte aligned", fn); return -2; }
+  const KfacBlocks K = kfac_blocks(s);
+  const KfacLayout l = kfac_layout(s);
+  DpQueue q;
+  q.B = s.B; q.shape = &s; q.kb = &K; q.factors = factors;
+  q.kws = (float*)scratch + l.kws; q.kpartial = (float*)scratch + l.kpartial;
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr,
+                      (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, &q);
+}
+
+size_t rd_ekfac_rows_scratch_bytes(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0) return 0;
+  return (size_t)ekfac_layout(s).total * sizeof(float);
+}
+
+int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
+                              const float* node_scale, const void* workspace, const float* d_logits, const float* bases,
+                              void* scratch, float* G, int64_t ldg, void* stream) {
+  const char* fn = "rd_raindrop_v2_ekfac_rows";
+  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !bases || !scratch || !G) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  DpQueue q;
+  const int64_t bucket = bucket_fields(s, &q.fields);
+  if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
+  if ((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(bases) | reinterpret_cast<uintptr_t>(scratch)) & 15) {
+    set_error("%s: G, bases and scratch must be 16-byte aligned", fn);
+    return -2;
+  }
+  const KfacBlocks K = kfac_blocks(s);
+  const EkfacLayout l = ekfac_layout(s);
+  float* S = (float*)scratch;
+  q.B = s.B; q.nf = q.fields.n; q.G = G; q.ldg = ldg;
+  q.scale = (float)s.B;      // as rd_raindrop_v2_per_sample_grads: rows are of l_b
+  q.shape = &s; q.kb = &K; q.bases = bases; q.bases_lo = S + l.lo; q.rot = S + l.rot;
+  cudaStream_t st = (cudaStream_t)stream;
+  RD_TRY(grad_lo_image(bases, K.base_floats, S + l.lo, st));
+  RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, S + l.bw,
                       RD_BWD_ALL, nullptr, st, &q);
 }
 

@@ -19,6 +19,10 @@ single-pass mode (obprop_mode 1).  One GPU per call.
 TracIn-RP (same paper): project() computes a GradientSketch of a data set once, its rows projected onto `dim` random +-1
 directions on the tensor cores (rd_grad_projection, Omega drawn from Philox and never stored); tracin_sketch() scores two
 sketches, an unbiased estimate of tracin's scores whose variance falls as 1 / dim.
+
+EK-FAC influence functions (George et al. 2018; Grosse et al. 2023): ekfac_factors() computes the Kronecker-factored
+Fisher of every encoder and ob-prop linear layer and its eigenbases once; ekfac_influence() scores
+g_q^T (F + lambda I)^-1 g_t with the rows rotated into those bases on the device (rd_raindrop_v2_ekfac_rows).
 """
 import ctypes as C
 import hashlib
@@ -608,3 +612,449 @@ def tracin_sketch(query_sketch, train_sketch, cap=DEFAULT_SCRATCH_BYTES):
                                                    sc.data_ptr(), st), "rd_per_sample_grad_dot")
                 del sc
     return scores
+
+
+# ---- EK-FAC influence functions (George et al. 2018; Grosse et al. 2023) -----------------------------------------------
+FISHER_MODES = ("true", "empirical")
+EKFAC_DAMPING_FACTOR = 0.1       # damping=None: lambda_f = 0.1 * mean(Lambda) over each block or diagonal field
+
+
+def kfac_blocks(model):
+    """[(weight key, bias key, Nout, Kin)] of the Kronecker-factored blocks, in bucket order: per encoder layer in_proj,
+    out_proj, linear1, linear2, then the lin_value of ob-prop layers 1 and 2 (the linear layers whose per-sample tiles the
+    backward writes).  Every other trained tensor (LayerNorm gamma / beta, the head) is a diagonal field."""
+    return _blocks_of_layout(tuple((k, tuple(s)) for k, _, s in grad_layout(model)))
+
+
+def _check_block_fields(model, fields):
+    """Selected keys; a linear weight without its bias (or the reverse) is refused: a block covers both."""
+    sel = _selected(grad_layout(model), fields)
+    for w, b, _, _ in kfac_blocks(model):
+        if (w in sel) != (b in sel):
+            raise ValueError("EK-FAC blocks cover a linear layer's weight and bias together: select both %s and %s, or "
+                             "neither" % (w, b))
+    return sel
+
+
+def _check_fisher(fisher, seed):
+    if fisher not in FISHER_MODES:
+        raise ValueError("fisher must be one of %s, got %r" % (FISHER_MODES, fisher))
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 1 << 64:
+        raise ValueError("seed must be an integer in [0, 2**64)")
+
+
+def _check_damping(damping):
+    if damping is None:
+        return None
+    if isinstance(damping, bool) or not isinstance(damping, (int, float, np.floating, np.integer)):
+        raise ValueError("damping must be None or a positive float")
+    d = float(damping)
+    if not (math.isfinite(d) and d > 0):
+        raise ValueError("damping must be None or a finite float > 0, got %r" % damping)
+    return d
+
+
+def _backward(model, src, static, times, lengths, y, kind, ldg=None, out=None, bases=None, fisher_seed=None, index0=0):
+    """One eval forward and data-gradient backward of a row batch.  y None: labels drawn from the softmax
+    (rd_fisher_labels, global indices index0..) when fisher_seed is set, else the predicted class.  kind "factors": adds
+    the K-FAC sums into `out` (fp64); "rows": returns [B, ldg] EK-FAC rows rotated by `bases` (fp32 on the device)."""
+    cl = _Call(model, src, static, times, lengths, None, False)
+    lib, plan, dev = cl.lib, cl.plan, cl.device
+    B = cl.x.shape[1]
+    dims = _dims(plan, B)
+    key = (B, dims.obprop_mode, dev.index)
+    ws = cl.scratch("_psg_workspace", key, lib.rd_workspace_bytes(C.byref(dims)))
+    f32 = dict(device=dev, dtype=torch.float32)
+    logits, dlog, loss = torch.empty(B, plan.n_classes, **f32), torch.empty(B, plan.n_classes, **f32), torch.empty(1, **f32)
+    st = L.stream_ptr(dev)
+
+    def fwd(yv):
+        L.check(lib.rd_raindrop_v2_fwd(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st), cl.tm.data_ptr(),
+                                       cl.ln.data_ptr(), plan.node_scale.data_ptr(), L.ptr(plan.rng_state), ws.data_ptr(),
+                                       logits.data_ptr(), L.ptr(yv), L.ptr(None if yv is None else loss),
+                                       L.ptr(None if yv is None else dlog), st), "rd_raindrop_v2_fwd")
+
+    if y is None:
+        fwd(None)
+        if fisher_seed is None:
+            y = logits.argmax(dim=1)
+        else:
+            y = torch.empty(B, dtype=torch.int64, device=dev)
+            L.check(lib.rd_fisher_labels(logits.data_ptr(), B, plan.n_classes, fisher_seed, index0, y.data_ptr(), st),
+                    "rd_fisher_labels")
+    fwd(y.to(device=dev, dtype=torch.int64).contiguous())
+    if kind == "factors":
+        scratch = cl.scratch("_kfac_scratch", key, lib.rd_kfac_factors_scratch_bytes(C.byref(dims)))
+        L.check(lib.rd_raindrop_v2_kfac_factors(C.byref(dims), C.byref(cl.params), L.ptr(cl.st), cl.ln.data_ptr(),
+                                                plan.node_scale.data_ptr(), ws.data_ptr(), dlog.data_ptr(),
+                                                scratch.data_ptr(), out.data_ptr(), st), "rd_raindrop_v2_kfac_factors")
+        return None
+    G = torch.empty(B, ldg, **f32)
+    scratch = cl.scratch("_ekfac_scratch", key, lib.rd_ekfac_rows_scratch_bytes(C.byref(dims)))
+    L.check(lib.rd_raindrop_v2_ekfac_rows(C.byref(dims), C.byref(cl.params), L.ptr(cl.st), cl.ln.data_ptr(),
+                                          plan.node_scale.data_ptr(), ws.data_ptr(), dlog.data_ptr(), bases.data_ptr(),
+                                          scratch.data_ptr(), G.data_ptr(), ldg, st), "rd_raindrop_v2_ekfac_rows")
+    return G
+
+
+def _ekfac_rows_aligned(model, fetch, i0, i1, R, ldg, bases, fisher_seed=None):
+    """EK-FAC rows of samples [i0, i1) (i0 a multiple of R), computed in batches [k R, (k + 1) R) as tracin's rows."""
+    G = None
+    for s0 in range(i0, i1, R):
+        s1 = min(i1, s0 + R)
+        src, static, times, lengths, y = fetch(s0, s1)
+        g = _backward(model, src, static, times, lengths, None if fisher_seed is not None else y, "rows", ldg=ldg,
+                      bases=bases, fisher_seed=fisher_seed, index0=s0)
+        if G is None:
+            if s1 == i1:
+                return g
+            G = torch.empty(i1 - i0, ldg, dtype=torch.float32, device=g.device)
+        G[s0 - i0:s1 - i0] = g
+        del g
+    return G
+
+
+def _factor_offsets(blocks):
+    """[(a, s)] offsets (doubles) of each block's A and S in the packed factors (include/raindrop_b200.h)."""
+    out, off = [], 0
+    for _, _, nout, kin in blocks:
+        out.append((off, off + (kin + 1) ** 2))
+        off += (kin + 1) ** 2 + nout * nout
+    return out, off
+
+
+def _flat_bases(blocks, bases):
+    """fp32 [rd_ekfac_bases_floats] on the host: per block Q_S^T [Nout, Nout] (padded to 4 floats), Q_A[:Kin]^T [Np, Kin]
+    and Q_A[Kin] [Np], Np = Kin + 1 rounded up to 4 (zero past Kin + 1)."""
+    parts = []
+    for (_, _, nout, kin), (QA, QS) in zip(blocks, bases):
+        npad = (kin + 4) // 4 * 4
+        qs = torch.zeros((nout * nout + 3) // 4 * 4, dtype=torch.float64)
+        qs[:nout * nout] = torch.as_tensor(QS).T.reshape(-1)
+        qa = torch.zeros(npad, kin, dtype=torch.float64)
+        qa[:kin + 1] = torch.as_tensor(QA)[:kin].T
+        qb = torch.zeros(npad, dtype=torch.float64)
+        qb[:kin + 1] = torch.as_tensor(QA)[kin]
+        parts += [qs, qa.reshape(-1), qb]
+    return torch.cat(parts).to(torch.float32)
+
+
+def _eigh(M):
+    """float64 eigendecomposition (ascending) with each eigenvector's largest-magnitude component made positive (the
+    first such component on ties), so the basis is reproducible."""
+    M = np.asarray(M, dtype=np.float64)
+    w, Q = np.linalg.eigh(0.5 * (M + M.T))
+    i = np.argmax(np.abs(Q), axis=0)
+    sign = np.where(Q[i, np.arange(Q.shape[1])] < 0, -1.0, 1.0)
+    return w, Q * sign
+
+
+@dataclass
+class EKFACFactors:
+    """EK-FAC factors of one model's current weights (ekfac_factors): per Kronecker block (kfac_blocks) the float64 bases
+    (Q_A [Kin + 1, Kin + 1], Q_S [Nout, Nout]), the corrected eigenvalues Lambda [bucket] float64 in the bucket layout
+    (Lambda_j = (1/n) sum_b G~_bj^2; 0 outside the selected fields), n, fisher, seed, fields, layout and the sha256
+    fingerprint of the trained tensors.  bases_flat: the fp32 bases as rd_raindrop_v2_ekfac_rows takes them."""
+    bases: tuple             # ((Q_A, Q_S) float64 numpy per block)
+    bases_flat: torch.Tensor
+    eigenvalues: torch.Tensor
+    n: int
+    fisher: str
+    seed: int
+    fields: tuple            # None: every trained tensor
+    layout: tuple            # ((state-dict key, shape), ...) of the gradient rows
+    fingerprint: str
+
+    def save(self, path):
+        torch.save(dict(bases=[[torch.from_numpy(np.ascontiguousarray(a)), torch.from_numpy(np.ascontiguousarray(s))]
+                               for a, s in self.bases],
+                        bases_flat=self.bases_flat.detach().cpu(), eigenvalues=self.eigenvalues.detach().cpu(), n=self.n,
+                        fisher=self.fisher, seed=self.seed, fields=None if self.fields is None else list(self.fields),
+                        layout=[[k, list(s)] for k, s in self.layout], fingerprint=self.fingerprint), path)
+
+    @classmethod
+    def load(cls, path, map_location=None):
+        d = torch.load(path, map_location=map_location, weights_only=True)
+        return cls(bases=tuple((a.cpu().numpy(), s.cpu().numpy()) for a, s in d["bases"]), bases_flat=d["bases_flat"],
+                   eigenvalues=d["eigenvalues"], n=int(d["n"]), fisher=str(d["fisher"]), seed=int(d["seed"]),
+                   fields=None if d["fields"] is None else tuple(d["fields"]),
+                   layout=tuple((k, tuple(int(x) for x in s)) for k, s in d["layout"]), fingerprint=str(d["fingerprint"]))
+
+
+def _data_device(data):
+    from .models_rd import _device_of
+    return _device_of(data["src"]) if isinstance(data, dict) else (data[0] if isinstance(data, tuple) else data).P.device
+
+
+def kfac_covariances(model, data, fisher="true", seed=0, internal_batch_size=None):
+    """[(A, S)] float64 on the device, per Kronecker block (kfac_blocks): A = (1/n) sum_b sum_r x~_r x~_r^T over the
+    layer's input rows x~ = [x | 1], S = (1/n) sum_b sum_r dy_r dy_r^T over its output gradients (of l_b, not l_b / B),
+    encoder rows t*B + b for all T, ob-prop rows b*N + n.  fisher "true": labels drawn from the model's softmax
+    (rd_fisher_labels, keyed by (seed, sample index)); "empirical": data's labels.  Computed in tracin's row batches, so
+    the result is bitwise the same for any internal_batch_size (accepted for symmetry; it rounds up to the row batch)."""
+    _check_fisher(fisher, seed)
+    _check_data(model, data, "data", allow_none_y=fisher == "true")
+    _check_batch_size(internal_batch_size)
+    if model.training:
+        raise ValueError("kfac_covariances runs the model in eval arithmetic: call model.eval() first")
+    if fisher == "empirical" and isinstance(data, dict) and data.get("y") is None:
+        raise ValueError("fisher='empirical' needs the data's labels y")
+    dev = _data_device(data)
+    lib = L.load()
+    plan = model._prepare(dev)
+    blocks = kfac_blocks(model)
+    offs, total = _factor_offsets(blocks)
+    n, fetch = _source(data, "data")
+    R = _row_batch(lib, plan, _bucket_length(grad_layout(model)))
+    d = _dims(plan, R)
+    if lib.rd_kfac_factors_doubles(C.byref(d)) != total:
+        raise L.RaindropB200Error("the K-FAC factor layout of the library and of influence.py disagree")
+    acc = torch.zeros(total, dtype=torch.float64, device=dev)
+    with torch.no_grad(), _Weights(model):
+        for s0 in range(0, n, R):
+            src, static, times, lengths, y = fetch(s0, min(n, s0 + R))
+            _backward(model, src, static, times, lengths, None if fisher == "true" else y, "factors", out=acc,
+                      fisher_seed=int(seed) if fisher == "true" else None, index0=s0)
+    acc /= max(n, 1)
+    return [(acc[a:a + (kin + 1) ** 2].view(kin + 1, kin + 1), acc[s:s + nout * nout].view(nout, nout))
+            for (a, s), (_, _, nout, kin) in zip(offs, blocks)]
+
+
+def _segments(seg_off, seg_len):
+    n_seg = len(seg_off)
+    return (C.c_int64 * n_seg)(*seg_off.tolist()), (C.c_int64 * n_seg)(*seg_len.tolist()), n_seg
+
+
+def ekfac_factors(model, train, fisher="true", seed=0, fields=None, internal_batch_size=None):
+    """EKFACFactors of `train` (tracin's train argument) at the model's current weights.  Two passes: the K-FAC factors
+    (kfac_covariances) and their float64 eigenbases (numpy eigh on the host, signs fixed), then the rotated rows
+    (rd_raindrop_v2_ekfac_rows, in tracin's row batches) whose squares rd_ekfac_accumulate_sq adds into Lambda; no rows
+    are kept.  The same labels serve both passes.  fields: a subset of the trained tensors, chosen at block granularity
+    (a linear layer's weight and bias together).  The weights, the mode and the dropout counter are restored."""
+    _check_fisher(fisher, seed)
+    sel = _check_block_fields(model, fields)
+    _check_data(model, train, "train", allow_none_y=fisher == "true")
+    _check_batch_size(internal_batch_size)
+    if model.training:
+        raise ValueError("ekfac_factors runs the model in eval arithmetic: call model.eval() first")
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    blocks = kfac_blocks(model)
+    cov = kfac_covariances(model, train, fisher, seed, internal_batch_size)
+    bases = []
+    for A, S in cov:
+        bases.append((_eigh(A.cpu().numpy())[1], _eigh(S.cpu().numpy())[1]))
+    dev = _data_device(train)
+    lib = L.load()
+    plan = model._prepare(dev)
+    flat = _flat_bases(blocks, bases)
+    R = _row_batch(lib, plan, ldg)
+    if lib.rd_ekfac_bases_floats(C.byref(_dims(plan, R))) != flat.numel():
+        raise L.RaindropB200Error("the EK-FAC basis layout of the library and of influence.py disagree")
+    flat_dev = flat.to(dev)
+    seg_off, seg_len = plan_segments(layout, None if fields is None else list(fields))
+    offs, lens, n_seg = _segments(seg_off, seg_len)
+    n, fetch = _source(train, "train")
+    lam = torch.zeros(ldg, dtype=torch.float64, device=dev)
+    st = L.stream_ptr(dev)
+    fs = int(seed) if fisher == "true" else None
+    with torch.no_grad(), _Weights(model) as w:
+        for s0 in range(0, n, R):
+            s1 = min(n, s0 + R)
+            G = _ekfac_rows_aligned(model, fetch, s0, s1, R, ldg, flat_dev, fs)
+            L.check(lib.rd_ekfac_accumulate_sq(G.data_ptr(), s1 - s0, ldg, offs, lens, n_seg, lam.data_ptr(), st),
+                    "rd_ekfac_accumulate_sq")
+            del G
+        fp = _fingerprint(w.params)
+    lam /= max(n, 1)
+    return EKFACFactors(bases=tuple(bases), bases_flat=flat, eigenvalues=lam, n=n, fisher=fisher, seed=int(seed),
+                        fields=None if fields is None else tuple(fields),
+                        layout=tuple((k, tuple(s)) for k, _, s in layout), fingerprint=fp)
+
+
+def _damping_groups(layout, blocks, fields):
+    """[(column ranges)] of the selected blocks (weight and bias together) and diagonal fields, in bucket order."""
+    sel = _selected(layout, None if fields is None else list(fields))
+    where = {k: (off, math.prod(shape)) for k, off, shape in layout}
+    in_block = {}
+    for w, b, _, _ in blocks:
+        in_block[w] = in_block[b] = (w, b)
+    groups, seen = [], set()
+    for k, _, _ in layout:
+        if k not in sel or k in seen:
+            continue
+        keys = in_block.get(k, (k,))
+        seen.update(keys)
+        groups.append([where[x] for x in keys])
+    return groups
+
+
+def ekfac_weights(factors, damping=None):
+    """float64 numpy [bucket]: w_j = 1 / (Lambda_j + lambda_f(j)) on the selected columns, 0 elsewhere.  damping None:
+    lambda_f = 0.1 * mean(Lambda) over each block (weight and bias) or diagonal field; a float: that value everywhere."""
+    damping = _check_damping(damping)
+    lam = factors.eigenvalues.detach().cpu().numpy().astype(np.float64)
+    layout = [(k, off, s) for (k, s), off in zip(factors.layout, _offsets(factors.layout))]
+    blocks = _blocks_of_layout(factors.layout)
+    w = np.zeros_like(lam)
+    for ranges in _damping_groups(layout, blocks, factors.fields):
+        cols = np.concatenate([np.arange(o, o + n) for o, n in ranges])
+        lf = EKFAC_DAMPING_FACTOR * lam[cols].mean() if damping is None else damping
+        if not lf > 0:
+            lf = np.finfo(np.float64).tiny
+        w[cols] = 1.0 / (lam[cols] + lf)
+    return w
+
+
+def _offsets(layout_shapes):
+    out, off = [], 0
+    for _, s in layout_shapes:
+        out.append(off)
+        off += (math.prod(s) + 3) // 4 * 4
+    return out
+
+
+def _blocks_of_layout(layout_shapes):
+    """kfac_blocks from a ((key, shape), ...) layout: the head has 6 fields with a static embedding, else 4."""
+    keys = [k for k, _ in layout_shapes]
+    head = 6 if keys[0].startswith("emb") else 4
+    nl = (len(keys) - head - 4) // 12
+    idx = [head + 12 * l + k for l in range(nl) for k in (0, 2, 4, 6)] + [head + 12 * nl, head + 12 * nl + 2]
+    return [(keys[i], keys[i + 1], layout_shapes[i][1][0], layout_shapes[i][1][1]) for i in idx]
+
+
+def _check_factors(model, factors):
+    if not isinstance(factors, EKFACFactors):
+        raise TypeError("factors must be an EKFACFactors (ekfac_factors)")
+    layout = tuple((k, tuple(s)) for k, _, s in grad_layout(model))
+    if factors.layout != layout:
+        raise ValueError("the factors were computed for a model of another layout")
+    if factors.fields is not None:
+        _check_block_fields(model, list(factors.fields))
+    if factors.eigenvalues.numel() != _bucket_length(grad_layout(model)):
+        raise ValueError("the factors' eigenvalues do not span the model's gradient rows")
+    if len(factors.bases) != len(kfac_blocks(model)):
+        raise ValueError("the factors hold %d bases; the model has %d blocks" % (len(factors.bases), len(kfac_blocks(model))))
+    fp = _fingerprint(model.used_parameters())
+    if fp != factors.fingerprint:
+        raise ValueError("the factors were computed for other weights (fingerprint %s..., the model's %s...)"
+                         % (factors.fingerprint[:12], fp[:12]))
+
+
+def ekfac_influence(model, query, train, factors, damping=None, internal_batch_size=None):
+    """EK-FAC influence scores [n_query, n_train] float64 on the device: sum_j G~_qj G~_tj / (Lambda_j + lambda_f(j))
+    over the factors' fields, G~ the gradient rows rotated into the Kronecker eigenbases (rd_raindrop_v2_ekfac_rows;
+    LayerNorm and head fields unrotated).  Positive = proponent, as for tracin.  query: dict (y None = the predicted
+    class); train: as tracin's (its true labels).  The query rows are scaled by w = 1 / (Lambda + lambda)
+    (rd_ekfac_scale_rows, fp32) and contracted with the train rows by rd_per_sample_grad_dot, in tracin's blocks, so
+    scores are bitwise the same for any internal_batch_size, data source or run.  Factors that do not match the model
+    (layout, fields, weight fingerprint) are refused on the host.  The weights, mode and dropout counter are restored."""
+    if not isinstance(query, dict):
+        raise TypeError("query must be a dict (src, static, times, lengths, y)")
+    _check_data(model, query, "query", allow_none_y=True)
+    _check_data(model, train, "train", allow_none_y=False)
+    _check_batch_size(internal_batch_size)
+    damping = _check_damping(damping)
+    _check_factors(model, factors)
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    seg_off, seg_len = plan_segments(layout, None if factors.fields is None else list(factors.fields))
+    dev = _data_device(query)
+    lib = L.load()
+    plan = model._prepare(dev)
+    nq, q_fetch = _source(query, "query")
+    nt, t_fetch = _source(train, "train")
+    offs, lens, n_seg = _segments(seg_off, seg_len)
+    scores = torch.zeros(nq, nt, dtype=torch.float64, device=dev)
+    if nq == 0 or nt == 0:
+        return scores
+    w = torch.from_numpy(ekfac_weights(factors, damping)).to(device=dev, dtype=torch.float32)
+    bases = factors.bases_flat.to(device=dev, dtype=torch.float32).contiguous()
+    qb, tc, R = _blocks(lib, plan, ldg, n_seg, nq, nt, internal_batch_size)
+    st = L.stream_ptr(dev)
+    with torch.no_grad(), _Weights(model):
+        for q0 in range(0, nq, qb):
+            q1 = min(nq, q0 + qb)
+            Gq = _ekfac_rows_aligned(model, q_fetch, q0, q1, R, ldg, bases)
+            L.check(lib.rd_ekfac_scale_rows(Gq.data_ptr(), q1 - q0, ldg, offs, lens, n_seg, w.data_ptr(), st),
+                    "rd_ekfac_scale_rows")
+            for t0 in range(0, nt, tc):
+                t1 = min(nt, t0 + tc)
+                Gt = _ekfac_rows_aligned(model, t_fetch, t0, t1, R, ldg, bases)
+                nb = lib.rd_per_sample_grad_dot_scratch_bytes(q1 - q0, t1 - t0, ldg, n_seg)
+                sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
+                L.check(lib.rd_per_sample_grad_dot(Gq.data_ptr(), q1 - q0, Gt.data_ptr(), t1 - t0, ldg, offs, lens, n_seg,
+                                                   1.0, scores.data_ptr() + 8 * (q0 * nt + t0), nt, sc.data_ptr(), st),
+                        "rd_per_sample_grad_dot")
+                del Gt, sc
+            del Gq
+    return scores
+
+
+def ekfac_self_influence(model, data, factors, damping=None, internal_batch_size=None):
+    """[n] float64 on the device: sum_j G~_j^2 / (Lambda_j + lambda_f(j)) of each sample with its own label, for ranking
+    candidate mislabels.  Each row batch's scaled rows are contracted with its rows by rd_per_sample_grad_dot and the
+    diagonal kept, so the result equals the diagonal of ekfac_influence(data, data) (data's labels on both sides)
+    bitwise.  internal_batch_size: accepted for symmetry (the work runs in tracin's row batches)."""
+    _check_data(model, data, "data", allow_none_y=False)
+    _check_batch_size(internal_batch_size)
+    damping = _check_damping(damping)
+    if model.training:
+        raise ValueError("ekfac_self_influence runs the model in eval arithmetic: call model.eval() first")
+    _check_factors(model, factors)
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    seg_off, seg_len = plan_segments(layout, None if factors.fields is None else list(factors.fields))
+    offs, lens, n_seg = _segments(seg_off, seg_len)
+    dev = _data_device(data)
+    lib = L.load()
+    plan = model._prepare(dev)
+    n, fetch = _source(data, "data")
+    out = torch.zeros(n, dtype=torch.float64, device=dev)
+    if n == 0:
+        return out
+    w = torch.from_numpy(ekfac_weights(factors, damping)).to(device=dev, dtype=torch.float32)
+    bases = factors.bases_flat.to(device=dev, dtype=torch.float32).contiguous()
+    R = _row_batch(lib, plan, ldg)
+    st = L.stream_ptr(dev)
+    with torch.no_grad(), _Weights(model):
+        for s0 in range(0, n, R):
+            s1 = min(n, s0 + R)
+            b = s1 - s0
+            G = _ekfac_rows_aligned(model, fetch, s0, s1, R, ldg, bases)
+            Gs = G.clone()
+            L.check(lib.rd_ekfac_scale_rows(Gs.data_ptr(), b, ldg, offs, lens, n_seg, w.data_ptr(), st),
+                    "rd_ekfac_scale_rows")
+            sq = torch.zeros(b, b, dtype=torch.float64, device=dev)
+            nb = lib.rd_per_sample_grad_dot_scratch_bytes(b, b, ldg, n_seg)
+            sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
+            L.check(lib.rd_per_sample_grad_dot(Gs.data_ptr(), b, G.data_ptr(), b, ldg, offs, lens, n_seg, 1.0,
+                                               sq.data_ptr(), b, sc.data_ptr(), st), "rd_per_sample_grad_dot")
+            out[s0:s1] = sq.diagonal()
+            del G, Gs, sc, sq
+    return out
+
+
+def ekfac_rotate(G, factors):
+    """float64 numpy restatement of the rotation: G [n, bucket] gradient rows -> G~ with each block's [Nout, Kin + 1]
+    tile [W | b] replaced by Q_S^T [W | b] Q_A (LayerNorm and head fields, and padding, unchanged)."""
+    G = np.array(G, dtype=np.float64, copy=True)
+    offs = dict(zip([k for k, _ in factors.layout], _offsets(factors.layout)))
+    for (wk, bk, nout, kin), (QA, QS) in zip(_blocks_of_layout(factors.layout), factors.bases):
+        ow, ob = offs[wk], offs[bk]
+        M = np.concatenate([G[:, ow:ow + nout * kin].reshape(-1, nout, kin), G[:, ob:ob + nout, None]], axis=2)
+        Mt = np.asarray(QS, np.float64).T @ M @ np.asarray(QA, np.float64)
+        G[:, ow:ow + nout * kin] = Mt[:, :, :kin].reshape(len(G), -1)
+        G[:, ob:ob + nout] = Mt[:, :, kin]
+    return G
+
+
+def ekfac_from_grads(Gq, Gt, factors, damping=None):
+    """Host restatement of ekfac_influence in float64: Gq [n_query, bucket] and Gt [n_train, bucket] plain gradient rows
+    (per_sample_grads), rotated with the factors' float64 bases (ekfac_rotate) and contracted with the weights
+    ekfac_weights(factors, damping) -> [n_query, n_train]."""
+    w = ekfac_weights(factors, damping)
+    Gq, Gt = np.asarray(Gq, dtype=np.float64), np.asarray(Gt, dtype=np.float64)
+    if Gq.ndim != 2 or Gt.ndim != 2 or Gq.shape[1] != w.shape[0] or Gt.shape[1] != w.shape[0]:
+        raise ValueError("Gq [q, %d] and Gt [t, %d] do not match: %s, %s" % (w.shape[0], w.shape[0], Gq.shape, Gt.shape))
+    return (ekfac_rotate(Gq, factors) * w) @ ekfac_rotate(Gt, factors).T

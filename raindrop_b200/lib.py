@@ -168,6 +168,19 @@ SIGNATURES = {
     "rd_debug_dropout_mask": (C.c_int, [C.c_void_p, C.c_uint32, C.c_int64, C.c_float, C.c_void_p,
                                         C.c_void_p]),
     "rd_debug_projection_signs": (C.c_int, [C.c_uint64, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "rd_kfac_factors_doubles": (C.c_int64, [C.POINTER(RdDims)]),
+    "rd_ekfac_bases_floats": (C.c_int64, [C.POINTER(RdDims)]),
+    "rd_kfac_factors_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
+    "rd_raindrop_v2_kfac_factors": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 8),
+    "rd_ekfac_rows_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
+    "rd_raindrop_v2_ekfac_rows": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 8 +
+                                  [C.c_int64, C.c_void_p]),
+    "rd_ekfac_accumulate_sq": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                         C.c_int32, C.c_void_p, C.c_void_p]),
+    "rd_ekfac_scale_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                      C.c_int32, C.c_void_p, C.c_void_p]),
+    "rd_fisher_labels": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "rd_debug_fisher_uniforms": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

@@ -15,6 +15,13 @@ passes (2 x 2 x rows x columns x dim) against the 495 TFLOP/s data sheet, the qu
 whole-set exact time, extrapolated from tracin timed on --exact-train training samples (labelled as extrapolated).
 
     python tools/bench_tracin.py --shape PAM --n-query 533 --n-train 4266 --projection 4096
+
+--ekfac times EK-FAC influence functions instead (influence.ekfac_*): the factor pass (kfac_covariances), the host
+eigendecompositions and the Lambda pass (the rest of ekfac_factors), and the scoring of n_query queries against
+--exact-train training samples next to tracin on the same samples, both extrapolated linearly to n_train (labelled as
+extrapolated).  The rotations' cost is the difference between the rotated and the plain row passes over those samples.
+
+    python tools/bench_tracin.py --shape P19 --n-query 3880 --n-train 31000 --ekfac
 """
 import argparse
 import ctypes as C
@@ -243,6 +250,48 @@ def run_projection(shape, nq, nt, dim, exact_nt):
                 exact_s_extrapolated=t_exact, sketch_bytes=4 * (nt + nq) * dim)
 
 
+def run_ekfac(shape, nq, nt, exact_nt):
+    cfg = model_config(shape, dropout=0.2)
+    model = build_dropin(cfg, 21)
+    model.eval()
+    dq = to_dev(make_batch(cfg, nq, seed=1))
+    dt = make_batch(cfg, nt, seed=2)
+    ds = DeviceDataset(dt["src"], dt["static"], dt["times"], dt["y"])
+    q = dict(src=dq["src"], static=dq["static"], times=dq["times"], lengths=dq["lengths"], y=None)
+    warm = (ds, torch.arange(min(nt, 64)))
+    IF.ekfac_influence(model, q, warm, IF.ekfac_factors(model, warm))                                    # warm-up
+
+    def timed(fn):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        out = fn()
+        torch.cuda.synchronize()
+        return out, time.perf_counter() - t0
+    _, t_cov = timed(lambda: IF.kfac_covariances(model, ds))
+    f, t_all = timed(lambda: IF.ekfac_factors(model, ds))
+    ne = min(nt, exact_nt)
+    sub = (ds, torch.arange(ne))
+    S, t_score = timed(lambda: IF.ekfac_influence(model, q, sub, f))
+    _, t_exact = timed(lambda: IF.tracin(model, q, sub))
+    # rotated against plain rows over the same samples, in the same row batches
+    lib, plan = L.load(), model._plan
+    ldg = IF._bucket_length(IF.grad_layout(model))
+    R = IF._row_batch(lib, plan, ldg)
+    _, fetch = IF._source(sub, "train")
+    bases = f.bases_flat.cuda()
+    with torch.no_grad():
+        _, t_plain = timed(lambda: [IF._rows_aligned(model, fetch, i, min(ne, i + R), R, ldg) for i in range(0, ne, R)])
+        _, t_rot = timed(lambda: [IF._ekfac_rows_aligned(model, fetch, i, min(ne, i + R), R, ldg, bases)
+                                  for i in range(0, ne, R)])
+    scale = nt / ne
+    return dict(shape=shape, card=card(), n_query=nq, n_train=nt, bucket=ldg, row_batch=R,
+                factor_pass_s=t_cov, eigh_and_lambda_pass_s=t_all - t_cov, factors_total_s=t_all,
+                scored_train_samples=ne, ekfac_scoring_s_extrapolated=t_score * scale,
+                tracin_s_extrapolated=t_exact * scale, scoring_ratio=t_score / t_exact,
+                rows_plain_s=t_plain, rows_rotated_s=t_rot, rotation_share_of_rows=(t_rot - t_plain) / t_rot,
+                scores_finite=bool(torch.isfinite(S).all()))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shape", default="P19")
@@ -250,8 +299,13 @@ def main():
     ap.add_argument("--n-train", type=int, default=31000)
     ap.add_argument("--loop", type=int, default=64)
     ap.add_argument("--projection", type=int, help="time TracIn-RP with this many projection dimensions")
-    ap.add_argument("--exact-train", type=int, default=1024, help="--projection: train samples of the timed exact call")
+    ap.add_argument("--exact-train", type=int, default=1024,
+                    help="--projection, --ekfac: train samples of the timed exact (and EK-FAC) scoring calls")
+    ap.add_argument("--ekfac", action="store_true", help="time EK-FAC influence functions")
     a = ap.parse_args()
+    if a.ekfac:
+        print(json.dumps(run_ekfac(a.shape, a.n_query, a.n_train, a.exact_train)), flush=True)
+        return
     if a.projection:
         print(json.dumps(run_projection(a.shape, a.n_query, a.n_train, a.projection, a.exact_train)), flush=True)
         return

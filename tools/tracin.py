@@ -18,6 +18,11 @@ class.  Files, under --out-dir with suffix _<name>.npy:
 onto DIM random +-1 directions fixed by --projection-seed); --save-sketch PATH writes the training set's sketch and
 --load-sketch PATH reuses one (it must match the checkpoints, fields, DIM and seed).  The files are the same; the
 self-influence stays exact.
+
+--method ekfac scores with EK-FAC influence functions instead (influence.ekfac_factors / ekfac_influence, the true
+Fisher at the single checkpoint's weights, preconditioned by its inverse with --damping or 0.1 of each block's mean
+eigenvalue); --save-factors PATH / --load-factors PATH write or reuse the training set's factors.  The files keep their
+names; the self-influence is EK-FAC's sum_j G~_j^2 / (Lambda_j + lambda).
 """
 import argparse
 import os
@@ -61,17 +66,27 @@ def main():
     ap.add_argument("--projection-seed", type=int, default=0, help="seed of the projection's +-1 directions")
     ap.add_argument("--save-sketch", metavar="PATH", help="--projection: write the training set's sketch here")
     ap.add_argument("--load-sketch", metavar="PATH", help="--projection: reuse this training-set sketch")
+    ap.add_argument("--method", default="tracin", choices=["tracin", "ekfac"],
+                    help="ekfac: EK-FAC influence functions at the first checkpoint's weights (influence.ekfac_*)")
+    ap.add_argument("--damping", type=float, help="--method ekfac: one damping for every block (default 0.1 mean)")
+    ap.add_argument("--save-factors", metavar="PATH", help="--method ekfac: write the training set's EK-FAC factors here")
+    ap.add_argument("--load-factors", metavar="PATH", help="--method ekfac: reuse these EK-FAC factors")
     ap.add_argument("--name", help="file name suffix (default: the synthetic configuration or 'dataset')")
     ap.add_argument("--out-dir", default=".")
     args = ap.parse_args()
 
     from raindrop_b200 import data as RD
-    from raindrop_b200.influence import GradientSketch, project, self_influence, tracin, tracin_sketch
+    from raindrop_b200.influence import (EKFACFactors, GradientSketch, ekfac_factors, ekfac_influence, ekfac_self_influence,
+                                         project, self_influence, tracin, tracin_sketch)
     from raindrop_b200.synth import make_batch, model_config
     if not torch.cuda.is_available():
         raise SystemExit("tracin runs on a CUDA device")
     if (args.save_sketch or args.load_sketch) and not args.projection:
         raise SystemExit("--save-sketch and --load-sketch need --projection")
+    if (args.save_factors or args.load_factors or args.damping is not None) and args.method != "ekfac":
+        raise SystemExit("--save-factors, --load-factors and --damping need --method ekfac")
+    if args.method == "ekfac" and (args.projection or len(args.checkpoint) != 1):
+        raise SystemExit("--method ekfac takes one --checkpoint and no --projection")
     lrs = args.lr or [1.0] * len(args.checkpoint)
     if len(lrs) != len(args.checkpoint):
         raise SystemExit("give one --lr per --checkpoint")
@@ -115,7 +130,16 @@ def main():
         test = dict(src=P, static=Ps, times=Pt, lengths=torch.sum(Pt > 0, dim=0), y=None)
         name = args.name or "dataset"
 
-    if args.projection:
+    if args.method == "ekfac":
+        if args.load_factors:
+            factors = EKFACFactors.load(args.load_factors, map_location=device)
+        else:
+            factors = ekfac_factors(model, train, fields=args.fields)
+        if args.save_factors:
+            factors.save(args.save_factors)
+        scores = ekfac_influence(model, test, train, factors, damping=args.damping).cpu().numpy()
+        si = ekfac_self_influence(model, train, factors, damping=args.damping).cpu().numpy()
+    elif args.projection:
         kw = dict(checkpoints=ckpts, dim=args.projection, seed=args.projection_seed, fields=args.fields)
         if args.load_sketch:
             train_sketch = GradientSketch.load(args.load_sketch, map_location=device)
@@ -126,7 +150,8 @@ def main():
         scores = tracin_sketch(project(model, test, **kw), train_sketch).cpu().numpy()
     else:
         scores = tracin(model, test, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
-    si = self_influence(model, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
+    if args.method != "ekfac":
+        si = self_influence(model, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
     pro, pro_s, opp, opp_s = top_k(scores, args.top_k)
     out = dict(tracin_proponents=pro, tracin_proponent_scores=pro_s, tracin_opponents=opp, tracin_opponent_scores=opp_s,
                tracin_self_influence_order=np.argsort(-si, kind="stable"), tracin_self_influence=si)

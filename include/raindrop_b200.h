@@ -153,7 +153,8 @@ int rd_obprop_bwd(const float* x, const float* out, const float* d_out, const fl
  * Raindrop_v2, code/models_rd.py:317, but part of the operator's API).  One sample: x [N, C=T*d_ob],
  * p_t [T, 16].  Keeps the K = E/2 edges with the highest mean gamma (in that order), regroups them by
  * SOURCE for the per-channel segment softmax and scatters to the source (as the reference does).
- * Outputs: out [N, C]; pruned edge list edge_src_out/edge_tgt_out [K]; alpha_out [K].  Forward only. */
+ * Outputs: out [N, C]; pruned edge list edge_src_out/edge_tgt_out [K]; alpha_out [K].  Needs E >= 2 (K >= 1): the
+ * forward, the backward and both scratch-size queries (which return 0) refuse fewer. */
 size_t rd_obprop_beta_scratch_bytes(int32_t N, int32_t T, int32_t d_ob, int32_t E);
 int rd_obprop_beta_fwd(const float* x, const float* p_t, const int64_t* edge_src, const int64_t* edge_tgt,
                        const float* edge_w, int32_t E, int32_t N, int32_t T, int32_t d_ob,
@@ -432,7 +433,9 @@ int rd_linear_wgrad_group(const rd_wgrad_item* items, int32_t n, void* stream);
 /* TransformerConv.forward (code/transformer_conv.py:139-207), concat=True, root_weight=True, beta=False, no edge
  * features -- and its backward.  Batched over `n_graphs` independent graphs that share ONE edge list (legacy Raindrop v1
  * applies the layer to every sample of a batch, code/models_rd.py:158-166): the row of node i of graph g in x / out is
- * i * node_stride + g * graph_stride (single graph: n_graphs = 1, node_stride = 1, graph_stride = 0).
+ * i * node_stride + g * graph_stride (single graph: n_graphs = 1, node_stride = 1, graph_stride = 0).  The rows must
+ * tile [0, n_nodes * n_graphs) densely: (node_stride, graph_stride) = (n_graphs, 1) or (1, n_nodes); anything else is
+ * refused.
  *   x [rows, in];  weights [H*F, in];  edge_w [E] or NULL (then the logits are q_i.k_j / sqrt(F));
  *   out [rows, H*F];  alpha [n_graphs, E, H] (post-softmax, as returned by the reference).
  * Backward: writes d_x (may be NULL), d_w* / d_b* (written, not accumulated; with edge_w the q/k projections take no

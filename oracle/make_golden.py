@@ -255,18 +255,31 @@ def operator_grad_cases():
     print("operators_grad     %d arrays: %s" % (len(out), sorted(out)[:60]))
 
 
-def v1_case():
-    """Legacy `Raindrop` v1 (code/models_rd.py:46-191; hard-coded to 36 sensors / 215 steps): logits, loss and the
-    gradient of every parameter that gets one, B = 3, eval mode.  Weights: seeded default init, but `encoder` / `emb`
-    re-drawn at a useful scale (the reference initialises them to +-1e-10, which would hide the graph layer)."""
+# name, batch, data seed, model seed, (d_model, nhead, nhid, nlayers), graph density, isolated sensor (or None)
+V1_CASES = [
+    ("v1_p12_b3", 3, 77, 5, (72, 2, 144, 2), 0.5, None),
+    ("v1_sparse_b5", 5, 78, 6, (36, 2, 64, 1), 0.15, 7),      # 1075 rows; sensor 7 keeps only its forced self loop
+    ("v1_b1", 1, 79, 7, (72, 4, 36, 1), 0.5, None),           # one graph: the batched operator with n_graphs = 1
+]
+
+
+def v1_case(name, B, data_seed, model_seed, shape, density, isolated):
+    """Legacy `Raindrop` v1 (code/models_rd.py:46-191; hard-coded to 36 sensors / 215 steps, so a case can vary the
+    batch, the encoder's shape and the sensor graph but not d_inp or T): logits, loss and the gradient of every
+    parameter that gets one, eval mode.  Weights: seeded default init, but `encoder` / `emb` re-drawn at a useful scale
+    (the reference initialises them to +-1e-10, which would hide the graph layer)."""
     ref = ref_harness.load_reference()
     from raindrop_b200.synth import CONFIGS
     cfg = dict(CONFIGS["P12"]); cfg["name"] = "P12"
-    B = 3
-    batch = make_batch(dict(cfg, d_ob=2), B, seed=77)
-    torch.manual_seed(5)
-    gs = (torch.rand(36, 36) < 0.5).float() * torch.rand(36, 36)
-    model = ref.Raindrop(36, 72, 2, 144, 2, 0.2, 215, 9, 100, 0.5, "mean", 2, gs.clone()).eval()
+    batch = make_batch(dict(cfg, d_ob=2), B, seed=data_seed)
+    torch.manual_seed(model_seed)
+    gs = (torch.rand(36, 36) < density).float() * torch.rand(36, 36)
+    if isolated is not None:
+        gs[isolated, :] = 0
+        gs[:, isolated] = 0
+    d_model, nhead, nhid, nlayers = shape
+    ctor = [36, d_model, nhead, nhid, nlayers, 0.2, 215, 9, 100, 0.5, "mean", 2]
+    model = ref.Raindrop(*ctor, gs.clone()).eval()
     with torch.no_grad():
         model.encoder.weight.uniform_(-0.3, 0.3)
         model.emb.weight.uniform_(-0.3, 0.3)
@@ -281,12 +294,12 @@ def v1_case():
     for k, prm in model.named_parameters():
         if prm.grad is not None:
             out["grad." + k] = prm.grad.numpy()
-    meta = dict(case="v1_p12_b3", batch=B, data_seed=77, torch=torch.__version__, reference_commit="892eb57",
+    meta = dict(case=name, batch=B, data_seed=data_seed, ctor=ctor, torch=torch.__version__, reference_commit="892eb57",
                 generator="oracle/make_golden.py v1")
     out["meta"] = np.frombuffer(json.dumps(meta).encode(), dtype=np.uint8)
-    np.savez_compressed(os.path.join(GOLDEN, "v1_p12_b3.npz"), **out)
-    print("v1_p12_b3  logits[0]=%s loss=%.6f distance=%g grads for %d tensors" %
-          (logits[0].tolist(), loss.item(), float(distance), sum(1 for k in out if k.startswith("grad."))))
+    np.savez_compressed(os.path.join(GOLDEN, name + ".npz"), **out)
+    print("%s  logits[0]=%s loss=%.6f distance=%g grads for %d tensors" %
+          (name, logits[0].tolist(), loss.item(), float(distance), sum(1 for k in out if k.startswith("grad."))))
 
 
 def data_utils_case():
@@ -335,8 +348,10 @@ if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "operators_grad":      # add-on fixtures: leaves the existing files untouched
         operator_grad_cases()
         sys.exit(0)
-    if len(sys.argv) > 1 and sys.argv[1] == "v1":
-        v1_case()
+    if len(sys.argv) > 1 and sys.argv[1] == "v1":          # optionally followed by the case names to (re)generate
+        for case in V1_CASES:
+            if len(sys.argv) == 2 or case[0] in sys.argv[2:]:
+                v1_case(*case)
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "hparams":
         hparam_cases()
@@ -349,7 +364,8 @@ if __name__ == "__main__":
         run_case(*case)
     operator_cases()
     operator_grad_cases()
-    v1_case()
+    for case in V1_CASES:
+        v1_case(*case)
     data_utils_case()
     live_tiny_case()
     hparam_cases()

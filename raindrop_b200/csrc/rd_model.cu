@@ -919,7 +919,7 @@ const char* rd_last_error_string(void) { return last_error(); }
 uint64_t rd_launch_count(void) { return launch_count(); }
 
 int rd_node_scale(const int64_t* edge_tgt, const float* edge_w, int32_t E, int32_t N, float* out, void* stream) {
-  if (!edge_tgt || !edge_w || !out || E < 0 || N < 1) { set_error("rd_node_scale: bad arguments"); return -2; }
+  if ((E > 0 && (!edge_tgt || !edge_w)) || !out || E < 0 || N < 1) { set_error("rd_node_scale: bad arguments"); return -2; }
   return node_scale(edge_tgt, edge_w, E, N, out, (cudaStream_t)stream);
 }
 

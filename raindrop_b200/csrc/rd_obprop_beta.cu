@@ -199,8 +199,10 @@ BLay blayout(int N, int T, int d_ob, int E) {
   l.mx = take((long long)N * C); l.den = take((long long)N * C); l.dot = take((long long)N * C);
   l.gp = take(K * C); l.dgam = take(K * C); l.dpre = take((long long)N * C); l.dbeta = take((long long)N * T);
   l.dHn = take((long long)N * 8 * C);
+  // both weight gradients share `partial`; the [C, C] one has fewer tiles, so it may split where the [8C, C] one does not
   int ns;
-  l.partial = take(gemm_splitk_plan((int)(8 * C), (int)C, N, &ns));
+  const int64_t p_inc = gemm_splitk_plan((int)(8 * C), (int)C, N, &ns), p_val = gemm_splitk_plan((int)C, (int)C, N, &ns);
+  l.partial = take(p_inc > p_val ? p_inc : p_val);
   l.total = o;
   return l;
 }
@@ -216,7 +218,7 @@ __global__ void gather_kept_w_kernel(const float* __restrict__ w, const int* __r
 using namespace rd;
 
 extern "C" size_t rd_obprop_beta_bwd_scratch_bytes(int32_t N, int32_t T, int32_t d_ob, int32_t E) {
-  if (N < 1 || T < 1 || d_ob < 1 || E < 1) return 0;
+  if (N < 1 || T < 1 || d_ob < 1 || E < 2) return 0;
   return (size_t)blayout(N, T, d_ob, E).total * sizeof(float);
 }
 
@@ -232,10 +234,11 @@ extern "C" int rd_obprop_beta_bwd(const float* x, const float* p_t, const int64_
                                   float* d_x, float* d_edge_w, float* d_p_t, float* d_inc_w, float* d_inc_b, float* d_map_w,
                                   float* d_val_w, float* d_val_b, void* scratch, void* stream) {
   if (!x || !p_t || !edge_src || !edge_tgt || !edge_w || !increase_dim_w || !increase_dim_b || !map_weights || !value_w ||
-      !value_b || !d_out || !d_edge_w || !d_inc_w || !d_inc_b || !d_map_w || !d_val_w || !d_val_b || !scratch || E < 2 || N < 1 || T < 1) {
+      !value_b || !d_out || !d_edge_w || !d_inc_w || !d_inc_b || !d_map_w || !d_val_w || !d_val_b || !scratch || N < 1 || T < 1) {
     set_error("rd_obprop_beta_bwd: bad arguments");
     return -2;
   }
+  if (E < 2) { set_error("rd_obprop_beta_bwd: E = %d, but keeping the top E / 2 edges needs E >= 2", E); return -2; }
   if (d_ob * 8 != 32) { set_error("use_beta needs d_ob == 4 (code/Ob_propagation.py:166)"); return -2; }
   cudaStream_t st = (cudaStream_t)stream;
   const int C = T * d_ob, K = E / 2;
@@ -307,10 +310,8 @@ extern "C" int rd_obprop_beta_bwd(const float* x, const float* p_t, const int64_
 }
 
 extern "C" size_t rd_obprop_beta_scratch_bytes(int32_t N, int32_t T, int32_t d_ob, int32_t E) {
-  int64_t C = (int64_t)T * d_ob;
-  int64_t f = round_up((int64_t)N * 8 * C, 64) + round_up((int64_t)N * C, 64) + round_up((int64_t)N * T, 64) +
-              round_up(E, 64) + round_up(E, 64);
-  return (size_t)f * sizeof(float);
+  if (N < 1 || T < 1 || d_ob < 1 || E < 2) return 0;
+  return (size_t)blayout(N, T, d_ob, E).eid * sizeof(float);   // the forward uses the layout up to `rank`
 }
 
 extern "C" int rd_obprop_beta_fwd(const float* x, const float* p_t, const int64_t* edge_src, const int64_t* edge_tgt,
@@ -319,18 +320,18 @@ extern "C" int rd_obprop_beta_fwd(const float* x, const float* p_t, const int64_
                                   const float* value_w, const float* value_b, float* out, int64_t* edge_src_out,
                                   int64_t* edge_tgt_out, float* alpha_out, void* scratch, void* stream) {
   if (!x || !p_t || !edge_src || !edge_tgt || !edge_w || !increase_dim_w || !increase_dim_b || !map_weights || !value_w ||
-      !value_b || !out || !edge_src_out || !edge_tgt_out || !alpha_out || !scratch || E < 1 || N < 1 || T < 1) {
+      !value_b || !out || !edge_src_out || !edge_tgt_out || !alpha_out || !scratch || N < 1 || T < 1) {
     set_error("rd_obprop_beta_fwd: bad arguments");
     return -2;
   }
+  if (E < 2) { set_error("rd_obprop_beta_fwd: E = %d, but keeping the top E / 2 edges needs E >= 2", E); return -2; }
   if (d_ob * 8 != 32) { set_error("use_beta needs out_channels*8 == T*32, i.e. d_ob == 4 (code/Ob_propagation.py:166)"); return -2; }
   cudaStream_t st = (cudaStream_t)stream;
   const int C = T * d_ob, K = E / 2;
-  float* Hn = (float*)scratch;
-  float* V = Hn + round_up((int64_t)N * 8 * C, 64);
-  float* beta = V + round_up((int64_t)N * C, 64);
-  float* score = beta + round_up((int64_t)N * T, 64);
-  int* rank = (int*)(score + round_up(E, 64));
+  const BLay l = blayout(N, T, d_ob, E);
+  float* sc = (float*)scratch;
+  float* Hn = sc + l.Hn; float* V = sc + l.V; float* beta = sc + l.beta; float* score = sc + l.score;
+  int* rank = (int*)(sc + l.rank);
   GemmP g;
   g.A = x; g.ta = 0; g.sAi = C; g.sAk = 1; g.B = increase_dim_w; g.tb = 1; g.sBj = C; g.sBk = 1;
   g.C = Hn; g.sCi = 8 * C; g.sCj = 1; g.M = N; g.N = 8 * C; g.K = C; g.bias = increase_dim_b;

@@ -193,9 +193,15 @@ Lay layout(int n_nodes, int n_graphs, int in_ch, int H, int F, int E, bool bwd) 
 
 int check_common(const char* who, const float* x, const int64_t* s, const int64_t* t, int n_nodes, int n_graphs, int in_ch, int H,
                  int F, int E, long long ns, long long gs) {
-  if (!x || !s || !t || n_nodes < 1 || n_graphs < 1 || in_ch < 1 || H < 1 || F < 1 || E < 0 || ns < 1 || gs < 0 ||
+  if (!x || (E > 0 && (!s || !t)) || n_nodes < 1 || n_graphs < 1 || in_ch < 1 || H < 1 || F < 1 || E < 0 || ns < 1 || gs < 0 ||
       (long long)n_nodes * n_graphs > 0x7fffffffLL) {
     set_error("%s: bad arguments", who);
+    return -2;
+  }
+  // rows of q/k/v are addressed as node * ns + graph * gs: only the two dense layouts stay inside n_nodes * n_graphs rows
+  const bool dense = n_graphs == 1 ? ns == 1 : ((ns == n_graphs && gs == 1) || (ns == 1 && gs == n_nodes));
+  if (!dense) {
+    set_error("%s: (node_stride, graph_stride) = (%lld, %lld) is not a dense layout of %d nodes x %d graphs", who, ns, gs, n_nodes, n_graphs);
     return -2;
   }
   return 0;
@@ -218,9 +224,10 @@ extern "C" int rd_transformer_conv_fwd(const float* x, int32_t n_nodes, int32_t 
                                        const float* wq, const float* bq, const float* wk, const float* bk, const float* wv,
                                        const float* bv, const float* ws, const float* bs, float* out, float* alpha,
                                        void* scratch, void* stream) {
+  // an empty edge list (E == 0) has no arrays: edge_src, edge_tgt and alpha may then be NULL
   RD_TRY(check_common("rd_transformer_conv_fwd", x, edge_src, edge_tgt, n_nodes, n_graphs, in_ch, heads, out_ch, E, node_stride,
                       graph_stride));
-  if (!wq || !wk || !wv || !ws || !out || !alpha || !scratch) { set_error("rd_transformer_conv_fwd: NULL argument"); return -2; }
+  if (!wq || !wk || !wv || !ws || !out || (E > 0 && !alpha) || !scratch) { set_error("rd_transformer_conv_fwd: NULL argument"); return -2; }
   cudaStream_t st = (cudaStream_t)stream;
   const Lay l = layout(n_nodes, n_graphs, in_ch, heads, out_ch, E, false);
   const int HF = heads * out_ch;
@@ -256,7 +263,7 @@ extern "C" int rd_transformer_conv_bwd(const float* x, int32_t n_nodes, int32_t 
                                        float* d_ws, float* d_bs, float* d_edge_w, void* scratch, void* stream) {
   RD_TRY(check_common("rd_transformer_conv_bwd", x, edge_src, edge_tgt, n_nodes, n_graphs, in_ch, heads, out_ch, E, node_stride,
                       graph_stride));
-  if (!wq || !wk || !wv || !ws || !alpha || !d_out || !d_wq || !d_bq || !d_wk || !d_bk || !d_wv || !d_bv || !d_ws || !d_bs || !scratch) {
+  if (!wq || !wk || !wv || !ws || (E > 0 && !alpha) || !d_out || !d_wq || !d_bq || !d_wk || !d_bk || !d_wv || !d_bv || !d_ws || !d_bs || !scratch) {
     set_error("rd_transformer_conv_bwd: NULL argument");
     return -2;
   }

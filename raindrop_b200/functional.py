@@ -423,6 +423,35 @@ class ObPropLayerFunction(torch.autograd.Function):
         return d_x, d_w, d_b, None, None
 
 
+def _check_edges(who, edge_index, edge_weights):
+    """edge_index must be [2, E] int64 and edge_weights (when given) [E]: the kernels index with them unchecked."""
+    if not torch.is_tensor(edge_index) or edge_index.dim() != 2 or edge_index.shape[0] != 2 or edge_index.dtype != torch.int64:
+        got = "%s %s" % (tuple(edge_index.shape), edge_index.dtype) if torch.is_tensor(edge_index) else type(edge_index).__name__
+        raise L.RaindropB200Error("%s: edge_index must be a [2, E] int64 tensor, got %s" % (who, got))
+    E = edge_index.shape[1]
+    if edge_weights is not None and (edge_weights.dim() != 1 or edge_weights.shape[0] != E):
+        raise L.RaindropB200Error("%s: edge_weights must have shape [E] = [%d] like edge_index, got %s"
+                                  % (who, E, tuple(edge_weights.shape)))
+    return E
+
+
+def _check_geom(who, geom, rows):
+    """geom = (n_nodes, n_graphs, node_stride, graph_stride) must map (node, graph) one-to-one onto the `rows` rows of x:
+    node-major (n_graphs, 1) or graph-major (1, n_nodes).  Anything else would index past the projections."""
+    n_nodes, n_graphs, node_stride, graph_stride = (int(v) for v in geom)
+    if n_nodes < 1 or n_graphs < 1:
+        raise L.RaindropB200Error("%s: geom needs n_nodes >= 1 and n_graphs >= 1, got %s" % (who, tuple(geom)))
+    dense = node_stride == 1 if n_graphs == 1 else (node_stride, graph_stride) in ((n_graphs, 1), (1, n_nodes))
+    if not dense:
+        raise L.RaindropB200Error("%s: geom strides (node_stride, graph_stride) = (%d, %d) are not a dense layout of %d "
+                                  "nodes x %d graphs: use (%d, 1) or (1, %d)"
+                                  % (who, node_stride, graph_stride, n_nodes, n_graphs, n_graphs, n_nodes))
+    if rows != n_nodes * n_graphs:
+        raise L.RaindropB200Error("%s: x has %d rows but geom describes n_nodes * n_graphs = %d * %d"
+                                  % (who, rows, n_nodes, n_graphs))
+    return n_nodes, n_graphs, node_stride, graph_stride
+
+
 class ObPropBetaFunction(torch.autograd.Function):
     """Observation_progation.forward(use_beta=True) for one sample (code/Ob_propagation.py:161-211) with gradients:
     rd_obprop_beta_fwd / rd_obprop_beta_bwd.  Returns (out [N, C], alpha [K], pruned edge list [2, K] (data))."""
@@ -460,14 +489,15 @@ class ObPropBetaFunction(torch.autograd.Function):
         d_out = _as_f32(d_out) if d_out is not None else torch.zeros(N, Cc, dtype=torch.float32, device=dev)
         d_alpha = None if d_alpha is None else _as_f32(d_alpha)
         f32 = dict(dtype=torch.float32, device=dev)
-        d_x = torch.empty(N, Cc, **f32)
-        d_w = torch.empty(E, **f32); d_pt = torch.empty(T, 16, **f32)
+        d_x = torch.empty(N, Cc, **f32) if ctx.needs_input_grad[0] else None
+        d_pt = torch.empty(T, 16, **f32) if ctx.needs_input_grad[1] else None
+        d_w = torch.empty(E, **f32)
         g_iw = torch.empty_like(inc_w); g_ib = torch.empty_like(inc_b); g_mw = torch.empty_like(map_w)
         g_vw = torch.empty_like(val_w); g_vb = torch.empty_like(val_b)
         sc = torch.empty(lib.rd_obprop_beta_bwd_scratch_bytes(N, T, d_ob, E) // 4, **f32)
         rc = lib.rd_obprop_beta_bwd(x.data_ptr(), p_t.data_ptr(), src_i.data_ptr(), tgt_i.data_ptr(), w.data_ptr(), E, N, T, d_ob,
                                     inc_w.data_ptr(), inc_b.data_ptr(), map_w.data_ptr(), val_w.data_ptr(), val_b.data_ptr(),
-                                    d_out.data_ptr(), L.ptr(d_alpha), d_x.data_ptr(), d_w.data_ptr(), d_pt.data_ptr(),
+                                    d_out.data_ptr(), L.ptr(d_alpha), L.ptr(d_x), d_w.data_ptr(), L.ptr(d_pt),
                                     g_iw.data_ptr(), g_ib.data_ptr(), g_mw.data_ptr(), g_vw.data_ptr(), g_vb.data_ptr(),
                                     sc.data_ptr(), L.stream_ptr(dev))
         L.check(rc, "rd_obprop_beta_bwd")
@@ -477,16 +507,19 @@ class ObPropBetaFunction(torch.autograd.Function):
 def obprop_beta(x, p_t, edge_index, edge_weights, d_ob, inc_w, inc_b, map_w, val_w, val_b):
     """Observation_progation.forward(use_beta=True) for one sample.  Returns (out [N, C], edge_index_pruned [2, K],
     alpha [K]); differentiable w.r.t. x, p_t, edge_weights and the five parameters."""
-    src_i, tgt_i = edge_index[0].contiguous().long(), edge_index[1].contiguous().long()
-
+    if _check_edges("obprop_beta", edge_index, edge_weights) < 2:
+        raise L.RaindropB200Error("obprop_beta: edge_index has E = %d edges, but use_beta keeps the top E // 2 of them "
+                                  "and needs E >= 2" % edge_index.shape[1])
+    src_i, tgt_i = edge_index[0].contiguous(), edge_index[1].contiguous()
     out, alpha, ei = ObPropBetaFunction.apply(x, p_t, edge_weights, src_i, tgt_i, d_ob, inc_w, inc_b, map_w, val_w, val_b)
     return out, ei, alpha
 
 
 def node_scale(edge_index, edge_weights, n_nodes):
     """s[n] = sum over incoming edges of the segment softmax (rd_node_scale)."""
+    _check_edges("node_scale", edge_index, edge_weights)
     lib = L.load()
-    tgt = edge_index[1].contiguous().long()
+    tgt = edge_index[1].contiguous()
     w = _as_f32(edge_weights)
     s = torch.empty(n_nodes, dtype=torch.float32, device=w.device)
     L.check(lib.rd_node_scale(tgt.data_ptr(), w.data_ptr(), tgt.numel(), n_nodes, s.data_ptr(), L.stream_ptr()),
@@ -546,13 +579,13 @@ class TransformerConvFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, edge_index, edge_weights, geom, heads, out_channels, wq, bq, wk, bk, wv, bv, ws, bs):
+        E = _check_edges("transformer_conv", edge_index, edge_weights)
+        n_nodes, n_graphs, node_stride, graph_stride = geom = _check_geom("transformer_conv", geom, x.shape[0])
         lib = L.load()
-        n_nodes, n_graphs, node_stride, graph_stride = geom
         x = _as_f32(x)
         rows, in_ch = x.shape
-        src_i = edge_index[0].contiguous().long()
-        tgt_i = edge_index[1].contiguous().long()
-        E = src_i.numel()
+        src_i = edge_index[0].contiguous()
+        tgt_i = edge_index[1].contiguous()
         ew = None if edge_weights is None else _as_f32(edge_weights)
         out = torch.empty(rows, heads * out_channels, dtype=torch.float32, device=x.device)
         alpha = torch.empty(n_graphs, E, heads, dtype=torch.float32, device=x.device)

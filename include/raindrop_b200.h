@@ -225,7 +225,8 @@ int rd_raindrop_v2_bwd(const rd_dims* dims, const rd_params* params, const float
  * [T, B, D = N*d_ob + d_pe] into the workspace buffer RD_WS_ENC_IN first (rd_workspace_offset), then calls _fwd;
  * _bwd fills every encoder / emb / mlp_static gradient of `grads` (the ob-prop members are ignored) and writes
  * d(loss)/d(encoder input) to d_enc_in [T, B, D].  Same workspace / scratch sizes and rng protocol as
- * rd_raindrop_v2_fwd / _bwd; grads may be NULL as there. */
+ * rd_raindrop_v2_fwd / _bwd; grads may be NULL as there.  As there, a training forward with Df = D + emb_dim > 722 (the
+ * head backward's limit) is refused before it writes anything or advances the rng counter. */
 int rd_encoder_head_fwd(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
                         uint64_t* rng_state, void* workspace, float* logits, const int64_t* y, float* loss,
                         float* d_logits, void* stream);

@@ -249,6 +249,47 @@ def encoder_layer_explicit(x, pad, p, nhead, eps=1e-5, masks=None, ffn_pre=None,
     return F.layer_norm(x1 + g, (D,), p["norm2.weight"], p["norm2.bias"], eps)
 
 
+def encoder_head_oracle(z0, static, lengths, params, nhead, eps=1e-5, masks=None, gates=None, stages=None, encoder=None):
+    """Temporal encoder + masked mean + head on a given encoder input: code/models_rd.py:354-385 (Raindrop_v2) and
+    :168-189 (legacy v1), what rd_encoder_head_fwd computes.
+
+    z0 [T, B, D] (any D = features + positional encoding); lengths [B]; static [B, d_static] or None (no emb branch);
+    params: state-dict keys -> tensors, "transformer_encoder.layers.<l>.<suffix>" (encoder_layer_explicit's suffixes;
+    the layer count is read from them), "emb.weight" [emb_dim, d_static] / "emb.bias" (any emb_dim) and
+    "mlp_static.{0,2}.{weight,bias}".  Post-LN layers with key-padding mask, pooled = sum of the valid rows /
+    (lengths + 1), cat emb(static), mlp_static written out (Linear, ReLU, Linear).
+    `masks`: one encoder_layer_explicit mask dict per layer (train mode with given dropout masks), or None (eval).
+    `gates` (optional dict, bool): "ffn" [[T*B, nhid]] * nlayers and "head" [B, Df], the ReLU decisions (relu_or_gate).
+    `stages` (optional dict) receives "enc" (the encoder output [T, B, D]), "ffn_pre" (one [T, B, nhid] linear1 output
+    per layer; empty when `encoder` is given) and "head_pre" (mlp_static.0 output [B, Df]).
+    `encoder` (optional callable (z0, pad) -> output) replaces the written-out layers, e.g. by the torch module."""
+    T, B = z0.shape[0], z0.shape[1]
+    g = gates or {}
+    pad = torch.arange(T, device=z0.device)[None, :] >= lengths.to(z0.device)[:, None]          # [B, T], True = padded
+    ffn_pre = []
+    if encoder is not None:
+        r = encoder(z0, pad)
+    else:
+        pre = "transformer_encoder.layers."
+        L = 1 + max(int(k[len(pre):].split(".")[0]) for k in params if k.startswith(pre))
+        masks = masks or [None] * L
+        ffn_gates = g.get("ffn") or [None] * L
+        assert len(masks) == L and len(ffn_gates) == L, (len(masks), len(ffn_gates), L)
+        r = z0
+        for l in range(L):
+            lp = "%s%d." % (pre, l)
+            p = {k[len(lp):]: v for k, v in params.items() if k.startswith(lp)}
+            r = encoder_layer_explicit(r, pad, p, nhead, eps, masks[l], ffn_pre, ffn_gates[l])
+    keep = (~pad).T[:, :, None].to(r.dtype)                                                        # [T, B, 1]
+    pooled = (r * keep).sum(0) / (lengths.to(z0.device)[:, None] + 1)
+    if static is not None:
+        pooled = torch.cat([pooled, F.linear(static, params["emb.weight"], params["emb.bias"])], dim=1)
+    h = F.linear(pooled, params["mlp_static.0.weight"], params["mlp_static.0.bias"])
+    if stages is not None:
+        stages.update(enc=r, ffn_pre=ffn_pre, head_pre=h.detach())
+    return F.linear(relu_or_gate(h, g.get("head")), params["mlp_static.2.weight"], params["mlp_static.2.bias"])
+
+
 # --------------------------------------------------------------------------------------------
 # Raindrop_v2 (code/models_rd.py:194-387)
 # --------------------------------------------------------------------------------------------
@@ -303,34 +344,29 @@ class RaindropV2Oracle(nn.Module):
             gs = torch.ones(self.d_inp, self.d_inp)
         return graph_from_adjacency(gs.float())
 
-    def _tail(self, obs, pe, static, lengths, pad, layer_masks=None, ffn_pre=None, gates=None, head_pre=None):
-        """code/models_rd.py:354-385: concat PE, temporal self-attention, masked mean, head.  With `layer_masks`
-        (one encoder_layer_explicit mask dict per layer) the layers run written out, with those dropout masks, and
-        append their FFN pre-activations to `ffn_pre` (a list) when one is given.  `gates` (forward_dense) gives the
-        decisions of the FFN ("ffn", written-out layers only) and head ("head") ReLUs; the head's pre-activation is
-        appended to `head_pre` (a list) when one is given."""
-        z = torch.cat([obs, pe], dim=2)
+    def _tail(self, obs, pe, static, lengths, layer_masks=None, ffn_pre=None, gates=None, head_pre=None):
+        """code/models_rd.py:354-385: concat PE, temporal self-attention, masked mean, head (encoder_head_oracle).
+        Without `layer_masks` the encoder is the torch module itself; with them (one encoder_layer_explicit mask dict
+        per layer) the layers run written out, with those dropout masks, and append their FFN pre-activations to
+        `ffn_pre` (a list) when one is given.  `gates` (forward_dense) gives the decisions of the FFN ("ffn",
+        written-out layers only) and head ("head") ReLUs; the head's pre-activation is appended to `head_pre` (a list)
+        when one is given.  The key-padding mask is built from `lengths`."""
         g = gates or {}
+        encoder = None
         if layer_masks is None:
             assert g.get("ffn") is None, "FFN gates need the written-out layers (masks)"
-            r = self.transformer_encoder(z, src_key_padding_mask=pad)
+            encoder = lambda z, pad_: self.transformer_encoder(z, src_key_padding_mask=pad_)
         else:
             assert len(layer_masks) == self.nlayers, (len(layer_masks), self.nlayers)
-            ffn_gates = g.get("ffn") or [None] * self.nlayers
-            r = z
-            for layer, lm, fg in zip(self.transformer_encoder.layers, layer_masks, ffn_gates):
-                r = encoder_layer_explicit(r, pad, dict(layer.named_parameters()), self.nhead, layer.norm1.eps, lm,
-                                           ffn_pre, fg)
-        keep = (~pad).T[:, :, None].to(r.dtype)                          # [T, B, 1]
-        pooled = (r * keep).sum(0) / (lengths[:, None] + 1)
-        if static is not None:
-            pooled = torch.cat([pooled, self.emb(static)], dim=1)
-        # mlp_static written out (Linear, ReLU, Linear: the same calls nn.Sequential makes) so that its ReLU can be gated
-        lin0, lin2 = self.mlp_static[0], self.mlp_static[2]
-        h = F.linear(pooled, lin0.weight, lin0.bias)
+        st = {}
+        logits = encoder_head_oracle(torch.cat([obs, pe], dim=2), static, lengths, dict(self.named_parameters()),
+                                     self.nhead, self.transformer_encoder.layers[0].norm1.eps, layer_masks, g, st,
+                                     encoder=encoder)
+        if ffn_pre is not None:
+            ffn_pre.extend(st["ffn_pre"])
         if head_pre is not None:
-            head_pre.append(h.detach())
-        return F.linear(relu_or_gate(h, g.get("head")), lin2.weight, lin2.bias), r
+            head_pre.append(st["head_pre"])
+        return logits, st["enc"]
 
     # -- the reference's own structure (what cpu_baseline times) ---------------------------------
     def forward(self, src, static, times, lengths, use_beta=False, stages=None):
@@ -338,7 +374,6 @@ class RaindropV2Oracle(nn.Module):
         N, d_ob = self.d_inp, self.d_ob
         h = self._lift(src)
         pe = positional_encoding(times, self.max_len).to(src.dtype)
-        pad = torch.arange(T)[None, :] >= lengths[:, None]                # :298-299
         edge_index, edge_w = self._graph()
         edge_w = edge_w.to(src.dtype)
         obs = torch.zeros(T, B, N * d_ob, dtype=src.dtype)
@@ -352,7 +387,7 @@ class RaindropV2Oracle(nn.Module):
             obs[:, b, :] = x.view(N, T, d_ob).permute(1, 0, 2).reshape(T, N * d_ob)
             alpha_all[:, b] = a2.reshape(-1)
         distance = torch.cdist(alpha_all.T, alpha_all.T, p=2).mean()      # :345-346
-        logits, r = self._tail(obs, pe, static, lengths, pad)
+        logits, r = self._tail(obs, pe, static, lengths)
         if stages is not None:
             stages.update(lift=h, pe=pe, obs=obs, enc=r, alpha_all=alpha_all)
         return logits, distance, None
@@ -389,7 +424,6 @@ class RaindropV2Oracle(nn.Module):
         h = self._lift(src, None if masks is None else masks["lift"])
         pe = positional_encoding(times, self.max_len).to(src.dtype)
         lengths = lengths.to(src.device)
-        pad = torch.arange(T, device=src.device)[None, :] >= lengths[:, None]
         edge_index, edge_w = self._graph()
         s = node_scale_from_graph(edge_index, edge_w, N, src.dtype).to(src.device)[None, :, None]   # [1, N, 1]
         x = h.reshape(T, B, N, d_ob).permute(1, 2, 0, 3).reshape(B, N, T * d_ob)
@@ -414,7 +448,7 @@ class RaindropV2Oracle(nn.Module):
         obs = h2.view(B, N, T, d_ob).permute(2, 0, 1, 3).reshape(T, B, N * d_ob)
         ffn_pre = [] if stages is not None and masks is not None else None
         head_pre = [] if stages is not None else None
-        logits, r = self._tail(obs, pe, static, lengths, pad, None if masks is None else masks["layers"], ffn_pre, g,
+        logits, r = self._tail(obs, pe, static, lengths, None if masks is None else masks["layers"], ffn_pre, g,
                                head_pre)
         if stages is not None:
             with torch.no_grad():

@@ -302,10 +302,18 @@ int head_fwd(int B, int T, int D, int N, int ds, int ncls, const float* x, const
   HeadP p = make(B, T, D, N, ds, ncls, statics, emb_w, emb_b, w0, b0, w2, b2, lengths);
   const int red = 8 * D > ncls ? 8 * D : ncls;
   const size_t smem = (size_t)(((2 * p.Df + 3) & ~3) + red) * sizeof(float);
-  if (smem > 48 * 1024) { set_error("head_fwd: feature width %d not supported", p.Df); return -2; }
+  auto kern = (D & 3) ? head_fwd_kernel<false> : head_fwd_kernel<true>;
+  // the 48 KB without opt-in hold the kernel's static shared memory (s_last) too
+  static size_t static_smem[2] = {~(size_t)0, ~(size_t)0};
+  size_t& st_smem = static_smem[(D & 3) ? 0 : 1];
+  if (st_smem == ~(size_t)0) {
+    cudaFuncAttributes attr;
+    if (cudaFuncGetAttributes(&attr, kern) != cudaSuccess) { set_error("head_fwd: cudaFuncGetAttributes failed"); return -1; }
+    st_smem = attr.sharedSizeBytes;
+  }
+  if (smem + st_smem > 48 * 1024) { set_error("head_fwd: feature width %d not supported", p.Df); return -2; }
   if (y && (!loss_ps || !dlogits || !loss || !counter)) { set_error("head_fwd: labels given without loss outputs"); return -2; }
-  launch_pdl((D & 3) ? head_fwd_kernel<false> : head_fwd_kernel<true>, dim3(B), dim3(HT), smem, st, p, x, feat, hpre, logits, y,
-             loss_ps, dlogits, loss, counter);
+  launch_pdl(kern, dim3(B), dim3(HT), smem, st, p, x, feat, hpre, logits, y, loss_ps, dlogits, loss, counter);
   RD_CHECK_LAUNCH("head_fwd_kernel");
   return 0;
 }

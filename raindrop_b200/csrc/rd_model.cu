@@ -613,7 +613,13 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
   Shape s;
   RD_TRY(make_shape(dims, &s));
   if (!encoder_only && (s.dpe != RD_D_PE || s.emb != s.N)) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (encoder_only) { s.tc = 0; s.exact = 0; }      // no observation propagation on this entry: no lin_value copies
+  // a training forward is followed by a backward: refuse before any output is written or the rng counter moves.  Monte
+  // Carlo replicates (rep_B > 0) are training forwards that no backward follows.
+  if (dims->training && rep_B == 0 && !head_bwd_supported(s.Df)) {
+    set_error("%s: training needs the head backward, feature width %d > 722", encoder_only ? "rd_encoder_head_fwd" : "rd_raindrop_v2_fwd",
+              s.Df);
+    return -2;
+  }
   if (s.ds > 0 && (!statics || !P->emb_weight || !P->emb_bias)) { set_error("static branch needs statics/emb"); return -2; }
   WsLayout w = ws_layout(s);
   uint64_t* rng = reinterpret_cast<uint64_t*>(ws + w.rng);
@@ -629,7 +635,9 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
   // Fast mode: tensor-core operands are kept exactly TF32-representable by their producers (lift, layer-1 epilogue,
   // rounded weight copies) so the MMA's operand truncation is exact.  Error-compensated mode (latency-bound row
   // counts): operands stay fp32, the weights come with their remainders, nothing is rounded.
-  const int tc = s.tc, exact = s.exact;
+  // No observation propagation on the encoder-only entry: no lin_value copies.  The workspace layout still follows the
+  // shape's own tc / exact, as rd_workspace_bytes / rd_workspace_offset and the backward compute it.
+  const int tc = encoder_only ? 0 : s.tc, exact = encoder_only ? 0 : s.exact;
   const float* W1 = P->ob1_value_weight; const float* W2 = P->ob2_value_weight;
   if (tc && !exact) { W1 = ws + w.W1r; W2 = ws + w.W2r; }   // rounded copies, produced by the weight-prep launch just below
   for (int l0 = 0; l0 < s.L; l0 += 3) {   // every derived weight tensor of the step in one launch (<= 16 tensors each)
@@ -1088,11 +1096,6 @@ int rd_raindrop_v2_fwd(const rd_dims* dims, const rd_params* params, const float
   if (!dims || !params || !src || !times || !lengths || !node_scale || !workspace || !logits) {
     set_error("rd_raindrop_v2_fwd: NULL argument");
     return -2;
-  }
-  if (dims->training) {       // a training forward is followed by a backward: refuse before any output is written
-    Shape s;
-    RD_TRY(make_shape(dims, &s));
-    if (!head_bwd_supported(s.Df)) { set_error("rd_raindrop_v2_fwd: training needs the head backward, feature width %d > 722", s.Df); return -2; }
   }
   return raindrop_fwd(dims, params, src, statics, times, lengths, node_scale, rng_state, (float*)workspace, logits,
                       y, loss, d_logits, 0, (cudaStream_t)stream);

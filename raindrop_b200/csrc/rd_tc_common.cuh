@@ -42,19 +42,22 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "WAIT_DONE:\n\t"
       "}" ::"r"(bar), "r"(parity) : "memory");
 }
+// non-blocking: has the phase of this parity completed?
+__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
+  uint32_t done;
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t"
+      "}" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+  return done != 0;
+}
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint32_t bar, uint32_t dst, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-// 16-byte asynchronous global -> shared copy; src_bytes < 16 zero-fills the rest (0: a zero vector, nothing is read)
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // ---- split of an fp32 operand for the error-compensated ("3xTF32") products ----------------------------------------
 // hi = the top 19 bits (exactly representable in TF32), lo = x - hi (exact).  hi*hi + hi*lo + lo*hi reproduces the fp32
 // product to ~2^-22 relative, independent of how the tensor core converts a raw fp32 bit pattern.

@@ -18,9 +18,9 @@
 //
 // tc_wgrad_group: dW = dY^T X (+ db) for up to WG_MAX problems in one launch.  Both operands are activations whose
 // contraction index runs over their ROWS; wgmma's TF32 form only reads K-major operands from shared memory, so dY^T is
-// gathered into registers from a row-major stage and X, delivered by TMA several k-blocks ahead, is transposed in shared
-// memory by a producer warpgroup into the K-major swizzled image wgmma reads (tc_wgrad_kernel below), followed by a
-// fixed-order split-K reduce.
+// gathered into registers from a row-major stage, and X is transposed in shared memory by a producer warpgroup into the
+// K-major swizzled image wgmma reads (tc_wgrad_kernel below); both arrive by TMA several k-blocks ahead.  A fixed-order
+// split-K reduce follows.
 #include <stdlib.h>
 
 #include "rd_tc_common.cuh"
@@ -283,16 +283,15 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 //   D_k[m, n] = sum_r A_k[r, m] * B_k[r, n]   (A = dY, B = X plus a "ones" column N for the bias gradient)
 // over one row split of problem k per work item (problem, m tile, n tile, split).  A training step has ten of these
 // (8 encoder weights + 2 lin_value).  Persistent: one CTA per SM walks the items blockIdx.x, + gridDim.x, ...
-//   warpgroup 2   producer, 128 threads.  Per 32-row k-block, issued nstages - 2 k-blocks ahead as soon as the stage
-//                 is released: the dY tile [32 x 128] by cp.async into a row-major stage (column XOR-ed with 8 (r % 4),
-//                 see wa_offset), completion tracked on the stage's full mbarrier; the raw X tile [32 x BN] by TMA
-//                 (32 x 32 boxes, 128B swizzle) into the stage's hi | lo region, on its own mbarrier.  When the
-//                 k-block's turn comes, the X tile is read into registers and TRANSPOSED into the K-major 128B-swizzled
-//                 images wgmma reads (sw128_offset(n, r)) as hi = top 19 bits and lo = exact remainder, with the ones
-//                 column written here (TMA cannot synthesise it).  Lane = row r and a warp's 32 stores share n, so
-//                 (((r >> 2) ^ n) & 7) * 4 + r % 4 hits 32 distinct banks.  fence.proxy.async, then arrive.
+//   warpgroup 2   producer, 128 threads.  Per 32-row k-block, issued by thread 256 alone nstages - 2 k-blocks ahead as
+//                 soon as the stage is released, all by TMA (32 x 32 boxes, 128B swizzle): the raw X tile [32 x BN] into
+//                 the stage's hi | lo region on the stage's xfull mbarrier, the dY tile [32 x 128] into the stage's
+//                 dY region on its full mbarrier.  When the k-block's turn comes, the X tile is read into registers and
+//                 TRANSPOSED into the K-major 128B-swizzled images wgmma reads (sw128_offset(n, r)) as hi = top 19 bits
+//                 and lo = exact remainder, one 16-byte store per 4 rows of one column, with the ones column written
+//                 here (TMA cannot synthesise it).  fence.proxy.async, then arrive.
 //   warpgroups    0 and 1: dW rows 0-63 and 64-127 of the tile, one wgmma.m64nBNk8 per k-step and term (lo.hi, hi.lo,
-//                 hi.hi) with A = dY^T gathered from the row-major stage (a transposed gather is addressing) and split in
+//                 hi.hi) with A = dY^T gathered from the swizzled row-major stage (a transposed gather is addressing) and split in
 //                 registers, exactly the tc_nt_kernel pipeline (one group in flight, two A-fragment buffers, a stage is
 //                 released only after the group that read it retired).  A warpgroup whose 64 rows lie past M waits and
 //                 releases the stages without MMAs.  Partial tiles go to slab [split][M][Nld] (Nld = N + 1 rounded up to 4).
@@ -300,20 +299,21 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 // widths dispatched per item inside one kernel, ptxas serialises the wgmma for lack of registers (C7512).
 // =================================================================================================
 struct WP {
-  const float* dY; long long ldy;    // X arrives through WGroup::tmX
-  float* partial;                    // [nsplit][M][Nld]
+  float* partial;                    // [nsplit][M][Nld]; dY and X arrive through WGroup::tmY / tmX
   int rows, M, N, Nld, n_tiles, m_tiles, nsplit, rows_per_split;
   int item0;                         // first work item of this problem inside the grouped list
 };
 struct WGroup {
   CUtensorMap tmX[WG_MAX];           // X of problem k: dims {Kin, rows}, boxes of 32 columns x 32 rows, 128B swizzle
+  CUtensorMap tmY[WG_MAX];           // dY of problem k: dims {Nout, rows}, boxes of 32 columns x 32 rows, 128B swizzle
   WP it[WG_MAX]; int n, total_items;
   unsigned long long* dbg;           // optional per-CTA phase cycles [CTA][16] (rd_debug_wgrad_timing)
 };
 
 // Phase timing of one CTA, clock64 deltas summed in registers and written once at the end when WGroup::dbg is set.
 // Slots: 0 / 1 clock64 at the start (after the grid dependency wait) / end of MMA thread 0; 2 / 3 / 4 the producer's
-// (thread 256) cycles waiting for an empty stage / for its X tile / transposing and storing; 5 / 6 MMA thread 0's cycles
+// (thread 256, which issues every TMA) cycles waiting for an empty stage (only when the k-block it is about to transpose
+// has not been issued) / for its X tile / transposing and storing; 5 / 6 MMA thread 0's cycles
 // waiting for a full stage / in the slab-store epilogue; 7 %globaltimer ns from start to end (the clock rate); 8 the
 // k-blocks the CTA produced; 9 clock64 at the producer's end; 10 the producer's cycles issuing the loads of a released
 // stage.
@@ -332,17 +332,8 @@ __host__ __device__ constexpr int w_nstages(int bn) { return (SMEM_LIMIT - 1280)
 // Tile widths the weight-gradient kernel is instantiated for (multiples of 8 up to MAX_BN)
 #define RD_WG_WIDTHS(X) X(32) X(64) X(96) X(128) X(144) X(160)
 
-// byte offset of element (r, m) of the staged dY tile: the fragment gathers read (r = 8ks + t (+4), m = arow + g (+8)),
-// so XOR-ing m with 8 (r % 4) = 8t spreads lanes (g, t) over 32 banks; 16-byte chunks stay contiguous for cp.async
-__device__ __forceinline__ uint32_t wa_offset(int r, int m) { return (uint32_t)(r * BM + (m ^ ((r & 3) << 3))) * 4u; }
-
-__device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-__device__ __forceinline__ float4 lds_v4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
+__device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
 struct WItem { int pi, n_t, m_t, split, k_blocks, r_begin, r_end; };
@@ -388,7 +379,18 @@ __device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRin
     }
     return;
   }
-  const int m0 = arow ^ (t << 3), m1 = (arow + 8) ^ (t << 3);     // the rows r of this thread's elements are = t (mod 4)
+  // The dY stage holds four TMA boxes of 32 rows x 32 columns m, 128B-swizzled: (r, m) at 4096 (m >> 5) +
+  // sw128_offset(r, m % 32), bank 4 ((((m % 32) >> 2) ^ r) & 7) + m % 4.  Lane (g, t) gathers m = arow + g (+8) at
+  // r = 8 ks + t (+4); arow % 32 = 16 w + g with w = wq % 2, and arow, arow + 8 share a box.  Read in the order
+  // (r, r + 4), the chunk index (4w + g/4 (+2)) ^ (t (+4)) would take 4 values over a warp (2-way conflicts).  So the
+  // lanes with g >= 4 (h = 1) read row r + 4 first: the chunk of the first load is (4w + h) ^ (t + 4h), whose bits are
+  // (h ^ t0, t1, w ^ h), a bijection of (h, t0, t1); with g % 4 as the word inside the chunk, 32 distinct banks.  The
+  // other three loads flip bit 1 (m + 8) and / or bit 2 (the other row), also bijections.  Selects put the values back.
+  const int h = (arow >> 2) & 1;
+  const uint32_t mbox = 4096u * (uint32_t)(arow >> 5);
+  const int mm = arow & 31, ra = t + 4 * h, rb = t + 4 - 4 * h;
+  const uint32_t o0 = mbox + sw128_offset(ra, mm), o1 = mbox + sw128_offset(ra, mm + 8);
+  const uint32_t o2 = mbox + sw128_offset(rb, mm), o3 = mbox + sw128_offset(rb, mm + 8);
   auto acquire = [&](uint32_t (&ah)[BK / 8][4], uint32_t (&al)[BK / 8][4]) {
     const long long c0 = clock64();
     mbar_wait(q.full(q.stage), q.phase);
@@ -396,9 +398,9 @@ __device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRin
     const uint32_t sa = q.addr(q.stage);
 #pragma unroll
     for (int ks = 0; ks < BK / 8; ++ks) {
-      const int r = ks * 8 + t;
-      const float x0 = lds_f32(sa + (uint32_t)(r * BM + m0) * 4u), x1 = lds_f32(sa + (uint32_t)(r * BM + m1) * 4u);
-      const float x2 = lds_f32(sa + (uint32_t)((r + 4) * BM + m0) * 4u), x3 = lds_f32(sa + (uint32_t)((r + 4) * BM + m1) * 4u);
+      const uint32_t sk = sa + 1024u * ks;     // rows + 8 ks: the swizzle depends on r % 8 only
+      const float v0 = lds_f32(sk + o0), v1 = lds_f32(sk + o1), v2 = lds_f32(sk + o2), v3 = lds_f32(sk + o3);
+      const float x0 = h ? v2 : v0, x1 = h ? v3 : v1, x2 = h ? v0 : v2, x3 = h ? v1 : v3;
       ah[ks][0] = tf32_hi(x0); ah[ks][1] = tf32_hi(x1); ah[ks][2] = tf32_hi(x2); ah[ks][3] = tf32_hi(x3);
       al[ks][0] = tf32_lo(x0); al[ks][1] = tf32_lo(x1); al[ks][2] = tf32_lo(x2); al[ks][3] = tf32_lo(x3);
     }
@@ -446,8 +448,9 @@ __device__ __forceinline__ void wgrad_consume(const WP& p, const WItem& it, WRin
 template <int BN>
 __global__ void __launch_bounds__(W_THREADS, 1)
 tc_wgrad_kernel(const __grid_constant__ WGroup g) {
-  constexpr int NQ = (BN / 4 + 3) / 4;      // X quads (4 columns) per producer thread and k-block
+  constexpr int NU = BN / 16;               // 4-row x 1-column chunks per producer thread and k-block
   constexpr int NBOX = (BN + 31) / 32;      // 32-column TMA boxes of X per k-block
+  static_assert(BN % 16 == 0, "the transpose covers the tile in groups of 16 columns");
   static_assert(NBOX * 4096 <= 2 * BN * 128, "the raw X boxes land in the stage's hi | lo images");
   static_assert(w_nstages(BN) >= 3, "the producer issues nstages - 2 k-blocks ahead of the one it transposes");
   extern __shared__ uint8_t smem_raw[];
@@ -459,8 +462,12 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
   q.bar_base = q.base + (uint32_t)(w_nstages(BN) * w_stage_bytes(BN));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 8 && lane == 0) {
-    for (int k = 0; k < g.n; ++k) asm volatile("prefetch.tensormap [%0];" ::"l"(&g.tmX[k]) : "memory");
-    for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(q.full(s), 128); mbar_init(q.empty(s), 8); mbar_init(q.xfull(s), 1); }
+    for (int k = 0; k < g.n; ++k) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&g.tmX[k]) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&g.tmY[k]) : "memory");
+    }
+    // full: the 128 transposing threads + the issuing thread's expect_tx for dY
+    for (int s = 0; s < MAX_STAGES; ++s) { mbar_init(q.full(s), 129); mbar_init(q.empty(s), 8); mbar_init(q.xfull(s), 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -475,35 +482,32 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
     const int pt = threadIdx.x - 256, pw = warp - 8;
     const int total = g.total_items;
     long long t_empty = 0, t_x = 0, t_store = 0, t_issue = 0, n_kb = 0;
-    // Two cursors walk the same (item, k-block) sequence.  The issue cursor sends a k-block's loads into its stage as
-    // soon as the MMA warpgroups release it: dY by cp.async (completion on the stage's full barrier), X by TMA (on the
-    // stage's xfull barrier).  It runs nstages - 2 k-blocks ahead of the transpose cursor: the stage one further ahead
-    // is released only after the consumers acquired the k-block being transposed.  The work item of each cursor is
-    // computed once per item: the walk over the group's problems reads kernel parameters at a register index.
+    // Two cursors walk the same (item, k-block) sequence.  The issue cursor, thread 256 alone, sends a k-block's loads
+    // into its stage as soon as the MMA warpgroups release it, all by TMA: X (NBOX boxes) on the stage's xfull
+    // barrier, then dY (four boxes of 32 rows x 32 columns, 128B swizzle, see wgrad_consume) on its full barrier.  It
+    // runs up to nstages - 2 k-blocks ahead of the transpose cursor, but waits for a release only when the k-block
+    // about to be transposed is not issued yet: so the transposes run ahead as far as the ring allows instead of
+    // waiting, every k-block, for the consumers to retire the group of two k-blocks back.  The work item of each
+    // cursor is computed once per item: the walk over the group's problems reads kernel parameters at a register index.
     int iw = blockIdx.x, ikb = 0, istage = 0, ahead = 0;
     uint32_t iphase = 0;
     WItem iit = wgrad_item(g, iw);
     auto issue = [&]() {
-      const WP& p = g.it[iit.pi];
       const long long c0 = clock64();
       mbar_wait(q.empty(istage), iphase ^ 1u);
       const long long c1 = clock64();
       t_empty += c1 - c0;
       const uint32_t sa = q.addr(istage);
-      const int r0 = iit.r_begin + ikb * BK, mc0 = iit.m_t * BM;
-      if (pt == 0) {      // rows past `rows` and columns past Kin arrive as zeros
-        mbar_expect_tx(q.xfull(istage), NBOX * 4096u);
+      const int r0 = iit.r_begin + ikb * BK;
+      // rows past `rows`, columns past Kin and m past Nout arrive as zeros
+      mbar_expect_tx(q.xfull(istage), NBOX * 4096u);
 #pragma unroll
-        for (int b = 0; b < NBOX; ++b)
-          tma_load_2d(&g.tmX[iit.pi], q.xfull(istage), sa + (uint32_t)WA_TILE + 4096u * b, iit.n_t * BN + 32 * b, r0);
-      }
+      for (int b = 0; b < NBOX; ++b)
+        tma_load_2d(&g.tmX[iit.pi], q.xfull(istage), sa + (uint32_t)WA_TILE + 4096u * b, iit.n_t * BN + 32 * b, r0);
+      mbar_expect_tx(q.full(istage), (uint32_t)WA_TILE);
 #pragma unroll
-      for (int j = 0; j < BK * BM / 4 / 128; ++j) {
-        const int v = pt + 128 * j, r = v >> 5, c = (v & 31) * 4;
-        const bool ok = r0 + r < iit.r_end && mc0 + c < p.M;
-        cp_async16(sa + wa_offset(r, c), ok ? p.dY + (long long)(r0 + r) * p.ldy + mc0 + c : p.dY, ok ? 16u : 0u);
-      }
-      asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(q.full(istage)) : "memory");
+      for (int b = 0; b < BM / 32; ++b)
+        tma_load_2d(&g.tmY[iit.pi], q.full(istage), sa + 4096u * b, iit.m_t * BM + 32 * b, r0);
       if (++istage == q.nstages) { istage = 0; iphase ^= 1u; }
       t_issue += clock64() - c1;
       if (++ikb == iit.k_blocks) {
@@ -512,46 +516,54 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
       }
     };
     // The transpose cursor: the raw X tile (NBOX boxes of 32 rows x 32 columns, 128B-swizzled, at the start of the
-    // stage's hi image) -> registers, row r = lane and quads pw, pw + 4, ... of the n tile (a quarter warp's 16-byte
-    // loads hit 8 distinct chunks of 8 rows: conflict-free), with the ones column N of the bias gradient set here ->
-    // hi / lo images.
+    // stage's hi image; (r, n) at 4096 (n >> 5) + sw128_offset(r, n % 32)) -> registers, with the ones column N of the
+    // bias gradient set here -> the K-major images, one 16-byte store per chunk of rows 4a .. 4a + 3 of one image row n
+    // (sw128_offset(n, 4a)) for hi and one for lo.  Lane = 8c + a, c = lane / 8, a = lane % 8, of warp pw holds, per
+    // 16-column group i < BN / 16, column n = 16 i + 4 cq + c with cq = (a >> 1) ^ pw, rows 4a .. 4a + 3: over the four
+    // warps every (n, a) of the group once.  It reads them with four scalar loads (no shuffles; as many shared-memory
+    // wavefronts as one 16-byte load per row).
+    //   load j (row 4a + j): chunk ((n % 32) >> 2) ^ (4a + j) = (4 (i % 2) + cq) ^ (4 (a % 2) + j), bits 0-1
+    //     (a >> 1) ^ pw ^ j and bit 2 (i % 2) ^ (a % 2): a bijection of a; word c inside the chunk -> 32 banks.
+    //   16-byte store: a quarter warp is one c and a = 0..7; the chunk (a ^ n) % 8 with n % 8 = 4 (cq % 2) + c has bits
+    //     0-1 (a ^ c) % 4 and bit 2 a2 ^ a1 ^ pw0 ^ c2 (c2 = 0): a bijection of a -> 8 distinct chunks, conflict-free.
+    const int a = lane & 7, c = lane >> 3, cq = (a >> 1) ^ pw;
+    uint32_t ld_off[2][4];        // raw X: group i reads box i >> 1 at ld_off[i % 2][j]
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) ld_off[e][j] = sw128_offset(4 * a + j, 16 * e + 4 * cq + c);
+    const uint32_t st_off = sw128_offset(4 * cq + c, 4 * a);     // image: + 2048 i (16 rows of 128 bytes per group)
     int w = blockIdx.x, kb = 0;
     WItem it = iit;
     while (w < total) {
-      for (; ahead < q.nstages - 1 && iw < total; ++ahead) issue();
+      // only the k-block about to be transposed has to be issued now (ahead == 0); the stages further ahead are issued
+      // if already released
+      if (pt == 0)
+        for (; ahead < q.nstages - 1 && iw < total; ++ahead) {
+          if (ahead > 0 && !mbar_test(q.empty(istage), iphase ^ 1u)) break;
+          issue();
+        }
       const WP& p = g.it[it.pi];
       const long long c0 = clock64();
       mbar_wait(q.xfull(q.stage), q.phase);
       const long long c1 = clock64();
       const uint32_t sb = q.addr(q.stage) + (uint32_t)WA_TILE, sl = sb + (uint32_t)BN * 128u;
-      const int r = it.r_begin + kb * BK + lane, nq = BN / 4, c0n = it.n_t * BN;
-      float4 xv[NQ];
+      const int r = it.r_begin + kb * BK + 4 * a, ones = p.N - it.n_t * BN - 4 * cq - c;     // ones: 16 i of column N
+      float xv[NU][4];
 #pragma unroll
-      for (int i = 0; i < NQ; ++i) {
-        const int qd = pw + 4 * i;
-        xv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (qd < nq) {
-          xv[i] = lds_v4(sb + 4096u * (uint32_t)(qd >> 3) + sw128_offset(lane, 4 * (qd & 7)));
-          if (c0n + 4 * qd == p.N && r < it.r_end) xv[i].x = 1.f;
+      for (int i = 0; i < NU; ++i) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          xv[i][j] = lds_f32(sb + 4096u * (uint32_t)(i >> 1) + ld_off[i & 1][j]);
+          if (16 * i == ones && r + j < it.r_end) xv[i][j] = 1.f;
         }
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");        // every raw read is done before the images overwrite it
-      // image row n = 4 qd + k = 4 pw + k + 16 i: the swizzle term depends on n % 8 only, so the offsets of quad i are
-      // those of quad 0 plus 16 i rows (keeps 4 address registers live instead of 4 NQ)
-      uint32_t off[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) off[k] = sw128_offset(4 * pw + k, lane);
-#pragma unroll
-      for (int i = 0; i < NQ; ++i) {
-        const int qd = pw + 4 * i;
-        if (qd < nq) {
-          const float e[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            sts_f32(sb + off[k] + 2048u * i, __uint_as_float(tf32_hi(e[k])));
-            sts_f32(sl + off[k] + 2048u * i, __uint_as_float(tf32_lo(e[k])));
-          }
-        }
+      for (int i = 0; i < NU; ++i) {
+        const uint32_t o = st_off + 2048u * i;
+        sts_v4(sb + o, tf32_hi(xv[i][0]), tf32_hi(xv[i][1]), tf32_hi(xv[i][2]), tf32_hi(xv[i][3]));
+        sts_v4(sl + o, tf32_lo(xv[i][0]), tf32_lo(xv[i][1]), tf32_lo(xv[i][2]), tf32_lo(xv[i][3]));
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> wgmma's reads
       mbar_arrive(q.full(q.stage));
@@ -971,12 +983,14 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
     WP& p = g.it[k];
     p.partial = a.partial;
     p.rows = (int)a.rows; p.M = a.Nout; p.N = a.Kin; p.Nld = w.Nld;
-    p.dY = a.dY; p.ldy = a.ldy;
     {
       cuuint64_t d[2] = {(cuuint64_t)a.Kin, (cuuint64_t)a.rows};
       cuuint64_t s[1] = {(cuuint64_t)a.ldx * 4};
       cuuint32_t b[2] = {BK, BK};
       RD_TRY(encode(&g.tmX[k], a.X, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "X"));
+      cuuint64_t dy[2] = {(cuuint64_t)a.Nout, (cuuint64_t)a.rows};
+      cuuint64_t sy[1] = {(cuuint64_t)a.ldy * 4};
+      RD_TRY(encode(&g.tmY[k], a.dY, 2, dy, sy, b, CU_TENSOR_MAP_SWIZZLE_128B, "dY"));
     }
     p.n_tiles = (int)ceil_div(a.Kin + 1, BN); p.m_tiles = (int)ceil_div(a.Nout, BM);
     p.nsplit = w.nsplit; p.rows_per_split = w.rows_per_split;

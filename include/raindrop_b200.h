@@ -234,7 +234,8 @@ int rd_encoder_head_bwd(const rd_dims* dims, const rd_params* params, const floa
                         const void* workspace, const float* d_logits, const rd_grads* grads, void* scratch,
                         float* d_enc_in, void* stream);
 /* ---- gradients with respect to the inputs src, static and times ----------------------------------------------
- * For saliency maps, integrated gradients and other attribution methods, and for adversarial training.  Call it
+ * For saliency maps, integrated gradients and other attribution methods, and for adversarial examples (the batched
+ * attack is rd_raindrop_v2_pgd).  Call it
  * after rd_raindrop_v2_bwd (phases including RD_BWD_OBPROP) or rd_encoder_head_bwd, on the same stream, with the
  * same dims / params, the forward's workspace and the backward's scratch `bwd_scratch` untouched in between: the
  * backward leaves d(loss)/d(encoder input), d(loss)/d(layer-1 pre-activation) and d(loss)/d(cat(pooled, emb)) there,
@@ -381,6 +382,50 @@ int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, cons
                               const float* times, const int64_t* lengths, const float* node_scale, const uint64_t* rng,
                               int32_t n_samples, int32_t replicates_per_chunk, void* scratch, float* mean_probs,
                               float* variance, float* entropies, float* samples, void* stream);
+
+/* ---- PGD adversarial examples of Raindrop_v2, in one call ------------------------------------------------------------
+ * Untargeted projected gradient descent (Madry et al. 2018) on each sample's own cross-entropy CE(logits_b, y_b) (y NULL:
+ * the argmax class of logits_clean), so a sample's result depends on neither B nor the chunking.
+ * Threat model: only the value half of src is perturbed, and only at observed cells (src[t, b, N + n] > 0; padded rows
+ * have mask 0) of sensors with sensor_perturbable[n] != 0 (NULL: every sensor) of samples with sample_attacked[b] != 0
+ * (NULL: every sample); with perturb_static also the statics of those samples.  These elements form S_b.  The mask half,
+ * times and lengths never change.  eps is in the units the model sees (per-feature standard deviations after
+ * normalisation).  norm RD_PGD_LINF: |delta| <= eps per element; RD_PGD_L2: ||delta_b||_2 <= eps over S_b.
+ * Iterates x_k = x + delta_k (an element with delta == 0 keeps x bit for bit):
+ *   start   delta_0 = 0; random_start: linf delta_0 ~ U(-eps, eps) per element, l2 uniform in the ball
+ *           eps r^(1/d) z / ||z|| (z ~ N(0, I) over S_b, r ~ U(0, 1), d = |S_b|), drawn from Philox4x32-10 at site 98
+ *           under rng = {seed, step} (device uint64[2], read only): element e of sample b (e = t*N + n for value cells,
+ *           T*N + j for statics) at index b*(T*N + d_static + 1) + e, r at b*(T*N + d_static + 1) + T*N + d_static; the
+ *           word of index i is word i & 3 of the block at counter i >> 2 (as for dropout), uniforms (word >> 8) 2^-24,
+ *           normals by Box-Muller on the block's word pairs as rd_dp_add_noise draws them
+ *   step k  g = d CE(logits_b, y_b) / d x at x_k; linf: delta = clip(delta + alpha sign(g), -eps, eps) (fp32);
+ *           l2: delta += alpha g / ||g|| (no step when ||g|| = 0), delta *= min(1, eps / ||delta||) (norms in fp64)
+ * Returned per sample: the iterate of highest loss among x_0 .. x_{n_steps} (ties: the earliest), so without a random
+ * start loss_adv >= CE at x.  FGSM is n_steps = 1, alpha = eps, random_start = 0.  The lift relu(v R_u) has gradient 0 at
+ * a cell whose d_ob channels are all inactive (d_ob = 1: every value of the wrong sign), so such a cell does not move
+ * from delta_0 = 0; random_start avoids that.
+ *   src_adv      [T, B, 2N]: the returned input (the mask half and every element outside S_b copied bit for bit)
+ *   statics_adv  [B, d_static] or NULL (skipped)
+ *   logits_adv   [B, n_classes] at src_adv;  loss_adv [B] its cross-entropy (fp64 rounded to fp32)
+ *   logits_clean [B, n_classes] at x
+ * Eval arithmetic (dims->training must be 0): no dropout, the model's rng state is neither read nor advanced, no
+ * parameter gradient is written.  Work: chunks of samples_per_chunk samples; per chunk the inputs expanded in one
+ * launch, the forward at x, with random_start one launch drawing x_0 and its forward, then per step the
+ * frozen-parameter backward, the dX0 GEMM, one step launch and the next forward, and after every forward one launch
+ * that takes the loss and keeps the best iterate: n_steps + 1 (+1 with random_start) forwards and n_steps backwards.
+ * Per-sample kernels are one CTA per sample with fixed-order fp64 sums (no atomics): bitwise independent of the
+ * chunking.  dims->obprop_mode 0 is resolved once from samples_per_chunk rows, so a shorter last chunk uses the same
+ * arithmetic.  scratch: rd_pgd_scratch_bytes(dims, samples_per_chunk) bytes.  Stream-ordered, allocation- and
+ * sync-free, CUDA-graph capturable. */
+#define RD_PGD_LINF 0
+#define RD_PGD_L2 1
+size_t rd_pgd_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk);
+int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                       const float* times, const int64_t* lengths, const float* node_scale, const int64_t* y,
+                       const uint8_t* sensor_perturbable, const uint8_t* sample_attacked, int32_t perturb_static,
+                       int32_t norm, float eps, float alpha, int32_t n_steps, int32_t random_start, const uint64_t* rng,
+                       int32_t samples_per_chunk, void* scratch, float* src_adv, float* statics_adv, float* logits_adv,
+                       float* logits_clean, float* loss_adv, void* stream);
 
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */

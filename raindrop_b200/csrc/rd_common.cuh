@@ -129,6 +129,15 @@ __device__ __forceinline__ float4 dropout_scale4(const RngKey& k, uint32_t site,
                      keep_scale(b.w, p, inv_keep));
 }
 
+// Two standard normals from two Philox words: u1 = ((a >> 8) + 1) 2^-24, u2 = (b >> 8) 2^-24, r = sqrt(-2 ln u1),
+// (r cos(2 pi u2), r sin(2 pi u2)) in fp64, rounded to fp32.
+__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float* z0, float* z1) {
+  const double u1 = ((double)(a >> 8) + 1.0) * (1.0 / 16777216.0), u2 = (double)(b >> 8) * (1.0 / 16777216.0);
+  const double r = sqrt(-2.0 * log(u1)), t = 6.283185307179586 * u2;
+  *z0 = (float)(r * cos(t));
+  *z1 = (float)(r * sin(t));
+}
+
 // ---- Monte Carlo dropout replicates in one forward ------------------------------------------------------------------
 // A forward over Bc = cc*B rows, replicate-major (row j = m*B + b), in which row j draws exactly the words that the
 // B-row forward at step (step + m) draws for row b.  Every site's index space is [T, Bc, width] (attention: T = 1,
@@ -154,6 +163,19 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// Sum of v over the CTA in a fixed order (butterfly within each warp, then the warps in order): deterministic.  red holds
+// blockDim.x / 32 doubles; every thread returns the sum.
+__device__ __forceinline__ double block_sum_fixed(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  double s = 0.0;
+  for (int w = 0; w < nw; ++w) s += red[w];
+  return s;
 }
 
 // ---- generic fp32 GEMM with a fused epilogue (rd_gemm.cu) ------------------------------------

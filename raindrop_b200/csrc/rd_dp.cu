@@ -20,17 +20,6 @@ namespace {
 
 constexpr int DP_TILE = 64, DP_BK = 16, DP_THREADS = 256, DP_SMEM_LD = DP_TILE + 4;
 
-__device__ __forceinline__ double block_sum_fixed(double v, double* red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < nw; ++w) s += red[w];
-  return s;
-}
-
 // dst[k][m] = P[(m0 + m) * ms + k0 + k] for m0 + m < mlim, k0 + k < klim, else 0 (rows contiguous along k)
 __device__ __forceinline__ void load_rows(float (*dst)[DP_SMEM_LD], const float* __restrict__ P, long long ms, int m0,
                                           int mlim, int k0, int klim) {
@@ -265,13 +254,6 @@ __global__ void __launch_bounds__(DP_THREADS) dp_clip_kernel(const double* __res
 // SITE_DP_NOISE, block i >> 2, Box-Muller on the block's word pairs (x, y) -> elements 4q, 4q+1 and (z, w) -> 4q+2, 4q+3:
 //   u1 = ((w0 >> 8) + 1) 2^-24, u2 = (w1 >> 8) 2^-24, r = sqrt(-2 ln u1), (r cos(2 pi u2), r sin(2 pi u2)) in fp64,
 // rounded to fp32.  key = {seed, step, ticket}: the last CTA to finish advances step (and resets the ticket).
-__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float* z0, float* z1) {
-  const double u1 = ((double)(a >> 8) + 1.0) * (1.0 / 16777216.0), u2 = (double)(b >> 8) * (1.0 / 16777216.0);
-  const double r = sqrt(-2.0 * log(u1)), t = 6.283185307179586 * u2;
-  *z0 = (float)(r * cos(t));
-  *z1 = (float)(r * sin(t));
-}
-
 __global__ void __launch_bounds__(DP_THREADS) dp_noise_kernel(float* __restrict__ g, long long n4, const __grid_constant__ DpFields fl,
                                                               float stdv, uint64_t* __restrict__ key) {
   pdl_launch_dependents();

@@ -293,37 +293,6 @@ struct InputGradArgs {
   const float* times; const float* g_pe; long long n_tokens, ld; int col0; const int64_t* lengths; float* d_times;
   const float* dfeat; const float* W_emb; int Df, feat_col0, emb, ds; float* d_static; long long n_static;
 };
-// The lift backward of one (sample, t, sensor n) with value sv: sum_k g[k] * keep_k/(1-p) * [sv*R_u[n*d_ob+k] > 0] *
-// R_u[n*d_ob+k], g = d(loss)/d(X0) of that (row, t); idx0 = the forward's dropout element index of channel 0
-__device__ __forceinline__ float lift_bwd(float sv, const float* __restrict__ R_u, const float* __restrict__ g, int n,
-                                          int d_ob, float drop_p, const uint64_t* __restrict__ rng, uint64_t idx0) {
-  const float ik = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
-  float acc = 0.f;
-  if (d_ob == 4) {
-    const float4 r = __ldg(reinterpret_cast<const float4*>(R_u) + n);
-    float4 d = __ldg(reinterpret_cast<const float4*>(g));
-    if (drop_p > 0.f) {
-      const float4 m = dropout_scale4(rng, SITE_LIFT, idx0, drop_p, ik);
-      d.x *= m.x; d.y *= m.y; d.z *= m.z; d.w *= m.w;
-    }
-    acc = (sv * r.x > 0.f ? d.x * r.x : 0.f) + (sv * r.y > 0.f ? d.y * r.y : 0.f) +
-          (sv * r.z > 0.f ? d.z * r.z : 0.f) + (sv * r.w > 0.f ? d.w * r.w : 0.f);
-  } else {
-    for (int k = 0; k < d_ob; ++k) {
-      const float r = __ldg(R_u + n * d_ob + k);
-      float d = __ldg(g + k);
-      if (drop_p > 0.f) d *= dropout_scale(rng, SITE_LIFT, idx0 + k, drop_p, ik);
-      acc += sv * r > 0.f ? d * r : 0.f;
-    }
-  }
-  return acc;
-}
-// d(loss)/d(static[b, k]) = sum_n df[n] * W_emb[n*ds + k], df = d(loss)/d(emb output) of sample b
-__device__ __forceinline__ float emb_bwd(const float* __restrict__ df, const float* __restrict__ W_emb, int emb, int ds, int k) {
-  float acc = 0.f;
-  for (int n = 0; n < emb; ++n) acc = fmaf(__ldg(df + n), __ldg(W_emb + (long long)n * ds + k), acc);
-  return acc;
-}
 __global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const __grid_constant__ TS8 ts) {
   pdl_launch_dependents();
   pdl_wait();

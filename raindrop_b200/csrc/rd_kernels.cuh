@@ -46,6 +46,38 @@ int input_grad(const float* src, const float* R_u, const float* dX0, int B, int 
                const float* ts_host, int d_pe, const int64_t* lengths, float* d_times, const float* dfeat, int Df, int feat_col0,
                const float* W_emb, int emb, int ds, float* d_static, cudaStream_t st);
 
+// The lift backward of one (sample, t, sensor n) with value sv: sum_k g[k] * keep_k/(1-p) * [sv*R_u[n*d_ob+k] > 0] *
+// R_u[n*d_ob+k], g = d(loss)/d(X0) of that (row, t); idx0 = the forward's dropout element index of channel 0
+__device__ __forceinline__ float lift_bwd(float sv, const float* __restrict__ R_u, const float* __restrict__ g, int n,
+                                          int d_ob, float drop_p, const uint64_t* __restrict__ rng, uint64_t idx0) {
+  const float ik = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  float acc = 0.f;
+  if (d_ob == 4) {
+    const float4 r = __ldg(reinterpret_cast<const float4*>(R_u) + n);
+    float4 d = __ldg(reinterpret_cast<const float4*>(g));
+    if (drop_p > 0.f) {
+      const float4 m = dropout_scale4(rng, SITE_LIFT, idx0, drop_p, ik);
+      d.x *= m.x; d.y *= m.y; d.z *= m.z; d.w *= m.w;
+    }
+    acc = (sv * r.x > 0.f ? d.x * r.x : 0.f) + (sv * r.y > 0.f ? d.y * r.y : 0.f) +
+          (sv * r.z > 0.f ? d.z * r.z : 0.f) + (sv * r.w > 0.f ? d.w * r.w : 0.f);
+  } else {
+    for (int k = 0; k < d_ob; ++k) {
+      const float r = __ldg(R_u + n * d_ob + k);
+      float d = __ldg(g + k);
+      if (drop_p > 0.f) d *= dropout_scale(rng, SITE_LIFT, idx0 + k, drop_p, ik);
+      acc += sv * r > 0.f ? d * r : 0.f;
+    }
+  }
+  return acc;
+}
+// d(loss)/d(static[b, k]) = sum_n df[n] * W_emb[n*ds + k], df = d(loss)/d(emb output) of sample b
+__device__ __forceinline__ float emb_bwd(const float* __restrict__ df, const float* __restrict__ W_emb, int emb, int ds, int k) {
+  float acc = 0.f;
+  for (int n = 0; n < emb; ++n) acc = fmaf(__ldg(df + n), __ldg(W_emb + (long long)n * ds + k), acc);
+  return acc;
+}
+
 // Integrated gradients along the straight path x0 + alpha (x - x0), chunks of m steps on B*m rows, step-major (j = k*B + b).
 // ig_expand: the chunk's inputs src_e [T, B*m, 2N] (value half interpolated, mask half copied from src), statics_e,
 // times_e, lengths_e and one-hot d_logits [B*m, ncls] of target[b] (target == nullptr: argmax of logits_x [B, ncls];
@@ -101,6 +133,30 @@ int mc_expand(const float* src, const float* statics, const float* times, const 
 // ent [3, B] = (predictive entropy, expected entropy, mutual information) over all M replicates.
 int mc_accumulate(const float* logits, int nc, int B, int ncls, int64_t m0, int64_t M, double* acc, float* samples,
                   float* mean, float* var, float* ent, int first, int last, cudaStream_t st);
+
+// ---- PGD adversarial examples (rd_adversarial.cu; rd_raindrop_v2_pgd) ----------------------------------------------
+// A chunk of m samples c0 .. c0+m-1 of a B-sample batch on m rows: the chunk's input buffers x_e [T, m, 2N], st_e [m, ds]
+// (ds = 0: NULL), times_e [T, m], len_e [m], the perturbation delta and the l2 gradient buffer grad [m, T*N + ds].
+// sens [N] / attacked [B] (uint8, NULL = all) and pst (perturb the statics) select the perturbable elements.
+constexpr uint32_t SITE_PGD_START = 98;     // Philox site of the random start (its key is the attack key {seed, step})
+struct PgdArgs {
+  const float* src; const float* statics; const float* times; const int64_t* lengths;
+  const uint8_t* sens; const uint8_t* attacked;
+  float* x_e; float* st_e; float* times_e; int64_t* len_e; float* delta; float* grad;
+  int B, T, N, ds, m, c0, pst;
+};
+// the chunk's inputs copied from the batch, delta = 0
+int pgd_expand(const PgdArgs& a, cudaStream_t st);
+// delta_0 drawn at key {seed, step} (device uint64[2]) and x_0 = x + delta_0 into x_e / st_e; one CTA per sample
+int pgd_start(const PgdArgs& a, int norm, float eps, const uint64_t* key, cudaStream_t st);
+// per-sample fp64 cross-entropy of logits [m, ncls] (label y[b], y == NULL: argmax of logits_clean [B, ncls]),
+// d_logits [m, ncls] = softmax - onehot, and when it beats best[j] (first: always) the iterate's src / statics / logits
+// rows and loss copied out to the batch-wide outputs (st_adv may be NULL)
+int pgd_track(const PgdArgs& a, int ncls, const float* logits, const float* logits_clean, const int64_t* y, double* best,
+              int first, float* dlogits, float* src_adv, float* st_adv, float* logits_adv, float* loss_adv, cudaStream_t st);
+// the step from dX0 [m*N, T*d_ob] and dfeat [m, Df] (statics gradient from columns D .. D+emb through W_emb [emb, ds])
+int pgd_step(const PgdArgs& a, int norm, float eps, float alpha, const float* R_u, int d_ob, const float* dX0,
+             const float* dfeat, int Df, int D, const float* W_emb, int emb, cudaStream_t st);
 
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 

@@ -340,6 +340,41 @@ int ig_layout(const rd_dims* dims, int mc, IgcLayout* l) {
   return 0;
 }
 
+// ---- PGD adversarial examples ---------------------------------------------------------------------------------------
+// A chunk of m <= spc samples runs on m rows in the arithmetic pinned from spc rows (ig_dims with one step per chunk).
+rd_dims pgd_dims(const rd_dims* d, int rows, int spc) {
+  rd_dims e = *d;
+  e.B = spc;
+  return ig_dims(&e, rows, 1);
+}
+// Scratch of rd_raindrop_v2_pgd: the forward workspace and backward scratch of spc rows, W1^T with its remainder, dX0,
+// the chunk's inputs, logits and d_logits, the perturbation and l2 gradient [spc, T*N + ds] and the best losses (fp64).
+struct PgdLayout { int64_t ws, sc, W1t, W1tlo, dX0, src, statics, times, lengths, logits, dlogits, delta, grad, best, total; };
+int pgd_layout(const rd_dims* dims, int spc, PgdLayout* l) {
+  if (spc < 1 || spc > (1 << 30)) { set_error("samples_per_chunk = %d out of range", spc); return -2; }
+  const rd_dims dc = pgd_dims(dims, spc, spc);
+  Shape s;
+  RD_TRY(make_shape(&dc, &s));
+  const int64_t E = (int64_t)s.T * s.N + s.ds;
+  Arena a;
+  l->ws = a.take(ws_layout(s).total);
+  l->sc = a.take(bw_layout(s).total);
+  l->W1t = a.take((int64_t)s.C * s.C);
+  l->W1tlo = a.take((int64_t)s.C * s.C);
+  l->dX0 = a.take(s.M1 * s.C);
+  l->src = a.take(s.M2 * 2 * s.N);
+  l->statics = a.take((int64_t)spc * s.ds);
+  l->times = a.take(s.M2);
+  l->lengths = a.take(2LL * spc);
+  l->logits = a.take((int64_t)spc * s.ncls);
+  l->dlogits = a.take((int64_t)spc * s.ncls);
+  l->delta = a.take(spc * E);
+  l->grad = a.take(spc * E);
+  l->best = a.take(2LL * spc);
+  l->total = a.off;
+  return 0;
+}
+
 // ---- coalition attribution (Shapley-value sampling, ablation) -------------------------------------------------------
 // Scratch of rd_raindrop_v2_coalition_attribution and rd_raindrop_v2_cell_coalition_attribution: the eval forward
 // workspace and the expanded inputs of max(B*cc, 2B) rows (chunks of cc coalitions and the endpoint forward), the
@@ -1226,6 +1261,94 @@ int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* pa
     RD_TRY(ig_accumulate(src, baseline_src, alphas + c0, weights + c0, m, B, s.T, s.N, s.dob, params->R_u, dX0, S + l.acc_src,
                          attr_src, statics, baseline_statics, sc + b.dfeat, s.Df, s.D, params->emb_weight, s.emb, s.ds,
                          S + l.acc_static, attr_st, c0 == 0, c0 + m >= n_steps, st));
+  }
+  return 0;
+}
+
+size_t rd_pgd_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk) {
+  if (!dims) return 0;
+  PgdLayout l;
+  if (pgd_layout(dims, samples_per_chunk, &l) != 0) return 0;
+  return (size_t)l.total * sizeof(float);
+}
+
+int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                       const float* times, const int64_t* lengths, const float* node_scale, const int64_t* y,
+                       const uint8_t* sensor_perturbable, const uint8_t* sample_attacked, int32_t perturb_static,
+                       int32_t norm, float eps, float alpha, int32_t n_steps, int32_t random_start, const uint64_t* rng,
+                       int32_t samples_per_chunk, void* scratch, float* src_adv, float* statics_adv, float* logits_adv,
+                       float* logits_clean, float* loss_adv, void* stream) {
+  const char* fn = "rd_raindrop_v2_pgd";
+  if (!dims || !params || !src || !times || !lengths || !node_scale || !scratch || !src_adv || !logits_adv ||
+      !logits_clean || !loss_adv || !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
+  if (norm != RD_PGD_LINF && norm != RD_PGD_L2) { set_error("%s: norm must be RD_PGD_LINF or RD_PGD_L2, got %d", fn, norm); return -2; }
+  if (!(eps >= 0.f) || !(alpha >= 0.f) || isinf(eps) || isinf(alpha) || n_steps < 0) {
+    set_error("%s: eps and alpha must be finite and >= 0, n_steps >= 0 (eps = %g, alpha = %g, n_steps = %d)", fn, eps,
+              alpha, n_steps);
+    return -2;
+  }
+  if (random_start && !rng) { set_error("%s: random_start needs rng", fn); return -2; }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s0.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  if (perturb_static && s0.ds == 0) { set_error("%s: perturb_static needs a static branch (d_static > 0)", fn); return -2; }
+  const int B = s0.B, spc = samples_per_chunk;
+  PgdLayout l;
+  RD_TRY(pgd_layout(dims, spc, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  float* S = (float*)scratch;
+  float* ws = S + l.ws; float* sc = S + l.sc; float* dX0 = S + l.dX0; float* W1t = S + l.W1t; float* W1tlo = S + l.W1tlo;
+  float* lg = S + l.logits; float* dlog = S + l.dlogits;
+  double* best = reinterpret_cast<double*>(S + l.best);
+  PgdArgs a;
+  a.src = src; a.statics = s0.ds > 0 ? statics : nullptr; a.times = times; a.lengths = lengths;
+  a.sens = sensor_perturbable; a.attacked = sample_attacked;
+  a.x_e = S + l.src; a.st_e = s0.ds > 0 ? S + l.statics : nullptr; a.times_e = S + l.times;
+  a.len_e = reinterpret_cast<int64_t*>(S + l.lengths); a.delta = S + l.delta; a.grad = S + l.grad;
+  a.B = B; a.T = s0.T; a.N = s0.N; a.ds = s0.ds; a.pst = perturb_static ? 1 : 0;
+  // W1^T with its remainder, once per call
+  {
+    const rd_dims dc = pgd_dims(dims, spc, spc);
+    Shape s;
+    RD_TRY(make_shape(&dc, &s));
+    if (s.tc && n_steps > 0) {
+      const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
+      RD_TRY(split_weights(&it, 1, st));
+    }
+  }
+  for (int c0 = 0; c0 < B; c0 += spc) {
+    const int m = B - c0 < spc ? B - c0 : spc;
+    const rd_dims dc = pgd_dims(dims, m, spc);
+    Shape s;
+    RD_TRY(make_shape(&dc, &s));
+    const BwLayout b = bw_layout(s);
+    a.m = m; a.c0 = c0;
+    float* clean = logits_clean + (int64_t)c0 * s.ncls;
+    RD_TRY(pgd_expand(a, st));
+    RD_TRY(raindrop_fwd(&dc, params, a.x_e, a.st_e, a.times_e, a.len_e, node_scale, nullptr, ws, clean, nullptr, nullptr,
+                        nullptr, 0, st));
+    const float* cur = clean;
+    if (random_start) {
+      RD_TRY(pgd_start(a, norm, eps, rng, st));
+      RD_TRY(raindrop_fwd(&dc, params, a.x_e, a.st_e, a.times_e, a.len_e, node_scale, nullptr, ws, lg, nullptr, nullptr,
+                          nullptr, 0, st));
+      cur = lg;
+    }
+    for (int k = 0;; ++k) {
+      RD_TRY(pgd_track(a, s.ncls, cur, logits_clean, y, best, k == 0, dlog, src_adv, statics_adv, logits_adv, loss_adv, st));
+      if (k == n_steps) break;
+      RD_TRY(raindrop_bwd(&dc, params, a.st_e, a.len_e, node_scale, ws, dlog, nullptr, sc, RD_BWD_ALL, nullptr, st));
+      RD_TRY(input_grad_dx0(s, params, sc + b.gO1, W1t, W1tlo, dX0, st));
+      RD_TRY(pgd_step(a, norm, eps, alpha, params->R_u, s.dob, dX0, sc + b.dfeat, s.Df, s.D, params->emb_weight, s.emb, st));
+      RD_TRY(raindrop_fwd(&dc, params, a.x_e, a.st_e, a.times_e, a.len_e, node_scale, nullptr, ws, lg, nullptr, nullptr,
+                          nullptr, 0, st));
+      cur = lg;
+    }
   }
   return 0;
 }

@@ -114,6 +114,10 @@ SIGNATURES = {
     "rd_mc_dropout_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
     "rd_raindrop_v2_mc_dropout": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 6 +
                                   [C.c_int32, C.c_int32] + [C.c_void_p] * 6),
+    "rd_pgd_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
+    "rd_raindrop_v2_pgd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 8 +
+                           [C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_int32] +
+                           [C.c_void_p] * 7),
     "rd_encoder_head_fwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
     "rd_encoder_head_bwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(RdGrads), C.c_void_p, C.c_void_p, C.c_void_p]),

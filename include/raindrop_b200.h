@@ -701,6 +701,51 @@ int rd_fisher_labels(const float* logits, int32_t B, int32_t n_classes, uint64_t
 /* debug: out[i] = U(seed, index0 + i) (fp64, device) for i < n. */
 int rd_debug_fisher_uniforms(uint64_t seed, uint64_t index0, int32_t n, double* out, void* stream);
 
+/* ---- Laplace approximation (MacKay 1992; Ritter et al. 2018; Daxberger et al. 2021) ----------------------------------
+ * Posterior N(theta*, H^-1), H = n F + delta I with F the EK-FAC Fisher above: diagonal in the Kronecker eigenbasis,
+ * n Lambda_j + delta.  The linearised predictive of sample b is f ~ N(f(x_b; theta*), Sigma_b) over its logits, with
+ *   Sigma_b[c, c'] = sum_j w_j J~_{b,c,j} J~_{b,c',j},   w_j = 1 / (n Lambda_j + delta) (0 off the selected fields),
+ * J~_{b,c} = the rotated gradient row of logit c (rd_raindrop_v2_ekfac_rows seeded with d_logits = e_c / B).
+ * At most RD_LAPLACE_MAX_CLASSES classes. */
+#define RD_LAPLACE_MAX_CLASSES 8
+/* Scratch of rd_raindrop_v2_laplace_logit_cov: the rows scratch of rd_raindrop_v2_ekfac_rows, the seed d_logits [B, C],
+ * the rows [C, B, bucket] fp32 and the Gram's fp64 slab partials [B, ceil(bucket / 16384), C (C + 1) / 2]; 0 for dims
+ * it refuses. */
+size_t rd_laplace_logit_cov_scratch_bytes(const rd_dims* dims);
+/* cov [B, C, C] (fp64, device) = Sigma_b of every sample of the batch whose eval rd_raindrop_v2_fwd (without labels) left
+ * `workspace`.  Per class c: one seed launch (d_logits = e_c / B on the device), the rotated rows of
+ * rd_raindrop_v2_ekfac_rows into the scratch (bases as there); then one Gram launch over (16384-column slab, sample)
+ * CTAs, products w_j J~_cj in fp32 times J~_c'j in fp32, summed in fp64 per thread in column order, across the CTA in a
+ * fixed tree, and one launch adding the slabs in order: no atomics, so a sample's Sigma_b is bitwise reproducible and
+ * depends on its own rows only.  w: fp32 [bucket] on the device, 16-byte aligned (0 outside the selected fields and on
+ * padding).  Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+int rd_raindrop_v2_laplace_logit_cov(const rd_dims* dims, const rd_params* params, const float* statics,
+                                     const int64_t* lengths, const float* node_scale, const void* workspace,
+                                     const float* bases, const float* w, void* scratch, double* cov, void* stream);
+/* Relative pivot tolerance of the predictive's Cholesky factor: a pivot <= RD_LAPLACE_PIVOT_TOL * trace(Sigma_b) counts
+ * as 0 and its column of L_b is zeroed, so positive semi-definite Sigma_b (a class whose logit has no gradient in the
+ * selected fields, or an all-zero Sigma_b) is factorised without NaN. */
+#define RD_LAPLACE_PIVOT_TOL 1e-12
+/* Scratch of rd_laplace_predictive_mc: L_b [B, C, C] fp64, the fp64 sums of mc_dropout's reduction and one chunk's
+ * logits [samples_per_chunk, B, C] fp32; 0 for sizes it refuses. */
+size_t rd_laplace_sample_scratch_bytes(int32_t B, int32_t n_classes, int32_t samples_per_chunk);
+/* Monte Carlo predictive of the linearised Laplace posterior: replicate m = 0 .. n_samples-1 draws for every sample b
+ *   f_{m,b} = mean_logits[b] + L_b eps_{m,b}   (fp64, rounded to fp32 once)
+ * with L_b the lower Cholesky factor of cov[b] (fp64, pivots as RD_LAPLACE_PIVOT_TOL says) and eps_{m,b,k} a standard
+ * normal from the Philox4x32-10 stream of the dropout masks with key {seed, step + m} (rng = {seed, step}, device
+ * uint64[2], read only), site 99 (96: DP noise, 97: Fisher labels, 98: PGD start), element index e = b*C + k: counter
+ * e >> 2, Box-Muller on the block's word pairs as rd_dp_add_noise (e & 3 in {0, 1}: words (x, y), {2, 3}: (z, w); even e
+ * takes the cosine, odd e the sine).  A draw depends on (seed, step + m, b, k) alone, not on B or the chunking.  The
+ * replicates are reduced as rd_raindrop_v2_mc_dropout reduces its replicates (the same launch): mean_probs [B, C],
+ * variance [B, C], entropies [3, B], samples [M, B, C] (optional, may be NULL).  Work: one Cholesky launch, then per
+ * chunk of samples_per_chunk replicates one draw launch and one reduction launch (fp64 sums in replicate order, bitwise
+ * independent of the chunking).  mean_logits [B, C] fp32, cov [B, C, C] fp64, scratch
+ * rd_laplace_sample_scratch_bytes(B, C, samples_per_chunk) bytes, 16-byte aligned.  Stream-ordered, allocation- and
+ * sync-free, CUDA-graph capturable. */
+int rd_laplace_predictive_mc(const float* mean_logits, const double* cov, int32_t B, int32_t n_classes, const uint64_t* rng,
+                             int32_t n_samples, int32_t samples_per_chunk, void* scratch, float* mean_probs,
+                             float* variance, float* entropies, float* samples, void* stream);
+
 /* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);

@@ -288,4 +288,13 @@ int kfac_accumulate(const float* Aw, const float* Ab, const float* Sw, int Kin, 
 // zeroes G[b, off[f] + numel[f] .. next field's offset) and the tail up to ldg: the bucket's padding columns
 int psg_pad(const DpFields& fields, int B, float* G, long long ldg, cudaStream_t st);
 
+// ---- Laplace approximation (rd_laplace.cu) ---------------------------------------------------------------------------
+// laplace_seed: d_logits [B, ncls] = e_c / B.  laplace_gram: cov [B, ncls, ncls] (fp64) = sum_j w_j G_c[b, j] G_c'[b, j]
+// over the rows G [ncls][B][ldg] (class-major, ldg % 4 == 0, 16-byte aligned), through the fp64 slab partials
+// `partial` [laplace_gram_partial_doubles(B, ncls, ldg)]; ncls <= RD_LAPLACE_MAX_CLASSES.
+int64_t laplace_gram_partial_doubles(int B, int ncls, int64_t ldg);
+int laplace_seed(float* d_logits, int B, int ncls, int c, cudaStream_t st);
+int laplace_gram(const float* G, int B, int ncls, int64_t ldg, const float* w, double* partial, double* cov,
+                 cudaStream_t st);
+
 }  // namespace rd

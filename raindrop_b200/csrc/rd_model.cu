@@ -1697,6 +1697,24 @@ size_t rd_ekfac_rows_scratch_bytes(const rd_dims* dims) {
   return (size_t)ekfac_layout(s).total * sizeof(float);
 }
 
+// The rotated rows on checked arguments (ldg = the bucket length; G, bases and scratch 16-byte aligned), scratch laid
+// out as ekfac_layout(s): the bases' remainder image, the padding columns, then the backward with the rows queue.
+static int ekfac_rows(const Shape& s, const rd_dims* dims, const rd_params* params, const float* statics,
+                      const int64_t* lengths, const float* node_scale, const void* workspace, const float* d_logits,
+                      const float* bases, float* S, float* G, cudaStream_t st) {
+  DpQueue q;
+  const int64_t ldg = bucket_fields(s, &q.fields);
+  const KfacBlocks K = kfac_blocks(s);
+  const EkfacLayout l = ekfac_layout(s);
+  q.B = s.B; q.nf = q.fields.n; q.G = G; q.ldg = ldg;
+  q.scale = (float)s.B;      // as rd_raindrop_v2_per_sample_grads: rows are of l_b
+  q.shape = &s; q.kb = &K; q.bases = bases; q.bases_lo = S + l.lo; q.rot = S + l.rot;
+  RD_TRY(grad_lo_image(bases, K.base_floats, S + l.lo, st));
+  RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, S + l.bw,
+                      RD_BWD_ALL, nullptr, st, &q);
+}
+
 int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
                               const float* node_scale, const void* workspace, const float* d_logits, const float* bases,
                               void* scratch, float* G, int64_t ldg, void* stream) {
@@ -1709,24 +1727,65 @@ int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, cons
   RD_TRY(make_shape(dims, &s));
   if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
   if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
-  DpQueue q;
-  const int64_t bucket = bucket_fields(s, &q.fields);
+  DpFields f;
+  const int64_t bucket = bucket_fields(s, &f);
   if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
   if ((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(bases) | reinterpret_cast<uintptr_t>(scratch)) & 15) {
     set_error("%s: G, bases and scratch must be 16-byte aligned", fn);
     return -2;
   }
-  const KfacBlocks K = kfac_blocks(s);
-  const EkfacLayout l = ekfac_layout(s);
+  return ekfac_rows(s, dims, params, statics, lengths, node_scale, workspace, d_logits, bases, (float*)scratch, G,
+                    (cudaStream_t)stream);
+}
+
+// Scratch of the logit covariance: the rows scratch, the seed d_logits, the rows of every class and the Gram partials.
+struct LaplaceLayout { int64_t rows_scratch, dlog, G, partial, total; };
+static LaplaceLayout laplace_layout(const Shape& s, int64_t ldg) {
+  LaplaceLayout l;
+  Arena a;
+  l.rows_scratch = a.take(ekfac_layout(s).total);
+  l.dlog = a.take((int64_t)s.B * s.ncls);
+  l.G = a.take((int64_t)s.ncls * s.B * ldg);
+  l.partial = a.take(2 * laplace_gram_partial_doubles(s.B, s.ncls, ldg));
+  l.total = a.off;
+  return l;
+}
+
+size_t rd_laplace_logit_cov_scratch_bytes(const rd_dims* dims) {
+  Shape s;
+  if (make_shape(dims, &s) != 0 || s.ncls > RD_LAPLACE_MAX_CLASSES) return 0;
+  DpFields f;
+  return (size_t)laplace_layout(s, bucket_fields(s, &f)).total * sizeof(float);
+}
+
+int rd_raindrop_v2_laplace_logit_cov(const rd_dims* dims, const rd_params* params, const float* statics,
+                                     const int64_t* lengths, const float* node_scale, const void* workspace,
+                                     const float* bases, const float* w, void* scratch, double* cov, void* stream) {
+  const char* fn = "rd_raindrop_v2_laplace_logit_cov";
+  if (!dims || !params || !lengths || !node_scale || !workspace || !bases || !w || !scratch || !cov) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  if (s.ncls > RD_LAPLACE_MAX_CLASSES) { set_error("%s: n_classes = %d, at most %d", fn, s.ncls, RD_LAPLACE_MAX_CLASSES); return -2; }
+  if ((reinterpret_cast<uintptr_t>(bases) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(scratch)) & 15) {
+    set_error("%s: bases, w and scratch must be 16-byte aligned", fn);
+    return -2;
+  }
+  DpFields f;
+  const int64_t ldg = bucket_fields(s, &f);
+  const LaplaceLayout l = laplace_layout(s, ldg);
   float* S = (float*)scratch;
-  q.B = s.B; q.nf = q.fields.n; q.G = G; q.ldg = ldg;
-  q.scale = (float)s.B;      // as rd_raindrop_v2_per_sample_grads: rows are of l_b
-  q.shape = &s; q.kb = &K; q.bases = bases; q.bases_lo = S + l.lo; q.rot = S + l.rot;
   cudaStream_t st = (cudaStream_t)stream;
-  RD_TRY(grad_lo_image(bases, K.base_floats, S + l.lo, st));
-  RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
-  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, S + l.bw,
-                      RD_BWD_ALL, nullptr, st, &q);
+  for (int c = 0; c < s.ncls; ++c) {
+    RD_TRY(laplace_seed(S + l.dlog, s.B, s.ncls, c, st));
+    RD_TRY(ekfac_rows(s, dims, params, statics, lengths, node_scale, workspace, S + l.dlog, bases, S + l.rows_scratch,
+                      S + l.G + (int64_t)c * s.B * ldg, st));
+  }
+  return laplace_gram(S + l.G, s.B, s.ncls, ldg, w, reinterpret_cast<double*>(S + l.partial), cov, st);
 }
 
 int rd_dp_clip_scale(const rd_dims* dims, const void* workspace, const double* sqnorms, const float* weight,

@@ -766,15 +766,22 @@ class EKFACFactors:
     fingerprint: str
 
     def save(self, path):
-        torch.save(dict(bases=[[torch.from_numpy(np.ascontiguousarray(a)), torch.from_numpy(np.ascontiguousarray(s))]
-                               for a, s in self.bases],
-                        bases_flat=self.bases_flat.detach().cpu(), eigenvalues=self.eigenvalues.detach().cpu(), n=self.n,
-                        fisher=self.fisher, seed=self.seed, fields=None if self.fields is None else list(self.fields),
-                        layout=[[k, list(s)] for k, s in self.layout], fingerprint=self.fingerprint), path)
+        torch.save(self._state(), path)
 
     @classmethod
     def load(cls, path, map_location=None):
-        d = torch.load(path, map_location=map_location, weights_only=True)
+        return cls._from_state(torch.load(path, map_location=map_location, weights_only=True))
+
+    def _state(self):
+        """The dict save() writes: tensors, numbers, strings and lists only (torch.load's weights_only)."""
+        return dict(bases=[[torch.from_numpy(np.ascontiguousarray(a)), torch.from_numpy(np.ascontiguousarray(s))]
+                           for a, s in self.bases],
+                    bases_flat=self.bases_flat.detach().cpu(), eigenvalues=self.eigenvalues.detach().cpu(), n=self.n,
+                    fisher=self.fisher, seed=self.seed, fields=None if self.fields is None else list(self.fields),
+                    layout=[[k, list(s)] for k, s in self.layout], fingerprint=self.fingerprint)
+
+    @classmethod
+    def _from_state(cls, d):
         return cls(bases=tuple((a.cpu().numpy(), s.cpu().numpy()) for a, s in d["bases"]), bases_flat=d["bases_flat"],
                    eigenvalues=d["eigenvalues"], n=int(d["n"]), fisher=str(d["fisher"]), seed=int(d["seed"]),
                    fields=None if d["fields"] is None else tuple(d["fields"]),

@@ -14,6 +14,8 @@ ABI_VERSION = 2
 BWD_ENCODER, BWD_OBPROP, BWD_ALL = 1, 2, 3
 RD_D_PE = 16
 GRAD_DOT_SEGMENT = 4096     # RD_GRAD_DOT_SEGMENT
+LAPLACE_MAX_CLASSES = 8     # RD_LAPLACE_MAX_CLASSES
+LAPLACE_PIVOT_TOL = 1e-12   # RD_LAPLACE_PIVOT_TOL
 
 # enum rd_ws_buffer
 WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
@@ -185,6 +187,11 @@ SIGNATURES = {
                                       C.c_int32, C.c_void_p, C.c_void_p]),
     "rd_fisher_labels": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
     "rd_debug_fisher_uniforms": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p]),
+    "rd_laplace_logit_cov_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
+    "rd_raindrop_v2_laplace_logit_cov": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
+    "rd_laplace_sample_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "rd_laplace_predictive_mc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32] +
+                                 [C.c_void_p] * 6),
 }
 
 _lib = None

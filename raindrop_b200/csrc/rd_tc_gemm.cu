@@ -283,10 +283,11 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 //   D_k[m, n] = sum_r A_k[r, m] * B_k[r, n]   (A = dY, B = X plus a "ones" column N for the bias gradient)
 // over one row split of problem k per work item (problem, m tile, n tile, split).  A training step has ten of these
 // (8 encoder weights + 2 lin_value).  Persistent: one CTA per SM walks the items blockIdx.x, + gridDim.x, ...
-//   warpgroup 2   producer, 128 threads.  Per 32-row k-block, issued by thread 256 alone nstages - 2 k-blocks ahead as
-//                 soon as the stage is released, all by TMA (32 x 32 boxes, 128B swizzle): the raw X tile [32 x BN] into
-//                 the stage's hi | lo region on the stage's xfull mbarrier, the dY tile [32 x 128] into the stage's
-//                 dY region on its full mbarrier.  When the k-block's turn comes, the X tile is read into registers and
+//   warpgroup 3   issuer: thread 384 alone sends each 32-row k-block's loads into its stage as soon as the MMA
+//                 warpgroups release it, all by TMA (32 x 32 boxes, 128B swizzle): the raw X tile [32 x BN] into the
+//                 stage's hi | lo region on the stage's xfull mbarrier, the dY tile [32 x 128] into the stage's dY region
+//                 on its full mbarrier.  It does nothing else, so waiting for a release delays no transpose.
+//   warpgroup 2   transposer, 128 threads.  When a k-block's X has landed, the X tile is read into registers and
 //                 TRANSPOSED into the K-major 128B-swizzled images wgmma reads (sw128_offset(n, r)) as hi = top 19 bits
 //                 and lo = exact remainder, one 16-byte store per 4 rows of one column, with the ones column written
 //                 here (TMA cannot synthesise it).  fence.proxy.async, then arrive.
@@ -311,19 +312,19 @@ struct WGroup {
 };
 
 // Phase timing of one CTA, clock64 deltas summed in registers and written once at the end when WGroup::dbg is set.
-// Slots: 0 / 1 clock64 at the start (after the grid dependency wait) / end of MMA thread 0; 2 / 3 / 4 the producer's
-// (thread 256, which issues every TMA) cycles waiting for an empty stage (only when the k-block it is about to transpose
-// has not been issued) / for its X tile / transposing and storing; 5 / 6 MMA thread 0's cycles
-// waiting for a full stage / in the slab-store epilogue; 7 %globaltimer ns from start to end (the clock rate); 8 the
-// k-blocks the CTA produced; 9 clock64 at the producer's end; 10 the producer's cycles issuing the loads of a released
-// stage.
+// Slots: 0 / 1 clock64 at the start (after the grid dependency wait) / end of MMA thread 0; 3 / 4 transposing thread
+// 256's cycles waiting for its X tile / transposing and storing; 5 / 6 MMA thread 0's cycles waiting for a full stage /
+// in the slab-store epilogue; 7 %globaltimer ns from start to end (the clock rate); 8 the k-blocks the CTA transposed;
+// 9 clock64 at thread 256's end; 11 / 12 the issuing thread's cycles waiting for an empty stage / issuing the loads of a
+// released stage; 13 clock64 at the issuing thread's end.  Slots 2 and 10 are unused: the transposing warps neither
+// wait for releases nor issue loads.
 __device__ __forceinline__ unsigned long long gtimer() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
 
-constexpr int W_THREADS = 384;            // warpgroups 0, 1: MMA; warpgroup 2: producer
+constexpr int W_THREADS = 512;            // warpgroups 0, 1: MMA; warpgroup 2: transposer; warpgroup 3: issuer
 constexpr int WA_TILE = BK * BM * 4;      // 16 KB: 32 rows of dY x 128 columns
 // ring stage: dY tile | X^T hi | X^T lo; as many stages (<= MAX_STAGES) as fit next to the barriers and the alignment slack
 __host__ __device__ constexpr int w_stage_bytes(int bn) { return WA_TILE + 2 * bn * 128; }
@@ -452,7 +453,7 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
   constexpr int NBOX = (BN + 31) / 32;      // 32-column TMA boxes of X per k-block
   static_assert(BN % 16 == 0, "the transpose covers the tile in groups of 16 columns");
   static_assert(NBOX * 4096 <= 2 * BN * 128, "the raw X boxes land in the stage's hi | lo images");
-  static_assert(w_nstages(BN) >= 3, "the producer issues nstages - 2 k-blocks ahead of the one it transposes");
+  static_assert(w_nstages(BN) >= 3, "the consumers hold two stages; a third lets the producers run ahead");
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();
   WRing q;
@@ -476,46 +477,52 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
   const unsigned long long gt0 = gtimer();
   unsigned long long* const dbg = g.dbg ? g.dbg + (size_t)blockIdx.x * 16 : nullptr;
 
+  if (warp >= 12) {
+    // ===== issuer warpgroup ========================================================================
+    // Thread 384 alone walks the (item, k-block) sequence and sends each k-block's loads into its stage as soon as the
+    // MMA warpgroups release it, all by TMA: X (NBOX boxes) on the stage's xfull barrier, then dY (four boxes of 32 rows
+    // x 32 columns, 128B swizzle, see wgrad_consume) on its full barrier.  Only the ring bounds how far it runs ahead.
+    // The work item is computed once per item: the walk over the group's problems reads kernel parameters at a register
+    // index.
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 32;" ::: "memory");
+    if (warp == 12 && lane == 0) {
+      long long t_empty = 0, t_issue = 0;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int w = blockIdx.x; w < g.total_items; w += gridDim.x) {
+        const WItem it = wgrad_item(g, w);
+        for (int kb = 0; kb < it.k_blocks; ++kb) {
+          const long long c0 = clock64();
+          mbar_wait(q.empty(stage), phase ^ 1u);
+          const long long c1 = clock64();
+          t_empty += c1 - c0;
+          const uint32_t sa = q.addr(stage);
+          const int r0 = it.r_begin + kb * BK;
+          // rows past `rows`, columns past Kin and m past Nout arrive as zeros
+          mbar_expect_tx(q.xfull(stage), NBOX * 4096u);
+#pragma unroll
+          for (int b = 0; b < NBOX; ++b)
+            tma_load_2d(&g.tmX[it.pi], q.xfull(stage), sa + (uint32_t)WA_TILE + 4096u * b, it.n_t * BN + 32 * b, r0);
+          mbar_expect_tx(q.full(stage), (uint32_t)WA_TILE);
+#pragma unroll
+          for (int b = 0; b < BM / 32; ++b)
+            tma_load_2d(&g.tmY[it.pi], q.full(stage), sa + 4096u * b, it.m_t * BM + 32 * b, r0);
+          if (++stage == q.nstages) { stage = 0; phase ^= 1u; }
+          t_issue += clock64() - c1;
+        }
+      }
+      if (dbg) { dbg[11] = t_empty; dbg[12] = t_issue; dbg[13] = clock64(); }
+    }
+    return;
+  }
+
   if (warp >= 8) {
-    // ===== producer warpgroup ======================================================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 120;" ::: "memory");
+    // ===== transposer warpgroup ====================================================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 112;" ::: "memory");
     const int pt = threadIdx.x - 256, pw = warp - 8;
     const int total = g.total_items;
-    long long t_empty = 0, t_x = 0, t_store = 0, t_issue = 0, n_kb = 0;
-    // Two cursors walk the same (item, k-block) sequence.  The issue cursor, thread 256 alone, sends a k-block's loads
-    // into its stage as soon as the MMA warpgroups release it, all by TMA: X (NBOX boxes) on the stage's xfull
-    // barrier, then dY (four boxes of 32 rows x 32 columns, 128B swizzle, see wgrad_consume) on its full barrier.  It
-    // runs up to nstages - 2 k-blocks ahead of the transpose cursor, but waits for a release only when the k-block
-    // about to be transposed is not issued yet: so the transposes run ahead as far as the ring allows instead of
-    // waiting, every k-block, for the consumers to retire the group of two k-blocks back.  The work item of each
-    // cursor is computed once per item: the walk over the group's problems reads kernel parameters at a register index.
-    int iw = blockIdx.x, ikb = 0, istage = 0, ahead = 0;
-    uint32_t iphase = 0;
-    WItem iit = wgrad_item(g, iw);
-    auto issue = [&]() {
-      const long long c0 = clock64();
-      mbar_wait(q.empty(istage), iphase ^ 1u);
-      const long long c1 = clock64();
-      t_empty += c1 - c0;
-      const uint32_t sa = q.addr(istage);
-      const int r0 = iit.r_begin + ikb * BK;
-      // rows past `rows`, columns past Kin and m past Nout arrive as zeros
-      mbar_expect_tx(q.xfull(istage), NBOX * 4096u);
-#pragma unroll
-      for (int b = 0; b < NBOX; ++b)
-        tma_load_2d(&g.tmX[iit.pi], q.xfull(istage), sa + (uint32_t)WA_TILE + 4096u * b, iit.n_t * BN + 32 * b, r0);
-      mbar_expect_tx(q.full(istage), (uint32_t)WA_TILE);
-#pragma unroll
-      for (int b = 0; b < BM / 32; ++b)
-        tma_load_2d(&g.tmY[iit.pi], q.full(istage), sa + 4096u * b, iit.m_t * BM + 32 * b, r0);
-      if (++istage == q.nstages) { istage = 0; iphase ^= 1u; }
-      t_issue += clock64() - c1;
-      if (++ikb == iit.k_blocks) {
-        ikb = 0; iw += gridDim.x;
-        if (iw < total) iit = wgrad_item(g, iw);
-      }
-    };
-    // The transpose cursor: the raw X tile (NBOX boxes of 32 rows x 32 columns, 128B-swizzled, at the start of the
+    long long t_x = 0, t_store = 0, n_kb = 0;
+    // The raw X tile (NBOX boxes of 32 rows x 32 columns, 128B-swizzled, at the start of the
     // stage's hi image; (r, n) at 4096 (n >> 5) + sw128_offset(r, n % 32)) -> registers, with the ones column N of the
     // bias gradient set here -> the K-major images, one 16-byte store per chunk of rows 4a .. 4a + 3 of one image row n
     // (sw128_offset(n, 4a)) for hi and one for lo.  Lane = 8c + a, c = lane / 8, a = lane % 8, of warp pw holds, per
@@ -534,15 +541,8 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
       for (int j = 0; j < 4; ++j) ld_off[e][j] = sw128_offset(4 * a + j, 16 * e + 4 * cq + c);
     const uint32_t st_off = sw128_offset(4 * cq + c, 4 * a);     // image: + 2048 i (16 rows of 128 bytes per group)
     int w = blockIdx.x, kb = 0;
-    WItem it = iit;
+    WItem it = wgrad_item(g, w);
     while (w < total) {
-      // only the k-block about to be transposed has to be issued now (ahead == 0); the stages further ahead are issued
-      // if already released
-      if (pt == 0)
-        for (; ahead < q.nstages - 1 && iw < total; ++ahead) {
-          if (ahead > 0 && !mbar_test(q.empty(istage), iphase ^ 1u)) break;
-          issue();
-        }
       const WP& p = g.it[it.pi];
       const long long c0 = clock64();
       mbar_wait(q.xfull(q.stage), q.phase);
@@ -568,21 +568,19 @@ tc_wgrad_kernel(const __grid_constant__ WGroup g) {
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> wgmma's reads
       mbar_arrive(q.full(q.stage));
       if (++q.stage == q.nstages) { q.stage = 0; q.phase ^= 1u; }
-      --ahead;
       t_x += c1 - c0; t_store += clock64() - c1; ++n_kb;
       if (++kb == it.k_blocks) {
         kb = 0; w += gridDim.x;
         if (w < total) it = wgrad_item(g, w);
       }
     }
-    if (dbg && pt == 0) {
-      dbg[2] = t_empty; dbg[3] = t_x; dbg[4] = t_store; dbg[8] = n_kb; dbg[9] = clock64(); dbg[10] = t_issue;
-    }
+    if (dbg && pt == 0) { dbg[3] = t_x; dbg[4] = t_store; dbg[8] = n_kb; dbg[9] = clock64(); }
     return;
   }
 
   // ===== warpgroups 0, 1: MMA ======================================================================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 192;" ::: "memory");
+  // 128 x (2 x 184 + 112 + 32) = 65,536: the whole register file
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 184;" ::: "memory");
   const int wg = warp >> 2, wq = warp & 3, gq = lane >> 2, t = lane & 3;
   const int arow = wg * 64 + wq * 16 + gq;
   long long t_full = 0, t_epi = 0;

@@ -54,9 +54,9 @@ def problems(config, batch):
     return enc + enc + [("ob-prop lin_value", m1, C, C)] * 2
 
 
-STAMP_PHASES = [("total", None), ("producer: wait empty stage", 2), ("producer: wait X", 3),
-                ("producer: transpose + store", 4), ("producer: issue loads", 10), ("producer: other", None),
-                ("MMA: wait full stage", 5), ("MMA: epilogue", 6)]
+STAMP_PHASES = [("total", None), ("transposer: wait X", 3), ("transposer: transpose + store", 4),
+                ("transposer: other", None), ("issuer: wait empty stage", 11), ("issuer: issue loads", 12),
+                ("issuer: other", None), ("MMA: wait full stage", 5), ("MMA: epilogue", 6)]
 
 
 def stamp_breakdown(lib, call, flush, sms, dev, reps=5):
@@ -78,8 +78,9 @@ def stamp_breakdown(lib, call, flush, sms, dev, reps=5):
         mhz = (s[:, 1] - s[:, 0]) / s[:, 7] * 1000.0          # cycles per ns -> MHz, per CTA
         us = {name: s[:, slot] / mhz for name, slot in STAMP_PHASES if slot is not None}
         us["total"] = (s[:, 1] - s[:, 0]) / mhz
-        # the producer's time outside the measured phases (its item walk and loop), start to its own end
-        us["producer: other"] = (s[:, 9] - s[:, 0] - s[:, 2] - s[:, 3] - s[:, 4] - s[:, 10]) / mhz
+        # each producer thread's time outside its measured phases (item walk, loop), from the start to its own end
+        us["transposer: other"] = (s[:, 9] - s[:, 0] - s[:, 3] - s[:, 4]) / mhz
+        us["issuer: other"] = (s[:, 13] - s[:, 0] - s[:, 11] - s[:, 12]) / mhz
         us = {name: us[name] for name, _ in STAMP_PHASES}
         us["k-blocks"] = s[:, 8]
         busiest = int(torch.argmax(us["total"]))

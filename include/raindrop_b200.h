@@ -427,6 +427,33 @@ int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float
                        int32_t samples_per_chunk, void* scratch, float* src_adv, float* statics_adv, float* logits_adv,
                        float* logits_clean, float* loss_adv, void* stream);
 
+/* ---- randomized smoothing of Raindrop_v2: Monte Carlo class votes, in one call --------------------------------------
+ * The smoothed classifier g(x) = argmax_c P(f(x + sigma z) = c) (Cohen, Rosenfeld & Kolter 2019) of the eval-mode model
+ * f, estimated by counting the argmax classes of n_samples noisy replicates of every sample.
+ * Perturbable set S_b (the threat model of rd_raindrop_v2_pgd): the value cells with src[t, b, N + n] > 0 of sensors with
+ * sensor_perturbable[n] != 0 (NULL: every sensor), plus the statics when perturb_static.  The mask half, times and
+ * lengths are copied bit for bit, and so is every element outside S_b.
+ * Noise: replicate m = 0 .. n_samples-1 is x + sigma z, z ~ N(0, I) on S_b and 0 elsewhere (an element whose noise is 0
+ * keeps x bit for bit), in normalised units.  z is drawn from Philox4x32-10 at site 100 (96: DP noise, 97: Fisher
+ * labels, 98: PGD start, 99: Laplace) under key {seed, step + m}, rng = {seed, step} (device uint64[2], read only):
+ * element e of sample b (e = t*N + n for value cells, T*N + j for statics) at index b*(T*N + d_static) + e, counter
+ * index >> 2, Box-Muller on the block's word pairs as rd_dp_add_noise draws them.  A replicate depends on
+ * (seed, step + m, b) alone, not on B or the chunking.
+ *   counts [B, n_classes] int64 = per sample, how many replicates' logits have their (first) maximum at each class.  A
+ *          replicate with a non-finite logit votes for no class, so counts.sum(1) <= n_samples.
+ * Eval arithmetic (dims->training must be 0): no dropout, the model's rng state is neither read nor advanced, no
+ * parameter gradient is written.  Work: chunks of replicates_per_chunk replicates; per chunk one launch expanding the
+ * noisy replicate-major rows (row j = m*B + b), ONE eval forward on B*replicates_per_chunk rows and one launch adding
+ * the rows' votes (integers: exact, independent of the chunking once dims->obprop_mode is pinned; mode 0 is resolved
+ * once from B*replicates_per_chunk rows).  scratch: rd_smooth_scratch_bytes(dims, replicates_per_chunk) bytes.
+ * Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+size_t rd_smooth_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk);
+int rd_raindrop_v2_smooth_counts(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                 const float* times, const int64_t* lengths, const float* node_scale,
+                                 const uint8_t* sensor_perturbable, int32_t perturb_static, float sigma,
+                                 const uint64_t* rng, int32_t n_samples, int32_t replicates_per_chunk, void* scratch,
+                                 int64_t* counts, void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);
@@ -767,6 +794,16 @@ int rd_debug_dropout_mask(const uint64_t* rng_captured, uint32_t site, int64_t n
 /* debug: materialise the block out[c * dim + m] = Omega(seed, col0 + c, m) (+1.0f / -1.0f) of rd_grad_projection's
  * projection, c < n_cols, m < dim, so tests can compare it with a host restatement of the mapping. */
 int rd_debug_projection_signs(uint64_t seed, int64_t col0, int32_t n_cols, int32_t dim, float* out, void* stream);
+
+/* debug: the noisy inputs of replicates m0 .. m0+nc-1 of rd_raindrop_v2_smooth_counts (same launch, same stream) in its
+ * replicate-major layout, row j = (m - m0)*B + b: src_e [T, nc*B, 2N], statics_e [nc*B, d_static] (d_static > 0),
+ * times_e [T, nc*B] and lengths_e [nc*B] (each of these two may be NULL: skipped).  Only dims' B, T, N (d_inp) and
+ * d_static are read.  With nc = 1 and m0 = 0 it is one Gaussian-augmented copy of the batch at key rng, which is how
+ * SmoothingTrainStep draws its noisy batch. */
+int rd_debug_smoothing_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                              const int64_t* lengths, const uint8_t* sensor_perturbable, int32_t perturb_static,
+                              float sigma, const uint64_t* rng, int64_t m0, int32_t nc, float* src_e, float* statics_e,
+                              float* times_e, int64_t* lengths_e, void* stream);
 
 #ifdef __cplusplus
 }

@@ -30,7 +30,7 @@ __device__ __forceinline__ Elem elem(const PgdArgs& a, int j, int e) {
     const long long r = ((long long)t * a.B + b) * (2 * a.N);
     o.x = __ldg(a.src + r + n);
     o.xe = a.x_e + ((long long)t * a.m + j) * (2 * a.N) + n;
-    o.p = (!a.sens || a.sens[n]) && __ldg(a.src + r + a.N + n) > 0.f;
+    o.p = perturbable_cell(a.src, r, a.N, n, a.sens);
   } else {
     const int k = e - TN;
     o.x = __ldg(a.statics + (long long)b * a.ds + k);
@@ -49,14 +49,6 @@ __device__ __forceinline__ uint32_t start_word(const RngKey& k, uint64_t idx) {
   const uint4 w = dropout_block(k, SITE_PGD_START, idx);
   const uint32_t s = (uint32_t)idx & 3u;
   return s == 0 ? w.x : (s == 1 ? w.y : (s == 2 ? w.z : w.w));
-}
-// standard normal of element idx: Box-Muller on the block's pair (x, y) for idx & 3 in {0, 1}, (z, w) for {2, 3}
-__device__ __forceinline__ float start_normal(const RngKey& k, uint64_t idx) {
-  const uint4 w = dropout_block(k, SITE_PGD_START, idx);
-  float z0, z1;
-  if ((idx & 3u) < 2u) box_muller(w.x, w.y, &z0, &z1);
-  else box_muller(w.z, w.w, &z0, &z1);
-  return (idx & 1u) ? z1 : z0;
 }
 
 // The chunk's inputs (src rows, statics, times, lengths of samples c0 .. c0+m-1) and delta = 0, one launch.
@@ -120,7 +112,7 @@ __global__ void __launch_bounds__(PGD_THREADS) pgd_start_kernel(const __grid_con
   double zz = 0.0, cnt = 0.0;
   for (int e = threadIdx.x; e < ne; e += PGD_THREADS) {
     if (!elem(a, j, e).p) continue;
-    const float z = start_normal(k, base + e);
+    const float z = philox_normal(k, SITE_PGD_START, base + e);
     dl[e] = z;
     zz += (double)z * (double)z;
     cnt += 1.0;

@@ -137,6 +137,15 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float* z0, fl
   *z0 = (float)(r * cos(t));
   *z1 = (float)(r * sin(t));
 }
+// Standard normal of element idx at `site`: Box-Muller on the pair (x, y) of the block at counter idx >> 2 for
+// idx & 3 in {0, 1}, (z, w) for {2, 3}; even idx takes the cosine, odd idx the sine (as rd_dp_add_noise draws them).
+__device__ __forceinline__ float philox_normal(const RngKey& k, uint32_t site, uint64_t idx) {
+  const uint4 w = dropout_block(k, site, idx);
+  float z0, z1;
+  if ((idx & 3u) < 2u) box_muller(w.x, w.y, &z0, &z1);
+  else box_muller(w.z, w.w, &z0, &z1);
+  return (idx & 1u) ? z1 : z0;
+}
 
 // ---- Monte Carlo dropout replicates in one forward ------------------------------------------------------------------
 // A forward over Bc = cc*B rows, replicate-major (row j = m*B + b), in which row j draws exactly the words that the

@@ -656,28 +656,15 @@ struct McExpandArgs {
 __global__ void mc_expand_kernel(const __grid_constant__ McExpandArgs a) {
   pdl_launch_dependents();
   pdl_wait();
-  const long long Bc = (long long)a.B * a.nc, W = 2LL * a.N;
-  const long long n_src = a.T * Bc * W, n_times = a.T * Bc, n_stat = a.statics ? Bc * a.ds : 0;
-  long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (o < n_src) {
-    const long long k = o % W, r = o / W, t = r / Bc, b = (r - t * Bc) % a.B;
-    a.src_e[o] = __ldg(a.src + (t * a.B + b) * W + k);
-    return;
+  const RepElem e = rep_expand_elem((long long)blockIdx.x * blockDim.x + threadIdx.x, a.B, a.nc, a.T, a.N,
+                                    a.statics ? a.ds : 0);
+  switch (e.part) {
+    case REP_SRC: a.src_e[e.out] = __ldg(a.src + e.in); break;
+    case REP_TIMES: a.times_e[e.out] = __ldg(a.times + e.in); break;
+    case REP_STATICS: a.statics_e[e.out] = __ldg(a.statics + e.in); break;
+    case REP_LENGTHS: a.lengths_e[e.out] = __ldg(a.lengths + e.in); break;
+    default: break;
   }
-  o -= n_src;
-  if (o < n_times) {
-    const long long t = o / Bc, b = (o - t * Bc) % a.B;
-    a.times_e[o] = __ldg(a.times + t * a.B + b);
-    return;
-  }
-  o -= n_times;
-  if (o < n_stat) {
-    const long long j = o / a.ds, k = o - j * a.ds;
-    a.statics_e[o] = __ldg(a.statics + (j % a.B) * a.ds + k);
-    return;
-  }
-  o -= n_stat;
-  if (o < Bc) a.lengths_e[o] = __ldg(a.lengths + o % a.B);
 }
 
 // mc_accum_kernel, one warp per sample b: for the chunk's replicates m0 .. m0+nc-1 IN ORDER, p = softmax(logits row

@@ -124,6 +124,51 @@ int kernel_shap_accumulate(const float* logits_c, const float* ends, const int64
 int kernel_shap_solve(const double* acc, const double* solve, const float* ends, const int64_t* target, int P, int B,
                       int ncls, float* attr, cudaStream_t st);
 
+// Replicate-major expansion of a B-sample batch into Bc = nc*B rows (row j = m*B + b): output element o of the
+// concatenation src_e [T, Bc, 2N] | times_e [T, Bc] | statics_e [Bc, ds] | lengths_e [Bc] is element `out` of its part
+// and reads element `in` of the batch's src [T, B, 2N] / times [T, B] / statics [B, ds] / lengths [B]; (m, b) is its
+// row's replicate and sample, t its time step (src, times) and k its column (src, statics).
+enum RepPart { REP_SRC, REP_TIMES, REP_STATICS, REP_LENGTHS, REP_NONE };
+struct RepElem { int part, m, b, t, k; long long out, in; };
+__device__ __forceinline__ RepElem rep_expand_elem(long long o, int B, int nc, int T, int N, int ds) {
+  const long long Bc = (long long)B * nc, W = 2LL * N;
+  const long long n_src = T * Bc * W, n_times = T * Bc, n_stat = Bc * ds;
+  RepElem e;
+  e.t = 0; e.k = 0;
+  long long j = 0;
+  if (o < n_src) {
+    const long long r = o / W, t = r / Bc;
+    e.part = REP_SRC; e.out = o; e.t = (int)t; e.k = (int)(o - r * W); j = r - t * Bc;
+  } else if ((o -= n_src) < n_times) {
+    const long long t = o / Bc;
+    e.part = REP_TIMES; e.out = o; e.t = (int)t; j = o - t * Bc;
+  } else if ((o -= n_times) < n_stat) {
+    j = o / ds;
+    e.part = REP_STATICS; e.out = o; e.k = (int)(o - j * ds);
+  } else if ((o -= n_stat) < Bc) {
+    e.part = REP_LENGTHS; e.out = o; j = o;
+  } else {
+    e.part = REP_NONE; e.out = e.in = 0; e.m = e.b = 0;
+    return e;
+  }
+  e.m = (int)(j / B);
+  e.b = (int)(j - (long long)e.m * B);
+  switch (e.part) {
+    case REP_SRC: e.in = ((long long)e.t * B + e.b) * W + e.k; break;
+    case REP_TIMES: e.in = (long long)e.t * B + e.b; break;
+    case REP_STATICS: e.in = (long long)e.b * ds + e.k; break;
+    default: e.in = e.b;
+  }
+  return e;
+}
+
+// The PGD / randomized-smoothing threat model: value cell n of the src row starting at `row` (= (t*B + b) * 2N) may be
+// perturbed when it is observed (mask > 0) and its sensor is perturbable (sens [N] uint8, NULL: every sensor).
+__device__ __forceinline__ bool perturbable_cell(const float* __restrict__ src, long long row, int N, int n,
+                                                 const uint8_t* __restrict__ sens) {
+  return (!sens || sens[n]) && __ldg(src + row + N + n) > 0.f;
+}
+
 // Monte Carlo dropout over chunks of nc replicates on B*nc rows, replicate-major (j = m*B + b).
 // mc_expand: src_e [T, B*nc, 2N], statics_e (ds > 0), times_e, lengths_e = nc copies of the batch.
 int mc_expand(const float* src, const float* statics, const float* times, const int64_t* lengths, int B, int nc, int T,
@@ -157,6 +202,17 @@ int pgd_track(const PgdArgs& a, int ncls, const float* logits, const float* logi
 // the step from dX0 [m*N, T*d_ob] and dfeat [m, Df] (statics gradient from columns D .. D+emb through W_emb [emb, ds])
 int pgd_step(const PgdArgs& a, int norm, float eps, float alpha, const float* R_u, int d_ob, const float* dX0,
              const float* dfeat, int Df, int D, const float* W_emb, int emb, cudaStream_t st);
+
+// ---- randomized smoothing (rd_smoothing.cu; rd_raindrop_v2_smooth_counts) -------------------------------------------
+constexpr uint32_t SITE_SMOOTH = 100;       // Philox site of the smoothing noise (its key is {seed, step + replicate})
+// smooth_expand: replicates m0 .. m0+nc-1 of the batch as mc_expand lays them out, with x + sigma z on the perturbable
+// elements (perturbable_cell over sens, the statics when pst), z drawn at key {rng[0], rng[1] + m0 + m} and index
+// b*(T*N + ds) + e.  times_e / lengths_e may be NULL (skipped).
+int smooth_expand(const float* src, const float* statics, const float* times, const int64_t* lengths, const uint8_t* sens,
+                  int pst, float sigma, const uint64_t* rng, int64_t m0, int B, int nc, int T, int N, int ds, float* src_e,
+                  float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
+// smooth_vote: counts [B, ncls] (+)= the argmax votes of logits [nc*B, ncls] (replicate-major; first: from 0)
+int smooth_vote(const float* logits, int B, int nc, int ncls, int first, int64_t* counts, cudaStream_t st);
 
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 

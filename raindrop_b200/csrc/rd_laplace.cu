@@ -125,11 +125,7 @@ __global__ void laplace_chol_kernel(const double* __restrict__ cov, int B, int C
 // standard normal of element e = b*C + k of replicate m (key {seed, step + m}): Box-Muller on the pair (x, y) of the
 // block at counter e >> 2 for e & 3 in {0, 1}, (z, w) for {2, 3}, as rd_dp_add_noise draws them
 __device__ __forceinline__ double laplace_normal(const RngKey& k, uint64_t e) {
-  const uint4 w = dropout_block(k, SITE_LAPLACE, e);
-  float z0, z1;
-  if ((e & 3u) < 2u) box_muller(w.x, w.y, &z0, &z1);
-  else box_muller(w.z, w.w, &z0, &z1);
-  return (double)((e & 1u) ? z1 : z0);
+  return (double)philox_normal(k, SITE_LAPLACE, e);
 }
 
 // logits [nc*B, C] replicate-major (row j = m*B + b, replicate m0 + m): f_c = mu_c + sum_{k <= c} L_ck eps_k in fp64,

@@ -430,6 +430,27 @@ int mc_layout(const rd_dims* dims, int cc, McLayout* l) {
   return 0;
 }
 
+// ---- randomized smoothing ------------------------------------------------------------------------------------------
+// Scratch of rd_raindrop_v2_smooth_counts: the eval forward workspace of B*cc rows, the chunk's noisy inputs and its
+// logits.  The ob-prop mode is pinned from B*cc rows by ig_dims, as for integrated gradients.
+struct SmoothLayout { int64_t ws, src, statics, times, lengths, logits, total; };
+int smooth_layout(const rd_dims* dims, int cc, SmoothLayout* l) {
+  if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("replicates_per_chunk = %d out of range", cc); return -2; }
+  const int Bc = dims->B * cc;
+  const rd_dims dc = ig_dims(dims, Bc, cc);
+  Shape sc;
+  RD_TRY(make_shape(&dc, &sc));
+  Arena a;
+  l->ws = a.take(ws_layout(sc).total);
+  l->src = a.take(sc.M2 * 2 * sc.N);
+  l->statics = a.take((int64_t)Bc * sc.ds);
+  l->times = a.take(sc.M2);
+  l->lengths = a.take(2LL * Bc);
+  l->logits = a.take((int64_t)Bc * sc.ncls);
+  l->total = a.off;
+  return 0;
+}
+
 // Y[M,N] = epi(X[M,K] . W[N,K]^T)
 GemmP nt(const float* X, int64_t ldx, const float* W, int64_t ldw, float* Y, int64_t ldy, int64_t M, int N, int K) {
   GemmP g;
@@ -1593,6 +1614,76 @@ int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, cons
                          c0 + nc >= M, st));
   }
   return 0;
+}
+
+size_t rd_smooth_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk) {
+  if (!dims) return 0;
+  SmoothLayout l;
+  if (smooth_layout(dims, replicates_per_chunk, &l) != 0) return 0;
+  return (size_t)l.total * sizeof(float);
+}
+
+// The checks rd_raindrop_v2_smooth_counts and rd_debug_smoothing_inputs share.
+static int smooth_check(const char* fn, const rd_dims* dims, const float* statics, int32_t perturb_static, float sigma,
+                        Shape* s0) {
+  if (!(sigma >= 0.f) || isinf(sigma)) { set_error("%s: sigma must be finite and >= 0, got %g", fn, sigma); return -2; }
+  RD_TRY(make_shape(dims, s0));
+  if (s0->ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  if (perturb_static && s0->ds == 0) { set_error("%s: perturb_static needs a static branch (d_static > 0)", fn); return -2; }
+  return 0;
+}
+
+// Chunks of cc replicates: one launch expanding the chunk's noisy inputs, one eval forward on B*cc replicate-major rows
+// and one launch adding each row's vote to counts.
+int rd_raindrop_v2_smooth_counts(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                 const float* times, const int64_t* lengths, const float* node_scale,
+                                 const uint8_t* sensor_perturbable, int32_t perturb_static, float sigma,
+                                 const uint64_t* rng, int32_t n_samples, int32_t replicates_per_chunk, void* scratch,
+                                 int64_t* counts, void* stream) {
+  const char* fn = "rd_raindrop_v2_smooth_counts";
+  if (!dims || !params || !src || !times || !lengths || !node_scale || !rng || !scratch || !counts || !params->R_u ||
+      !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
+  if (n_samples < 1 || replicates_per_chunk < 1) { set_error("%s: n_samples and replicates_per_chunk must be >= 1", fn); return -2; }
+  Shape s0;
+  RD_TRY(smooth_check(fn, dims, statics, perturb_static, sigma, &s0));
+  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  SmoothLayout l;
+  RD_TRY(smooth_layout(dims, replicates_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, cc = replicates_per_chunk;
+  float* S = (float*)scratch;
+  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
+  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  for (int c0 = 0; c0 < n_samples; c0 += cc) {
+    const int nc = n_samples - c0 < cc ? n_samples - c0 : cc;
+    const rd_dims dc = ig_dims(dims, B * nc, cc);
+    RD_TRY(smooth_expand(src, statics, times, lengths, sensor_perturbable, perturb_static, sigma, rng, c0, B, nc, s0.T, s0.N,
+                         s0.ds, src_e, stat_e, times_e, len_e, st));
+    RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, S + l.ws, S + l.logits, nullptr,
+                        nullptr, nullptr, 0, st));
+    RD_TRY(smooth_vote(S + l.logits, B, nc, s0.ncls, c0 == 0, counts, st));
+    if (n_samples - c0 <= cc) break;
+  }
+  return 0;
+}
+
+int rd_debug_smoothing_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                              const int64_t* lengths, const uint8_t* sensor_perturbable, int32_t perturb_static,
+                              float sigma, const uint64_t* rng, int64_t m0, int32_t nc, float* src_e, float* statics_e,
+                              float* times_e, int64_t* lengths_e, void* stream) {
+  const char* fn = "rd_debug_smoothing_inputs";
+  if (!dims || !src || !times || !lengths || !rng || !src_e) { set_error("%s: NULL argument", fn); return -2; }
+  if (nc < 1 || m0 < 0) { set_error("%s: nc must be >= 1 and m0 >= 0 (nc = %d, m0 = %lld)", fn, nc, (long long)m0); return -2; }
+  Shape s0;
+  RD_TRY(smooth_check(fn, dims, statics, perturb_static, sigma, &s0));
+  if (s0.ds > 0 && !statics_e) { set_error("%s: d_static > 0 needs statics_e", fn); return -2; }
+  if ((int64_t)s0.B * nc > (1LL << 30)) { set_error("%s: B * nc = %lld rows are too many", fn, (long long)s0.B * nc); return -2; }
+  return smooth_expand(src, statics, times, lengths, sensor_perturbable, perturb_static, sigma, rng, m0, s0.B, nc, s0.T,
+                       s0.N, s0.ds, src_e, statics_e, times_e, lengths_e, (cudaStream_t)stream);
 }
 
 size_t rd_dp_scratch_bytes(const rd_dims* dims) {

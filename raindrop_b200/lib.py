@@ -120,6 +120,13 @@ SIGNATURES = {
     "rd_raindrop_v2_pgd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 8 +
                            [C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_int32] +
                            [C.c_void_p] * 7),
+    "rd_smooth_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
+    "rd_raindrop_v2_smooth_counts": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 6 +
+                                     [C.c_int32, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]),
+    "rd_debug_smoothing_inputs": (C.c_int, [C.POINTER(RdDims)] + [C.c_void_p] * 5 + [C.c_int32, C.c_float, C.c_void_p,
+                                                                                       C.c_int64, C.c_int32] +
+                                  [C.c_void_p] * 5),
     "rd_encoder_head_fwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
     "rd_encoder_head_bwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(RdGrads), C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -805,6 +805,57 @@ int rd_debug_smoothing_inputs(const rd_dims* dims, const float* src, const float
                               float sigma, const uint64_t* rng, int64_t m0, int32_t nc, float* src_e, float* statics_e,
                               float* times_e, int64_t* lengths_e, void* stream);
 
+/* ---- the forward GEMM engines on their own (debug: operator-level tests) -------------------------------------------
+ * Fields are grouped by size (pointers, 64-bit, 32-bit) so the layout has no interior padding. */
+/* One tc_nt_kernel launch: C[M, N] = epi(A[M, K] . B[N, K]^T), A with row stride lda, B (and B_lo) with row stride K,
+ * C with row stride N.  B_lo = B - trunc19(B) selects the error-compensated mode (3xTF32); NULL selects single-pass TF32
+ * on operands the caller keeps TF32-representable.  epi = +bias[col] -> relu -> *scale[row % scale_mod] ->
+ * *(gate[row * gate_ld + col] > 0 ? gate_scale : 0) -> dropout (site drop_site, index row * N + col, or through the
+ * replicate rows rep_B / rep_Bc; keep bits to drop_mask[row * drop_mask_ld + col / 32], bit col % 32, the bits past N of
+ * the row's last word zeroed) -> +resid[row * resid_ld + col] -> RN to TF32 (round_out); perm != 0 stores row b*pN + n,
+ * col t*4 + k to C[(t*pB + b)*pD + n*4 + k].  Only the epilogue combinations the model uses are instantiated; others are
+ * refused.  BN = 0 or n_tiles = 0: the plan of tc_nt_plan, written back into the struct. */
+typedef struct rd_debug_tc_nt_args {
+  const float* A; const float* B; const float* B_lo; float* C;
+  const float* bias; const float* scale; const float* gate; const uint64_t* rng; uint32_t* drop_mask; const float* resid;
+  int64_t lda, M, gate_ld, resid_ld;
+  int32_t N, K, BN, n_tiles;
+  int32_t relu, scale_mod; float gate_scale;
+  float drop_p; uint32_t drop_site; int32_t rep_B, rep_Bc, drop_mask_ld;
+  int32_t round_out;
+  int32_t perm, pB, pN, pD;
+} rd_debug_tc_nt_args;
+int rd_debug_tc_nt(rd_debug_tc_nt_args* args, void* stream);
+/* One call of the CUDA-core GEMM (rd_gemm.cu): C(i, j) = epi(alpha * sum_k A(i, k) B(k, j)) with element strides
+ * (ta: A(i, k) = A[k*sAk + i], else A[i*sAi + k]; tb: B(k, j) = B[j*sBj + k], else B[k*sBk + j]), batched over
+ * z = zo * nz_inner + zi (offsets s?zo, s?zi), C(i, j) at C[i*sCi + j*sCj].  epi = +bias[j] -> relu ->
+ * *rowscale[i % rowscale_mod] -> *(gate[i*gate_ld + j] > 0 ? gate_scale : 0) -> dropout (site drop_site, index i*N + j,
+ * or through the replicate rows rep_B / rep_Bc) -> +resid[i*resid_ld + j] -> store (perm != 0: row b*pN + n, col
+ * t*pdob + k to C[(t*pB + b)*pD + n*pdob + k]).  asum (optional): asum[i] = sum_k A(i, k).  Split-K (nz = 1): nsplit
+ * partial products in `partial` (partial_floats floats), summed in split order; it takes alpha and asum but no other
+ * epilogue field and a contiguous C (sCi = N, sCj = 1).  nsplit = 0: the count of gemm_splitk_plan, written back with
+ * partial_floats (0 when it is 1); with no `partial` for a plan that needs one the call is refused after the write-back. */
+typedef struct rd_debug_gemm_args {
+  const float* A; const float* B; float* C; float* asum;
+  const float* bias; const float* rowscale; const float* gate; const uint64_t* rng; const float* resid;
+  int64_t sAi, sAk, sBk, sBj, sCi, sCj;
+  int64_t sAzo, sAzi, sBzo, sBzi, sCzo, sCzi;
+  int64_t gate_ld, resid_ld, partial_floats;
+  int32_t M, N, K, ta, tb, nz, nz_inner, nsplit;
+  float alpha; int32_t relu, rowscale_mod; float gate_scale;
+  float drop_p; uint32_t drop_site; int32_t rep_B, rep_Bc;
+  int32_t perm, pB, pN, pdob, pD;
+} rd_debug_gemm_args;
+int rd_debug_gemm_f32(rd_debug_gemm_args* args, float* partial, void* stream);
+/* One item of the per-step weight split (split_weights): for w [rows, cols], lo = w - trunc19(w), t = w^T, t_lo =
+ * w^T - trunc19(w^T), rn = RN_tf32(w) (ties away from zero), rn_t = rn^T.  Every output but w may be NULL (t and t_lo
+ * together). */
+int rd_debug_split_weights(const float* w, int32_t rows, int32_t cols, float* lo, float* t, float* t_lo, float* rn,
+                           float* rn_t, void* stream);
+/* out[j] = sum_{i < rows} x[i*ld + j], j < cols: per chunk of 32 rows in row order, then the chunks in order.
+ * scratch: ceil(rows / 32) * cols floats. */
+int rd_debug_colsum(const float* x, int64_t rows, int32_t cols, int64_t ld, float* out, float* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

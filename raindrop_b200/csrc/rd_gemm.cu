@@ -207,6 +207,22 @@ int gemm(const GemmP& p, cudaStream_t st) {
     set_error("gemm: split-K needs nz == 1 and a partial buffer");
     return -2;
   }
+  // the split kernel stores alpha-scaled partial sums and reduce_partials2 writes their sum to C[i*N + j]: no other
+  // epilogue step runs, so a split-K call that asks for one (or for other C strides) would silently lose it
+  if (p.nsplit > 1 && (p.bias || p.relu || p.rowscale || p.gate || p.drop_p > 0.f || p.resid || p.perm)) {
+    set_error("gemm: split-K applies alpha only (bias, relu, rowscale, gate, dropout, resid and perm need nsplit == 1)");
+    return -2;
+  }
+  if (p.nsplit > 1 && (p.sCi != p.N || p.sCj != 1)) {
+    set_error("gemm: split-K stores C contiguously (sCi = N, sCj = 1), got sCi=%lld sCj=%lld", p.sCi, p.sCj);
+    return -2;
+  }
+  if ((p.rowscale && p.rowscale_mod < 1) || (p.drop_p > 0.f && !p.rng) || (p.drop_p > 0.f && p.rep.B && p.rep.Bc < 1) ||
+      (p.perm && (p.pB < 1 || p.pN < 1 || p.pdob < 1 || p.pD < 1))) {
+    set_error("gemm: bad epilogue (rowscale_mod=%d, dropout without rng, replicate rows Bc=%d or perm sizes)", p.rowscale_mod,
+              p.rep.Bc);
+    return -2;
+  }
   dim3 grid((unsigned)ceil_div(p.M, BM), (unsigned)ceil_div(p.N, BN), (unsigned)(p.nsplit > 1 ? p.nsplit : p.nz));
   if (grid.y > 65535 || grid.z > 65535) {
     set_error("gemm: grid too large (N tiles %u, z %u)", grid.y, grid.z);

@@ -2022,4 +2022,63 @@ int rd_debug_dropout_mask(const uint64_t* rng_captured, uint32_t site, int64_t n
   return apply_dropout(nullptr, n, p, rng_captured, site, out, (cudaStream_t)stream);
 }
 
+int rd_debug_tc_nt(rd_debug_tc_nt_args* a, void* stream) {
+  if (!a) { set_error("rd_debug_tc_nt: bad arguments"); return -2; }
+  if (a->BN == 0 || a->n_tiles == 0) tc_nt_plan(a->M, a->N, a->B_lo != nullptr, &a->BN, &a->n_tiles);
+  TcNtArgs n;
+  n.A = a->A; n.lda = a->lda; n.B = a->B; n.B_lo = a->B_lo;
+  n.M = a->M; n.N = a->N; n.K = a->K; n.BN = a->BN; n.n_tiles = a->n_tiles;
+  n.C = a->C;
+  n.bias = a->bias; n.relu = a->relu;
+  n.scale = a->scale; n.scale_mod = a->scale_mod;
+  n.gate = a->gate; n.gate_ld = a->gate_ld; n.gate_scale = a->gate_scale;
+  n.drop_p = a->drop_p; n.rng = a->rng; n.drop_site = a->drop_site; n.rep.B = a->rep_B; n.rep.Bc = a->rep_Bc;
+  n.drop_mask = a->drop_mask; n.drop_mask_ld = a->drop_mask_ld;
+  n.resid = a->resid; n.resid_ld = a->resid_ld;
+  n.round_out = a->round_out;
+  n.perm = a->perm; n.pB = a->pB; n.pN = a->pN; n.pD = a->pD;
+  return tc_nt(n, (cudaStream_t)stream);
+}
+
+int rd_debug_gemm_f32(rd_debug_gemm_args* a, float* partial, void* stream) {
+  if (!a) { set_error("rd_debug_gemm_f32: bad arguments"); return -2; }
+  GemmP g;
+  g.A = a->A; g.B = a->B; g.C = a->C;
+  g.M = a->M; g.N = a->N; g.K = a->K; g.ta = a->ta; g.tb = a->tb;
+  g.sAi = a->sAi; g.sAk = a->sAk; g.sBk = a->sBk; g.sBj = a->sBj; g.sCi = a->sCi; g.sCj = a->sCj;
+  g.nz = a->nz; g.nz_inner = a->nz_inner;
+  g.sAzo = a->sAzo; g.sAzi = a->sAzi; g.sBzo = a->sBzo; g.sBzi = a->sBzi; g.sCzo = a->sCzo; g.sCzi = a->sCzi;
+  if (a->nsplit == 0) {
+    a->partial_floats = gemm_splitk_plan(a->M, a->N, a->K, &a->nsplit);
+    if (a->partial_floats > 0 && !partial) {
+      set_error("rd_debug_gemm_f32: the split-K plan (%d splits) needs a partial buffer of %lld floats", a->nsplit,
+                (long long)a->partial_floats);
+      return -2;
+    }
+  }
+  g.nsplit = a->nsplit; g.partial = partial; g.asum = a->asum;
+  g.alpha = a->alpha; g.bias = a->bias; g.relu = a->relu;
+  g.rowscale = a->rowscale; g.rowscale_mod = a->rowscale_mod;
+  g.gate = a->gate; g.gate_ld = a->gate_ld; g.gate_scale = a->gate_scale;
+  g.drop_p = a->drop_p; g.rng = a->rng; g.drop_site = a->drop_site; g.rep.B = a->rep_B; g.rep.Bc = a->rep_Bc;
+  g.resid = a->resid; g.resid_ld = a->resid_ld;
+  g.perm = a->perm; g.pB = a->pB; g.pN = a->pN; g.pdob = a->pdob; g.pD = a->pD;
+  return gemm(g, (cudaStream_t)stream);
+}
+
+int rd_debug_split_weights(const float* w, int32_t rows, int32_t cols, float* lo, float* t, float* t_lo, float* rn,
+                           float* rn_t, void* stream) {
+  if (!w || rows < 1 || cols < 1 || (t == nullptr) != (t_lo == nullptr)) {
+    set_error("rd_debug_split_weights: bad arguments");
+    return -2;
+  }
+  WeightSplit it{w, rows, cols, lo, t, t_lo, rn, rn_t};
+  return split_weights(&it, 1, (cudaStream_t)stream);
+}
+
+int rd_debug_colsum(const float* x, int64_t rows, int32_t cols, int64_t ld, float* out, float* scratch, void* stream) {
+  if (!x || !out || !scratch || rows < 1 || cols < 0 || ld < cols) { set_error("rd_debug_colsum: bad arguments"); return -2; }
+  return colsum(x, rows, cols, ld, out, scratch, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -829,6 +829,14 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
     set_error("tc_nt: pointers must be 16-byte aligned");
     return -2;
   }
+  // the epilogue reads gate and resid as float2, writes keep-bit bytes up to column N - 1 and divides by the perm sizes
+  if ((a.gate && a.gate_ld % 2) || (a.resid && a.resid_ld % 2) || (a.drop_p > 0.f && !a.rng) ||
+      (a.drop_p > 0.f && a.rep.B && a.rep.Bc < 1) || (a.drop_mask && 32LL * a.drop_mask_ld < a.N) ||
+      (a.perm && (a.pB < 1 || a.pN < 1 || a.pD < 1))) {
+    set_error("tc_nt: bad epilogue (odd gate_ld / resid_ld, dropout without rng, replicate rows Bc=%d, keep-bit ld %d "
+              "for N=%d or perm sizes)", a.rep.Bc, a.drop_mask_ld, a.N);
+    return -2;
+  }
   NtP p;
   p.M = a.M; p.N = a.N; p.K = a.K; p.n_tiles = a.n_tiles;
   p.m_tiles = (int)ceil_div(a.M, BM);
@@ -848,27 +856,28 @@ int tc_nt(const TcNtArgs& a, cudaStream_t st) {
   p.pB = a.pB; p.pN = a.pN; p.pD = a.pD;
   p.dbg = g_gemm_dbg;
 
-  CUtensorMap tmA, tmB, tmBlo;
-  {
-    cuuint64_t d[2] = {(cuuint64_t)a.K, (cuuint64_t)a.M};
-    cuuint64_t s[1] = {(cuuint64_t)a.lda * 4};
-    cuuint32_t b[2] = {BK, BM};
-    RD_TRY(encode(&tmA, a.A, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "A"));
-  }
-  {
-    cuuint64_t d[2] = {(cuuint64_t)a.K, (cuuint64_t)a.N};
-    cuuint64_t s[1] = {(cuuint64_t)a.K * 4};
-    cuuint32_t b[2] = {BK, (cuuint32_t)a.BN};
-    RD_TRY(encode(&tmB, a.B, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "B"));
-    if (exact) RD_TRY(encode(&tmBlo, a.B_lo, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "B_lo"));
-    else tmBlo = tmB;
-  }
-  const int total = p.m_tiles * p.n_tiles;
-  const int grid = total < num_sms() ? total : num_sms();
   const int f = (a.relu ? F_RELU : 0) | (a.scale ? F_SCALE : 0) | (a.gate ? F_GATE : 0) | (a.drop_p > 0.f ? F_DROP : 0) |
                 (a.resid ? F_RESID : 0) | (a.round_out ? F_ROUND : 0) | (a.perm ? F_PERM : 0) |
                 (a.drop_p > 0.f && a.rep.B ? F_REP : 0);
+  // the tensor maps and the device queries come after every argument check (an uninstantiated epilogue included)
   auto launch = [&](auto kern) -> int {
+    CUtensorMap tmA, tmB, tmBlo;
+    {
+      cuuint64_t d[2] = {(cuuint64_t)a.K, (cuuint64_t)a.M};
+      cuuint64_t s[1] = {(cuuint64_t)a.lda * 4};
+      cuuint32_t b[2] = {BK, BM};
+      RD_TRY(encode(&tmA, a.A, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "A"));
+    }
+    {
+      cuuint64_t d[2] = {(cuuint64_t)a.K, (cuuint64_t)a.N};
+      cuuint64_t s[1] = {(cuuint64_t)a.K * 4};
+      cuuint32_t b[2] = {BK, (cuuint32_t)a.BN};
+      RD_TRY(encode(&tmB, a.B, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "B"));
+      if (exact) RD_TRY(encode(&tmBlo, a.B_lo, 2, d, s, b, CU_TENSOR_MAP_SWIZZLE_128B, "B_lo"));
+      else tmBlo = tmB;
+    }
+    const int total = p.m_tiles * p.n_tiles;
+    const int grid = total < num_sms() ? total : num_sms();
     RD_TRY(ensure_max_smem((const void*)kern, SMEM_LIMIT));   // once per (instantiation, device)
     launch_pdl(kern, dim3(grid), dim3(NT_THREADS), smem_bytes, st, tmA, tmB, tmBlo, p);
     return 0;

@@ -68,6 +68,24 @@ class RdWgradItem(C.Structure):
                 ("in_features", C.c_int32), ("d_weight", C.c_void_p), ("d_bias", C.c_void_p), ("partial", C.c_void_p)]
 
 
+class RdDebugTcNtArgs(C.Structure):
+    _fields_ = ([(f, C.c_void_p) for f in ("A", "B", "B_lo", "C", "bias", "scale", "gate", "rng", "drop_mask", "resid")] +
+                [(f, C.c_int64) for f in ("lda", "M", "gate_ld", "resid_ld")] +
+                [(f, C.c_int32) for f in ("N", "K", "BN", "n_tiles", "relu", "scale_mod")] +
+                [("gate_scale", C.c_float), ("drop_p", C.c_float), ("drop_site", C.c_uint32)] +
+                [(f, C.c_int32) for f in ("rep_B", "rep_Bc", "drop_mask_ld", "round_out", "perm", "pB", "pN", "pD")])
+
+
+class RdDebugGemmArgs(C.Structure):
+    _fields_ = ([(f, C.c_void_p) for f in ("A", "B", "C", "asum", "bias", "rowscale", "gate", "rng", "resid")] +
+                [(f, C.c_int64) for f in ("sAi", "sAk", "sBk", "sBj", "sCi", "sCj", "sAzo", "sAzi", "sBzo", "sBzi", "sCzo",
+                                          "sCzi", "gate_ld", "resid_ld", "partial_floats")] +
+                [(f, C.c_int32) for f in ("M", "N", "K", "ta", "tb", "nz", "nz_inner", "nsplit")] +
+                [("alpha", C.c_float), ("relu", C.c_int32), ("rowscale_mod", C.c_int32), ("gate_scale", C.c_float),
+                 ("drop_p", C.c_float), ("drop_site", C.c_uint32)] +
+                [(f, C.c_int32) for f in ("rep_B", "rep_Bc", "perm", "pB", "pN", "pdob", "pD")])
+
+
 # name -> (restype, argtypes); every symbol include/raindrop_b200.h declares
 SIGNATURES = {
     "rd_abi_version": (C.c_int, []),
@@ -181,6 +199,10 @@ SIGNATURES = {
     "rd_debug_dropout_mask": (C.c_int, [C.c_void_p, C.c_uint32, C.c_int64, C.c_float, C.c_void_p,
                                         C.c_void_p]),
     "rd_debug_projection_signs": (C.c_int, [C.c_uint64, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "rd_debug_tc_nt": (C.c_int, [C.POINTER(RdDebugTcNtArgs), C.c_void_p]),
+    "rd_debug_gemm_f32": (C.c_int, [C.POINTER(RdDebugGemmArgs), C.c_void_p, C.c_void_p]),
+    "rd_debug_split_weights": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 6),
+    "rd_debug_colsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rd_kfac_factors_doubles": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_ekfac_bases_floats": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_kfac_factors_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),

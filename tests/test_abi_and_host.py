@@ -37,6 +37,9 @@ def test_struct_layout_matches_header_sizes():
     assert C.sizeof(L.RdDims) == 4 * 10 + 4 * 2 + 4 * 8 + 4 * 3
     assert C.sizeof(L.RdParams) == 8 * 11 + 8 * 12 * L.RD_MAX_LAYERS
     assert C.sizeof(L.RdGrads) == 8 * 10 + 8 * 12 * L.RD_MAX_LAYERS
+    # pointers, 64-bit fields, then 17 / 21 32-bit fields and 4 bytes of tail padding
+    assert C.sizeof(L.RdDebugTcNtArgs) == 8 * 10 + 8 * 4 + 4 * 17 + 4
+    assert C.sizeof(L.RdDebugGemmArgs) == 8 * 9 + 8 * 15 + 4 * 21 + 4
 
 
 def test_workspace_queries_are_pure_host_code():

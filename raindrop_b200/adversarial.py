@@ -29,7 +29,7 @@ import torch
 import torch.distributed as dist
 
 from . import lib as L
-from .attribution import DEFAULT_SCRATCH_BYTES, _Call, _check_call, _largest_chunk
+from .attribution import _Call, _check_call
 from .train import TrainStep
 from .uncertainty import _device_key
 
@@ -119,14 +119,8 @@ def pgd(model, src, static, times, lengths, y=None, *, eps, norm="linf", n_steps
         lib, B, dev = cl.lib, src.shape[1], cl.device
         sens = _sensor_mask(sensors, plan.N, dev)
         dims = plan.dims(B, False)
-        if internal_batch_size is None:
-            spc = _largest_chunk(lambda c: lib.rd_pgd_scratch_bytes(C.byref(dims), c), B, DEFAULT_SCRATCH_BYTES)
-        else:
-            spc = min(B, int(internal_batch_size))
-        nbytes = lib.rd_pgd_scratch_bytes(C.byref(dims), spc)
-        if nbytes == 0:
-            L.check(-2, "rd_pgd_scratch_bytes")
-        scratch = cl.scratch("_pgd_scratch", (B, spc, dims.obprop_mode, dev.index), nbytes)
+        spc, scratch = cl.chunk_scratch("_pgd_scratch", "rd_pgd_scratch_bytes", dims, B, internal_batch_size,
+                                        per_sample=True)
         key = _device_key(plan, seed, step, dev) if random_start else None
         f32 = dict(device=dev, dtype=torch.float32)
         src_adv = torch.empty_like(cl.x)

@@ -81,17 +81,6 @@ def _largest_chunk(scratch_bytes, n, cap=DEFAULT_SCRATCH_BYTES):
     return lo
 
 
-def _default_steps_per_chunk(lib, dims, n_steps, cap=DEFAULT_SCRATCH_BYTES):
-    """Largest steps_per_chunk <= n_steps whose integrated-gradients scratch fits in `cap` bytes; at least 1."""
-    return _largest_chunk(lambda c: lib.rd_integrated_gradients_scratch_bytes(C.byref(dims), c), n_steps, cap)
-
-
-def _default_coalitions_per_chunk(lib, dims, n_players, n_coalitions, cap=DEFAULT_SCRATCH_BYTES):
-    """Largest coalitions_per_chunk <= n_coalitions whose coalition-attribution scratch fits in `cap` bytes; at least 1."""
-    return _largest_chunk(lambda c: lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), n_players, c), n_coalitions,
-                          cap)
-
-
 def _check_target(target, B, n_classes):
     """None, an int, or an integer tensor [B]; the range is checked on the host (one sync for a device tensor)."""
     if target is None:
@@ -131,12 +120,13 @@ def _baseline(b, like):
         raise ValueError("baseline of shape %s does not broadcast to %s" % (tuple(b.shape), tuple(like.shape))) from exc
 
 
-def _check_call(fn, model, src, static, baselines, internal_batch_size):
-    """The argument checks every attribution call shares (host only, before anything touches the device)."""
+def _check_call(fn, model, src, static, baselines, internal_batch_size, train_ok=False):
+    """The argument checks every attribution call shares (host only, before anything touches the device); a model in
+    training mode is refused unless train_ok."""
     from .models_rd import Raindrop_v2
     if not isinstance(model, Raindrop_v2):
         raise TypeError("%s takes a raindrop_b200 Raindrop_v2 model, got %s" % (fn, type(model).__name__))
-    if model.training:
+    if model.training and not train_ok:
         raise ValueError("%s runs the model in eval arithmetic: call model.eval() first" % fn)
     if internal_batch_size is not None and int(internal_batch_size) < 1:
         raise ValueError("internal_batch_size must be >= 1")
@@ -199,6 +189,27 @@ class _Call:
                 held.append(cached[1])
         return cached[1]
 
+    def chunk_scratch(self, name, query, dims, n, internal_batch_size, *query_args, per_sample=False, key=None):
+        """(chunk, scratch) of a chunked entry point whose scratch-size query is lib.<query>(dims, *query_args, chunk).
+        A chunk is internal_batch_size samples (per_sample, at most n) or max(1, internal_batch_size // B) replicates of
+        the batch, clamped to [1, n]; None: the largest chunk <= n whose scratch fits in DEFAULT_SCRATCH_BYTES.  The
+        scratch is scratch(name, key, ...), key defaulting to (B, chunk, obprop_mode, device index)."""
+        B = self.x.shape[1]
+
+        def nbytes(c):
+            return getattr(self.lib, query)(C.byref(dims), *query_args, c)
+        if internal_batch_size is None:
+            chunk = _largest_chunk(nbytes, n)
+        elif per_sample:
+            chunk = min(n, int(internal_batch_size))
+        else:
+            chunk = max(1, min(int(internal_batch_size) // B, n))
+        nb = nbytes(chunk)
+        if nb == 0:
+            L.check(-2, query)
+        key = (B, chunk, dims.obprop_mode, self.device.index) if key is None else key
+        return chunk, self.scratch(name, key, nb)
+
 
 def integrated_gradients(model, src, static, times, lengths, target=None, baselines=None, n_steps=50,
                          method="gausslegendre", internal_batch_size=None, return_convergence_delta=False):
@@ -231,15 +242,8 @@ def integrated_gradients(model, src, static, times, lengths, target=None, baseli
     lib, plan, B = cl.lib, cl.plan, src.shape[1]
 
     dims = plan.dims(B, False)
-    if internal_batch_size is None:
-        mc = _default_steps_per_chunk(lib, dims, n_steps)
-    else:
-        mc = max(1, int(internal_batch_size) // B)
-    mc = min(mc, n_steps)
-    nbytes = lib.rd_integrated_gradients_scratch_bytes(C.byref(dims), mc)
-    if nbytes == 0:
-        L.check(-2, "rd_integrated_gradients_scratch_bytes")
-    scratch = cl.scratch("_ig_attr_scratch", (B, mc, dims.obprop_mode, cl.device.index), nbytes)
+    mc, scratch = cl.chunk_scratch("_ig_attr_scratch", "rd_integrated_gradients_scratch_bytes", dims, n_steps,
+                                   internal_batch_size)
     alphas, weights = _nodes(plan, n_steps, method, cl.device)
 
     attr_src = torch.empty_like(cl.x)
@@ -454,17 +458,10 @@ def _coalition_attribution(fn, method, model, src, static, times, lengths, targe
         player, stride_t, stride_b = _cell_players(plan, cells, device)
 
     dims = plan.dims(B, False)
-    if internal_batch_size is None:
-        cc = _default_coalitions_per_chunk(lib, dims, P, n_coal)
-    else:
-        cc = max(1, int(internal_batch_size) // B)
-    cc = max(1, min(cc, n_coal))
-    nbytes = lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), P, cc)
-    if nbytes == 0:
-        L.check(-2, "rd_coalition_attribution_scratch_bytes")
     # the scratch layout follows (B, P, cc) on every call, so a buffer that is large enough is reused: with feature_mask
     # P changes whenever a batch does not reach the last time window, and that must not reallocate the scratch
-    scratch = cl.scratch("_coal_attr_scratch", device.index, nbytes)
+    cc, scratch = cl.chunk_scratch("_coal_attr_scratch", "rd_coalition_attribution_scratch_bytes", dims, n_coal,
+                                   internal_batch_size, P, key=device.index)
 
     attr = torch.empty(B, P, device=device, dtype=torch.float32)
     ends = torch.empty(2, B, plan.n_classes, device=device, dtype=torch.float32)
@@ -734,15 +731,8 @@ def kernel_shap(model, src, static, times, lengths, target=None, baselines=None,
         player, stride_t, stride_b = _cell_players(plan, cells, device)
 
     dims = plan.dims(B, False)
-    if internal_batch_size is None:
-        cc = _default_coalitions_per_chunk(lib, dims, P, max(M, 1))
-    else:
-        cc = max(1, int(internal_batch_size) // B)
-    cc = max(1, min(cc, M))
-    nbytes = lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), P, cc)
-    if nbytes == 0:
-        L.check(-2, "rd_coalition_attribution_scratch_bytes")
-    scratch = cl.scratch("_coal_attr_scratch", device.index, nbytes)
+    cc, scratch = cl.chunk_scratch("_coal_attr_scratch", "rd_coalition_attribution_scratch_bytes", dims, M,
+                                   internal_batch_size, P, key=device.index)
 
     attr = torch.empty(B, P, device=device, dtype=torch.float32)
     ends = torch.empty(2, B, plan.n_classes, device=device, dtype=torch.float32)

@@ -51,6 +51,26 @@ int make_shape(const rd_dims* d, Shape* s) {
   return 0;
 }
 
+// Raindrop_v2 embeds positions in d_pe = 16 columns and the statics in d_inp: the only embedding its entry points take.
+int check_raindrop_v2(const char* fn, const Shape& s) {
+  if (s.dpe == RD_D_PE && s.emb == s.N) return 0;
+  set_error("%s: Raindrop_v2 has d_pe = 16 and emb_dim = d_inp", fn);
+  return -2;
+}
+
+// The checks every Raindrop_v2 model entry point makes before it writes anything: dims, params, lengths and node_scale
+// not NULL, dims->training == 0 when `eval` (the entry point runs eval arithmetic), a valid Raindrop_v2 shape, and
+// statics when d_static > 0.  The caller checks its own pointer arguments after these.
+int check_model_call(const char* fn, const rd_dims* dims, const rd_params* params, const int64_t* lengths,
+                     const float* node_scale, const float* statics, bool eval, Shape* s) {
+  if (!dims || !params || !lengths || !node_scale) { set_error("%s: NULL argument", fn); return -2; }
+  if (eval && dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
+  RD_TRY(make_shape(dims, s));
+  RD_TRY(check_raindrop_v2(fn, *s));
+  if (s->ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  return 0;
+}
+
 struct Arena {
   int64_t off = 0;  // floats
   int64_t take(int64_t n) { int64_t o = off; off += round_up(n > 0 ? n : 1, 64); return o; }
@@ -299,155 +319,95 @@ IgLayout input_grad_layout(const Shape& s) {
   return l;
 }
 
-// ---- integrated gradients ------------------------------------------------------------------------------------------
-// A chunk of mc path steps runs on B*mc rows.  The arithmetic of its ob-prop GEMMs is resolved once, from the FULL
-// chunk's row count (obprop_mode 0 depends on it), and every chunk and the endpoint forward run with that explicit mode:
-// a ragged tail chunk with fewer rows cannot switch arithmetic.
-rd_dims ig_dims(const rd_dims* d, int rows, int mc) {
+// ---- chunked drivers ------------------------------------------------------------------------------------------------
+// Integrated gradients, PGD, coalition attribution, KernelSHAP, Monte Carlo dropout and smoothing run the model on chunks
+// of rows expanded from the batch.  The arithmetic of a chunk's ob-prop GEMMs is resolved once, from the row count
+// pin_rows of a FULL chunk (obprop_mode 0 depends on it), and every chunk and endpoint forward runs with that explicit
+// mode: a ragged tail chunk with fewer rows cannot switch arithmetic.
+rd_dims chunk_dims(const rd_dims* d, int rows, int64_t pin_rows, int training) {
   rd_dims e = *d;
-  e.obprop_mode = obprop_tc_exact((int64_t)d->B * mc * d->N, d->T * d->d_ob, d->obprop_mode) ? 2 : 1;
+  e.obprop_mode = obprop_tc_exact(pin_rows * d->N, d->T * d->d_ob, d->obprop_mode) ? 2 : 1;
   e.B = rows;
-  e.training = 0;
+  e.training = training;
   return e;
 }
 
-// Scratch of rd_raindrop_v2_integrated_gradients: the forward workspace of max(B*mc, 2B) rows (chunks and the endpoint
-// forward), the chunk's backward scratch, the input-gradient buffers (W1^T, its remainder, dX0), the expanded inputs
-// (max(B*mc, 2B) rows), the chunk's one-hot d_logits and logits, and the running sums [B*N*T] and [B, d_static].
-struct IgcLayout { int64_t ws, sc, W1t, W1tlo, dX0, src, statics, times, lengths, dlogits, logits, acc_src, acc_static, total; };
-int ig_layout(const rd_dims* dims, int mc, IgcLayout* l) {
-  if (mc < 1 || (int64_t)dims->B * mc > (1LL << 30)) { set_error("steps_per_chunk = %d out of range", mc); return -2; }
-  const int Bc = dims->B * mc, Bx = Bc > 2 * dims->B ? Bc : 2 * dims->B;
-  const rd_dims dc = ig_dims(dims, Bc, mc), dx = ig_dims(dims, Bx, mc);
+// The expanded inputs of a chunk; statics is nullptr without a static branch.
+struct Expanded { float* src; float* statics; float* times; int64_t* lengths; };
+
+// Scratch of a chunked driver whose chunk is n units of `per` rows (`what` names n in the range check): the forward
+// workspace and the expanded inputs of the forward's rows (the chunk's, or at least 2B with an endpoint forward), the
+// chunk's logits and, when the chunk runs a backward, its backward scratch, W1^T with its remainder, dX0 and d_logits.
+// A driver takes its own pieces from `a` after these.
+struct ChunkLayout {
+  Arena a;
+  int64_t ws, sc, W1t, W1tlo, dX0, dlogits, src, statics, times, lengths, logits;
+  Expanded inputs(float* S, int ds) const {
+    return {S + src, ds > 0 ? S + statics : nullptr, S + times, reinterpret_cast<int64_t*>(S + lengths)};
+  }
+};
+int chunk_layout(const rd_dims* dims, const char* what, int n, int per, bool endpoints, int training, bool bwd,
+                 ChunkLayout* l) {
+  if (n < 1 || (int64_t)per * n > (1LL << 30)) { set_error("%s = %d out of range", what, n); return -2; }
+  const int rows = per * n, fwd_rows = endpoints && rows < 2 * dims->B ? 2 * dims->B : rows;
+  const rd_dims dc = chunk_dims(dims, rows, rows, training), dx = chunk_dims(dims, fwd_rows, rows, training);
   Shape sc, sx;
   RD_TRY(make_shape(&dc, &sc));
   RD_TRY(make_shape(&dx, &sx));
-  Arena a;
+  Arena& a = l->a;
   l->ws = a.take(ws_layout(sx).total);
-  l->sc = a.take(bw_layout(sc).total);
-  l->W1t = a.take((int64_t)sc.C * sc.C);
-  l->W1tlo = a.take((int64_t)sc.C * sc.C);
-  l->dX0 = a.take(sc.M1 * sc.C);
+  if (bwd) {
+    l->sc = a.take(bw_layout(sc).total);
+    l->W1t = a.take((int64_t)sc.C * sc.C);
+    l->W1tlo = a.take((int64_t)sc.C * sc.C);
+    l->dX0 = a.take(sc.M1 * sc.C);
+    l->dlogits = a.take((int64_t)rows * sc.ncls);
+  }
   l->src = a.take(sx.M2 * 2 * sx.N);
-  l->statics = a.take((int64_t)Bx * sx.ds);
+  l->statics = a.take((int64_t)fwd_rows * sx.ds);
   l->times = a.take(sx.M2);
-  l->lengths = a.take(2LL * Bx);
-  l->dlogits = a.take((int64_t)Bc * sc.ncls);
-  l->logits = a.take((int64_t)Bc * sc.ncls);
-  l->acc_src = a.take((int64_t)dims->B * sc.N * sc.T);
-  l->acc_static = a.take((int64_t)dims->B * sc.ds);
-  l->total = a.off;
+  l->lengths = a.take(2LL * fwd_rows);
+  l->logits = a.take((int64_t)rows * sx.ncls);
   return 0;
 }
 
-// ---- PGD adversarial examples ---------------------------------------------------------------------------------------
-// A chunk of m <= spc samples runs on m rows in the arithmetic pinned from spc rows (ig_dims with one step per chunk).
-rd_dims pgd_dims(const rd_dims* d, int rows, int spc) {
-  rd_dims e = *d;
-  e.B = spc;
-  return ig_dims(&e, rows, 1);
-}
-// Scratch of rd_raindrop_v2_pgd: the forward workspace and backward scratch of spc rows, W1^T with its remainder, dX0,
-// the chunk's inputs, logits and d_logits, the perturbation and l2 gradient [spc, T*N + ds] and the best losses (fp64).
-struct PgdLayout { int64_t ws, sc, W1t, W1tlo, dX0, src, statics, times, lengths, logits, dlogits, delta, grad, best, total; };
-int pgd_layout(const rd_dims* dims, int spc, PgdLayout* l) {
-  if (spc < 1 || spc > (1 << 30)) { set_error("samples_per_chunk = %d out of range", spc); return -2; }
-  const rd_dims dc = pgd_dims(dims, spc, spc);
-  Shape s;
-  RD_TRY(make_shape(&dc, &s));
-  const int64_t E = (int64_t)s.T * s.N + s.ds;
-  Arena a;
-  l->ws = a.take(ws_layout(s).total);
-  l->sc = a.take(bw_layout(s).total);
-  l->W1t = a.take((int64_t)s.C * s.C);
-  l->W1tlo = a.take((int64_t)s.C * s.C);
-  l->dX0 = a.take(s.M1 * s.C);
-  l->src = a.take(s.M2 * 2 * s.N);
-  l->statics = a.take((int64_t)spc * s.ds);
-  l->times = a.take(s.M2);
-  l->lengths = a.take(2LL * spc);
-  l->logits = a.take((int64_t)spc * s.ncls);
-  l->dlogits = a.take((int64_t)spc * s.ncls);
-  l->delta = a.take(spc * E);
-  l->grad = a.take(spc * E);
-  l->best = a.take(2LL * spc);
-  l->total = a.off;
+// Integrated gradients: chunks of mc path steps (B*mc rows) with a backward, the endpoint forward on 2B rows, and the
+// running sums [B*N*T] and [B, d_static].
+struct IgScratch : ChunkLayout { int64_t acc_src, acc_static; };
+int ig_scratch(const rd_dims* dims, int mc, IgScratch* l) {
+  RD_TRY(chunk_layout(dims, "steps_per_chunk", mc, dims->B, true, 0, true, l));
+  l->acc_src = l->a.take((int64_t)dims->B * dims->N * dims->T);
+  l->acc_static = l->a.take((int64_t)dims->B * dims->d_static);
   return 0;
 }
 
-// ---- coalition attribution (Shapley-value sampling, ablation) -------------------------------------------------------
-// Scratch of rd_raindrop_v2_coalition_attribution and rd_raindrop_v2_cell_coalition_attribution: the eval forward
-// workspace and the expanded inputs of max(B*cc, 2B) rows (chunks of cc coalitions and the endpoint forward), the
-// chunk's logits, the fp64 running sums [B, P] and the chunk's keep table [cc, P] (uint8, Shapley).  The ob-prop mode is pinned
-// from B*cc rows by ig_dims, as for integrated gradients.
-struct CoalLayout { int64_t ws, src, statics, times, lengths, logits, acc, keep, total; };
-int coalition_layout(const rd_dims* dims, int n_players, int cc, CoalLayout* l) {
-  if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("coalitions_per_chunk = %d out of range", cc); return -2; }
+// PGD: chunks of spc samples with a backward, the perturbation and l2 gradient [spc, T*N + ds] and the best losses (fp64).
+struct PgdScratch : ChunkLayout { int64_t delta, grad, best; };
+int pgd_scratch(const rd_dims* dims, int spc, PgdScratch* l) {
+  RD_TRY(chunk_layout(dims, "samples_per_chunk", spc, 1, false, 0, true, l));
+  const int64_t E = (int64_t)dims->T * dims->N + dims->d_static;
+  l->delta = l->a.take(spc * E);
+  l->grad = l->a.take(spc * E);
+  l->best = l->a.take(2LL * spc);
+  return 0;
+}
+
+// Coalition attribution (Shapley-value sampling, ablation, KernelSHAP): chunks of cc coalitions (B*cc rows), the
+// endpoint forward on 2B rows, the fp64 running sums [B, P] and the chunk's keep table [cc, P] (uint8, Shapley).
+struct CoalScratch : ChunkLayout { int64_t acc, keep; };
+int coalition_scratch(const rd_dims* dims, int n_players, int cc, CoalScratch* l) {
+  RD_TRY(chunk_layout(dims, "coalitions_per_chunk", cc, dims->B, true, 0, false, l));
   if (n_players < 1) { set_error("n_players = %d must be >= 1", n_players); return -2; }
-  const int Bc = dims->B * cc, Bx = Bc > 2 * dims->B ? Bc : 2 * dims->B;
-  const rd_dims dx = ig_dims(dims, Bx, cc);
-  Shape sx;
-  RD_TRY(make_shape(&dx, &sx));
-  Arena a;
-  l->ws = a.take(ws_layout(sx).total);
-  l->src = a.take(sx.M2 * 2 * sx.N);
-  l->statics = a.take((int64_t)Bx * sx.ds);
-  l->times = a.take(sx.M2);
-  l->lengths = a.take(2LL * Bx);
-  l->logits = a.take((int64_t)Bc * sx.ncls);
-  l->acc = a.take(2LL * dims->B * n_players);
-  l->keep = a.take(ceil_div((int64_t)cc * n_players, 4));
-  l->total = a.off;
+  l->acc = l->a.take(2LL * dims->B * n_players);
+  l->keep = l->a.take(ceil_div((int64_t)cc * n_players, 4));
   return 0;
 }
 
-// ---- Monte Carlo dropout -------------------------------------------------------------------------------------------
-// A chunk of cc replicates is one training-mode forward on B*cc replicate-major rows.  Its ob-prop arithmetic is pinned
-// from the full chunk's row count, as for integrated gradients, so a ragged tail chunk cannot switch it.
-rd_dims mc_dims(const rd_dims* d, int rows, int cc) {
-  rd_dims e = ig_dims(d, rows, cc);
-  e.training = 1;
-  return e;
-}
-// Scratch of rd_raindrop_v2_mc_dropout: the training forward workspace of B*cc rows, the expanded inputs, the chunk's
-// logits and the fp64 sums [B, 2*n_classes + 1].
-struct McLayout { int64_t ws, src, statics, times, lengths, logits, acc, total; };
-int mc_layout(const rd_dims* dims, int cc, McLayout* l) {
-  if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("replicates_per_chunk = %d out of range", cc); return -2; }
-  const int Bc = dims->B * cc;
-  const rd_dims dc = mc_dims(dims, Bc, cc);
-  Shape sc;
-  RD_TRY(make_shape(&dc, &sc));
-  Arena a;
-  l->ws = a.take(ws_layout(sc).total);
-  l->src = a.take(sc.M2 * 2 * sc.N);
-  l->statics = a.take((int64_t)Bc * sc.ds);
-  l->times = a.take(sc.M2);
-  l->lengths = a.take(2LL * Bc);
-  l->logits = a.take((int64_t)Bc * sc.ncls);
-  l->acc = a.take(2LL * dims->B * (2 * sc.ncls + 1));
-  l->total = a.off;
-  return 0;
-}
-
-// ---- randomized smoothing ------------------------------------------------------------------------------------------
-// Scratch of rd_raindrop_v2_smooth_counts: the eval forward workspace of B*cc rows, the chunk's noisy inputs and its
-// logits.  The ob-prop mode is pinned from B*cc rows by ig_dims, as for integrated gradients.
-struct SmoothLayout { int64_t ws, src, statics, times, lengths, logits, total; };
-int smooth_layout(const rd_dims* dims, int cc, SmoothLayout* l) {
-  if (cc < 1 || (int64_t)dims->B * cc > (1LL << 30)) { set_error("replicates_per_chunk = %d out of range", cc); return -2; }
-  const int Bc = dims->B * cc;
-  const rd_dims dc = ig_dims(dims, Bc, cc);
-  Shape sc;
-  RD_TRY(make_shape(&dc, &sc));
-  Arena a;
-  l->ws = a.take(ws_layout(sc).total);
-  l->src = a.take(sc.M2 * 2 * sc.N);
-  l->statics = a.take((int64_t)Bc * sc.ds);
-  l->times = a.take(sc.M2);
-  l->lengths = a.take(2LL * Bc);
-  l->logits = a.take((int64_t)Bc * sc.ncls);
-  l->total = a.off;
+// Monte Carlo dropout: chunks of cc replicates (B*cc rows, training forwards) and the fp64 sums [B, 2*n_classes + 1].
+struct McScratch : ChunkLayout { int64_t acc; };
+int mc_scratch(const rd_dims* dims, int cc, McScratch* l) {
+  RD_TRY(chunk_layout(dims, "replicates_per_chunk", cc, dims->B, false, 1, false, l));
+  l->acc = l->a.take(2LL * dims->B * (2 * dims->n_classes + 1));
   return 0;
 }
 
@@ -668,7 +628,7 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
                         cudaStream_t st, int rep_B = 0, uint64_t rep_step = 0) {
   Shape s;
   RD_TRY(make_shape(dims, &s));
-  if (!encoder_only && (s.dpe != RD_D_PE || s.emb != s.N)) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
+  if (!encoder_only) RD_TRY(check_raindrop_v2("rd_raindrop_v2_fwd", s));
   // a training forward is followed by a backward: refuse before any output is written or the rng counter moves.  Monte
   // Carlo replicates (rep_B > 0) are training forwards that no backward follows.
   if (dims->training && rep_B == 0 && !head_bwd_supported(s.Df)) {
@@ -969,6 +929,22 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   return 0;
 }
 
+// W1^T with its error-compensation remainder, which input_grad_dx0 reads on the tensor cores (nothing on the CUDA cores)
+static int prepare_w1t(const Shape& s, const rd_params* P, float* W1t, float* W1tlo, cudaStream_t st) {
+  if (!s.tc) return 0;
+  const WeightSplit it = {P->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
+  return split_weights(&it, 1, st);
+}
+
+// The input gradient of a chunk of a chunked driver (rows dc, shape s) after its forward: the backward from the chunk's
+// d_logits into its backward scratch, then dX0.
+static int chunk_input_grad(const rd_dims* dc, const Shape& s, const rd_params* P, const Expanded& x,
+                            const float* node_scale, float* S, const ChunkLayout& l, cudaStream_t st) {
+  RD_TRY(raindrop_bwd(dc, P, x.statics, x.lengths, node_scale, S + l.ws, S + l.dlogits, nullptr, S + l.sc, RD_BWD_ALL,
+                      nullptr, st));
+  return input_grad_dx0(s, P, S + l.sc + bw_layout(s).gO1, S + l.W1t, S + l.W1tlo, S + l.dX0, st);
+}
+
 }  // namespace rd
 
 // =================================================================================================
@@ -1200,10 +1176,7 @@ int rd_raindrop_v2_input_grad(const rd_dims* dims, const rd_params* params, cons
     const IgLayout il = input_grad_layout(s);
     float* W1t = (float*)scratch + il.W1t; float* W1tlo = (float*)scratch + il.W1tlo;
     dX0 = (float*)scratch + il.dX0;
-    if (s.tc) {
-      const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
-      RD_TRY(split_weights(&it, 1, st));
-    }
+    RD_TRY(prepare_w1t(s, params, W1t, W1tlo, st));
     RD_TRY(input_grad_dx0(s, params, sc + b.gO1, W1t, W1tlo, dX0, st));
   }
   return input_grad(src, params->R_u, dX0, s.B, s.T, s.N, s.dob, s.p, reinterpret_cast<const uint64_t*>(ws + w.rng), d_src,
@@ -1212,10 +1185,9 @@ int rd_raindrop_v2_input_grad(const rd_dims* dims, const rd_params* params, cons
 }
 
 size_t rd_integrated_gradients_scratch_bytes(const rd_dims* dims, int32_t steps_per_chunk) {
-  if (!dims) return 0;
-  IgcLayout l;
-  if (ig_layout(dims, steps_per_chunk, &l) != 0) return 0;
-  return (size_t)l.total * sizeof(float);
+  IgScratch l;
+  if (!dims || ig_scratch(dims, steps_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
 }
 
 int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
@@ -1224,73 +1196,54 @@ int rd_raindrop_v2_integrated_gradients(const rd_dims* dims, const rd_params* pa
                                         const float* alphas, const float* weights, int32_t n_steps, int32_t steps_per_chunk,
                                         void* scratch, float* attr_src, float* attr_statics, float* endpoint_logits,
                                         void* stream) {
-  if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !alphas || !weights || !scratch ||
-      !attr_src || !endpoint_logits || !params->R_u || !params->ob1_value_weight) {
-    set_error("rd_raindrop_v2_integrated_gradients: NULL argument");
-    return -2;
-  }
-  if (n_steps < 1 || steps_per_chunk < 1) { set_error("rd_raindrop_v2_integrated_gradients: n_steps and steps_per_chunk must be >= 1"); return -2; }
-  if (dims->training) { set_error("rd_raindrop_v2_integrated_gradients: runs eval arithmetic, dims->training must be 0"); return -2; }
+  const char* fn = "rd_raindrop_v2_integrated_gradients";
   Shape s0;
-  RD_TRY(make_shape(dims, &s0));
-  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s0.ds > 0 && (!statics || !baseline_statics)) {
-    set_error("rd_raindrop_v2_integrated_gradients: d_static > 0 needs statics and baseline_statics");
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !baseline_src || !alphas || !weights || !scratch || !attr_src || !endpoint_logits || !params->R_u ||
+      !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
     return -2;
   }
-  IgcLayout l;
-  RD_TRY(ig_layout(dims, steps_per_chunk, &l));
+  if (s0.ds > 0 && !baseline_statics) { set_error("%s: d_static > 0 needs baseline_statics", fn); return -2; }
+  if (n_steps < 1 || steps_per_chunk < 1) { set_error("%s: n_steps and steps_per_chunk must be >= 1", fn); return -2; }
+  IgScratch l;
+  RD_TRY(ig_scratch(dims, steps_per_chunk, &l));
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s0.B, mc = steps_per_chunk;
   float* S = (float*)scratch;
-  float* ws = S + l.ws; float* sc = S + l.sc; float* dX0 = S + l.dX0;
-  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
-  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
-  float* dlog = S + l.dlogits;
-  float* W1t = S + l.W1t; float* W1tlo = S + l.W1tlo;
+  const Expanded x = l.inputs(S, s0.ds);
   float* attr_st = s0.ds > 0 ? attr_statics : nullptr;
 
   // 1. the endpoints: one forward on 2B rows (baseline rows, then input rows) -> endpoint_logits [2, B, ncls]
-  const rd_dims de = ig_dims(dims, 2 * B, mc);
+  const rd_dims de = chunk_dims(dims, 2 * B, (int64_t)B * mc, 0);
   RD_TRY(ig_expand(src, baseline_src, statics, baseline_statics, times, lengths, nullptr, 2, B, s0.T, s0.N, s0.ds, s0.ncls,
-                   nullptr, nullptr, src_e, stat_e, times_e, len_e, nullptr, st));
-  RD_TRY(raindrop_fwd(&de, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, endpoint_logits, nullptr, nullptr,
-                      nullptr, 0, st));
+                   nullptr, nullptr, x.src, x.statics, x.times, x.lengths, nullptr, st));
+  RD_TRY(raindrop_fwd(&de, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, endpoint_logits,
+                      nullptr, nullptr, nullptr, 0, st));
   // 2. W1^T with its remainder, once per call
-  {
-    const rd_dims dc = ig_dims(dims, B * mc, mc);
-    Shape s;
-    RD_TRY(make_shape(&dc, &s));
-    if (s.tc) {
-      const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
-      RD_TRY(split_weights(&it, 1, st));
-    }
-  }
+  RD_TRY(prepare_w1t(s0, params, S + l.W1t, S + l.W1tlo, st));
   // 3. chunks of mc steps (the last one possibly shorter, same scratch, same arithmetic mode)
   for (int c0 = 0; c0 < n_steps; c0 += mc) {
     const int m = n_steps - c0 < mc ? n_steps - c0 : mc;
-    const rd_dims dc = ig_dims(dims, B * m, mc);
+    const rd_dims dc = chunk_dims(dims, B * m, (int64_t)B * mc, 0);
     Shape s;
     RD_TRY(make_shape(&dc, &s));
-    const BwLayout b = bw_layout(s);
     RD_TRY(ig_expand(src, baseline_src, statics, baseline_statics, times, lengths, alphas + c0, m, B, s.T, s.N, s.ds, s.ncls,
-                     target, endpoint_logits + (int64_t)B * s.ncls, src_e, stat_e, times_e, len_e, dlog, st));
-    RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, ws, S + l.logits, nullptr, nullptr,
-                        nullptr, 0, st));
-    RD_TRY(raindrop_bwd(&dc, params, stat_e, len_e, node_scale, ws, dlog, nullptr, sc, RD_BWD_ALL, nullptr, st));
-    RD_TRY(input_grad_dx0(s, params, sc + b.gO1, W1t, W1tlo, dX0, st));
-    RD_TRY(ig_accumulate(src, baseline_src, alphas + c0, weights + c0, m, B, s.T, s.N, s.dob, params->R_u, dX0, S + l.acc_src,
-                         attr_src, statics, baseline_statics, sc + b.dfeat, s.Df, s.D, params->emb_weight, s.emb, s.ds,
-                         S + l.acc_static, attr_st, c0 == 0, c0 + m >= n_steps, st));
+                     target, endpoint_logits + (int64_t)B * s.ncls, x.src, x.statics, x.times, x.lengths, S + l.dlogits, st));
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, S + l.logits,
+                        nullptr, nullptr, nullptr, 0, st));
+    RD_TRY(chunk_input_grad(&dc, s, params, x, node_scale, S, l, st));
+    RD_TRY(ig_accumulate(src, baseline_src, alphas + c0, weights + c0, m, B, s.T, s.N, s.dob, params->R_u, S + l.dX0,
+                         S + l.acc_src, attr_src, statics, baseline_statics, S + l.sc + bw_layout(s).dfeat, s.Df, s.D,
+                         params->emb_weight, s.emb, s.ds, S + l.acc_static, attr_st, c0 == 0, c0 + m >= n_steps, st));
   }
   return 0;
 }
 
 size_t rd_pgd_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk) {
-  if (!dims) return 0;
-  PgdLayout l;
-  if (pgd_layout(dims, samples_per_chunk, &l) != 0) return 0;
-  return (size_t)l.total * sizeof(float);
+  PgdScratch l;
+  if (!dims || pgd_scratch(dims, samples_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
 }
 
 int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
@@ -1300,12 +1253,13 @@ int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float
                        int32_t samples_per_chunk, void* scratch, float* src_adv, float* statics_adv, float* logits_adv,
                        float* logits_clean, float* loss_adv, void* stream) {
   const char* fn = "rd_raindrop_v2_pgd";
-  if (!dims || !params || !src || !times || !lengths || !node_scale || !scratch || !src_adv || !logits_adv ||
-      !logits_clean || !loss_adv || !params->R_u || !params->ob1_value_weight) {
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !scratch || !src_adv || !logits_adv || !logits_clean || !loss_adv || !params->R_u ||
+      !params->ob1_value_weight) {
     set_error("%s: NULL argument", fn);
     return -2;
   }
-  if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
   if (norm != RD_PGD_LINF && norm != RD_PGD_L2) { set_error("%s: norm must be RD_PGD_LINF or RD_PGD_L2, got %d", fn, norm); return -2; }
   if (!(eps >= 0.f) || !(alpha >= 0.f) || isinf(eps) || isinf(alpha) || n_steps < 0) {
     set_error("%s: eps and alpha must be finite and >= 0, n_steps >= 0 (eps = %g, alpha = %g, n_steps = %d)", fn, eps,
@@ -1313,61 +1267,49 @@ int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float
     return -2;
   }
   if (random_start && !rng) { set_error("%s: random_start needs rng", fn); return -2; }
-  Shape s0;
-  RD_TRY(make_shape(dims, &s0));
-  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s0.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
   if (perturb_static && s0.ds == 0) { set_error("%s: perturb_static needs a static branch (d_static > 0)", fn); return -2; }
   const int B = s0.B, spc = samples_per_chunk;
-  PgdLayout l;
-  RD_TRY(pgd_layout(dims, spc, &l));
+  PgdScratch l;
+  RD_TRY(pgd_scratch(dims, spc, &l));
   cudaStream_t st = (cudaStream_t)stream;
   float* S = (float*)scratch;
-  float* ws = S + l.ws; float* sc = S + l.sc; float* dX0 = S + l.dX0; float* W1t = S + l.W1t; float* W1tlo = S + l.W1tlo;
-  float* lg = S + l.logits; float* dlog = S + l.dlogits;
+  float* lg = S + l.logits;
   double* best = reinterpret_cast<double*>(S + l.best);
+  const Expanded x = l.inputs(S, s0.ds);
   PgdArgs a;
   a.src = src; a.statics = s0.ds > 0 ? statics : nullptr; a.times = times; a.lengths = lengths;
   a.sens = sensor_perturbable; a.attacked = sample_attacked;
-  a.x_e = S + l.src; a.st_e = s0.ds > 0 ? S + l.statics : nullptr; a.times_e = S + l.times;
-  a.len_e = reinterpret_cast<int64_t*>(S + l.lengths); a.delta = S + l.delta; a.grad = S + l.grad;
+  a.x_e = x.src; a.st_e = x.statics; a.times_e = x.times; a.len_e = x.lengths; a.delta = S + l.delta; a.grad = S + l.grad;
   a.B = B; a.T = s0.T; a.N = s0.N; a.ds = s0.ds; a.pst = perturb_static ? 1 : 0;
   // W1^T with its remainder, once per call
-  {
-    const rd_dims dc = pgd_dims(dims, spc, spc);
-    Shape s;
-    RD_TRY(make_shape(&dc, &s));
-    if (s.tc && n_steps > 0) {
-      const WeightSplit it = {params->ob1_value_weight, s.C, s.C, nullptr, W1t, W1tlo};
-      RD_TRY(split_weights(&it, 1, st));
-    }
-  }
+  if (n_steps > 0) RD_TRY(prepare_w1t(s0, params, S + l.W1t, S + l.W1tlo, st));
   for (int c0 = 0; c0 < B; c0 += spc) {
     const int m = B - c0 < spc ? B - c0 : spc;
-    const rd_dims dc = pgd_dims(dims, m, spc);
+    const rd_dims dc = chunk_dims(dims, m, spc, 0);
     Shape s;
     RD_TRY(make_shape(&dc, &s));
-    const BwLayout b = bw_layout(s);
+    const float* dfeat = S + l.sc + bw_layout(s).dfeat;
     a.m = m; a.c0 = c0;
     float* clean = logits_clean + (int64_t)c0 * s.ncls;
     RD_TRY(pgd_expand(a, st));
-    RD_TRY(raindrop_fwd(&dc, params, a.x_e, a.st_e, a.times_e, a.len_e, node_scale, nullptr, ws, clean, nullptr, nullptr,
-                        nullptr, 0, st));
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, clean, nullptr,
+                        nullptr, nullptr, 0, st));
     const float* cur = clean;
     if (random_start) {
       RD_TRY(pgd_start(a, norm, eps, rng, st));
-      RD_TRY(raindrop_fwd(&dc, params, a.x_e, a.st_e, a.times_e, a.len_e, node_scale, nullptr, ws, lg, nullptr, nullptr,
-                          nullptr, 0, st));
+      RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, lg, nullptr,
+                          nullptr, nullptr, 0, st));
       cur = lg;
     }
     for (int k = 0;; ++k) {
-      RD_TRY(pgd_track(a, s.ncls, cur, logits_clean, y, best, k == 0, dlog, src_adv, statics_adv, logits_adv, loss_adv, st));
+      RD_TRY(pgd_track(a, s.ncls, cur, logits_clean, y, best, k == 0, S + l.dlogits, src_adv, statics_adv, logits_adv,
+                       loss_adv, st));
       if (k == n_steps) break;
-      RD_TRY(raindrop_bwd(&dc, params, a.st_e, a.len_e, node_scale, ws, dlog, nullptr, sc, RD_BWD_ALL, nullptr, st));
-      RD_TRY(input_grad_dx0(s, params, sc + b.gO1, W1t, W1tlo, dX0, st));
-      RD_TRY(pgd_step(a, norm, eps, alpha, params->R_u, s.dob, dX0, sc + b.dfeat, s.Df, s.D, params->emb_weight, s.emb, st));
-      RD_TRY(raindrop_fwd(&dc, params, a.x_e, a.st_e, a.times_e, a.len_e, node_scale, nullptr, ws, lg, nullptr, nullptr,
-                          nullptr, 0, st));
+      RD_TRY(chunk_input_grad(&dc, s, params, x, node_scale, S, l, st));
+      RD_TRY(pgd_step(a, norm, eps, alpha, params->R_u, s.dob, S + l.dX0, dfeat, s.Df, s.D, params->emb_weight, s.emb,
+                      st));
+      RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, lg, nullptr,
+                          nullptr, nullptr, 0, st));
       cur = lg;
     }
   }
@@ -1375,50 +1317,44 @@ int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float
 }
 
 size_t rd_coalition_attribution_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t coalitions_per_chunk) {
-  if (!dims) return 0;
-  CoalLayout l;
-  if (coalition_layout(dims, n_players, coalitions_per_chunk, &l) != 0) return 0;
-  return (size_t)l.total * sizeof(float);
+  CoalScratch l;
+  if (!dims || coalition_scratch(dims, n_players, coalitions_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
 }
 
 // What every coalition entry point (Shapley sampling and ablation, KernelSHAP) shares: the argument checks, the scratch
-// carved by coalition_layout and the endpoint forward.  `fn` names the caller in error messages.
+// carved by coalition_scratch and the endpoint forward.  `fn` names the caller in error messages.
 struct CoalRun {
   Shape s0;
   int P, G, B, cc;
-  float* ws; float* logits; float* src_e; float* stat_e; float* times_e; int64_t* len_e; double* acc; uint8_t* keep;
+  Expanded x;
+  float* ws; float* logits; double* acc; uint8_t* keep;
 };
 static int coalition_setup(const char* fn, const rd_dims* dims, const rd_params* params, const float* src,
                            const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
                            const float* baseline_src, const float* baseline_statics, const int32_t* cell_player,
                            int64_t stride_t, int64_t stride_b, int32_t n_players, int32_t coalitions_per_chunk, void* scratch,
                            const float* attr, const float* endpoint_logits, CoalRun* r) {
-  if (!dims || !params || !src || !times || !lengths || !node_scale || !baseline_src || !cell_player || !scratch || !attr ||
-      !endpoint_logits || !params->R_u || !params->ob1_value_weight) {
+  Shape& s0 = r->s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !baseline_src || !cell_player || !scratch || !attr || !endpoint_logits || !params->R_u ||
+      !params->ob1_value_weight) {
     set_error("%s: NULL argument", fn);
     return -2;
   }
-  if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
-  Shape& s0 = r->s0;
-  RD_TRY(make_shape(dims, &s0));
-  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s0.ds > 0 && (!statics || !baseline_statics)) {
-    set_error("%s: d_static > 0 needs statics and baseline_statics", fn);
-    return -2;
-  }
+  if (s0.ds > 0 && !baseline_statics) { set_error("%s: d_static > 0 needs baseline_statics", fn); return -2; }
   const int P = n_players, G = P - (s0.ds > 0 ? 1 : 0);
   if (G < 1) { set_error("%s: n_players = %d gives %d players of the value cells, need >= 1", fn, P, G); return -2; }
   if (stride_t < 0 || stride_b < 0) {
     set_error("%s: player strides must be >= 0, got (%lld, %lld)", fn, (long long)stride_t, (long long)stride_b);
     return -2;
   }
-  CoalLayout l;
-  RD_TRY(coalition_layout(dims, P, coalitions_per_chunk, &l));
+  CoalScratch l;
+  RD_TRY(coalition_scratch(dims, P, coalitions_per_chunk, &l));
   r->P = P; r->G = G; r->B = s0.B; r->cc = coalitions_per_chunk;
   float* S = (float*)scratch;
+  r->x = l.inputs(S, s0.ds);
   r->ws = S + l.ws; r->logits = S + l.logits;
-  r->src_e = S + l.src; r->stat_e = s0.ds > 0 ? S + l.statics : nullptr; r->times_e = S + l.times;
-  r->len_e = reinterpret_cast<int64_t*>(S + l.lengths);
   r->acc = reinterpret_cast<double*>(S + l.acc);
   r->keep = reinterpret_cast<uint8_t*>(S + l.keep);
   return 0;
@@ -1430,12 +1366,12 @@ static int coalition_endpoints(const CoalRun& r, const rd_dims* dims, const rd_p
                                const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
                                const float* baseline_src, const float* baseline_statics, const int32_t* cell_player,
                                int64_t stride_t, int64_t stride_b, float* endpoint_logits, cudaStream_t st) {
-  const rd_dims de = ig_dims(dims, 2 * r.B, r.cc);
+  const rd_dims de = chunk_dims(dims, 2 * r.B, (int64_t)r.B * r.cc, 0);
   RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
-                          nullptr, r.P, r.G, COALITION_ENDPOINTS, 0, 2, r.B, r.s0.T, r.s0.N, r.s0.ds, nullptr, r.src_e,
-                          r.stat_e, r.times_e, r.len_e, st));
-  return raindrop_fwd(&de, params, r.src_e, r.stat_e, r.times_e, r.len_e, node_scale, nullptr, r.ws, endpoint_logits, nullptr,
-                      nullptr, nullptr, 0, st);
+                          nullptr, r.P, r.G, COALITION_ENDPOINTS, 0, 2, r.B, r.s0.T, r.s0.N, r.s0.ds, nullptr, r.x.src,
+                          r.x.statics, r.x.times, r.x.lengths, st));
+  return raindrop_fwd(&de, params, r.x.src, r.x.statics, r.x.times, r.x.lengths, node_scale, nullptr, r.ws, endpoint_logits,
+                      nullptr, nullptr, nullptr, 0, st);
 }
 
 // The one implementation behind both Shapley-sampling / ablation entry points.
@@ -1469,12 +1405,12 @@ static int coalition_attribution(const char* fn, const rd_dims* dims, const rd_p
   do {
     const int nc = n_coal - c0 < cc ? n_coal - c0 : cc;
     if (nc > 0) {
-      const rd_dims dc = ig_dims(dims, B * nc, cc);
+      const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
       RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, stride_t, stride_b,
-                              orders, P, G, method, c0, nc, B, r.s0.T, r.s0.N, r.s0.ds, r.keep, r.src_e, r.stat_e, r.times_e,
-                              r.len_e, st));
-      RD_TRY(raindrop_fwd(&dc, params, r.src_e, r.stat_e, r.times_e, r.len_e, node_scale, nullptr, r.ws, r.logits, nullptr,
-                          nullptr, nullptr, 0, st));
+                              orders, P, G, method, c0, nc, B, r.s0.T, r.s0.N, r.s0.ds, r.keep, r.x.src, r.x.statics,
+                              r.x.times, r.x.lengths, st));
+      RD_TRY(raindrop_fwd(&dc, params, r.x.src, r.x.statics, r.x.times, r.x.lengths, node_scale, nullptr, r.ws, r.logits,
+                          nullptr, nullptr, nullptr, 0, st));
     }
     RD_TRY(coalition_accumulate(r.logits, endpoint_logits, target, orders, P, method, m, c0, nc, B, r.s0.ncls, r.acc, attr,
                                 c0 == 0, c0 + nc >= n_coal, st));
@@ -1551,12 +1487,13 @@ int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, con
   do {
     const int nc = (int)(M - c0 < cc ? M - c0 : cc);
     if (nc > 0) {
-      const rd_dims dc = ig_dims(dims, B * nc, cc);
+      const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
       RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, player_stride_t,
                               player_stride_b, nullptr, P, G, COALITION_TABLE, (int)c0, nc, B, r.s0.T, r.s0.N, r.s0.ds,
-                              const_cast<uint8_t*>(coalitions + c0 * P), r.src_e, r.stat_e, r.times_e, r.len_e, st));
-      RD_TRY(raindrop_fwd(&dc, params, r.src_e, r.stat_e, r.times_e, r.len_e, node_scale, nullptr, r.ws, r.logits, nullptr,
-                          nullptr, nullptr, 0, st));
+                              const_cast<uint8_t*>(coalitions + c0 * P), r.x.src, r.x.statics, r.x.times, r.x.lengths,
+                              st));
+      RD_TRY(raindrop_fwd(&dc, params, r.x.src, r.x.statics, r.x.times, r.x.lengths, node_scale, nullptr, r.ws, r.logits,
+                          nullptr, nullptr, nullptr, 0, st));
     }
     RD_TRY(kernel_shap_accumulate(r.logits, endpoint_logits, target, coalitions, weights, P, (int)c0, nc, B, r.s0.ncls, r.acc,
                                   c0 == 0, st));
@@ -1567,10 +1504,9 @@ int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, con
 }
 
 size_t rd_mc_dropout_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk) {
-  if (!dims) return 0;
-  McLayout l;
-  if (mc_layout(dims, replicates_per_chunk, &l) != 0) return 0;
-  return (size_t)l.total * sizeof(float);
+  McScratch l;
+  if (!dims || mc_scratch(dims, replicates_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
 }
 
 // Chunks of cc replicates: the inputs expanded when the chunk size changes (the first and a ragged last chunk), one
@@ -1581,34 +1517,31 @@ int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, cons
                               int32_t n_samples, int32_t replicates_per_chunk, void* scratch, float* mean_probs,
                               float* variance, float* entropies, float* samples, void* stream) {
   const char* fn = "rd_raindrop_v2_mc_dropout";
-  if (!dims || !params || !src || !times || !lengths || !node_scale || !rng || !scratch || !mean_probs || !variance ||
-      !entropies || !params->R_u || !params->ob1_value_weight) {
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s0));
+  if (!src || !times || !rng || !scratch || !mean_probs || !variance || !entropies || !params->R_u ||
+      !params->ob1_value_weight) {
     set_error("%s: NULL argument", fn);
     return -2;
   }
   if (n_samples < 1 || replicates_per_chunk < 1) { set_error("%s: n_samples and replicates_per_chunk must be >= 1", fn); return -2; }
-  Shape s0;
-  RD_TRY(make_shape(dims, &s0));
-  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s0.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
-  McLayout l;
-  RD_TRY(mc_layout(dims, replicates_per_chunk, &l));
+  McScratch l;
+  RD_TRY(mc_scratch(dims, replicates_per_chunk, &l));
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s0.B, cc = replicates_per_chunk;
   const int64_t M = n_samples;
   float* S = (float*)scratch;
-  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
-  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  const Expanded x = l.inputs(S, s0.ds);
   double* acc = reinterpret_cast<double*>(S + l.acc);
   int expanded = 0;
   for (int64_t c0 = 0; c0 < M; c0 += cc) {
     const int nc = (int)(M - c0 < cc ? M - c0 : cc);
-    const rd_dims dc = mc_dims(dims, B * nc, cc);
+    const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 1);
     if (nc != expanded) {
-      RD_TRY(mc_expand(src, statics, times, lengths, B, nc, s0.T, s0.N, s0.ds, src_e, stat_e, times_e, len_e, st));
+      RD_TRY(mc_expand(src, statics, times, lengths, B, nc, s0.T, s0.N, s0.ds, x.src, x.statics, x.times, x.lengths, st));
       expanded = nc;
     }
-    RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, const_cast<uint64_t*>(rng), S + l.ws,
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, const_cast<uint64_t*>(rng), S + l.ws,
                         S + l.logits, nullptr, nullptr, nullptr, 0, st, B, (uint64_t)c0));
     RD_TRY(mc_accumulate(S + l.logits, nc, B, s0.ncls, c0, M, acc, samples, mean_probs, variance, entropies, c0 == 0,
                          c0 + nc >= M, st));
@@ -1617,19 +1550,15 @@ int rd_raindrop_v2_mc_dropout(const rd_dims* dims, const rd_params* params, cons
 }
 
 size_t rd_smooth_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk) {
-  if (!dims) return 0;
-  SmoothLayout l;
-  if (smooth_layout(dims, replicates_per_chunk, &l) != 0) return 0;
-  return (size_t)l.total * sizeof(float);
+  ChunkLayout l;
+  if (!dims || chunk_layout(dims, "replicates_per_chunk", replicates_per_chunk, dims->B, false, 0, false, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
 }
 
-// The checks rd_raindrop_v2_smooth_counts and rd_debug_smoothing_inputs share.
-static int smooth_check(const char* fn, const rd_dims* dims, const float* statics, int32_t perturb_static, float sigma,
-                        Shape* s0) {
+// The checks rd_raindrop_v2_smooth_counts and rd_debug_smoothing_inputs share, after the shape's.
+static int smooth_check(const char* fn, const Shape& s0, int32_t perturb_static, float sigma) {
   if (!(sigma >= 0.f) || isinf(sigma)) { set_error("%s: sigma must be finite and >= 0, got %g", fn, sigma); return -2; }
-  RD_TRY(make_shape(dims, s0));
-  if (s0->ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
-  if (perturb_static && s0->ds == 0) { set_error("%s: perturb_static needs a static branch (d_static > 0)", fn); return -2; }
+  if (perturb_static && s0.ds == 0) { set_error("%s: perturb_static needs a static branch (d_static > 0)", fn); return -2; }
   return 0;
 }
 
@@ -1641,30 +1570,27 @@ int rd_raindrop_v2_smooth_counts(const rd_dims* dims, const rd_params* params, c
                                  const uint64_t* rng, int32_t n_samples, int32_t replicates_per_chunk, void* scratch,
                                  int64_t* counts, void* stream) {
   const char* fn = "rd_raindrop_v2_smooth_counts";
-  if (!dims || !params || !src || !times || !lengths || !node_scale || !rng || !scratch || !counts || !params->R_u ||
-      !params->ob1_value_weight) {
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !rng || !scratch || !counts || !params->R_u || !params->ob1_value_weight) {
     set_error("%s: NULL argument", fn);
     return -2;
   }
-  if (dims->training) { set_error("%s: runs eval arithmetic, dims->training must be 0", fn); return -2; }
   if (n_samples < 1 || replicates_per_chunk < 1) { set_error("%s: n_samples and replicates_per_chunk must be >= 1", fn); return -2; }
-  Shape s0;
-  RD_TRY(smooth_check(fn, dims, statics, perturb_static, sigma, &s0));
-  if (s0.dpe != RD_D_PE || s0.emb != s0.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  SmoothLayout l;
-  RD_TRY(smooth_layout(dims, replicates_per_chunk, &l));
+  RD_TRY(smooth_check(fn, s0, perturb_static, sigma));
+  ChunkLayout l;
+  RD_TRY(chunk_layout(dims, "replicates_per_chunk", replicates_per_chunk, dims->B, false, 0, false, &l));
   cudaStream_t st = (cudaStream_t)stream;
   const int B = s0.B, cc = replicates_per_chunk;
   float* S = (float*)scratch;
-  float* src_e = S + l.src; float* stat_e = s0.ds > 0 ? S + l.statics : nullptr; float* times_e = S + l.times;
-  int64_t* len_e = reinterpret_cast<int64_t*>(S + l.lengths);
+  const Expanded x = l.inputs(S, s0.ds);
   for (int c0 = 0; c0 < n_samples; c0 += cc) {
     const int nc = n_samples - c0 < cc ? n_samples - c0 : cc;
-    const rd_dims dc = ig_dims(dims, B * nc, cc);
+    const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
     RD_TRY(smooth_expand(src, statics, times, lengths, sensor_perturbable, perturb_static, sigma, rng, c0, B, nc, s0.T, s0.N,
-                         s0.ds, src_e, stat_e, times_e, len_e, st));
-    RD_TRY(raindrop_fwd(&dc, params, src_e, stat_e, times_e, len_e, node_scale, nullptr, S + l.ws, S + l.logits, nullptr,
-                        nullptr, nullptr, 0, st));
+                         s0.ds, x.src, x.statics, x.times, x.lengths, st));
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, S + l.logits,
+                        nullptr, nullptr, nullptr, 0, st));
     RD_TRY(smooth_vote(S + l.logits, B, nc, s0.ncls, c0 == 0, counts, st));
     if (n_samples - c0 <= cc) break;
   }
@@ -1679,8 +1605,9 @@ int rd_debug_smoothing_inputs(const rd_dims* dims, const float* src, const float
   if (!dims || !src || !times || !lengths || !rng || !src_e) { set_error("%s: NULL argument", fn); return -2; }
   if (nc < 1 || m0 < 0) { set_error("%s: nc must be >= 1 and m0 >= 0 (nc = %d, m0 = %lld)", fn, nc, (long long)m0); return -2; }
   Shape s0;
-  RD_TRY(smooth_check(fn, dims, statics, perturb_static, sigma, &s0));
-  if (s0.ds > 0 && !statics_e) { set_error("%s: d_static > 0 needs statics_e", fn); return -2; }
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.ds > 0 && (!statics || !statics_e)) { set_error("%s: d_static > 0 needs statics and statics_e", fn); return -2; }
+  RD_TRY(smooth_check(fn, s0, perturb_static, sigma));
   if ((int64_t)s0.B * nc > (1LL << 30)) { set_error("%s: B * nc = %lld rows are too many", fn, (long long)s0.B * nc); return -2; }
   return smooth_expand(src, statics, times, lengths, sensor_perturbable, perturb_static, sigma, rng, m0, s0.B, nc, s0.T,
                        s0.N, s0.ds, src_e, statics_e, times_e, lengths_e, (cudaStream_t)stream);
@@ -1696,14 +1623,9 @@ int rd_raindrop_v2_per_sample_grad_sqnorms(const rd_dims* dims, const rd_params*
                                            const int64_t* lengths, const float* node_scale, const void* workspace,
                                            const float* d_logits, void* scratch, double* sqnorms, void* stream) {
   const char* fn = "rd_raindrop_v2_per_sample_grad_sqnorms";
-  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch || !sqnorms) {
-    set_error("%s: NULL argument", fn);
-    return -2;
-  }
   Shape s;
-  RD_TRY(make_shape(dims, &s));
-  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
+  if (!workspace || !d_logits || !scratch || !sqnorms) { set_error("%s: NULL argument", fn); return -2; }
   const DpLayout l = dp_layout(s);
   DpQueue q;
   q.B = s.B; q.nf = dp_n_fields(s); q.sqnorms = sqnorms;
@@ -1722,14 +1644,9 @@ int rd_raindrop_v2_per_sample_grads(const rd_dims* dims, const rd_params* params
                                     const float* node_scale, const void* workspace, const float* d_logits, void* scratch,
                                     float* G, int64_t ldg, void* stream) {
   const char* fn = "rd_raindrop_v2_per_sample_grads";
-  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch || !G) {
-    set_error("%s: NULL argument", fn);
-    return -2;
-  }
   Shape s;
-  RD_TRY(make_shape(dims, &s));
-  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
+  if (!workspace || !d_logits || !scratch || !G) { set_error("%s: NULL argument", fn); return -2; }
   DpQueue q;
   const int64_t bucket = bucket_fields(s, &q.fields);
   if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
@@ -1764,14 +1681,9 @@ int rd_raindrop_v2_kfac_factors(const rd_dims* dims, const rd_params* params, co
                                 const float* node_scale, const void* workspace, const float* d_logits, void* scratch,
                                 double* factors, void* stream) {
   const char* fn = "rd_raindrop_v2_kfac_factors";
-  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !scratch || !factors) {
-    set_error("%s: NULL argument", fn);
-    return -2;
-  }
   Shape s;
-  RD_TRY(make_shape(dims, &s));
-  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
+  if (!workspace || !d_logits || !scratch || !factors) { set_error("%s: NULL argument", fn); return -2; }
   if (reinterpret_cast<uintptr_t>(scratch) & 15) { set_error("%s: scratch must be 16-byte aligned", fn); return -2; }
   const KfacBlocks K = kfac_blocks(s);
   const KfacLayout l = kfac_layout(s);
@@ -1810,14 +1722,9 @@ int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, cons
                               const float* node_scale, const void* workspace, const float* d_logits, const float* bases,
                               void* scratch, float* G, int64_t ldg, void* stream) {
   const char* fn = "rd_raindrop_v2_ekfac_rows";
-  if (!dims || !params || !lengths || !node_scale || !workspace || !d_logits || !bases || !scratch || !G) {
-    set_error("%s: NULL argument", fn);
-    return -2;
-  }
   Shape s;
-  RD_TRY(make_shape(dims, &s));
-  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
+  if (!workspace || !d_logits || !bases || !scratch || !G) { set_error("%s: NULL argument", fn); return -2; }
   DpFields f;
   const int64_t bucket = bucket_fields(s, &f);
   if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
@@ -1853,14 +1760,9 @@ int rd_raindrop_v2_laplace_logit_cov(const rd_dims* dims, const rd_params* param
                                      const int64_t* lengths, const float* node_scale, const void* workspace,
                                      const float* bases, const float* w, void* scratch, double* cov, void* stream) {
   const char* fn = "rd_raindrop_v2_laplace_logit_cov";
-  if (!dims || !params || !lengths || !node_scale || !workspace || !bases || !w || !scratch || !cov) {
-    set_error("%s: NULL argument", fn);
-    return -2;
-  }
   Shape s;
-  RD_TRY(make_shape(dims, &s));
-  if (s.dpe != RD_D_PE || s.emb != s.N) { set_error("Raindrop_v2 has d_pe = 16 and emb_dim = d_inp"); return -2; }
-  if (s.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
+  if (!workspace || !bases || !w || !scratch || !cov) { set_error("%s: NULL argument", fn); return -2; }
   if (s.ncls > RD_LAPLACE_MAX_CLASSES) { set_error("%s: n_classes = %d, at most %d", fn, s.ncls, RD_LAPLACE_MAX_CLASSES); return -2; }
   if ((reinterpret_cast<uintptr_t>(bases) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(scratch)) & 15) {
     set_error("%s: bases, w and scratch must be 16-byte aligned", fn);

@@ -29,7 +29,7 @@ import torch.distributed as dist
 
 from . import lib as L
 from .adversarial import _check_key, _sensor_mask
-from .attribution import DEFAULT_SCRATCH_BYTES, _Call, _check_call, _largest_chunk
+from .attribution import _Call, _check_call
 from .train import TrainStep
 from .uncertainty import _device_key
 
@@ -111,15 +111,7 @@ def smooth_counts(model, src, static, times, lengths, *, sigma, n_samples, seed=
         lib, B, dev = cl.lib, src.shape[1], cl.device
         sens = _sensor_mask(sensors, plan.N, dev)
         dims = plan.dims(B, False)
-        if internal_batch_size is None:
-            cc = _largest_chunk(lambda c: lib.rd_smooth_scratch_bytes(C.byref(dims), c), n_samples, DEFAULT_SCRATCH_BYTES)
-        else:
-            cc = max(1, int(internal_batch_size) // B)
-        cc = min(cc, n_samples)
-        nbytes = lib.rd_smooth_scratch_bytes(C.byref(dims), cc)
-        if nbytes == 0:
-            L.check(-2, "rd_smooth_scratch_bytes")
-        scratch = cl.scratch("_smooth_scratch", (B, cc, dims.obprop_mode, dev.index), nbytes)
+        cc, scratch = cl.chunk_scratch("_smooth_scratch", "rd_smooth_scratch_bytes", dims, n_samples, internal_batch_size)
         key = _device_key(plan, seed, step, dev)
         counts = torch.empty(B, plan.n_classes, dtype=torch.int64, device=dev)
         L.check(lib.rd_raindrop_v2_smooth_counts(C.byref(dims), C.byref(cl.params), cl.x.data_ptr(), L.ptr(cl.st),

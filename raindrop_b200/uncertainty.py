@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import lib as L
-from .attribution import DEFAULT_SCRATCH_BYTES, _Call, _largest_chunk
+from .attribution import _Call, _check_call
 
 
 @dataclass
@@ -96,14 +96,10 @@ def mc_dropout(model, src, static, times, lengths, n_samples=30, seed=None, step
     Works in train() and eval() mode alike and leaves the mode, the parameters, their .grad and the model's dropout
     counter unchanged; runs under no_grad, stream-ordered and sync-free, and can be captured in a CUDA graph (after an
     eager call with the same key and shapes).  Raises RaindropB200Error without CUDA or without the built library."""
-    from .models_rd import Raindrop_v2
-    if not isinstance(model, Raindrop_v2):
-        raise TypeError("mc_dropout takes a raindrop_b200 Raindrop_v2 model, got %s" % type(model).__name__)
+    _check_call("mc_dropout", model, src, static, None, internal_batch_size, train_ok=True)
     n_samples = int(n_samples)
     if n_samples < 1 or n_samples > 0x7FFFFFFF:
         raise ValueError("n_samples must be in [1, 2^31), got %d" % n_samples)
-    if internal_batch_size is not None and int(internal_batch_size) < 1:
-        raise ValueError("internal_batch_size must be >= 1")
     seed = model._seed if seed is None else int(seed)
     step = int(step)
     if not 0 <= seed < 1 << 64:
@@ -111,24 +107,11 @@ def mc_dropout(model, src, static, times, lengths, n_samples=30, seed=None, step
     if step < 0 or step + n_samples > 1 << 64:
         raise ValueError("step must be >= 0 with step + n_samples <= 2^64, got %d" % step)
     plan = model._plan
-    if src.dim() != 3 or src.shape[0] != plan.T or src.shape[2] != 2 * plan.N:
-        raise ValueError("src must be [max_len=%d, B, 2*d_inp=%d], got %s" % (plan.T, 2 * plan.N, tuple(src.shape)))
-    if model.static and static is None:
-        raise ValueError("this model was built with static=True: `static` must be a tensor")
     with torch.no_grad():
         cl = _Call(model, src, static, times, lengths, None, False)
         lib, B = cl.lib, src.shape[1]
         dims = plan.dims(B, True)
-        if internal_batch_size is None:
-            cc = _largest_chunk(lambda c: lib.rd_mc_dropout_scratch_bytes(C.byref(dims), c), n_samples,
-                                DEFAULT_SCRATCH_BYTES)
-        else:
-            cc = max(1, int(internal_batch_size) // B)
-        cc = min(cc, n_samples)
-        nbytes = lib.rd_mc_dropout_scratch_bytes(C.byref(dims), cc)
-        if nbytes == 0:
-            L.check(-2, "rd_mc_dropout_scratch_bytes")
-        scratch = cl.scratch("_mc_scratch", (B, cc, dims.obprop_mode, cl.device.index), nbytes)
+        cc, scratch = cl.chunk_scratch("_mc_scratch", "rd_mc_dropout_scratch_bytes", dims, n_samples, internal_batch_size)
         key = _device_key(plan, seed, step, cl.device)
         f32 = dict(device=cl.device, dtype=torch.float32)
         mean = torch.empty(B, plan.n_classes, **f32)

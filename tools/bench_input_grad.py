@@ -26,6 +26,7 @@ players, --window included) with the loop of M + 2 B-row module forwards over th
 fp64 solve (the operator [K | k] is computed once, outside the timing, for both).
 """
 import argparse
+import ctypes as C
 import json
 import os
 import subprocess
@@ -59,7 +60,7 @@ def launches_of(lib, fn):
 
 def ig_compare(args, lib, cfg_name, model, b, device):
     """Alternating timing of one integrated_gradients call and of the loop of M input-gradient calls."""
-    from raindrop_b200.attribution import _default_steps_per_chunk, integrated_gradients, quadrature
+    from raindrop_b200.attribution import _largest_chunk, integrated_gradients, quadrature
     M = args.ig_steps
     B = b["src"].shape[1]
     N = b["src"].shape[2] // 2
@@ -97,8 +98,9 @@ def ig_compare(args, lib, cfg_name, model, b, device):
         t_b += timed_steps(batched, 1, flush)
         t_l += timed_steps(loop, 1, flush)
     sb, sl = summarize(t_b, 1, device), summarize(t_l, 1, device)
+    dims = model._plan.dims(B, False)
     steps_per_chunk = min(M, max(1, args.ig_rows // B)) if args.ig_rows else \
-        _default_steps_per_chunk(lib, model._plan.dims(B, False), M)
+        _largest_chunk(lambda c: lib.rd_integrated_gradients_scratch_bytes(C.byref(dims), c), M)
     res = {"metric": "integrated gradients, %d steps, samples/s (%s-shape synthetic)" % (M, cfg_name), "batch": B,
            "ig_steps": M, "ig_rows": args.ig_rows, "steps_per_chunk": steps_per_chunk, "steps": args.steps, "card": card()}
     for tag, t, n in (("batched", sb, n_batched), ("loop", sl, n_loop)):
@@ -110,7 +112,7 @@ def ig_compare(args, lib, cfg_name, model, b, device):
 
 def coalition_compare(args, lib, cfg_name, model, b, device):
     """Alternating timing of one feature_ablation / shapley_value_sampling call and of the loop of module forwards."""
-    from raindrop_b200.attribution import (_default_coalitions_per_chunk, feature_ablation, kernel_shap,
+    from raindrop_b200.attribution import (_largest_chunk, feature_ablation, kernel_shap,
                                            kernel_shap_operator, sample_coalitions, sample_permutations,
                                            shapley_value_sampling, time_window_mask)
     src, static, times, lengths, y = b["src"], b["static"], b["times"], b["lengths"], b["y"]
@@ -191,8 +193,9 @@ def coalition_compare(args, lib, cfg_name, model, b, device):
         t_b += timed_steps(batched, 1, flush)
         t_l += timed_steps(loop, 1, flush)
     sb, sl = summarize(t_b, 1, device), summarize(t_l, 1, device)
+    dims = model._plan.dims(B, False)
     cc = min(n_coal, max(1, args.coalition_rows // B)) if args.coalition_rows else \
-        _default_coalitions_per_chunk(lib, model._plan.dims(B, False), P, n_coal)
+        _largest_chunk(lambda c: lib.rd_coalition_attribution_scratch_bytes(C.byref(dims), P, c), n_coal)
     what = "Shapley-value sampling, %d permutations" % M if M else "leave-one-out ablation"
     if K:
         what = "KernelSHAP, %d coalitions" % n_coal

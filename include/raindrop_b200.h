@@ -454,6 +454,39 @@ int rd_raindrop_v2_smooth_counts(const rd_dims* dims, const rd_params* params, c
                                  const uint64_t* rng, int32_t n_samples, int32_t replicates_per_chunk, void* scratch,
                                  int64_t* counts, void* stream);
 
+/* ---- randomized ablation of Raindrop_v2: class votes over random sensor subsets, in one call -----------------------
+ * The ablation-smoothed classifier g(x) = argmax_c P(f(ablate(x, S)) = c) over uniform k-subsets S of the players
+ * (Levine & Feizi 2020) of the eval-mode model f, estimated (sampled) or computed exactly (exhaustive) by counting the
+ * argmax classes of n_samples ablated replicates of every sample.
+ * Players: the sensors n with sensor_player[n] != 0 (NULL: every sensor) in increasing n, then the static vector when
+ * ablate_static (last).  n_players = P must be their number (1 <= P <= RD_ABLATION_MAX_PLAYERS); a sensor past the
+ * first P - ablate_static players counts as no player.  Sensors that are not players are always kept.
+ * Ablating a player writes +0.0 into its value column src[:, b, n] at every time step, also into its mask column
+ * src[:, b, N + n] when ablate_mask, and into every static for the static player.  Everything else (kept players, the
+ * other sensors, times, lengths) is copied bit for bit.
+ * Replicate m = 0 .. n_samples-1 keeps keep = k players (1 <= k <= P), rng = {seed, step} (device uint64[2], read only):
+ *   sampled (exhaustive = 0): the first k positions of a partial Fisher-Yates shuffle of 0 .. P-1 (position i swaps
+ *     with i + U(P - i), i < k), U(r) Lemire's unbiased bounded integer with rejection, over the 32-bit Philox4x32-10
+ *     words of key {seed, step + m} at site 101: word j of sample b at index (b << 32) + j, word index & 3 of the block
+ *     at counter index >> 2.  An exactly uniform k-subset; a replicate depends on (seed, step + m, b) alone.
+ *   exhaustive (exhaustive = 1): the subset of lexicographic rank step + m among the J = C(P, k) <= 2^31 - 1 subsets
+ *     (itertools.combinations order); the seed is ignored and a rank >= J keeps no player.
+ *   counts [B, n_classes] int64 = per sample, how many replicates' logits have their (first) maximum at each class; a
+ *          replicate with a non-finite logit votes for no class.
+ * Eval arithmetic (dims->training must be 0), as rd_raindrop_v2_smooth_counts: per chunk of replicates_per_chunk
+ * replicates a keep-table launch, an expansion launch, ONE eval forward on B*replicates_per_chunk rows and one vote
+ * launch (exact, independent of the chunking once dims->obprop_mode is pinned).
+ * scratch: rd_ablation_scratch_bytes(dims, n_players, replicates_per_chunk) bytes (0: invalid arguments).
+ * Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+#define RD_ABLATION_MAX_PLAYERS 4096
+size_t rd_ablation_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t replicates_per_chunk);
+int rd_raindrop_v2_ablation_counts(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                   const float* times, const int64_t* lengths, const float* node_scale,
+                                   const uint8_t* sensor_player, int32_t n_players, int32_t ablate_static,
+                                   int32_t ablate_mask, int32_t keep, int32_t exhaustive, const uint64_t* rng,
+                                   int32_t n_samples, int32_t replicates_per_chunk, void* scratch, int64_t* counts,
+                                   void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);
@@ -804,6 +837,17 @@ int rd_debug_smoothing_inputs(const rd_dims* dims, const float* src, const float
                               const int64_t* lengths, const uint8_t* sensor_perturbable, int32_t perturb_static,
                               float sigma, const uint64_t* rng, int64_t m0, int32_t nc, float* src_e, float* statics_e,
                               float* times_e, int64_t* lengths_e, void* stream);
+
+/* debug: the keep table and ablated inputs of replicates m0 .. m0+nc-1 of rd_raindrop_v2_ablation_counts (the same two
+ * launches, same stream): keep_table [nc*B, n_players] uint8 (1 = kept; row j = (m - m0)*B + b), src_e, statics_e,
+ * times_e and lengths_e as rd_debug_smoothing_inputs lays them out (times_e / lengths_e may be NULL: skipped).  Only
+ * dims' B, T, N (d_inp) and d_static are read.  With nc = 1 and m0 = 0 it is one ablated copy of the batch at key rng,
+ * which is how AblationTrainStep draws its batch. */
+int rd_debug_ablation_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                             const int64_t* lengths, const uint8_t* sensor_player, int32_t n_players, int32_t ablate_static,
+                             int32_t ablate_mask, int32_t keep, int32_t exhaustive, const uint64_t* rng, int64_t m0,
+                             int32_t nc, uint8_t* keep_table, float* src_e, float* statics_e, float* times_e,
+                             int64_t* lengths_e, void* stream);
 
 /* ---- the forward GEMM engines on their own (debug: operator-level tests) -------------------------------------------
  * Fields are grouped by size (pointers, 64-bit, 32-bit) so the layout has no interior padding. */

@@ -214,6 +214,18 @@ int smooth_expand(const float* src, const float* statics, const float* times, co
 // smooth_vote: counts [B, ncls] (+)= the argmax votes of logits [nc*B, ncls] (replicate-major; first: from 0)
 int smooth_vote(const float* logits, int B, int nc, int ncls, int first, int64_t* counts, cudaStream_t st);
 
+// ---- randomized ablation (rd_smoothing.cu; rd_raindrop_v2_ablation_counts) ------------------------------------------
+constexpr uint32_t SITE_ABLATE = 101;       // Philox site of the sampled subsets (its key is {seed, step + replicate})
+// The P players: the sensors n with sens[n] != 0 (sens NULL: every sensor) in increasing n, then the static vector when
+// ast.  ablate_inputs runs two launches for replicates m0 .. m0+nc-1: the keep table keep [nc*B, P] (uint8, row
+// j = m*B + b; J > 0: the subset of lexicographic rank rng[1] + m0 + m among the J = C(P, k) k-subsets, none for a rank
+// >= J; J = 0: a partial Fisher-Yates shuffle drawn at key {rng[0], rng[1] + m0 + m}), then the replicate-major rows of
+// mc_expand with each ablated player's value column (and mask column when amask, the statics for the static player)
+// written as +0.0.  times_e / lengths_e may be NULL (skipped).
+int ablate_inputs(const float* src, const float* statics, const float* times, const int64_t* lengths, const uint8_t* sens,
+                  int P, int ast, int amask, int k, int64_t J, const uint64_t* rng, int64_t m0, int B, int nc, int T, int N,
+                  int ds, uint8_t* keep, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
+
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 
 // y = LN(x) * gamma + beta over the last dim (width D); stats[row] = {mean, rstd}

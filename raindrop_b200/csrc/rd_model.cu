@@ -1613,6 +1613,111 @@ int rd_debug_smoothing_inputs(const rd_dims* dims, const float* src, const float
                        s0.N, s0.ds, src_e, statics_e, times_e, lengths_e, (cudaStream_t)stream);
 }
 
+// Randomized ablation: the smoothing layout plus the chunk's keep table [cc*B, P] (uint8).
+struct AblationScratch : ChunkLayout { int64_t keep; };
+static int ablation_scratch(const rd_dims* dims, int n_players, int cc, AblationScratch* l) {
+  RD_TRY(chunk_layout(dims, "replicates_per_chunk", cc, dims->B, false, 0, false, l));
+  if (n_players < 1 || n_players > RD_ABLATION_MAX_PLAYERS) {
+    set_error("n_players = %d must be in [1, %d]", n_players, RD_ABLATION_MAX_PLAYERS);
+    return -2;
+  }
+  l->keep = l->a.take(ceil_div((int64_t)cc * dims->B * n_players, 4));
+  return 0;
+}
+
+size_t rd_ablation_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t replicates_per_chunk) {
+  AblationScratch l;
+  if (!dims || ablation_scratch(dims, n_players, replicates_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+// The checks rd_raindrop_v2_ablation_counts and rd_debug_ablation_inputs share, after the shape's.  *J: C(P, keep) in
+// exhaustive mode, 0 in sampled mode (the keep kernel's mode switch).
+static int ablation_check(const char* fn, const Shape& s0, int32_t n_players, int32_t ablate_static, int32_t ablate_mask,
+                          int32_t keep, int32_t exhaustive, int64_t* J) {
+  const int P = n_players, st = ablate_static ? 1 : 0;
+  if (ablate_static && s0.ds == 0) { set_error("%s: ablate_static needs a static branch (d_static > 0)", fn); return -2; }
+  if (P < 1 || P > RD_ABLATION_MAX_PLAYERS || P - st > s0.N) {
+    set_error("%s: n_players = %d must be in [1, %d] and at most d_inp%s = %d", fn, P, RD_ABLATION_MAX_PLAYERS,
+              st ? " + 1" : "", s0.N + st);
+    return -2;
+  }
+  if (keep < 1 || keep > P) { set_error("%s: keep = %d must be in [1, n_players = %d]", fn, keep, P); return -2; }
+  if ((ablate_mask != 0 && ablate_mask != 1) || (exhaustive != 0 && exhaustive != 1)) {
+    set_error("%s: ablate_mask and exhaustive must be 0 or 1 (got %d, %d)", fn, ablate_mask, exhaustive);
+    return -2;
+  }
+  *J = 0;
+  if (exhaustive) {
+    // C(P, keep) = prod_{i < m} (P - i) / (i + 1) with m = min(keep, P - keep); every partial product is a binomial
+    int64_t c = 1;
+    const int m = keep < P - keep ? keep : P - keep;
+    for (int i = 0; i < m && c <= 0x7fffffffLL; ++i) c = c * (P - i) / (i + 1);
+    if (c > 0x7fffffffLL) {
+      set_error("%s: exhaustive mode needs C(n_players, keep) <= 2^31 - 1 (n_players = %d, keep = %d)", fn, P, keep);
+      return -2;
+    }
+    *J = c;
+  }
+  return 0;
+}
+
+// Chunks of cc replicates: the keep-table and expansion launches (ablate_inputs), one eval forward on B*cc
+// replicate-major rows and one launch adding each row's vote to counts.
+int rd_raindrop_v2_ablation_counts(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                   const float* times, const int64_t* lengths, const float* node_scale,
+                                   const uint8_t* sensor_player, int32_t n_players, int32_t ablate_static,
+                                   int32_t ablate_mask, int32_t keep, int32_t exhaustive, const uint64_t* rng,
+                                   int32_t n_samples, int32_t replicates_per_chunk, void* scratch, int64_t* counts,
+                                   void* stream) {
+  const char* fn = "rd_raindrop_v2_ablation_counts";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !rng || !scratch || !counts || !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (n_samples < 1 || replicates_per_chunk < 1) { set_error("%s: n_samples and replicates_per_chunk must be >= 1", fn); return -2; }
+  int64_t J;
+  RD_TRY(ablation_check(fn, s0, n_players, ablate_static, ablate_mask, keep, exhaustive, &J));
+  AblationScratch l;
+  RD_TRY(ablation_scratch(dims, n_players, replicates_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, cc = replicates_per_chunk;
+  float* S = (float*)scratch;
+  const Expanded x = l.inputs(S, s0.ds);
+  uint8_t* table = reinterpret_cast<uint8_t*>(S + l.keep);
+  for (int c0 = 0; c0 < n_samples; c0 += cc) {
+    const int nc = n_samples - c0 < cc ? n_samples - c0 : cc;
+    const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
+    RD_TRY(ablate_inputs(src, statics, times, lengths, sensor_player, n_players, ablate_static, ablate_mask, keep, J, rng, c0,
+                         B, nc, s0.T, s0.N, s0.ds, table, x.src, x.statics, x.times, x.lengths, st));
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, S + l.logits,
+                        nullptr, nullptr, nullptr, 0, st));
+    RD_TRY(smooth_vote(S + l.logits, B, nc, s0.ncls, c0 == 0, counts, st));
+    if (n_samples - c0 <= cc) break;
+  }
+  return 0;
+}
+
+int rd_debug_ablation_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                             const int64_t* lengths, const uint8_t* sensor_player, int32_t n_players, int32_t ablate_static,
+                             int32_t ablate_mask, int32_t keep, int32_t exhaustive, const uint64_t* rng, int64_t m0,
+                             int32_t nc, uint8_t* keep_table, float* src_e, float* statics_e, float* times_e,
+                             int64_t* lengths_e, void* stream) {
+  const char* fn = "rd_debug_ablation_inputs";
+  if (!dims || !src || !times || !lengths || !rng || !keep_table || !src_e) { set_error("%s: NULL argument", fn); return -2; }
+  if (nc < 1 || m0 < 0) { set_error("%s: nc must be >= 1 and m0 >= 0 (nc = %d, m0 = %lld)", fn, nc, (long long)m0); return -2; }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.ds > 0 && (!statics || !statics_e)) { set_error("%s: d_static > 0 needs statics and statics_e", fn); return -2; }
+  int64_t J;
+  RD_TRY(ablation_check(fn, s0, n_players, ablate_static, ablate_mask, keep, exhaustive, &J));
+  if ((int64_t)s0.B * nc > (1LL << 30)) { set_error("%s: B * nc = %lld rows are too many", fn, (long long)s0.B * nc); return -2; }
+  return ablate_inputs(src, statics, times, lengths, sensor_player, n_players, ablate_static, ablate_mask, keep, J, rng, m0,
+                       s0.B, nc, s0.T, s0.N, s0.ds, keep_table, src_e, statics_e, times_e, lengths_e, (cudaStream_t)stream);
+}
+
 size_t rd_dp_scratch_bytes(const rd_dims* dims) {
   Shape s;
   if (make_shape(dims, &s) != 0) return 0;

@@ -139,25 +139,33 @@ def predict_from_counts(counts, alpha=0.001):
     return out
 
 
-def certify_from_counts(counts0, counts, sigma, alpha=0.001, n=None):
-    """Cohen's CERTIFY from selection votes counts0 and estimation votes counts ([B, C], tensors or arrays), in float64
-    on the host: c_A = argmax counts0 (ties: the lowest index), k = counts[b, c_A], p_lower = the one-sided
-    (1 - alpha) Clopper-Pearson lower bound beta.ppf(alpha, k, n - k + 1) (0 for k = 0), and radius = sigma
-    Phi^-1(p_lower), or prediction -1 and radius -1 when p_lower < 1/2.  n: the estimation draws per sample (default:
-    the row sums of counts; give it when replicates may have voted for no class, so that they count against c_A).
-    Returns (prediction int64 [B], radius float64 [B], p_lower float64 [B])."""
-    from scipy.stats import beta, norm
+def selection_lower_bound(counts0, counts, alpha, n=None):
+    """The step CERTIFY shares between smoothing and ablation, in float64 on the host: c_A = argmax counts0 (ties: the
+    lowest index) and p_lower = the one-sided (1 - alpha) Clopper-Pearson lower bound beta.ppf(alpha, k, n - k + 1) of
+    P(f = c_A) from k = counts[b, c_A] of n draws (0 for k = 0).  n: the estimation draws per sample (default: the row
+    sums of counts; give it when replicates may have voted for no class, so that they count against c_A).  alpha is
+    checked by the caller.  Returns (c_A int64 [B], p_lower float64 [B])."""
+    from scipy.stats import beta
     c0, c = _counts(counts0), _counts(counts)
     if c0.shape != c.shape:
         raise ValueError("counts0 and counts must have the same shape, got %s and %s" % (c0.shape, c.shape))
-    sigma, alpha = _check_sigma(sigma), _check_alpha(alpha)
     ca = np.argmax(c0, axis=1)
     k = c[np.arange(c.shape[0]), ca].astype(np.float64)
     nn = c.sum(axis=1) if n is None else np.broadcast_to(np.asarray(n, dtype=np.int64), k.shape)
     if (nn < c.sum(axis=1)).any() or (nn < 1).any():
         raise ValueError("n must be >= 1 and at least each row's vote count")
     nn = nn.astype(np.float64)
-    p_lower = np.where(k > 0, beta.ppf(alpha, np.maximum(k, 1.0), nn - k + 1.0), 0.0)
+    return ca, np.where(k > 0, beta.ppf(alpha, np.maximum(k, 1.0), nn - k + 1.0), 0.0)
+
+
+def certify_from_counts(counts0, counts, sigma, alpha=0.001, n=None):
+    """Cohen's CERTIFY from selection votes counts0 and estimation votes counts ([B, C], tensors or arrays), in float64
+    on the host: c_A and p_lower as selection_lower_bound computes them, and radius = sigma Phi^-1(p_lower), or
+    prediction -1 and radius -1 when p_lower < 1/2.  n: the estimation draws per sample (default: the row sums of
+    counts).  Returns (prediction int64 [B], radius float64 [B], p_lower float64 [B])."""
+    from scipy.stats import norm
+    sigma, alpha = _check_sigma(sigma), _check_alpha(alpha)
+    ca, p_lower = selection_lower_bound(counts0, counts, alpha, n)
     ok = p_lower >= 0.5
     radius = np.where(ok, sigma * norm.ppf(np.where(ok, p_lower, 0.5)), -1.0)
     return np.where(ok, ca, -1).astype(np.int64), radius.astype(np.float64), p_lower.astype(np.float64)
@@ -194,38 +202,31 @@ def certify(model, src, static, times, lengths, *, sigma, n0=100, n_samples=100_
     return CertifyResult(pred, radius, p_lower, counts0, counts)
 
 
-class SmoothingTrainStep(TrainStep):
-    """Gaussian data augmentation (Cohen et al. 2019; Lecuyer et al. 2019) on static device buffers: each step draws
-    x + sigma z for the loaded batch with smooth_counts' noise (one replicate at the device key {seed, step}, on the
-    same perturbable set), then runs TrainStep's forward, backward and Adam on the noisy copy -- all on the device, one
-    CUDA graph per step.  A model trained this way keeps its accuracy under the noise that certify adds.
+class AugmentedTrainStep(TrainStep):
+    """A TrainStep that trains on a copy of the loaded batch augmented on the device every step (Gaussian noise,
+    random ablation), the whole step one CUDA graph.  The clean batch goes where TrainStep keeps it (load_batch,
+    DeviceDataset.fill); the augmented copy lands in noisy_src / noisy_static, which the training forward reads.  The
+    augmentation is drawn at a device key {seed, step} that every step advances by one, so a resumed run restores it
+    with noise_key_state() / set_noise_key().  A subclass checks its arguments and refuse_distributed() before calling
+    __init__ (which touches the model), and implements _augment(stream).  One GPU only."""
 
-    The clean batch goes where TrainStep keeps it (load_batch, DeviceDataset.fill); the noisy copy lands in noisy_src /
-    noisy_static, which the training forward reads.  noise_seed: the Philox seed (default: 64 bits from os.urandom);
-    the key lives on the device and every step advances its step by one, so a resumed run restores it with
-    noise_key_state() / set_noise_key().  At sigma = 0 a step is TrainStep's bit for bit.  adam_eps is Adam's epsilon.
-    One GPU only."""
+    augmentation = None     # the kind of training, in the one-GPU error
 
-    def __init__(self, model, batch_size, sigma, sensors=None, perturb_static=False, noise_seed=None, lr=1e-4,
-                 use_graph=True, betas=(0.9, 0.999), adam_eps=1e-8, group=None):
+    @classmethod
+    def refuse_distributed(cls, group):
         if dist.is_initialized() and dist.get_world_size(group) > 1:
-            raise L.RaindropB200Error("SmoothingTrainStep runs on one GPU; data-parallel smoothing training is not supported")
-        self.sigma = _check_sigma(sigma)
-        self.perturb_static = bool(perturb_static)
-        if self.perturb_static and not model.static:
-            raise ValueError("perturb_static needs a model with a static branch")
-        if sensors is not None:
-            _sensor_mask(sensors, model._plan.N, "cpu")
+            raise L.RaindropB200Error("%s runs on one GPU; data-parallel %s training is not supported"
+                                      % (cls.__name__, cls.augmentation))
+
+    def __init__(self, model, batch_size, noise_seed, lr, use_graph, betas, adam_eps, group):
         seed = int.from_bytes(os.urandom(8), "little") if noise_seed is None else int(noise_seed)
         _check_key(seed, 0)
         super().__init__(model, batch_size, lr=lr, betas=betas, eps=adam_eps, group=group, use_graph=use_graph,
                          distributed=False)
-        dev = self.device
-        self.sensors = _sensor_mask(sensors, self.plan.N, dev)
         self.noise_dims = self.plan.dims(self.B, False)
         self.noisy_src = torch.zeros_like(self.src)
         self.noisy_static = torch.zeros_like(self.static) if self.static is not None else None
-        self.noise_key = torch.tensor(np.array([seed, 0], dtype=np.uint64).view(np.int64), device=dev)
+        self.noise_key = torch.tensor(np.array([seed, 0], dtype=np.uint64).view(np.int64), device=self.device)
 
     def _inputs(self):
         return self.noisy_src, self.noisy_static
@@ -234,16 +235,12 @@ class SmoothingTrainStep(TrainStep):
         extra = (self.noise_key, self.noisy_src) + ((self.noisy_static,) if self.noisy_static is not None else ())
         return super()._state() + extra
 
-    def _noise(self, st):
-        L.check(self.lib.rd_debug_smoothing_inputs(C.byref(self.noise_dims), self.src.data_ptr(), L.ptr(self.static),
-                                                   self.times.data_ptr(), self.lengths.data_ptr(), L.ptr(self.sensors),
-                                                   int(self.perturb_static), self.sigma, self.noise_key.data_ptr(), 0, 1,
-                                                   self.noisy_src.data_ptr(), L.ptr(self.noisy_static), None, None, st),
-                "rd_debug_smoothing_inputs")
-        self.noise_key[1:].add_(1)
+    def _augment(self, st):
+        raise NotImplementedError
 
     def _enqueue(self):
-        self._noise(L.stream_ptr(self.device))
+        self._augment(L.stream_ptr(self.device))
+        self.noise_key[1:].add_(1)
         super()._enqueue()
 
     def noise_key_state(self):
@@ -255,3 +252,35 @@ class SmoothingTrainStep(TrainStep):
         """Restores a saved noise_key_state(); the next step draws the noise of that step."""
         seed, step = _check_key(seed, step)
         self.noise_key.copy_(torch.tensor(np.array([seed, step], dtype=np.uint64).view(np.int64)))
+
+
+class SmoothingTrainStep(AugmentedTrainStep):
+    """Gaussian data augmentation (Cohen et al. 2019; Lecuyer et al. 2019) on static device buffers: each step draws
+    x + sigma z for the loaded batch with smooth_counts' noise (one replicate at the device key {seed, step}, on the
+    same perturbable set), then runs TrainStep's forward, backward and Adam on the noisy copy -- all on the device, one
+    CUDA graph per step.  A model trained this way keeps its accuracy under the noise that certify adds.
+
+    The noisy copy lands in noisy_src / noisy_static (AugmentedTrainStep).  noise_seed: the Philox seed (default: 64
+    bits from os.urandom); save and restore the key with noise_key_state() / set_noise_key().  At sigma = 0 a step is
+    TrainStep's bit for bit.  adam_eps is Adam's epsilon.  One GPU only."""
+
+    augmentation = "smoothing"
+
+    def __init__(self, model, batch_size, sigma, sensors=None, perturb_static=False, noise_seed=None, lr=1e-4,
+                 use_graph=True, betas=(0.9, 0.999), adam_eps=1e-8, group=None):
+        self.refuse_distributed(group)
+        self.sigma = _check_sigma(sigma)
+        self.perturb_static = bool(perturb_static)
+        if self.perturb_static and not model.static:
+            raise ValueError("perturb_static needs a model with a static branch")
+        if sensors is not None:
+            _sensor_mask(sensors, model._plan.N, "cpu")
+        super().__init__(model, batch_size, noise_seed, lr, use_graph, betas, adam_eps, group)
+        self.sensors = _sensor_mask(sensors, self.plan.N, self.device)
+
+    def _augment(self, st):
+        L.check(self.lib.rd_debug_smoothing_inputs(C.byref(self.noise_dims), self.src.data_ptr(), L.ptr(self.static),
+                                                   self.times.data_ptr(), self.lengths.data_ptr(), L.ptr(self.sensors),
+                                                   int(self.perturb_static), self.sigma, self.noise_key.data_ptr(), 0, 1,
+                                                   self.noisy_src.data_ptr(), L.ptr(self.noisy_static), None, None, st),
+                "rd_debug_smoothing_inputs")

@@ -6,6 +6,8 @@ Rosenfeld & Kolter 2019):
         --outcomes P19data/processed_data/arr_outcomes.npy --split P19data/splits/phy19_split1_new.npy --part test \\
         --sigma 0.25 --out certify.tsv
     python tools/certify.py --synthetic P19 --n-samples 256 --sigma 0.25 --n 10000
+    python tools/certify.py --synthetic P19 --n-samples 256 --ablate 5 --n 10000        # randomized ablation
+    python tools/certify.py --synthetic P19 --n-samples 256 --ablate 3 --exhaustive     # all C(P, 3) subsets
 
 The data arguments are those of tools/adv_robustness.py; without --checkpoint the model has the synthetic weights of
 raindrop_b200.synth (a smoke run, not a trained model).  sigma and the radii are in normalised units (per-feature
@@ -13,6 +15,12 @@ standard deviations); the noise and the certificate cover the observed values (t
 the threat model of pgd(norm="l2").  Writes one row per sample (index, label, prediction, radius, correct, time; -1 =
 abstain) to --out as Cohen's certify.py does, prints the certified accuracy at each --radii and the abstain rate, then
 one JSON line.
+
+--ablate K certifies by randomized ablation instead (raindrop_b200.ablation.certify, Levine & Feizi 2020): each
+replicate keeps K sensors (players: every sensor, plus the statics with --ablate-static) and zeroes the values and masks
+of the others (--keep-mask: the values only).  The radius is a number of sensors whose data may change arbitrarily;
+the rows and the printed certified accuracy are per rho = 0, 1, 2, ... up to P - K.  --exhaustive enumerates all
+C(P, K) subsets once and certifies deterministically (no alpha, --n0 and --n unused).
 """
 import argparse
 import json
@@ -50,10 +58,17 @@ def main():
     ap.add_argument("--alpha", type=float, default=0.001)
     ap.add_argument("--radii", type=float, nargs="+", default=[0.0, 0.25, 0.5, 0.75, 1.0])
     ap.add_argument("--perturb-static", action="store_true")
+    ap.add_argument("--ablate", type=int, metavar="K", help="randomized ablation keeping K players (instead of --sigma)")
+    ap.add_argument("--exhaustive", action="store_true", help="--ablate: every C(P, K) subset once (deterministic)")
+    ap.add_argument("--ablate-static", action="store_true", help="--ablate: the static vector is a player too")
+    ap.add_argument("--keep-mask", action="store_true", help="--ablate: zero an ablated sensor's values, keep its mask")
     ap.add_argument("--out", help="per-sample rows (tab-separated); default: not written")
     args = ap.parse_args()
 
+    from raindrop_b200 import ablation
     from raindrop_b200.smoothing import certify
+    if args.ablate is None and (args.exhaustive or args.ablate_static or args.keep_mask):
+        raise SystemExit("--exhaustive, --ablate-static and --keep-mask need --ablate")
     if not torch.cuda.is_available():
         raise SystemExit("certify runs on a CUDA device")
     device = torch.device("cuda", torch.cuda.current_device())
@@ -79,8 +94,15 @@ def main():
         static = None if Pstatic is None else Pstatic[s:e]
         t0 = time.perf_counter()
         # each batch draws from its own replicate range, so no two samples of the run share noise
-        r = certify(model, P[:, s:e], static, times, lengths, sigma=args.sigma, n0=args.n0, n_samples=args.n,
-                    alpha=args.alpha, seed=args.seed, step=s * (args.n0 + args.n), perturb_static=args.perturb_static)
+        if args.ablate is not None:
+            r = ablation.certify(model, P[:, s:e], static, times, lengths, keep=args.ablate, n0=args.n0,
+                                 n_samples=args.n, alpha=args.alpha, exhaustive=args.exhaustive, seed=args.seed,
+                                 step=s * (args.n0 + args.n), ablate_static=args.ablate_static,
+                                 ablate_mask=not args.keep_mask)
+            n_players = r.n_players
+        else:
+            r = certify(model, P[:, s:e], static, times, lengths, sigma=args.sigma, n0=args.n0, n_samples=args.n,
+                        alpha=args.alpha, seed=args.seed, step=s * (args.n0 + args.n), perturb_static=args.perturb_static)
         dt = (time.perf_counter() - t0) / (e - s)
         pred[s:e], radius[s:e] = r.prediction, r.radius
         y = labels[s:e].cpu().numpy()
@@ -94,15 +116,25 @@ def main():
                 f.write("%d\t%d\t%d\t%.6g\t%d\t%.6g\n" % row)
     y = labels.cpu().numpy()
     correct = pred == y
-    acc = {"%g" % r: float(np.mean(correct & (radius >= r))) for r in args.radii}
+    radii = args.radii if args.ablate is None else list(range(n_players - args.ablate + 1))
+    acc = {"%g" % r: float(np.mean(correct & (radius >= r))) for r in radii}
     abstain = float(np.mean(pred < 0))
-    print("sigma %g, n0 %d, n %d, alpha %g: %d samples in %.2f s (%.1f samples/s)"
-          % (args.sigma, args.n0, args.n, args.alpha, n, elapsed, n / elapsed))
-    for r in args.radii:
+    if args.ablate is None:
+        print("sigma %g, n0 %d, n %d, alpha %g: %d samples in %.2f s (%.1f samples/s)"
+              % (args.sigma, args.n0, args.n, args.alpha, n, elapsed, n / elapsed))
+        head = dict(sigma=args.sigma, n0=args.n0, n=args.n, alpha=args.alpha)
+    else:
+        mode = "exhaustive" if args.exhaustive else "n0 %d, n %d, alpha %g" % (args.n0, args.n, args.alpha)
+        print("ablation keeping %d of %d players, %s: %d samples in %.2f s (%.1f samples/s)"
+              % (args.ablate, n_players, mode, n, elapsed, n / elapsed))
+        head = dict(keep=args.ablate, players=n_players, exhaustive=args.exhaustive, ablate_static=args.ablate_static,
+                    ablate_mask=not args.keep_mask)
+        if not args.exhaustive:
+            head.update(n0=args.n0, n=args.n, alpha=args.alpha)
+    for r in radii:
         print("certified accuracy at radius %-6g %.4f" % (r, acc["%g" % r]))
     print("abstain rate %.4f" % abstain)
-    print(json.dumps(dict(sigma=args.sigma, n0=args.n0, n=args.n, alpha=args.alpha, samples=n, seconds=elapsed,
-                          certified_accuracy=acc, abstain=abstain)))
+    print(json.dumps(dict(head, samples=n, seconds=elapsed, certified_accuracy=acc, abstain=abstain)))
 
 
 if __name__ == "__main__":

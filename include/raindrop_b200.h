@@ -487,6 +487,78 @@ int rd_raindrop_v2_ablation_counts(const rd_dims* dims, const rd_params* params,
                                    int32_t n_samples, int32_t replicates_per_chunk, void* scratch, int64_t* counts,
                                    void* stream);
 
+/* ---- out-of-distribution detection for Raindrop_v2: penultimate features, their moments, and per-sample scores -------
+ * Post-hoc detectors on the features of a trained eval-mode model (Lee et al. 2018, Mahalanobis; Sun et al. 2022, deep
+ * k-nearest neighbours; Hendrycks & Gimpel 2017, maximum softmax probability; Liu et al. 2020, energy).  Every score is
+ * oriented so that larger means more likely out of distribution.  Features f [B, Df] of one of two layers:
+ *   RD_OOD_POOLED: cat(pooled, emb(static)), the workspace view RD_WS_FEAT;
+ *   RD_OOD_HIDDEN: relu(mlp_static.0(f_pooled)), the view RD_WS_HEAD_HIDDEN (the penultimate activation).
+ * Fp = Df rounded up to a multiple of 4: the device copies of query rows, the bank and W^T carry zero columns up to Fp
+ * (the tensor-core GEMM takes K % 4 == 0), which add exact zeros to every dot product. */
+enum rd_ood_layer { RD_OOD_POOLED = 0, RD_OOD_HIDDEN = 1 };
+#define RD_OOD_MAX_K 256
+#define RD_OOD_SEL_EXTRA 32      /* candidates the kNN selection keeps per query beyond k (rd_raindrop_v2_ood_scores) */
+
+/* features [B, Df] fp32 of `layer` and logits [B, n_classes] (either may be NULL: skipped), copied out of the workspace
+ * of eval forwards over chunks of samples_per_chunk samples (the chunk's inputs are copied out of the batch when a
+ * chunk does not cover it; the ob-prop arithmetic of mode 0 is resolved from samples_per_chunk rows).  Bitwise the
+ * rows the forward writes; independent of the chunking once dims->obprop_mode is pinned.  dims->training must be 0.
+ * scratch: rd_ood_features_scratch_bytes(dims, samples_per_chunk) bytes (0: invalid arguments).  Stream-ordered,
+ * allocation- and sync-free, CUDA-graph capturable. */
+size_t rd_ood_features_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk);
+int rd_raindrop_v2_features(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                            const float* times, const int64_t* lengths, const float* node_scale, int32_t layer,
+                            int32_t samples_per_chunk, void* scratch, float* features, float* logits, void* stream);
+
+/* The moments of n feature rows feats [n, F] (fp32, contiguous) with labels [n] (int64), in float64:
+ *   class_sums [n_classes, F] = sum of the rows of each class, class_counts [n_classes] int64 = class sizes (labels
+ *   outside [0, n_classes) count nowhere; class_sums NULL skips both), gram [F, F] = sum_b f_b f_b^T (NULL: skipped).
+ * accumulate != 0 adds to the values already there, else they are overwritten.  Every entry adds the samples one at a
+ * time in index order (the products of two fp32 values are exact in fp64, so each step rounds once): the result is
+ * bitwise independent of the launch configuration and of how a data set is split across accumulating calls.  One pass
+ * over a training set gives the class means and the tied covariance S = gram - sum_c n_c mu_c mu_c^T (on the host).
+ * Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+int rd_feature_moments(const float* feats, const int64_t* labels, int64_t n, int32_t F, int32_t n_classes,
+                       int32_t accumulate, double* class_sums, int64_t* class_counts, double* gram, void* stream);
+
+/* The kNN bank of n feature rows feats [n, F]: bank [n, ld] = the L2-normalised rows f / max(||f||_2, 1e-12) (norm in
+ * fp64, as F.normalize divides) with zero columns F .. ld-1, and bank_lo = bank - trunc19(bank), the remainder the
+ * error-compensated GEMM reads.  ld a multiple of 4, both 16-byte aligned.  rd_raindrop_v2_ood_scores reads the bank
+ * with round_up(n, 4) rows: the caller allocates those (their values are never used). */
+int rd_ood_prepare_bank(const float* feats, int64_t n, int32_t F, int32_t ld, float* bank, float* bank_lo, void* stream);
+
+/* Per-sample OOD scores of a batch, per chunk of samples_per_chunk samples: ONE eval forward, then
+ *   logits [B, C] (a copy of the forward's), msp [B] = -max_c softmax(logits)_c and energy [B] = -T logsumexp(logits/T),
+ *   T = temperature > 0 (both in fp64 from the fp32 logits);
+ *   Mahalanobis: Z = (f - mean) W on the tensor cores (3xTF32, mean [Df] fp64 subtracted before rounding to fp32),
+ *     W^T = w_t [rp, Fp] (rp = r rounded up to 4; zero rows past r and zero columns past Df), then per class
+ *     d_c = ||Z - class_proj[c]||^2 in fp64 over rp columns (class_proj [n_classes, rp] = (mu_c - mean) W):
+ *     mahalanobis_per_class [B, C], mahalanobis [B] = min_c d_c over the d_c that are numbers and
+ *     mahalanobis_class [B] = its first argmin (NaN and class 0 when none is).
+ *     With W = V_r Lambda_r^-1/2 from the tied covariance this is min_c (f - mu_c)^T Sigma^+ (f - mu_c);
+ *   kNN: the L2-normalised rows q [B, Fp] against the bank [round_up(n_bank, 4), Fp] (rd_ood_prepare_bank) on the
+ *     tensor cores (3xTF32, one full-K dot per pair, so a similarity depends on neither the chunking nor the bank
+ *     slicing), in slices whose similarities fit in 64 MiB, each merged by a selection launch into a running list of
+ *     the ks = min(k + RD_OOD_SEL_EXTRA, n_bank) largest; the last launch recomputes those ks similarities as fp64
+ *     dots of the fp32 rows (NaN, from non-finite features, ranks last) and keeps the k largest of them:
+ *     knn_index [B, k] int64 = their bank rows (ties: the lower index first) and knn [B] = 2 - 2 s_(k), the squared
+ *     distance to the k-th neighbour.  A 3xTF32 similarity is within delta = (6 ceil(Fp/8) + 48) 2^-24 of exact (unit
+ *     rows), so the result is the top k of the fp64 dots whenever fewer than RD_OOD_SEL_EXTRA + 1 bank rows have dots
+ *     within 2 delta below the k-th.  1 <= k <= min(RD_OOD_MAX_K, n_bank).
+ * Any output may be NULL: Mahalanobis runs when one of its three outputs is given (then mean, w_t, class_proj and
+ * r >= 1 are needed), kNN when one of its two is (then bank, bank_lo and n_bank >= 1).  Eval arithmetic (dims->training
+ * must be 0); every output is bitwise independent of the chunking once dims->obprop_mode is pinned.  scratch:
+ * rd_ood_scores_scratch_bytes(dims, r, n_bank, k, samples_per_chunk) bytes, with r = 0 / n_bank = 0 for a call without
+ * Mahalanobis / kNN (0: invalid arguments).  Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+size_t rd_ood_scores_scratch_bytes(const rd_dims* dims, int32_t r, int64_t n_bank, int32_t k, int32_t samples_per_chunk);
+int rd_raindrop_v2_ood_scores(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                              const float* times, const int64_t* lengths, const float* node_scale, int32_t layer,
+                              const double* mean, const float* w_t, const float* class_proj, int32_t r, const float* bank,
+                              const float* bank_lo, int64_t n_bank, int32_t k, float temperature,
+                              int32_t samples_per_chunk, void* scratch, float* logits, float* msp, float* energy,
+                              float* mahalanobis, int64_t* mahalanobis_class, float* mahalanobis_per_class, float* knn,
+                              int64_t* knn_index, void* stream);
+
 /* y[i] = x[i] * keep(site, i) / (1 - p): nn.Dropout driven by the library's counter-based stream (rng_captured =
  * {seed, counter} on the device).  The same call on a gradient is its backward. */
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream);

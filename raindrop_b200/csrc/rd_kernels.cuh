@@ -226,6 +226,30 @@ int ablate_inputs(const float* src, const float* statics, const float* times, co
                   int P, int ast, int amask, int k, int64_t J, const uint64_t* rng, int64_t m0, int B, int nc, int T, int N,
                   int ds, uint8_t* keep, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
 
+// ---- out-of-distribution detection (rd_ood.cu; rd_feature_moments, rd_raindrop_v2_ood_scores) ------------------------
+// ood_moments: for feats f [n, F] and labels y [n], sums [C, F] (+)= the per-class sums and counts [C] (+)= the class
+// sizes (sums NULL: both skipped), gram [F, F] (+)= f^T f (NULL: skipped), fp64, each entry one sample at a time in index
+// order.  Labels outside [0, C) count nowhere.
+int ood_moments(const float* f, const int64_t* y, int64_t n, int F, int C, int accumulate, double* sums, int64_t* counts,
+                double* gram, cudaStream_t st);
+// ood_rows: out [n, ld] from f [n, F] (row stride ldf): mu NULL: the L2-normalised rows (F.normalize, eps 1e-12); else
+// fp32(f - mu).  Columns F .. ld-1 are 0.
+int ood_rows(const float* f, int64_t ldf, int64_t n, int F, const double* mu, int ld, float* out, cudaStream_t st);
+// ood_logit_scores: msp [n] = -max softmax, energy [n] = -T logsumexp(logits / T) (either may be NULL)
+int ood_logit_scores(const float* logits, int n, int C, float temperature, float* msp, float* energy, cudaStream_t st);
+// ood_class_dist: dist [n, C] = ||Z[r] - M[c]||^2 over rp columns (NULL: skipped), dmin [n] its minimum, cls [n] the
+// first argmin (each may be NULL)
+int ood_class_dist(const float* Z, const float* M, int n, int C, int rp, float* dist, float* dmin, int64_t* cls,
+                   cudaStream_t st);
+// ood_topk: merges sim [n, ncols] (row stride ld; column c is bank row col0 + c) into the running list run [n, ks] of
+// the ks largest (3xTF32 similarity, index) keys (first: it starts empty); last: recomputes the ks candidates'
+// similarities as fp64 dots of the query rows q [n, Fp] and the bank rows [., Fp], and writes the k largest of those,
+// idx [n, k] in (similarity descending, index ascending) order and knn [n] = 2 - 2 s_(k) (either may be NULL), instead
+// of run.  k <= ks <= RD_OOD_MAX_K + RD_OOD_SEL_EXTRA.
+int ood_topk(const float* sim, int64_t ld, int n, int ncols, int64_t col0, int k, int ks, int first, int last,
+             uint64_t* run,
+             const float* q, const float* bank, int Fp, float* knn, int64_t* idx, cudaStream_t st);
+
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 
 // y = LN(x) * gamma + beta over the last dim (width D); stats[row] = {mean, rstd}

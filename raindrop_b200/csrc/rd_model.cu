@@ -1718,6 +1718,218 @@ int rd_debug_ablation_inputs(const rd_dims* dims, const float* src, const float*
                        s0.B, nc, s0.T, s0.N, s0.ds, keep_table, src_e, statics_e, times_e, lengths_e, (cudaStream_t)stream);
 }
 
+// ---- out-of-distribution scores ---------------------------------------------------------------------------------------
+// Bank columns per similarity GEMM: as many as keep a chunk's [spc, slice] similarities within 64 MiB, a multiple of 4,
+// at most the whole (padded) bank.  Slicing does not change a similarity: every one is a full-K dot of the same rows.
+static int64_t ood_slice(int64_t n_bank, int spc) {
+  const int64_t cap = ((1LL << 24) / spc) / 4 * 4, all = round_up(n_bank, 4);
+  return cap < 4 ? 4 : (cap < all ? cap : all);
+}
+
+// Candidates the kNN selection keeps per query row: k plus RD_OOD_SEL_EXTRA, at most the bank.
+static int ood_selected(int k, int64_t n_bank) {
+  return (int)(k + RD_OOD_SEL_EXTRA < n_bank ? k + RD_OOD_SEL_EXTRA : n_bank);
+}
+
+// A chunk of spc samples (ChunkLayout), then the centred or normalised query rows q [spc, Fp], Z [spc, rp], the
+// remainder of W^T [rp, Fp], the similarities of one bank slice [spc, slice] and the running candidates [spc, ks] (uint64).
+struct OodScratch : ChunkLayout { int64_t q, Z, Wlo, sim, run; };
+static int ood_scratch(const rd_dims* dims, int r, int64_t n_bank, int k, int spc, OodScratch* l) {
+  RD_TRY(chunk_layout(dims, "samples_per_chunk", spc, 1, false, 0, false, l));
+  Shape s;
+  RD_TRY(make_shape(dims, &s));
+  if (r < 0 || r > s.Df || n_bank < 0 || n_bank > 0x7fffffffLL) {
+    set_error("rank r = %d must be in [0, %d] and n_bank = %lld in [0, 2^31)", r, s.Df, (long long)n_bank);
+    return -2;
+  }
+  if (n_bank > 0 && (k < 1 || k > RD_OOD_MAX_K || k > n_bank)) {
+    set_error("k = %d must be in [1, min(%d, n_bank = %lld)]", k, RD_OOD_MAX_K, (long long)n_bank);
+    return -2;
+  }
+  const int64_t Fp = round_up(s.Df, 4), rp = round_up(r, 4);
+  l->q = l->a.take(spc * Fp);
+  l->Z = l->a.take(spc * rp);
+  l->Wlo = l->a.take(rp * Fp);
+  l->sim = l->a.take(n_bank > 0 ? spc * ood_slice(n_bank, spc) : 0);
+  l->run = l->a.take(n_bank > 0 ? 2LL * spc * ood_selected(k, n_bank) : 0);
+  return 0;
+}
+
+// Samples b0 .. b0+m-1 of the batch into the chunk's input buffers (src [T, m, 2N], times [T, m], statics, lengths).
+static int ood_slice_inputs(const Shape& s0, const float* src, const float* statics, const float* times,
+                            const int64_t* lengths, int b0, int m, const Expanded& x, cudaStream_t st) {
+  const size_t w = (size_t)2 * s0.N * sizeof(float);
+  cudaError_t e = cudaMemcpy2DAsync(x.src, m * w, src + (int64_t)b0 * 2 * s0.N, s0.B * w, m * w, s0.T,
+                                    cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess)
+    e = cudaMemcpy2DAsync(x.times, m * sizeof(float), times + b0, s0.B * sizeof(float), m * sizeof(float), s0.T,
+                          cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess && s0.ds > 0)
+    e = cudaMemcpyAsync(x.statics, statics + (int64_t)b0 * s0.ds, (size_t)m * s0.ds * sizeof(float),
+                        cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(x.lengths, lengths + b0, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToDevice, st);
+  if (e != cudaSuccess) { set_error("ood: chunk copy: %s", cudaGetErrorString(e)); return -1; }
+  return 0;
+}
+
+// The eval forward of samples b0 .. b0+m-1 (the inputs themselves when one chunk covers the batch); returns the chunk's
+// shape and, through feat, the chosen layer's rows [m, Df] in the workspace.  The logits land at S + l.logits.
+static int ood_chunk_forward(const rd_dims* dims, const rd_params* params, const Shape& s0, const float* src,
+                             const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
+                             int layer, int spc, int b0, int m, float* S, const ChunkLayout& l, const float** feat,
+                             cudaStream_t st) {
+  const rd_dims dc = chunk_dims(dims, m, spc, 0);
+  Shape s;
+  RD_TRY(make_shape(&dc, &s));
+  Expanded x{const_cast<float*>(src), const_cast<float*>(statics), const_cast<float*>(times),
+             const_cast<int64_t*>(lengths)};
+  if (m < s0.B) {
+    x = l.inputs(S, s0.ds);
+    RD_TRY(ood_slice_inputs(s0, src, statics, times, lengths, b0, m, x, st));
+  }
+  RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, S + l.logits,
+                      nullptr, nullptr, nullptr, 0, st));
+  const WsLayout w = ws_layout(s);
+  *feat = S + l.ws + (layer == RD_OOD_HIDDEN ? w.hpre : w.feat);
+  return 0;
+}
+
+static int ood_model_check(const char* fn, const rd_params* params, const float* src, const float* times, int layer,
+                           int spc, const void* scratch) {
+  if (!src || !times || !scratch || !params->R_u || !params->ob1_value_weight) { set_error("%s: NULL argument", fn); return -2; }
+  if (layer != RD_OOD_POOLED && layer != RD_OOD_HIDDEN) { set_error("%s: layer must be RD_OOD_POOLED or RD_OOD_HIDDEN", fn); return -2; }
+  if (spc < 1) { set_error("%s: samples_per_chunk must be >= 1", fn); return -2; }
+  return 0;
+}
+
+static int ood_copy(void* dst, const void* src, size_t bytes, cudaStream_t st) {
+  const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st);
+  if (e != cudaSuccess) { set_error("ood: copy: %s", cudaGetErrorString(e)); return -1; }
+  return 0;
+}
+
+size_t rd_ood_features_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk) {
+  ChunkLayout l;
+  if (!dims || chunk_layout(dims, "samples_per_chunk", samples_per_chunk, 1, false, 0, false, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+int rd_raindrop_v2_features(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                            const float* times, const int64_t* lengths, const float* node_scale, int32_t layer,
+                            int32_t samples_per_chunk, void* scratch, float* feats, float* logits, void* stream) {
+  const char* fn = "rd_raindrop_v2_features";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  RD_TRY(ood_model_check(fn, params, src, times, layer, samples_per_chunk, scratch));
+  ChunkLayout l;
+  RD_TRY(chunk_layout(dims, "samples_per_chunk", samples_per_chunk, 1, false, 0, false, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  float* S = (float*)scratch;
+  for (int b0 = 0; b0 < s0.B; b0 += samples_per_chunk) {
+    const int m = s0.B - b0 < samples_per_chunk ? s0.B - b0 : samples_per_chunk;
+    const float* f;
+    RD_TRY(ood_chunk_forward(dims, params, s0, src, statics, times, lengths, node_scale, layer, samples_per_chunk, b0, m, S,
+                             l, &f, st));
+    if (feats) RD_TRY(ood_copy(feats + (int64_t)b0 * s0.Df, f, (size_t)m * s0.Df * sizeof(float), st));
+    if (logits) RD_TRY(ood_copy(logits + (int64_t)b0 * s0.ncls, S + l.logits, (size_t)m * s0.ncls * sizeof(float), st));
+  }
+  return 0;
+}
+
+int rd_feature_moments(const float* feats, const int64_t* labels, int64_t n, int32_t F, int32_t n_classes,
+                       int32_t accumulate, double* class_sums, int64_t* class_counts, double* gram, void* stream) {
+  const char* fn = "rd_feature_moments";
+  if (!feats || (class_sums && (!labels || !class_counts))) { set_error("%s: NULL argument", fn); return -2; }
+  if (n < 0 || F < 1 || n_classes < 1) { set_error("%s: n = %lld must be >= 0, F = %d and n_classes = %d >= 1", fn, (long long)n, F, n_classes); return -2; }
+  if (n == 0 && accumulate) return 0;
+  return ood_moments(feats, labels, n, F, n_classes, accumulate, class_sums, class_counts, gram, (cudaStream_t)stream);
+}
+
+int rd_ood_prepare_bank(const float* feats, int64_t n, int32_t F, int32_t ld, float* bank, float* bank_lo, void* stream) {
+  const char* fn = "rd_ood_prepare_bank";
+  if (!feats || !bank || !bank_lo) { set_error("%s: NULL argument", fn); return -2; }
+  if (n < 1 || n > 0x7fffffffLL || F < 1 || ld < F || ld % 4) {
+    set_error("%s: n = %lld must be in [1, 2^31), F >= 1 and ld >= F a multiple of 4 (F = %d, ld = %d)", fn, (long long)n, F, ld);
+    return -2;
+  }
+  if ((reinterpret_cast<uintptr_t>(bank) | reinterpret_cast<uintptr_t>(bank_lo)) & 15) {
+    set_error("%s: bank and bank_lo must be 16-byte aligned", fn);
+    return -2;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  RD_TRY(ood_rows(feats, F, n, F, nullptr, ld, bank, st));
+  return grad_lo_image(bank, n * ld, bank_lo, st);
+}
+
+size_t rd_ood_scores_scratch_bytes(const rd_dims* dims, int32_t r, int64_t n_bank, int32_t k, int32_t samples_per_chunk) {
+  OodScratch l;
+  if (!dims || ood_scratch(dims, r, n_bank, k, samples_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+// Per chunk: one eval forward; msp / energy from its logits; Z = (f - mean) W (tc_nt, 3xTF32) and the class distances;
+// the normalised rows against each bank slice (tc_nt, 3xTF32) merged into the running top-k.
+int rd_raindrop_v2_ood_scores(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                              const float* times, const int64_t* lengths, const float* node_scale, int32_t layer,
+                              const double* mean, const float* w_t, const float* class_proj, int32_t r, const float* bank,
+                              const float* bank_lo, int64_t n_bank, int32_t k, float temperature,
+                              int32_t samples_per_chunk, void* scratch, float* logits, float* msp, float* energy,
+                              float* mahalanobis, int64_t* mahalanobis_class, float* mahalanobis_per_class, float* knn,
+                              int64_t* knn_index, void* stream) {
+  const char* fn = "rd_raindrop_v2_ood_scores";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  RD_TRY(ood_model_check(fn, params, src, times, layer, samples_per_chunk, scratch));
+  const bool do_maha = mahalanobis || mahalanobis_class || mahalanobis_per_class, do_knn = knn || knn_index;
+  if (do_maha && (!mean || !w_t || !class_proj || r < 1)) { set_error("%s: Mahalanobis outputs need mean, w_t, class_proj and r >= 1", fn); return -2; }
+  if (do_knn && (!bank || !bank_lo || n_bank < 1)) { set_error("%s: kNN outputs need bank, bank_lo and n_bank >= 1", fn); return -2; }
+  if ((msp || energy) && !(temperature > 0.f && isfinite(temperature))) {
+    set_error("%s: temperature must be finite and > 0, got %g", fn, temperature);
+    return -2;
+  }
+  OodScratch l;
+  RD_TRY(ood_scratch(dims, do_maha ? r : 0, do_knn ? n_bank : 0, k, samples_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  float* S = (float*)scratch;
+  const int spc = samples_per_chunk, Fp = (int)round_up(s0.Df, 4), rp = (int)round_up(r, 4);
+  if (do_maha) RD_TRY(grad_lo_image(w_t, (long long)rp * Fp, S + l.Wlo, st));
+  const int64_t slice = do_knn ? ood_slice(n_bank, spc) : 0;
+  for (int b0 = 0; b0 < s0.B; b0 += spc) {
+    const int m = s0.B - b0 < spc ? s0.B - b0 : spc;
+    const float* f;
+    RD_TRY(ood_chunk_forward(dims, params, s0, src, statics, times, lengths, node_scale, layer, spc, b0, m, S, l, &f, st));
+    const float* lg = S + l.logits;
+    if (logits) RD_TRY(ood_copy(logits + (int64_t)b0 * s0.ncls, lg, (size_t)m * s0.ncls * sizeof(float), st));
+    if (msp || energy) RD_TRY(ood_logit_scores(lg, m, s0.ncls, temperature, msp ? msp + b0 : nullptr, energy ? energy + b0 : nullptr, st));
+    if (do_maha) {
+      RD_TRY(ood_rows(f, s0.Df, m, s0.Df, mean, Fp, S + l.q, st));
+      TcNtArgs g;
+      g.A = S + l.q; g.lda = Fp; g.B = w_t; g.B_lo = S + l.Wlo; g.M = m; g.N = rp; g.K = Fp; g.C = S + l.Z;
+      tc_nt_plan(m, rp, true, &g.BN, &g.n_tiles);
+      RD_TRY(tc_nt(g, st));
+      RD_TRY(ood_class_dist(S + l.Z, class_proj, m, s0.ncls, rp,
+                            mahalanobis_per_class ? mahalanobis_per_class + (int64_t)b0 * s0.ncls : nullptr,
+                            mahalanobis ? mahalanobis + b0 : nullptr, mahalanobis_class ? mahalanobis_class + b0 : nullptr, st));
+    }
+    if (do_knn) {
+      RD_TRY(ood_rows(f, s0.Df, m, s0.Df, nullptr, Fp, S + l.q, st));
+      for (int64_t c0 = 0; c0 < n_bank; c0 += slice) {
+        const int nc = (int)(n_bank - c0 < slice ? n_bank - c0 : slice), ncp = (int)round_up(nc, 4);
+        TcNtArgs g;
+        g.A = S + l.q; g.lda = Fp; g.B = bank + c0 * Fp; g.B_lo = bank_lo + c0 * Fp; g.M = m; g.N = ncp; g.K = Fp;
+        g.C = S + l.sim;
+        tc_nt_plan(m, ncp, true, &g.BN, &g.n_tiles);
+        RD_TRY(tc_nt(g, st));
+        RD_TRY(ood_topk(S + l.sim, ncp, m, nc, c0, k, ood_selected(k, n_bank), c0 == 0, c0 + slice >= n_bank,
+                        reinterpret_cast<uint64_t*>(S + l.run),
+                        S + l.q, bank, Fp, knn ? knn + b0 : nullptr, knn_index ? knn_index + (int64_t)b0 * k : nullptr, st));
+      }
+    }
+  }
+  return 0;
+}
+
 size_t rd_dp_scratch_bytes(const rd_dims* dims) {
   Shape s;
   if (make_shape(dims, &s) != 0) return 0;

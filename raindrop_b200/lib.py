@@ -17,6 +17,8 @@ GRAD_DOT_SEGMENT = 4096     # RD_GRAD_DOT_SEGMENT
 LAPLACE_MAX_CLASSES = 8     # RD_LAPLACE_MAX_CLASSES
 LAPLACE_PIVOT_TOL = 1e-12   # RD_LAPLACE_PIVOT_TOL
 ABLATION_MAX_PLAYERS = 4096  # RD_ABLATION_MAX_PLAYERS
+OOD_MAX_K = 256             # RD_OOD_MAX_K
+OOD_POOLED, OOD_HIDDEN = 0, 1   # enum rd_ood_layer
 
 # enum rd_ws_buffer
 WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
@@ -152,6 +154,16 @@ SIGNATURES = {
                                                           C.c_void_p]),
     "rd_debug_ablation_inputs": (C.c_int, [C.POINTER(RdDims)] + [C.c_void_p] * 5 + [C.c_int32] * 5 +
                                  [C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 6),
+    "rd_ood_features_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
+    "rd_raindrop_v2_features": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 5 +
+                                [C.c_int32, C.c_int32] + [C.c_void_p] * 4),
+    "rd_feature_moments": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32] +
+                           [C.c_void_p] * 4),
+    "rd_ood_prepare_bank": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rd_ood_scores_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
+    "rd_raindrop_v2_ood_scores": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 5 + [C.c_int32] +
+                                  [C.c_void_p] * 3 + [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float,
+                                                      C.c_int32] + [C.c_void_p] * 10),
     "rd_encoder_head_fwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
     "rd_encoder_head_bwd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(RdGrads), C.c_void_p, C.c_void_p, C.c_void_p]),

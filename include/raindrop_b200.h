@@ -878,6 +878,56 @@ int rd_laplace_predictive_mc(const float* mean_logits, const double* cov, int32_
                              int32_t n_samples, int32_t samples_per_chunk, void* scratch, float* mean_probs,
                              float* variance, float* entropies, float* samples, void* stream);
 
+/* ---- SWA / SWAG of Raindrop_v2 (Izmailov et al. 2018; Maddox et al. 2019; MultiSWAG, Wilson & Izmailov 2020) ---------
+ * theta is a flat fp32 parameter bucket of n floats (n % 4 == 0; TrainStep's layout, padding lanes 0).  A SWAG posterior
+ * is the fp64 running moments mean [n], sq_mean [n] of the snapshots collected so far and up to `rank` deviation
+ * columns dev [rank, n] fp32 (slot-major: each column is contiguous); with c snapshots, k = min(c, rank) columns hold
+ * data.  Every fp64 operation is rounded on its own (no FMA contraction), so a float64 restatement matches bit for bit.
+ * Buffers are 16-byte aligned. */
+#define RD_SWAG_MAX_RANK 1024
+/* Folds snapshot c = n_collected into the moments:
+ *   mean' = (c mean + theta) / (c + 1),  sq_mean' = (c sq_mean + theta^2) / (c + 1)   (fp64)
+ * and, when rank > 0, writes slot c % rank of dev = fp32(theta - mean') (fp64 difference).  rank = 0 keeps the moments
+ * only (SWAG-diagonal; dev may be NULL).  One launch; theta is only read. */
+int rd_swag_collect(const float* theta, int64_t n, int64_t n_collected, int32_t rank, double* mean, double* sq_mean,
+                    float* dev, void* stream);
+/* Draws one weight vector of the posterior (fp64, the slot sum in slot order j = 0 .. k-1):
+ *   theta_out = fp32(mean + sqrt(scale) (sqrt(max(sq_mean - mean^2, 0)) z1 + [k >= 2] sum_{j<k} dev[j] z2_j / sqrt(k - 1)))
+ * scale = 0.5 is Maddox et al.'s 1/sqrt(2) on both terms; scale = 0 returns fp32(mean).  z is a standard normal of the
+ * Philox4x32-10 stream of the dropout masks with key {seed, step + replicate} (rng = {seed, step}, device uint64[2], read
+ * only), site 102 (96: DP noise, 97: Fisher labels, 98: PGD start, 99: Laplace, 100: smoothing, 101: ablation): element
+ * index i for z1[i] (i < n) and n + j for z2_j, counter index >> 2, Box-Muller on the block's word pairs as
+ * rd_dp_add_noise draws them.  Lanes where mean, sq_mean and dev are 0 (the bucket's padding) come out as +0.
+ * 0 <= k <= RD_SWAG_MAX_RANK (dev may be NULL when k < 2), scale finite and >= 0, replicate >= 0.  One launch. */
+int rd_swag_sample(const double* mean, const double* sq_mean, const float* dev, int64_t n, int32_t k, double scale,
+                   const uint64_t* rng, int64_t replicate, float* theta_out, void* stream);
+/* One member of a (Multi)SWAG predictive: a posterior as rd_swag_sample reads it. */
+typedef struct rd_swag_member {
+  const double* mean;
+  const double* sq_mean;
+  const float* dev;
+  int32_t k;
+} rd_swag_member;
+/* Scratch of rd_raindrop_v2_swag_predictive: the forward workspace and inputs of rows_per_chunk samples, the fp64 sums
+ * of mc_dropout's reduction and one replicate's logits [B, C]; 0 for arguments it refuses. */
+size_t rd_swag_predictive_scratch_bytes(const rd_dims* dims, int32_t rows_per_chunk);
+/* The Bayesian model average of the batch over sampled weights.  Replicate r = member * n_samples + s (M = n_members *
+ * n_samples in all) is the eval forward of the batch with the weights theta_s = rd_swag_sample(members[member], scale,
+ * rng, replicate = r): one sample launch into theta_s [n], then the eval forward over chunks of rows_per_chunk samples
+ * with `params`, whose trained pointers lie in theta_s (R_u and the untrained tensors are the model's), writing the
+ * replicate's logits [B, C], then one reduction launch of rd_raindrop_v2_mc_dropout (replicate offset r, total M):
+ * mean_probs [B, C], variance [B, C], entropies [3, B] and samples [M, B, C] (optional, may be NULL), defined as there.
+ * scale = 0 with n_samples = 1 is the deep ensemble of the members' mean weights.  Eval arithmetic: dims->training must
+ * be 0; the model's rng is neither read nor written.  dims->obprop_mode 0 is resolved once from rows_per_chunk rows, so
+ * the result is bitwise independent of the chunking.  `members` is a host array of n_members >= 1 entries, read during
+ * the call.  scratch: rd_swag_predictive_scratch_bytes(dims, rows_per_chunk) bytes.  Stream-ordered, allocation- and
+ * sync-free, CUDA-graph capturable. */
+int rd_raindrop_v2_swag_predictive(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                   const float* times, const int64_t* lengths, const float* node_scale,
+                                   const rd_swag_member* members, int32_t n_members, double scale, const uint64_t* rng,
+                                   int32_t n_samples, float* theta_s, int64_t n, int32_t rows_per_chunk, void* scratch,
+                                   float* mean_probs, float* variance, float* entropies, float* samples, void* stream);
+
 /* debug: when `buffer` is non-NULL ([n_ctas][16] uint64 on the device), the tensor-core attention kernels write the
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);

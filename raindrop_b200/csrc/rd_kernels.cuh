@@ -226,6 +226,18 @@ int ablate_inputs(const float* src, const float* statics, const float* times, co
                   int P, int ast, int amask, int k, int64_t J, const uint64_t* rng, int64_t m0, int B, int nc, int T, int N,
                   int ds, uint8_t* keep, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
 
+// ---- SWA / SWAG (rd_swag.cu; rd_swag_collect, rd_swag_sample, rd_raindrop_v2_swag_predictive) ----------------------
+constexpr uint32_t SITE_SWAG = 102;         // Philox site of the SWAG weight draws (its key is {seed, step + replicate})
+// swag_collect: with c snapshots folded in, mean = (c mean + theta) / (c + 1) and sq = (c sq + theta^2) / (c + 1) in
+// fp64, and (rank > 0) slot c % rank of dev [rank, n] = fp32(theta - mean).  n % 4 == 0, 16-byte aligned buffers.
+int swag_collect(const float* theta, int64_t n, int64_t c, int rank, double* mean, double* sq, float* dev, cudaStream_t st);
+// swag_sample: out [n] = fp32(mean + sqrt(scale) (sqrt(max(sq - mean^2, 0)) z1 + [k >= 2] sum_{j<k} dev[j] z2_j /
+// sqrt(k - 1))) in fp64, z drawn at key {rng[0], rng[1] + replicate}, element i for z1[i] and n + j for z2_j.
+int swag_sample(const double* mean, const double* sq, const float* dev, int64_t n, int k, double scale,
+                const uint64_t* rng, int64_t replicate, float* out, cudaStream_t st);
+int swag_sample_check(const char* fn, const double* mean, const double* sq, const float* dev, int64_t n, int k,
+                      double scale);
+
 // ---- out-of-distribution detection (rd_ood.cu; rd_feature_moments, rd_raindrop_v2_ood_scores) ------------------------
 // ood_moments: for feats f [n, F] and labels y [n], sums [C, F] (+)= the per-class sums and counts [C] (+)= the class
 // sizes (sums NULL: both skipped), gram [F, F] (+)= f^T f (NULL: skipped), fp64, each entry one sample at a time in index

@@ -1930,6 +1930,73 @@ int rd_raindrop_v2_ood_scores(const rd_dims* dims, const rd_params* params, cons
   return 0;
 }
 
+// SWAG predictive: a chunk of rpc samples (ChunkLayout), then the fp64 sums of mc_accumulate [B, 2*n_classes + 1] and
+// one replicate's logits [B, n_classes].
+struct SwagScratch : ChunkLayout { int64_t acc, rep; };
+static int swag_scratch(const rd_dims* dims, int rpc, SwagScratch* l) {
+  RD_TRY(chunk_layout(dims, "rows_per_chunk", rpc, 1, false, 0, false, l));
+  l->acc = l->a.take(2LL * dims->B * (2 * dims->n_classes + 1));
+  l->rep = l->a.take((int64_t)dims->B * dims->n_classes);
+  return 0;
+}
+
+size_t rd_swag_predictive_scratch_bytes(const rd_dims* dims, int32_t rows_per_chunk) {
+  SwagScratch l;
+  if (!dims || swag_scratch(dims, rows_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+// Per replicate: one sample launch into theta_s (the weights are drawn once per replicate), the eval forward of every
+// chunk of rpc samples into the replicate's logits, and one mc_accumulate launch.
+int rd_raindrop_v2_swag_predictive(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                   const float* times, const int64_t* lengths, const float* node_scale,
+                                   const rd_swag_member* members, int32_t n_members, double scale, const uint64_t* rng,
+                                   int32_t n_samples, float* theta_s, int64_t n, int32_t rows_per_chunk, void* scratch,
+                                   float* mean_probs, float* variance, float* entropies, float* samples, void* stream) {
+  const char* fn = "rd_raindrop_v2_swag_predictive";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !members || !rng || !theta_s || !scratch || !mean_probs || !variance || !entropies ||
+      !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (n_members < 1 || n_samples < 1 || rows_per_chunk < 1 || (int64_t)n_members * n_samples > 0x7fffffffLL) {
+    set_error("%s: n_members = %d, n_samples = %d and rows_per_chunk = %d must be >= 1 with n_members * n_samples < 2^31",
+              fn, n_members, n_samples, rows_per_chunk);
+    return -2;
+  }
+  for (int i = 0; i < n_members; ++i)
+    RD_TRY(swag_sample_check(fn, members[i].mean, members[i].sq_mean, members[i].dev, n, members[i].k, scale));
+  if (reinterpret_cast<uintptr_t>(theta_s) & 15) { set_error("%s: theta_s must be 16-byte aligned", fn); return -2; }
+  SwagScratch l;
+  RD_TRY(swag_scratch(dims, rows_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, rpc = rows_per_chunk;
+  const int64_t M = (int64_t)n_members * n_samples;
+  float* S = (float*)scratch;
+  double* acc = reinterpret_cast<double*>(S + l.acc);
+  float* rep = S + l.rep;
+  for (int64_t r = 0; r < M; ++r) {
+    const rd_swag_member& mb = members[r / n_samples];
+    RD_TRY(swag_sample(mb.mean, mb.sq_mean, mb.dev, n, mb.k, scale, rng, r, theta_s, st));
+    for (int b0 = 0; b0 < B; b0 += rpc) {
+      const int m = B - b0 < rpc ? B - b0 : rpc;
+      const rd_dims dc = chunk_dims(dims, m, rpc, 0);
+      Expanded x{const_cast<float*>(src), const_cast<float*>(statics), const_cast<float*>(times),
+                 const_cast<int64_t*>(lengths)};
+      if (m < B) {
+        x = l.inputs(S, s0.ds);
+        RD_TRY(ood_slice_inputs(s0, src, statics, times, lengths, b0, m, x, st));
+      }
+      RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws,
+                          rep + (int64_t)b0 * s0.ncls, nullptr, nullptr, nullptr, 0, st));
+    }
+    RD_TRY(mc_accumulate(rep, 1, B, s0.ncls, r, M, acc, samples, mean_probs, variance, entropies, r == 0, r == M - 1, st));
+  }
+  return 0;
+}
+
 size_t rd_dp_scratch_bytes(const rd_dims* dims) {
   Shape s;
   if (make_shape(dims, &s) != 0) return 0;

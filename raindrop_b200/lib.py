@@ -19,6 +19,7 @@ LAPLACE_PIVOT_TOL = 1e-12   # RD_LAPLACE_PIVOT_TOL
 ABLATION_MAX_PLAYERS = 4096  # RD_ABLATION_MAX_PLAYERS
 OOD_MAX_K = 256             # RD_OOD_MAX_K
 OOD_POOLED, OOD_HIDDEN = 0, 1   # enum rd_ood_layer
+SWAG_MAX_RANK = 1024        # RD_SWAG_MAX_RANK
 
 # enum rd_ws_buffer
 WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
@@ -69,6 +70,10 @@ class RdGrads(C.Structure):
 class RdWgradItem(C.Structure):
     _fields_ = [("d_out", C.c_void_p), ("x", C.c_void_p), ("rows", C.c_int64), ("out_features", C.c_int32),
                 ("in_features", C.c_int32), ("d_weight", C.c_void_p), ("d_bias", C.c_void_p), ("partial", C.c_void_p)]
+
+
+class RdSwagMember(C.Structure):
+    _fields_ = [("mean", C.c_void_p), ("sq_mean", C.c_void_p), ("dev", C.c_void_p), ("k", C.c_int32)]
 
 
 class RdDebugTcNtArgs(C.Structure):
@@ -240,6 +245,14 @@ SIGNATURES = {
     "rd_laplace_sample_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "rd_laplace_predictive_mc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32] +
                                  [C.c_void_p] * 6),
+    "rd_swag_collect": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
+    "rd_swag_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_double, C.c_void_p,
+                                 C.c_int64, C.c_void_p, C.c_void_p]),
+    "rd_swag_predictive_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
+    "rd_raindrop_v2_swag_predictive": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 5 +
+                                       [C.POINTER(RdSwagMember), C.c_int32, C.c_double, C.c_void_p, C.c_int32,
+                                        C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 6),
 }
 
 _lib = None

@@ -19,6 +19,12 @@ It prints delta, log Z and, per method, the NLL, the Brier score, the 15-bin exp
 at 100 / 90 / 80 / 70 % coverage (coverage_accuracy of tools/mc_uncertainty.py; samples ranked by mutual information
 where the method defines it, else by predictive entropy).  The file holds float32 [n, C] probabilities of every method
 (mc_dropout_probs, probit_probs, mc_probs, eval_probs), the scores used for the ranking, labels [n] and delta / log Z.
+
+--swag PATH (an SWAG posterior of this model, raindrop_b200.swag.SWAG.save; tools/swag_train.py writes one) adds three
+rows: SWA (the eval forward at the posterior's mean weights, ranked by predictive entropy), SWAG (swag_predictive with
+--swag-samples weight samples, ranked by mutual information) and, with --multi PATH ..., MultiSWAG over the --swag
+posterior and every --multi one (--swag-samples per member).  The file then also holds swa_probs, swag_probs and
+multiswag_probs with their scores.
 """
 import argparse
 import os
@@ -73,6 +79,9 @@ def main():
     ap.add_argument("--mc-samples", type=int, default=30, help="Monte Carlo dropout replicates")
     ap.add_argument("--laplace-samples", type=int, default=100, help="draws of the mc link")
     ap.add_argument("--batch-size", type=int, default=512)
+    ap.add_argument("--swag", help="an SWAG posterior of this model (SWAG.save): SWA and SWAG rows")
+    ap.add_argument("--multi", nargs="+", default=[], help="further SWAG posteriors (--swag needed): a MultiSWAG row")
+    ap.add_argument("--swag-samples", type=int, default=30, help="weight samples per SWAG member")
     ap.add_argument("--name")
     ap.add_argument("--out-dir", default=".")
     args = ap.parse_args()
@@ -136,6 +145,12 @@ def main():
 
     P, Pst, Pt, y = evl
     labels = y.cpu().numpy().astype(np.int64)
+    if args.multi and not args.swag:
+        raise SystemExit("--multi needs --swag")
+    posts = []
+    if args.swag:
+        from raindrop_b200.swag import SWAG
+        posts = [SWAG.load(p_, model) for p_ in [args.swag] + args.multi]
     methods = {"mc_dropout": args.dropout > 0, "probit": True, "mc": True}
     probs = {k: [] for k in methods}
     scores = {k: [] for k in methods}
@@ -162,13 +177,44 @@ def main():
         if on:
             out[k + "_probs"] = np.concatenate(probs[k])
             out[k + "_score"] = np.concatenate(scores[k])
+    swag_rows = []
+    if posts:
+        from raindrop_b200.swag import swag_predictive
+        swag_methods = {"swag": [posts[0]]}
+        if len(posts) > 1:
+            swag_methods["multiswag"] = posts
+        res = {k: ([], []) for k in ["swa"] + list(swag_methods)}
+        saved = [p_.detach().clone() for p_ in model.used_parameters()]
+        posts[0].load_mean(model)
+        for s in range(0, n, args.batch_size):
+            e = min(n, s + args.batch_size)
+            a = (P[:, s:e], None if Pst is None else Pst[s:e], Pt[:, s:e], torch.sum(Pt[:, s:e] > 0, dim=0))
+            with torch.no_grad():
+                p_swa = torch.softmax(model(*a)[0].double(), dim=1)
+            res["swa"][0].append(p_swa.float().cpu().numpy())
+            res["swa"][1].append((-(p_swa * torch.log(p_swa.clamp_min(1e-300))).sum(1)).float().cpu().numpy())
+        with torch.no_grad():
+            for p_, s_ in zip(model.used_parameters(), saved):
+                p_.copy_(s_)
+        for s in range(0, n, args.batch_size):
+            e = min(n, s + args.batch_size)
+            a = (P[:, s:e], None if Pst is None else Pst[s:e], Pt[:, s:e], torch.sum(Pt[:, s:e] > 0, dim=0))
+            for k, members in swag_methods.items():
+                r = swag_predictive(model, members, *a, n_samples=args.swag_samples, seed=args.seed)
+                res[k][0].append(r.mean_probs.cpu().numpy())
+                res[k][1].append(r.mutual_information.cpu().numpy())
+        labels_of = {"swa": "SWA (entropy)", "swag": "SWAG (M=%d, MI)" % args.swag_samples,
+                     "multiswag": "MultiSWAG (%d x %d, MI)" % (len(posts), args.swag_samples)}
+        for k, (pp, sc) in res.items():
+            out[k + "_probs"], out[k + "_score"] = np.concatenate(pp), np.concatenate(sc)
+            swag_rows.append((labels_of[k], out[k + "_probs"], out[k + "_score"]))
     path = os.path.join(args.out_dir, "Laplace_uncertainty_%s.npz" % name)
     np.savez(path, **out)
     print("wrote %s: %d samples" % (path, n))
     rows = [("eval forward", out["eval_probs"], None)] + \
         [({"mc_dropout": "MC dropout (M=%d, MI)" % args.mc_samples, "probit": "Laplace probit (entropy)",
            "mc": "Laplace mc (M=%d, MI)" % args.laplace_samples}[k], out[k + "_probs"], out[k + "_score"])
-         for k, on in methods.items() if on]
+         for k, on in methods.items() if on] + swag_rows
     print("%-28s %8s %8s %8s   accuracy at coverage 100 / 90 / 80 / 70 %%" % ("method", "NLL", "Brier", "ECE"))
     for label, p, score in rows:
         nll, brier, ece = calibration(p, labels)

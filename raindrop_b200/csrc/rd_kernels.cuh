@@ -309,7 +309,7 @@ int attn_small_bwd(const float* qkv, const float* dctx, const int64_t* lengths, 
 
 // the same on the tensor cores (rd_attn_tc.cu: mma.sync 3xTF32, T <= 64, hd <= 96, hd % 4 == 0)
 bool attn_tc_supported(int T, int hd);
-void attn_tc_set_debug(unsigned long long* buf);   // start / end clock64 stamps per CTA: [CTA][16], slots 0 and 12 (debug)
+void attn_tc_set_debug(unsigned long long* buf);   // clock64 phase stamps per CTA: [CTA][16], slots 0-5 and 12 (debug)
 int attn_tc_fwd(const float* qkv, const int64_t* lengths, int B, int H, int T, int hd, float drop_p,
                 const uint64_t* rng, uint32_t site, float* ctx, cudaStream_t st, DropRep rep = {});
 int attn_tc_bwd(const float* qkv, const float* dctx, const int64_t* lengths, int B, int H, int T, int hd,

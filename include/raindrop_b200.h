@@ -932,7 +932,9 @@ int rd_raindrop_v2_swag_predictive(const rd_dims* dims, const rd_params* params,
  * SM clock (clock64) of each CTA's start into slot 0 and of its end into slot 12; NULL switches it off. */
 int rd_debug_attention_timing(uint64_t* buffer);
 /* same for the tensor-core GEMM kernel (rd_linear_fwd, the encoder and ob-prop GEMMs): [n_ctas][8] uint64,
- * %globaltimer at the CTA's start (slot 0) and end (slot 7) */
+ * %globaltimer at the CTA's entry (slot 5), after its grid dependency wait (0), at the first full stage seen by MMA
+ * thread 0 (1), at that thread's last wgmma retired (2), at the epilogue end of MMA warpgroup 0 / 1 (3 / 4) and at the
+ * end of thread 0 (7) */
 int rd_debug_gemm_timing(uint64_t* buffer);
 /* same for the grouped weight-gradient kernel (rd_linear_wgrad_group and the training backward): [n_ctas][16] uint64
  * per launch CTA (at most one per SM), clock64 at the CTA's start (slot 0) and end (1); summed cycles of the producer

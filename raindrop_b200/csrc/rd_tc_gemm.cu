@@ -49,7 +49,7 @@ struct NtP {
   uint32_t* drop_mask; int drop_mask_ld;
   const float* resid; long long resid_ld;
   int pB, pN, pD;
-  unsigned long long* dbg;     // optional %globaltimer stamps [CTA][8] (rd_debug_gemm_timing)
+  unsigned long long* dbg;     // optional %globaltimer stamps [CTA][8] (rd_debug_gemm_timing, slots in tc_nt_kernel)
 };
 
 __device__ __forceinline__ void gstamp(const NtP& p, int slot) {
@@ -64,6 +64,15 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
   return v;
+}
+
+// 8-column groups per epilogue chunk: the registers a group holds across the chunk (bias 2, gate 4, residual 4, keep
+// bits and the Philox state 7, 2 more with the replicate rows' keys) beside the BN / 2 accumulators, within a budget
+// fitted to ptxas's allocation
+__host__ __device__ constexpr int nt_epi_chunk(int F, int BN) {
+  const int per_group = 2 + 4 * !!(F & F_GATE) + 4 * !!(F & F_RESID) + 7 * !!(F & F_DROP) + 2 * !!(F & F_REP);
+  const int jc = (128 - BN / 2) / per_group;
+  return jc > 8 ? 8 : (jc < 2 ? 2 : jc);
 }
 
 // one k-block: per 8-wide k-step one wgmma across the whole tile width per term, small terms first (lo.hi, hi.lo, hi.hi)
@@ -108,7 +117,10 @@ template <int F, bool EXACT, int BN>
 __global__ void __launch_bounds__(NT_THREADS, 1)
 tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmBlo, const NtP p) {
+  // %globaltimer stamps when p.dbg is set, per CTA: 5 entry, 0 after the grid dependency wait, 1 the first full stage
+  // seen by MMA thread 0, 2 its last wgmma retired, 3 / 4 the epilogue end of warpgroup 0 / 1, 7 the end of thread 0
   extern __shared__ uint8_t smem_raw[];
+  if (threadIdx.x == 0) gstamp(p, 5);
   pdl_launch_dependents();
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -181,6 +193,7 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     // kb + 1 are loaded and split into the other buffer (its previous group retired at the wait<1> before)
     uint32_t ah0[BK / 8][4], al0[BK / 8][4], ah1[BK / 8][4], al1[BK / 8][4];
     uint32_t sb0 = acquire(ah0, al0), sb1 = 0;
+    if (threadIdx.x == 0 && tile == blockIdx.x) gstamp(p, 1);
     for (int kb = 0; kb < p.k_blocks; kb += 2) {
       issue_kblock<BN, EXACT>(acc, ah0, al0, sb0, b_tile);
       wgmma_wait<1>();
@@ -196,6 +209,7 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 #pragma unroll
     for (int e = 0; e < BN / 2; ++e) fence_operand(acc[e]);
     release();
+    if (threadIdx.x == 0) gstamp(p, 2);
 
     // ---- epilogue on the accumulator registers: element (row0 + 8i, col0 + 8j + 2t + {0, 1}) ----
     const long long row0 = (long long)m_t * BM + arow;
@@ -211,69 +225,107 @@ tc_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 #pragma unroll
       for (int i = 0; i < 2; ++i) sc[i] = row0 + 8 * i < p.M ? __ldg(p.scale + ((row0 + 8 * i) % p.scale_mod)) : 0.f;
     }
+    // In chunks of JC 8-column groups: first every global load of the chunk (bias, gate, residual) and its dropout
+    // draws, then the arithmetic and the stores.  The compiler keeps a load after any store that may alias it, so with
+    // loads and stores interleaved per group every group cost one memory round trip.  JC is as many groups as fit
+    // next to the accumulators in the 168 registers ptxas allocates for this launch shape (no spills at any width).
+    constexpr int NJ = BN / 8;
+    constexpr int JC = nt_epi_chunk(F, BN);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = col0 + 8 * j + 2 * t;
-      const bool col_ok = col < p.N;                 // N even, col even: the pair is all in or all out
-      float b0 = 0.f, b1 = 0.f;
-      if (p.bias && col_ok) { b0 = __ldg(p.bias + col); b1 = __ldg(p.bias + col + 1); }
-      uint32_t bits[2] = {0u, 0u};
+    for (int j0 = 0; j0 < NJ; j0 += JC) {
+      float2 bv[JC], gv[JC][2], rv[JC][2];
+      uint32_t keep2[JC][2];     // keep bits of this lane's two columns, per row
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const long long row = row0 + 8 * i;
-        const bool ok = col_ok && row < p.M;
-        float v0 = acc[4 * j + 2 * i] + b0, v1 = acc[4 * j + 2 * i + 1] + b1;
-        if (F & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        if (F & F_SCALE) { v0 *= sc[i]; v1 *= sc[i]; }
-        if (!ok) continue;
-        if (F & F_GATE) {   // backward: pass the gradient only where the forward output was positive
-          const float2 gv = __ldg(reinterpret_cast<const float2*>(p.gate + row * p.gate_ld + col));
-          v0 = gv.x > 0.f ? v0 * p.gate_scale : 0.f;
-          v1 = gv.y > 0.f ? v1 * p.gate_scale : 0.f;
-        }
-        if (F & F_DROP) {   // element index row*N + col; N % 4 == 0, so the pair shares one Philox block
-          const uint64_t idx = (F & F_REP) ? rbase[i] + (uint64_t)col : (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
-          const uint4 u = dropout_block((F & F_REP) ? rkey[i] : key, p.drop_site, idx);
-          const bool lo_half = (idx & 3u) == 0;
-          const float m0 = keep_scale(lo_half ? u.x : u.z, p.drop_p, ik), m1 = keep_scale(lo_half ? u.y : u.w, p.drop_p, ik);
-          v0 *= m0; v1 *= m1;
-          bits[i] = (m0 > 0.f ? 1u : 0u) | (m1 > 0.f ? 2u : 0u);
-        }
-        if (F & F_RESID) {
-          const float2 r = __ldg(reinterpret_cast<const float2*>(p.resid + row * p.resid_ld + col));
-          v0 += r.x; v1 += r.y;
-        }
-        if (F & F_ROUND) { v0 = rn_tf32(v0); v1 = rn_tf32(v1); }
-        float* dst;
-        if (F & F_PERM) {   // row = b*pN + n, col = tt*4 + k  ->  encoder input [T, B, D] (code/models_rd.py:338-341)
-          const long long b = row / p.pN, n = row - b * p.pN;
-          dst = p.C + ((long long)(col >> 2) * p.pB + b) * p.pD + n * 4 + (col & 3);
-        } else {
-          dst = p.C + row * p.ldc + col;
-        }
-        *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
-      }
-      if ((F & F_DROP) && p.drop_mask) {
-        // the backward of the consumer (LayerNorm) reads these bits instead of regenerating the Philox stream.  Columns
-        // 8j .. 8j+7 are one byte of the row's bit words (col0 % 8 == 0) and belong to this tile alone, so tiles that
-        // share a word never write the same byte.  Bytes past N up to the word's end are written as zeros by the tile
-        // holding column N - 1.
-        const int cb = col0 + 8 * j;
+      for (int jj = 0; jj < JC && j0 + jj < NJ; ++jj) {
+        const int col = col0 + 8 * (j0 + jj) + 2 * t;
+        const bool col_ok = col < p.N;               // N even, col even: the pair is all in or all out
+        // plain loads, not ld.global.nc: a non-coherent load may be scheduled after the chunk's stores, and ptxas
+        // sinks it to its use there, which brings back one round trip per group
+        bv[jj] = make_float2(0.f, 0.f);
+        if (p.bias && col_ok) bv[jj] = make_float2(p.bias[col], p.bias[col + 1]);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-          uint32_t b8 = bits[i] << (2 * t);
-          b8 |= __shfl_xor_sync(0xffffffffu, b8, 1);
-          b8 |= __shfl_xor_sync(0xffffffffu, b8, 2);
           const long long row = row0 + 8 * i;
-          if (t == 0 && row < p.M && cb < p.N) {
-            uint8_t* w = reinterpret_cast<uint8_t*>(p.drop_mask + row * p.drop_mask_ld);
-            w[cb >> 3] = (uint8_t)b8;
-            if (cb + 8 >= p.N)
-              for (int z = (cb >> 3) + 1; z < 4 * p.drop_mask_ld && z < 4 * ((p.N + 31) >> 5); ++z) w[z] = 0;
+          const bool ok = col_ok && row < p.M;
+          if (F & F_GATE) gv[jj][i] = ok ? *reinterpret_cast<const float2*>(p.gate + row * p.gate_ld + col) : make_float2(0.f, 0.f);
+          if (F & F_RESID) rv[jj][i] = ok ? *reinterpret_cast<const float2*>(p.resid + row * p.resid_ld + col) : make_float2(0.f, 0.f);
+        }
+        if (F & F_DROP) {
+          // element index row*N + col (or through the replicate rows); N % 4 == 0, so lanes t and t^1 share the Philox
+          // block of their 4-column group in each of their two rows.  Lane t draws the block of row 8 (t & 1) only and
+          // hands its partner the keep bits of the partner's two columns: same block, word and decision per element.
+          const int ir = t & 1;             // the row this lane draws; its own columns are words 2 ir, 2 ir + 1
+          const long long row = row0 + 8 * ir;
+          uint32_t own = 0u, other = 0u;
+          if (col_ok && row < p.M) {
+            const uint64_t idx = (F & F_REP) ? rbase[ir] + (uint64_t)col : (uint64_t)row * (uint64_t)p.N + (uint64_t)col;
+            const uint4 u = dropout_block((F & F_REP) ? rkey[ir] : key, p.drop_site, idx);
+            const uint32_t lo = (keep_scale(u.x, p.drop_p, ik) > 0.f ? 1u : 0u) | (keep_scale(u.y, p.drop_p, ik) > 0.f ? 2u : 0u);
+            const uint32_t hi = (keep_scale(u.z, p.drop_p, ik) > 0.f ? 1u : 0u) | (keep_scale(u.w, p.drop_p, ik) > 0.f ? 2u : 0u);
+            own = ir ? hi : lo;
+            other = ir ? lo : hi;
+          }
+          keep2[jj][ir] = own;
+          keep2[jj][ir ^ 1] = __shfl_xor_sync(0xffffffffu, other, 1);
+        }
+      }
+#pragma unroll
+      for (int jj = 0; jj < JC && j0 + jj < NJ; ++jj) {
+        const int j = j0 + jj;
+        const int col = col0 + 8 * j + 2 * t;
+        const bool col_ok = col < p.N;
+        uint32_t bits[2] = {0u, 0u};
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const long long row = row0 + 8 * i;
+          const bool ok = col_ok && row < p.M;
+          float v0 = acc[4 * j + 2 * i] + bv[jj].x, v1 = acc[4 * j + 2 * i + 1] + bv[jj].y;
+          if (F & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (F & F_SCALE) { v0 *= sc[i]; v1 *= sc[i]; }
+          if (!ok) continue;
+          if (F & F_GATE) {   // backward: pass the gradient only where the forward output was positive
+            v0 = gv[jj][i].x > 0.f ? v0 * p.gate_scale : 0.f;
+            v1 = gv[jj][i].y > 0.f ? v1 * p.gate_scale : 0.f;
+          }
+          if (F & F_DROP) {
+            v0 *= (keep2[jj][i] & 1u) ? ik : 0.f;
+            v1 *= (keep2[jj][i] & 2u) ? ik : 0.f;
+            bits[i] = keep2[jj][i];
+          }
+          if (F & F_RESID) { v0 += rv[jj][i].x; v1 += rv[jj][i].y; }
+          if (F & F_ROUND) { v0 = rn_tf32(v0); v1 = rn_tf32(v1); }
+          float* dst;
+          if (F & F_PERM) {   // row = b*pN + n, col = tt*4 + k  ->  encoder input [T, B, D] (code/models_rd.py:338-341)
+            const long long b = row / p.pN, n = row - b * p.pN;
+            dst = p.C + ((long long)(col >> 2) * p.pB + b) * p.pD + n * 4 + (col & 3);
+          } else {
+            dst = p.C + row * p.ldc + col;
+          }
+          *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+        }
+        if ((F & F_DROP) && p.drop_mask) {
+          // the backward of the consumer (LayerNorm) reads these bits instead of regenerating the Philox stream.  Columns
+          // 8j .. 8j+7 are one byte of the row's bit words (col0 % 8 == 0) and belong to this tile alone, so tiles that
+          // share a word never write the same byte.  Bytes past N up to the word's end are written as zeros by the tile
+          // holding column N - 1.
+          const int cb = col0 + 8 * j;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            uint32_t b8 = bits[i] << (2 * t);
+            b8 |= __shfl_xor_sync(0xffffffffu, b8, 1);
+            b8 |= __shfl_xor_sync(0xffffffffu, b8, 2);
+            const long long row = row0 + 8 * i;
+            if (t == 0 && row < p.M && cb < p.N) {
+              uint8_t* w = reinterpret_cast<uint8_t*>(p.drop_mask + row * p.drop_mask_ld);
+              w[cb >> 3] = (uint8_t)b8;
+              if (cb + 8 >= p.N)
+                for (int z = (cb >> 3) + 1; z < 4 * p.drop_mask_ld && z < 4 * ((p.N + 31) >> 5); ++z) w[z] = 0;
+            }
           }
         }
       }
     }
+    if ((threadIdx.x & 127) == 0) gstamp(p, 3 + wg);
   }
   if (threadIdx.x == 0) gstamp(p, 7);
 }

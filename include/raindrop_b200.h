@@ -427,6 +427,70 @@ int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float
                        int32_t samples_per_chunk, void* scratch, float* src_adv, float* statics_adv, float* logits_adv,
                        float* logits_clean, float* loss_adv, void* stream);
 
+/* ---- counterfactual explanations of Raindrop_v2, in one call --------------------------------------------------------
+ * For each sample b and target class t_b (target NULL: the clean prediction's runner-up, the first argmax over
+ * c != the first argmax of logits_clean), a sparse, bounded change delta of the recorded values that makes the model
+ * predict t_b (Wachter et al. 2017; the elastic-net form of Dhurandhar et al. 2018).
+ * Mutable set S_b (the threat model of rd_raindrop_v2_pgd): the value cells with src[t, b, N + n] > 0 of sensors with
+ * sensor_mutable[n] != 0 (NULL: every sensor), plus the statics when opt->perturb_static.  The mask half, times and
+ * lengths never change; an element with delta == 0 is written as x bit for bit.
+ * Per element, given per sensor n (then per static column j at index N + j, read when perturb_static): a weight
+ * w > 0 (weights NULL: 1) and a box [lower, upper] (NULL: -inf / +inf), in normalised units.  The effective box is
+ * [min(lower, x), max(upper, x)], so delta = 0 is always feasible; clip_box clips to it.
+ * Objective over delta supported on S_b:  c_b max(0, kappa - m(x + delta)) + beta ||w delta||_1 + ||w delta||_2^2, with
+ * the logit margin m = z_t - max_{c != t} z_c (first index c* on ties).  The hinge is active when m <= kappa; its logit
+ * gradient c_b (e_{c*} - e_t) seeds the frozen-parameter backward.
+ * Round s = 0 .. n_search-1 of replica r restarts FISTA at the replica's start point (x_0 = y_0), then for
+ * k = 0 .. n_steps-1:  forward at y_k and track;  g = c grad(hinge)(y_k) + 2 w^2 y_k;
+ *   x_{k+1} = clip_box(S(y_k - alpha g, alpha beta w))  (S the soft-threshold);
+ *   y_{k+1} = clip_box(x_{k+1} + k/(k+3) (x_{k+1} - x_k));
+ * and a last forward and track at y_{n_steps}: n_steps + 1 forwards and n_steps backwards per round.  Element arithmetic
+ * is fp32 (the iterate the model reads is x + delta clamped to the box); per-sample sums, the distance and c are fp64.
+ * A point is valid when m > 0 and m >= kappa; its distance is d = beta ||w delta||_1 + ||w delta||_2^2 (fp64).  The
+ * result of sample b is the valid evaluated point of smallest d over all rounds, steps and replicas; ties go to the
+ * earliest (round, step), then the lowest replica.  Without a valid point: src_cf is x bit for bit, logits_cf =
+ * logits_clean, distance = +inf, valid = 0.
+ * Bisection per (sample, replica), lo = 0, hi = +inf, c = c_init; after each round (fp64):
+ *   the round found a valid point: hi = min(hi, c), c = (lo + hi) / 2;  else lo = max(lo, c), c = (lo + hi) / 2 if
+ *   hi < inf, else 10 c.
+ * Restarts: n_restarts = R independent replicas per sample, each with its own c.  Replica 0 starts at delta = 0; replica
+ * r >= 1 at clip_box(init_scale (2u - 1)) on S_b, u = (word >> 8) 2^-24 drawn from Philox4x32-10 at site 103 (96: DP
+ * noise, 97: Fisher labels, 98: PGD start, 99: Laplace, 100: smoothing, 101: ablation, 102: SWAG) under rng =
+ * {seed, step} (device uint64[2], read only; may be NULL when R = 1), element e (t*N + n for value cells, T*N + j for
+ * statics) at index (b*R + r)*(T*N + d_static) + e, the word of index i being word i & 3 of the block at counter i >> 2.
+ * A replica's search depends on (b, r) alone: replica 0 of an R-replica call is the R = 1 call.
+ *   src_cf       [T, B, 2N]: the returned input;  statics_cf [B, d_static] or NULL (skipped)
+ *   logits_cf    [B, n_classes] at it;  logits_clean [B, n_classes] at x;  target_out [B] int64
+ *   valid        [B] uint8;  distance [B] fp64
+ *   c_final      [B, R] fp64: c after the last round's update;  round_valid [B, R, n_search] uint8
+ * Eval arithmetic (dims->training must be 0): no dropout, the model's rng state is neither read nor advanced, no
+ * parameter gradient is written.  Work: chunks of samples_per_chunk samples on samples_per_chunk*R rows (sample-major);
+ * per chunk one launch expanding the inputs, the forward at x and one launch taking the clean logits and target, then
+ * per round one start launch and the steps (frozen-parameter backward, dX0 GEMM, one step launch, forward, one track
+ * launch), and one bisection launch.  Per-row and per-sample kernels are one CTA each with fixed-order fp64 sums (no
+ * atomics): bitwise independent of the chunking once dims->obprop_mode is pinned (mode 0 is resolved once from
+ * samples_per_chunk*R rows).  scratch: rd_counterfactual_scratch_bytes(dims, samples_per_chunk, n_restarts) bytes.
+ * Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+typedef struct rd_cf_options {
+  double kappa;          /* margin the target must win by, >= 0 */
+  double c_init;         /* the hinge's first loss weight, > 0 */
+  float beta;            /* L1 weight, >= 0 */
+  float step_size;       /* FISTA step alpha, > 0 */
+  float init_scale;      /* half-width of the restarts' uniform start, >= 0 */
+  int32_t n_search;      /* bisection rounds, >= 1 */
+  int32_t n_steps;       /* FISTA steps per round, >= 0 */
+  int32_t n_restarts;    /* replicas per sample, >= 1 */
+  int32_t perturb_static;
+} rd_cf_options;
+size_t rd_counterfactual_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk, int32_t n_restarts);
+int rd_raindrop_v2_counterfactual(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                  const float* times, const int64_t* lengths, const float* node_scale,
+                                  const int64_t* target, const uint8_t* sensor_mutable, const float* weights,
+                                  const float* lower, const float* upper, const rd_cf_options* opt, const uint64_t* rng,
+                                  int32_t samples_per_chunk, void* scratch, float* src_cf, float* statics_cf,
+                                  float* logits_cf, float* logits_clean, int64_t* target_out, uint8_t* valid,
+                                  double* distance, double* c_final, uint8_t* round_valid, void* stream);
+
 /* ---- randomized smoothing of Raindrop_v2: Monte Carlo class votes, in one call --------------------------------------
  * The smoothed classifier g(x) = argmax_c P(f(x + sigma z) = c) (Cohen, Rosenfeld & Kolter 2019) of the eval-mode model
  * f, estimated by counting the argmax classes of n_samples noisy replicates of every sample.

@@ -203,6 +203,39 @@ int pgd_track(const PgdArgs& a, int ncls, const float* logits, const float* logi
 int pgd_step(const PgdArgs& a, int norm, float eps, float alpha, const float* R_u, int d_ob, const float* dX0,
              const float* dfeat, int Df, int D, const float* W_emb, int emb, cudaStream_t st);
 
+// ---- counterfactual explanations (rd_counterfactual.cu; rd_raindrop_v2_counterfactual) -----------------------------
+// A chunk of m samples c0 .. c0+m-1 of a B-sample batch on m*R rows, sample-major (row j = i*R + r: replica r of chunk
+// sample i): the chunk's input buffers x_e [T, m*R, 2N], st_e [m*R, ds] (ds = 0: NULL), times_e [T, m*R], len_e [m*R],
+// the deltas of the FISTA iterates x_k and y_k, xd and yd [m*R, T*N + ds], the per-row state row [m*R, CF_ROW] (fp64)
+// and the per-sample best distance best [m].  sens [N] (uint8, NULL = all) and pst (the statics too) select the mutable
+// elements; w, lo, hi [N + ds] (NULL: 1, -inf, +inf) are the per-sensor / per-static-column weights and bounds.
+constexpr uint32_t SITE_CF_START = 103;     // Philox site of the restarts' start points (key {seed, step})
+enum CfRow { CF_C, CF_LO, CF_HI, CF_DIST, CF_FLAG, CF_ROW };   // c, bisection bounds, distance of y, round found valid
+struct CfArgs {
+  const float* src; const float* statics; const float* times; const int64_t* lengths;
+  const uint8_t* sens; const float* w; const float* lo; const float* hi;
+  float* x_e; float* st_e; float* times_e; int64_t* len_e; float* xd; float* yd; double* row; double* best;
+  int B, T, N, ds, m, c0, R, pst;
+};
+// the chunk's logits [m*R, ncls] and the batch-wide outputs (st_cf may be NULL)
+struct CfOut {
+  const float* logits; float* logits_clean; float* logits_cf; float* src_cf; float* st_cf; int64_t* target_out;
+  uint8_t* valid; double* distance; int ncls;
+};
+// every row a copy of its sample's inputs
+int cf_expand(const CfArgs& a, cudaStream_t st);
+// after the forward at x: clean logits, target (NULL: the runner-up), the outputs of "no valid point", c = c_init
+int cf_init(const CfArgs& a, const CfOut& k, const int64_t* target, double c_init, cudaStream_t st);
+// each row at its start point (key {seed, step}: device uint64[2], read for replicas r >= 1), its distance, flag cleared
+int cf_start(const CfArgs& a, float init_scale, float beta, const uint64_t* key, cudaStream_t st);
+// margins, hinge seeds d_logits [m*R, ncls], validity, and the best point per sample copied out
+int cf_track(const CfArgs& a, const CfOut& k, double kappa, float* dlogits, cudaStream_t st);
+// FISTA step k from dX0 [m*R*N, T*d_ob] and dfeat [m*R, Df] (statics gradient from columns D .. D+emb through W_emb)
+int cf_step(const CfArgs& a, int k, float alpha, float beta, const float* R_u, int d_ob, const float* dX0,
+            const float* dfeat, int Df, int D, const float* W_emb, int emb, cudaStream_t st);
+// the bisection after round `round`; round_valid [B, R, n_search] (uint8), c_final [B, R]
+int cf_round(const CfArgs& a, int round, int n_search, uint8_t* round_valid, double* c_final, cudaStream_t st);
+
 // ---- randomized smoothing (rd_smoothing.cu; rd_raindrop_v2_smooth_counts) -------------------------------------------
 constexpr uint32_t SITE_SMOOTH = 100;       // Philox site of the smoothing noise (its key is {seed, step + replicate})
 // smooth_expand: replicates m0 .. m0+nc-1 of the batch as mc_expand lays them out, with x + sigma z on the perturbable

@@ -392,6 +392,20 @@ int pgd_scratch(const rd_dims* dims, int spc, PgdScratch* l) {
   return 0;
 }
 
+// Counterfactuals: chunks of spc samples on spc*R rows with a backward, the deltas of x_k and y_k [spc*R, T*N + ds], the
+// per-row state [spc*R, CF_ROW] and the per-sample best distances (fp64).
+struct CfScratch : ChunkLayout { int64_t xd, yd, row, best; };
+int cf_scratch(const rd_dims* dims, int spc, int R, CfScratch* l) {
+  if (R < 1) { set_error("n_restarts = %d must be >= 1", R); return -2; }
+  RD_TRY(chunk_layout(dims, "samples_per_chunk", spc, R, false, 0, true, l));
+  const int64_t rows = (int64_t)spc * R, E = (int64_t)dims->T * dims->N + dims->d_static;
+  l->xd = l->a.take(rows * E);
+  l->yd = l->a.take(rows * E);
+  l->row = l->a.take(2 * rows * CF_ROW);
+  l->best = l->a.take(2LL * spc);
+  return 0;
+}
+
 // Coalition attribution (Shapley-value sampling, ablation, KernelSHAP): chunks of cc coalitions (B*cc rows), the
 // endpoint forward on 2B rows, the fp64 running sums [B, P] and the chunk's keep table [cc, P] (uint8, Shapley).
 struct CoalScratch : ChunkLayout { int64_t acc, keep; };
@@ -1311,6 +1325,90 @@ int rd_raindrop_v2_pgd(const rd_dims* dims, const rd_params* params, const float
       RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, lg, nullptr,
                           nullptr, nullptr, 0, st));
       cur = lg;
+    }
+  }
+  return 0;
+}
+
+size_t rd_counterfactual_scratch_bytes(const rd_dims* dims, int32_t samples_per_chunk, int32_t n_restarts) {
+  CfScratch l;
+  if (!dims || cf_scratch(dims, samples_per_chunk, n_restarts, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+int rd_raindrop_v2_counterfactual(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                  const float* times, const int64_t* lengths, const float* node_scale,
+                                  const int64_t* target, const uint8_t* sensor_mutable, const float* weights,
+                                  const float* lower, const float* upper, const rd_cf_options* opt, const uint64_t* rng,
+                                  int32_t samples_per_chunk, void* scratch, float* src_cf, float* statics_cf,
+                                  float* logits_cf, float* logits_clean, int64_t* target_out, uint8_t* valid,
+                                  double* distance, double* c_final, uint8_t* round_valid, void* stream) {
+  const char* fn = "rd_raindrop_v2_counterfactual";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !opt || !scratch || !src_cf || !logits_cf || !logits_clean || !target_out || !valid || !distance ||
+      !c_final || !round_valid || !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  const rd_cf_options o = *opt;
+  if (o.n_search < 1 || o.n_steps < 0 || o.n_restarts < 1) {
+    set_error("%s: n_search and n_restarts must be >= 1, n_steps >= 0 (%d, %d, %d)", fn, o.n_search, o.n_restarts,
+              o.n_steps);
+    return -2;
+  }
+  if (!(o.kappa >= 0.0) || isinf(o.kappa) || !(o.c_init > 0.0) || isinf(o.c_init) || !(o.beta >= 0.f) || isinf(o.beta) ||
+      !(o.step_size > 0.f) || isinf(o.step_size) || !(o.init_scale >= 0.f) || isinf(o.init_scale)) {
+    set_error("%s: kappa, beta and init_scale must be finite and >= 0, c_init and step_size finite and > 0 (kappa = %g, "
+              "c_init = %g, beta = %g, step_size = %g, init_scale = %g)", fn, o.kappa, o.c_init, o.beta, o.step_size,
+              o.init_scale);
+    return -2;
+  }
+  if (s0.ncls < 2) { set_error("%s: a counterfactual needs n_classes >= 2", fn); return -2; }
+  if (o.n_restarts > 1 && !rng) { set_error("%s: n_restarts > 1 needs rng", fn); return -2; }
+  if (o.perturb_static && s0.ds == 0) { set_error("%s: perturb_static needs a static branch (d_static > 0)", fn); return -2; }
+  const int B = s0.B, spc = samples_per_chunk, R = o.n_restarts;
+  CfScratch l;
+  RD_TRY(cf_scratch(dims, spc, R, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  float* S = (float*)scratch;
+  float* lg = S + l.logits;
+  const Expanded x = l.inputs(S, s0.ds);
+  CfArgs a;
+  a.src = src; a.statics = s0.ds > 0 ? statics : nullptr; a.times = times; a.lengths = lengths;
+  a.sens = sensor_mutable; a.w = weights; a.lo = lower; a.hi = upper;
+  a.x_e = x.src; a.st_e = x.statics; a.times_e = x.times; a.len_e = x.lengths; a.xd = S + l.xd; a.yd = S + l.yd;
+  a.row = reinterpret_cast<double*>(S + l.row); a.best = reinterpret_cast<double*>(S + l.best);
+  a.B = B; a.T = s0.T; a.N = s0.N; a.ds = s0.ds; a.R = R; a.pst = o.perturb_static ? 1 : 0;
+  CfOut k;
+  k.logits = lg; k.logits_clean = logits_clean; k.logits_cf = logits_cf; k.src_cf = src_cf;
+  k.st_cf = s0.ds > 0 ? statics_cf : nullptr; k.target_out = target_out; k.valid = valid; k.distance = distance;
+  k.ncls = s0.ncls;
+  // W1^T with its remainder, once per call
+  if (o.n_steps > 0) RD_TRY(prepare_w1t(s0, params, S + l.W1t, S + l.W1tlo, st));
+  for (int c0 = 0; c0 < B; c0 += spc) {
+    const int m = B - c0 < spc ? B - c0 : spc;
+    const rd_dims dc = chunk_dims(dims, m * R, (int64_t)spc * R, 0);
+    Shape s;
+    RD_TRY(make_shape(&dc, &s));
+    const float* dfeat = S + l.sc + bw_layout(s).dfeat;
+    a.m = m; a.c0 = c0;
+    RD_TRY(cf_expand(a, st));
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, lg, nullptr,
+                        nullptr, nullptr, 0, st));
+    RD_TRY(cf_init(a, k, target, o.c_init, st));
+    for (int round = 0; round < o.n_search; ++round) {
+      RD_TRY(cf_start(a, o.init_scale, o.beta, rng, st));
+      for (int step = 0;; ++step) {
+        RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, lg, nullptr,
+                            nullptr, nullptr, 0, st));
+        RD_TRY(cf_track(a, k, o.kappa, S + l.dlogits, st));
+        if (step == o.n_steps) break;
+        RD_TRY(chunk_input_grad(&dc, s, params, x, node_scale, S, l, st));
+        RD_TRY(cf_step(a, step, o.step_size, o.beta, params->R_u, s.dob, S + l.dX0, dfeat, s.Df, s.D, params->emb_weight,
+                       s.emb, st));
+      }
+      RD_TRY(cf_round(a, round, o.n_search, round_valid, c_final, st));
     }
   }
   return 0;

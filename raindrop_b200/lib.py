@@ -76,6 +76,12 @@ class RdSwagMember(C.Structure):
     _fields_ = [("mean", C.c_void_p), ("sq_mean", C.c_void_p), ("dev", C.c_void_p), ("k", C.c_int32)]
 
 
+class RdCfOptions(C.Structure):
+    _fields_ = [("kappa", C.c_double), ("c_init", C.c_double), ("beta", C.c_float), ("step_size", C.c_float),
+                ("init_scale", C.c_float), ("n_search", C.c_int32), ("n_steps", C.c_int32), ("n_restarts", C.c_int32),
+                ("perturb_static", C.c_int32)]
+
+
 class RdDebugTcNtArgs(C.Structure):
     _fields_ = ([(f, C.c_void_p) for f in ("A", "B", "B_lo", "C", "bias", "scale", "gate", "rng", "drop_mask", "resid")] +
                 [(f, C.c_int64) for f in ("lda", "M", "gate_ld", "resid_ld")] +
@@ -146,6 +152,9 @@ SIGNATURES = {
     "rd_raindrop_v2_pgd": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 8 +
                            [C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_int32] +
                            [C.c_void_p] * 7),
+    "rd_counterfactual_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32, C.c_int32]),
+    "rd_raindrop_v2_counterfactual": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 10 +
+                                      [C.POINTER(RdCfOptions), C.c_void_p, C.c_int32] + [C.c_void_p] * 11),
     "rd_smooth_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
     "rd_raindrop_v2_smooth_counts": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 6 +
                                      [C.c_int32, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,

@@ -1088,6 +1088,28 @@ int rd_debug_split_weights(const float* w, int32_t rows, int32_t cols, float* lo
  * scratch: ceil(rows / 32) * cols floats. */
 int rd_debug_colsum(const float* x, int64_t rows, int32_t cols, int64_t ld, float* out, float* scratch, void* stream);
 
+/* ---- the weight-gradient launch on its own (debug: operator-level tests) ----------------------------------------------
+ * One grouped weight-gradient launch exactly as the training backward issues it: one tc_wgrad_kernel launch over the
+ * n <= 12 problems (none when n = 0) and one reduce launch that sums their row splits and the ncs <= 36 column sums.
+ * items[i].d_bias may be NULL (no bias gradient); partial_bytes[i] is the size of items[i].partial, which must be at
+ * least rd_linear_wgrad_partial_bytes(rows, out_features, in_features) and 16-byte aligned.  A problem the tensor-core
+ * kernel does not take (out_features or in_features not a multiple of 4 or below 16, d_out / x not 16-byte aligned, or
+ * the tensor-core path switched off with RD_TC_WGRAD=0) is refused: there is no CUDA-core fallback here.
+ * RD_TC_WGRAD_BN=<width> forces the tile width as it does for every grouped launch. */
+typedef struct rd_debug_colsum_item {          /* out[c] = sum_{s < nsplit} partial[s*stride + c], c < ncols */
+  const float* partial; float* out;
+  int64_t stride;
+  int32_t nsplit, ncols;
+} rd_debug_colsum_item;
+/* The plan the launch ran: the tile width (0 when n = 0), the group's rows target, and per problem in the caller's
+ * order the row split count and the rows per split (a multiple of 32; the last split holds the remainder). */
+typedef struct rd_debug_wgrad_plan {
+  int32_t BN, rows_target;
+  int32_t nsplit[12], rows_per_split[12];
+} rd_debug_wgrad_plan;
+int rd_debug_wgrad_group(const rd_wgrad_item* items, const uint64_t* partial_bytes, int32_t n,
+                         const rd_debug_colsum_item* cs, int32_t ncs, rd_debug_wgrad_plan* plan, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

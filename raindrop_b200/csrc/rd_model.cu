@@ -2465,4 +2465,51 @@ int rd_debug_colsum(const float* x, int64_t rows, int32_t cols, int64_t ld, floa
   return colsum(x, rows, cols, ld, out, scratch, (cudaStream_t)stream);
 }
 
+int rd_debug_wgrad_group(const rd_wgrad_item* items, const uint64_t* partial_bytes, int32_t n,
+                         const rd_debug_colsum_item* cs, int32_t ncs, rd_debug_wgrad_plan* plan, void* stream) {
+  if (n < 0 || ncs < 0 || n > WG_MAX || ncs > CS_MAX) {
+    set_error("rd_debug_wgrad_group: at most %d problems and %d column sums per launch", WG_MAX, CS_MAX);
+    return -2;
+  }
+  if (!plan || (n > 0 && (!items || !partial_bytes)) || (ncs > 0 && !cs)) { set_error("rd_debug_wgrad_group: bad arguments"); return -2; }
+  WgradItem it[WG_MAX];
+  ColsumItem c[CS_MAX];
+  for (int i = 0; i < n; ++i) {
+    const rd_wgrad_item& a = items[i];
+    if (!a.d_out || !a.x || !a.d_weight || !a.partial || a.rows < 1) {
+      set_error("rd_debug_wgrad_group: problem %d has a NULL pointer or no rows", i);
+      return -2;
+    }
+    if (!tc_wgrad_supported(a.out_features, a.in_features, a.out_features, a.in_features, a.d_out, a.x) ||
+        (reinterpret_cast<uintptr_t>(a.partial) & 15)) {
+      set_error("rd_debug_wgrad_group: problem %d is not one the tensor-core kernel takes (out / in features multiples "
+                "of 4 and >= 16, d_out, x and partial 16-byte aligned)", i);
+      return -2;
+    }
+    const size_t need = rd_linear_wgrad_partial_bytes(a.rows, a.out_features, a.in_features);
+    if (partial_bytes[i] < need) {
+      set_error("rd_debug_wgrad_group: problem %d has a partial buffer of %llu bytes, it needs %llu", i,
+                (unsigned long long)partial_bytes[i], (unsigned long long)need);
+      return -2;
+    }
+    it[i] = WgradItem{a.d_out, a.out_features, a.x, a.in_features, a.rows, a.out_features, a.in_features, a.d_weight,
+                      a.d_bias, (float*)a.partial};
+  }
+  for (int i = 0; i < ncs; ++i) {
+    const rd_debug_colsum_item& s = cs[i];
+    if (!s.partial || !s.out || s.nsplit < 1 || s.ncols < 1 || (s.nsplit > 1 && s.stride < s.ncols)) {
+      set_error("rd_debug_wgrad_group: bad column sum %d", i);
+      return -2;
+    }
+    c[i] = ColsumItem{s.partial, s.stride, s.nsplit, s.ncols, s.out};
+  }
+  static_assert(WG_MAX == 12 && CS_MAX == 36, "the limits rd_debug_wgrad_group and its plan are declared with");
+  WgradPlan pl{};
+  RD_TRY(tc_wgrad_group(it, n, c, ncs, (cudaStream_t)stream, &pl));
+  plan->BN = pl.BN;
+  plan->rows_target = pl.rows_target;
+  for (int i = 0; i < n; ++i) { plan->nsplit[i] = pl.sp[i].nsplit; plan->rows_per_split[i] = pl.sp[i].rows_per_split; }
+  return 0;
+}
+
 }  // extern "C"

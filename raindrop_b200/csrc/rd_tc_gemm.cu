@@ -716,7 +716,6 @@ static const int kWgWidths[] = {
 // ~512 rows (16 k-blocks) per item so the pipeline amortises its fill, but never more than ~2 rounds of items per
 // problem in 128 x 160 tiles (bounds the partial buffer for the big configurations).  512 sizes the partial buffers
 // (the CAPACITY in row splits); wgrad_rows_target may raise it for a group, which only lowers the split count.
-struct WSplit { int nsplit, rows_per_split, Nld; };
 WSplit wgrad_split(int M, int N, long long rows, int rows_target = 512) {
   WSplit w;
   w.Nld = (int)round_up(N + 1, 4);                          // + the ones column
@@ -1002,15 +1001,24 @@ long long tc_wgrad_partial_floats(int Nout, int Kin, long long rows) {
 static unsigned long long* g_wgrad_dbg = nullptr;
 void tc_wgrad_set_debug(unsigned long long* buf) { g_wgrad_dbg = buf; }
 
-int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st) {
+// The group's plan: one rows target, each problem's row split under it, one tile width
+static WgradPlan wgrad_plan(const WgradItem* items, int n) {
+  WgradPlan pl;
+  pl.rows_target = n > 0 ? wgrad_rows_target(items, n) : 512;
+  pl.BN = n > 0 ? wgrad_width(items, n) : 0;
+  for (int i = 0; i < n; ++i) pl.sp[i] = wgrad_split(items[i].Nout, items[i].Kin, items[i].rows, pl.rows_target);
+  return pl;
+}
+
+int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st, WgradPlan* plan) {
   if (n <= 0 && ncs <= 0) return 0;
   if (n > WG_MAX || ncs > CS_MAX) { set_error("tc_wgrad_group: at most %d problems (+ %d column sums) per launch", WG_MAX, CS_MAX); return -2; }
   WGroup g;
   RGroup r;
   g.n = n; r.n = n + (ncs > 0 ? ncs : 0);
   g.dbg = g_wgrad_dbg;
-  WSplit sp[WG_MAX];
-  const int target = n > 0 ? wgrad_rows_target(items, n) : 512;
+  const WgradPlan pl = wgrad_plan(items, n > 0 ? n : 0);
+  const WSplit* sp = pl.sp;
   int order[WG_MAX];
   long long tot = 0;
   for (int i = 0; i < n; ++i) {
@@ -1021,7 +1029,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
       return -2;
     }
     if (a.rows > 0x7fffffffLL) { set_error("tc_wgrad_group: too many rows"); return -2; }
-    const WSplit& w = sp[i] = wgrad_split(a.Nout, a.Kin, a.rows, target);
+    const WSplit& w = sp[i];
     order[i] = i;
     RItem& q = r.it[i];
     q.partial = a.partial; q.dW = a.dW; q.db = a.db; q.nsplit = w.nsplit; q.M = a.Nout; q.N = a.Kin; q.Mpad = a.Nout; q.Nld = w.Nld;
@@ -1029,7 +1037,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
     q.start = tot;
     tot += (long long)a.Nout * (a.Kin / 4 + 1);
   }
-  const int BN = n > 0 ? wgrad_width(items, n) : MAX_BN;
+  const int BN = pl.BN;
   // the persistent grid deals the items round robin: problems with the longest items (rows per split) go first
   for (int i = 1; i < n; ++i)
     for (int j = i; j > 0 && sp[order[j]].rows_per_split > sp[order[j - 1]].rows_per_split; --j) {
@@ -1057,7 +1065,6 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
     item += w.nsplit * p.m_tiles * p.n_tiles;
   }
   g.total_items = item;
-  const int smem_bytes = 1280 + w_nstages(BN) * w_stage_bytes(BN);
   for (int i = 0; i < ncs; ++i) {
     RItem& q = r.it[n + i];
     q.partial = cs[i].partial; q.dW = cs[i].out; q.db = nullptr; q.nsplit = cs[i].nsplit; q.M = 1; q.N = cs[i].ncols;
@@ -1068,6 +1075,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
   }
   r.total = tot;
   if (n > 0) {
+    const int smem_bytes = 1280 + w_nstages(BN) * w_stage_bytes(BN);
     const int grid = item < num_sms() ? item : num_sms();
     auto launch = [&](auto kern) -> int {
       RD_TRY(ensure_max_smem((const void*)kern, SMEM_LIMIT));
@@ -1086,6 +1094,7 @@ int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs,
   }
   launch_pdl(wgrad_reduce_kernel, dim3((unsigned)ceil_div(tot, 256)), dim3(256), 0, st, r);
   RD_CHECK_LAUNCH("wgrad_reduce_kernel");
+  if (plan) *plan = pl;
   return 0;
 }
 

@@ -67,7 +67,14 @@ struct WgradItem { const float* dY; long long ldy; const float* X; long long ldx
 // Column sums riding along in the group's reduction launch: out[c] = sum_{s < nsplit} partial[s*stride + c], c < ncols
 constexpr int CS_MAX = 36;
 struct ColsumItem { const float* partial; long long stride; int nsplit, ncols; float* out; };
-int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st);
+// The plan of one group: the tile width (0 when n = 0: no tensor-core launch), the rows target of its row splits and,
+// per problem in the caller's order, the split count and the rows per split (a multiple of 32; the last split may be
+// shorter).  Nld = N + 1 rounded up to 4 is the row stride of a problem's partial slabs.
+struct WSplit { int nsplit, rows_per_split, Nld; };
+struct WgradPlan { int BN, rows_target; WSplit sp[WG_MAX]; };
+// plan (optional): the plan the call ran, written back
+int tc_wgrad_group(const WgradItem* items, int n, const ColsumItem* cs, int ncs, cudaStream_t st,
+                   WgradPlan* plan = nullptr);
 void tc_wgrad_set_debug(unsigned long long* buf);    // per-CTA phase cycles [CTA][16] of tc_wgrad_kernel (debug)
 
 // One launch for all weights of a step: lo = W - trunc19(W); t = W^T; t_lo = W^T - trunc19(W^T).

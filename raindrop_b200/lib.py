@@ -100,6 +100,16 @@ class RdDebugGemmArgs(C.Structure):
                 [(f, C.c_int32) for f in ("rep_B", "rep_Bc", "perm", "pB", "pN", "pdob", "pD")])
 
 
+class RdDebugColsumItem(C.Structure):
+    _fields_ = [("partial", C.c_void_p), ("out", C.c_void_p), ("stride", C.c_int64), ("nsplit", C.c_int32),
+                ("ncols", C.c_int32)]
+
+
+class RdDebugWgradPlan(C.Structure):
+    _fields_ = [("BN", C.c_int32), ("rows_target", C.c_int32), ("nsplit", C.c_int32 * 12),
+                ("rows_per_split", C.c_int32 * 12)]
+
+
 # name -> (restype, argtypes); every symbol include/raindrop_b200.h declares
 SIGNATURES = {
     "rd_abi_version": (C.c_int, []),
@@ -236,6 +246,8 @@ SIGNATURES = {
     "rd_debug_gemm_f32": (C.c_int, [C.POINTER(RdDebugGemmArgs), C.c_void_p, C.c_void_p]),
     "rd_debug_split_weights": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 6),
     "rd_debug_colsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rd_debug_wgrad_group": (C.c_int, [C.POINTER(RdWgradItem), C.POINTER(C.c_uint64), C.c_int32,
+                                       C.POINTER(RdDebugColsumItem), C.c_int32, C.POINTER(RdDebugWgradPlan), C.c_void_p]),
     "rd_kfac_factors_doubles": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_ekfac_bases_floats": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_kfac_factors_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),

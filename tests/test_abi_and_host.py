@@ -40,6 +40,8 @@ def test_struct_layout_matches_header_sizes():
     # pointers, 64-bit fields, then 17 / 21 32-bit fields and 4 bytes of tail padding
     assert C.sizeof(L.RdDebugTcNtArgs) == 8 * 10 + 8 * 4 + 4 * 17 + 4
     assert C.sizeof(L.RdDebugGemmArgs) == 8 * 9 + 8 * 15 + 4 * 21 + 4
+    assert C.sizeof(L.RdDebugColsumItem) == 8 * 3 + 4 * 2
+    assert C.sizeof(L.RdDebugWgradPlan) == 4 * 2 + 4 * 24
 
 
 def test_workspace_queries_are_pure_host_code():

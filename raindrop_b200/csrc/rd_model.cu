@@ -125,14 +125,83 @@ WsLayout ws_layout(const Shape& s) {
   return w;
 }
 
+// ---- the trained tensors ------------------------------------------------------------------------------------------
+// Every trained tensor, in flat-bucket order (TrainStep's layout, used_param_fields in functional.py), each at a
+// 4-aligned offset: the head (emb when d_static > 0, mlp_static.0, mlp_static.2; dp_head_sqnorm_kernel and psg_head in
+// rd_dp.cu number these fields themselves, in this order), 12 per encoder layer (in_proj, out_proj, linear1, linear2,
+// norm1, norm2; weight then bias), the lin_value pairs of ob-prop layers 1 and 2.  A linear's bias field follows its
+// weight, and ord numbers the linears in the same order (the backward's partial buffer, the EK-FAC block).  Sample b's
+// R rows of a linear's operands are b*sstride + t*rstride, t < R; ob: the ob-prop phase queues it.  EK-FAC block:
+// offsets a, s (doubles) of A [(Kin + 1)^2] and S [Nout^2] in the factors, qs, qa, qb (floats) of Q_S^T [Nout, Nout],
+// Q_A[:Kin]^T [Np, Kin] and Q_A[Kin] [Np] in the bases, Np = Kin + 1 rounded up to 4 (rows past Kin + 1 are 0).
+enum Role { IN_PROJ, OUT_PROJ, LINEAR1, LINEAR2 };     // an encoder layer's linears, in bucket order
+struct Linear { int Nout, Kin, R, fw, ord, ob, Np; int64_t rows, sstride, rstride, a, s, qs, qa, qb; };
+struct Trained {
+  DpFields f;                          // bucket offset and size of every field
+  int64_t bucket;                      // the bucket length
+  float* grad[DP_MAX_FIELDS];          // each field's rd_grads member (NULL when built without one)
+  Linear lin[4 * RD_MAX_LAYERS + 2];   // lin[ord]
+  int nlin, L;
+  int norm1[RD_MAX_LAYERS], norm2[RD_MAX_LAYERS];   // weight fields of encoder layer l's LayerNorms
+  int64_t factor_doubles, base_floats;              // EK-FAC factors and bases of all blocks
+  const Linear& layer(int l, Role r) const { return lin[4 * l + r]; }
+  const Linear& obprop(int k) const { return lin[4 * L + k - 1]; }   // lin_value of ob-prop layer k = 1, 2
+};
+
+const rd_grads kNoGrads = {};
+
+Trained trained(const Shape& s, const rd_grads* G = nullptr) {
+  const rd_grads& g = G ? *G : kNoGrads;
+  Trained t;
+  t.f.n = 0; t.bucket = 0; t.nlin = 0; t.L = s.L; t.factor_doubles = 0; t.base_floats = 0;
+  auto field = [&](int64_t numel, float* grad) {
+    t.f.off[t.f.n] = t.bucket; t.f.numel[t.f.n] = numel; t.grad[t.f.n] = grad;
+    t.bucket += round_up(numel, 4);
+    return t.f.n++;
+  };
+  auto linear = [&](int Nout, int Kin, int ob, float* gw, float* gb) {
+    Linear& o = t.lin[t.nlin];
+    o.Nout = Nout; o.Kin = Kin; o.ord = t.nlin++; o.ob = ob;
+    o.R = ob ? s.N : s.T; o.sstride = ob ? s.N : 1; o.rstride = ob ? 1 : s.B; o.rows = (int64_t)s.B * o.R;
+    o.fw = field((int64_t)Nout * Kin, gw); field(Nout, gb);
+    o.Np = (int)round_up(Kin + 1, 4);     // each EK-FAC piece starts 4-aligned
+    o.a = t.factor_doubles; t.factor_doubles += (int64_t)(Kin + 1) * (Kin + 1);
+    o.s = t.factor_doubles; t.factor_doubles += (int64_t)Nout * Nout;
+    o.qs = t.base_floats; t.base_floats += round_up((int64_t)Nout * Nout, 4);
+    o.qa = t.base_floats; t.base_floats += (int64_t)o.Np * Kin;
+    o.qb = t.base_floats; t.base_floats += o.Np;
+  };
+  if (s.ds > 0) { field((int64_t)s.emb * s.ds, g.emb_weight); field(s.emb, g.emb_bias); }
+  field((int64_t)s.Df * s.Df, g.mlp0_weight); field(s.Df, g.mlp0_bias);
+  field((int64_t)s.ncls * s.Df, g.mlp2_weight); field(s.ncls, g.mlp2_bias);
+  for (int l = 0; l < s.L; ++l) {
+    const rd_encoder_layer_grads& e = g.layer[l];
+    linear(3 * s.D, s.D, 0, e.in_proj_weight, e.in_proj_bias);
+    linear(s.D, s.D, 0, e.out_proj_weight, e.out_proj_bias);
+    linear(s.nhid, s.D, 0, e.linear1_weight, e.linear1_bias);
+    linear(s.D, s.nhid, 0, e.linear2_weight, e.linear2_bias);
+    t.norm1[l] = field(s.D, e.norm1_weight); field(s.D, e.norm1_bias);
+    t.norm2[l] = field(s.D, e.norm2_weight); field(s.D, e.norm2_bias);
+  }
+  linear(s.C, s.C, 1, g.ob1_value_weight, g.ob1_value_bias);
+  linear(s.C, s.C, 1, g.ob2_value_weight, g.ob2_value_bias);
+  return t;
+}
+
+// the larger of the two backward phases' sums of cost(linear)
+template <class F> int64_t phase_max(const Trained& t, F cost) {
+  int64_t sum[2] = {0, 0};
+  for (int i = 0; i < t.nlin; ++i) sum[t.lin[i].ob] += cost(t.lin[i]);
+  return sum[0] > sum[1] ? sum[0] : sum[1];
+}
+
 // Backward scratch.  The weight gradients are DEFERRED: every linear layer's (dY, X) operand pair stays alive in
 // its own buffer until one grouped tensor-core launch (tc_wgrad_group) reduces them all, so dY buffers and the
 // split-K partial buffers are per layer / per problem instead of ping-pong.
 struct BwLayout {
   int64_t dfeat, dhpre, gA, gB, gD, dP, gO2, gO1, partial, total;
-  struct { int64_t K2, gF, K1, dqkv, wp[4], ln[2]; } l[RD_MAX_LAYERS];   // wp: linear2, linear1, out_proj, in_proj partials; ln: norm2, norm1
-  int64_t wp_ob[2];
-  int64_t partial_floats;
+  struct { int64_t K2, gF, K1, dqkv, ln[2]; } l[RD_MAX_LAYERS];   // ln: norm2, norm1
+  int64_t wp[4 * RD_MAX_LAYERS + 2];   // tensor-core partial buffer of each linear, by ord
 };
 
 int64_t splitk_partial_floats(int Nout, int Kin, int64_t rows) {
@@ -141,8 +210,10 @@ int64_t splitk_partial_floats(int Nout, int Kin, int64_t rows) {
 }
 
 BwLayout bw_layout(const Shape& s) {
+  const Trained t = trained(s);
   BwLayout b;
   Arena a;
+  auto wp = [&](const Linear& o) { b.wp[o.ord] = a.take(tc_wgrad_partial_floats(o.Nout, o.Kin, o.rows)); };
   b.dfeat = a.take((int64_t)s.B * s.Df);
   b.dhpre = a.take((int64_t)s.B * s.Df);
   b.gA = a.take(s.M2 * s.D);
@@ -154,145 +225,25 @@ BwLayout bw_layout(const Shape& s) {
     b.l[l].gF = a.take(s.M2 * s.nhid);
     b.l[l].K1 = a.take(s.M2 * s.D);
     b.l[l].dqkv = a.take(s.M2 * 3 * s.D);
-    b.l[l].wp[0] = a.take(tc_wgrad_partial_floats(s.D, s.nhid, s.M2));
-    b.l[l].wp[1] = a.take(tc_wgrad_partial_floats(s.nhid, s.D, s.M2));
-    b.l[l].wp[2] = a.take(tc_wgrad_partial_floats(s.D, s.D, s.M2));
-    b.l[l].wp[3] = a.take(tc_wgrad_partial_floats(3 * s.D, s.D, s.M2));
+    wp(t.layer(l, LINEAR2)); wp(t.layer(l, LINEAR1)); wp(t.layer(l, OUT_PROJ)); wp(t.layer(l, IN_PROJ));
     b.l[l].ln[0] = a.take(ln_bwd_scratch_floats(s.M2, s.D));      // per-CTA dgamma/dbeta partial rows, reduced with the group
     b.l[l].ln[1] = a.take(ln_bwd_scratch_floats(s.M2, s.D));
   }
   b.gO2 = a.take(s.M1 * s.C);
   b.gO1 = a.take(s.M1 * s.C);
-  b.wp_ob[0] = a.take(tc_wgrad_partial_floats(s.C, s.C, s.M1));
-  b.wp_ob[1] = a.take(tc_wgrad_partial_floats(s.C, s.C, s.M1));
+  wp(t.obprop(2)); wp(t.obprop(1));
   // shared split-K scratch of the CUDA-core fallback (shapes the tensor-core kernel does not take)
   int64_t pf = 0;
-  auto upd = [&](int no, int ki, int64_t rows) { int64_t v = splitk_partial_floats(no, ki, rows); if (v > pf) pf = v; };
-  upd(s.C, s.C, s.M1);
-  upd(3 * s.D, s.D, s.M2); upd(s.D, s.D, s.M2); upd(s.nhid, s.D, s.M2); upd(s.D, s.nhid, s.M2);
-  b.partial_floats = pf;
+  for (int i = 0; i < t.nlin; ++i) { const int64_t v = splitk_partial_floats(t.lin[i].Nout, t.lin[i].Kin, t.lin[i].rows); if (v > pf) pf = v; }
   b.partial = a.take(pf);
   b.total = a.off;
   return b;
 }
 
-// ---- DP-SGD per-sample norm pass -----------------------------------------------------------------------------------
-// Trained tensors, in used_param_fields order: the head (emb weight / bias when d_static > 0, mlp_static.0, mlp_static.2),
-// 12 per encoder layer, the two lin_value pairs.
-int dp_head_fields(const Shape& s) { return s.ds > 0 ? 6 : 4; }
-int dp_n_fields(const Shape& s) { return dp_head_fields(s) + 12 * s.L + 4; }
-
-// Field table of the flat gradient bucket (TrainStep's layout): each trained tensor at a 4-aligned offset, in the order
-// above.  Returns the bucket length.
-int64_t bucket_fields(const Shape& s, DpFields* f) {
-  int64_t n[DP_MAX_FIELDS];
-  int k = 0;
-  if (s.ds > 0) { n[k++] = (int64_t)s.emb * s.ds; n[k++] = s.emb; }
-  n[k++] = (int64_t)s.Df * s.Df; n[k++] = s.Df; n[k++] = (int64_t)s.ncls * s.Df; n[k++] = s.ncls;
-  for (int l = 0; l < s.L; ++l) {
-    const int64_t D = s.D, H = s.nhid;
-    const int64_t v[12] = {3 * D * D, 3 * D, D * D, D, H * D, H, D * H, D, D, D, D, D};
-    for (int i = 0; i < 12; ++i) n[k++] = v[i];
-  }
-  for (int i = 0; i < 2; ++i) { n[k++] = (int64_t)s.C * s.C; n[k++] = s.C; }
-  int64_t off = 0;
-  for (int i = 0; i < k; ++i) { f->off[i] = off; f->numel[i] = n[i]; off += round_up(n[i], 4); }
-  f->n = k;
-  return off;
-}
-
-// EK-FAC blocks: one per queued linear layer, in bucket order (per encoder layer in_proj, out_proj, linear1, linear2;
-// then lin_value of ob-prop layers 1 and 2).  a, s: offsets (doubles) of A [(Kin + 1)^2] and S [Nout^2] in the caller's
-// factors; qs, qa, qb: offsets (floats) of Q_S^T [Nout, Nout], Q_A[:Kin]^T [Np, Kin] and Q_A[Kin] [Np] in the caller's
-// bases, Np = Kin + 1 rounded up to 4 (rows past Kin + 1 are 0); each piece starts 4-aligned.
-struct KfacBlock { int Nout, Kin, Np; int64_t a, s, qs, qa, qb; };
-struct KfacBlocks { KfacBlock b[4 * RD_MAX_LAYERS + 2]; int n; int64_t factor_doubles, base_floats; };
-KfacBlocks kfac_blocks(const Shape& s) {
-  KfacBlocks k;
-  k.n = 0;
-  int64_t a = 0, q = 0;
-  auto add = [&](int Nout, int Kin) {
-    KfacBlock& o = k.b[k.n++];
-    o.Nout = Nout; o.Kin = Kin; o.Np = (int)round_up(Kin + 1, 4);
-    o.a = a; a += (int64_t)(Kin + 1) * (Kin + 1);
-    o.s = a; a += (int64_t)Nout * Nout;
-    o.qs = q; q += round_up((int64_t)Nout * Nout, 4);
-    o.qa = q; q += (int64_t)o.Np * Kin;
-    o.qb = q; q += o.Np;
-  };
-  for (int l = 0; l < s.L; ++l) { add(3 * s.D, s.D); add(s.D, s.D); add(s.nhid, s.D); add(s.D, s.nhid); }
-  add(s.C, s.C); add(s.C, s.C);
-  k.factor_doubles = a; k.base_floats = q;
-  return k;
-}
-// the block of the weight field fw (a queued item's)
-int kfac_block_of(const Shape& s, int fw) {
-  const int f = fw - dp_head_fields(s);
-  return f < 12 * s.L ? 4 * (f / 12) + (f % 12) / 2 : 4 * s.L + (f - 12 * s.L) / 2;
-}
-
-// Per-sample items of one backward phase, queued where the training path queues the weight-gradient items of the same
-// (dY, X) pairs, and flushed as one group launch.  Modes: squared norms into `sqnorms` (dp_norm_group; the partial
-// sums of a phase start at `partial` again: the previous phase's launches have completed by then, stream order); with
-// G set, the per-sample gradient rows themselves (psg_group), scaled by `scale`, and with `bases` also set, the EK-FAC
-// rows: each item's operands rotated into `rot` first (kfac_flush); with `factors` set, the EK-FAC factor sums of
-// every item (kfac_flush).
-struct DpQueue;
-int kfac_flush(DpQueue& q, cudaStream_t st);
-struct DpQueue {
-  DpNormGroup g;
-  PsgGroup pg;
-  long long blk = 0;
-  int B = 0, nf = 0;
-  double* sqnorms = nullptr; double* partial = nullptr;
-  float* G = nullptr; long long ldg = 0; float scale = 1.f; DpFields fields;     // rows mode
-  const Shape* shape = nullptr; const KfacBlocks* kb = nullptr; int blk_of[DP_MAX_ITEMS];   // EK-FAC modes
-  const float* bases = nullptr; const float* bases_lo = nullptr; float* rot = nullptr;     // rotated rows
-  double* factors = nullptr; float* kws = nullptr; float* kpartial = nullptr;             // factors
-  DpQueue() { g.n = 0; pg.n = 0; }
-  void add(const float* Y, int64_t ldy, const float* X, int64_t ldx, int Nout, int Kin, int R, int64_t sstride,
-           int64_t rstride, int fw) {
-    if (G || factors) {
-      if (kb) blk_of[pg.n] = kfac_block_of(*shape, fw);
-      PsgItem& o = pg.it[pg.n++];
-      o.Y = Y; o.X = X; o.ldy = ldy; o.ldx = ldx; o.sstride = sstride; o.rstride = rstride; o.blk0 = blk;
-      o.gw = G ? fields.off[fw] : 0; o.gb = G ? fields.off[fw + 1] : 0;
-      o.Nout = Nout; o.Kin = Kin; o.R = R; o.ntiles = psg_tiles(Nout, Kin, &o.tn);
-      blk += (long long)B * o.ntiles;
-      return;
-    }
-    DpNormItem& o = g.it[g.n++];
-    o.Y = Y; o.X = X; o.ldy = ldy; o.ldx = ldx; o.sstride = sstride; o.rstride = rstride; o.blk0 = blk;
-    o.Nout = Nout; o.Kin = Kin; o.R = R; o.ghost = dp_ghost(R, Nout, Kin) ? 1 : 0;
-    o.ntiles = dp_norm_tiles(R, Nout, Kin, &o.tm, &o.tn);
-    o.fw = fw; o.fb = fw + 1;
-    blk += (long long)B * o.ntiles;
-  }
-  int ln(const float* x, const float* stats, const float* dy, int T, int D, int fw, int fb, cudaStream_t st) {
-    if (factors) return 0;
-    if (G) return psg_ln(x, stats, dy, T, B, D, G, ldg, fields.off[fw], fields.off[fb], scale, st);
-    return dp_ln_sqnorm(x, stats, dy, T, B, D, sqnorms, nf, fw, fb, st);
-  }
-  int head(const Shape& s, const float* dlogits, const float* hpre, const float* dh, const float* feat, const float* dfeat,
-           const float* statics, cudaStream_t st) {
-    if (factors) return 0;
-    if (G) return psg_head(B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dh, feat, dfeat, statics, G, ldg, fields.off, scale, st);
-    return dp_head_sqnorm(B, s.D, s.Df, s.ds, s.ncls, dlogits, hpre, dh, feat, dfeat, statics, sqnorms, nf, st);
-  }
-  int flush(cudaStream_t st) {
-    int rc = kb ? kfac_flush(*this, st) : G ? psg_group(pg, B, G, ldg, scale, st) : dp_norm_group(g, B, partial, sqnorms, nf, st);
-    g.n = 0; pg.n = 0; blk = 0;
-    return rc;
-  }
-};
-
 // CTAs (= partial pairs) of the larger of the two phases' group launches
 int64_t dp_partial_blocks(const Shape& s) {
   int tm, tn;
-  int64_t enc = (int64_t)s.L * (dp_norm_tiles(s.T, s.D, s.nhid, &tm, &tn) + dp_norm_tiles(s.T, s.nhid, s.D, &tm, &tn) +
-                                dp_norm_tiles(s.T, s.D, s.D, &tm, &tn) + dp_norm_tiles(s.T, 3 * s.D, s.D, &tm, &tn));
-  int64_t ob = 2LL * dp_norm_tiles(s.N, s.C, s.C, &tm, &tn);
-  return (int64_t)s.B * (enc > ob ? enc : ob);
+  return (int64_t)s.B * phase_max(trained(s), [&](const Linear& o) { return (int64_t)dp_norm_tiles(o.R, o.Nout, o.Kin, &tm, &tn); });
 }
 
 // Scratch of rd_raindrop_v2_per_sample_grad_sqnorms: the backward scratch of the data-gradient chain, then the partial
@@ -510,75 +461,153 @@ static bool linear_nt_is_tc(const GemmP& g, const float* W_lo) {
   return W_lo && tc_gemm_supported(a);
 }
 
-// ---- EK-FAC: the factor pass and the rotated rows (DpQueue's kfac modes) ------------------------------------------
+// ---- the backward's gradient consumer ------------------------------------------------------------------------------
 namespace {
-// Factors: per item, dW = X^T X with db = column sums of X, and dW = dY^T dY (tn: queued for one grouped tensor-core
-// launch when the shape fits, else CUDA cores), then each block's sums are added into the fp64 factors (dY carries
-// the gradient of l_b / B, so S is scaled by B^2).  Rotated rows: Y^ = dY Q_S and X^ = [X | 1] Q_A on the error-compensated
-// tensor-core GEMM (linear_nt, bias = the last row of Q_A), then psg_group on the rotated operands without a ones column.
-int kfac_flush(DpQueue& q, cudaStream_t st) {
-  if (q.pg.n == 0) return 0;
-  const KfacBlocks& K = *q.kb;
-  if (q.factors) {
-    WgradQueue wq;
+// raindrop_bwd hands each linear's (dY, X) operand pair, each LayerNorm and the head to one consumer, whose mode says
+// what becomes of them: NONE nothing (the data-gradient chain alone: frozen parameters); WEIGHTS the weight gradients
+// into `grads`, items of one grouped tensor-core launch (tn, WgradQueue; head_bwd writes the head's); SQNORMS DP-SGD's
+// per-sample squared norms; ROWS TracIn's per-sample gradient rows into G, times `scale`; ROTATED the EK-FAC rows, each
+// linear's operands rotated into the bases first; FACTORS the EK-FAC factor sums (none from LayerNorms and the head).
+// The per-sample modes flush a phase's linears as one group launch at the end of every phase, which lays its buffers
+// (`partial`, `kws`, `rot`) out from their start again: the previous phase's launches have completed (stream order).
+enum GradMode { GRAD_NONE, GRAD_WEIGHTS, GRAD_SQNORMS, GRAD_ROWS, GRAD_ROTATED, GRAD_FACTORS };
+struct GradConsumer {
+  GradMode mode = GRAD_NONE;
+  const rd_grads* grads = nullptr;                                                      // WEIGHTS
+  double* sqnorms = nullptr; double* partial = nullptr;                                 // SQNORMS
+  float* G = nullptr; float scale = 1.f;                                                // ROWS, ROTATED (ldg = the bucket length)
+  const float* bases = nullptr; const float* bases_lo = nullptr; float* rot = nullptr;  // ROTATED
+  double* factors = nullptr; float* kws = nullptr; float* kpartial = nullptr;           // FACTORS
+  // set by raindrop_bwd: the shape, its trained tensors (built with `grads`) and the backward scratch
+  const Shape* s = nullptr; const Trained* t = nullptr; const BwLayout* b = nullptr; float* sc = nullptr;
+  WgradQueue wq;
+  struct Item { const Linear* o; const float* Y; const float* X; } it[DP_MAX_ITEMS];   // a per-sample mode's phase
+  int n = 0;
+
+  int linear(const Linear& o, const float* Y, const float* X, cudaStream_t st) {
+    if (mode == GRAD_WEIGHTS)
+      return tn(&wq, Y, o.Nout, X, o.Kin, t->grad[o.fw], t->grad[o.fw + 1], o.Nout, o.Kin, o.rows, sc + b->wp[o.ord], sc + b->partial, st);
+    if (mode != GRAD_NONE) it[n++] = Item{&o, Y, X};
+    return 0;
+  }
+
+  // LayerNorm with weight field fw over the T*B rows of its input x, stats {mean, rstd} and output gradient dy; part:
+  // layernorm_bwd's deferred per-CTA partial rows [chunks][2][D]
+  int ln(int fw, const float* part, int chunks, const float* x, const float* stats, const float* dy, cudaStream_t st) {
+    const int D = s->D;
+    if (mode == GRAD_WEIGHTS) {
+      RD_TRY(wq.colsum(part, 2 * D, chunks, D, t->grad[fw], st));
+      return wq.colsum(part + D, 2 * D, chunks, D, t->grad[fw + 1], st);
+    }
+    if (mode == GRAD_SQNORMS) return dp_ln_sqnorm(x, stats, dy, s->T, s->B, D, sqnorms, t->f.n, fw, fw + 1, st);
+    if (mode != GRAD_ROWS && mode != GRAD_ROTATED) return 0;
+    return psg_ln(x, stats, dy, s->T, s->B, D, G, t->bucket, t->f.off[fw], t->f.off[fw + 1], scale, st);
+  }
+
+  int head(const float* dlogits, const float* hpre, const float* dh, const float* feat, const float* dfeat,
+           const float* statics, cudaStream_t st) {
+    const Shape& z = *s;
+    if (mode == GRAD_SQNORMS)
+      return dp_head_sqnorm(z.B, z.D, z.Df, z.ds, z.ncls, dlogits, hpre, dh, feat, dfeat, statics, sqnorms, t->f.n, st);
+    if (mode != GRAD_ROWS && mode != GRAD_ROTATED) return 0;
+    return psg_head(z.B, z.D, z.Df, z.ds, z.ncls, dlogits, hpre, dh, feat, dfeat, statics, G, t->bucket, t->f.off, scale, st);
+  }
+
+  // The end of a backward phase.  Weights mode keeps its items when the ob-prop phase follows, so that the encoder's
+  // last items share the ob-prop items' group launch.
+  int flush(bool obprop_follows, cudaStream_t st) {
+    if (mode == GRAD_WEIGHTS) return obprop_follows ? 0 : wq.flush(st);
+    const int rc = n == 0 ? 0 : mode == GRAD_SQNORMS ? sqnorm_group(st) : mode == GRAD_FACTORS ? factor_sums(st) : row_group(st);
+    n = 0;
+    return rc;
+  }
+
+  // every queued linear's per-sample squared norms: one dp_norm_group launch pair (B * ntiles CTAs per item, in order)
+  int sqnorm_group(cudaStream_t st) {
+    DpNormGroup g;
+    long long blk = 0;
+    for (g.n = 0; g.n < n; ++g.n) {
+      const Linear& o = *it[g.n].o;
+      DpNormItem& q = g.it[g.n];
+      q.Y = it[g.n].Y; q.X = it[g.n].X; q.ldy = o.Nout; q.ldx = o.Kin; q.sstride = o.sstride; q.rstride = o.rstride; q.blk0 = blk;
+      q.Nout = o.Nout; q.Kin = o.Kin; q.R = o.R; q.ghost = dp_ghost(o.R, o.Nout, o.Kin) ? 1 : 0;
+      q.ntiles = dp_norm_tiles(o.R, o.Nout, o.Kin, &q.tm, &q.tn);
+      q.fw = o.fw; q.fb = o.fw + 1;
+      blk += (long long)s->B * q.ntiles;
+    }
+    return dp_norm_group(g, s->B, partial, sqnorms, t->f.n, st);
+  }
+
+  // Every queued linear's per-sample gradient rows: one psg_group launch.  Rotated rows first turn each item into
+  // Y^ = dY Q_S and X^ = [X | 1] Q_A on the error-compensated tensor-core GEMM (linear_nt, bias = the last row of Q_A),
+  // and psg_group appends no ones column to them.
+  int row_group(cudaStream_t st) {
+    PsgGroup pg;
+    long long blk = 0;
     int64_t off = 0;
-    float* ws = q.kws;
+    for (pg.n = 0; pg.n < n; ++pg.n) {
+      const Linear& o = *it[pg.n].o;
+      PsgItem& q = pg.it[pg.n];
+      q.Y = it[pg.n].Y; q.X = it[pg.n].X; q.ldy = o.Nout; q.ldx = o.Kin;
+      if (mode == GRAD_ROTATED) {
+        float* yh = rot + off; off += round_up(o.rows * o.Nout, 64);
+        float* xh = rot + off; off += round_up(o.rows * o.Np, 64);
+        RD_TRY(linear_nt(nt(q.Y, o.Nout, bases + o.qs, o.Nout, yh, o.Nout, o.rows, o.Nout, o.Nout), bases_lo + o.qs, st));
+        GemmP r = nt(q.X, o.Kin, bases + o.qa, o.Kin, xh, o.Np, o.rows, o.Np, o.Kin);
+        r.bias = bases + o.qb;
+        RD_TRY(linear_nt(r, bases_lo + o.qa, st));
+        q.Y = yh; q.X = xh; q.ldx = o.Np;
+      }
+      q.sstride = o.sstride; q.rstride = o.rstride; q.blk0 = blk; q.gw = t->f.off[o.fw]; q.gb = t->f.off[o.fw + 1];
+      q.Nout = o.Nout; q.Kin = o.Kin; q.R = o.R; q.ntiles = psg_tiles(o.Nout, o.Kin, &q.tn);
+      blk += (long long)s->B * q.ntiles;
+    }
+    return psg_group(pg, s->B, G, t->bucket, scale, st, mode == GRAD_ROTATED);
+  }
+
+  // EK-FAC factors: per item, dW = X^T X with db = column sums of X, and dW = dY^T dY (tn: queued for one grouped
+  // tensor-core launch when the shape fits, else CUDA cores), then each block's sums are added into the fp64 factors
+  // (dY carries the gradient of l_b / B, so S is scaled by B^2).
+  int factor_sums(cudaStream_t st) {
+    int64_t off = 0;
     const float* Aw[DP_MAX_ITEMS]; const float* Ab[DP_MAX_ITEMS]; const float* Sw[DP_MAX_ITEMS];
-    for (int i = 0; i < q.pg.n; ++i) {
-      const PsgItem& o = q.pg.it[i];
-      const int64_t rows = (int64_t)q.B * o.R;
-      float* aw = ws + off; off += round_up((int64_t)o.Kin * o.Kin, 64);
-      float* ab = ws + off; off += round_up(o.Kin, 64);
-      float* sw = ws + off; off += round_up((int64_t)o.Nout * o.Nout, 64);
-      float* sb = ws + off; off += round_up(o.Nout, 64);
-      float* pa = ws + off; off += round_up(tc_wgrad_partial_floats(o.Kin, o.Kin, rows), 64);
-      float* ps = ws + off; off += round_up(tc_wgrad_partial_floats(o.Nout, o.Nout, rows), 64);
-      RD_TRY(tn(&wq, o.X, o.ldx, o.X, o.ldx, aw, ab, o.Kin, o.Kin, rows, pa, q.kpartial, st));
-      RD_TRY(tn(&wq, o.Y, o.ldy, o.Y, o.ldy, sw, sb, o.Nout, o.Nout, rows, ps, q.kpartial, st));
+    for (int i = 0; i < n; ++i) {
+      const Linear& o = *it[i].o;
+      float* aw = kws + off; off += round_up((int64_t)o.Kin * o.Kin, 64);
+      float* ab = kws + off; off += round_up(o.Kin, 64);
+      float* sw = kws + off; off += round_up((int64_t)o.Nout * o.Nout, 64);
+      float* sb = kws + off; off += round_up(o.Nout, 64);
+      float* pa = kws + off; off += round_up(tc_wgrad_partial_floats(o.Kin, o.Kin, o.rows), 64);
+      float* ps = kws + off; off += round_up(tc_wgrad_partial_floats(o.Nout, o.Nout, o.rows), 64);
+      RD_TRY(tn(&wq, it[i].X, o.Kin, it[i].X, o.Kin, aw, ab, o.Kin, o.Kin, o.rows, pa, kpartial, st));
+      RD_TRY(tn(&wq, it[i].Y, o.Nout, it[i].Y, o.Nout, sw, sb, o.Nout, o.Nout, o.rows, ps, kpartial, st));
       Aw[i] = aw; Ab[i] = ab; Sw[i] = sw;
     }
     RD_TRY(wq.flush(st));
-    for (int i = 0; i < q.pg.n; ++i) {
-      const PsgItem& o = q.pg.it[i];
-      const KfacBlock& b = K.b[q.blk_of[i]];
-      RD_TRY(kfac_accumulate(Aw[i], Ab[i], Sw[i], o.Kin, o.Nout, (long long)q.B * o.R, (double)q.B * (double)q.B,
-                             q.factors + b.a, q.factors + b.s, st));
+    for (int i = 0; i < n; ++i) {
+      const Linear& o = *it[i].o;
+      RD_TRY(kfac_accumulate(Aw[i], Ab[i], Sw[i], o.Kin, o.Nout, o.rows, (double)s->B * (double)s->B, factors + o.a, factors + o.s, st));
     }
     return 0;
   }
-  int64_t off = 0;
-  for (int i = 0; i < q.pg.n; ++i) {
-    PsgItem& o = q.pg.it[i];
-    const KfacBlock& b = K.b[q.blk_of[i]];
-    const int64_t rows = (int64_t)q.B * o.R;
-    float* yh = q.rot + off; off += round_up(rows * o.Nout, 64);
-    float* xh = q.rot + off; off += round_up(rows * b.Np, 64);
-    RD_TRY(linear_nt(nt(o.Y, o.ldy, q.bases + b.qs, o.Nout, yh, o.Nout, rows, o.Nout, o.Nout), q.bases_lo + b.qs, st));
-    GemmP g = nt(o.X, o.ldx, q.bases + b.qa, o.Kin, xh, b.Np, rows, b.Np, o.Kin);
-    g.bias = q.bases + b.qb;
-    RD_TRY(linear_nt(g, q.bases_lo + b.qa, st));
-    o.Y = yh; o.ldy = o.Nout; o.X = xh; o.ldx = b.Np;
-  }
-  return psg_group(q.pg, q.B, q.G, q.ldg, q.scale, st, true);
-}
+};
 
 // Scratch of the factor pass: the backward scratch, then per block the fp32 sums X^T X, x, dY^T dY, dY colsums and two
-// tensor-core partial buffers (kfac_flush lays a phase's items out from the start of that region, in queue order), and
+// tensor-core partial buffers (factor_sums lays a phase's items out from the start of that region, in queue order), and
 // the CUDA-core fallback's split-K partial buffer.
 struct KfacLayout { int64_t bw, kws, kpartial, total; };
 KfacLayout kfac_layout(const Shape& s) {
   KfacLayout l;
   Arena a;
   l.bw = a.take(bw_layout(s).total);
-  const KfacBlocks K = kfac_blocks(s);
+  const Trained t = trained(s);
   int64_t ws = 0, pf = 0;
-  for (int i = 0; i < K.n; ++i) {
-    const KfacBlock& b = K.b[i];
-    const int64_t rows = i < 4 * s.L ? s.M2 : s.M1;
-    ws += round_up((int64_t)b.Kin * b.Kin, 64) + round_up(b.Kin, 64) + round_up((int64_t)b.Nout * b.Nout, 64) +
-          round_up(b.Nout, 64) + round_up(tc_wgrad_partial_floats(b.Kin, b.Kin, rows), 64) +
-          round_up(tc_wgrad_partial_floats(b.Nout, b.Nout, rows), 64);
-    const int64_t p1 = splitk_partial_floats(b.Kin, b.Kin, rows), p2 = splitk_partial_floats(b.Nout, b.Nout, rows);
+  for (int i = 0; i < t.nlin; ++i) {
+    const Linear& o = t.lin[i];
+    ws += round_up((int64_t)o.Kin * o.Kin, 64) + round_up(o.Kin, 64) + round_up((int64_t)o.Nout * o.Nout, 64) +
+          round_up(o.Nout, 64) + round_up(tc_wgrad_partial_floats(o.Kin, o.Kin, o.rows), 64) +
+          round_up(tc_wgrad_partial_floats(o.Nout, o.Nout, o.rows), 64);
+    const int64_t p1 = splitk_partial_floats(o.Kin, o.Kin, o.rows), p2 = splitk_partial_floats(o.Nout, o.Nout, o.rows);
     if (p1 > pf) pf = p1;
     if (p2 > pf) pf = p2;
   }
@@ -595,15 +624,9 @@ EkfacLayout ekfac_layout(const Shape& s) {
   EkfacLayout l;
   Arena a;
   l.bw = a.take(bw_layout(s).total);
-  const KfacBlocks K = kfac_blocks(s);
-  l.lo = a.take(K.base_floats);
-  int64_t enc = 0, ob = 0;
-  for (int i = 0; i < K.n; ++i) {
-    const KfacBlock& b = K.b[i];
-    const int64_t rows = i < 4 * s.L ? s.M2 : s.M1;
-    (i < 4 * s.L ? enc : ob) += round_up(rows * b.Nout, 64) + round_up(rows * b.Np, 64);
-  }
-  l.rot = a.take(enc > ob ? enc : ob);
+  const Trained t = trained(s);
+  l.lo = a.take(t.base_floats);
+  l.rot = a.take(phase_max(t, [&](const Linear& o) { return round_up(o.rows * o.Nout, 64) + round_up(o.rows * o.Np, 64); }));
   l.total = a.off;
   return l;
 }
@@ -778,39 +801,33 @@ static int raindrop_fwd(const rd_dims* dims, const rd_params* P, const float* sr
 }
 
 static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* statics, const int64_t* lengths,
-                        const float* nscale, const float* ws, const float* dlogits, const rd_grads* G, float* sc,
-                        int phases, float* d_z0_out, cudaStream_t st, DpQueue* dp = nullptr) {
+                        const float* nscale, const float* ws, const float* dlogits, float* sc, int phases,
+                        float* d_z0_out, cudaStream_t st, GradConsumer& c) {
   Shape s;
   RD_TRY(make_shape(dims, &s));
   if ((phases & ~3) || phases == 0) { set_error("rd_raindrop_v2_bwd: phases must be 1, 2 or 3"); return -2; }
   WsLayout w = ws_layout(s);
   BwLayout b = bw_layout(s);
+  const Trained t = trained(s, c.grads);
+  c.s = &s; c.t = &t; c.b = &b; c.sc = sc;
+  const rd_grads& G = c.mode == GRAD_WEIGHTS ? *c.grads : kNoGrads;   // the head's outer products: weights mode only
   const uint64_t* rng = reinterpret_cast<const uint64_t*>(ws + w.rng);
-  float* partial = sc + b.partial;
   const float ik = s.p > 0.f ? 1.f / (1.f - s.p) : 1.f;
   float* gA = sc + b.gA; float* gB = sc + b.gB; float* gD = sc + b.gD; float* dP = sc + b.dP;
-  WgradQueue wq;     // weight gradients wait here for ONE grouped tensor-core launch per phase
-  // G == NULL (frozen parameters): only the data-gradient chain runs -- no weight-gradient GEMMs, column sums or
-  // head outer products; the scratch ends up holding the same d(loss)/d(activation) buffers
-  const bool wg = G != nullptr;
-  static const rd_grads kNoGrads = {};
-  if (!wg) G = &kNoGrads;
 
   if (phases & RD_BWD_ENCODER) {
   // ---- head: logits = mlp2(relu(mlp0(feat))), pooled = masked mean          code/models_rd.py:366-385
   const float* feat = ws + w.feat; const float* hpre = ws + w.hpre;
   float* dfeat = sc + b.dfeat; float* dhpre = sc + b.dhpre;
   RD_TRY(head_bwd(s.B, s.T, s.D, s.emb, s.ds, s.ncls, lengths, statics, P->mlp0_weight, P->mlp2_weight, feat, hpre, dlogits,
-                  dhpre, dfeat, gA, G->mlp0_weight, G->mlp0_bias, G->mlp2_weight, G->mlp2_bias, G->emb_weight, G->emb_bias, st));
-  if (dp) RD_TRY(dp->head(s, dlogits, hpre, dhpre, feat, dfeat, statics, st));
+                  dhpre, dfeat, gA, G.mlp0_weight, G.mlp0_bias, G.mlp2_weight, G.mlp2_bias, G.emb_weight, G.emb_bias, st));
+  RD_TRY(c.head(dlogits, hpre, dhpre, feat, dfeat, statics, st));
 
   const float scale = 1.f / sqrtf((float)s.hd);
   const int64_t row3 = (int64_t)s.B * 3 * s.D;
   const int64_t TT = (int64_t)s.T * s.T;
   for (int l = s.L - 1; l >= 0; --l) {
     const rd_encoder_layer_params& E = P->layer[l];
-    const rd_encoder_layer_grads& GE = G->layer[l];
-    const int fl = dp ? dp_head_fields(s) + 12 * l : 0;     // this layer's first field (in_proj_weight)
     const float* x = ws + w.Z[l];
     const float* qkv = ws + w.l[l].qkv; const float* Pm = ws + w.l[l].P;
     const float* Pd = s.p > 0.f ? ws + w.l[l].Pd : Pm;
@@ -832,20 +849,16 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
       g1.bias = E.out_proj_bias; g1.drop_p = s.p; g1.rng = rng; g1.resid = x; g1.resid_ld = s.D;
       if (linear_nt_is_tc(g1, ws + w.wsp[l].out_lo)) m1 = reinterpret_cast<const uint32_t*>(ws + w.l[l].m1);
     }
-    RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, GE.norm2_weight, GE.norm2_bias,
-                         sc + b.l[l].ln[0], K2, s.p, rng, SITE_RESID2 + l, &chunks, st, m2, mld));
-    if (dp) RD_TRY(dp->ln(r2, ws + w.l[l].st2, gA, s.T, s.D, fl + 10, fl + 11, st));
-    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0], 2 * s.D, chunks, s.D, GE.norm2_weight, st));
-    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[0] + s.D, 2 * s.D, chunks, s.D, GE.norm2_bias, st));
-    if (wg) RD_TRY(tn(&wq, K2, s.D, f, s.nhid, GE.linear2_weight, GE.linear2_bias, s.D, s.nhid, s.M2, sc + b.l[l].wp[0], partial, st));
-    if (dp) dp->add(K2, s.D, f, s.nhid, s.D, s.nhid, s.T, 1, s.B, fl + 6);
+    RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, nullptr, nullptr, sc + b.l[l].ln[0],
+                         K2, s.p, rng, SITE_RESID2 + l, &chunks, st, m2, mld));
+    RD_TRY(c.ln(t.norm2[l], sc + b.l[l].ln[0], chunks, r2, ws + w.l[l].st2, gA, st));
+    RD_TRY(c.linear(t.layer(l, LINEAR2), K2, f, st));
     {   // gF = (K2 . W2) * [f > 0] / (1-p)   ("NT" against W2^T so that the tensor-core kernel applies)
       GemmP g = nt(K2, s.D, ws + w.wsp[l].l2_t, s.D, gF, s.nhid, s.M2, s.nhid, s.D);
       g.gate = f; g.gate_ld = s.nhid; g.gate_scale = ik;  // relu' and the FFN dropout mask in one
       RD_TRY(linear_nt(g, ws + w.wsp[l].l2_tlo, st));
     }
-    if (wg) RD_TRY(tn(&wq, gF, s.nhid, x1, s.D, GE.linear1_weight, GE.linear1_bias, s.nhid, s.D, s.M2, sc + b.l[l].wp[1], partial, st));
-    if (dp) dp->add(gF, s.nhid, x1, s.D, s.nhid, s.D, s.T, 1, s.B, fl + 4);
+    RD_TRY(c.linear(t.layer(l, LINEAR1), gF, x1, st));
     {
       GemmP g = nt(gF, s.nhid, ws + w.wsp[l].l1_t, s.nhid, gA, s.D, s.M2, s.D, s.nhid);
       g.resid = res; g.resid_ld = s.D;
@@ -853,13 +866,10 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     }
     // norm1 + self-attention block
     res = s.p > 0.f ? gB : K1;
-    RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, GE.norm1_weight, GE.norm1_bias,
-                         sc + b.l[l].ln[1], K1, s.p, rng, SITE_RESID1 + l, &chunks, st, m1, mld));
-    if (dp) RD_TRY(dp->ln(r1, ws + w.l[l].st1, gA, s.T, s.D, fl + 8, fl + 9, st));
-    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1], 2 * s.D, chunks, s.D, GE.norm1_weight, st));
-    if (wg) RD_TRY(wq.colsum(sc + b.l[l].ln[1] + s.D, 2 * s.D, chunks, s.D, GE.norm1_bias, st));
-    if (wg) RD_TRY(tn(&wq, K1, s.D, ctx, s.D, GE.out_proj_weight, GE.out_proj_bias, s.D, s.D, s.M2, sc + b.l[l].wp[2], partial, st));
-    if (dp) dp->add(K1, s.D, ctx, s.D, s.D, s.D, s.T, 1, s.B, fl + 2);
+    RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, nullptr, nullptr, sc + b.l[l].ln[1],
+                         K1, s.p, rng, SITE_RESID1 + l, &chunks, st, m1, mld));
+    RD_TRY(c.ln(t.norm1[l], sc + b.l[l].ln[1], chunks, r1, ws + w.l[l].st1, gA, st));
+    RD_TRY(c.linear(t.layer(l, OUT_PROJ), K1, ctx, st));
     RD_TRY(linear_nt(nt(K1, s.D, ws + w.wsp[l].out_t, s.D, gD, s.D, s.M2, s.D, s.D), ws + w.wsp[l].out_tlo, st));
     if (attn_tc_supported(s.T, s.hd)) {
       RD_TRY(attn_tc_bwd(qkv, gD, lengths, s.B, s.H, s.T, s.hd, s.p, rng, SITE_ATTN + l, dqkv, st));
@@ -900,8 +910,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
         RD_TRY(gemm(g, st));
       }
     }
-    if (wg) RD_TRY(tn(&wq, dqkv, 3 * s.D, x, s.D, GE.in_proj_weight, GE.in_proj_bias, 3 * s.D, s.D, s.M2, sc + b.l[l].wp[3], partial, st));
-    if (dp) dp->add(dqkv, 3 * s.D, x, s.D, 3 * s.D, s.D, s.T, 1, s.B, fl);
+    RD_TRY(c.linear(t.layer(l, IN_PROJ), dqkv, x, st));
     {
       // the first layer's input gradient is d(loss)/d(encoder input): optionally delivered straight to the caller
       GemmP g = nt(dqkv, 3 * s.D, ws + w.wsp[l].in_t, 3 * s.D, (l == 0 && d_z0_out) ? d_z0_out : gA, s.D, s.M2, s.D, 3 * s.D);
@@ -909,8 +918,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
       RD_TRY(linear_nt(g, ws + w.wsp[l].in_tlo, st));
     }
   }
-  if (!(phases & RD_BWD_OBPROP)) RD_TRY(wq.flush(st));   // encoder + head gradients complete: the caller may reduce them now
-  if (dp) RD_TRY(dp->flush(st));
+  RD_TRY(c.flush(phases & RD_BWD_OBPROP, st));   // without the ob-prop phase the caller may reduce the gradients now
   }
 
   if (phases & RD_BWD_OBPROP) {
@@ -919,9 +927,7 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
   const float* X0 = ws + w.X0; const float* H1 = ws + w.H1;
   const int tc = s.tc;
   RD_TRY(obprop_out_grad(gA, ws + w.Z[0], nscale, s.B, s.T, s.N, s.dob, s.D, tc && !s.exact, gO2, st));
-  if (wg) RD_TRY(tn(&wq, gO2, s.C, H1, s.C, G->ob2_value_weight, G->ob2_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[0], partial, st));
-  const int fob = dp ? dp_head_fields(s) + 12 * s.L : 0;    // ob1 weight, ob1 bias, ob2 weight, ob2 bias
-  if (dp) dp->add(gO2, s.C, H1, s.C, s.C, s.C, s.N, s.N, 1, fob + 2);
+  RD_TRY(c.linear(t.obprop(2), gO2, H1, st));
   if (tc) {
     // dZ1 = (dZ2 . W2) * s * [H1 > 0] on the tensor cores: "NT" form against a transposed, TF32-rounded W2
     const float* W2t = ws + w.W2t;      // written by the forward's weight-prep launch
@@ -935,10 +941,8 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     g.rowscale = nscale; g.rowscale_mod = s.N; g.gate = H1; g.gate_ld = s.C;
     RD_TRY(gemm(g, st));
   }
-  if (wg) RD_TRY(tn(&wq, gO1, s.C, X0, s.C, G->ob1_value_weight, G->ob1_value_bias, s.C, s.C, s.M1, sc + b.wp_ob[1], partial, st));
-  if (dp) dp->add(gO1, s.C, X0, s.C, s.C, s.C, s.N, s.N, 1, fob);
-  RD_TRY(wq.flush(st));
-  if (dp) RD_TRY(dp->flush(st));
+  RD_TRY(c.linear(t.obprop(1), gO1, X0, st));
+  RD_TRY(c.flush(false, st));
   }
   return 0;
 }
@@ -954,8 +958,8 @@ static int prepare_w1t(const Shape& s, const rd_params* P, float* W1t, float* W1
 // d_logits into its backward scratch, then dX0.
 static int chunk_input_grad(const rd_dims* dc, const Shape& s, const rd_params* P, const Expanded& x,
                             const float* node_scale, float* S, const ChunkLayout& l, cudaStream_t st) {
-  RD_TRY(raindrop_bwd(dc, P, x.statics, x.lengths, node_scale, S + l.ws, S + l.dlogits, nullptr, S + l.sc, RD_BWD_ALL,
-                      nullptr, st));
+  GradConsumer none;
+  RD_TRY(raindrop_bwd(dc, P, x.statics, x.lengths, node_scale, S + l.ws, S + l.dlogits, S + l.sc, RD_BWD_ALL, nullptr, st, none));
   return input_grad_dx0(s, P, S + l.sc + bw_layout(s).gO1, S + l.W1t, S + l.W1tlo, S + l.dX0, st);
 }
 
@@ -1154,8 +1158,9 @@ int rd_raindrop_v2_bwd(const rd_dims* dims, const rd_params* params, const float
     set_error("rd_raindrop_v2_bwd: NULL argument");
     return -2;
   }
-  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, grads,
-                      (float*)scratch, phases, nullptr, (cudaStream_t)stream);
+  GradConsumer c{grads ? GRAD_WEIGHTS : GRAD_NONE, grads};
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, (float*)scratch,
+                      phases, nullptr, (cudaStream_t)stream, c);
 }
 
 size_t rd_input_grad_scratch_bytes(const rd_dims* dims) {
@@ -2109,11 +2114,10 @@ int rd_raindrop_v2_per_sample_grad_sqnorms(const rd_dims* dims, const rd_params*
   RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
   if (!workspace || !d_logits || !scratch || !sqnorms) { set_error("%s: NULL argument", fn); return -2; }
   const DpLayout l = dp_layout(s);
-  DpQueue q;
-  q.B = s.B; q.nf = dp_n_fields(s); q.sqnorms = sqnorms;
-  q.partial = reinterpret_cast<double*>((float*)scratch + l.partial);
-  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr,
-                      (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, &q);
+  GradConsumer c;
+  c.mode = GRAD_SQNORMS; c.sqnorms = sqnorms; c.partial = reinterpret_cast<double*>((float*)scratch + l.partial);
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits,
+                      (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, c);
 }
 
 size_t rd_per_sample_grads_scratch_bytes(const rd_dims* dims) {
@@ -2129,28 +2133,28 @@ int rd_raindrop_v2_per_sample_grads(const rd_dims* dims, const rd_params* params
   Shape s;
   RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
   if (!workspace || !d_logits || !scratch || !G) { set_error("%s: NULL argument", fn); return -2; }
-  DpQueue q;
-  const int64_t bucket = bucket_fields(s, &q.fields);
-  if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
+  const Trained t = trained(s);
+  if (ldg != t.bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)t.bucket); return -2; }
   if (reinterpret_cast<uintptr_t>(G) & 15) { set_error("%s: G must be 16-byte aligned", fn); return -2; }
-  q.B = s.B; q.nf = q.fields.n; q.G = G; q.ldg = ldg;
-  q.scale = (float)s.B;      // d_logits holds the gradient of l_b / B (the forward's batch mean): rows are of l_b
+  GradConsumer c;
+  c.mode = GRAD_ROWS; c.G = G;
+  c.scale = (float)s.B;      // d_logits holds the gradient of l_b / B (the forward's batch mean): rows are of l_b
   cudaStream_t st = (cudaStream_t)stream;
-  RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
-  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, (float*)scratch,
-                      RD_BWD_ALL, nullptr, st, &q);
+  RD_TRY(psg_pad(t.f, s.B, G, ldg, st));
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, (float*)scratch,
+                      RD_BWD_ALL, nullptr, st, c);
 }
 
 int64_t rd_kfac_factors_doubles(const rd_dims* dims) {
   Shape s;
   if (make_shape(dims, &s) != 0) return 0;
-  return kfac_blocks(s).factor_doubles;
+  return trained(s).factor_doubles;
 }
 
 int64_t rd_ekfac_bases_floats(const rd_dims* dims) {
   Shape s;
   if (make_shape(dims, &s) != 0) return 0;
-  return kfac_blocks(s).base_floats;
+  return trained(s).base_floats;
 }
 
 size_t rd_kfac_factors_scratch_bytes(const rd_dims* dims) {
@@ -2167,13 +2171,11 @@ int rd_raindrop_v2_kfac_factors(const rd_dims* dims, const rd_params* params, co
   RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
   if (!workspace || !d_logits || !scratch || !factors) { set_error("%s: NULL argument", fn); return -2; }
   if (reinterpret_cast<uintptr_t>(scratch) & 15) { set_error("%s: scratch must be 16-byte aligned", fn); return -2; }
-  const KfacBlocks K = kfac_blocks(s);
   const KfacLayout l = kfac_layout(s);
-  DpQueue q;
-  q.B = s.B; q.shape = &s; q.kb = &K; q.factors = factors;
-  q.kws = (float*)scratch + l.kws; q.kpartial = (float*)scratch + l.kpartial;
-  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr,
-                      (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, &q);
+  GradConsumer c;
+  c.mode = GRAD_FACTORS; c.factors = factors; c.kws = (float*)scratch + l.kws; c.kpartial = (float*)scratch + l.kpartial;
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits,
+                      (float*)scratch + l.bw, RD_BWD_ALL, nullptr, (cudaStream_t)stream, c);
 }
 
 size_t rd_ekfac_rows_scratch_bytes(const rd_dims* dims) {
@@ -2183,21 +2185,19 @@ size_t rd_ekfac_rows_scratch_bytes(const rd_dims* dims) {
 }
 
 // The rotated rows on checked arguments (ldg = the bucket length; G, bases and scratch 16-byte aligned), scratch laid
-// out as ekfac_layout(s): the bases' remainder image, the padding columns, then the backward with the rows queue.
+// out as ekfac_layout(s): the bases' remainder image, the padding columns, then the backward in rotated-rows mode.
 static int ekfac_rows(const Shape& s, const rd_dims* dims, const rd_params* params, const float* statics,
                       const int64_t* lengths, const float* node_scale, const void* workspace, const float* d_logits,
                       const float* bases, float* S, float* G, cudaStream_t st) {
-  DpQueue q;
-  const int64_t ldg = bucket_fields(s, &q.fields);
-  const KfacBlocks K = kfac_blocks(s);
+  const Trained t = trained(s);
   const EkfacLayout l = ekfac_layout(s);
-  q.B = s.B; q.nf = q.fields.n; q.G = G; q.ldg = ldg;
-  q.scale = (float)s.B;      // as rd_raindrop_v2_per_sample_grads: rows are of l_b
-  q.shape = &s; q.kb = &K; q.bases = bases; q.bases_lo = S + l.lo; q.rot = S + l.rot;
-  RD_TRY(grad_lo_image(bases, K.base_floats, S + l.lo, st));
-  RD_TRY(psg_pad(q.fields, s.B, G, ldg, st));
-  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, nullptr, S + l.bw,
-                      RD_BWD_ALL, nullptr, st, &q);
+  GradConsumer c;
+  c.mode = GRAD_ROTATED; c.G = G; c.bases = bases; c.bases_lo = S + l.lo; c.rot = S + l.rot;
+  c.scale = (float)s.B;      // as rd_raindrop_v2_per_sample_grads: rows are of l_b
+  RD_TRY(grad_lo_image(bases, t.base_floats, S + l.lo, st));
+  RD_TRY(psg_pad(t.f, s.B, G, t.bucket, st));
+  return raindrop_bwd(dims, params, statics, lengths, node_scale, (const float*)workspace, d_logits, S + l.bw, RD_BWD_ALL,
+                      nullptr, st, c);
 }
 
 int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, const float* statics, const int64_t* lengths,
@@ -2207,8 +2207,7 @@ int rd_raindrop_v2_ekfac_rows(const rd_dims* dims, const rd_params* params, cons
   Shape s;
   RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, false, &s));
   if (!workspace || !d_logits || !bases || !scratch || !G) { set_error("%s: NULL argument", fn); return -2; }
-  DpFields f;
-  const int64_t bucket = bucket_fields(s, &f);
+  const int64_t bucket = trained(s).bucket;
   if (ldg != bucket) { set_error("%s: ldg = %lld must be the bucket length %lld", fn, (long long)ldg, (long long)bucket); return -2; }
   if ((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(bases) | reinterpret_cast<uintptr_t>(scratch)) & 15) {
     set_error("%s: G, bases and scratch must be 16-byte aligned", fn);
@@ -2234,8 +2233,7 @@ static LaplaceLayout laplace_layout(const Shape& s, int64_t ldg) {
 size_t rd_laplace_logit_cov_scratch_bytes(const rd_dims* dims) {
   Shape s;
   if (make_shape(dims, &s) != 0 || s.ncls > RD_LAPLACE_MAX_CLASSES) return 0;
-  DpFields f;
-  return (size_t)laplace_layout(s, bucket_fields(s, &f)).total * sizeof(float);
+  return (size_t)laplace_layout(s, trained(s).bucket).total * sizeof(float);
 }
 
 int rd_raindrop_v2_laplace_logit_cov(const rd_dims* dims, const rd_params* params, const float* statics,
@@ -2250,8 +2248,7 @@ int rd_raindrop_v2_laplace_logit_cov(const rd_dims* dims, const rd_params* param
     set_error("%s: bases, w and scratch must be 16-byte aligned", fn);
     return -2;
   }
-  DpFields f;
-  const int64_t ldg = bucket_fields(s, &f);
+  const int64_t ldg = trained(s).bucket;
   const LaplaceLayout l = laplace_layout(s, ldg);
   float* S = (float*)scratch;
   cudaStream_t st = (cudaStream_t)stream;
@@ -2277,7 +2274,7 @@ int rd_dp_clip_scale(const rd_dims* dims, const void* workspace, const double* s
   Shape s;
   RD_TRY(make_shape(dims, &s));
   const WsLayout w = ws_layout(s);
-  return dp_clip(sqnorms, s.B, dp_n_fields(s), s.ncls, weight, (double)max_grad_norm, (double)expected_batch_size,
+  return dp_clip(sqnorms, s.B, trained(s).f.n, s.ncls, weight, (double)max_grad_norm, (double)expected_batch_size,
                  (const float*)workspace + w.loss_ps, d_logits, clip_factors, loss, (cudaStream_t)stream);
 }
 
@@ -2334,8 +2331,9 @@ int rd_encoder_head_bwd(const rd_dims* dims, const rd_params* params, const floa
     set_error("rd_encoder_head_bwd: NULL argument");
     return -2;
   }
-  return raindrop_bwd(dims, params, statics, lengths, nullptr, (const float*)workspace, d_logits, grads, (float*)scratch,
-                      RD_BWD_ENCODER, d_enc_in, (cudaStream_t)stream);
+  GradConsumer c{grads ? GRAD_WEIGHTS : GRAD_NONE, grads};
+  return raindrop_bwd(dims, params, statics, lengths, nullptr, (const float*)workspace, d_logits, (float*)scratch,
+                      RD_BWD_ENCODER, d_enc_in, (cudaStream_t)stream, c);
 }
 
 int rd_dropout(const float* x, int64_t n, float p, const uint64_t* rng_captured, uint32_t site, float* y, void* stream) {

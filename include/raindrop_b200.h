@@ -551,6 +551,35 @@ int rd_raindrop_v2_ablation_counts(const rd_dims* dims, const rd_params* params,
                                    int32_t n_samples, int32_t replicates_per_chunk, void* scratch, int64_t* counts,
                                    void* stream);
 
+/* ---- early prediction of Raindrop_v2: the logits of every prefix of every record, in one call ------------------------
+ * Prefix r of sample b (0 <= r <= T) is the record cut after row r: rows t < r bit for bit, +0.0 in both halves of src
+ * and in times at rows t >= r (how a shorter record is padded), the statics unchanged, and the length lengths[b] when
+ * r >= T (the input itself), else min(lengths[b], #{t < r : times[t, b] > 0}) -- the rule lengths follow (one count of
+ * times > 0 per sample) applied to the truncated record; it also keeps the quirk of records whose first time is 0.
+ * Prefix k = 0 .. n_prefixes-1 is given either
+ *   by row count: rows [K] (device int32), r = rows[k] clipped to [0, T], or
+ *   by horizon:   horizons [K] (device fp32, in the units of times), r = the number of leading rows with times <= h,
+ *                 counted up to the first row whose time exceeds h (a prefix even for unsorted times; padding rows have
+ *                 time 0 and count, which changes nothing they hold).
+ * Exactly one of the two is given.  A prefix of length 0 is computed as the model computes any length-0 sample: finite,
+ * and outside the reference's envelope.
+ *   logits  [K, B, n_classes]: the eval-mode logits of prefix k of sample b at [k, b, :]
+ *   cutoffs [K, B] int32: r of each (prefix, sample), or NULL (not written)
+ *   prefix_lengths [K, B] int64: the prefix's length, or NULL (not written)
+ * Eval arithmetic (dims->training must be 0): no dropout, the model's rng state is neither read nor advanced, no
+ * parameter gradient is written.  Work: chunks of prefixes_per_chunk prefixes; per chunk one launch computing the
+ * cutoffs and lengths (one thread per (prefix, sample)), one launch expanding the prefix-major rows (row j = m*B + b)
+ * and ONE eval forward on B*prefixes_per_chunk rows that writes the chunk's logits into its slice of `logits`.  Bitwise
+ * the forward on those rows, independent of the chunking once dims->obprop_mode is pinned (mode 0 is resolved once from
+ * B*prefixes_per_chunk rows).  scratch: rd_prefix_scratch_bytes(dims, prefixes_per_chunk) bytes (0: invalid
+ * arguments).  Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+size_t rd_prefix_scratch_bytes(const rd_dims* dims, int32_t prefixes_per_chunk);
+int rd_raindrop_v2_prefix_logits(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                 const float* times, const int64_t* lengths, const float* node_scale,
+                                 const float* horizons, const int32_t* rows, int32_t n_prefixes,
+                                 int32_t prefixes_per_chunk, void* scratch, float* logits, int32_t* cutoffs,
+                                 int64_t* prefix_lengths, void* stream);
+
 /* ---- out-of-distribution detection for Raindrop_v2: penultimate features, their moments, and per-sample scores -------
  * Post-hoc detectors on the features of a trained eval-mode model (Lee et al. 2018, Mahalanobis; Sun et al. 2022, deep
  * k-nearest neighbours; Hendrycks & Gimpel 2017, maximum softmax probability; Liu et al. 2020, energy).  Every score is
@@ -1036,6 +1065,23 @@ int rd_debug_ablation_inputs(const rd_dims* dims, const float* src, const float*
                              int32_t ablate_mask, int32_t keep, int32_t exhaustive, const uint64_t* rng, int64_t m0,
                              int32_t nc, uint8_t* keep_table, float* src_e, float* statics_e, float* times_e,
                              int64_t* lengths_e, void* stream);
+
+/* debug: the prefix inputs of rd_raindrop_v2_prefix_logits (the same two launches, same stream) for all n_prefixes = K
+ * prefixes at once: cutoffs [K, B] int32, src_e [T, K*B, 2N], statics_e [K*B, d_static] (NULL: skipped), times_e
+ * [T, K*B] and lengths_e [K*B], prefix-major (row k*B + b).  rng NULL: the prefixes given by horizons or rows as there.
+ * rng = {seed, step} (device uint64[2]): K = 1 and one cutoff per slot drawn on the device from Philox4x32-10 at site
+ * 104 (96: DP noise, 97: Fisher labels, 98: PGD start, 99: Laplace, 100: smoothing, 101: ablation, 102: SWAG, 103:
+ * counterfactual starts), the 32-bit words (b << 32) + j of key {seed, step}, word index & 3 of the block at counter
+ * index >> 2.  With R_b = 1 + the last row with times > 0 (0 if none: the slot keeps its record) and f_b the first: the
+ * first word keeps the whole record when it is < floor(p_full 2^32); otherwise r = lo_b + U(R_b - lo_b + 1), U Lemire's
+ * unbiased bounded integer with rejection over the next words and lo_b = max(f_b + 1, ceil(min_fraction R_b)), so a
+ * drawn prefix keeps row f_b.  rows (optional, [B] int32 in this mode): a slot with rows[b] >= 0 takes cutoff
+ * min(rows[b], T) instead.  p_full and min_fraction lie in [0, 1].  Only dims' B, T, N (d_inp) and d_static are read.
+ * With K = 1 it is one truncated copy of the batch, which is how PrefixTrainStep draws its batch. */
+int rd_debug_prefix_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                           const int64_t* lengths, const float* horizons, const int32_t* rows, int32_t n_prefixes,
+                           const uint64_t* rng, double p_full, double min_fraction, int32_t* cutoffs, float* src_e,
+                           float* statics_e, float* times_e, int64_t* lengths_e, void* stream);
 
 /* ---- the forward GEMM engines on their own (debug: operator-level tests) -------------------------------------------
  * Fields are grouped by size (pointers, 64-bit, 32-bit) so the layout has no interior padding. */

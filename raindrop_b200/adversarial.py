@@ -184,7 +184,7 @@ class AdversarialTrainStep(TrainStep):
             self.attack.fill_(True)
 
     def _inputs(self):
-        return self.adv_src, self.adv_static
+        return self.adv_src, self.adv_static, self.times, self.lengths
 
     def _state(self):
         extra = (self.attack_key, self.adv_src, self.adv_logits, self.clean_logits, self.adv_loss)

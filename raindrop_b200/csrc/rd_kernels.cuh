@@ -162,6 +162,30 @@ __device__ __forceinline__ RepElem rep_expand_elem(long long o, int B, int nc, i
   return e;
 }
 
+// The 32-bit words (b << 32) + j, j = 0, 1, ... of one key at one Philox site: word idx & 3 of the block at counter
+// idx >> 2, one block per four words (randomized ablation's subsets, early prediction's training cutoffs).
+struct WordStream {
+  RngKey key;
+  uint32_t site;
+  uint64_t idx;
+  uint4 blk;
+  __device__ uint32_t next() {
+    if ((idx & 3) == 0) blk = dropout_block(key, site, idx);
+    const uint32_t s = (uint32_t)idx++ & 3u;
+    return s == 0 ? blk.x : (s == 1 ? blk.y : (s == 2 ? blk.z : blk.w));
+  }
+};
+
+// Lemire's unbiased integer in [0, r), r >= 1: the high word of x * r, redrawn while the low word is below 2^32 mod r.
+__device__ __forceinline__ uint32_t bounded(WordStream& w, uint32_t r) {
+  uint64_t x = (uint64_t)w.next() * r;
+  if ((uint32_t)x < r) {
+    const uint32_t t = (0u - r) % r;
+    while ((uint32_t)x < t) x = (uint64_t)w.next() * r;
+  }
+  return (uint32_t)(x >> 32);
+}
+
 // The PGD / randomized-smoothing threat model: value cell n of the src row starting at `row` (= (t*B + b) * 2N) may be
 // perturbed when it is observed (mask > 0) and its sensor is perturbable (sens [N] uint8, NULL: every sensor).
 __device__ __forceinline__ bool perturbable_cell(const float* __restrict__ src, long long row, int N, int n,
@@ -258,6 +282,24 @@ constexpr uint32_t SITE_ABLATE = 101;       // Philox site of the sampled subset
 int ablate_inputs(const float* src, const float* statics, const float* times, const int64_t* lengths, const uint8_t* sens,
                   int P, int ast, int amask, int k, int64_t J, const uint64_t* rng, int64_t m0, int B, int nc, int T, int N,
                   int ds, uint8_t* keep, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
+
+// ---- early prediction (rd_prefix.cu; rd_raindrop_v2_prefix_logits) -----------------------------------------------
+constexpr uint32_t SITE_PREFIX = 104;       // Philox site of the training cutoffs (its key is {seed, step})
+// prefix_inputs: prefixes k0 .. k0+nc-1 of the batch as mc_expand lays them out (row j = m*B + b for prefix k0 + m).
+// One launch writes the cutoff r of each (m, b) into table [nc, B] and the prefix's length into lengths_e (and both into
+// cutoffs / lengths_out [K, B] at row k0 + m when not NULL); one launch writes src_e, times_e (rows t >= r as +0.0) and statics_e
+// (copied; NULL: skipped).  The cutoff of prefix k comes from horizons[k] (NULL: from rows[k], clipped to [0, T]); with
+// rng the nc = 1 training cutoffs are drawn per slot instead (rows, when given, is per slot: rows[b] >= 0 overrides).
+struct PrefixArgs {
+  const float* src; const float* statics; const float* times; const int64_t* lengths;
+  const float* horizons; const int32_t* rows; const uint64_t* rng;
+  int32_t* table; int32_t* cutoffs; int64_t* lengths_out; float* src_e; float* statics_e; float* times_e;
+  int64_t* lengths_e;
+  uint64_t full_below;     // a first word below this keeps the whole record: floor(p_full 2^32)
+  double min_fraction;
+  int B, T, N, ds, k0, nc;
+};
+int prefix_inputs(const PrefixArgs& a, cudaStream_t st);
 
 // ---- SWA / SWAG (rd_swag.cu; rd_swag_collect, rd_swag_sample, rd_raindrop_v2_swag_predictive) ----------------------
 constexpr uint32_t SITE_SWAG = 102;         // Philox site of the SWAG weight draws (its key is {seed, step + replicate})

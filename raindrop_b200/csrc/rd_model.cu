@@ -1821,6 +1821,111 @@ int rd_debug_ablation_inputs(const rd_dims* dims, const float* src, const float*
                        s0.B, nc, s0.T, s0.N, s0.ds, keep_table, src_e, statics_e, times_e, lengths_e, (cudaStream_t)stream);
 }
 
+// ---- early prediction -------------------------------------------------------------------------------------------------
+// Chunks of kc prefixes: the smoothing layout plus the chunk's cutoff table [kc, B] (int32).
+struct PrefixScratch : ChunkLayout { int64_t table; };
+static int prefix_scratch(const rd_dims* dims, int kc, PrefixScratch* l) {
+  RD_TRY(chunk_layout(dims, "prefixes_per_chunk", kc, dims->B, false, 0, false, l));
+  l->table = l->a.take((int64_t)kc * dims->B);
+  return 0;
+}
+
+size_t rd_prefix_scratch_bytes(const rd_dims* dims, int32_t prefixes_per_chunk) {
+  PrefixScratch l;
+  if (!dims || prefix_scratch(dims, prefixes_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+// The checks of the prefixes given by horizon or by row count, after the shape's.
+static int prefix_check(const char* fn, const float* horizons, const int32_t* rows, int32_t K) {
+  if ((horizons != nullptr) == (rows != nullptr)) { set_error("%s: give exactly one of horizons and rows", fn); return -2; }
+  if (K < 1) { set_error("%s: n_prefixes = %d must be >= 1", fn, K); return -2; }
+  return 0;
+}
+
+static PrefixArgs prefix_args(const Shape& s0, const float* src, const float* statics, const float* times,
+                              const int64_t* lengths, const float* horizons, const int32_t* rows) {
+  PrefixArgs a{};
+  a.src = src; a.statics = s0.ds > 0 ? statics : nullptr; a.times = times; a.lengths = lengths;
+  a.horizons = horizons; a.rows = rows;
+  a.B = s0.B; a.T = s0.T; a.N = s0.N; a.ds = s0.ds;
+  return a;
+}
+
+// Chunks of kc prefixes: the cutoff and expansion launches (prefix_inputs), then ONE eval forward on B*kc prefix-major
+// rows that writes its logits straight into rows k0*B .. of the output.
+int rd_raindrop_v2_prefix_logits(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                 const float* times, const int64_t* lengths, const float* node_scale,
+                                 const float* horizons, const int32_t* rows, int32_t n_prefixes,
+                                 int32_t prefixes_per_chunk, void* scratch, float* logits, int32_t* cutoffs,
+                                 int64_t* prefix_lengths, void* stream) {
+  const char* fn = "rd_raindrop_v2_prefix_logits";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !scratch || !logits || !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  RD_TRY(prefix_check(fn, horizons, rows, n_prefixes));
+  if (prefixes_per_chunk < 1) { set_error("%s: prefixes_per_chunk must be >= 1", fn); return -2; }
+  PrefixScratch l;
+  RD_TRY(prefix_scratch(dims, prefixes_per_chunk, &l));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B, kc = prefixes_per_chunk;
+  float* S = (float*)scratch;
+  const Expanded x = l.inputs(S, s0.ds);
+  PrefixArgs a = prefix_args(s0, src, statics, times, lengths, horizons, rows);
+  a.table = reinterpret_cast<int32_t*>(S + l.table);
+  a.cutoffs = cutoffs;
+  a.lengths_out = prefix_lengths;
+  a.src_e = x.src; a.statics_e = x.statics; a.times_e = x.times; a.lengths_e = x.lengths;
+  for (int k0 = 0; k0 < n_prefixes; k0 += kc) {
+    const int nc = n_prefixes - k0 < kc ? n_prefixes - k0 : kc;
+    const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * kc, 0);
+    a.k0 = k0; a.nc = nc;
+    RD_TRY(prefix_inputs(a, st));
+    RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws,
+                        logits + (int64_t)k0 * B * s0.ncls, nullptr, nullptr, nullptr, 0, st));
+    if (n_prefixes - k0 <= kc) break;
+  }
+  return 0;
+}
+
+int rd_debug_prefix_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                           const int64_t* lengths, const float* horizons, const int32_t* rows, int32_t n_prefixes,
+                           const uint64_t* rng, double p_full, double min_fraction, int32_t* cutoffs, float* src_e,
+                           float* statics_e, float* times_e, int64_t* lengths_e, void* stream) {
+  const char* fn = "rd_debug_prefix_inputs";
+  if (!dims || !src || !times || !lengths || !cutoffs || !src_e || !times_e || !lengths_e) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.ds > 0 && !statics) { set_error("%s: d_static > 0 needs statics", fn); return -2; }
+  if (rng) {
+    if (horizons || n_prefixes != 1) { set_error("%s: drawn cutoffs take no horizons and n_prefixes = 1", fn); return -2; }
+    if (!(p_full >= 0.0 && p_full <= 1.0) || !(min_fraction >= 0.0 && min_fraction <= 1.0)) {
+      set_error("%s: p_full and min_fraction must lie in [0, 1] (got %g, %g)", fn, p_full, min_fraction);
+      return -2;
+    }
+  } else {
+    RD_TRY(prefix_check(fn, horizons, rows, n_prefixes));
+  }
+  if ((int64_t)s0.B * n_prefixes > (1LL << 30)) {
+    set_error("%s: B * n_prefixes = %lld rows are too many", fn, (long long)s0.B * n_prefixes);
+    return -2;
+  }
+  PrefixArgs a = prefix_args(s0, src, statics, times, lengths, horizons, rows);
+  a.rng = rng;
+  a.full_below = (uint64_t)floor(p_full * 4294967296.0);
+  a.min_fraction = min_fraction;
+  a.table = cutoffs;
+  a.src_e = src_e; a.statics_e = s0.ds > 0 ? statics_e : nullptr; a.times_e = times_e; a.lengths_e = lengths_e;
+  a.k0 = 0; a.nc = n_prefixes;
+  return prefix_inputs(a, (cudaStream_t)stream);
+}
+
 // ---- out-of-distribution scores ---------------------------------------------------------------------------------------
 // Bank columns per similarity GEMM: as many as keep a chunk's [spc, slice] similarities within 64 MiB, a multiple of 4,
 // at most the whole (padded) bank.  Slicing does not change a similarity: every one is a full-K dot of the same rows.

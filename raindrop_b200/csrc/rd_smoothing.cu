@@ -104,28 +104,6 @@ struct AblateKeepArgs {
   int B, nc, P, k;
 };
 
-// The 32-bit words (b << 32) + j, j = 0, 1, ... of one row's key, one Philox block per four words.
-struct WordStream {
-  RngKey key;
-  uint64_t idx;
-  uint4 blk;
-  __device__ uint32_t next() {
-    if ((idx & 3) == 0) blk = dropout_block(key, SITE_ABLATE, idx);
-    const uint32_t s = (uint32_t)idx++ & 3u;
-    return s == 0 ? blk.x : (s == 1 ? blk.y : (s == 2 ? blk.z : blk.w));
-  }
-};
-
-// Lemire's unbiased integer in [0, r), r >= 1: the high word of x * r, redrawn while the low word is below 2^32 mod r.
-__device__ __forceinline__ uint32_t bounded(WordStream& w, uint32_t r) {
-  uint64_t x = (uint64_t)w.next() * r;
-  if ((uint32_t)x < r) {
-    const uint32_t t = (0u - r) % r;
-    while ((uint32_t)x < t) x = (uint64_t)w.next() * r;
-  }
-  return (uint32_t)(x >> 32);
-}
-
 // One thread per row j = m*B + b of the chunk.  Sampled mode (J == 0) shuffles in shared memory: thread i's
 // permutation holds position q at perm[q * blockDim.x + i] (uint16, P <= RD_ABLATION_MAX_PLAYERS).
 __global__ void __launch_bounds__(ABLATE_ROWS_TPB) ablate_keep_kernel(const __grid_constant__ AblateKeepArgs a) {
@@ -161,6 +139,7 @@ __global__ void __launch_bounds__(ABLATE_ROWS_TPB) ablate_keep_kernel(const __gr
   }
   WordStream w;
   w.key = RngKey{(uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(step >> 32), (uint32_t)step};
+  w.site = SITE_ABLATE;
   w.idx = (uint64_t)b << 32;
   uint16_t* perm = perm_s + threadIdx.x;
   const int ld = blockDim.x;

@@ -178,6 +178,11 @@ SIGNATURES = {
                                                           C.c_void_p]),
     "rd_debug_ablation_inputs": (C.c_int, [C.POINTER(RdDims)] + [C.c_void_p] * 5 + [C.c_int32] * 5 +
                                  [C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 6),
+    "rd_prefix_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
+    "rd_raindrop_v2_prefix_logits": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 7 +
+                                     [C.c_int32, C.c_int32] + [C.c_void_p] * 5),
+    "rd_debug_prefix_inputs": (C.c_int, [C.POINTER(RdDims)] + [C.c_void_p] * 6 + [C.c_int32, C.c_void_p, C.c_double,
+                                                                                    C.c_double] + [C.c_void_p] * 6),
     "rd_ood_features_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
     "rd_raindrop_v2_features": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 5 +
                                 [C.c_int32, C.c_int32] + [C.c_void_p] * 4),

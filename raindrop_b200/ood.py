@@ -363,14 +363,20 @@ def _average_precision(pos, neg):
     return float(np.sum(np.diff(np.r_[0.0, rec]) * prec))
 
 
+def _auroc(pos, neg):
+    """The probability that a `pos` score exceeds a `neg` score, ties counting 1/2 (the Mann-Whitney U statistic over
+    |pos| |neg|)."""
+    from scipy.stats import rankdata
+    r = rankdata(np.concatenate([neg, pos]))
+    u = r[neg.size:].sum() - pos.size * (pos.size + 1) / 2.0
+    return float(u / (neg.size * pos.size))
+
+
 def ood_metrics(score_in, score_out):
     """Detection metrics of scores on in-distribution and out-of-distribution samples (larger = OOD), float64 on the
     host: auroc (Mann-Whitney, ties count 1/2), aupr_in (in-distribution positive, ranked by -score), aupr_out (OOD
     positive) and fpr_at_95_tpr, the fraction of OOD scores <= ood_threshold(score_in, 0.95)."""
-    from scipy.stats import rankdata
     si, so = _scores(score_in, "score_in"), _scores(score_out, "score_out")
-    r = rankdata(np.concatenate([si, so]))
-    u = r[si.size:].sum() - so.size * (so.size + 1) / 2.0
     tau = ood_threshold(si, 0.95)
-    return dict(auroc=float(u / (si.size * so.size)), aupr_in=_average_precision(-si, -so),
+    return dict(auroc=_auroc(so, si), aupr_in=_average_precision(-si, -so),
                 aupr_out=_average_precision(so, si), fpr_at_95_tpr=float(np.mean(so <= tau)))

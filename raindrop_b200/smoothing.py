@@ -229,7 +229,7 @@ class AugmentedTrainStep(TrainStep):
         self.noise_key = torch.tensor(np.array([seed, 0], dtype=np.uint64).view(np.int64), device=self.device)
 
     def _inputs(self):
-        return self.noisy_src, self.noisy_static
+        return self.noisy_src, self.noisy_static, self.times, self.lengths
 
     def _state(self):
         extra = (self.noise_key, self.noisy_src) + ((self.noisy_static,) if self.noisy_static is not None else ())

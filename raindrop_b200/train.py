@@ -161,19 +161,21 @@ class TrainStep:
             self.static.copy_(batch["static"], non_blocking=non_blocking)
 
     def _inputs(self):
-        """(src, static) the forward and backward read: the loaded batch (AdversarialTrainStep reads its perturbed copy)."""
-        return self.src, self.static
+        """(src, static, times, lengths) the forward and backward read: the loaded batch (AdversarialTrainStep reads its
+        perturbed copy, PrefixTrainStep its truncated one)."""
+        return self.src, self.static, self.times, self.lengths
 
     def _bwd(self, phases, st):
-        L.check(self.lib.rd_raindrop_v2_bwd(C.byref(self.dims), C.byref(self.P), L.ptr(self._inputs()[1]), self.lengths.data_ptr(),
+        _, static, _, lengths = self._inputs()
+        L.check(self.lib.rd_raindrop_v2_bwd(C.byref(self.dims), C.byref(self.P), L.ptr(static), lengths.data_ptr(),
                                             self.plan.node_scale.data_ptr(), self.ws.data_ptr(), self.d_logits.data_ptr(),
                                             C.byref(self.G), self.scratch.data_ptr(), phases, st), "rd_raindrop_v2_bwd")
 
     def _forward(self, st):
         """forward incl. CrossEntropyLoss + d(loss)/d(logits) (fused into the head kernel)"""
-        src, static = self._inputs()
+        src, static, times, lengths = self._inputs()
         L.check(self.lib.rd_raindrop_v2_fwd(C.byref(self.dims), C.byref(self.P), src.data_ptr(), L.ptr(static),
-                                            self.times.data_ptr(), self.lengths.data_ptr(), self.plan.node_scale.data_ptr(),
+                                            times.data_ptr(), lengths.data_ptr(), self.plan.node_scale.data_ptr(),
                                             self.plan.rng_state.data_ptr(), self.ws.data_ptr(), self.logits.data_ptr(),
                                             self.y.data_ptr(), self.loss.data_ptr(), self.d_logits.data_ptr(), st),
                 "rd_raindrop_v2_fwd")

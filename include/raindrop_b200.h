@@ -551,6 +551,43 @@ int rd_raindrop_v2_ablation_counts(const rd_dims* dims, const rd_params* params,
                                    int32_t n_samples, int32_t replicates_per_chunk, void* scratch, int64_t* counts,
                                    void* stream);
 
+/* ---- worst-case sensor removal of Raindrop_v2: the fewest missing players that flip a prediction, in one call --------
+ * Players and removal as rd_raindrop_v2_ablation_counts (sensor_player, n_players = P, remove_static, remove_mask):
+ * removing a player writes +0.0 into its value column (and mask column when remove_mask, every static for the static
+ * player); times and lengths are copied bit for bit.
+ * Score of the eval-mode logits z of a row against the reference class: untargeted (target NULL) y = y[b], or the
+ * clean prediction (first argmax) when y is NULL, s = z_y - max_{c != y} z_c, success when the first argmax of z is not
+ * y; targeted, s = max_{c != t} z_c - z_t with t = target[b], success when the first argmax is t.  fp32; a row with a
+ * non-finite logit has s = +inf and never succeeds.  Candidates are ordered by (s, sorted tuple of removed players).
+ * Round 0 evaluates the empty set (the clean forward, clean_logits [B, n_classes]).  Round r = 1 .. R = max_removed:
+ *   beam (exhaustive = 0): every set S of the beam extended by every player p not in S, W_r * P rows per sample with
+ *     W_r = min(W, C(P, r-1)) (rows whose p is in S or whose beam slot is empty are evaluated and ignored); the next
+ *     beam is the W = beam_width smallest distinct candidates.  W = 1 is the greedy attack.
+ *   exhaustive (exhaustive = 1): every one of the C(P, r) sets of r players; sum_{r <= R} C(P, r) <= 2^31 - 1.
+ *   best_score [B, R+1]: the smallest score of each round.  In the first round r with a success, n_removed [B] = r and
+ *   the result is the smallest successful candidate of that round; with none by round R, n_removed = -1 and the result
+ *   is the smallest candidate of round R.  removed [B, P] (uint8, 1 = removed), logits [B, n_classes] and score [B]
+ *   describe the result.
+ * 1 <= W <= RD_SENSOR_ATTACK_MAX_BEAM, 1 <= R <= min(P, RD_SENSOR_ATTACK_MAX_REMOVED); y and target are device int64
+ * [B] class indices (at most one of them).  Eval arithmetic (dims->training must be 0).  Work: chunks of
+ * candidates_per_chunk candidates of a round; per chunk a keep-table launch (beam rounds) or ablation's unranking launch
+ * (round 0 and exhaustive rounds), the expansion launch, ONE eval forward on B*candidates_per_chunk rows and one
+ * selection launch (one CTA per sample, fixed order, no atomics).  Bitwise independent of the chunking once
+ * dims->obprop_mode is pinned.  scratch: rd_sensor_attack_scratch_bytes(dims, n_players, beam_width, max_removed,
+ * candidates_per_chunk) bytes (0: invalid arguments).  Stream-ordered, allocation- and sync-free, CUDA-graph
+ * capturable. */
+#define RD_SENSOR_ATTACK_MAX_BEAM 32
+#define RD_SENSOR_ATTACK_MAX_REMOVED 32
+size_t rd_sensor_attack_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t beam_width, int32_t max_removed,
+                                      int32_t candidates_per_chunk);
+int rd_raindrop_v2_sensor_attack(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                 const float* times, const int64_t* lengths, const float* node_scale,
+                                 const uint8_t* sensor_player, int32_t n_players, int32_t remove_static,
+                                 int32_t remove_mask, const int64_t* y, const int64_t* target, int32_t beam_width,
+                                 int32_t max_removed, int32_t exhaustive, int32_t candidates_per_chunk, void* scratch,
+                                 uint8_t* removed, int64_t* n_removed, float* logits, float* clean_logits, float* score,
+                                 float* best_score, void* stream);
+
 /* ---- early prediction of Raindrop_v2: the logits of every prefix of every record, in one call ------------------------
  * Prefix r of sample b (0 <= r <= T) is the record cut after row r: rows t < r bit for bit, +0.0 in both halves of src
  * and in times at rows t >= r (how a shorter record is padded), the statics unchanged, and the length lengths[b] when

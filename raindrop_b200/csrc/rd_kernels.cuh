@@ -282,6 +282,38 @@ constexpr uint32_t SITE_ABLATE = 101;       // Philox site of the sampled subset
 int ablate_inputs(const float* src, const float* statics, const float* times, const int64_t* lengths, const uint8_t* sens,
                   int P, int ast, int amask, int k, int64_t J, const uint64_t* rng, int64_t m0, int B, int nc, int T, int N,
                   int ds, uint8_t* keep, float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
+// ablate_expand: ablate_inputs' second launch alone, the rows of a keep table [nc*B, P] the caller wrote.
+int ablate_expand(const float* src, const float* statics, const float* times, const int64_t* lengths, const uint8_t* sens,
+                  int P, int ast, int amask, int B, int nc, int T, int N, int ds, const uint8_t* keep, float* src_e,
+                  float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st);
+
+// ---- worst-case sensor removal (rd_sensor_attack.cu; rd_raindrop_v2_sensor_attack) --------------------------------
+// One round's candidates are slots s0 .. s0+nc-1 of the chunk on nc*B rows, slot-major (row j = m*B + b for slot s0 + m).
+// A candidate is a set of removed players, written as a keep row of P bytes (0 = removed), the table
+// ablate_expand reads.  The beam of sample b is beam_n[b] sets of r - 1 players, sorted index lists
+// beam [B, W, R] (int16).
+struct SaKeepArgs {
+  const int16_t* beam; const int32_t* beam_n; uint8_t* keep; uint8_t* valid;
+  long long s0;
+  int B, nc, P, W, R, r;
+};
+// sa_keep: the keep row of slot (w, p) = (s / P, s % P) is beam set w with player p also removed; valid[j] = 0 when
+// w >= beam_n[b] or p is in set w (the row is then evaluated and ignored).
+int sa_keep(const SaKeepArgs& a, cudaStream_t st);
+// The running selection of one round and the result, per sample (sa_select: one CTA per sample).  Candidates and list
+// entries are ordered by (score, sorted tuple of removed players); the list keeps the wsel smallest distinct ones.
+struct SaSelectArgs {
+  const float* logits; const uint8_t* keep; const uint8_t* valid;   // the chunk's rows; valid NULL: every row
+  const int64_t* cls;                                               // y or the target [B] (NULL: the clean prediction)
+  float* cscore; uint8_t* csucc;                                    // per candidate [B, cc]
+  int32_t* yref; int32_t* done;                                     // [B]
+  float* top_score; uint8_t* top_keep; int32_t* top_n;              // list ping-pong [2][B*W], [2][B*W*P], [2][B]
+  float* trk_score; uint8_t* trk_keep; float* trk_logits; int32_t* trk_ok;   // best, best successful: [2][B], [2][B*P], ...
+  int16_t* beam; int32_t* beam_n;
+  uint8_t* removed; int64_t* n_removed; float* logits_out; float* clean_logits; float* score; float* best_score;
+  int B, C, P, W, R, r, nc, cc, wsel, cur, first, last, targeted;
+};
+int sa_select(const SaSelectArgs& a, cudaStream_t st);
 
 // ---- early prediction (rd_prefix.cu; rd_raindrop_v2_prefix_logits) -----------------------------------------------
 constexpr uint32_t SITE_PREFIX = 104;       // Philox site of the training cutoffs (its key is {seed, step})

@@ -1926,6 +1926,160 @@ int rd_debug_prefix_inputs(const rd_dims* dims, const float* src, const float* s
   return prefix_inputs(a, (cudaStream_t)stream);
 }
 
+// ---- worst-case sensor removal ----------------------------------------------------------------------------------------
+// Chunks of cc candidates: the smoothing layout plus the chunk's keep table [cc*B, P] (uint8), validity [cc*B] and
+// per-candidate score and success [B, cc]; per sample the reference class, the zero rank key of the exhaustive
+// unranking, the beam [B, W, R] (int16) and its size, the list (ping-pong: scores [2][B, W], keep rows [2][B, W, P],
+// sizes [2][B]), the best and best successful candidate of the round (scores [2][B], keep rows [2][B, P], logits
+// [2][B, n_classes], flags [2][B]) and the done flags [B].
+struct SensorAttackScratch : ChunkLayout {
+  int64_t keep, valid, cscore, csucc, yref, key, beam, beam_n, top_score, top_keep, top_n, trk_score, trk_keep,
+      trk_logits, trk_ok, done;
+};
+static int sensor_attack_scratch(const rd_dims* dims, int P, int W, int R, int cc, SensorAttackScratch* l) {
+  if (P < 1 || P > RD_ABLATION_MAX_PLAYERS) { set_error("n_players = %d must be in [1, %d]", P, RD_ABLATION_MAX_PLAYERS); return -2; }
+  if (W < 1 || W > RD_SENSOR_ATTACK_MAX_BEAM) {
+    set_error("beam_width = %d must be in [1, %d]", W, RD_SENSOR_ATTACK_MAX_BEAM);
+    return -2;
+  }
+  if (R < 1 || R > P || R > RD_SENSOR_ATTACK_MAX_REMOVED) {
+    set_error("max_removed = %d must be in [1, min(n_players = %d, %d)]", R, P, RD_SENSOR_ATTACK_MAX_REMOVED);
+    return -2;
+  }
+  RD_TRY(chunk_layout(dims, "candidates_per_chunk", cc, dims->B, false, 0, false, l));
+  const int64_t B = dims->B, rows = (int64_t)cc * B;
+  Arena& a = l->a;
+  l->keep = a.take(ceil_div(rows * P, 4));
+  l->valid = a.take(ceil_div(rows, 4));
+  l->cscore = a.take(rows);
+  l->csucc = a.take(ceil_div(rows, 4));
+  l->yref = a.take(B);
+  l->key = a.take(4);
+  l->beam = a.take(ceil_div(B * W * R, 2));
+  l->beam_n = a.take(B);
+  l->top_score = a.take(2 * B * W);
+  l->top_keep = a.take(ceil_div(2 * B * W * P, 4));
+  l->top_n = a.take(2 * B);
+  l->trk_score = a.take(2 * B);
+  l->trk_keep = a.take(ceil_div(2 * B * P, 4));
+  l->trk_logits = a.take(2 * B * dims->n_classes);
+  l->trk_ok = a.take(2 * B);
+  l->done = a.take(B);
+  return 0;
+}
+
+size_t rd_sensor_attack_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t beam_width, int32_t max_removed,
+                                      int32_t candidates_per_chunk) {
+  SensorAttackScratch l;
+  if (!dims || sensor_attack_scratch(dims, n_players, beam_width, max_removed, candidates_per_chunk, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+// C(n, k) saturated at cap + 1
+static int64_t binom_capped(int n, int k, int64_t cap) {
+  if (k < 0 || k > n) return 0;
+  if (k > n - k) k = n - k;
+  int64_t c = 1;
+  for (int i = 0; i < k; ++i) {
+    c = c * (n - i) / (i + 1);       // a binomial at every step
+    if (c > cap) return cap + 1;
+  }
+  return c;
+}
+
+// Round 0 evaluates the empty set.  Round r = 1 .. R evaluates W_r * P slots (w, p) of the beam, W_r = min(W, C(P, r-1))
+// (beam mode), or the C(P, r) sets of r players (exhaustive).  Per chunk of cc candidates: the keep table (sa_keep, or
+// ablate_inputs' unranking of the kept (P - r)-subsets in exhaustive mode and in round 0), the expansion
+// (ablate_expand), ONE eval forward on B*cc rows and the selection (sa_select).
+int rd_raindrop_v2_sensor_attack(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                 const float* times, const int64_t* lengths, const float* node_scale,
+                                 const uint8_t* sensor_player, int32_t n_players, int32_t remove_static,
+                                 int32_t remove_mask, const int64_t* y, const int64_t* target, int32_t beam_width,
+                                 int32_t max_removed, int32_t exhaustive, int32_t candidates_per_chunk, void* scratch,
+                                 uint8_t* removed, int64_t* n_removed, float* logits, float* clean_logits, float* score,
+                                 float* best_score, void* stream) {
+  const char* fn = "rd_raindrop_v2_sensor_attack";
+  Shape s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !scratch || !removed || !n_removed || !logits || !clean_logits || !score || !best_score ||
+      !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (y && target) { set_error("%s: give y or target, not both", fn); return -2; }
+  int64_t J;
+  RD_TRY(ablation_check(fn, s0, n_players, remove_static, remove_mask, 1, exhaustive, &J));
+  const int P = n_players, W = beam_width, R = max_removed, cc = candidates_per_chunk;
+  SensorAttackScratch l;
+  RD_TRY(sensor_attack_scratch(dims, P, W, R, cc, &l));
+  const int64_t cap = 0x7fffffffLL;
+  if (exhaustive) {
+    int64_t total = 0;
+    for (int r = 0; r <= R && total <= cap; ++r) total += binom_capped(P, r, cap);
+    if (total > cap) {
+      set_error("%s: exhaustive mode needs sum_{r <= max_removed} C(n_players, r) <= 2^31 - 1 (n_players = %d, "
+                "max_removed = %d)", fn, P, R);
+      return -2;
+    }
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = s0.B;
+  float* S = (float*)scratch;
+  const Expanded x = l.inputs(S, s0.ds);
+  uint8_t* keep = reinterpret_cast<uint8_t*>(S + l.keep);
+  uint64_t* key = reinterpret_cast<uint64_t*>(S + l.key);
+  if (cudaMemsetAsync(key, 0, 2 * sizeof(uint64_t), st) != cudaSuccess) {
+    set_error("%s: cudaMemsetAsync failed", fn);
+    return -1;
+  }
+  SaKeepArgs ka{};
+  ka.beam = reinterpret_cast<int16_t*>(S + l.beam); ka.beam_n = reinterpret_cast<int32_t*>(S + l.beam_n);
+  ka.keep = keep; ka.valid = reinterpret_cast<uint8_t*>(S + l.valid);
+  ka.B = B; ka.P = P; ka.W = W; ka.R = R;
+  SaSelectArgs sa{};
+  sa.logits = S + l.logits; sa.keep = keep;
+  sa.cls = target ? target : y;
+  sa.cscore = S + l.cscore; sa.csucc = reinterpret_cast<uint8_t*>(S + l.csucc);
+  sa.yref = reinterpret_cast<int32_t*>(S + l.yref); sa.done = reinterpret_cast<int32_t*>(S + l.done);
+  sa.top_score = S + l.top_score; sa.top_keep = reinterpret_cast<uint8_t*>(S + l.top_keep);
+  sa.top_n = reinterpret_cast<int32_t*>(S + l.top_n);
+  sa.trk_score = S + l.trk_score; sa.trk_keep = reinterpret_cast<uint8_t*>(S + l.trk_keep);
+  sa.trk_logits = S + l.trk_logits; sa.trk_ok = reinterpret_cast<int32_t*>(S + l.trk_ok);
+  sa.beam = reinterpret_cast<int16_t*>(S + l.beam); sa.beam_n = reinterpret_cast<int32_t*>(S + l.beam_n);
+  sa.removed = removed; sa.n_removed = n_removed; sa.logits_out = logits; sa.clean_logits = clean_logits;
+  sa.score = score; sa.best_score = best_score;
+  sa.B = B; sa.C = s0.ncls; sa.P = P; sa.W = W; sa.R = R; sa.cc = cc; sa.targeted = target ? 1 : 0;
+  int cur = 0;
+  for (int r = 0; r <= R; ++r) {
+    const bool unrank = exhaustive || r == 0;
+    const int64_t wr = r > 0 ? binom_capped(P, r - 1, W) : 1;
+    const int64_t n_r = unrank ? binom_capped(P, r, cap) : (wr < W ? wr : W) * P;
+    sa.r = r;
+    sa.wsel = exhaustive || r == R ? 0 : (r == 0 ? 1 : W);
+    sa.valid = unrank ? nullptr : ka.valid;
+    for (int64_t c0 = 0; c0 < n_r; c0 += cc) {
+      const int nc = (int)(n_r - c0 < cc ? n_r - c0 : cc);
+      const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
+      if (unrank) {
+        RD_TRY(ablate_inputs(src, statics, times, lengths, sensor_player, P, remove_static, remove_mask, P - r,
+                             binom_capped(P, r, cap), key, c0, B, nc, s0.T, s0.N, s0.ds, keep, x.src, x.statics, x.times,
+                             x.lengths, st));
+      } else {
+        ka.r = r; ka.s0 = c0; ka.nc = nc;
+        RD_TRY(sa_keep(ka, st));
+        RD_TRY(ablate_expand(src, statics, times, lengths, sensor_player, P, remove_static, remove_mask, B, nc, s0.T,
+                             s0.N, s0.ds, keep, x.src, x.statics, x.times, x.lengths, st));
+      }
+      RD_TRY(raindrop_fwd(&dc, params, x.src, x.statics, x.times, x.lengths, node_scale, nullptr, S + l.ws, S + l.logits,
+                          nullptr, nullptr, nullptr, 0, st));
+      sa.nc = nc; sa.cur = cur; sa.first = c0 == 0; sa.last = c0 + nc >= n_r;
+      RD_TRY(sa_select(sa, st));
+      cur ^= 1;
+    }
+  }
+  return 0;
+}
+
 // ---- out-of-distribution scores ---------------------------------------------------------------------------------------
 // Bank columns per similarity GEMM: as many as keep a chunk's [spc, slice] similarities within 64 MiB, a multiple of 4,
 // at most the whole (padded) bank.  Slicing does not change a similarity: every one is a full-K dot of the same rows.

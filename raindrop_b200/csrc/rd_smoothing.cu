@@ -215,6 +215,16 @@ int ablate_inputs(const float* src, const float* statics, const float* times, co
   const size_t smem = J > 0 ? 0 : (size_t)tpb * P * sizeof(uint16_t);
   launch_pdl(ablate_keep_kernel, dim3((unsigned)ceil_div(Bc, tpb)), dim3(tpb), smem, st, ka);
   RD_CHECK_LAUNCH("ablate_keep_kernel");
+  return ablate_expand(src, statics, times, lengths, sens, P, ast, amask, B, nc, T, N, ds, keep, src_e, statics_e, times_e,
+                       lengths_e, st);
+}
+
+int ablate_expand(const float* src, const float* statics, const float* times, const int64_t* lengths, const uint8_t* sens,
+                  int P, int ast, int amask, int B, int nc, int T, int N, int ds, const uint8_t* keep, float* src_e,
+                  float* statics_e, float* times_e, int64_t* lengths_e, cudaStream_t st) {
+  const int64_t Bc = (int64_t)B * nc;
+  const int64_t n = Bc * T * 2 * N + Bc * T + Bc * ds + Bc;
+  if (ceil_div(n, SMOOTH_TPB) > 0x7fffffffLL) { set_error("ablate_expand: %lld elements are too many", (long long)n); return -2; }
   AblateExpandArgs a;
   a.src = src; a.statics = ds > 0 ? statics : nullptr; a.times = times; a.lengths = lengths; a.sens = sens; a.keep = keep;
   a.src_e = src_e; a.statics_e = statics_e; a.times_e = times_e; a.lengths_e = lengths_e;

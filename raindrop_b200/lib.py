@@ -17,6 +17,8 @@ GRAD_DOT_SEGMENT = 4096     # RD_GRAD_DOT_SEGMENT
 LAPLACE_MAX_CLASSES = 8     # RD_LAPLACE_MAX_CLASSES
 LAPLACE_PIVOT_TOL = 1e-12   # RD_LAPLACE_PIVOT_TOL
 ABLATION_MAX_PLAYERS = 4096  # RD_ABLATION_MAX_PLAYERS
+SENSOR_ATTACK_MAX_BEAM = 32  # RD_SENSOR_ATTACK_MAX_BEAM
+SENSOR_ATTACK_MAX_REMOVED = 32  # RD_SENSOR_ATTACK_MAX_REMOVED
 OOD_MAX_K = 256             # RD_OOD_MAX_K
 OOD_POOLED, OOD_HIDDEN = 0, 1   # enum rd_ood_layer
 SWAG_MAX_RANK = 1024        # RD_SWAG_MAX_RANK
@@ -178,6 +180,9 @@ SIGNATURES = {
                                                           C.c_void_p]),
     "rd_debug_ablation_inputs": (C.c_int, [C.POINTER(RdDims)] + [C.c_void_p] * 5 + [C.c_int32] * 5 +
                                  [C.c_void_p, C.c_int64, C.c_int32] + [C.c_void_p] * 6),
+    "rd_sensor_attack_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)] + [C.c_int32] * 4),
+    "rd_raindrop_v2_sensor_attack": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 6 +
+                                     [C.c_int32] * 3 + [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_void_p] * 8),
     "rd_prefix_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
     "rd_raindrop_v2_prefix_logits": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 7 +
                                      [C.c_int32, C.c_int32] + [C.c_void_p] * 5),

@@ -882,9 +882,12 @@ int rd_raindrop_v2_per_sample_grads(const rd_dims* dims, const rd_params* params
 size_t rd_per_sample_grad_dot_scratch_bytes(int32_t Bq, int32_t Bt, int64_t ldg, int32_t n_seg);
 /* scores[q * lds + t] += alpha * sum_s < Gq[q, seg_s], Gt[t, seg_s] > for q < Bq, t < Bt (fp64, device).  Gq [Bq, ldg]
  * and Gt [Bt, ldg]: fp32 rows, device, 16-byte aligned, ldg % 4 == 0.  Segment s = columns [seg_off[s], + seg_len[s])
- * (host arrays, n_seg <= 65535, offsets % 4 == 0, 1 <= length <= RD_GRAD_DOT_SEGMENT, inside the row).  A segment's
- * last 32-column block may reach past its end: those columns of Gq are read and multiplied by 0, so the rows must be
- * finite.  One psg_lo launch (the remainder image), one launch of wgmma 3xTF32 tiles over (64 queries, 128 train rows, segment), each segment summed in
+ * (host arrays, n_seg <= 65535, offsets % 4 == 0, 1 <= length <= RD_GRAD_DOT_SEGMENT, inside the row).  Precondition:
+ * a segment runs in 32-column blocks from its offset, and its last block may reach past its end (into the next field,
+ * or past ldg, where nothing is read).  Gt's columns there are replaced by 0, but Gq's are read and multiplied by that
+ * 0, so they must be finite: a NaN or Inf in Gq[q, seg_off[s] + seg_len[s] .. seg_off[s] + 32 ceil(seg_len[s] / 32))
+ * makes every score of query q NaN (0 * Inf is NaN).  Columns further from every segment are never multiplied into a
+ * score.  One psg_lo launch (the remainder image), one launch of wgmma 3xTF32 tiles over (64 queries, 128 train rows, segment), each segment summed in
  * fp32, and one reduce launch adding the segments in order in fp64: every score is the same product sequence whatever
  * Bq, Bt and the segment count, hence bitwise reproducible across query blockings and train chunkings.  Stream-ordered;
  * the segment table is copied from the host (not CUDA-graph capturable). */
@@ -1192,6 +1195,41 @@ typedef struct rd_debug_wgrad_plan {
 } rd_debug_wgrad_plan;
 int rd_debug_wgrad_group(const rd_wgrad_item* items, const uint64_t* partial_bytes, int32_t n,
                          const rd_debug_colsum_item* cs, int32_t ncs, rd_debug_wgrad_plan* plan, void* stream);
+
+/* ---- the per-sample gradient tiles of the linear layers on their own (debug: operator-level tests) --------------------
+ * One group of 1 <= n <= 32 linear items exactly as the backward's per-sample modes issue it.  Item i's sample b has the
+ * R rows r = b*sstride + t*rstride (t < R) of d_out [., ld_out] (first out_features columns read) and x [., ld_x];
+ * its gradient is the [out_features, in_features + 1] product d_out_b^T [x_b | 1].
+ *   RD_PS_SQNORMS  one dp_norm_tile_kernel and one dp_norm_finalize_kernel launch: sqnorms[b*nf + fw] = the squared
+ *                  Frobenius norm of the weight part, sqnorms[b*nf + fb] = that of the bias column (fp64, device), in
+ *                  the item's form: -1 the backward's choice (ghost iff R (out + in + 1) < out (in + 1)), 0 explicit
+ *                  (64 x 64 tiles of the product), 1 ghost (64 x 64 tiles of the R x R Gram triangle).  partial: 16
+ *                  bytes per CTA, at least 16 * B * (sum over the items of ntiles) bytes (partial_bytes, checked).
+ *   RD_PS_ROWS     one psg_tile_kernel launch: G[b*ldg + gw + m*in_features + n] = scale * product[m, n] and
+ *                  G[b*ldg + gb + m] = scale * product[m, in_features], each value rounded to fp32 once; no other
+ *                  column of G is written (the padding between fields is left as it was).
+ *   RD_PS_ROTATED  the same launch with x holding in_features + 1 columns that already include the bias column (the
+ *                  EK-FAC rotated [x | 1] Q_A): product = d_out_b^T x_b, no ones column appended.
+ * fw / fb / form are read in sqnorms mode only, gw / gb in the rows modes only.  Refused: a NULL pointer, n out of
+ * range, an unknown mode or form, B, R, a width or a stride below 1, ld_out below out_features or ld_x below the columns
+ * read, field indices outside [0, nf), fields that leave the row of ldg floats, and an undersized partial buffer.  The
+ * plan that ran is written back per item: the form (1 ghost), tm, tn and the tiles per sample. */
+#define RD_PS_SQNORMS 0
+#define RD_PS_ROWS 1
+#define RD_PS_ROTATED 2
+typedef struct rd_debug_per_sample_item {
+  const float* d_out; const float* x;
+  int64_t ld_out, ld_x, sstride, rstride;
+  int64_t gw, gb;                                  /* rows modes: bucket offsets of the weight and bias fields */
+  int32_t R, out_features, in_features;
+  int32_t fw, fb, form;                            /* sqnorms mode: field indices and the form */
+} rd_debug_per_sample_item;
+typedef struct rd_debug_per_sample_plan {
+  int32_t ghost, tm, tn, ntiles;
+} rd_debug_per_sample_plan;
+int rd_debug_per_sample_linear(const rd_debug_per_sample_item* items, int32_t n, int32_t B, int32_t mode, double* sqnorms,
+                               int32_t nf, double* partial, uint64_t partial_bytes, float* G, int64_t ldg, float scale,
+                               rd_debug_per_sample_plan* plan, void* stream);
 
 #ifdef __cplusplus
 }

@@ -450,8 +450,8 @@ bool dp_ghost(int R, int Nout, int Kin) {
   return (int64_t)R * (Nout + Kin + 1) < (int64_t)Nout * (Kin + 1);
 }
 
-int dp_norm_tiles(int R, int Nout, int Kin, int* tm, int* tn) {
-  if (dp_ghost(R, Nout, Kin)) {
+int dp_norm_tiles(int R, int Nout, int Kin, bool ghost, int* tm, int* tn) {
+  if (ghost) {
     *tm = (int)ceil_div(R, DP_TILE); *tn = *tm;
     return *tm * (*tm + 1) / 2;
   }

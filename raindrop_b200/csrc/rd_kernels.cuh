@@ -444,8 +444,9 @@ int adam(float* p, const float* g, float* m, float* v, int64_t n, float lr, cons
 // ---- differentially private training (rd_dp.cu) ---------------------------------------------------------------------
 // Per-sample squared gradient norms of the linear layers.  Item = one (dY, X) operand pair of a weight gradient; sample
 // b's rows are r = b*sstride + t*rstride, t < R (encoder: sstride 1, rstride B, R = T; ob-prop: sstride N, rstride 1,
-// R = N).  Its weight and bias sums land in sqnorms[b*nf + fw] and [b*nf + fb].  ghost / tm / tn / ntiles come from
-// dp_norm_tiles; blk0 = the item's first CTA in the group launch (items in order, B*ntiles CTAs each).
+// R = N).  Its weight and bias sums land in sqnorms[b*nf + fw] and [b*nf + fb].  ghost is the item's form (dp_ghost's
+// choice in the backward), tm / tn / ntiles come from dp_norm_tiles for that form; blk0 = the item's first CTA in the
+// group launch (items in order, B*ntiles CTAs each).
 constexpr uint32_t SITE_DP_NOISE = 96;      // Philox site of the DP-SGD noise (its key is the noise key, not the dropout key)
 constexpr int DP_MAX_ITEMS = 4 * RD_MAX_LAYERS;
 constexpr int DP_MAX_FIELDS = 128;
@@ -457,7 +458,8 @@ struct DpNormItem {
 struct DpNormGroup { DpNormItem it[DP_MAX_ITEMS]; int n; };
 // ghost iff R (Nout + Kin + 1) < Nout (Kin + 1): the form with fewer multiply-adds
 bool dp_ghost(int R, int Nout, int Kin);
-int dp_norm_tiles(int R, int Nout, int Kin, int* tm, int* tn);     // tiles per sample; sets tm, tn
+// tiles per sample of the given form (ghost: the R x R upper triangle, else the [Nout, Kin + 1] product); sets tm, tn
+int dp_norm_tiles(int R, int Nout, int Kin, bool ghost, int* tm, int* tn);
 // one launch over every item's tiles (partial: 2 doubles per CTA), one launch adding them into sqnorms
 int dp_norm_group(const DpNormGroup& g, int B, double* partial, double* sqnorms, int nf, cudaStream_t st);
 // LayerNorm gamma / beta of each sample (rows t*B + b, t < T) from its input x, stats {mean, rstd} and output gradient dy

@@ -243,7 +243,9 @@ BwLayout bw_layout(const Shape& s) {
 // CTAs (= partial pairs) of the larger of the two phases' group launches
 int64_t dp_partial_blocks(const Shape& s) {
   int tm, tn;
-  return (int64_t)s.B * phase_max(trained(s), [&](const Linear& o) { return (int64_t)dp_norm_tiles(o.R, o.Nout, o.Kin, &tm, &tn); });
+  return (int64_t)s.B * phase_max(trained(s), [&](const Linear& o) {
+    return (int64_t)dp_norm_tiles(o.R, o.Nout, o.Kin, dp_ghost(o.R, o.Nout, o.Kin), &tm, &tn);
+  });
 }
 
 // Scratch of rd_raindrop_v2_per_sample_grad_sqnorms: the backward scratch of the data-gradient chain, then the partial
@@ -531,7 +533,7 @@ struct GradConsumer {
       DpNormItem& q = g.it[g.n];
       q.Y = it[g.n].Y; q.X = it[g.n].X; q.ldy = o.Nout; q.ldx = o.Kin; q.sstride = o.sstride; q.rstride = o.rstride; q.blk0 = blk;
       q.Nout = o.Nout; q.Kin = o.Kin; q.R = o.R; q.ghost = dp_ghost(o.R, o.Nout, o.Kin) ? 1 : 0;
-      q.ntiles = dp_norm_tiles(o.R, o.Nout, o.Kin, &q.tm, &q.tn);
+      q.ntiles = dp_norm_tiles(o.R, o.Nout, o.Kin, q.ghost != 0, &q.tm, &q.tn);
       q.fw = o.fw; q.fb = o.fw + 1;
       blk += (long long)s->B * q.ntiles;
     }
@@ -2767,6 +2769,80 @@ int rd_debug_wgrad_group(const rd_wgrad_item* items, const uint64_t* partial_byt
   plan->rows_target = pl.rows_target;
   for (int i = 0; i < n; ++i) { plan->nsplit[i] = pl.sp[i].nsplit; plan->rows_per_split[i] = pl.sp[i].rows_per_split; }
   return 0;
+}
+
+int rd_debug_per_sample_linear(const rd_debug_per_sample_item* items, int32_t n, int32_t B, int32_t mode, double* sqnorms,
+                               int32_t nf, double* partial, uint64_t partial_bytes, float* G, int64_t ldg, float scale,
+                               rd_debug_per_sample_plan* plan, void* stream) {
+  const char* fn = "rd_debug_per_sample_linear";
+  static_assert(DP_MAX_ITEMS == 32, "the item limit rd_debug_per_sample_linear is declared with");
+  if (n < 1 || n > DP_MAX_ITEMS) { set_error("%s: %d items, it takes 1 to %d", fn, n, DP_MAX_ITEMS); return -2; }
+  if (mode != RD_PS_SQNORMS && mode != RD_PS_ROWS && mode != RD_PS_ROTATED) {
+    set_error("%s: unknown mode %d", fn, mode);
+    return -2;
+  }
+  const bool sq = mode == RD_PS_SQNORMS;
+  if (!items || !plan || (sq && (!sqnorms || !partial)) || (!sq && !G)) { set_error("%s: NULL argument", fn); return -2; }
+  if (B < 1 || (sq && nf < 1) || (!sq && ldg < 1)) {
+    set_error("%s: bad sizes (B=%d nf=%d ldg=%lld)", fn, B, nf, (long long)ldg);
+    return -2;
+  }
+  DpNormGroup g;
+  PsgGroup pg;
+  long long blk = 0;
+  for (int i = 0; i < n; ++i) {
+    const rd_debug_per_sample_item& a = items[i];
+    const int xw = a.in_features + (mode == RD_PS_ROTATED ? 1 : 0);     // the columns of x the kernel reads
+    if (!a.d_out || !a.x) { set_error("%s: item %d has a NULL pointer", fn, i); return -2; }
+    if (a.R < 1 || a.out_features < 1 || a.in_features < 1 || a.sstride < 1 || a.rstride < 1 || a.ld_out < a.out_features ||
+        a.ld_x < xw) {
+      set_error("%s: item %d has bad sizes (R=%d out=%d in=%d sstride=%lld rstride=%lld ld_out=%lld ld_x=%lld)", fn, i, a.R,
+                a.out_features, a.in_features, (long long)a.sstride, (long long)a.rstride, (long long)a.ld_out,
+                (long long)a.ld_x);
+      return -2;
+    }
+    plan[i].ghost = 0;
+    plan[i].tm = (int32_t)ceil_div(a.out_features, 64);
+    if (sq) {
+      if (a.form < -1 || a.form > 1) { set_error("%s: item %d has unknown form %d", fn, i, a.form); return -2; }
+      if (a.fw < 0 || a.fw >= nf || a.fb < 0 || a.fb >= nf) {
+        set_error("%s: item %d has fields (%d, %d) outside nf=%d", fn, i, a.fw, a.fb, nf);
+        return -2;
+      }
+      DpNormItem& q = g.it[i];
+      q.Y = a.d_out; q.X = a.x; q.ldy = a.ld_out; q.ldx = a.ld_x; q.sstride = a.sstride; q.rstride = a.rstride; q.blk0 = blk;
+      q.Nout = a.out_features; q.Kin = a.in_features; q.R = a.R;
+      q.ghost = (a.form < 0 ? dp_ghost(a.R, a.out_features, a.in_features) : a.form == 1) ? 1 : 0;
+      q.ntiles = dp_norm_tiles(q.R, q.Nout, q.Kin, q.ghost != 0, &q.tm, &q.tn);
+      q.fw = a.fw; q.fb = a.fb;
+      plan[i].ghost = q.ghost; plan[i].tm = q.tm; plan[i].tn = q.tn; plan[i].ntiles = q.ntiles;
+    } else {
+      const long long wn = (long long)a.out_features * a.in_features;
+      if (a.gw < 0 || a.gw + wn > ldg || a.gb < 0 || a.gb + a.out_features > ldg) {
+        set_error("%s: item %d has fields at (%lld, %lld) that leave the row of %lld", fn, i, (long long)a.gw,
+                  (long long)a.gb, (long long)ldg);
+        return -2;
+      }
+      PsgItem& q = pg.it[i];
+      q.Y = a.d_out; q.X = a.x; q.ldy = a.ld_out; q.ldx = a.ld_x; q.sstride = a.sstride; q.rstride = a.rstride; q.blk0 = blk;
+      q.gw = a.gw; q.gb = a.gb; q.Nout = a.out_features; q.Kin = a.in_features; q.R = a.R;
+      q.ntiles = psg_tiles(q.Nout, q.Kin, &q.tn);
+      plan[i].tn = q.tn; plan[i].ntiles = q.ntiles;
+    }
+    blk += (long long)B * plan[i].ntiles;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!sq) {
+    pg.n = n;
+    return psg_group(pg, B, G, ldg, scale, st, mode == RD_PS_ROTATED);
+  }
+  if (partial_bytes < 16ull * (unsigned long long)blk) {
+    set_error("%s: a partial buffer of %llu bytes, it needs %llu", fn, (unsigned long long)partial_bytes,
+              16ull * (unsigned long long)blk);
+    return -2;
+  }
+  g.n = n;
+  return dp_norm_group(g, B, partial, sqnorms, nf, st);
 }
 
 }  // extern "C"

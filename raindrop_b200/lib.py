@@ -112,6 +112,19 @@ class RdDebugWgradPlan(C.Structure):
                 ("rows_per_split", C.c_int32 * 12)]
 
 
+class RdDebugPerSampleItem(C.Structure):
+    _fields_ = ([("d_out", C.c_void_p), ("x", C.c_void_p)] +
+                [(f, C.c_int64) for f in ("ld_out", "ld_x", "sstride", "rstride", "gw", "gb")] +
+                [(f, C.c_int32) for f in ("R", "out_features", "in_features", "fw", "fb", "form")])
+
+
+class RdDebugPerSamplePlan(C.Structure):
+    _fields_ = [(f, C.c_int32) for f in ("ghost", "tm", "tn", "ntiles")]
+
+
+RD_PS_SQNORMS, RD_PS_ROWS, RD_PS_ROTATED = 0, 1, 2
+
+
 # name -> (restype, argtypes); every symbol include/raindrop_b200.h declares
 SIGNATURES = {
     "rd_abi_version": (C.c_int, []),
@@ -258,6 +271,9 @@ SIGNATURES = {
     "rd_debug_colsum": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rd_debug_wgrad_group": (C.c_int, [C.POINTER(RdWgradItem), C.POINTER(C.c_uint64), C.c_int32,
                                        C.POINTER(RdDebugColsumItem), C.c_int32, C.POINTER(RdDebugWgradPlan), C.c_void_p]),
+    "rd_debug_per_sample_linear": (C.c_int, [C.POINTER(RdDebugPerSampleItem), C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64,
+                                             C.c_float, C.POINTER(RdDebugPerSamplePlan), C.c_void_p]),
     "rd_kfac_factors_doubles": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_ekfac_bases_floats": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_kfac_factors_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),

@@ -1231,6 +1231,50 @@ int rd_debug_per_sample_linear(const rd_debug_per_sample_item* items, int32_t n,
                                int32_t nf, double* partial, uint64_t partial_bytes, float* G, int64_t ldg, float scale,
                                rd_debug_per_sample_plan* plan, void* stream);
 
+/* ---- the encoder's LayerNorm on its own (debug: operator-level tests) -------------------------------------------------
+ * Forward (forward != 0): one layernorm_fwd call, y [rows, D] = (x - mean) rstd gamma + beta, stats [rows][2] = {mean,
+ * rstd}, rstd = 1 / sqrt(var + eps).  Backward (backward != 0): one layernorm_bwd call on x, stats (the forward's when
+ * both run, else the caller's), gamma and dy [rows, D]: dx, and when drop_p > 0 dx_drop = dx times the dropout mask of
+ * `site` (keep_bits [rows][keep_ld] words when given, bit j % 32 of word j / 32, read by the fused kernel only; else
+ * Philox at index row * D + j with key rng = {seed, step}); its per-CTA partial rows land in scratch [chunks][2][D] and
+ * are reduced into dgamma and dbeta [D] by one tc_wgrad_group launch with two column sums and no weight problems, as
+ * the training backward's gradient consumer folds them.  Written back: the classes that ran (fwd_class: RD_LN_GENERIC
+ * or the vector kernel's float4 per lane RD_LN_VEC1 / 2 / 5; bwd_class: the fused kernel's RD_LN_VEC1 / 2 / 5 or
+ * RD_LN_SPLIT_VEC / RD_LN_SPLIT_SCALAR), chunks (the partial rows) and keep_source (RD_LN_KEEP_*, the mask dx_drop
+ * took).  Refused: a NULL pointer a half needs, neither half, rows or D below 1, scratch_floats below
+ * rd_debug_layernorm_scratch_floats(rows, D), keep_bits with keep_ld below ceil(D / 32), drop_p outside [0, 1), and
+ * drop_p > 0 without rng or dx_drop. */
+#define RD_LN_GENERIC 0
+#define RD_LN_VEC1 1
+#define RD_LN_VEC2 2
+#define RD_LN_VEC5 5
+#define RD_LN_SPLIT_VEC 16
+#define RD_LN_SPLIT_SCALAR 17
+#define RD_LN_KEEP_NONE 0
+#define RD_LN_KEEP_PHILOX 1
+#define RD_LN_KEEP_BITS 2
+typedef struct rd_debug_layernorm_args {
+  const float* x; const float* gamma; const float* beta; float* y; float* stats;
+  const float* dy; float* dx; float* dx_drop; const uint64_t* rng; const uint32_t* keep_bits;
+  float* scratch; float* dgamma; float* dbeta;
+  int64_t rows, scratch_floats;
+  int32_t D, keep_ld; float eps, drop_p; uint32_t site;
+  int32_t forward, backward;
+  int32_t fwd_class, bwd_class, chunks, keep_source;      /* written back */
+} rd_debug_layernorm_args;
+int64_t rd_debug_layernorm_scratch_floats(int64_t rows, int32_t D);
+int rd_debug_layernorm(rd_debug_layernorm_args* args, void* stream);
+/* One per-sample LayerNorm launch exactly as the backward's gradient consumer issues it, over the T*B rows r = t*B + b of
+ * x, stats and dy (the encoder layout): sample b's gamma gradient is sum_t dy_r (x_r - mean_r) rstd_r, its beta gradient
+ * sum_t dy_r.  RD_PS_SQNORMS: one dp_ln_sqnorm_kernel launch, sqnorms[b*nf + fw] and [b*nf + fb] = their squared norms
+ * (fp64).  RD_PS_ROWS: one psg_ln_kernel launch, G[b*ldg + gw + d] and G[b*ldg + gb + d] = scale times them, rounded to
+ * fp32 once (the rotated modes of the consumer issue the same launch: LayerNorms are not rotated); nothing else of G is
+ * written.  Refused: a NULL pointer, an unknown mode, T, B or D below 1, fields outside [0, nf), fields that leave the
+ * row of ldg floats. */
+int rd_debug_per_sample_layernorm(int32_t mode, const float* x, const float* stats, const float* dy, int32_t T, int32_t B,
+                                  int32_t D, double* sqnorms, int32_t nf, int32_t fw, int32_t fb, float* G, int64_t ldg,
+                                  int64_t gw, int64_t gb, float scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1464,13 +1464,19 @@ int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float
   return 0;
 }
 
+int layernorm_fwd_class(const float* x, const float* gamma, const float* beta, const float* y, int D) {
+  const uintptr_t bits = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta);
+  if ((D & 3) != 0 || D > 640 || (bits & 15) != 0) return LN_GENERIC;
+  return D <= 128 ? 1 : (D <= 256 ? 2 : 5);
+}
+
 int layernorm_fwd(const float* x, const float* gamma, const float* beta, int64_t rows, int D, float eps, float* y,
                   float* stats, cudaStream_t st) {
-  const uintptr_t bits = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta);
-  if ((D & 3) == 0 && D <= 640 && (bits & 15) == 0) {
+  const int cls = layernorm_fwd_class(x, gamma, beta, y, D);
+  if (cls != LN_GENERIC) {
     const unsigned blocks = (unsigned)ceil_div(rows, (int64_t)(TPB / 32));          // 8 warps, one row each
-    if (D <= 128) launch_pdl(layernorm_fwd_vec_kernel<1>, dim3(blocks), dim3(TPB), 0, st, x, gamma, beta, (long long)rows, D, eps, y, stats);
-    else if (D <= 256) launch_pdl(layernorm_fwd_vec_kernel<2>, dim3(blocks), dim3(TPB), 0, st, x, gamma, beta, (long long)rows, D, eps, y, stats);
+    if (cls == 1) launch_pdl(layernorm_fwd_vec_kernel<1>, dim3(blocks), dim3(TPB), 0, st, x, gamma, beta, (long long)rows, D, eps, y, stats);
+    else if (cls == 2) launch_pdl(layernorm_fwd_vec_kernel<2>, dim3(blocks), dim3(TPB), 0, st, x, gamma, beta, (long long)rows, D, eps, y, stats);
     else launch_pdl(layernorm_fwd_vec_kernel<5>, dim3(blocks), dim3(TPB), 0, st, x, gamma, beta, (long long)rows, D, eps, y, stats);
     RD_CHECK_LAUNCH("layernorm_fwd_vec_kernel");
     return 0;
@@ -1485,33 +1491,39 @@ int64_t ln_bwd_scratch_floats(int64_t rows, int D) {
   return (a > b ? a : b) * 2 * D;
 }
 
-int layernorm_bwd(const float* x, const float* stats, const float* gamma, const float* dy, int64_t rows, int D,
-                  float* dx, float* dgamma, float* dbeta, float* scratch, float* dx_drop, float drop_p,
-                  const uint64_t* rng, uint32_t site, int* deferred_chunks, cudaStream_t st, const uint32_t* keep_bits,
-                  int keep_ld) {
+int layernorm_bwd_class(const float* x, const float* gamma, const float* dy, const float* dx, const float* dx_drop,
+                        float drop_p, int D) {
   const uintptr_t bits = reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) |
-                         reinterpret_cast<uintptr_t>(dx) | reinterpret_cast<uintptr_t>(dx_drop);
-  int chunks;
-  if ((D & 3) == 0 && D <= 128 * LNB_MAXIT && (bits & 15) == 0) {     // fused single pass
-    chunks = (int)ceil_div(rows, D <= 256 ? LNB_ROWS_NARROW : LNB_ROWS);
-    auto kern = D <= 128 ? layernorm_bwd_fused_kernel<1, 1, LNB_ROWS_NARROW>
-                         : (D <= 256 ? layernorm_bwd_fused_kernel<2, 1, LNB_ROWS_NARROW> : layernorm_bwd_fused_kernel<LNB_MAXIT, 1, LNB_ROWS>);
-    launch_pdl(kern, dim3(chunks), dim3(256), 8 * 2 * D * sizeof(float), st, x, stats, gamma, dy, (long long)rows, D,
+                         reinterpret_cast<uintptr_t>(dx);
+  if ((D & 3) == 0 && D <= 128 * LNB_MAXIT && ((bits | reinterpret_cast<uintptr_t>(dx_drop)) & 15) == 0)
+    return D <= 128 ? 1 : (D <= 256 ? 2 : LNB_MAXIT);
+  // layernorm_bwd_dx_kernel's own test for its 128-bit path: the same pointers, dx_drop only when it writes it
+  const uintptr_t split = bits | reinterpret_cast<uintptr_t>(drop_p > 0.f ? dx_drop : nullptr);
+  return (D & 3) == 0 && (split & 15) == 0 ? LN_SPLIT_VEC : LN_SPLIT_SCALAR;
+}
+
+int layernorm_bwd(const float* x, const float* stats, const float* gamma, const float* dy, int64_t rows, int D,
+                  float* dx, float* scratch, float* dx_drop, float drop_p, const uint64_t* rng, uint32_t site, int* chunks,
+                  cudaStream_t st, const uint32_t* keep_bits, int keep_ld) {
+  const int cls = layernorm_bwd_class(x, gamma, dy, dx, dx_drop, drop_p, D);
+  if (cls != LN_SPLIT_VEC && cls != LN_SPLIT_SCALAR) {     // fused single pass
+    *chunks = (int)ceil_div(rows, D <= 256 ? LNB_ROWS_NARROW : LNB_ROWS);
+    auto kern = cls == 1 ? layernorm_bwd_fused_kernel<1, 1, LNB_ROWS_NARROW>
+                         : (cls == 2 ? layernorm_bwd_fused_kernel<2, 1, LNB_ROWS_NARROW> : layernorm_bwd_fused_kernel<LNB_MAXIT, 1, LNB_ROWS>);
+    launch_pdl(kern, dim3(*chunks), dim3(256), 8 * 2 * D * sizeof(float), st, x, stats, gamma, dy, (long long)rows, D,
                dx, drop_p > 0.f ? dx_drop : (float*)nullptr, drop_p, rng, site, scratch, keep_bits, keep_ld);
     RD_CHECK_LAUNCH("layernorm_bwd_fused_kernel");
   } else {
     layernorm_bwd_dx_kernel<<<blocks_for(rows * 32), TPB, 0, st>>>(x, stats, gamma, dy, rows, D, dx,
                                                                 drop_p > 0.f ? dx_drop : nullptr, drop_p, rng, site);
     RD_CHECK_LAUNCH("layernorm_bwd_dx_kernel");
-    chunks = (int)ceil_div(rows, LN_ROWS);
-    if (chunks > 65535) { set_error("layernorm_bwd: too many row chunks"); return -2; }
-    dim3 grid((unsigned)ceil_div(D, 32), (unsigned)chunks);
+    *chunks = (int)ceil_div(rows, LN_ROWS);
+    if (*chunks > 65535) { set_error("layernorm_bwd: too many row chunks"); return -2; }
+    dim3 grid((unsigned)ceil_div(D, 32), (unsigned)*chunks);
     layernorm_bwd_param_kernel<<<grid, dim3(32, 8), 0, st>>>(x, stats, dy, rows, D, scratch);
     RD_CHECK_LAUNCH("layernorm_bwd_param_kernel");
   }
-  // scratch = [chunks][2][D] partial column sums -> dgamma, dbeta (fixed order, deterministic)
-  if (deferred_chunks) { *deferred_chunks = chunks; return 0; }     // the caller folds this into a later reduction launch
-  return reduce_partials2(scratch, chunks, D, dgamma, D, dbeta, st);
+  return 0;
 }
 
 int attn_softmax_fwd(float* S, const int64_t* lengths, int B, int H, int T, float drop_p, const uint64_t* rng,

@@ -371,19 +371,28 @@ int ood_topk(const float* sim, int64_t ld, int n, int ncols, int64_t col0, int k
 
 int node_scale(const int64_t* edge_tgt, const float* edge_w, int E, int N, float* s, cudaStream_t st);
 
+// The kernel classes of the LayerNorm launches (RD_LN_* in the public header): the forward's and the backward fused
+// kernel's ITERS (1, 2, 5: D <= 128, 256, 640, D % 4 == 0, every pointer 16-byte aligned), else the generic forward,
+// and the split backward with layernorm_bwd_dx_kernel's 128-bit or scalar path.
+constexpr int LN_GENERIC = RD_LN_GENERIC, LN_SPLIT_VEC = RD_LN_SPLIT_VEC, LN_SPLIT_SCALAR = RD_LN_SPLIT_SCALAR;
+int layernorm_fwd_class(const float* x, const float* gamma, const float* beta, const float* y, int D);
+int layernorm_bwd_class(const float* x, const float* gamma, const float* dy, const float* dx, const float* dx_drop,
+                        float drop_p, int D);
 // y = LN(x) * gamma + beta over the last dim (width D); stats[row] = {mean, rstd}
 int layernorm_fwd(const float* x, const float* gamma, const float* beta, int64_t rows, int D, float eps,
                   float* y, float* stats, cudaStream_t st);
-// dx from dy; dgamma/dbeta via partials. scratch >= ln_bwd_scratch_floats(rows, D)
+// dx from dy; the dgamma / dbeta column sums as per-CTA partial rows scratch[chunks][2][D] (dgamma row, dbeta row),
+// scratch >= ln_bwd_scratch_floats(rows, D).  Their reduction is the caller's (*chunks = chunks): it is folded into a
+// later grouped reduction launch (tc_wgrad_group column sums).
 int64_t ln_bwd_scratch_floats(int64_t rows, int D);
-// dx_drop (optional, used when drop_p > 0): dx with the dropout mask of `site` re-applied, i.e. the
-// gradient w.r.t. the sub-layer output that was dropped before the residual add
-// deferred_chunks != nullptr: the reduction of the per-CTA partial rows scratch[chunks][2][D] is left to the caller
-// (*deferred_chunks = chunks), who folds it into a later grouped reduction launch (tc_wgrad_group)
+// dx_drop (written when drop_p > 0): dx with the dropout mask of `site` re-applied, i.e. the gradient w.r.t. the
+// sub-layer output that was dropped before the residual add.  keep_bits (optional, [rows][keep_ld] words, bit j % 32 of
+// word j / 32): the decisions the forward GEMM epilogue stored.  Only the fused kernel reads them; the split path draws
+// Philox (site, index row * D + j) whether or not they are passed.  So stored bits must be exactly the Philox decisions
+// of that site and index, as the tensor-core epilogue writes them: then both paths apply the same mask.
 int layernorm_bwd(const float* x, const float* stats, const float* gamma, const float* dy, int64_t rows,
-                  int D, float* dx, float* dgamma, float* dbeta, float* scratch, float* dx_drop, float drop_p,
-                  const uint64_t* rng, uint32_t site, int* deferred_chunks, cudaStream_t st,
-                  const uint32_t* keep_bits = nullptr, int keep_ld = 0);   // keep_bits: decisions stored by the forward (else Philox)
+                  int D, float* dx, float* scratch, float* dx_drop, float drop_p, const uint64_t* rng, uint32_t site,
+                  int* chunks, cudaStream_t st, const uint32_t* keep_bits = nullptr, int keep_ld = 0);
 
 // in-place masked softmax over rows of S [B,H,T,T]; key j masked when j >= lengths[b].
 // If Pd != nullptr also writes the dropped probabilities (training; rep.B > 0: of replicate-major rows, rep_remap).

@@ -851,8 +851,8 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
       g1.bias = E.out_proj_bias; g1.drop_p = s.p; g1.rng = rng; g1.resid = x; g1.resid_ld = s.D;
       if (linear_nt_is_tc(g1, ws + w.wsp[l].out_lo)) m1 = reinterpret_cast<const uint32_t*>(ws + w.l[l].m1);
     }
-    RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, nullptr, nullptr, sc + b.l[l].ln[0],
-                         K2, s.p, rng, SITE_RESID2 + l, &chunks, st, m2, mld));
+    RD_TRY(layernorm_bwd(r2, ws + w.l[l].st2, E.norm2_weight, gA, s.M2, s.D, res, sc + b.l[l].ln[0], K2, s.p, rng,
+                         SITE_RESID2 + l, &chunks, st, m2, mld));
     RD_TRY(c.ln(t.norm2[l], sc + b.l[l].ln[0], chunks, r2, ws + w.l[l].st2, gA, st));
     RD_TRY(c.linear(t.layer(l, LINEAR2), K2, f, st));
     {   // gF = (K2 . W2) * [f > 0] / (1-p)   ("NT" against W2^T so that the tensor-core kernel applies)
@@ -868,8 +868,8 @@ static int raindrop_bwd(const rd_dims* dims, const rd_params* P, const float* st
     }
     // norm1 + self-attention block
     res = s.p > 0.f ? gB : K1;
-    RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, nullptr, nullptr, sc + b.l[l].ln[1],
-                         K1, s.p, rng, SITE_RESID1 + l, &chunks, st, m1, mld));
+    RD_TRY(layernorm_bwd(r1, ws + w.l[l].st1, E.norm1_weight, gA, s.M2, s.D, res, sc + b.l[l].ln[1], K1, s.p, rng,
+                         SITE_RESID1 + l, &chunks, st, m1, mld));
     RD_TRY(c.ln(t.norm1[l], sc + b.l[l].ln[1], chunks, r1, ws + w.l[l].st1, gA, st));
     RD_TRY(c.linear(t.layer(l, OUT_PROJ), K1, ctx, st));
     RD_TRY(linear_nt(nt(K1, s.D, ws + w.wsp[l].out_t, s.D, gD, s.D, s.M2, s.D, s.D), ws + w.wsp[l].out_tlo, st));
@@ -2843,6 +2843,76 @@ int rd_debug_per_sample_linear(const rd_debug_per_sample_item* items, int32_t n,
   }
   g.n = n;
   return dp_norm_group(g, B, partial, sqnorms, nf, st);
+}
+
+int64_t rd_debug_layernorm_scratch_floats(int64_t rows, int32_t D) {
+  return rows < 1 || D < 1 ? 0 : ln_bwd_scratch_floats(rows, D);
+}
+
+int rd_debug_layernorm(rd_debug_layernorm_args* a, void* stream) {
+  const char* fn = "rd_debug_layernorm";
+  if (!a) { set_error("%s: NULL argument", fn); return -2; }
+  if (!a->forward && !a->backward) { set_error("%s: neither half requested", fn); return -2; }
+  if (a->rows < 1 || a->D < 1) { set_error("%s: bad sizes (rows=%lld D=%d)", fn, (long long)a->rows, a->D); return -2; }
+  if (!a->x || !a->gamma || !a->stats || (a->forward && (!a->beta || !a->y)) ||
+      (a->backward && (!a->dy || !a->dx || !a->scratch || !a->dgamma || !a->dbeta))) {
+    set_error("%s: NULL pointer", fn);
+    return -2;
+  }
+  if (a->backward) {
+    if (!(a->drop_p >= 0.f && a->drop_p < 1.f)) { set_error("%s: drop_p %g outside [0, 1)", fn, (double)a->drop_p); return -2; }
+    if (a->drop_p > 0.f && (!a->rng || !a->dx_drop)) { set_error("%s: drop_p > 0 needs rng and dx_drop", fn); return -2; }
+    if (a->keep_bits && a->keep_ld < (a->D + 31) / 32) {
+      set_error("%s: keep_ld %d below ceil(D / 32) = %d", fn, a->keep_ld, (a->D + 31) / 32);
+      return -2;
+    }
+    const int64_t need = ln_bwd_scratch_floats(a->rows, a->D);
+    if (a->scratch_floats < need) {
+      set_error("%s: a scratch buffer of %lld floats, it needs %lld", fn, (long long)a->scratch_floats, (long long)need);
+      return -2;
+    }
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  a->fwd_class = a->bwd_class = -1;
+  a->chunks = 0;
+  a->keep_source = RD_LN_KEEP_NONE;
+  if (a->forward) {
+    a->fwd_class = layernorm_fwd_class(a->x, a->gamma, a->beta, a->y, a->D);
+    RD_TRY(layernorm_fwd(a->x, a->gamma, a->beta, a->rows, a->D, a->eps, a->y, a->stats, st));
+  }
+  if (!a->backward) return 0;
+  a->bwd_class = layernorm_bwd_class(a->x, a->gamma, a->dy, a->dx, a->dx_drop, a->drop_p, a->D);
+  const bool fused = a->bwd_class != LN_SPLIT_VEC && a->bwd_class != LN_SPLIT_SCALAR;
+  if (a->drop_p > 0.f) a->keep_source = fused && a->keep_bits ? RD_LN_KEEP_BITS : RD_LN_KEEP_PHILOX;
+  int chunks = 0;
+  RD_TRY(layernorm_bwd(a->x, a->stats, a->gamma, a->dy, a->rows, a->D, a->dx, a->scratch, a->dx_drop, a->drop_p, a->rng,
+                       a->site, &chunks, st, a->keep_bits, a->keep_ld));
+  a->chunks = chunks;
+  // GradConsumer::ln in weights mode: the two column sums of the partial rows, items of one grouped reduction launch
+  WgradQueue q;
+  RD_TRY(q.colsum(a->scratch, 2LL * a->D, chunks, a->D, a->dgamma, st));
+  RD_TRY(q.colsum(a->scratch + a->D, 2LL * a->D, chunks, a->D, a->dbeta, st));
+  return q.flush(st);
+}
+
+int rd_debug_per_sample_layernorm(int32_t mode, const float* x, const float* stats, const float* dy, int32_t T, int32_t B,
+                                  int32_t D, double* sqnorms, int32_t nf, int32_t fw, int32_t fb, float* G, int64_t ldg,
+                                  int64_t gw, int64_t gb, float scale, void* stream) {
+  const char* fn = "rd_debug_per_sample_layernorm";
+  if (mode != RD_PS_SQNORMS && mode != RD_PS_ROWS) { set_error("%s: unknown mode %d", fn, mode); return -2; }
+  const bool sq = mode == RD_PS_SQNORMS;
+  if (!x || !stats || !dy || (sq && !sqnorms) || (!sq && !G)) { set_error("%s: NULL argument", fn); return -2; }
+  if (T < 1 || B < 1 || D < 1) { set_error("%s: bad sizes (T=%d B=%d D=%d)", fn, T, B, D); return -2; }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (sq) {
+    if (fw < 0 || fw >= nf || fb < 0 || fb >= nf) { set_error("%s: fields (%d, %d) outside nf=%d", fn, fw, fb, nf); return -2; }
+    return dp_ln_sqnorm(x, stats, dy, T, B, D, sqnorms, nf, fw, fb, st);
+  }
+  if (gw < 0 || gw + D > ldg || gb < 0 || gb + D > ldg) {
+    set_error("%s: fields at (%lld, %lld) that leave the row of %lld", fn, (long long)gw, (long long)gb, (long long)ldg);
+    return -2;
+  }
+  return psg_ln(x, stats, dy, T, B, D, G, ldg, gw, gb, scale, st);
 }
 
 }  // extern "C"

@@ -125,6 +125,18 @@ class RdDebugPerSamplePlan(C.Structure):
 RD_PS_SQNORMS, RD_PS_ROWS, RD_PS_ROTATED = 0, 1, 2
 
 
+class RdDebugLayernormArgs(C.Structure):
+    _fields_ = ([(f, C.c_void_p) for f in ("x", "gamma", "beta", "y", "stats", "dy", "dx", "dx_drop", "rng", "keep_bits",
+                                           "scratch", "dgamma", "dbeta")] +
+                [("rows", C.c_int64), ("scratch_floats", C.c_int64), ("D", C.c_int32), ("keep_ld", C.c_int32),
+                 ("eps", C.c_float), ("drop_p", C.c_float), ("site", C.c_uint32)] +
+                [(f, C.c_int32) for f in ("forward", "backward", "fwd_class", "bwd_class", "chunks", "keep_source")])
+
+
+RD_LN_GENERIC, RD_LN_VEC1, RD_LN_VEC2, RD_LN_VEC5, RD_LN_SPLIT_VEC, RD_LN_SPLIT_SCALAR = 0, 1, 2, 5, 16, 17
+RD_LN_KEEP_NONE, RD_LN_KEEP_PHILOX, RD_LN_KEEP_BITS = 0, 1, 2
+
+
 # name -> (restype, argtypes); every symbol include/raindrop_b200.h declares
 SIGNATURES = {
     "rd_abi_version": (C.c_int, []),
@@ -274,6 +286,11 @@ SIGNATURES = {
     "rd_debug_per_sample_linear": (C.c_int, [C.POINTER(RdDebugPerSampleItem), C.c_int32, C.c_int32, C.c_int32,
                                              C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64,
                                              C.c_float, C.POINTER(RdDebugPerSamplePlan), C.c_void_p]),
+    "rd_debug_layernorm_scratch_floats": (C.c_int64, [C.c_int64, C.c_int32]),
+    "rd_debug_layernorm": (C.c_int, [C.POINTER(RdDebugLayernormArgs), C.c_void_p]),
+    "rd_debug_per_sample_layernorm": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                                C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p]),
     "rd_kfac_factors_doubles": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_ekfac_bases_floats": (C.c_int64, [C.POINTER(RdDims)]),
     "rd_kfac_factors_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),

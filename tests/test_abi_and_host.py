@@ -44,6 +44,7 @@ def test_struct_layout_matches_header_sizes():
     assert C.sizeof(L.RdDebugWgradPlan) == 4 * 2 + 4 * 24
     assert C.sizeof(L.RdDebugPerSampleItem) == 8 * 2 + 8 * 6 + 4 * 6
     assert C.sizeof(L.RdDebugPerSamplePlan) == 4 * 4
+    assert C.sizeof(L.RdDebugLayernormArgs) == 8 * 13 + 8 * 2 + 4 * 5 + 4 * 6 + 4
 
 
 def test_workspace_queries_are_pure_host_code():

@@ -966,6 +966,32 @@ int rd_fisher_labels(const float* logits, int32_t B, int32_t n_classes, uint64_t
 /* debug: out[i] = U(seed, index0 + i) (fp64, device) for i < n. */
 int rd_debug_fisher_uniforms(uint64_t seed, uint64_t index0, int32_t n, double* out, void* stream);
 
+/* ---- TRAK (Park et al. 2023) ------------------------------------------------------------------------------------------
+ * tau(q, i) = [(1/M) sum_k sum_j w_kj (phi_k(q) v_kj)(phi_k(z_i) v_kj)] [(1/M) sum_k Q_k(i)], phi = the projected margin
+ * gradient rows (rd_grad_projection of rows seeded by rd_trak_margin_seed), K = Phi^T Phi = V diag(lambda) V^T over the
+ * training set, w = 1 / (lambda + damping), Q = sigmoid(-margin).  dim: a multiple of 128 in [128, RD_TRAK_DIM_MAX]. */
+#define RD_TRAK_DIM_MAX 8192
+/* The margin seed: for each b < B, with m_b = z_y - log sum_{c != y} exp(z_c) (z = logits[b], y = y[b]),
+ * d_logits[b, y] = 1 / B and d_logits[b, c] = -exp(z_c - M) / S / B for c != y (M = max_{c != y} z_c, S =
+ * sum_{c != y} exp(z_c - M)), the gradient of m_b / B as rd_raindrop_v2_fwd writes the loss's, so that
+ * rd_raindrop_v2_per_sample_grads on an eval forward without labels gives grad_theta m_b; Q[b] = sigmoid(-m_b) (fp64).
+ * Everything in fp64, d_logits rounded to fp32 once: saturated rows stay finite and Q >= 0 without cancellation.
+ * n_classes >= 2; labels outside [0, n_classes) give NaN rows.  Stream-ordered, sync-free. */
+int rd_trak_margin_seed(const float* logits, int32_t B, int32_t n_classes, const int64_t* y, float* d_logits, double* Q,
+                        void* stream);
+/* K[i, j] += sum_{r < n} Phi[r, i] Phi[r, j] for i, j < dim (fp64, device, [dim, dim] row-major).  Phi [n, dim]: fp32,
+ * device, 16-byte aligned.  One launch of 64 x 64 tiles over the upper triangle, mma.sync m16n8k16 f64 (the products of
+ * fp32 inputs are exact in fp64) summed over 32-row k-blocks in row order; each tile is added at (bi, bj) and its
+ * transpose at (bj, bi), a diagonal tile's upper triangle on both sides, so K stays exactly symmetric when it was.  The
+ * order of every sum is fixed by (n, dim) alone and there are no atomics: bitwise reproducible.  Stream-ordered,
+ * sync-free. */
+int rd_trak_gram(const float* Phi, int64_t n, int32_t dim, double* K, void* stream);
+/* out[r, j] = fp32(sum_k Phi[r, k] V[k, j]) for r < n, j < dim.  Phi [n, dim] fp32, V [dim, dim] fp64 row-major, out
+ * [n, dim] fp32 (device, 16-byte aligned, n <= 65535 * 64).  mma.sync m16n8k16 f64 over 32-column k-blocks in order,
+ * rounded once: a row's output depends on its row of Phi and on V alone, whatever the other rows of the launch.
+ * Stream-ordered, sync-free. */
+int rd_trak_rotate(const float* Phi, int64_t n, int32_t dim, const double* V, float* out, void* stream);
+
 /* ---- Laplace approximation (MacKay 1992; Ritter et al. 2018; Daxberger et al. 2021) ----------------------------------
  * Posterior N(theta*, H^-1), H = n F + delta I with F the EK-FAC Fisher above: diagonal in the Kronecker eigenbasis,
  * n Lambda_j + delta.  The linearised predictive of sample b is f ~ N(f(x_b; theta*), Sigma_b) over its logits, with

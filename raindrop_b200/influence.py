@@ -23,6 +23,11 @@ sketches, an unbiased estimate of tracin's scores whose variance falls as 1 / di
 EK-FAC influence functions (George et al. 2018; Grosse et al. 2023): ekfac_factors() computes the Kronecker-factored
 Fisher of every encoder and ob-prop linear layer and its eigenbases once; ekfac_influence() scores
 g_q^T (F + lambda I)^-1 g_t with the rows rotated into those bases on the device (rd_raindrop_v2_ekfac_rows).
+
+TRAK (Park et al. 2023): trak_features() projects the margin gradient rows of a training set (per_sample_margin_grads)
+as TracIn-RP does, per ensemble member, and computes their fp64 Gram (rd_trak_gram), its eigenbasis and the features
+rotated into it (rd_trak_rotate); trak() scores queries against them with the inverse Gram and the training samples'
+1 - p weights.
 """
 import ctypes as C
 import hashlib
@@ -113,23 +118,30 @@ def _row_batch(lib, plan, ldg, cap=DEFAULT_SCRATCH_BYTES):
     return r
 
 
-def _rows_aligned(model, fetch, i0, i1, R, ldg):
-    """Rows of samples [i0, i1) (i0 a multiple of R), computed in batches [k R, (k + 1) R)."""
-    G = None
+def _rows_aligned(model, fetch, i0, i1, R, ldg, margin=False):
+    """Rows of samples [i0, i1) (i0 a multiple of R), computed in batches [k R, (k + 1) R).  margin: (rows, Q) as _rows
+    returns them."""
+    G = Q = None
     for s0 in range(i0, i1, R):
         s1 = min(i1, s0 + R)
-        g = _rows(model, *fetch(s0, s1), ldg)
+        g = _rows(model, *fetch(s0, s1), ldg, margin)
+        g, q = g if margin else (g, None)
         if G is None:
             if s1 == i1:
-                return g
+                return (g, q) if margin else g
             G = torch.empty(i1 - i0, ldg, dtype=torch.float32, device=g.device)
+            Q = torch.empty(i1 - i0, dtype=torch.float64, device=g.device) if margin else None
         G[s0 - i0:s1 - i0] = g
+        if margin:
+            Q[s0 - i0:s1 - i0] = q
         del g
-    return G
+    return (G, Q) if margin else G
 
 
-def _rows(model, src, static, times, lengths, y, ldg):
-    """[B, ldg] float32 gradient rows of CrossEntropy(logits_b, y_b); y None: the predicted class (argmax of the logits)."""
+def _rows(model, src, static, times, lengths, y, ldg, margin=False):
+    """[B, ldg] float32 gradient rows of CrossEntropy(logits_b, y_b); y None: the predicted class (argmax of the logits).
+    margin: the rows of the margin m_b = z_y - log sum_{c != y} exp(z_c) instead, seeded by rd_trak_margin_seed on the
+    eval forward without labels, returned with Q [B] = sigmoid(-m_b) float64."""
     cl = _Call(model, src, static, times, lengths, None, False)
     lib, plan, dev = cl.lib, cl.plan, cl.device
     B = cl.x.shape[1]
@@ -146,16 +158,24 @@ def _rows(model, src, static, times, lengths, y, ldg):
                                        logits.data_ptr(), L.ptr(yv), L.ptr(None if yv is None else loss),
                                        L.ptr(None if yv is None else dlog), st), "rd_raindrop_v2_fwd")
 
-    if y is None:
+    Q = None
+    if margin:
         fwd(None)
-        y = logits.argmax(dim=1)
-    fwd(y.to(device=dev, dtype=torch.int64).contiguous())
+        yv = (logits.argmax(dim=1) if y is None else y).to(device=dev, dtype=torch.int64).contiguous()
+        Q = torch.empty(B, dtype=torch.float64, device=dev)
+        L.check(lib.rd_trak_margin_seed(logits.data_ptr(), B, plan.n_classes, yv.data_ptr(), dlog.data_ptr(),
+                                        Q.data_ptr(), st), "rd_trak_margin_seed")
+    else:
+        if y is None:
+            fwd(None)
+            y = logits.argmax(dim=1)
+        fwd(y.to(device=dev, dtype=torch.int64).contiguous())
     G = torch.empty(B, ldg, **f32)
     scratch = cl.scratch("_psg_scratch", key, lib.rd_per_sample_grads_scratch_bytes(C.byref(dims)))
     L.check(lib.rd_raindrop_v2_per_sample_grads(C.byref(dims), C.byref(cl.params), L.ptr(cl.st), cl.ln.data_ptr(),
                                                 plan.node_scale.data_ptr(), ws.data_ptr(), dlog.data_ptr(), scratch.data_ptr(),
                                                 G.data_ptr(), ldg, st), "rd_raindrop_v2_per_sample_grads")
-    return G
+    return (G, Q) if margin else G
 
 
 def _check_labels(y, B, n_classes, allow_none=False):
@@ -183,6 +203,24 @@ def per_sample_grads(model, src, static, times, lengths, y):
     y = _check_labels(y, src.shape[1], model._plan.n_classes)
     with torch.no_grad():
         return _rows(model, src, static, times, lengths, y, _bucket_length(grad_layout(model)))
+
+
+def per_sample_margin_grads(model, src, static, times, lengths, y=None):
+    """(G [B, bucket] float32, Q [B] float64) on the device: row b = the gradient of the margin
+    m_b = z_y - log sum_{c != y} exp(z_c) of the eval logits z (y None: the predicted class) with respect to every trained
+    tensor, laid out as per_sample_grads; Q_b = 1 - p_y = sigmoid(-m_b).  The loss rows are -Q times these, since
+    d CE / d logits = -Q d m / d logits.  The model needs 2 classes or more.  Eval mode only; parameters and their .grad
+    are left unchanged.  Raises RaindropB200Error without CUDA or without the built library."""
+    _check_call("per_sample_margin_grads", model, src, static, None, None)
+    y = _check_labels(y, src.shape[1], model._plan.n_classes, allow_none=True)
+    _check_margin_classes(model)
+    with torch.no_grad():
+        return _rows(model, src, static, times, lengths, y, _bucket_length(grad_layout(model)), margin=True)
+
+
+def _check_margin_classes(model):
+    if model._plan.n_classes < 2:
+        raise ValueError("the margin needs a model of 2 classes or more")
 
 
 # ---- data sources: a dict of tensors, or a DeviceDataset (optionally with an index subset) ----------------------------
@@ -554,13 +592,19 @@ def project(model, data, checkpoints=None, dim=4096, seed=0, fields=None, intern
             for i0 in range(0, n, chunk):
                 i1 = min(n, i0 + chunk)
                 G = _rows_aligned(model, fetch, i0, i1, R, ldg)
-                nb = lib.rd_grad_projection_scratch_bytes(i1 - i0, ldg, dim, n_seg)
-                sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
-                L.check(lib.rd_grad_projection(G.data_ptr(), i1 - i0, ldg, offs, lens, n_seg, dim, seed,
-                                               features[c, i0:i1].data_ptr(), dim, sc.data_ptr(), st), "rd_grad_projection")
-                del G, sc
+                _project_rows(lib, G, ldg, offs, lens, n_seg, dim, seed, features[c, i0:i1], st)
+                del G
     return GradientSketch(features=features, lrs=tuple(lr for _, lr in ckpts), dim=dim, seed=seed, fields=sel_fields,
                           layout=tuple((k, tuple(s)) for k, _, s in layout), fingerprints=tuple(prints))
+
+
+def _project_rows(lib, G, ldg, offs, lens, n_seg, dim, seed, out, st):
+    """out [rows, dim] (a contiguous float32 view) = rd_grad_projection of the rows G [rows, ldg]."""
+    rows = G.shape[0]
+    nb = lib.rd_grad_projection_scratch_bytes(rows, ldg, dim, n_seg)
+    sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=G.device)
+    L.check(lib.rd_grad_projection(G.data_ptr(), rows, ldg, offs, lens, n_seg, dim, seed, out.data_ptr(), dim,
+                                   sc.data_ptr(), st), "rd_grad_projection")
 
 
 def _check_sketches(q, t):
@@ -1065,3 +1109,322 @@ def ekfac_from_grads(Gq, Gt, factors, damping=None):
     if Gq.ndim != 2 or Gt.ndim != 2 or Gq.shape[1] != w.shape[0] or Gt.shape[1] != w.shape[0]:
         raise ValueError("Gq [q, %d] and Gt [t, %d] do not match: %s, %s" % (w.shape[0], w.shape[0], Gq.shape, Gt.shape))
     return (ekfac_rotate(Gq, factors) * w) @ ekfac_rotate(Gt, factors).T
+
+
+# ---- TRAK (Park et al. 2023) -------------------------------------------------------------------------------------------
+TRAK_DIM_MAX = L.TRAK_DIM_MAX
+
+
+@dataclass
+class TRAKFeatures:
+    """TRAK features of a training set (trak_features), one block per model k (an ensemble member's weights):
+    features [M, n, dim] float32, the projected margin rows rotated into the eigenbasis of their Gram, Phi_k V_k;
+    eigenvalues [M, dim] float64 (ascending) and eigenvectors V [M, dim, dim] float64 of K_k = Phi_k^T Phi_k; Q [M, n]
+    float64 = sigmoid(-margin) of each training sample under each model.  Omega is rd_grad_projection's +-1 matrix for
+    `seed`; scoring (trak) refuses features whose dim, fields, layout or weight fingerprints (sha256 of each model's
+    trained tensors) do not match the model and checkpoints it is given."""
+    features: torch.Tensor
+    eigenvalues: torch.Tensor
+    eigenvectors: torch.Tensor
+    Q: torch.Tensor
+    dim: int
+    seed: int
+    fields: tuple            # None: every trained tensor
+    layout: tuple            # ((state-dict key, shape), ...) of the gradient rows
+    fingerprints: tuple      # sha256 hex digest per model
+
+    def save(self, path):
+        torch.save(dict(features=self.features.detach().cpu(), eigenvalues=self.eigenvalues.detach().cpu(),
+                        eigenvectors=self.eigenvectors.detach().cpu(), Q=self.Q.detach().cpu(), dim=self.dim,
+                        seed=self.seed, fields=None if self.fields is None else list(self.fields),
+                        layout=[[k, list(s)] for k, s in self.layout], fingerprints=list(self.fingerprints)), path)
+
+    @classmethod
+    def load(cls, path, map_location=None):
+        d = torch.load(path, map_location=map_location, weights_only=True)
+        return cls(features=d["features"], eigenvalues=d["eigenvalues"], eigenvectors=d["eigenvectors"], Q=d["Q"],
+                   dim=int(d["dim"]), seed=int(d["seed"]), fields=None if d["fields"] is None else tuple(d["fields"]),
+                   layout=tuple((k, tuple(int(x) for x in s)) for k, s in d["layout"]),
+                   fingerprints=tuple(d["fingerprints"]))
+
+
+def _check_trak_dim(dim, seed):
+    if isinstance(dim, bool) or not isinstance(dim, (int, np.integer)):
+        raise ValueError("dim must be an integer")
+    if dim % PROJECTION_DIM_MULTIPLE or not PROJECTION_DIM_MULTIPLE <= dim <= TRAK_DIM_MAX:
+        raise ValueError("dim must be a multiple of %d in [%d, %d] (the Gram and its eigenvectors are dim^2 float64 per "
+                         "model), got %d" % (PROJECTION_DIM_MULTIPLE, PROJECTION_DIM_MULTIPLE, TRAK_DIM_MAX, dim))
+    _check_projection(int(dim), seed)
+
+
+def _check_trak_regularisation(damping, rcond):
+    """(damping, rcond) as floats: damping finite >= 0; rcond None (dim * 2^-52 at use) or finite >= 0."""
+    out = []
+    for name, v in (("damping", damping), ("rcond", rcond)):
+        if v is None and name == "rcond":
+            out.append(None)
+            continue
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)):
+            raise ValueError("%s must be a float >= 0" % name)
+        f = float(v)
+        if not (math.isfinite(f) and f >= 0):
+            raise ValueError("%s must be a finite float >= 0, got %r" % (name, v))
+        out.append(f)
+    return tuple(out)
+
+
+def trak_weights(eigenvalues, damping=0.0, rcond=None):
+    """float64 numpy [M, dim]: w_kj = 1 / (lambda_kj + damping), and 0 where lambda_kj <= rcond * max_j lambda_kj
+    (rcond None: dim * 2^-52, the usual pseudo-inverse rule, so rank-deficient sketches work)."""
+    damping, rcond = _check_trak_regularisation(damping, rcond)
+    lam = np.atleast_2d(np.asarray(eigenvalues.detach().cpu() if torch.is_tensor(eigenvalues) else eigenvalues,
+                                   dtype=np.float64))
+    rc = lam.shape[1] * 2.0 ** -52 if rcond is None else rcond
+    keep = lam > rc * lam.max(axis=1, keepdims=True)
+    return np.where(keep, 1.0 / np.where(keep, lam + damping, 1.0), 0.0)
+
+
+def _trak_models(model, checkpoints):
+    """[(state_dict or None, 1.0)] of the ensemble: checkpoints is None (the current weights) or a list of state dicts."""
+    from collections.abc import Mapping
+    if checkpoints is None:
+        return _checkpoints(model, None)
+    if isinstance(checkpoints, Mapping) or not all(isinstance(sd, Mapping) for sd in checkpoints):
+        raise ValueError("checkpoints must be a list of state dicts (one per model)")
+    return _checkpoints(model, [(sd, 1.0) for sd in checkpoints])
+
+
+def _model_fingerprints(model, ckpts):
+    keys = [k for k, _ in model._plan.fields]
+    return tuple(_fingerprint(model.used_parameters() if sd is None else [sd[k] for k in keys]) for sd, _ in ckpts)
+
+
+def _trak_chunk(lib, plan, ldg, dim, n_seg, n, R, internal_batch_size, cap=DEFAULT_SCRATCH_BYTES):
+    """Rows per chunk of the margin rows: a multiple of R (internal_batch_size rounded up to one; default the largest
+    whose rows, row buffers, projection scratch and projected / rotated rows fit in `cap`)."""
+    if internal_batch_size is not None:
+        return max(R, (int(internal_batch_size) + R - 1) // R * R)
+    return max(R, _largest_chunk(lambda b: 4 * b * ldg + _rows_bytes(lib, plan, min(b, R), ldg) + 8 * b * dim +
+                                 lib.rd_grad_projection_scratch_bytes(b, ldg, dim, n_seg), max(n, 1), cap) // R * R)
+
+
+def _trak_sketch(model, fetch, n, dim, seed, seg, chunk, R, ldg):
+    """(Phi [n, dim] float32, Q [n] float64) of the current weights: the margin rows of samples [0, n), projected by
+    rd_grad_projection chunk by chunk (the full rows of the set are never held)."""
+    lib, dev = L.load(), model._plan.node_scale.device
+    offs, lens, n_seg = seg
+    Phi = torch.empty(n, dim, dtype=torch.float32, device=dev)
+    Q = torch.empty(n, dtype=torch.float64, device=dev)
+    st = L.stream_ptr(dev)
+    for i0 in range(0, n, chunk):
+        i1 = min(n, i0 + chunk)
+        G, Q[i0:i1] = _rows_aligned(model, fetch, i0, i1, R, ldg, margin=True)
+        _project_rows(lib, G, ldg, offs, lens, n_seg, dim, seed, Phi[i0:i1], st)
+        del G
+    return Phi, Q
+
+
+def _trak_gram(Phi):
+    """K = Phi^T Phi [dim, dim] float64 on the device (rd_trak_gram: one pass, rows in order, exactly symmetric)."""
+    n, dim = Phi.shape
+    K = torch.zeros(dim, dim, dtype=torch.float64, device=Phi.device)
+    L.check(L.load().rd_trak_gram(Phi.data_ptr(), n, dim, K.data_ptr(), L.stream_ptr(Phi.device)), "rd_trak_gram")
+    return K
+
+
+def _trak_eigh(K):
+    """(lambda ascending, V) of K by torch.linalg.eigh in float64 on K's device, each eigenvector's largest-magnitude
+    component made positive (the first such component on ties), so the basis is reproducible."""
+    lam, V = torch.linalg.eigh(K)
+    i = V.abs().argmax(dim=0)
+    sign = torch.where(V.gather(0, i[None]).squeeze(0) < 0, -1.0, 1.0).to(V.dtype)
+    return lam, (V * sign).contiguous()
+
+
+def _trak_rotate(Phi, V, out=None):
+    """Phi V [n, dim] float32 on the device (rd_trak_rotate: fp64 products and sums, one rounding per element)."""
+    n, dim = Phi.shape
+    out = torch.empty(n, dim, dtype=torch.float32, device=Phi.device) if out is None else out
+    L.check(L.load().rd_trak_rotate(Phi.data_ptr(), n, dim, V.data_ptr(), out.data_ptr(), L.stream_ptr(Phi.device)),
+            "rd_trak_rotate")
+    return out
+
+
+def trak_features(model, train, checkpoints=None, dim=4096, seed=0, fields=None, internal_batch_size=None):
+    """TRAKFeatures of `train` (tracin's train argument: a dict with y, a DeviceDataset or (DeviceDataset, indices)).
+    Per model k (checkpoints: a list of state dicts holding the trained tensors, e.g. independently seeded runs; default
+    the current weights): the margin gradient rows of every training sample with its label (per_sample_margin_grads, in
+    tracin's row batches), projected onto `dim` +-1 directions (rd_grad_projection; phi = g Omega / sqrt(dim)), their fp64
+    Gram K (rd_trak_gram), its eigendecomposition (torch.linalg.eigh in float64 on the device) and the features rotated
+    into that basis (rd_trak_rotate).  fields: as for tracin.  dim: a multiple of 128 in [128, 8192] (K and V are dim^2
+    float64 per model).  internal_batch_size: rows per chunk, rounded up to a multiple of the row batch.  The result is
+    bitwise the same for any internal_batch_size, data source or run.  The weights, mode and dropout counter are
+    restored.  Eval mode only."""
+    _check_trak_dim(dim, seed)
+    _check_data(model, train, "train", allow_none_y=False)
+    _check_batch_size(internal_batch_size)
+    if model.training:
+        raise ValueError("trak_features runs the model in eval arithmetic: call model.eval() first")
+    _check_margin_classes(model)
+    dim, seed = int(dim), int(seed)
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    seg = _segments(*plan_segments(layout, fields))
+    ckpts = _trak_models(model, checkpoints)
+    dev = _data_device(train)
+    lib = L.load()
+    plan = model._prepare(dev)
+    n, fetch = _source(train, "train")
+    M = len(ckpts)
+    R = _row_batch(lib, plan, ldg)
+    chunk = _trak_chunk(lib, plan, ldg, dim, seg[2], n, R, internal_batch_size)
+    features = torch.empty(M, n, dim, dtype=torch.float32, device=dev)
+    lam = torch.empty(M, dim, dtype=torch.float64, device=dev)
+    V = torch.empty(M, dim, dim, dtype=torch.float64, device=dev)
+    Q = torch.empty(M, n, dtype=torch.float64, device=dev)
+    prints = []
+    with torch.no_grad(), _Weights(model) as w:
+        for k, (sd, _) in enumerate(ckpts):
+            if sd is not None:
+                w.load(sd)
+            prints.append(_fingerprint(w.params))
+            Phi, Q[k] = _trak_sketch(model, fetch, n, dim, seed, seg, chunk, R, ldg)
+            lam[k], V[k] = _trak_eigh(_trak_gram(Phi))
+            _trak_rotate(Phi, V[k], out=features[k])
+            del Phi
+    return TRAKFeatures(features=features, eigenvalues=lam, eigenvectors=V, Q=Q, dim=dim, seed=seed,
+                        fields=None if fields is None else tuple(fields),
+                        layout=tuple((k, tuple(s)) for k, _, s in layout), fingerprints=tuple(prints))
+
+
+def _check_trak_features(model, features, ckpts):
+    if not isinstance(features, TRAKFeatures):
+        raise TypeError("features must be a TRAKFeatures (trak_features)")
+    layout = tuple((k, tuple(s)) for k, _, s in grad_layout(model))
+    if features.layout != layout:
+        raise ValueError("the features were computed for a model of another layout")
+    if features.fields is not None:
+        _selected(grad_layout(model), list(features.fields))
+    _check_trak_dim(features.dim, features.seed)
+    M, dim = len(features.fingerprints), features.dim
+    F, lam, V, Q = features.features, features.eigenvalues, features.eigenvectors, features.Q
+    if F.dim() != 3 or tuple(F.shape[::2]) != (M, dim) or tuple(lam.shape) != (M, dim) or \
+            tuple(V.shape) != (M, dim, dim) or tuple(Q.shape) != (M, F.shape[1]):
+        raise ValueError("features [M, n, dim], eigenvalues [M, dim], eigenvectors [M, dim, dim] and Q [M, n] do not "
+                         "match M = %d, dim = %d" % (M, dim))
+    if len(ckpts) != M:
+        raise ValueError("the features hold %d models; %d were given" % (M, len(ckpts)))
+    prints = _model_fingerprints(model, ckpts)
+    for k, (a, b) in enumerate(zip(prints, features.fingerprints)):
+        if a != b:
+            raise ValueError("the features of model %d were computed for other weights (fingerprint %s..., the "
+                             "weights' %s...)" % (k, b[:12], a[:12]))
+
+
+def trak(model, query, features, damping=0.0, rcond=None, internal_batch_size=None, checkpoints=None):
+    """TRAK scores [n_query, n_train] float64 on the device:
+        tau(q, i) = [(1/M) sum_k sum_j w_kj phi~_k(q)_j phi~_k(z_i)_j] [(1/M) sum_k Q_k(i)],
+    w_kj = 1 / (lambda_kj + damping) (0 where lambda_kj <= rcond max lambda_k; trak_weights), phi~ = the projected margin
+    rows rotated into each model's eigenbasis.  Positive = proponent, as for tracin.  query: dict (y None = each model's
+    predicted class).  checkpoints: the state dicts the features were computed with (default: the current weights, one
+    model); features of other weights, layout, fields or dim are refused on the host.  Per model and query block: the
+    margin rows (tracin's row batches), rd_grad_projection, rd_trak_rotate, rd_ekfac_scale_rows by w (fp32), and
+    rd_per_sample_grad_dot with alpha = 1/M into the fp64 scores, whose columns are then scaled by the mean Q.  Bitwise
+    the same for any internal_batch_size, data source or run.  The weights, mode and dropout counter are restored."""
+    if not isinstance(query, dict):
+        raise TypeError("query must be a dict (src, static, times, lengths, y)")
+    _check_data(model, query, "query", allow_none_y=True)
+    _check_batch_size(internal_batch_size)
+    damping, rcond = _check_trak_regularisation(damping, rcond)
+    if model.training:
+        raise ValueError("trak runs the model in eval arithmetic: call model.eval() first")
+    _check_margin_classes(model)
+    ckpts = _trak_models(model, checkpoints)
+    _check_trak_features(model, features, ckpts)
+    dim, seed, M = features.dim, features.seed, len(ckpts)
+    layout = grad_layout(model)
+    ldg = _bucket_length(layout)
+    seg = _segments(*plan_segments(layout, None if features.fields is None else list(features.fields)))
+    dev = _data_device(query)
+    lib = L.load()
+    plan = model._prepare(dev)
+    nq, q_fetch = _source(query, "query")
+    nt = features.features.shape[1]
+    scores = torch.zeros(nq, nt, dtype=torch.float64, device=dev)
+    if nq == 0 or nt == 0:
+        return scores
+    W = torch.from_numpy(trak_weights(features.eigenvalues, damping, rcond)).to(device=dev, dtype=torch.float32)
+    Ft = features.features.to(device=dev, dtype=torch.float32).contiguous()
+    R = _row_batch(lib, plan, ldg)
+    qb = _trak_chunk(lib, plan, ldg, dim, seg[2], nq, R, internal_batch_size)
+    dot_off, dot_len, dot_n = _segments(np.arange(0, dim, SEGMENT, dtype=np.int64),
+                                        np.minimum(SEGMENT, dim - np.arange(0, dim, SEGMENT, dtype=np.int64)))
+    tc = _largest_chunk(lambda b: lib.rd_per_sample_grad_dot_scratch_bytes(min(qb, nq), b, dim, dot_n), nt)
+    whole = _segments(np.zeros(1, np.int64), np.full(1, dim, np.int64))
+    st = L.stream_ptr(dev)
+    with torch.no_grad(), _Weights(model) as w:
+        for k, (sd, _) in enumerate(ckpts):
+            if sd is not None:
+                w.load(sd)
+            V = features.eigenvectors[k].to(device=dev, dtype=torch.float64).contiguous()
+            for q0 in range(0, nq, qb):
+                q1 = min(nq, q0 + qb)
+                Phi, _ = _trak_sketch(model, lambda a, b: q_fetch(q0 + a, q0 + b), q1 - q0, dim, seed, seg, qb, R, ldg)
+                Pr = _trak_rotate(Phi, V)
+                del Phi
+                L.check(lib.rd_ekfac_scale_rows(Pr.data_ptr(), q1 - q0, dim, *whole, W[k].data_ptr(), st),
+                        "rd_ekfac_scale_rows")
+                for t0 in range(0, nt, tc):
+                    t1 = min(nt, t0 + tc)
+                    nb = lib.rd_per_sample_grad_dot_scratch_bytes(q1 - q0, t1 - t0, dim, dot_n)
+                    sc = torch.empty((nb + 3) // 4, dtype=torch.float32, device=dev)
+                    L.check(lib.rd_per_sample_grad_dot(Pr.data_ptr(), q1 - q0, Ft[k, t0].data_ptr(), t1 - t0, dim,
+                                                       dot_off, dot_len, dot_n, 1.0 / M,
+                                                       scores.data_ptr() + 8 * (q0 * nt + t0), nt, sc.data_ptr(), st),
+                            "rd_per_sample_grad_dot")
+                    del sc
+                del Pr
+    scores *= features.Q.to(device=dev, dtype=torch.float64).mean(dim=0)[None, :]
+    return scores
+
+
+def trak_self_influence(features, damping=0.0, rcond=None):
+    """[n] float64 on the device: the leverages (1/M) sum_k sum_j w_kj phi~_k(z_i)_j^2 times the mean Q of each training
+    sample, the diagonal of trak(train, train) with each model's labels on both sides (to rounding: this sums the
+    float32 features' squares in float64).  With one model and damping 0 the leverage (before Q) lies in [0, 1] and the
+    leverages sum to the rank of the sketch; large values flag candidate mislabels or outliers, as self_influence."""
+    if not isinstance(features, TRAKFeatures):
+        raise TypeError("features must be a TRAKFeatures (trak_features)")
+    _check_trak_regularisation(damping, rcond)
+    F = features.features
+    if F.device.type != "cuda":
+        raise L.RaindropB200Error("trak_self_influence runs on a CUDA device; the features are on %s" % F.device)
+    W = torch.from_numpy(trak_weights(features.eigenvalues, damping, rcond)).to(F.device)
+    M, n = F.shape[0], F.shape[1]
+    out = torch.zeros(n, dtype=torch.float64, device=F.device)
+    step = max(1, (1 << 27) // max(1, features.dim))
+    for k in range(M):
+        for i0 in range(0, n, step):
+            out[i0:i0 + step] += F[k, i0:i0 + step].double().square() @ W[k]
+    return out / M * features.Q.to(F.device).double().mean(dim=0)
+
+
+def trak_from_features(Fq, Ft, Q, damping=0.0, rcond=None):
+    """Host restatement of trak in float64: Fq [M, n_query, dim] and Ft [M, n_train, dim] projected (unrotated) margin
+    features, Q [M, n_train] (2-D / 1-D arrays: one model) -> [n_query, n_train]: per model the eigendecomposition of
+    Ft^T Ft (numpy eigh), the weights trak_weights(lambda, damping, rcond), the weighted products of the rotated
+    features averaged over models, times the mean Q of each training sample."""
+    Fq, Ft, Q = (np.asarray(a, dtype=np.float64) for a in (Fq, Ft, Q))
+    if Fq.ndim == 2:
+        Fq, Ft, Q = Fq[None], Ft[None], Q[None]
+    if Fq.ndim != 3 or Ft.ndim != 3 or Q.ndim != 2 or Fq.shape[0] != Ft.shape[0] or Fq.shape[2] != Ft.shape[2] or \
+            Q.shape != Ft.shape[:2]:
+        raise ValueError("Fq [M, q, dim], Ft [M, t, dim] and Q [M, t] do not match: %s, %s, %s"
+                         % (Fq.shape, Ft.shape, Q.shape))
+    M = Fq.shape[0]
+    S = np.zeros((Fq.shape[1], Ft.shape[1]))
+    for k in range(M):
+        lam, V = np.linalg.eigh(Ft[k].T @ Ft[k])
+        w = trak_weights(lam[None], damping, rcond)[0]
+        S += ((Fq[k] @ V) * w) @ (Ft[k] @ V).T
+    return S / M * Q.mean(axis=0)[None, :]

@@ -22,6 +22,14 @@ eigendecompositions and the Lambda pass (the rest of ekfac_factors), and the sco
 extrapolated).  The rotations' cost is the difference between the rotated and the plain row passes over those samples.
 
     python tools/bench_tracin.py --shape P19 --n-query 3880 --n-train 31000 --ekfac
+
+--trak times TRAK instead (influence.trak_features / trak, one model): the margin rows plus their projection, the fp64
+Gram kernel (rd_trak_gram), torch.linalg.eigh in float64, the rotation kernel (rd_trak_rotate) and the scoring of
+n_query queries, each on its own.  On the same Phi it times the cuBLAS DGEMM Phi.double().T @ Phi.double(), with and
+without the conversion, and reports the FP64 TFLOP/s of both (2 n dim^2 for the full product, the Gram kernel's
+issued triangle tiles apart) with the card's name and power limit.
+
+    python tools/bench_tracin.py --shape P19 --n-query 128 --n-train 31000 --trak --projection 4096
 """
 import argparse
 import ctypes as C
@@ -292,6 +300,59 @@ def run_ekfac(shape, nq, nt, exact_nt):
                 scores_finite=bool(torch.isfinite(S).all()))
 
 
+def run_trak(shape, nq, nt, dim, reps=5):
+    cfg = model_config(shape, dropout=0.2)
+    model = build_dropin(cfg, 21)
+    model.eval()
+    dq = to_dev(make_batch(cfg, nq, seed=1))
+    dt = make_batch(cfg, nt, seed=2)
+    ds = DeviceDataset(dt["src"], dt["static"], dt["times"], dt["y"])
+    q = dict(src=dq["src"], static=dq["static"], times=dq["times"], lengths=dq["lengths"], y=None)
+    warm = (ds, torch.arange(min(nt, 256)))
+    IF.trak(model, q, IF.trak_features(model, warm, dim=dim), damping=1e-3)                              # warm-up
+
+    def timed(fn, n=1):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(n):
+            out = fn()
+        torch.cuda.synchronize()
+        return out, (time.perf_counter() - t0) / n
+    lib, plan = L.load(), model._plan
+    layout = IF.grad_layout(model)
+    ldg = IF._bucket_length(layout)
+    seg = IF._segments(*IF.plan_segments(layout))
+    R = IF._row_batch(lib, plan, ldg)
+    chunk = IF._trak_chunk(lib, plan, ldg, dim, seg[2], nt, R, None)
+    n, fetch = IF._source(ds, "train")
+    with torch.no_grad():
+        (Phi, Q), t_rows = timed(lambda: IF._trak_sketch(model, fetch, n, dim, 0, seg, chunk, R, ldg))
+    IF._trak_gram(Phi)
+    K, t_gram = timed(lambda: IF._trak_gram(Phi), reps)
+    (lam, V), t_eigh = timed(lambda: IF._trak_eigh(K))
+    Pr, t_rot = timed(lambda: IF._trak_rotate(Phi, V), reps)
+    Pd = Phi.double()
+    Kd, t_dgemm = timed(lambda: Pd.T @ Pd, reps)
+    _, t_dgemm_conv = timed(lambda: Phi.double().T @ Phi.double(), reps)
+    gram_err = ((K - Kd).norm() / Kd.norm()).item()
+    del Pd, Kd
+    feats, t_features = timed(lambda: IF.trak_features(model, ds, dim=dim))
+    assert torch.equal(feats.features[0], Pr) and torch.equal(feats.eigenvalues[0], lam), \
+        "the split run must reproduce trak_features bitwise"
+    S, t_score = timed(lambda: IF.trak(model, q, feats))
+    T = dim // 64
+    full = 2.0 * nt * dim * dim
+    issued = 2.0 * (-(-nt // 32) * 32) * 64 * 64 * T * (T + 1) // 2
+    return dict(shape=shape, card=card(), projection_dim=dim, n_query=nq, n_train=nt, bucket=ldg, chunk=chunk,
+                margin_rows_and_projection_s=t_rows, gram_s=t_gram, eigh_s=t_eigh, rotation_s=t_rot,
+                scoring_s=t_score, trak_features_total_s=t_features,
+                gram_fp64_tflops_full_product=full / t_gram / 1e12, gram_fp64_tflops_issued=issued / t_gram / 1e12,
+                dgemm_s=t_dgemm, dgemm_fp64_tflops=full / t_dgemm / 1e12, dgemm_with_conversion_s=t_dgemm_conv,
+                gram_vs_dgemm_rel_diff=gram_err, dgemm_faster=t_dgemm < t_gram,
+                rotation_fp64_tflops=full / t_rot / 1e12, scores_finite=bool(torch.isfinite(S).all()),
+                rank=int((IF.trak_weights(lam) > 0).sum()))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shape", default="P19")
@@ -302,7 +363,11 @@ def main():
     ap.add_argument("--exact-train", type=int, default=1024,
                     help="--projection, --ekfac: train samples of the timed exact (and EK-FAC) scoring calls")
     ap.add_argument("--ekfac", action="store_true", help="time EK-FAC influence functions")
+    ap.add_argument("--trak", action="store_true", help="time TRAK (--projection DIM, default 4096)")
     a = ap.parse_args()
+    if a.trak:
+        print(json.dumps(run_trak(a.shape, a.n_query, a.n_train, a.projection or 4096)), flush=True)
+        return
     if a.ekfac:
         print(json.dumps(run_ekfac(a.shape, a.n_query, a.n_train, a.exact_train)), flush=True)
         return

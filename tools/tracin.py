@@ -23,6 +23,12 @@ self-influence stays exact.
 Fisher at the single checkpoint's weights, preconditioned by its inverse with --damping or 0.1 of each block's mean
 eigenvalue); --save-factors PATH / --load-factors PATH write or reuse the training set's factors.  The files keep their
 names; the self-influence is EK-FAC's sum_j G~_j^2 / (Lambda_j + lambda).
+
+--method trak scores with TRAK instead (influence.trak_features / trak): each --checkpoint is one ensemble member (e.g.
+an independently seeded run), the margin gradients are projected onto --projection DIM directions (default 4096) and
+preconditioned by the inverse Gram of the training features, plus --damping (default 0); --save-features PATH /
+--load-features PATH write or reuse the training set's features.  The files keep their names; the self-influence is
+TRAK's leverage times the mean 1 - p (trak_self_influence).
 """
 import argparse
 import os
@@ -66,9 +72,13 @@ def main():
     ap.add_argument("--projection-seed", type=int, default=0, help="seed of the projection's +-1 directions")
     ap.add_argument("--save-sketch", metavar="PATH", help="--projection: write the training set's sketch here")
     ap.add_argument("--load-sketch", metavar="PATH", help="--projection: reuse this training-set sketch")
-    ap.add_argument("--method", default="tracin", choices=["tracin", "ekfac"],
-                    help="ekfac: EK-FAC influence functions at the first checkpoint's weights (influence.ekfac_*)")
-    ap.add_argument("--damping", type=float, help="--method ekfac: one damping for every block (default 0.1 mean)")
+    ap.add_argument("--method", default="tracin", choices=["tracin", "ekfac", "trak"],
+                    help="ekfac: EK-FAC influence functions at the first checkpoint's weights (influence.ekfac_*); "
+                         "trak: TRAK over the checkpoints as an ensemble (influence.trak_*)")
+    ap.add_argument("--damping", type=float, help="--method ekfac: one damping for every block (default 0.1 mean); "
+                                                  "--method trak: added to every eigenvalue (default 0)")
+    ap.add_argument("--save-features", metavar="PATH", help="--method trak: write the training set's TRAK features here")
+    ap.add_argument("--load-features", metavar="PATH", help="--method trak: reuse these TRAK features")
     ap.add_argument("--save-factors", metavar="PATH", help="--method ekfac: write the training set's EK-FAC factors here")
     ap.add_argument("--load-factors", metavar="PATH", help="--method ekfac: reuse these EK-FAC factors")
     ap.add_argument("--name", help="file name suffix (default: the synthetic configuration or 'dataset')")
@@ -76,15 +86,20 @@ def main():
     args = ap.parse_args()
 
     from raindrop_b200 import data as RD
-    from raindrop_b200.influence import (EKFACFactors, GradientSketch, ekfac_factors, ekfac_influence, ekfac_self_influence,
-                                         project, self_influence, tracin, tracin_sketch)
+    from raindrop_b200.influence import (EKFACFactors, GradientSketch, TRAKFeatures, ekfac_factors, ekfac_influence,
+                                         ekfac_self_influence, project, self_influence, tracin, tracin_sketch, trak,
+                                         trak_features, trak_self_influence)
     from raindrop_b200.synth import make_batch, model_config
     if not torch.cuda.is_available():
         raise SystemExit("tracin runs on a CUDA device")
-    if (args.save_sketch or args.load_sketch) and not args.projection:
-        raise SystemExit("--save-sketch and --load-sketch need --projection")
-    if (args.save_factors or args.load_factors or args.damping is not None) and args.method != "ekfac":
-        raise SystemExit("--save-factors, --load-factors and --damping need --method ekfac")
+    if (args.save_sketch or args.load_sketch) and (not args.projection or args.method != "tracin"):
+        raise SystemExit("--save-sketch and --load-sketch need --projection with --method tracin")
+    if (args.save_factors or args.load_factors) and args.method != "ekfac":
+        raise SystemExit("--save-factors and --load-factors need --method ekfac")
+    if args.damping is not None and args.method == "tracin":
+        raise SystemExit("--damping needs --method ekfac or trak")
+    if (args.save_features or args.load_features) and args.method != "trak":
+        raise SystemExit("--save-features and --load-features need --method trak")
     if args.method == "ekfac" and (args.projection or len(args.checkpoint) != 1):
         raise SystemExit("--method ekfac takes one --checkpoint and no --projection")
     lrs = args.lr or [1.0] * len(args.checkpoint)
@@ -130,7 +145,19 @@ def main():
         test = dict(src=P, static=Ps, times=Pt, lengths=torch.sum(Pt > 0, dim=0), y=None)
         name = args.name or "dataset"
 
-    if args.method == "ekfac":
+    if args.method == "trak":
+        members = [sd for sd, _ in ckpts]
+        if args.load_features:
+            feats = TRAKFeatures.load(args.load_features, map_location=device)
+        else:
+            feats = trak_features(model, train, checkpoints=members, dim=args.projection or 4096,
+                                  seed=args.projection_seed, fields=args.fields)
+        if args.save_features:
+            feats.save(args.save_features)
+        damping = 0.0 if args.damping is None else args.damping
+        scores = trak(model, test, feats, damping=damping, checkpoints=members).cpu().numpy()
+        si = trak_self_influence(feats, damping=damping).cpu().numpy()
+    elif args.method == "ekfac":
         if args.load_factors:
             factors = EKFACFactors.load(args.load_factors, map_location=device)
         else:
@@ -150,7 +177,7 @@ def main():
         scores = tracin_sketch(project(model, test, **kw), train_sketch).cpu().numpy()
     else:
         scores = tracin(model, test, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
-    if args.method != "ekfac":
+    if args.method == "tracin":
         si = self_influence(model, train, checkpoints=ckpts, fields=args.fields).cpu().numpy()
     pro, pro_s, opp, opp_s = top_k(scores, args.top_k)
     out = dict(tracin_proponents=pro, tracin_proponent_scores=pro_s, tracin_opponents=opp, tracin_opponent_scores=opp_s,

@@ -992,6 +992,43 @@ int rd_trak_gram(const float* Phi, int64_t n, int32_t dim, double* K, void* stre
  * Stream-ordered, sync-free. */
 int rd_trak_rotate(const float* Phi, int64_t n, int32_t dim, const double* V, float* out, void* stream);
 
+/* ---- Batch active learning: BatchBALD (Kirsch et al. 2019) and BADGE (Ash et al. 2020) --------------------------------
+ * Both pick k points of an unlabelled pool of N, greedily, in one stream-ordered call whose loop has no host
+ * synchronisation (the argmax and the CDF search run on the device), so it can be captured in a CUDA graph.  Random
+ * draws are Philox4x32-10 with key (seed & 0xffffffff, (seed >> 32) ^ (step >> 32)) and counter (c0, c1, site,
+ * step & 0xffffffff), word 0 (and 1): sites 105 (BatchBALD) and 106 (BADGE), past every dropout and sampling site. */
+#define RD_ACTIVE_MAX_CLASSES 8
+#define RD_ACTIVE_MAX_REPLICATES 1024
+#define RD_ACTIVE_MAX_CONFIGS 65536
+/* Bytes of scratch rd_batch_bald needs (0 for sizes it refuses).  chunk: candidates per joint-entropy launch. */
+size_t rd_batch_bald_scratch_bytes(int64_t N, int32_t M, int32_t C, int32_t n_configs, int64_t chunk);
+/* Greedy BatchBALD over logits [M, N, C] (fp32, device; replicate-major).  Step i, with the chosen set A (|A| = i), picks
+ * the unchosen n maximising H(y_A, y_n) - sum_{a in A u {n}} E_m H(y_a | theta_m), ties to the lowest index.  The joint
+ * entropy is exact while C^i <= n_configs (the C^i configurations of A as mixed-radix rows), otherwise Kirsch's
+ * importance-weighted estimate over n_configs configurations drawn from the mixture: configuration s draws its
+ * replicate m_s = (w M) >> 32 from w = word 0 at counter (s, 0), and its label for the pick of step j as
+ * min{c : (w >> 8) 2^-24 < fp32 cumsum_c p[m_s, a_j, c]} from w = word 0 at counter (s, j + 1) (the largest class with
+ * p > 0 if none).  Rows of configurations are kept scaled to max 1 with their log-scale in fp64.  The products
+ * Q = P_A . p run on the tensor cores in 3xTF32 with the entropy in the epilogue (fp32 logarithm, fp64 sums).  Outputs
+ * (device): indices [k] int64, scores [k] fp64 (the joint mutual information of the batch after each pick), exact [k]
+ * (1 where the pick enumerated), bald [N] fp64 (the single-point mutual information).  Every sum has an order fixed
+ * by (N, M, C, n_configs): the result is bitwise independent of `chunk`.  2 <= C <= RD_ACTIVE_MAX_CLASSES, 1 <= M <=
+ * RD_ACTIVE_MAX_REPLICATES, 1 <= n_configs <= RD_ACTIVE_MAX_CONFIGS, 1 <= k <= N; scratch 256-byte aligned. */
+int rd_batch_bald(const float* logits, int64_t N, int32_t M, int32_t C, int32_t k, int32_t n_configs, uint64_t seed,
+                  uint64_t step, int64_t chunk, void* scratch, int64_t* indices, double* scores, uint8_t* exact,
+                  double* bald, void* stream);
+/* Bytes of scratch rd_badge needs (0 for sizes it refuses). */
+size_t rd_badge_scratch_bytes(int64_t N, int32_t F, int32_t C);
+/* BADGE's k-means++ seeding over g_n = (p_n - e_yhat_n) (x) [h_n; 1], hidden [N, F] and logits [N, C] (fp32, device),
+ * p = softmax, yhat = argmax (ties to the lowest class).  Distances use the factorised form |a_i|^2 |h~_i|^2 +
+ * |a_c|^2 |h~_c|^2 - 2 (a_i . a_c)(h~_i . h~_c) (fp32 products in fp64, fp64 sums, clamped at 0): the embedding is never
+ * formed.  The first centre has the largest norm (ties to the lowest index); pick i >= 1 draws U = ((w0 >> 5) 2^26 +
+ * (w1 >> 6)) 2^-53 at counter (i, 0) and takes the first point whose running sum of D^2, in tiles of 256 points in
+ * index order, exceeds U sum D^2 (the lowest unchosen index when every D^2 is 0).  Outputs (device): indices [k] int64
+ * and d2 [k] fp64, D^2 at pick time (inf for the first).  2 <= C <= RD_ACTIVE_MAX_CLASSES, 1 <= k <= N. */
+int rd_badge(const float* hidden, const float* logits, int64_t N, int32_t F, int32_t C, int32_t k, uint64_t seed,
+             uint64_t step, void* scratch, int64_t* indices, double* d2, void* stream);
+
 /* ---- Laplace approximation (MacKay 1992; Ritter et al. 2018; Daxberger et al. 2021) ----------------------------------
  * Posterior N(theta*, H^-1), H = n F + delta I with F the EK-FAC Fisher above: diagonal in the Kronecker eigenbasis,
  * n Lambda_j + delta.  The linearised predictive of sample b is f ~ N(f(x_b; theta*), Sigma_b) over its logits, with

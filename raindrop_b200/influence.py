@@ -224,9 +224,10 @@ def _check_margin_classes(model):
 
 
 # ---- data sources: a dict of tensors, or a DeviceDataset (optionally with an index subset) ----------------------------
-def _source(data, what):
+def _source(data, what, unlabelled=False):
     """-> (n, fetch(i0, i1) -> (src, static, times, lengths, y)).  data: dict(src, static, times, lengths, y),
-    a data.DeviceDataset, or a pair (DeviceDataset, indices)."""
+    a data.DeviceDataset, or a pair (DeviceDataset, indices).  unlabelled: a DeviceDataset without labels is served
+    with y = None."""
     from .data import BatchBuffers, DeviceDataset
     idx = None
     if isinstance(data, tuple) and len(data) == 2 and isinstance(data[0], DeviceDataset):
@@ -236,14 +237,14 @@ def _source(data, what):
         idx = torch.arange(ds.n, dtype=torch.int64) if idx is None else torch.as_tensor(idx, dtype=torch.int64).reshape(-1)
         if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= ds.n):
             raise ValueError("%s indices must lie in [0, %d)" % (what, ds.n))
-        if ds.y is None:
+        if ds.y is None and not unlabelled:
             raise ValueError("%s DeviceDataset has no labels" % what)
         idx = idx.to(ds.P.device)
 
         def fetch(i0, i1):
             buf = BatchBuffers(ds.T, i1 - i0, ds.width, 0 if ds.Pstatic is None else ds.Pstatic.shape[1], device=ds.P.device)
             ds.fill(buf, idx[i0:i1])
-            return buf.src, buf.static, buf.times, buf.lengths, buf.y
+            return buf.src, buf.static, buf.times, buf.lengths, None if ds.y is None else buf.y
         return idx.numel(), fetch
     if not isinstance(data, dict):
         raise TypeError("%s must be a dict (src, static, times, lengths, y) or a DeviceDataset" % what)
@@ -258,9 +259,10 @@ def _source(data, what):
     return src.shape[1], fetch
 
 
-def _check_data(model, data, what, allow_none_y):
+def _check_data(model, data, what, allow_none_y, unlabelled=False):
     """Host-side checks of a data argument against the model, before anything touches the device: a dict's tensor
-    shapes and labels, or a DeviceDataset's T, width, static width, indices and the labels it will serve."""
+    shapes and labels, or a DeviceDataset's T, width, static width, indices and the labels it will serve.  unlabelled:
+    a DeviceDataset may have no labels (as _source(..., unlabelled=True) serves it)."""
     from .data import DeviceDataset
     from .models_rd import Raindrop_v2
     plan = model._plan
@@ -280,9 +282,9 @@ def _check_data(model, data, what, allow_none_y):
                                           plan.d_static if model.static else 0))
         if tuple(ds.Ptime.shape) != (ds.T, ds.n):
             raise ValueError("%s DeviceDataset times must be [T, n]" % what)
-        if ds.y is None:
+        if ds.y is None and not unlabelled:
             raise ValueError("%s DeviceDataset has no labels" % what)
-        if tuple(ds.y.shape) != (ds.n,):
+        if ds.y is not None and tuple(ds.y.shape) != (ds.n,):
             raise ValueError("%s DeviceDataset labels must be [n]" % what)
         sel = torch.arange(ds.n, dtype=torch.int64) if idx is None else torch.as_tensor(idx).reshape(-1)
         if sel.is_floating_point() or sel.dtype == torch.bool:
@@ -291,6 +293,8 @@ def _check_data(model, data, what, allow_none_y):
             lo, hi = torch.stack(torch.aminmax(sel.to(torch.int64))).tolist()
             if lo < 0 or hi >= ds.n:
                 raise ValueError("%s indices must lie in [0, %d)" % (what, ds.n))
+            if ds.y is None:
+                return
             ys = ds.y[sel.to(ds.y.device)] if idx is not None else ds.y
             lo, hi = torch.stack(torch.aminmax(ys)).tolist()         # one host sync
             if lo < 0 or hi >= plan.n_classes:

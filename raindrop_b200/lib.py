@@ -23,6 +23,9 @@ OOD_MAX_K = 256             # RD_OOD_MAX_K
 OOD_POOLED, OOD_HIDDEN = 0, 1   # enum rd_ood_layer
 SWAG_MAX_RANK = 1024        # RD_SWAG_MAX_RANK
 TRAK_DIM_MAX = 8192         # RD_TRAK_DIM_MAX
+ACTIVE_MAX_CLASSES = 8      # RD_ACTIVE_MAX_CLASSES
+ACTIVE_MAX_REPLICATES = 1024  # RD_ACTIVE_MAX_REPLICATES
+ACTIVE_MAX_CONFIGS = 65536  # RD_ACTIVE_MAX_CONFIGS
 
 # enum rd_ws_buffer
 WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
@@ -308,6 +311,12 @@ SIGNATURES = {
     "rd_trak_margin_seed": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 4),
     "rd_trak_gram": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
     "rd_trak_rotate": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rd_batch_bald_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
+    "rd_batch_bald": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_uint64,
+                                C.c_uint64, C.c_int64] + [C.c_void_p] * 6),
+    "rd_badge_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32]),
+    "rd_badge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64] +
+                 [C.c_void_p] * 4),
     "rd_laplace_logit_cov_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
     "rd_raindrop_v2_laplace_logit_cov": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
     "rd_laplace_sample_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),

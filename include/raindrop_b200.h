@@ -1029,6 +1029,38 @@ size_t rd_badge_scratch_bytes(int64_t N, int32_t F, int32_t C);
 int rd_badge(const float* hidden, const float* logits, int64_t N, int32_t F, int32_t C, int32_t k, uint64_t seed,
              uint64_t step, void* scratch, int64_t* indices, double* d2, void* stream);
 
+/* ---- KNN-Shapley data valuation (Jia et al., VLDB 2019) ----------------------------------------------------------------
+ * The exact Shapley value of every training record under the utility of a K-nearest-neighbour classifier, per query:
+ * U(S) = (1/K) #{the min(K, |S|) records of S most similar to q that carry q's label}.  Similarity = the fp64 dot of two
+ * L2-normalised fp32 rows (rd_ood_prepare_bank); the N candidates are ranked by similarity descending, ties to the lower
+ * index (alpha_1 .. alpha_N).  With m_r = 1[y_train(alpha_r) = y_q] and c_r = min(K, r) / (r K), the record at rank r
+ * gets s_r = m_r c_r - sum_{j = max(r, K) + 1}^{N} m_j / (j (j - 1)), which is Theorem 1's recursion s_r = s_{r+1} +
+ * (m_r - m_{r+1}) c_r from s_N = m_N c_N, exact for K > N too; sum_r s_r = U(all). */
+/* Bytes of scratch rd_knn_shapley needs for chunks of queries_per_chunk queries (0 for sizes it refuses). */
+size_t rd_knn_shapley_scratch_bytes(int64_t n_train, int32_t ld, int32_t queries_per_chunk);
+/* values [n_train] (+)= sum_q s^(q) (fp64, device), the queries added one at a time in query index order, so the result
+ * is bitwise independent of queries_per_chunk and of how a query set is split across accumulating calls (accumulate != 0
+ * adds to the values stored, else they are overwritten).  per_query [n_query, n_train] (fp64; NULL: skipped) = s^(q) in
+ * record order; utility [n_query] (fp64; NULL: skipped) = U_q(all).  bank [n_train, ld] and queries [n_query, ld]: the
+ * normalised fp32 rows with zero columns up to ld (a multiple of 4; both 16-byte aligned); y_train [n_train] and y_query
+ * [n_query] int64 labels.  self_offset >= 0: query q is training record self_offset + q and is left out of its own
+ * ranking (N = n_train - 1, s = 0 at its own record); -1: no exclusion (N = n_train).  Per chunk: one DMMA launch of the
+ * similarities as descending-order 64-bit keys (every element over the same k-order, so identical rows get identical
+ * similarities), one CTA per query for a stable LSD radix sort (eight 8-bit passes through scratch, the index as payload)
+ * and the suffix sums in a fixed order, then one thread per record adds the chunk's rows in order.  Refused with -2
+ * before any launch: k < 1, n_train outside [1, 2^31), fewer than 2 records with self_offset >= 0, a self range outside
+ * the bank, a NULL required pointer, misaligned pointers (scratch 256-byte aligned).  Non-finite rows rank after every
+ * number (the Python layer refuses them).  Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+int rd_knn_shapley(const float* bank, int64_t n_train, int32_t ld, const int64_t* y_train, const float* queries,
+                   int64_t n_query, const int64_t* y_query, int32_t k, int64_t self_offset, int32_t queries_per_chunk,
+                   int32_t accumulate, void* scratch, double* values, double* per_query, double* utility, void* stream);
+/* debug: the ranking of rd_knn_shapley as one chunk of n_query queries (scratch: rd_knn_shapley_scratch_bytes(n_train,
+ * ld, n_query)): order [n_query, n_train] int64 = the records in ranked order (with self_offset >= 0 the query's own
+ * record last), sim [n_query, n_train] fp64 = each record's similarity, read back from its sort key (NaN at the query's
+ * own record). */
+int rd_debug_knn_rank(const float* bank, int64_t n_train, int32_t ld, const float* queries, int64_t n_query,
+                      int64_t self_offset, void* scratch, double* sim, int64_t* order, void* stream);
+
 /* ---- Laplace approximation (MacKay 1992; Ritter et al. 2018; Daxberger et al. 2021) ----------------------------------
  * Posterior N(theta*, H^-1), H = n F + delta I with F the EK-FAC Fisher above: diagonal in the Kronecker eigenbasis,
  * n Lambda_j + delta.  The linearised predictive of sample b is f ~ N(f(x_b; theta*), Sigma_b) over its logits, with

@@ -317,6 +317,11 @@ SIGNATURES = {
     "rd_badge_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32]),
     "rd_badge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64] +
                  [C.c_void_p] * 4),
+    "rd_knn_shapley_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32]),
+    "rd_knn_shapley": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                 C.c_int32, C.c_int64, C.c_int32, C.c_int32] + [C.c_void_p] * 5),
+    "rd_debug_knn_rank": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int64] +
+                          [C.c_void_p] * 4),
     "rd_laplace_logit_cov_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims)]),
     "rd_raindrop_v2_laplace_logit_cov": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9),
     "rd_laplace_sample_scratch_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),

@@ -363,6 +363,76 @@ int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, con
                                const double* weights, int32_t n_coalitions, const double* solve, int32_t coalitions_per_chunk,
                                void* scratch, float* attr, float* endpoint_logits, void* stream);
 
+/* ---- faithfulness of attributions by removal: deletion / insertion curves and infidelity, in one call each ----------
+ * Players, removal, cell_player and its strides ((0, 0): one player per sensor), target, baselines and eval arithmetic
+ * as for rd_raindrop_v2_kernel_shap; n_players = P = G + (d_static > 0), 1 <= P <= RD_REMOVAL_MAX_PLAYERS.
+ * attributions [B, P] (device fp32) are the scores phi under test, the static player last.  F = logits[b, target[b]].
+ *
+ * rd_raindrop_v2_removal_curves: rank [B, P] (int32) = the position of player g when sample b's players are sorted by
+ * `order` (RD_REMOVAL_DESCENDING: phi high to low; _ASCENDING: low to high; _ABSOLUTE: |phi| high to low), ties to the
+ * lower index, -0 as +0, NaN after every number.  counts [K] (device int32, strictly increasing in [0, P]; not checked
+ * on the device) are the removal counts.  Deletion point (k, b) removes the players with rank < counts[k]; insertion
+ * point (k, b) removes all others.  Outputs:
+ *   curve_logits     [2, K, B, n_classes]: deletion ([0]) and insertion ([1]) logits
+ *   endpoint_logits  [2, B, n_classes]: logits at x' ([0]) and at x ([1])
+ *   values           [2, B, K]: F of the curve points;  target_out [B] int64: the class F reads
+ *   summaries        [B, RD_REMOVAL_SUMMARIES] fp64: deletion AUC, insertion AUC, AOPC of the logit F, then the same of
+ *                    softmax(logits)[target] (fp64 softmax of the fp32 logits).  AUC: trapezoid rule over
+ *                    x_k = counts[k] / P;  AOPC = (1/K) sum_k (F(x) - deletion F at k).
+ * Work: the endpoint forward on 2B rows, one rank launch (one CTA per sample, the keys sorted in shared memory), then
+ * the 2K (curve, count) pairs in chunks of pairs_per_chunk on B*pairs_per_chunk rows (pair-major): one launch writes
+ * the chunk's per-row keep table [nc*B, P] into scratch, one expands the rows, and one eval forward writes its logits
+ * straight into curve_logits; finally one summary launch.  scratch: rd_removal_curves_scratch_bytes(dims, n_players,
+ * pairs_per_chunk) bytes.
+ *
+ * rd_raindrop_v2_removal_infidelity: replicate m = 0 .. n_samples-1 removes from sample b the set S_mb of players g
+ * whose Philox word b*P + g (word idx & 3 of the block idx >> 2) at site 107 under key {rng[0], rng[1] + m} (rng device
+ * uint64[2] = {seed, step}) is below floor(p_remove 2^32), 0 < p_remove <= 1 (1: every player).  With
+ * a = sum_{g in S} phi[b, g] and d = F(x) - F(x with S removed), both fp64, moments [B, RD_REMOVAL_MOMENTS] (fp64) =
+ * [sum 1, sum a, sum d, sum a^2, sum a d, sum d^2] over the replicates, added in replicate order; clean_logits
+ * [B, n_classes] are the logits at x and target_out [B] (may be NULL) the class F reads.  Work: one forward on the B rows
+ * of x, then chunks of replicates_per_chunk replicates on B*replicates_per_chunk rows: the keep-table launch, the
+ * expansion, the eval forward and one launch adding the chunk to the moments (one CTA per sample).  scratch:
+ * rd_removal_infidelity_scratch_bytes(dims, n_players, replicates_per_chunk) bytes.
+ *
+ * rd_debug_removal_inputs: the keep-table and expansion launches of one chunk, nc pairs or replicates from q0: curve
+ * pairs when rank is given (pair q < K: deletion at counts[q], else insertion at counts[q - K]), else infidelity
+ * replicates from rng and p_remove.  Writes keep_table [nc*B, P] (uint8, nonzero = kept) and the rows src_e
+ * [T, nc*B, 2N], statics_e [nc*B, d_static] (when d_static > 0), times_e [T, nc*B] and lengths_e [nc*B].
+ *
+ * dims->obprop_mode 0 is resolved once from the full chunk's row count, so every forward of a call uses the same
+ * arithmetic; with it pinned the results are bitwise independent of the chunk size.  Every sum is in a fixed order, no
+ * atomics.  Stream-ordered, allocation- and sync-free, CUDA-graph capturable. */
+#define RD_REMOVAL_MAX_PLAYERS 16384
+#define RD_REMOVAL_DESCENDING 0
+#define RD_REMOVAL_ASCENDING 1
+#define RD_REMOVAL_ABSOLUTE 2
+#define RD_REMOVAL_SUMMARIES 6
+#define RD_REMOVAL_MOMENTS 6
+size_t rd_removal_curves_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t pairs_per_chunk);
+int rd_raindrop_v2_removal_curves(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                  const float* times, const int64_t* lengths, const float* node_scale,
+                                  const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                  const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                                  int32_t n_players, const float* attributions, int32_t order, const int32_t* counts,
+                                  int32_t n_counts, int32_t pairs_per_chunk, void* scratch, int32_t* rank,
+                                  float* curve_logits, float* endpoint_logits, float* values, double* summaries,
+                                  int64_t* target_out, void* stream);
+size_t rd_removal_infidelity_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t replicates_per_chunk);
+int rd_raindrop_v2_removal_infidelity(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                      const float* times, const int64_t* lengths, const float* node_scale,
+                                      const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                      const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                                      int32_t n_players, const float* attributions, const uint64_t* rng, double p_remove,
+                                      int32_t n_samples, int32_t replicates_per_chunk, void* scratch, float* clean_logits,
+                                      double* moments, int64_t* target_out, void* stream);
+int rd_debug_removal_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                            const int64_t* lengths, const float* baseline_src, const float* baseline_statics,
+                            const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                            int32_t n_players, const int32_t* rank, const int32_t* counts, int32_t n_counts,
+                            const uint64_t* rng, double p_remove, int64_t q0, int32_t nc, uint8_t* keep_table,
+                            float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, void* stream);
+
 /* ---- Monte Carlo dropout predictive uncertainty of Raindrop_v2, in one call ------------------------------------------
  * Replicate m = 0 .. n_samples-1 is exactly the training-mode forward of the B-row batch with the dropout stream at
  * {seed, step + m}, rng = {seed, step} (device uint64[2]; read, never written -- the model's own counter is not

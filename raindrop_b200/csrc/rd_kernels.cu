@@ -337,20 +337,6 @@ __global__ void input_grad_kernel(const __grid_constant__ InputGradArgs a, const
 // Point alpha of the straight path from the baseline x0 to x.  Exact at both ends: alpha = 0 gives x0, alpha = 1 gives x.
 __device__ __forceinline__ float ig_interp(float x, float x0, float a) { return fmaf(a, x, (1.f - a) * x0); }
 
-// The attributed class of sample b: target[b], or (target == NULL) the first maximum of logits_x[b, :], as torch.argmax
-__device__ __forceinline__ int target_class(const int64_t* __restrict__ target, const float* __restrict__ logits_x, int b,
-                                            int ncls) {
-  if (target) return (int)__ldg(target + b);
-  const float* l = logits_x + (long long)b * ncls;
-  float best = __ldg(l);
-  int tgt = 0;
-  for (int c = 1; c < ncls; ++c) {
-    const float v = __ldg(l + c);
-    if (v > best) { best = v; tgt = c; }
-  }
-  return tgt;
-}
-
 // Inputs of one chunk of m path steps on B*m rows, step-major (row j = k*B + b), in one launch with four thread ranges:
 //   src_e[t, j, n] = interp(src[t, b, n], src0[t, b, n], alpha_k) (value half), src[t, b, n] (mask half, copied)
 //   times_e[t, j] = times[t, b]
@@ -486,6 +472,7 @@ __global__ void coalition_keep_kernel(const __grid_constant__ CoalitionKeepArgs 
 //                    src[t, b, n] (mask half, copied)
 //   times_e[t, j] = times[t, b];  lengths_e[j] = lengths[b]
 //   statics_e[j, :] = kept(ci, P-1) ? statics[b, :] : statics0[b, :]  (the static player is the last one, P = G + 1)
+// COALITION_ROWS (removal curves, infidelity): kept(ci, g) of row j = ci*B + b is keep[j, g] of a per-row table [nc*B, P].
 struct CoalitionExpandArgs {
   const float* src; const float* src0; const float* statics; const float* statics0; const float* times;
   const int64_t* lengths; const int32_t* player; const uint8_t* keep;
@@ -494,9 +481,10 @@ struct CoalitionExpandArgs {
   int P, G, method, c0, nc, B, T, N, ds;
   long long n_src, n_tok, n_stat, n_rows;
 };
-__device__ __forceinline__ bool coalition_kept(const CoalitionExpandArgs& a, int ci, int g) {
+__device__ __forceinline__ bool coalition_kept(const CoalitionExpandArgs& a, int ci, long long j, int g) {
   if (a.method == RD_ATTR_SHAPLEY) return __ldg(a.keep + (long long)ci * a.P + g);
   if (a.method == RD_ATTR_ABLATION) return a.c0 + ci != g;
+  if (a.method == COALITION_ROWS) return __ldg(a.keep + j * a.P + g);
   return ci != 0;                                             // COALITION_ENDPOINTS
 }
 __global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandArgs a) {
@@ -514,7 +502,7 @@ __global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandA
     bool x = true;
     if (c < a.N) {
       const int g = __ldg(a.player + t * a.stride_t + b * a.stride_b + c);
-      x = (unsigned)g >= (unsigned)a.G || coalition_kept(a, ci, g);
+      x = (unsigned)g >= (unsigned)a.G || coalition_kept(a, ci, j, g);
     }
     a.src_e[o] = __ldg((x ? a.src : a.src0) + i);
     return;
@@ -530,7 +518,7 @@ __global__ void coalition_expand_kernel(const __grid_constant__ CoalitionExpandA
   if (o < a.n_stat) {
     const long long j = o / a.ds;
     const int kk = (int)(o - j * a.ds), ci = (int)(j / a.B), b = (int)(j - (long long)ci * a.B);
-    const bool x = coalition_kept(a, ci, a.P - 1);
+    const bool x = coalition_kept(a, ci, j, a.P - 1);
     a.statics_e[o] = __ldg((x ? a.statics : a.statics0) + (long long)b * a.ds + kk);
     return;
   }

@@ -95,6 +95,20 @@ int ig_accumulate(const float* src, const float* src0, const float* alphas, cons
                   const float* statics0, const float* dfeat, int Df, int feat_col0, const float* W_emb, int emb, int ds,
                   float* acc_static, float* attr_static, int first, int last, cudaStream_t st);
 
+// The attributed class of sample b: target[b], or (target == NULL) the first maximum of logits_x[b, :], as torch.argmax
+__device__ __forceinline__ int target_class(const int64_t* __restrict__ target, const float* __restrict__ logits_x, int b,
+                                            int ncls) {
+  if (target) return (int)__ldg(target + b);
+  const float* l = logits_x + (long long)b * ncls;
+  float best = __ldg(l);
+  int tgt = 0;
+  for (int c = 1; c < ncls; ++c) {
+    const float v = __ldg(l + c);
+    if (v > best) { best = v; tgt = c; }
+  }
+  return tgt;
+}
+
 // Coalition attribution over P players (value cell (t, b, n) belongs to player[t*stride_t + b*stride_b + n], ids in
 // [0, G) are players, any other id none; the static player G = P-1 when ds > 0), chunks of nc coalitions c0 .. c0+nc-1
 // on B*nc rows, coalition-major (j = ci*B + b); method RD_ATTR_SHAPLEY: coalition c = p*(P-1) + k-1 keeps orders[p, :k],
@@ -116,6 +130,9 @@ int coalition_accumulate(const float* logits_c, const float* ends, const int64_t
 // COALITION_TABLE (KernelSHAP): coalition_expand reads `keep` as the chunk's rows of the caller's coalition table
 // [nc, P] (uint8, nonzero = kept) and launches nothing to fill it; orders is not read.
 #define COALITION_TABLE 3
+// COALITION_ROWS (removal curves, infidelity): coalition_expand reads `keep` as a per-row table [nc*B, P] (uint8,
+// nonzero = kept; row j = ci*B + b), which the caller filled, and launches nothing to fill it; orders is not read.
+#define COALITION_ROWS 4
 // kernel_shap_accumulate: adds sum_ci w[c] z[c, g] (F(c) - F(x')) over the chunk's coalitions c = c0 .. c0+nc-1 (F at
 // target[b], nullptr: argmax of ends[1]) into the fp64 sums acc [B, P]; first: start from 0.
 int kernel_shap_accumulate(const float* logits_c, const float* ends, const int64_t* target, const uint8_t* z,
@@ -332,6 +349,30 @@ struct PrefixArgs {
   int B, T, N, ds, k0, nc;
 };
 int prefix_inputs(const PrefixArgs& a, cudaStream_t st);
+
+// ---- faithfulness of attributions by removal (rd_faithfulness.cu; rd_raindrop_v2_removal_curves / _infidelity) -----
+constexpr uint32_t SITE_REMOVAL = 107;      // Philox site of infidelity's removal sets (its key is {seed, step + replicate})
+// removal_rank: rank [B, P] (int32) = position of each player when sample b's attributions attr [B, P] are sorted by
+// `order` (RD_REMOVAL_*), ties to the lower index, -0 as +0, NaN last; one CTA per sample, P <= RD_REMOVAL_MAX_PLAYERS.
+int removal_rank(const float* attr, int B, int P, int order, int32_t* rank, cudaStream_t st);
+// removal_curve_keep: the keep table [nc*B, P] of (curve, count) pairs q0 .. q0+nc-1 (pair q: deletion at counts[q] for
+// q < K, insertion at counts[q - K] after), row j = (q - q0)*B + b: deletion keeps rank >= count, insertion rank < count.
+int removal_curve_keep(const int32_t* rank, const int32_t* counts, int K, int64_t q0, int nc, int B, int P, uint8_t* keep,
+                       cudaStream_t st);
+// removal_sample_keep: the keep table [nc*B, P] of replicates m0 .. m0+nc-1: player g of row (m, b) is removed iff word
+// b*P + g at SITE_REMOVAL, key {rng[0], rng[1] + m}, is below `below` (= floor(p_remove 2^32)).
+int removal_sample_keep(const uint64_t* rng, uint64_t below, int64_t m0, int nc, int B, int P, uint8_t* keep,
+                        cudaStream_t st);
+// removal_curve_summary: from curve_logits [2, K, B, ncls] and ends [2, B, ncls] (x', x): values [2, B, K] (F at the
+// target), summaries [B, RD_REMOVAL_SUMMARIES] (fp64) and target_out [B] (target NULL: the argmax at x).
+int removal_curve_summary(const float* curve_logits, const float* ends, const int64_t* target, const int32_t* counts,
+                          int K, int B, int P, int ncls, float* values, double* summaries, int64_t* target_out,
+                          cudaStream_t st);
+// removal_moments: adds replicates (logits [nc*B, ncls], keep [nc*B, P]) into moments [B, RD_REMOVAL_MOMENTS] in
+// replicate order (first: from 0, and target_out [B] written when not NULL); clean [B, ncls] are the logits at x.
+int removal_moments(const float* logits, const float* clean, const int64_t* target, const float* attr,
+                    const uint8_t* keep, int nc, int B, int P, int ncls, int first, double* moments, int64_t* target_out,
+                    cudaStream_t st);
 
 // ---- SWA / SWAG (rd_swag.cu; rd_swag_collect, rd_swag_sample, rd_raindrop_v2_swag_predictive) ----------------------
 constexpr uint32_t SITE_SWAG = 102;         // Philox site of the SWAG weight draws (its key is {seed, step + replicate})

@@ -1608,6 +1608,206 @@ int rd_raindrop_v2_kernel_shap(const rd_dims* dims, const rd_params* params, con
   return kernel_shap_solve(r.acc, solve, endpoint_logits, target, P, B, r.s0.ncls, attr, st);
 }
 
+// ---- faithfulness of attributions by removal -------------------------------------------------------------------------
+// Chunks of cc (curve, count) pairs or replicates (B*cc rows; curves also run the 2B-row endpoint forward) and the
+// chunk's per-row keep table [cc*B, P] (uint8) at the arena's tail.
+struct RemovalScratch : ChunkLayout { int64_t keep; };
+static int removal_scratch(const rd_dims* dims, int n_players, int cc, bool curves, RemovalScratch* l) {
+  RD_TRY(chunk_layout(dims, curves ? "pairs_per_chunk" : "replicates_per_chunk", cc, dims->B, curves, 0, false, l));
+  if (n_players < 1 || n_players > RD_REMOVAL_MAX_PLAYERS) {
+    set_error("n_players = %d must be in [1, %d]", n_players, RD_REMOVAL_MAX_PLAYERS);
+    return -2;
+  }
+  l->keep = l->a.take(ceil_div((int64_t)cc * dims->B * n_players, 4));
+  return 0;
+}
+
+size_t rd_removal_curves_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t pairs_per_chunk) {
+  RemovalScratch l;
+  if (!dims || removal_scratch(dims, n_players, pairs_per_chunk, true, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+size_t rd_removal_infidelity_scratch_bytes(const rd_dims* dims, int32_t n_players, int32_t replicates_per_chunk) {
+  RemovalScratch l;
+  if (!dims || removal_scratch(dims, n_players, replicates_per_chunk, false, &l) != 0) return 0;
+  return (size_t)l.a.off * sizeof(float);
+}
+
+// The player checks both removal calls and the debug entry share, after the shape's.
+static int removal_players(const char* fn, const Shape& s0, const int32_t* cell_player, int64_t stride_t, int64_t stride_b,
+                           int32_t n_players, int* G) {
+  if (!cell_player) { set_error("%s: NULL argument", fn); return -2; }
+  *G = n_players - (s0.ds > 0 ? 1 : 0);
+  if (n_players > RD_REMOVAL_MAX_PLAYERS || *G < 1) {
+    set_error("%s: n_players = %d must be in [1 + (d_static > 0), %d]", fn, n_players, RD_REMOVAL_MAX_PLAYERS);
+    return -2;
+  }
+  if (stride_t < 0 || stride_b < 0) {
+    set_error("%s: player strides must be >= 0, got (%lld, %lld)", fn, (long long)stride_t, (long long)stride_b);
+    return -2;
+  }
+  return 0;
+}
+
+// floor(p_remove 2^32): a word below it removes its player (p_remove = 1: every word)
+static int removal_threshold(const char* fn, double p_remove, uint64_t* below) {
+  if (!(p_remove > 0.0 && p_remove <= 1.0)) { set_error("%s: p_remove = %g must lie in (0, 1]", fn, p_remove); return -2; }
+  *below = (uint64_t)floor(p_remove * 4294967296.0);
+  return 0;
+}
+
+// What both removal calls share: the checks, the scratch carved by removal_scratch, in the CoalRun the coalition calls'
+// endpoint forward reads.
+static int removal_setup(const char* fn, const rd_dims* dims, const rd_params* params, const float* src,
+                         const float* statics, const float* times, const int64_t* lengths, const float* node_scale,
+                         const float* baseline_src, const float* baseline_statics, const int32_t* cell_player,
+                         int64_t stride_t, int64_t stride_b, int32_t n_players, const float* attributions, int32_t cc,
+                         bool curves, void* scratch, CoalRun* r) {
+  Shape& s0 = r->s0;
+  RD_TRY(check_model_call(fn, dims, params, lengths, node_scale, statics, true, &s0));
+  if (!src || !times || !baseline_src || !attributions || !scratch || !params->R_u || !params->ob1_value_weight) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (s0.ds > 0 && !baseline_statics) { set_error("%s: d_static > 0 needs baseline_statics", fn); return -2; }
+  RD_TRY(removal_players(fn, s0, cell_player, stride_t, stride_b, n_players, &r->G));
+  RemovalScratch l;
+  RD_TRY(removal_scratch(dims, n_players, cc, curves, &l));
+  r->P = n_players; r->B = s0.B; r->cc = cc;
+  float* S = (float*)scratch;
+  r->x = l.inputs(S, s0.ds);
+  r->ws = S + l.ws; r->logits = S + l.logits;
+  r->acc = nullptr;
+  r->keep = reinterpret_cast<uint8_t*>(S + l.keep);
+  return 0;
+}
+
+// The endpoints, the rank launch, then per chunk of pairs the keep table, the expansion and one eval forward into
+// curve_logits; the summaries after the last chunk.
+int rd_raindrop_v2_removal_curves(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                  const float* times, const int64_t* lengths, const float* node_scale,
+                                  const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                  const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                                  int32_t n_players, const float* attributions, int32_t order, const int32_t* counts,
+                                  int32_t n_counts, int32_t pairs_per_chunk, void* scratch, int32_t* rank,
+                                  float* curve_logits, float* endpoint_logits, float* values, double* summaries,
+                                  int64_t* target_out, void* stream) {
+  const char* fn = "rd_raindrop_v2_removal_curves";
+  if (!counts || !rank || !curve_logits || !endpoint_logits || !values || !summaries || !target_out) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  if (order != RD_REMOVAL_DESCENDING && order != RD_REMOVAL_ASCENDING && order != RD_REMOVAL_ABSOLUTE) {
+    set_error("%s: order = %d is not an RD_REMOVAL_* order", fn, order);
+    return -2;
+  }
+  CoalRun r;
+  RD_TRY(removal_setup(fn, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                       cell_player, player_stride_t, player_stride_b, n_players, attributions, pairs_per_chunk, true,
+                       scratch, &r));
+  const int P = r.P, G = r.G, B = r.B, cc = r.cc, K = n_counts;
+  if (K < 1 || K > P + 1) { set_error("%s: n_counts = %d must be in [1, n_players + 1 = %d]", fn, K, P + 1); return -2; }
+  cudaStream_t st = (cudaStream_t)stream;
+  RD_TRY(coalition_endpoints(r, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                             cell_player, player_stride_t, player_stride_b, endpoint_logits, st));
+  RD_TRY(removal_rank(attributions, B, P, order, rank, st));
+  const int n_pairs = 2 * K;
+  for (int q0 = 0; q0 < n_pairs; q0 += cc) {
+    const int nc = n_pairs - q0 < cc ? n_pairs - q0 : cc;
+    const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
+    RD_TRY(removal_curve_keep(rank, counts, K, q0, nc, B, P, r.keep, st));
+    RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, player_stride_t,
+                            player_stride_b, nullptr, P, G, COALITION_ROWS, 0, nc, B, r.s0.T, r.s0.N, r.s0.ds, r.keep,
+                            r.x.src, r.x.statics, r.x.times, r.x.lengths, st));
+    RD_TRY(raindrop_fwd(&dc, params, r.x.src, r.x.statics, r.x.times, r.x.lengths, node_scale, nullptr, r.ws,
+                        curve_logits + (int64_t)q0 * B * r.s0.ncls, nullptr, nullptr, nullptr, 0, st));
+  }
+  return removal_curve_summary(curve_logits, endpoint_logits, target, counts, K, B, P, r.s0.ncls, values, summaries,
+                               target_out, st);
+}
+
+// One forward on the B rows of x, then per chunk of replicates the keep table, the expansion, one eval forward and the
+// moment launch.
+int rd_raindrop_v2_removal_infidelity(const rd_dims* dims, const rd_params* params, const float* src, const float* statics,
+                                      const float* times, const int64_t* lengths, const float* node_scale,
+                                      const float* baseline_src, const float* baseline_statics, const int64_t* target,
+                                      const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                                      int32_t n_players, const float* attributions, const uint64_t* rng, double p_remove,
+                                      int32_t n_samples, int32_t replicates_per_chunk, void* scratch, float* clean_logits,
+                                      double* moments, int64_t* target_out, void* stream) {
+  const char* fn = "rd_raindrop_v2_removal_infidelity";
+  if (!rng || !clean_logits || !moments) { set_error("%s: NULL argument", fn); return -2; }
+  if (n_samples < 1) { set_error("%s: n_samples = %d must be >= 1", fn, n_samples); return -2; }
+  uint64_t below;
+  RD_TRY(removal_threshold(fn, p_remove, &below));
+  CoalRun r;
+  RD_TRY(removal_setup(fn, dims, params, src, statics, times, lengths, node_scale, baseline_src, baseline_statics,
+                       cell_player, player_stride_t, player_stride_b, n_players, attributions, replicates_per_chunk, false,
+                       scratch, &r));
+  const int P = r.P, G = r.G, B = r.B, cc = r.cc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const rd_dims de = chunk_dims(dims, B, (int64_t)B * cc, 0);
+  RD_TRY(raindrop_fwd(&de, params, src, r.s0.ds > 0 ? statics : nullptr, times, lengths, node_scale, nullptr, r.ws,
+                      clean_logits, nullptr, nullptr, nullptr, 0, st));
+  for (int m0 = 0; m0 < n_samples; m0 += cc) {
+    const int nc = n_samples - m0 < cc ? n_samples - m0 : cc;
+    const rd_dims dc = chunk_dims(dims, B * nc, (int64_t)B * cc, 0);
+    RD_TRY(removal_sample_keep(rng, below, m0, nc, B, P, r.keep, st));
+    RD_TRY(coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, player_stride_t,
+                            player_stride_b, nullptr, P, G, COALITION_ROWS, 0, nc, B, r.s0.T, r.s0.N, r.s0.ds, r.keep,
+                            r.x.src, r.x.statics, r.x.times, r.x.lengths, st));
+    RD_TRY(raindrop_fwd(&dc, params, r.x.src, r.x.statics, r.x.times, r.x.lengths, node_scale, nullptr, r.ws, r.logits,
+                        nullptr, nullptr, nullptr, 0, st));
+    RD_TRY(removal_moments(r.logits, clean_logits, target, attributions, r.keep, nc, B, P, r.s0.ncls, m0 == 0, moments,
+                           target_out, st));
+    if (n_samples - m0 <= cc) break;
+  }
+  return 0;
+}
+
+int rd_debug_removal_inputs(const rd_dims* dims, const float* src, const float* statics, const float* times,
+                            const int64_t* lengths, const float* baseline_src, const float* baseline_statics,
+                            const int32_t* cell_player, int64_t player_stride_t, int64_t player_stride_b,
+                            int32_t n_players, const int32_t* rank, const int32_t* counts, int32_t n_counts,
+                            const uint64_t* rng, double p_remove, int64_t q0, int32_t nc, uint8_t* keep_table,
+                            float* src_e, float* statics_e, float* times_e, int64_t* lengths_e, void* stream) {
+  const char* fn = "rd_debug_removal_inputs";
+  if (!dims || !src || !times || !lengths || !baseline_src || !keep_table || !src_e || !times_e || !lengths_e) {
+    set_error("%s: NULL argument", fn);
+    return -2;
+  }
+  Shape s0;
+  RD_TRY(make_shape(dims, &s0));
+  if (s0.ds > 0 && (!statics || !baseline_statics || !statics_e)) {
+    set_error("%s: d_static > 0 needs statics, baseline_statics and statics_e", fn);
+    return -2;
+  }
+  int G;
+  RD_TRY(removal_players(fn, s0, cell_player, player_stride_t, player_stride_b, n_players, &G));
+  if (nc < 1 || q0 < 0 || (int64_t)s0.B * nc > (1LL << 30)) {
+    set_error("%s: nc = %d must be >= 1 with B * nc <= 2^30, and q0 = %lld >= 0", fn, nc, (long long)q0);
+    return -2;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int P = n_players, B = s0.B;
+  if (rank) {
+    if (!counts || n_counts < 1 || n_counts > P + 1 || q0 + nc > 2LL * n_counts) {
+      set_error("%s: curve pairs need counts, 1 <= n_counts <= n_players + 1 and q0 + nc <= 2 n_counts", fn);
+      return -2;
+    }
+    RD_TRY(removal_curve_keep(rank, counts, n_counts, q0, nc, B, P, keep_table, st));
+  } else {
+    if (!rng) { set_error("%s: give rank (curves) or rng (infidelity)", fn); return -2; }
+    uint64_t below;
+    RD_TRY(removal_threshold(fn, p_remove, &below));
+    RD_TRY(removal_sample_keep(rng, below, q0, nc, B, P, keep_table, st));
+  }
+  return coalition_expand(src, baseline_src, statics, baseline_statics, times, lengths, cell_player, player_stride_t,
+                          player_stride_b, nullptr, P, G, COALITION_ROWS, 0, nc, B, s0.T, s0.N, s0.ds, keep_table, src_e,
+                          s0.ds > 0 ? statics_e : nullptr, times_e, lengths_e, st);
+}
+
 size_t rd_mc_dropout_scratch_bytes(const rd_dims* dims, int32_t replicates_per_chunk) {
   McScratch l;
   if (!dims || mc_scratch(dims, replicates_per_chunk, &l) != 0) return 0;

@@ -26,6 +26,9 @@ TRAK_DIM_MAX = 8192         # RD_TRAK_DIM_MAX
 ACTIVE_MAX_CLASSES = 8      # RD_ACTIVE_MAX_CLASSES
 ACTIVE_MAX_REPLICATES = 1024  # RD_ACTIVE_MAX_REPLICATES
 ACTIVE_MAX_CONFIGS = 65536  # RD_ACTIVE_MAX_CONFIGS
+REMOVAL_MAX_PLAYERS = 16384  # RD_REMOVAL_MAX_PLAYERS
+REMOVAL_DESCENDING, REMOVAL_ASCENDING, REMOVAL_ABSOLUTE = 0, 1, 2   # RD_REMOVAL_*
+REMOVAL_SUMMARIES = REMOVAL_MOMENTS = 6   # RD_REMOVAL_SUMMARIES, RD_REMOVAL_MOMENTS
 
 # enum rd_ws_buffer
 WS_X0, WS_H1, WS_ENC_IN, WS_ENC_OUT, WS_FEAT, WS_RNG, WS_HEAD_HIDDEN = range(7)
@@ -186,6 +189,17 @@ SIGNATURES = {
     "rd_raindrop_v2_kernel_shap": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9 +
                                    [C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                     C.c_int32] + [C.c_void_p] * 4),
+    "rd_removal_curves_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32, C.c_int32]),
+    "rd_raindrop_v2_removal_curves": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9 +
+                                      [C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                       C.c_int32] + [C.c_void_p] * 8),
+    "rd_removal_infidelity_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32, C.c_int32]),
+    "rd_raindrop_v2_removal_infidelity": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 9 +
+                                          [C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
+                                           C.c_int32, C.c_int32] + [C.c_void_p] * 5),
+    "rd_debug_removal_inputs": (C.c_int, [C.POINTER(RdDims)] + [C.c_void_p] * 7 + [C.c_int64, C.c_int64, C.c_int32] +
+                                [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_int64, C.c_int32] +
+                                [C.c_void_p] * 6),
     "rd_mc_dropout_scratch_bytes": (C.c_size_t, [C.POINTER(RdDims), C.c_int32]),
     "rd_raindrop_v2_mc_dropout": (C.c_int, [C.POINTER(RdDims), C.POINTER(RdParams)] + [C.c_void_p] * 6 +
                                   [C.c_int32, C.c_int32] + [C.c_void_p] * 6),
